@@ -421,11 +421,13 @@ int launch_reset(dm_handle* h, int force, const double* kt, const double* mt, co
 
 }  // namespace
 
-// Launch plan of dm_step_kernel: tile width, row capacity, shared-memory layout, environments per block (one block per SM: shared memory and
-// kStepMaxThreads cap the environments per block; the environments are spread evenly over the fewest waves of blocks that hold them, since a
-// wave takes as long as its fullest block), padded environment count.  Pure host arithmetic (also reachable without a device through
-// dm_plan_launch, for the CPU tests of the wave property).
-static bool plan_launch(dm_handle& H, int num_envs, int smem_optin, int sms, int max_tiles_env) {
+// Launch plan of dm_step_kernel: tile width, row capacity, shared-memory layout, environments per block, padded environment count.  Shared
+// memory and kStepMaxThreads cap the environments per block; the environments are spread evenly over the fewest waves of blocks that hold them,
+// since a wave takes as long as its fullest block.  A wave is one block per SM, or two when two blocks of the even split fit an SM's shared
+// memory (smem_sm, with reserved bytes per block) and its register file (regs per thread): the kernel is latency-bound, so two blocks of 16
+// humanoid environments per SM run in one wave what one block per SM needs two waves for.  With equally many waves the larger blocks win.  Pure
+// host arithmetic (also reachable without a device through dm_plan_launch, for the CPU tests of the wave property).
+static bool plan_launch(dm_handle& H, int num_envs, int smem_optin, int sms, int max_tiles_env, int smem_sm, int smem_reserved, int regs) {
     const auto& M = H.hm;
     H.W = (M.nl <= 16) ? 16 : 32;   // lanes per environment: one lane per link
     if (const char* w = std::getenv("DM_TILE_WIDTH")) { int v = std::atoi(w); if (v == 32 || (v == 16 && M.nl <= 16)) H.W = v; }
@@ -444,9 +446,20 @@ static bool plan_launch(dm_handle& H, int num_envs, int smem_optin, int sms, int
                 std::to_string(static_cast<long long>(smem_optin)) + ")";
         return false;
     }
-    const int waves = ((num_envs + max_tiles - 1) / max_tiles + sms - 1) / sms;
-    int tiles = std::min(max_tiles, std::max(min_tiles, (num_envs + waves * sms - 1) / (waves * sms)));
-    if (H.W == 16 && (tiles & 1)) tiles = (tiles + 1 <= max_tiles) ? tiles + 1 : tiles - 1;   // whole warps; tiles >= 2 here, so tiles - 1 >= 2 when odd
+    auto even_split = [&](int slots, int cap) {   // environments per block when num_envs is spread evenly over waves of `slots` blocks
+        const int waves = ((num_envs + cap - 1) / cap + slots - 1) / slots;
+        int t = std::min(cap, std::max(min_tiles, (num_envs + waves * slots - 1) / (waves * slots)));
+        if (H.W == 16 && (t & 1)) t = (t + 1 <= cap) ? t + 1 : t - 1;   // whole warps; t >= 2 here, so t - 1 >= 2 when odd
+        return std::make_pair(waves, t);
+    };
+    auto [waves, tiles] = even_split(sms, max_tiles);
+    {   // two blocks per SM: each within half the SM's shared memory and registers
+        const int cap2 = std::min({max_tiles, (smem_sm / 2 - smem_reserved - hot) / per_env, 65536 / (2 * regs * H.W)});
+        if (cap2 >= min_tiles) {
+            const auto [waves2, tiles2] = even_split(2 * sms, cap2);
+            if (waves2 < waves) { waves = waves2; tiles = tiles2; }
+        }
+    }
     H.tiles = tiles;
     const int quantum = (tiles * (64 / H.W)) / std::__gcd(tiles, 64 / H.W);   // multiple of both the update block and the 64-thread policy blocks
     H.padded_envs = ((num_envs + quantum - 1) / quantum) * quantum;
@@ -518,7 +531,8 @@ int dm_plan_launch(dm_handle* h, int num_envs, int smem_bytes_per_block, int num
     if (!h || num_envs <= 0 || num_sms <= 0) { g_err = "dm_plan_launch: bad arguments"; return fail(); }
     dm_handle tmp;
     tmp.hm = h->hm;
-    if (!plan_launch(tmp, num_envs, smem_bytes_per_block, num_sms, 0)) return fail();
+    // an SM holds the per-block maximum plus the 1 KB the runtime reserves per block (H100: 227 KB + 1 KB = 228 KB)
+    if (!plan_launch(tmp, num_envs, smem_bytes_per_block, num_sms, 0, smem_bytes_per_block + 1024, 1024, dmk::kStepRegs)) return fail();
     out[0] = tmp.W; out[1] = tmp.tiles; out[2] = tmp.padded_envs / tmp.tiles; out[3] = tmp.smem_bytes; out[4] = tmp.maxrows; out[5] = tmp.lay.env_floats;
     out[6] = tmp.lay.hot_floats; out[7] = tmp.lay.oY; out[8] = tmp.padded_envs;
     return 0;
@@ -571,7 +585,16 @@ dm_handle* dm_create(const char* asset_root, int argc, const char** argv, int nu
         if (!chk(cudaGetDeviceProperties(&prop, device), "cudaGetDeviceProperties")) { fail(); return nullptr; }
         int max_tiles_env = 0;
         if (const char* t = std::getenv("DM_TILES_PER_BLOCK")) max_tiles_env = std::atoi(t);
-        if (!plan_launch(*h, num_envs, static_cast<int>(prop.sharedMemPerBlockOptin), prop.multiProcessorCount, max_tiles_env)) { fail(); return nullptr; }
+        int regs = 0;   // registers per thread of the step kernel: the most any instantiation was compiled with
+        for (const void* f : {(const void*)dmk::dm_step_kernel<16, false, 0>, (const void*)dmk::dm_step_kernel<16, true, 0>, (const void*)dmk::dm_step_kernel<16, false, dmk::kVarTask>,
+                              (const void*)dmk::dm_step_kernel<16, false, dmk::kVarRootRot>, (const void*)dmk::dm_step_kernel<32, false, 0>, (const void*)dmk::dm_step_kernel<32, true, 0>,
+                              (const void*)dmk::dm_step_kernel<32, false, dmk::kVarTask>, (const void*)dmk::dm_step_kernel<32, false, dmk::kVarRootRot>}) {
+            cudaFuncAttributes fa;
+            if (!chk(cudaFuncGetAttributes(&fa, f), "cudaFuncGetAttributes dm_step_kernel")) { fail(); return nullptr; }
+            regs = std::max(regs, fa.numRegs);
+        }
+        if (!plan_launch(*h, num_envs, static_cast<int>(prop.sharedMemPerBlockOptin), prop.multiProcessorCount, max_tiles_env,
+                         static_cast<int>(prop.sharedMemPerMultiprocessor), static_cast<int>(prop.reservedSharedMemPerBlock), regs)) { fail(); return nullptr; }
     }
     const size_t N = static_cast<size_t>(h->padded_envs);
     const int ss = dmk::sim_stride(M.nl);

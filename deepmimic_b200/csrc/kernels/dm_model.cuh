@@ -21,7 +21,8 @@ constexpr int kMaxDofs = 96;    // 6 + joint dofs (humanoid3d 34, dog3d 70)
 constexpr int kMaxChain = 24;   // longest root->leaf dof chain (humanoid3d 13, dog3d 22)
 constexpr int kMaxChildren = 4;
 enum StepVariant { kVarTask = 1, kVarRootRot = 2 };   // dm_step_kernel<W, DEBUG, VAR>: optional scene features, one instantiation each
-constexpr int kStepMaxThreads = 448;    // dm_step_kernel: 28 (W=16) / 14 (W=32) environments per block (14 warps: 128 registers per thread)
+constexpr int kStepMaxThreads = 448;    // dm_step_kernel: 28 (W=16) / 14 (W=32) environments per block (14 warps)
+constexpr int kStepRegs = 128;          // registers per thread ptxas allocates for every dm_step_kernel instantiation (host-only launch plans; dm_create reads the real count)
 constexpr int kManifoldFloats = 48;  // per link: 4 points x 12 floats
 constexpr int kDebugFloats = 8 * kMaxDofs + 2048;   // test hook (dm_debug_*): stage dumps of one update
 
@@ -152,7 +153,8 @@ struct ObsFan {
 
 // Row capacity of the constraint solver per tile width = row stride of the Y block.  W = 16 (humanoid3d): 2 rows per lane (8 foot points x 3 + limits
 // <= 28).  W = 32: 52 = 16 points x 3 + 4 limit rows (dog3d: four feet flat + its four revolute joints at a limit), which is what lets 14
-// dog environments share a block: 2048 environments then run as ONE wave of 147 blocks instead of 171 blocks in two waves.
+// dog environments share a block: on 148 SMs 2048 environments then run as ONE wave of 147 blocks instead of 171 blocks in two waves.  (The
+// 132 SMs of an H100 would need two blocks of 8 per SM for one wave; DESIGN.md section 9 has what that lacks.)
 __host__ __device__ constexpr int dm_step_y_stride(int W) { return W == 16 ? 32 : 52; }
 
 // shared-memory layout of dm_step_kernel (float offsets inside one environment's block), filled by dm_step_layout on the host and

@@ -135,17 +135,19 @@ int dm_step_layout(int nl, int n, int chain_len, int maxrows, int W, StepLayout*
     L->nl = nl; L->n = n; L->chain_len = chain_len; L->maxrows = maxrows; L->maxpts = maxpts;
     L->oU = o; o += nl * 24;                       // per link: U0 U1 U2 (6 each), 1/D (3), sqrt(1/D) (3)
     L->oR = o; o += nl * 12;                       // per link: joint axes in world axes (9), parent pivot -> pivot (3)
-    L->oA = o;                                     // union { world frames + link velocities | packed lower triangle of J M^-1 J^T }
+    L->oA = o;                                     // union { world frames + link velocities, contact points, limit rows | packed lower triangle of J M^-1 J^T }
     const int world = nl * 24, tri = maxrows * (maxrows + 1) / 2;   // world: Rwl 9 + pivot 3 | link velocity 6 + pivot->COM 3 (+3 pad)
     L->oW = o; L->oV = o + nl * 12;
-    o += (world > tri ? world : tri);
-    o = (o + 3) & ~3;                              // 16-byte aligned: the articulated-body pass borrows the block as float4 scratch (28 floats per lane)
-    const int ys = dm_step_y_stride(W);
-    L->oY = o; o += (chain_len * ys > 28 * W) ? chain_len * ys : 28 * W;   // Yt[depth][row], row stride = the tile width's row capacity (a compile-time constant of the kernel: immediate offsets)
+    // the contact points (collide) and the limit rows of a sub-step are read only while solve_rows builds the rows, before it forms A in this region
+    L->oPp = o + world; L->oQ = L->oPp + maxpts * 4;   // limit rows: link, dir, penetration, joint rate (<= 8)
+    const int pre = world + maxpts * 4 + 4 * 8;
+    o += (pre > tri ? pre : tri);
+    o = (o + 3) & ~3;                              // 16-byte aligned: the articulated-body pass borrows the block as float4 scratch (28 floats per publishing link)
+    const int ys = dm_step_y_stride(W), scr = 28 * (nl - 1);   // links 1 .. nl-1 publish (aba_solve: the root link only gathers)
+    L->oY = o; o += (chain_len * ys > scr) ? chain_len * ys : scr;   // Yt[depth][row], row stride = the tile width's row capacity (a compile-time constant of the kernel: immediate offsets)
     L->oLam = o; o += maxrows; o += (o & 1); L->oRhs = o; o += maxrows; L->oInv = o; o += maxrows;   // oRhs .. : interleaved (rhs, 1 / A_ii) pairs, 8-byte aligned
     L->oRl = o; o += maxrows;                      // row -> link (int)
-    L->oPp = o; o += maxpts * 4; L->oPi = o; o += maxpts; L->oPr = o; o += maxpts;
-    L->oQ = o; o += 4 * 8;                         // limit rows: link, dir, penetration, joint rate (<= 8)
+    L->oPi = o; o += maxpts; L->oPr = o; o += maxpts;   // per contact point: cached impulse, manifold slot (Pr is read after the sweeps)
     L->oG = o; o += 21 + 13 + 2;                   // base Cholesky factor (21), base state: position 3, quaternion 4, omega 3, velocity 3
     L->oZ = o; o += ((n + 3) / 4) * 4;
     L->env_floats = ((o + 15) / 32) * 32 + 16;     // stride == 16 (mod 32 banks): the two environments of a warp (W = 16) hit disjoint bank halves
@@ -882,7 +884,9 @@ __device__ __noinline__ float3 aba_solve(float g0, float g1, float g2, float kdt
     // U_d = IA s_d goes straight to the environment's factor table (sU: read back by the acceleration pass below and, in the Bullet sub-steps,
     // by the constraint rows and the velocity correction) instead of living in 18 registers across the leaves -> root loop
     float* const uown = sU + c.lane * 24;
-    float* const scr = c.E + LY.oY;   // 28 floats per lane (dm_step_layout guarantees the room and the 16-byte alignment)
+    // 28 floats per publishing link, link j >= 1 at scr + 28 j = Y block + 28 (j - 1): only links with a dynamics level publish, and the root
+    // (lane 0, level -1) is not one of them (dm_step_layout guarantees the room for nl - 1 slots and the 16-byte alignment)
+    float* const scr = c.E + (LY.oY - 28);
     auto eliminate = [&](V3 dir, float g, int d, float& invo, float& uo) {
         const V3 Ua = sym_mul(IA.ww, dir), Ul = wvT_mul(IA.wv, dir);
         const float D = dot(dir, Ua) + kdt;
