@@ -19,7 +19,7 @@ DM_STATE_OFFSET, DM_STATE_SCALE, DM_ACTION_OFFSET, DM_ACTION_SCALE, DM_ACTION_BO
 
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
            "dm_update", "dm_record_state", "dm_record_goal", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
-           "dm_set_snapshot", "dm_get_counters", "dm_debug_enable", "dm_get_debug", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_launches", "dm_mlp_destroy"]
+           "dm_set_snapshot", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_launches", "dm_mlp_destroy"]
 
 
 def lib():
@@ -82,8 +82,7 @@ def lib():
         L.dm_get_snapshot.argtypes = [vp, C.c_int, dp]
         L.dm_set_snapshot.argtypes = [vp, C.c_int, dp]
         L.dm_get_counters.argtypes = [vp, C.POINTER(C.c_int64)]
-        L.dm_debug_enable.argtypes = [vp, C.c_int]
-        L.dm_get_debug.argtypes = [vp, C.c_int, C.c_void_p]
+        L.dm_get_section_profile.argtypes = [vp, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
         fpp = C.POINTER(C.c_float)
         L.dm_mlp_create.restype = vp
         L.dm_mlp_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, fpp, fpp, fpp, fpp, fpp, fpp, fpp, fpp, C.c_float, fpp, fpp, C.c_int]
@@ -285,12 +284,12 @@ class BatchedCore:
         self._chk(lib().dm_get_counters(self.h, out))
         return int(out[0]), int(out[1])
 
-    def debug_enable(self, on=True):
-        self._chk(lib().dm_debug_enable(self.h, 1 if on else 0))
-
-    def get_debug(self, env):
-        out = np.zeros(8 * 96 + 2048, dtype=np.float32)
-        self._chk(lib().dm_get_debug(self.h, env, C.c_void_p(out.ctypes.data)))
+    def section_profile(self):
+        """profile build only: [blocks, warps per block, 16] uint32 section cycle counters of the last update launch"""
+        nb, nw = C.c_int(0), C.c_int(0)
+        self._chk(lib().dm_get_section_profile(self.h, None, C.byref(nb), C.byref(nw)))
+        out = np.zeros((nb.value, nw.value, 16), dtype=np.uint32)
+        self._chk(lib().dm_get_section_profile(self.h, C.c_void_p(out.ctypes.data), None, None))
         return out
 
     def stream(self):

@@ -31,8 +31,8 @@ __global__ void dm_reset_kernel(const DevModel*, DevState, const double*, const 
 __global__ void dm_set_action_kernel(const DevModel*, DevState, const float*, int);
 template <int W, int BLOCK, bool TASKV>
 __global__ void dm_amp_obs_kernel(const DevModel*, DevState, const double*, const float*, const float*, float*, int, const double*, int, const int*);
-template <int W, bool DEBUG, int VAR>
-__global__ void dm_step_kernel(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout, int);
+template <int W, bool TASK>
+__global__ void dm_step_kernel(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout);
 __global__ void dm_task_reset_kernel(const DevModel*, DevState, int);
 __global__ void dm_task_observe_kernel(const DevModel*, DevState, float*, float*, int);
 int dm_step_layout(int nl, int n, int chain_len, int maxrows, int W, StepLayout* L);
@@ -112,7 +112,7 @@ struct dm_handle {
     float *d_act = nullptr, *d_obs = nullptr, *d_rew = nullptr;            // staging for dm_step_host
     float *p_act = nullptr, *p_obs = nullptr, *p_rew = nullptr; int32_t* p_flags = nullptr;  // pinned host staging
     cudaStream_t stream = nullptr;
-    int device = 0, num_envs = 0, padded_envs = 0, W = 32, tiles = 2, maxrows = 36, smem_bytes = 0, mode = 0, minb = 4, sync_every_stage = 1;   // block barrier after every stage (Stable-PD stage, each Bullet sub-step): measured 2.12 M vs 2.11 M per update, 1.94 / 1.89 / 1.78 M every 2 / 4 updates / never (warps that drift apart thrash the instruction cache)
+    int device = 0, num_envs = 0, padded_envs = 0, W = 32, tiles = 2, maxrows = 36, smem_bytes = 0, mode = 0;
     dmk::StepLayout lay{};
     uint64_t seed = 0, env_offset = 0;
     int64_t launches = 0;
@@ -352,9 +352,9 @@ void build_statics(dm_handle& H) {
     }
 }
 
-template <int W, bool DEBUG, int VAR>
+template <int W, bool TASK>
 int launch_step(dm_handle* h, double dt, int n_updates) {
-    auto kern = dmk::dm_step_kernel<W, DEBUG, VAR>;
+    auto kern = dmk::dm_step_kernel<W, TASK>;
     // opt in to the large dynamic shared-memory carve-out; the limit is raised whenever a handle needs more than any earlier one on
     // this device (attributes are per device and per function: several handles of different sizes may live in one process)
     static std::mutex mu;
@@ -369,23 +369,10 @@ int launch_step(dm_handle* h, double dt, int n_updates) {
         }
     }
     const int grid = h->padded_envs / h->tiles;
-    kern<<<grid, h->tiles * W, h->smem_bytes, h->stream>>>(h->d_model, h->st, h->d_frame_times, h->d_frames, dt, n_updates, h->sa.cfg.num_sim_substeps, h->lay, h->sync_every_stage);
+    kern<<<grid, h->tiles * W, h->smem_bytes, h->stream>>>(h->d_model, h->st, h->d_frame_times, h->d_frames, dt, n_updates, h->sa.cfg.num_sim_substeps, h->lay);
     DM_CUDA(cudaGetLastError());
     h->launches++;
     return 0;
-}
-template <int W, bool DEBUG>
-int launch_update(dm_handle* h, double dt, int n_updates) {
-    if (h->hm.task_kind != dmk::kTaskNone) {   // AMP task scenes: the instantiation that also advances the task block (no debug dumps there)
-        if (DEBUG) { g_err = "dm_debug_enable is not available in the AMP task scenes"; return fail(); }
-        if (h->hm.sync_root_rot) { g_err = "--sync_char_root_rot in an AMP task scene is not built"; return fail(); }
-        return launch_step<W, false, dmk::kVarTask>(h, dt, n_updates);
-    }
-    if (h->hm.sync_root_rot) {   // --sync_char_root_rot true: the instantiation with the heading sync at clip wraps
-        if (DEBUG) { g_err = "dm_debug_enable is not available with --sync_char_root_rot"; return fail(); }
-        return launch_step<W, false, dmk::kVarRootRot>(h, dt, n_updates);
-    }
-    return launch_step<W, DEBUG, 0>(h, dt, n_updates);
 }
 template <int W>
 int launch_observe_fan(dm_handle* h, const dmk::ObsFan& fan) {
@@ -427,19 +414,16 @@ int launch_reset(dm_handle* h, int force, const double* kt, const double* mt, co
 // memory (smem_sm, with reserved bytes per block) and its register file (regs per thread): the kernel is latency-bound, so two blocks of 16
 // humanoid environments per SM run in one wave what one block per SM needs two waves for.  With equally many waves the larger blocks win.  Pure
 // host arithmetic (also reachable without a device through dm_plan_launch, for the CPU tests of the wave property).
-static bool plan_launch(dm_handle& H, int num_envs, int smem_optin, int sms, int max_tiles_env, int smem_sm, int smem_reserved, int regs) {
+static bool plan_launch(dm_handle& H, int num_envs, int smem_optin, int sms, int smem_sm, int smem_reserved, int regs) {
     const auto& M = H.hm;
     H.W = (M.nl <= 16) ? 16 : 32;   // lanes per environment: one lane per link
-    if (const char* w = std::getenv("DM_TILE_WIDTH")) { int v = std::atoi(w); if (v == 32 || (v == 16 && M.nl <= 16)) H.W = v; }
     H.maxrows = dmk::dm_step_y_stride(H.W);   // humanoid3d: 8 foot points x 3 + limit rows <= 28 of 32; dog3d: 4 feet x 4 points x 3 + 4 limit rows = 52
-    if (const char* r = std::getenv("DM_MAX_ROWS")) { int v = std::atoi(r); if (v >= 12 && v <= dmk::dm_step_y_stride(H.W)) H.maxrows = v; }
     int chain_len = 0;
     for (int j = 0; j < M.nl; ++j) chain_len = std::max(chain_len, M.link[j].last_depth + 1);
     dmk::dm_step_layout(M.nl, M.n, chain_len, H.maxrows, H.W, &H.lay);
     const int per_env = H.lay.env_floats * 4;
     const int hot = H.lay.hot_floats * 4 + 1024;
-    int max_tiles = std::min(dmk::kStepMaxThreads / H.W, (smem_optin - hot) / per_env);
-    if (max_tiles_env > 0) max_tiles = std::min(max_tiles, std::max(H.W == 16 ? 2 : 1, max_tiles_env));
+    const int max_tiles = std::min(dmk::kStepMaxThreads / H.W, (smem_optin - hot) / per_env);
     const int min_tiles = (H.W == 16) ? 2 : 1;   // W = 16: two environments share a warp
     if (max_tiles < min_tiles) {
         g_err = "not enough shared memory per block for one environment tile (need " + std::to_string(hot + min_tiles * per_env) + " bytes, the device offers " +
@@ -496,6 +480,7 @@ static bool load_host_model(dm_handle& H, const char* asset_root, int argc, cons
             bool soft = false;
             if (ap.ParseBool("enable_char_soft_contact", soft) && soft) throw std::runtime_error("Unsupported: --enable_char_soft_contact true");
             if (c.enable_root_rot_fail) throw std::runtime_error("Unsupported: --enable_root_rot_fail true");
+            if (c.is_task_scene() && c.sync_char_root_rot) throw std::runtime_error("Unsupported: --sync_char_root_rot true in an AMP task scene");
             if (!c.terrain_file.empty()) {   // cGroundBuilder: only the flat plane (data/terrain/plane.txt) is on the path
                 dmh::Json t = dmh::Json::parseFile(dmh::resolve_path(root, c.terrain_file));
                 if (t["Type"].asString("") != "plane") throw std::runtime_error("Unsupported terrain type: " + t["Type"].asString("") + " (supported: plane)");
@@ -532,7 +517,7 @@ int dm_plan_launch(dm_handle* h, int num_envs, int smem_bytes_per_block, int num
     dm_handle tmp;
     tmp.hm = h->hm;
     // an SM holds the per-block maximum plus the 1 KB the runtime reserves per block (H100: 227 KB + 1 KB = 228 KB)
-    if (!plan_launch(tmp, num_envs, smem_bytes_per_block, num_sms, 0, smem_bytes_per_block + 1024, 1024, dmk::kStepRegs)) return fail();
+    if (!plan_launch(tmp, num_envs, smem_bytes_per_block, num_sms, smem_bytes_per_block + 1024, 1024, dmk::kStepRegs)) return fail();
     out[0] = tmp.W; out[1] = tmp.tiles; out[2] = tmp.padded_envs / tmp.tiles; out[3] = tmp.smem_bytes; out[4] = tmp.maxrows; out[5] = tmp.lay.env_floats;
     out[6] = tmp.lay.hot_floats; out[7] = tmp.lay.oY; out[8] = tmp.padded_envs;
     return 0;
@@ -579,22 +564,18 @@ dm_handle* dm_create(const char* asset_root, int argc, const char** argv, int nu
     h->device = device; h->seed = seed; h->env_offset = global_env_offset; h->num_envs = num_envs;
     h->hm.task_seed = seed ^ 0x7461736b73ull; h->hm.env_id_base = global_env_offset;   // the model blob is uploaded below
     const auto& M = h->hm;
-    if (const char* sv = std::getenv("DM_SYNC_EVERY_STAGE")) h->sync_every_stage = std::atoi(sv);
     {
         cudaDeviceProp prop;
         if (!chk(cudaGetDeviceProperties(&prop, device), "cudaGetDeviceProperties")) { fail(); return nullptr; }
-        int max_tiles_env = 0;
-        if (const char* t = std::getenv("DM_TILES_PER_BLOCK")) max_tiles_env = std::atoi(t);
         int regs = 0;   // registers per thread of the step kernel: the most any instantiation was compiled with
-        for (const void* f : {(const void*)dmk::dm_step_kernel<16, false, 0>, (const void*)dmk::dm_step_kernel<16, true, 0>, (const void*)dmk::dm_step_kernel<16, false, dmk::kVarTask>,
-                              (const void*)dmk::dm_step_kernel<16, false, dmk::kVarRootRot>, (const void*)dmk::dm_step_kernel<32, false, 0>, (const void*)dmk::dm_step_kernel<32, true, 0>,
-                              (const void*)dmk::dm_step_kernel<32, false, dmk::kVarTask>, (const void*)dmk::dm_step_kernel<32, false, dmk::kVarRootRot>}) {
+        for (const void* f : {(const void*)dmk::dm_step_kernel<16, false>, (const void*)dmk::dm_step_kernel<16, true>, (const void*)dmk::dm_step_kernel<32, false>,
+                              (const void*)dmk::dm_step_kernel<32, true>}) {
             cudaFuncAttributes fa;
             if (!chk(cudaFuncGetAttributes(&fa, f), "cudaFuncGetAttributes dm_step_kernel")) { fail(); return nullptr; }
             regs = std::max(regs, fa.numRegs);
         }
-        if (!plan_launch(*h, num_envs, static_cast<int>(prop.sharedMemPerBlockOptin), prop.multiProcessorCount, max_tiles_env,
-                         static_cast<int>(prop.sharedMemPerMultiprocessor), static_cast<int>(prop.reservedSharedMemPerBlock), regs)) { fail(); return nullptr; }
+        if (!plan_launch(*h, num_envs, static_cast<int>(prop.sharedMemPerBlockOptin), prop.multiProcessorCount, static_cast<int>(prop.sharedMemPerMultiprocessor),
+                         static_cast<int>(prop.reservedSharedMemPerBlock), regs)) { fail(); return nullptr; }
     }
     const size_t N = static_cast<size_t>(h->padded_envs);
     const int ss = dmk::sim_stride(M.nl);
@@ -631,8 +612,13 @@ dm_handle* dm_create(const char* asset_root, int argc, const char** argv, int nu
               chk(cudaMallocHost(&h->p_obs, N * M.state_size * sizeof(float)), "cudaMallocHost") && chk(cudaMallocHost(&h->p_rew, N * sizeof(float)), "cudaMallocHost") &&
               chk(cudaMallocHost(&h->p_flags, N * 4 * sizeof(int32_t)), "cudaMallocHost");
     for (int k = 0; k < 3 && ok; ++k) ok = chk(cudaMalloc(&h->d_inj[k], N * sizeof(double)), "cudaMalloc inject");
+#ifdef DM_PROFILE
+    const size_t prof_counters = static_cast<size_t>(h->padded_envs / h->tiles) * (h->tiles * h->W / 32) * dmk::kProfCounters;   // blocks x warps per block
+    ok = ok && chk(cudaMalloc(&h->st.prof, prof_counters * sizeof(unsigned int)), "cudaMalloc section profile") &&
+         chk(cudaMemset(h->st.prof, 0, prof_counters * sizeof(unsigned int)), "memset section profile");
+#endif
     if (!ok) { fail(); dm_destroy(h.release()); return nullptr; }
-    h->st.pdbg = nullptr; h->st.num_envs = h->padded_envs; h->st.num_real = h->num_envs;
+    h->st.num_envs = h->padded_envs; h->st.num_real = h->num_envs;
     if (M.task_kind != dmk::kTaskNone) {
         if (!(chk(cudaMalloc(&h->st.task, N * dmk::kTaskDoubles * sizeof(double)), "cudaMalloc task") &&
               chk(cudaMemset(h->st.task, 0, N * dmk::kTaskDoubles * sizeof(double)), "memset task") &&
@@ -691,7 +677,7 @@ void dm_destroy(dm_handle* h) {
     cudaSetDevice(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
     dm_exchange_destroy(h);
-    cudaFree(h->st.task); cudaFree(h->st.taskx); cudaFree(h->d_goal); cudaFreeHost(h->p_goal); cudaFree(h->st.clip); cudaFree(h->d_clip_inj); cudaFree(h->d_ctab);
+    cudaFree(h->st.prof); cudaFree(h->st.task); cudaFree(h->st.taskx); cudaFree(h->d_goal); cudaFreeHost(h->p_goal); cudaFree(h->st.clip); cudaFree(h->d_clip_inj); cudaFree(h->d_ctab);
     cudaFree(h->d_amp); cudaFreeHost(h->p_amp); cudaFree(h->st.hist); cudaFree(h->d_model); cudaFree(h->st.sim); cudaFree(h->st.time); cudaFree(h->st.flags); cudaFree(h->st.manifold);
     cudaFree(h->d_frame_times); cudaFree(h->d_frames); cudaFree(h->d_frame_vel); cudaFree(h->d_flags4); cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew);
     for (auto& p : h->d_inj) cudaFree(p);
@@ -825,12 +811,9 @@ int dm_set_action(dm_handle* h, const float* d_actions) {
 }
 int dm_update(dm_handle* h, double dt, int n_updates) {
     DM_DEVICE(h);
-    bool dbg = h->st.pdbg != nullptr;
-#ifdef DM_PROFILE
-    dbg = false;   // profile build: the production kernel writes its per-warp section counters into the debug buffer
-#endif
-    if (h->W == 16) return dbg ? launch_update<16, true>(h, dt, n_updates) : launch_update<16, false>(h, dt, n_updates);
-    return dbg ? launch_update<32, true>(h, dt, n_updates) : launch_update<32, false>(h, dt, n_updates);
+    const bool task = h->hm.task_kind != dmk::kTaskNone;   // AMP task scenes: the instantiation that also advances the task block
+    if (h->W == 16) return task ? launch_step<16, true>(h, dt, n_updates) : launch_step<16, false>(h, dt, n_updates);
+    return task ? launch_step<32, true>(h, dt, n_updates) : launch_step<32, false>(h, dt, n_updates);
 }
 static int launch_task_observe(dm_handle* h, float* d_goal, float* d_reward) {
     dmk::dm_task_observe_kernel<<<(h->num_envs + 127) / 128, 128, 0, h->stream>>>(h->d_model, h->st, d_goal, d_reward, h->num_envs);
@@ -1212,20 +1195,16 @@ int dm_set_snapshot(dm_handle* h, int env, const double* s) {
     DM_CUDA(cudaMemcpy(h->st.flags + static_cast<size_t>(env) * dmk::kFlagInts, fl, sizeof(fl), cudaMemcpyHostToDevice));
     return 0;
 }
-int dm_debug_enable(dm_handle* h, int on) {
+int dm_get_section_profile(dm_handle* h, uint32_t* out, int* num_blocks, int* warps_per_block) {
     DM_DEVICE(h);
-    DM_CUDA(cudaStreamSynchronize(h->stream));
-    if (on && !h->st.pdbg) {
-        DM_CUDA(cudaMalloc(&h->st.pdbg, static_cast<size_t>(h->padded_envs) * dmk::kDebugFloats * sizeof(float)));
-        DM_CUDA(cudaMemset(h->st.pdbg, 0, static_cast<size_t>(h->padded_envs) * dmk::kDebugFloats * sizeof(float)));
-    } else if (!on && h->st.pdbg) { cudaFree(h->st.pdbg); h->st.pdbg = nullptr; }
-    return 0;
-}
-int dm_get_debug(dm_handle* h, int env, float* out) {
-    DM_DEVICE(h);
-    DM_CUDA(cudaStreamSynchronize(h->stream));
-    if (!h->st.pdbg) { g_err = "debug dumps are not enabled"; return fail(); }
-    DM_CUDA(cudaMemcpy(out, h->st.pdbg + static_cast<size_t>(env) * dmk::kDebugFloats, dmk::kDebugFloats * sizeof(float), cudaMemcpyDeviceToHost));
+    if (!h->st.prof) { g_err = "dm_get_section_profile: this library is not the profile build (make -C deepmimic_b200/csrc profile)"; return fail(); }
+    const int blocks = h->padded_envs / h->tiles, warps = h->tiles * h->W / 32;
+    if (num_blocks) *num_blocks = blocks;
+    if (warps_per_block) *warps_per_block = warps;
+    if (out) {
+        DM_CUDA(cudaStreamSynchronize(h->stream));
+        DM_CUDA(cudaMemcpy(out, h->st.prof, static_cast<size_t>(blocks) * warps * dmk::kProfCounters * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    }
     return 0;
 }
 int dm_get_counters(dm_handle* h, int64_t* out) {

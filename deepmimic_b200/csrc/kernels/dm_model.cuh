@@ -20,11 +20,10 @@ constexpr int kMaxLinks = 32;   // one lane per link
 constexpr int kMaxDofs = 96;    // 6 + joint dofs (humanoid3d 34, dog3d 70)
 constexpr int kMaxChain = 24;   // longest root->leaf dof chain (humanoid3d 13, dog3d 22)
 constexpr int kMaxChildren = 4;
-enum StepVariant { kVarTask = 1, kVarRootRot = 2 };   // dm_step_kernel<W, DEBUG, VAR>: optional scene features, one instantiation each
 constexpr int kStepMaxThreads = 448;    // dm_step_kernel: 28 (W=16) / 14 (W=32) environments per block (14 warps)
 constexpr int kStepRegs = 128;          // registers per thread ptxas allocates for every dm_step_kernel instantiation (host-only launch plans; dm_create reads the real count)
 constexpr int kManifoldFloats = 48;  // per link: 4 points x 12 floats
-constexpr int kDebugFloats = 8 * kMaxDofs + 2048;   // test hook (dm_debug_*): stage dumps of one update
+constexpr int kProfCounters = 16;    // DM_PROFILE builds: section cycle counters per warp of dm_step_kernel
 
 enum DevJointType { kJRevolute = 0, kJSpherical = 1, kJFixed = 2 };
 enum DevShape { kSBox = 1, kSCapsule = 2, kSSphere = 3 };
@@ -132,7 +131,7 @@ struct DevState {
     int* flags;
     float* manifold;
     float* hist;  // AMP history: DeepMimic pose | vel vectors (2 * pose_dim floats per env) of the simulated character at the last applied action
-    float* pdbg;  // optional debug scratch (n x ...), may be null
+    unsigned int* prof;   // DM_PROFILE builds: kProfCounters per warp of every step-kernel block; null otherwise
     double* task; // AMP task scenes: kTaskDoubles per env (dm_task.cuh), null otherwise
     double* taskx; // ... and kTaskExtDoubles per env (dm_task_ext.cuh)
     int* clip;    // --kin_ctrl clips: active clip of every env, null for single-clip scenes

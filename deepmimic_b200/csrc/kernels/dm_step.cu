@@ -156,9 +156,7 @@ int dm_step_layout(int nl, int n, int chain_len, int maxrows, int W, StepLayout*
 }
 int dm_step_smem_bytes(const StepLayout& L, int tiles) { return (L.hot_floats + L.env_floats * tiles) * static_cast<int>(sizeof(float)); }
 
-#ifndef DM_PGS_BLOCK
-#define DM_PGS_BLOCK 2   // solver steps evaluated per block of the projected Gauss-Seidel sweeps (chosen by measuring 1, 2, 4 and 8; 2 was the fastest)
-#endif
+constexpr int kPgsBlock = 2;   // solver steps evaluated per block of the projected Gauss-Seidel sweeps (chosen by measuring 1, 2, 4 and 8; 2 was the fastest)
 // Projected Gauss-Seidel in impulse space, 10 sweeps in btMultiBodyConstraintSolver::solveSingleIteration's row order (joint limits in
 // alternating order, contact normals, friction pairs).  Lanes = rows for the state that is wide: every lane keeps w = (A lambda)_row of ITS rows in
 // registers (S rows per lane: row = lane + s W).  The sequential part is evaluated in blocks of B consecutive solver steps of one section:
@@ -301,7 +299,7 @@ __device__ __noinline__ void solve_rows(int NL, int P, float* mani, int alive, u
 #endif
     const StepLayout& LY = *reinterpret_cast<const StepLayout*>(LYS);
     const int nl = LY.nl, CL = LY.chain_len, MR = LY.maxrows;
-    constexpr int YS = dm_step_y_stride(W);   // row stride of Yt (>= maxrows: the host caps the row capacity there)
+    constexpr int YS = dm_step_y_stride(W);   // row stride of Yt (= maxrows: the row capacity of the tile width)
     float* const E = sm_ + LY.hot_floats + (threadIdx.x / W) * LY.env_floats;
     const unsigned char* CD = reinterpret_cast<const unsigned char*>(LK + nl * kLkFloats);
     const unsigned char* CH = CD + nl * nl;
@@ -315,8 +313,7 @@ __device__ __noinline__ void solve_rows(int NL, int P, float* mani, int alive, u
     const int NR = NL + 3 * P;
     const int NRmax = (W == 32) ? NR : wmax(NR);
     const int nslots = (NRmax + W - 1) / W;
-    constexpr int kPgsBlock = DM_PGS_BLOCK;
-    constexpr int kSlots = 2;   // rows per lane in the general path: the host caps the row capacity at dm_step_y_stride(W) (32 humanoid3d, 52 dog3d)
+    constexpr int kSlots = 2;   // rows per lane in the general path: the row capacity is dm_step_y_stride(W) (32 humanoid3d, 52 dog3d)
 #pragma unroll
     for (int s = 0; s < kSlots; ++s) {
         const int rid = lane + s * W;
@@ -802,8 +799,8 @@ __device__ __noinline__ int collide(float* mani, int alive, int mcnt) {
 //   (deepest first) = one step of the tree-structured L^T D L; base: 6x6 Cholesky in world axes (= the generalised base coordinates);
 //   root -> leaves: accelerations.  Bullet sub-steps (bullet != 0) also publish the factors (sU, sG), advance the link velocities in sV
 //   and the base velocity in sB by h * acceleration.  Returns this link's joint accelerations.
-template <int W, bool DEBUG>
-__device__ __noinline__ float3 aba_solve(float g0, float g1, float g2, float kdt, int bullet, float jvx, float jvy, float jvz, float* dbg_acc) {
+template <int W>
+__device__ __noinline__ float3 aba_solve(float g0, float g1, float g2, float kdt, int bullet, float jvx, float jvy, float jvz) {
     const Ctx c = make_ctx<W>();
     const float gx = step_smem()[kHGrav], gy = step_smem()[kHGrav + 1], gz = step_smem()[kHGrav + 2], h = step_smem()[kHh];
     using T = Tl<W>;
@@ -992,7 +989,6 @@ __device__ __noinline__ float3 aba_solve(float g0, float g1, float g2, float kdt
 #pragma unroll
             for (int i = 0; i < 6; ++i) sB[7 + i] = cl100(sB[7 + i] + h * x[i]);
         }
-        if (DEBUG && dbg_acc) for (int i = 0; i < 6; ++i) dbg_acc[i] = x[i];
     }
     // ---- accelerations (root -> leaves): qdd_d = (u_d - U_d . a') / D_d
     float qd0 = 0.f, qd1 = 0.f, qd2 = 0.f;
@@ -1119,13 +1115,11 @@ __device__ __noinline__ void vel_pass(float jvx, float jvy, float jvz, bool want
     __syncwarp();
 }
 
-// VAR selects optional scene features compiled into separate instantiations so that the plain imitate kernel carries none of their code:
-//   bit 0 (kVarTask)    AMP task scenes: task block advanced after every update (dm_task.cuh)
-//   bit 1 (kVarRootRot) --sync_char_root_rot: the heading sync of cSceneImitate::SyncKinCharNewCycle at a clip wrap
-template <int W, bool DEBUG, int VAR>
+// TASK: the AMP task scenes' instantiation, which also advances the environment's task block after every update (dm_task.cuh); the plain
+// imitate kernel carries none of that code.
+template <int W, bool TASK>
 __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevModel* __restrict__ gm, DevState st, const double* __restrict__ frame_times,
-                                                                       const float* __restrict__ frames, double dt, int n_updates, int sim_substeps, StepLayout LY, int sync_mode) {
-    constexpr bool TASK = (VAR & kVarTask) != 0, ROOTROT = (VAR & kVarRootRot) != 0;
+                                                                       const float* __restrict__ frames, double dt, int n_updates, int sim_substeps, StepLayout LY) {
     using T = Tl<W>;
     extern __shared__ __align__(16) float sm[];
     const int tiles = blockDim.x / W;
@@ -1233,7 +1227,6 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
     float* sV = E + LY.oV; float* sG = E + LY.oG; float* sQ = E + LY.oQ; float* sLam = E + LY.oLam;
     const float* LKo = LK + li * kLkFloats;
     const int jtype = (reinterpret_cast<const int*>(LKo)[kLInt] >> 8) & 0xff, ndof = act ? ((reinterpret_cast<const int*>(LKo)[kLInt] >> 16) & 0xff) : 0;
-    const int dof0 = reinterpret_cast<const int*>(LKo)[kLInt2] & 0xff;
     const int lflags = reinterpret_cast<const int*>(LKo)[kLFlg];
     const bool fall_contact = ((lflags >> 8) & 0xff) != 0, has_limit = ((lflags >> 16) & 0xff) != 0;
 
@@ -1268,15 +1261,14 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
     const float fdt = static_cast<float>(dt);
     const float gx = M.gravity[0], gy = M.gravity[1], gz = M.gravity[2];
     const float scale = M.scale, mu = M.friction;
-    float* dbg = (DEBUG && st.pdbg) ? st.pdbg + static_cast<size_t>(env) * kDebugFloats : nullptr;   // test hook: stage dumps of the first update
 
     float tau0 = 0.f, tau1 = 0.f, tau2 = 0.f;   // joint torques of the current update (body-frame components / revolute scalar)
     bool in_contact_tol = false;
 
 #ifdef DM_PROFILE
-    // per-warp cycle counters per code section (profile build only): lane 0 accumulates, written to st.pdbg at the end
-    unsigned int* PRF = reinterpret_cast<unsigned int*>(sm + LY.hot_floats + tiles * LY.env_floats) + (threadIdx.x / 32) * 16;
-    if ((threadIdx.x & 31) == 0) for (int k = 0; k < 16; ++k) PRF[k] = 0u;
+    // per-warp cycle counters per code section (profile build only): lane 0 accumulates, written to st.prof at the end
+    unsigned int* PRF = reinterpret_cast<unsigned int*>(sm + LY.hot_floats + tiles * LY.env_floats) + (threadIdx.x / 32) * kProfCounters;
+    if ((threadIdx.x & 31) == 0) for (int k = 0; k < kProfCounters; ++k) PRF[k] = 0u;
     unsigned int prf_t = static_cast<unsigned int>(clock64());
 #define PROF(sec) do { if ((threadIdx.x & 31) == 0) { unsigned int t_ = static_cast<unsigned int>(clock64()); PRF[sec] += t_ - prf_t; prf_t = t_; } } while (0)
     unsigned int* PRFP = PRF;
@@ -1288,7 +1280,6 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
     int mcnt = 4;   // cached points of this lane's link after the last collision pass; unknown at the start of a launch: forces the first read
     const int stages_per_upd = sim_substeps + 1;
     const int total_stages = n_updates * stages_per_upd;
-    const int sync_period = sync_mode > 0 ? 1 : (sync_mode == 0 ? stages_per_upd : (sync_mode <= -1000 ? 0 : -sync_mode * stages_per_upd));
 #pragma unroll 1
     for (int stage = 0; stage <= total_stages; ++stage) {
         // the manifold of this lane's link is read by the collision pass of a Bullet sub-step: start pulling its two cache lines in now
@@ -1388,11 +1379,12 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
         }
         PROF(1);
         if (stage == total_stages) break;
-        if (sync_period != 0 && (stage % sync_period) == 0) { if (__syncthreads_and(!alive)) break; }
+        // a block barrier after every stage keeps the warps in lockstep: warps that drift apart thrash the instruction cache (measured throughput:
+        // 2.12 M with this barrier, 2.11 M with one per update, 1.94 / 1.89 / 1.78 M with one every 2 / 4 updates / none)
+        if (__syncthreads_and(!alive)) break;
         PROF(2);
         if (__ballot_sync(0xffffffffu, alive) == 0u) continue;   // both environments of this warp are frozen
         const int ph = stage % stages_per_upd;      // 0: Stable-PD stage, 1..sim_substeps: Bullet sub-steps
-        const bool first_upd = stage < stages_per_upd;
         if (ph == 0) {
             // ---------------- clocks: cScene::Update, cSceneImitate::UpdateKinChar, cDeepMimicCharController::UpdateCalcTau
             int cb = 0;
@@ -1412,49 +1404,19 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
                 double p0 = kin_time / dur; p0 -= floor(p0);
                 kin_time += dt;
                 double p1 = kin_time / dur; p1 -= floor(p1);
-                if constexpr (ROOTROT) {
-                    // --sync_char_root_rot instantiation: the whole wrap handling is the shared host / device routine of dm_task.cuh
-                    // (checked against the oracle on the host, tests/test_task_scenes_cpu.py)
-                    if (M.loop_motion && p1 < p0 && (M.sync_root_pos || M.sync_root_rot)) {
-                        const double simq[4] = {static_cast<double>(sB[3]), static_cast<double>(sB[4]), static_cast<double>(sB[5]), static_cast<double>(sB[6])};
-                        kin_wrap_sync(frame_times, frames, M.pose_dim, M.num_frames, M.cycle_delta, dur, kin_time, tm + kTOrigin, tm + kTOriginRot,
-                                      static_cast<double>(sB[0]) / M.scale, static_cast<double>(sB[2]) / M.scale, simq, M.sync_root_pos != 0, M.sync_root_rot != 0);
-                    }
-                }
+                // cSceneImitate::SyncKinCharNewCycle at a clip wrap: the shared host / device routine of dm_task.cuh (checked against the oracle on
+                // the host, tests/test_task_scenes_cpu.py).  The task scenes run it on the environment's own clip of the dataset.
                 if constexpr (TASK) {
-                    // task scenes: same wrap handling on the environment's own clip of the dataset
                     const ClipInfo& ci = st.ctab->info[st.clip[env]];
                     if (ci.loop && p1 < p0 && M.sync_root_pos) {
                         const double simq[4] = {static_cast<double>(sB[3]), static_cast<double>(sB[4]), static_cast<double>(sB[5]), static_cast<double>(sB[6])};
                         kin_wrap_sync(frame_times + ci.frame_off, frames + static_cast<size_t>(ci.frame_off) * M.pose_dim, M.pose_dim, ci.num_frames, ci.cycle_delta, dur, kin_time,
                                       tm + kTOrigin, tm + kTOriginRot, static_cast<double>(sB[0]) / M.scale, static_cast<double>(sB[2]) / M.scale, simq, true, false);
                     }
-                }
-                if (!ROOTROT && !TASK && M.loop_motion && p1 < p0 && M.sync_root_pos) {
-                    // SyncKinCharNewCycle: snap the clip's root x,z (at the new time) onto the simulated root
-                    double org_x = tm[kTOrigin], org_z = tm[kTOrigin + 2];
-                    int cyc = static_cast<int>(floor(kin_time / dur));
-                    double tt = kin_time - cyc * dur;
-                    int lo = 0, hi = M.num_frames - 1;   // upper_bound - 1
-                    while (hi - lo > 1) { int mid = (lo + hi) >> 1; if (frame_times[mid] <= tt) lo = mid; else hi = mid; }
-                    double bl = (tt - frame_times[lo]) / (frame_times[lo + 1] - frame_times[lo]);
-                    bl = fmin(fmax(bl, 0.0), 1.0);
-                    const float* f0 = frames + static_cast<size_t>(lo) * M.pose_dim; const float* f1 = f0 + M.pose_dim;
-                    double rx = (1 - bl) * f0[0] + bl * f1[0] + cyc * static_cast<double>(M.cycle_delta[0]);
-                    double rz = (1 - bl) * f0[2] + bl * f1[2] + cyc * static_cast<double>(M.cycle_delta[2]);
-                    double qw = tm[kTOriginRot], qx = tm[kTOriginRot + 1], qy = tm[kTOriginRot + 2], qz = tm[kTOriginRot + 3];
-                    double ry_ = (1 - bl) * f0[1] + bl * f1[1];
-                    double ux = qy * rz - qz * ry_, uy = qz * rx - qx * rz, uz = qx * ry_ - qy * rx;
-                    ux *= 2; uy *= 2; uz *= 2;
-                    double kx = rx + qw * ux + (qy * uz - qz * uy);
-                    double kz = rz + qw * uz + (qx * uy - qy * ux);
-                    double sx = static_cast<double>(sB[0]) / M.scale, sz = static_cast<double>(sB[2]) / M.scale;
-                    if (M.sync_root_pos) {
-                        org_x += sx - (kx + org_x);
-                        org_z += sz - (kz + org_z);
-                        tm[kTOrigin + 1] = 0.0;   // kin_root.y := ground_h + (kin_root.y - origin.y)  =>  origin.y returns to 0
-                    }
-                    tm[kTOrigin] = org_x; tm[kTOrigin + 2] = org_z;
+                } else if (M.loop_motion && p1 < p0 && (M.sync_root_pos || M.sync_root_rot)) {
+                    const double simq[4] = {static_cast<double>(sB[3]), static_cast<double>(sB[4]), static_cast<double>(sB[5]), static_cast<double>(sB[6])};
+                    kin_wrap_sync(frame_times, frames, M.pose_dim, M.num_frames, M.cycle_delta, dur, kin_time, tm + kTOrigin, tm + kTOriginRot,
+                                  static_cast<double>(sB[0]) / M.scale, static_cast<double>(sB[2]) / M.scale, simq, M.sync_root_pos != 0, M.sync_root_rot != 0);
                 }
                 const double ctrl_time = tm[kTCtrl] + dt;
                 if (need_action) tm[kTPrevAct] = ctrl_time;
@@ -1485,7 +1447,7 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
             }
             const float kp = LKo[kLKp], kd = LKo[kLKd];
             const float pe0 = kp * e0, pe1 = kp * e1, pe2 = kp * e2;
-            const float3 qdd = aba_solve<W, DEBUG>(pe0 - kd * jv.x, pe1 - kd * jv.y, pe2 - kd * jv.z, fdt * kd, 0, jv.x, jv.y, jv.z, nullptr);
+            const float3 qdd = aba_solve<W>(pe0 - kd * jv.x, pe1 - kd * jv.y, pe2 - kd * jv.z, fdt * kd, 0, jv.x, jv.y, jv.z);
             // ---------------- torques: tau = Kp e + Kd (edot - dt a), clamped by norm (cSimBodyJoint::ClampTotalTorque, SimBodyJoint.cpp:299-307)
             float t0 = 0, t1 = 0, t2 = 0;
             if (ndof >= 1) t0 = pe0 + kd * (-jv.x - fdt * qdd.x);
@@ -1493,16 +1455,10 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
             const float mag = sqrtf(t0 * t0 + t1 * t1 + t2 * t2), tlim = LKo[kLTl];
             if (mag > tlim) { float s = tlim / mag; t0 *= s; t1 *= s; t2 *= s; }
             tau0 = t0; tau1 = t1; tau2 = t2;
-            if (DEBUG && dbg && first_upd) {
-                if (ndof >= 1) { dbg[2 * kMaxDofs + dof0] = t0; dbg[3 * kMaxDofs + dof0] = qdd.x; }
-                if (ndof == 3) { dbg[2 * kMaxDofs + dof0 + 1] = t1; dbg[2 * kMaxDofs + dof0 + 2] = t2; dbg[3 * kMaxDofs + dof0 + 1] = qdd.y; dbg[3 * kMaxDofs + dof0 + 2] = qdd.z; }
-                if (lane == 0) for (int k = 0; k < 6; ++k) dbg[2 * kMaxDofs + k] = 0.f;
-            }
             PROF(4);
             continue;
         }
         // =================================================================== Bullet sub-step
-        const int sub = ph - 1;
         int P;
         {
             const int r = collide<W>(mani, alive ? 1 : 0, mcnt);
@@ -1510,9 +1466,7 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
         }
         PROF(3);
         {   // unconstrained accelerations, v += a h (the base and the link velocities are advanced inside)
-            float* dacc = (DEBUG && dbg && first_upd) ? dbg + (sub == 0 ? 4 * kMaxDofs : 8 * kMaxDofs + 1024) : nullptr;
-            const float3 qdd = aba_solve<W, DEBUG>(tau0, tau1, tau2, 0.f, 1, jv.x, jv.y, jv.z, dacc);
-            if (DEBUG && dacc) { if (ndof >= 1) dacc[dof0] = qdd.x; if (ndof == 3) { dacc[dof0 + 1] = qdd.y; dacc[dof0 + 2] = qdd.z; } }
+            const float3 qdd = aba_solve<W>(tau0, tau1, tau2, 0.f, 1, jv.x, jv.y, jv.z);
             bool hit = false;   // a generalised velocity reached Bullet's clamp: the link velocities must be rebuilt from the clamped values
             if (ndof >= 1) { const float v = jv.x + h * qdd.x; jv.x = cl100(v); hit |= fabsf(v) > 100.f; }
             if (ndof == 3) { const float v1 = jv.y + h * qdd.y, v2 = jv.z + h * qdd.z; jv.y = cl100(v1); jv.z = cl100(v2); hit |= fabsf(v1) > 100.f || fabsf(v2) > 100.f; }
@@ -1521,12 +1475,6 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
             if (hb != 0u) {
                 const unsigned hseg = (W == 32) ? hb : ((hb >> (threadIdx.x & 16)) & 0xffffu);
                 vel_pass<W>(jv.x, jv.y, jv.z, hseg != 0u);
-            }
-            if (DEBUG && dbg && first_upd) {
-                const int o = (sub == 0 ? 5 * kMaxDofs : 9 * kMaxDofs + 1024);
-                if (lane == 0) { for (int k = 0; k < 6; ++k) dbg[o + k] = sB[7 + k]; dbg[(sub == 0 ? 7 * kMaxDofs : 11 * kMaxDofs + 1024)] = static_cast<float>(P); }
-                if (ndof >= 1) dbg[o + dof0] = jv.x;
-                if (ndof == 3) { dbg[o + dof0 + 1] = jv.y; dbg[o + dof0 + 2] = jv.z; }
             }
         }
         PROF(4);
@@ -1561,21 +1509,7 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
                 if (ndof >= 1) jv.x = cl100(jv.x + dq.x);
                 if (ndof == 3) { jv.y = cl100(jv.y + dq.y); jv.z = cl100(jv.z + dq.z); }
             }
-            if (DEBUG && dbg && first_upd) {   // solver rows in solver order: right-hand side, 1 / A_ii, impulse (test hook)
-                const float2* sRI_ = reinterpret_cast<const float2*>(E + LY.oRhs);
-                for (int k = lane; k < NR && k < 64; k += W) { float* o = dbg + 8 * kMaxDofs + sub * 256; o[k] = sRI_[k].x; o[64 + k] = sRI_[k].y; o[128 + k] = sLam[k]; }
-            }
-            if (DEBUG && dbg && first_upd) {   // impulses in the order [normals | friction pairs | limits]
-                const int lo_ = (sub == 0 ? 7 * kMaxDofs : 11 * kMaxDofs + 1024) + 1;
-                for (int k = lane; k < NR && k < 60; k += W) { const int src = (k < 3 * P) ? NL + k : k - 3 * P; dbg[lo_ + k] = sLam[src]; }
-            }
             PROF(11);
-        }
-        if (DEBUG && dbg && first_upd) {
-            const int o = (sub == 0 ? 6 * kMaxDofs : 10 * kMaxDofs + 1024);
-            if (lane == 0) for (int k = 0; k < 6; ++k) dbg[o + k] = sB[7 + k];
-            if (ndof >= 1) dbg[o + dof0] = jv.x;
-            if (ndof == 3) { dbg[o + dof0 + 1] = jv.y; dbg[o + dof0 + 2] = jv.z; }
         }
         // ---- integrate positions (btMultiBody::stepPositionsMultiDof)
         if (lane == 0) {
@@ -1592,20 +1526,14 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
     }
 #ifdef DM_PROFILE
     __syncwarp();
-    if ((threadIdx.x & 31) == 0 && st.pdbg) { unsigned int* o = reinterpret_cast<unsigned int*>(st.pdbg) + (blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32) * 16; for (int k = 0; k < 16; ++k) o[k] = PRF[k]; }
+    if ((threadIdx.x & 31) == 0 && st.prof) { unsigned int* o = st.prof + (blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32) * kProfCounters; for (int k = 0; k < kProfCounters; ++k) o[k] = PRF[k]; }
 #endif
 }
 
-// explicit instantiations used by capi.cu: (tile width, debug dumps)
-template __global__ void dm_step_kernel<16, false, 0>(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout, int);
-template __global__ void dm_step_kernel<32, false, 0>(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout, int);
-template __global__ void dm_step_kernel<16, true, 0>(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout, int);
-template __global__ void dm_step_kernel<32, true, 0>(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout, int);
-// AMP task scenes (target_amp / heading_amp): same step with the task block advanced after every update
-template __global__ void dm_step_kernel<16, false, kVarTask>(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout, int);
-template __global__ void dm_step_kernel<32, false, kVarTask>(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout, int);
-// --sync_char_root_rot true (dog3d_spin)
-template __global__ void dm_step_kernel<16, false, kVarRootRot>(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout, int);
-template __global__ void dm_step_kernel<32, false, kVarRootRot>(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout, int);
+// explicit instantiations used by capi.cu: (tile width, AMP task scene)
+template __global__ void dm_step_kernel<16, false>(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout);
+template __global__ void dm_step_kernel<32, false>(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout);
+template __global__ void dm_step_kernel<16, true>(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout);
+template __global__ void dm_step_kernel<32, true>(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout);
 
 }  // namespace dmk

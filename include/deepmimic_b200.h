@@ -183,8 +183,10 @@ void dm_mlp_destroy(dm_mlp* m);
  *  [29 + 55nl + 4j ..] PD target of joint j in DeepMimic joint-frame convention (w,x,y,z or angle) */
 int dm_get_snapshot(dm_handle* h, int env, double* h_out);
 int dm_set_snapshot(dm_handle* h, int env, const double* h_in);
-int dm_debug_enable(dm_handle* h, int on);                     /* test hook: per-env stage dumps of the first update of each launch */
-int dm_get_debug(dm_handle* h, int env, float* h_out);        /* 8*96 + 2048 floats, layout in kernels/dm_update.cu */
+/* profile build only (DM_PROFILE, `make -C deepmimic_b200/csrc profile`; fails in a normal build): per-warp cycle counters by code section of the
+ * last dm_update's step kernel, 16 uint32 per warp, block-major ([num_blocks][warps_per_block][16], tools/section_profile.py names them).
+ * h_out may be NULL to query the two sizes only. */
+int dm_get_section_profile(dm_handle* h, uint32_t* h_out, int* num_blocks, int* warps_per_block);
 int dm_get_counters(dm_handle* h, int64_t* h_out);           /* {kernel launches so far, row-capacity overflows seen (must stay 0)} */
 
 #ifdef __cplusplus

@@ -29,7 +29,7 @@ double shim_reward(const double* p, const double* t, int fallen, double root_x, 
     return task_reward(static_cast<int>(p[0]), params_from(p), t, fallen != 0, root_x, root_z, step_dur);
 }
 int shim_task_doubles() { return kTaskDoubles; }
-// cSceneImitate::SyncKinCharNewCycle as the kVarRootRot instantiation of dm_step_kernel runs it
+// cSceneImitate::SyncKinCharNewCycle as dm_step_kernel runs it at a clip wrap
 void shim_wrap_sync(const double* frame_times, const float* frames, int pose_dim, int num_frames, const float* cycle_delta, double dur, double kin_time,
                     double* origin, double* origin_rot, double sim_x, double sim_z, const double* sim_quat, int sync_pos, int sync_rot) {
     kin_wrap_sync(frame_times, frames, pose_dim, num_frames, cycle_delta, dur, kin_time, origin, origin_rot, sim_x, sim_z, sim_quat, sync_pos != 0, sync_rot != 0);

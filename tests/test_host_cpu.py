@@ -78,7 +78,9 @@ def test_loader_errors_are_reported(asset_root):
         capi.HostModel(["--scene", "dribble_amp", "--arg_file", ARG_FILES[0]], asset_root)     # first key wins: the scene is overridden
     for extra, msg in ((["--char_ctrls", "ct_vel"], "Unsupported character controller"), (["--enable_char_soft_contact", "true"], "enable_char_soft_contact"),
                        (["--enable_root_rot_fail", "true"], "enable_root_rot_fail"), (["--char_types", "biped3d"], "Unsupported character type"),
-                       (["--character_files", "data/characters/humanoid3d.txt", "data/characters/dog3d.txt"], "more than one character")):
+                       (["--character_files", "data/characters/humanoid3d.txt", "data/characters/dog3d.txt"], "more than one character"),
+                       (["--sync_char_root_rot", "true", "--motion_file", "data/datasets/test_clips_mini.txt", "--arg_file",
+                         "args/train_amp_target_humanoid3d_locomotion_args.txt"], "sync_char_root_rot true in an AMP task scene")):
         with pytest.raises(RuntimeError, match=msg):
             capi.HostModel(extra + ["--arg_file", ARG_FILES[0]], asset_root)
     with pytest.raises(RuntimeError, match="Unsupported timer type"):

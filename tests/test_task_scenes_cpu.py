@@ -430,7 +430,7 @@ def test_unvalidated_task_scenes_stay_refused_without_the_opt_in(asset_root, mon
 
 @pytest.mark.parametrize("sync_rot", [True, False])
 def test_device_clip_wrap_sync_matches_the_oracle_on_the_host(asset_root, task_shim, sync_rot):
-    """kin_wrap_sync (dm_task.cuh; what dm_step_kernel<.., kVarRootRot> runs at a clip wrap) against the oracle's SyncKinCharNewCycle: the
+    """kin_wrap_sync (dm_task.cuh; what dm_step_kernel runs at a clip wrap) against the oracle's SyncKinCharNewCycle: the
     character is turned by 0.7 rad and drifts until the walk clip wraps; the routine gets the pre-update clocks, origin and simulated base
     state from the oracle's snapshot and the fp32 clip table the device holds, and must reproduce the oracle's origin after that update."""
     import ctypes as C

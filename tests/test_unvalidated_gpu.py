@@ -4,8 +4,7 @@ round 2 (tests/test_task_scenes_gpu.py, tests/test_parity2_gpu.py).
 
 OPT-IN: the device half of the task scenes (dm_task.cuh inside dm_step_kernel<.., TASK>, dm_task_reset_kernel, dm_task_observe_kernel) was
 written after round 1's GPU budget was spent and has never run on hardware.  dm_create refuses the scenes unless
-DM_EXPERIMENTAL_TASK_SCENES=1; --sync_char_root_rot needs DM_EXPERIMENTAL_ROOT_ROT_SYNC=1 (dm_step_kernel<.., kVarRootRot>);
-these tests additionally need DM_RUN_UNVALIDATED_GPU_TESTS=1 so that the default `pytest -m gpu` run only
+DM_EXPERIMENTAL_TASK_SCENES=1; these tests additionally need DM_RUN_UNVALIDATED_GPU_TESTS=1 so that the default `pytest -m gpu` run only
 contains tests of code that has been validated on hardware.  To validate: run with both variables set, fix what breaks, then drop the gates."""
 import os
 

@@ -21,14 +21,12 @@ with torch.cuda.stream(stream):
     for step in range(int(os.environ.get("PROF_PREROLL", "52"))):   # bench.py's preroll + warm-up: the steady-state mix of the 8(d) workload
         a = torch.clamp(-off + 0.25 / scl * torch.randn(N, A, device="cuda", generator=g), lo, hi).contiguous()
         core.set_action(a); core.update(1 / 600., 20); core.reset(False)
-    core.debug_enable(True)
     a = torch.clamp(-off + 0.25 / scl * torch.randn(N, A, device="cuda", generator=g), lo, hi).contiguous()
     core.set_action(a); core.update(1 / 600., 20)
 core.sync()
-buf = np.concatenate([core.get_debug(e).view(np.uint32) for e in range(14)])
-warps_per_block = 14
-nblocks = (N + 27) // 28
-d = buf[: nblocks * warps_per_block * 16].reshape(nblocks, warps_per_block, 16).astype(np.float64)
+d = core.section_profile().astype(np.float64)   # [blocks, warps per block, 16] counters of the last launch
+nblocks, warps_per_block = d.shape[:2]
+print("%d blocks of %d warps" % (nblocks, warps_per_block))
 names = ["kin", "flags", "sync", "clock/collide", "ab+up", "base", "descend(+torque/vel)", "limits+publish", "rows", "Abuild", "warm+PGS", "z+down", "integrate"]
 tot = d[:, :, :13].sum(axis=2)
 print("cycles per launch (20 updates): mean warp %.0f, mean of slowest warp per block %.0f, max %.0f" % (tot.mean(), tot.max(axis=1).mean(), tot.max()))
@@ -48,7 +46,7 @@ print("busiest warp per block: constraint sub-steps %.1f of 40, mean max-rows pe
 sr = d[:, :, 10]
 print("solve_rows cycles per call: busiest %.0f, all %.0f" % ((sr[np.arange(nblocks), busy] / np.maximum(1, nr_cnt[np.arange(nblocks), busy])).mean(), sr.sum() / max(1, nr_cnt.sum())))
 
-# ---- where does the single wave end?  kernel time = the slowest block; a block's time = sum over updates of its slowest warp (per-update barrier)
+# ---- where does the single wave end?  kernel time = the slowest block; a block's time = sum over stages of its slowest warp (barrier after every stage)
 bt = tot.max(axis=1)
 print("block time (max warp incl. barrier wait) percentiles: p10 %.0f p50 %.0f p90 %.0f p99 %.0f max %.0f ; mean/max = %.2f" % (
     np.percentile(bt, 10), np.percentile(bt, 50), np.percentile(bt, 90), np.percentile(bt, 99), bt.max(), bt.mean() / bt.max()))
