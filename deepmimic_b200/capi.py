@@ -15,11 +15,23 @@ class DmDims(C.Structure):
                                         "updates_per_action", "num_update_substeps")] + [("motion_duration", C.c_double), ("amp_obs_size", C.c_int)]
 
 
+_fp = C.POINTER(C.c_float)
+
+
+class DmMlpGatedWeights(C.Structure):
+    """dm_mlp_gated_weights of include/deepmimic_b200.h"""
+    _fields_ = ([(n, C.c_int) for n in ("in_dim", "goal_dim", "h0", "h1", "out_dim", "gate_common", "gate_hidden")]
+                + [(n, _fp) for n in ("w0", "b0", "w1", "b1", "w2", "b2", "gc_w", "gc_b")]
+                + [(n, _fp * 2) for n in ("gh_w", "gh_b", "gs_w", "gs_b", "gb_w", "gb_b")]
+                + [(n, _fp) for n in ("s_mean", "s_std", "g_mean", "g_std", "a_mean", "a_std")] + [("s_clip", C.c_float), ("g_clip", C.c_float)])
+
+
 DM_STATE_OFFSET, DM_STATE_SCALE, DM_ACTION_OFFSET, DM_ACTION_SCALE, DM_ACTION_BOUND_MIN, DM_ACTION_BOUND_MAX, DM_STATE_NORM_GROUPS = range(7)
 
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
            "dm_update", "dm_record_state", "dm_record_goal", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
-           "dm_set_snapshot", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_launches", "dm_mlp_destroy"]
+           "dm_set_snapshot", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
+           "dm_mlp_launches", "dm_mlp_destroy"]
 
 
 def lib():
@@ -87,6 +99,9 @@ def lib():
         L.dm_mlp_create.restype = vp
         L.dm_mlp_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, fpp, fpp, fpp, fpp, fpp, fpp, fpp, fpp, C.c_float, fpp, fpp, C.c_int]
         L.dm_mlp_forward.argtypes = [vp, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+        L.dm_mlp_create_gated.restype = vp
+        L.dm_mlp_create_gated.argtypes = [C.c_int, C.POINTER(DmMlpGatedWeights), C.c_int]
+        L.dm_mlp_forward_gated.argtypes = [vp, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.dm_mlp_launches.restype = C.c_longlong
         L.dm_mlp_launches.argtypes = [vp]
         L.dm_mlp_destroy.argtypes = [vp]
@@ -403,6 +418,61 @@ class TensorCoreMLP:
                                   C.c_void_p(stream) if stream else None)
         if rc != 0:
             raise RuntimeError("dm_mlp_forward: %s" % lib().dm_last_error().decode())
+        return actions
+
+    def launches(self):
+        return int(lib().dm_mlp_launches(self.h))
+
+    def close(self):
+        if self.h:
+            lib().dm_mlp_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class TensorCoreGatedMLP:
+    """dm_mlp_* handle of the gated (goal-conditioned) actor of the AMP task scenes, fc_2layers_gated_1024units, on the tensor cores (wgmma).
+    actor: the reference's layout (deepmimic_b200.tf_checkpoint.load_actor, tests.test_task_scenes_cpu.fixture_task_actor): hidden [(w, b)] x 2,
+    mean (w, b), gate_common (w, b), gates [dict(hidden=(w, b), scale=(w, b), bias=(w, b))] x 2; dense kernels are [inputs x units] arrays."""
+
+    def __init__(self, actor, s_mean=None, s_std=None, s_clip=float("inf"), g_mean=None, g_std=None, g_clip=float("inf"), a_mean=None, a_std=None,
+                 max_rows=4096, device=0):
+        L = lib()
+        f = lambda a: None if a is None else np.ascontiguousarray(a, dtype=np.float32)
+        hidden, gates = actor["hidden"], actor["gates"]
+        if len(hidden) != 2 or len(gates) != 2:
+            raise ValueError("the tensor-core gated actor implements exactly two hidden layers (got %d, %d gates)" % (len(hidden), len(gates)))
+        (w0, b0), (w1, b1), (w2, b2), (gcw, gcb) = [(f(w), f(b)) for w, b in list(hidden) + [actor["mean"], actor["gate_common"]]]
+        gh, gs, gb = ([(f(g[k][0]), f(g[k][1])) for g in gates] for k in ("hidden", "scale", "bias"))
+        norms = [f(x) for x in (s_mean, s_std, g_mean, g_std, a_mean, a_std)]
+        self.goal_dim, gate_common = gcw.shape
+        self.in_dim, self.out_dim = w0.shape[0] - self.goal_dim, w2.shape[1]
+        gate_hidden = gh[0][0].shape[1]
+        p = lambda a: None if a is None else a.ctypes.data_as(_fp)
+        pair = lambda ab, i: (_fp * 2)(p(ab[0][i]), p(ab[1][i]))
+        W = DmMlpGatedWeights(self.in_dim, self.goal_dim, w0.shape[1], w1.shape[1], self.out_dim, gate_common, gate_hidden,
+                              p(w0), p(b0), p(w1), p(b1), p(w2), p(b2), p(gcw), p(gcb),
+                              pair(gh, 0), pair(gh, 1), pair(gs, 0), pair(gs, 1), pair(gb, 0), pair(gb, 1),
+                              *[p(a) for a in norms], 0.0 if not np.isfinite(s_clip) else float(s_clip), 0.0 if not np.isfinite(g_clip) else float(g_clip))
+        self.h = L.dm_mlp_create_gated(device, C.byref(W), max_rows)
+        if not self.h:
+            raise RuntimeError("dm_mlp_create_gated failed: %s" % L.dm_last_error().decode())
+        self.h = C.c_void_p(self.h)
+        self.max_rows = max_rows
+
+    def forward(self, obs, goal, actions, noise=None, stream=None):
+        """obs [rows, in_dim], goal [rows, goal_dim], actions [rows, out_dim] (written), noise [rows, out_dim] or None: contiguous float32 CUDA
+        tensors; stream: cudaStream_t handle (int) or None"""
+        rows = obs.shape[0]
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+        rc = lib().dm_mlp_forward_gated(self.h, ptr(obs), ptr(goal), ptr(noise), ptr(actions), rows, C.c_void_p(stream) if stream else None)
+        if rc != 0:
+            raise RuntimeError("dm_mlp_forward_gated: %s" % lib().dm_last_error().decode())
         return actions
 
     def launches(self):

@@ -14,6 +14,10 @@
 //     rounding beyond the fp32 reference is the fp16 rounding of the activations (measured action error < 1e-3, tests/test_mlp_gpu.py),
 //   * epilogue straight from the accumulator registers: bias, ReLU, fp16 pairs into the next layer's operand tiles (a warp's store covers one
 //     128-byte core matrix); the last layer adds the exploration noise and un-normalises into the DeepMimic action layout (fp32).
+// The gated actor of the AMP task scenes (R/learning/nets/fc_2layers_gated_1024units.py) reuses these pieces: the preparation kernel also writes
+// the normalised goal (into the trunk's columns after the state, and alone as the gate trunk's operand), the gate trunk and both gate hidden
+// layers are launches of the 128-column kernel, and each trunk layer is a GATED instantiation whose pipeline appends the gate's scale and bias
+// chunks (DESIGN.md section 8).
 // This is the one dense contraction next to the hot path (the simulation itself has none); it replaces cuBLAS / eager torch in the rollout shim.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -36,6 +40,14 @@ struct MlpPrepParams {
     float in_clip;
     int in_dim, M, NC;         // NC = padded K / 64
     __half* tiles;             // [m tiles][NC][kMlpATile]
+    // gated actor only: the goal, normalised with its own statistics, fills the trunk columns [in_dim, in_dim + goal_dim) and, alone, the
+    // gate trunk's 64-wide operand tile (written by the extra chunk blockIdx.y == NC)
+    const float* goal;         // [M x goal_dim] fp32
+    const float* g_mean;
+    const float* g_istd;
+    float g_clip;
+    int goal_dim;
+    __half* g_tiles;           // [m tiles][kMlpATile]
 };
 struct MlpGemmParams {
     const __half* a_tiles;     // [m tiles][K / 64][kMlpATile] fp16 activations in operand layout
@@ -48,6 +60,14 @@ struct MlpGemmParams {
     const float* noise;        // LAST, optional: [M x out_dim] added in normalised action space (exploration), may be null
     int out_dim;
     int M, K, N;               // rows, padded K (multiple of 64), padded N (multiple of BN)
+    // gated trunk layer only: two more K-chunks after the trunk's, both with this layer's gate-hidden chunk as A, against the gate's scale and
+    // bias weights; the epilogue is relu(2 sigmoid(acc_s + bias_s) (acc + bias) + acc_b + bias_b)
+    const __half* gate_tiles;  // A of the gate chunks: m tile t at gate_tiles + t * gate_stride
+    const __half* ws_tiles;    // [n tiles][1][hi | lo][BN x 64]
+    const __half* wb_tiles;
+    const float* bias_s;       // [N padded]
+    const float* bias_b;
+    int gate_stride;           // halves
 };
 
 namespace {
@@ -89,11 +109,14 @@ __device__ __forceinline__ void fence_acc(float& r) { asm volatile("" : "+f"(r):
 
 }  // namespace
 
-// Observations -> normalised, clipped fp16 activations in operand layout.  grid = (m tiles, K chunks), 128 threads: 8 consecutive threads cover
-// 64 consecutive inputs of one row (coalesced 256-byte reads), a thread writes one 16-byte core-matrix row.
-__global__ void __launch_bounds__(kMlpThreads) dm_mlp_prep_kernel(MlpPrepParams P) {
-    const int m0 = blockIdx.x * kMlpBM, c = blockIdx.y;
-    __half* tile = P.tiles + (static_cast<size_t>(blockIdx.x) * P.NC + c) * kMlpATile;
+// Observations -> normalised, clipped fp16 activations in operand layout.  grid = (m tiles, K chunks [+ 1 for the goal's own tile]), 128 threads:
+// 8 consecutive threads cover 64 consecutive inputs of one row (coalesced 256-byte reads), a thread writes one 16-byte core-matrix row.
+template <bool GOAL>
+__device__ __forceinline__ void mlp_prep(const MlpPrepParams& P) {
+    const int m0 = blockIdx.x * kMlpBM;
+    const bool gate = GOAL && blockIdx.y == P.NC;   // the gate trunk's operand: the normalised goal from column 0
+    const int c = gate ? 0 : blockIdx.y;
+    __half* tile = gate ? P.g_tiles + static_cast<size_t>(blockIdx.x) * kMlpATile : P.tiles + (static_cast<size_t>(blockIdx.x) * P.NC + c) * kMlpATile;
 #pragma unroll
     for (int i = 0; i < (kMlpBM * 8) / kMlpThreads; ++i) {
         const int u = threadIdx.x + i * kMlpThreads, row = u >> 3, k8 = u & 7;
@@ -102,9 +125,15 @@ __global__ void __launch_bounds__(kMlpThreads) dm_mlp_prep_kernel(MlpPrepParams 
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
             float x = 0.f;
-            if (grow < P.M && k + e < P.in_dim) {
+            if (grow < P.M && !gate && k + e < P.in_dim) {
                 x = (P.obs[static_cast<size_t>(grow) * P.in_dim + k + e] - P.in_mean[k + e]) * P.in_istd[k + e];
                 x = fminf(fmaxf(x, -P.in_clip), P.in_clip);
+            } else if (GOAL && grow < P.M) {
+                const int j = gate ? k + e : k + e - P.in_dim;
+                if (j < P.goal_dim) {
+                    x = (P.goal[static_cast<size_t>(grow) * P.goal_dim + j] - P.g_mean[j]) * P.g_istd[j];
+                    x = fminf(fmaxf(x, -P.g_clip), P.g_clip);
+                }
             }
             h[e] = __float2half_rn(x);
         }
@@ -112,20 +141,28 @@ __global__ void __launch_bounds__(kMlpThreads) dm_mlp_prep_kernel(MlpPrepParams 
     }
 }
 
+__global__ void __launch_bounds__(kMlpThreads) dm_mlp_prep_kernel(MlpPrepParams P) { mlp_prep<false>(P); }
+// [normalised state | normalised goal] trunk tiles, and the normalised goal's own tile
+__global__ void __launch_bounds__(kMlpThreads) dm_mlp_gated_prep_kernel(MlpPrepParams P) { mlp_prep<true>(P); }
+
 // C[M x N] = act(A[M x K] W + b); grid = (M / 128, N / BN), block = 256 threads (two warpgroups),
-// dynamic shared memory = 2 stages x (A 16 KB + W hi/lo 2 x BN x 128 B) + 1 KB (barriers)
-template <int BN, bool LAST>
-__global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_gemm_kernel(MlpGemmParams P) {
+// dynamic shared memory = 2 stages x (A 16 KB + W hi/lo 2 x BN x 128 B) + 1 KB (barriers).
+// GATED (a hidden layer of the gated actor): two more pipeline chunks after the K loop (MlpGemmParams::gate_tiles) accumulate the gate's scale
+// and bias pre-activations in registers of their own; with BN = 64 that is 3 x 32 accumulator registers per thread.
+template <int BN, bool LAST, bool GATED>
+__device__ __forceinline__ void mlp_gemm(const MlpGemmParams& P) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     constexpr int kABytes = kMlpATile * 2;               // 16 KB
     constexpr int kWBytes = 2 * BN * kMlpBK * 2;         // hi + lo
     constexpr int kStage = kABytes + kWBytes;
     constexpr int NH = BN / 64;                          // 64-column accumulators per warpgroup
+    static_assert(!GATED || (!LAST && NH == 1), "the gated epilogue is written for one 64-column accumulator of a hidden layer");
     uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem_raw + kMlpStages * kStage);   // [stages] both operands of the stage have landed
     uint64_t* bar_empty = bar_full + kMlpStages;                                         // [stages] every thread's MMAs reading the stage have completed
     const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127;
     const int mt = blockIdx.x, m0 = mt * kMlpBM, nt = blockIdx.y, n0 = nt * BN;
     const int NC = P.K / kMlpBK;
+    const int NT = GATED ? NC + 2 : NC;                  // pipeline chunks: the K loop, then the gate's scale and bias chunks
     const __half* a_src = P.a_tiles + static_cast<size_t>(mt) * NC * kMlpATile;
     const __half* w_src = P.w_tiles + static_cast<size_t>(nt) * NC * (kWBytes / 2);
     // one bulk copy per operand and K-chunk (both are contiguous blocks in operand layout)
@@ -133,6 +170,11 @@ __global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_gemm_kernel(MlpGemm
         const int s = c % kMlpStages;
         uint8_t* sA = smem_raw + s * kStage;
         mbar_expect_tx(&bar_full[s], kStage);
+        if (GATED && c >= NC) {
+            bulk_g2s(sA, P.gate_tiles + static_cast<size_t>(mt) * P.gate_stride, kABytes, &bar_full[s]);
+            bulk_g2s(sA + kABytes, (c == NC ? P.ws_tiles : P.wb_tiles) + static_cast<size_t>(nt) * (kWBytes / 2), kWBytes, &bar_full[s]);
+            return;
+        }
         bulk_g2s(sA, a_src + static_cast<size_t>(c) * kMlpATile, kABytes, &bar_full[s]);
         bulk_g2s(sA + kABytes, w_src + static_cast<size_t>(c) * (kWBytes / 2), kWBytes, &bar_full[s]);
     };
@@ -141,18 +183,18 @@ __global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_gemm_kernel(MlpGemm
 #pragma unroll
         for (int s = 0; s < kMlpStages; ++s) { mbar_init(&bar_full[s], 1); mbar_init(&bar_empty[s], kMlpGemmThreads); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        for (int c = 0; c < NC && c < kMlpStages; ++c) load(c);
+        for (int c = 0; c < NT && c < kMlpStages; ++c) load(c);
     }
     __syncthreads();
 
-    float acc[NH][32];
+    float acc[NH][32], acc_s[NH][32], acc_b[NH][32];     // acc_s / acc_b: GATED only
 #pragma unroll
     for (int h = 0; h < NH; ++h)
 #pragma unroll
-        for (int i = 0; i < 32; ++i) acc[h][i] = 0.f;
+        for (int i = 0; i < 32; ++i) acc[h][i] = acc_s[h][i] = acc_b[h][i] = 0.f;
     constexpr uint32_t kALbo = (kMlpBM / 8) * 128, kBLbo = (BN / 8) * 128;
-#pragma unroll 1
-    for (int c = 0; c < NC; ++c) {
+    // MMAs of pipeline chunk c into d, then release its stage and refill it with chunk c + 2
+    auto mma_chunk = [&](int c, float (&d)[NH][32]) {
         const int s = c % kMlpStages;
         mbar_wait(&bar_full[s], (c / kMlpStages) & 1);
         // this warpgroup's 64 rows start 8 row groups (1 KB) into each K slice of the A tile; columns [64 h, 64 h + 64) likewise in W
@@ -160,7 +202,7 @@ __global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_gemm_kernel(MlpGemm
 #pragma unroll
         for (int h = 0; h < NH; ++h)
 #pragma unroll
-            for (int i = 0; i < 32; ++i) fence_acc(acc[h][i]);
+            for (int i = 0; i < 32; ++i) fence_acc(d[h][i]);
         asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
         for (int j = 0; j < kMlpBK / 16; ++j) {
@@ -168,8 +210,8 @@ __global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_gemm_kernel(MlpGemm
 #pragma unroll
             for (int h = 0; h < NH; ++h) {
                 const uint32_t bh = b0 + h * 1024 + j * 2 * kBLbo;
-                wgmma_64x64x16(acc[h], ad, wgmma_desc(bh, kBLbo, 128), 1u);
-                wgmma_64x64x16(acc[h], ad, wgmma_desc(bh + BN * kMlpBK * 2, kBLbo, 128), 1u);
+                wgmma_64x64x16(d[h], ad, wgmma_desc(bh, kBLbo, 128), 1u);
+                wgmma_64x64x16(d[h], ad, wgmma_desc(bh + BN * kMlpBK * 2, kBLbo, 128), 1u);
             }
         }
         asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
@@ -177,13 +219,19 @@ __global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_gemm_kernel(MlpGemm
 #pragma unroll
         for (int h = 0; h < NH; ++h)
 #pragma unroll
-            for (int i = 0; i < 32; ++i) fence_acc(acc[h][i]);
+            for (int i = 0; i < 32; ++i) fence_acc(d[h][i]);
         mbar_arrive(&bar_empty[s]);
-        if (tid == 0 && c + kMlpStages < NC) {
+        if (tid == 0 && c + kMlpStages < NT) {
             mbar_wait(&bar_empty[s], (c / kMlpStages) & 1);
             load(c + kMlpStages);
         }
         __syncwarp();
+    };
+#pragma unroll 1
+    for (int c = 0; c < NC; ++c) mma_chunk(c, acc);
+    if constexpr (GATED) {
+        mma_chunk(NC, acc_s);
+        mma_chunk(NC + 1, acc_b);
     }
 
     // ---- epilogue from the accumulator fragments: register i of accumulator h holds row 16 w + lane / 4 (+ 8 for i & 2) of the warpgroup's
@@ -195,7 +243,8 @@ __global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_gemm_kernel(MlpGemm
         for (int q = 0; q < 16; ++q) {
             const int r = wg * 64 + warp * 16 + (lane >> 2) + 8 * (q & 1), row = m0 + r;
             const int n = n0 + h * 64 + 8 * (q >> 1) + 2 * (lane & 3);
-            const float v0 = acc[h][4 * (q >> 1) + 2 * (q & 1)], v1 = acc[h][4 * (q >> 1) + 2 * (q & 1) + 1];
+            const int i0 = 4 * (q >> 1) + 2 * (q & 1);
+            const float v0 = acc[h][i0], v1 = acc[h][i0 + 1];
             if constexpr (LAST) {
                 if (row < P.M) {
 #pragma unroll
@@ -210,13 +259,27 @@ __global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_gemm_kernel(MlpGemm
                 }
             } else {
                 // next layer's operand tiles: K index = this layer's column; rows past M carry relu(bias) (never read back as results)
-                const __half2 hv = __floats2half2_rn(fmaxf(v0 + P.bias[n], 0.f), fmaxf(v1 + P.bias[n + 1], 0.f));
+                __half2 hv;
+                if constexpr (GATED) {
+                    auto gated = [&](float v, int i, int ne) {
+                        const float scale = 2.f / (1.f + __expf(-(acc_s[h][i] + P.bias_s[ne])));
+                        return fmaxf(scale * (v + P.bias[ne]) + acc_b[h][i] + P.bias_b[ne], 0.f);
+                    };
+                    hv = __floats2half2_rn(gated(v0, i0, n), gated(v1, i0 + 1, n + 1));
+                } else {
+                    hv = __floats2half2_rn(fmaxf(v0 + P.bias[n], 0.f), fmaxf(v1 + P.bias[n + 1], 0.f));
+                }
                 __half* tile = P.out_tiles + (static_cast<size_t>(mt) * (P.N >> 6) + (n >> 6)) * kMlpATile;
                 *reinterpret_cast<__half2*>(tile + ((((n & 63) >> 3) * (kMlpBM / 8) + (r >> 3)) * 64 + (r & 7) * 8 + (n & 7))) = hv;
             }
         }
     }
 }
+
+template <int BN, bool LAST>
+__global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_gemm_kernel(MlpGemmParams P) { mlp_gemm<BN, LAST, false>(P); }
+// a hidden layer of the gated actor, 64-column tiles
+__global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_gated_gemm_kernel(MlpGemmParams P) { mlp_gemm<64, false, true>(P); }
 
 int dm_mlp_smem_bytes(int bn) { return kMlpStages * (kMlpATile * 2 + 2 * bn * kMlpBK * 2) + 1024; }
 

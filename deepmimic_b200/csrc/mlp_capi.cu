@@ -1,5 +1,6 @@
-// C ABI of the tensor-core policy network (include/deepmimic_b200.h, dm_mlp_*): host-side weight tiling + the four launches (operand preparation, three GEMMs) of
-// kernels/dm_mlp.cu.  Same library, same rules: no CPU fallback, errors through dm_last_error.
+// C ABI of the tensor-core policy network (include/deepmimic_b200.h, dm_mlp_*): host-side weight tiling + the launches of kernels/dm_mlp.cu: four for
+// the plain actor (operand preparation, three GEMMs), six for the gated one (operand preparation, gate trunk, both gate hidden layers, two gated
+// trunk layers, output layer).  Same library, same rules: no CPU fallback, errors through dm_last_error.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
@@ -12,26 +13,40 @@
 #include "../../include/deepmimic_b200.h"
 
 namespace dmk {
-struct MlpPrepParams { const float* obs; const float* in_mean; const float* in_istd; float in_clip; int in_dim, M, NC; __half* tiles; };
+struct MlpPrepParams {
+    const float* obs; const float* in_mean; const float* in_istd; float in_clip; int in_dim, M, NC; __half* tiles;
+    const float* goal; const float* g_mean; const float* g_istd; float g_clip; int goal_dim; __half* g_tiles;
+};
 struct MlpGemmParams {
     const __half* a_tiles; const __half* w_tiles; const float* bias; __half* out_tiles; float* actions; const float* out_mean; const float* out_std; const float* noise;
     int out_dim; int M, K, N;
+    const __half* gate_tiles; const __half* ws_tiles; const __half* wb_tiles; const float* bias_s; const float* bias_b; int gate_stride;
 };
 __global__ void dm_mlp_prep_kernel(MlpPrepParams);
+__global__ void dm_mlp_gated_prep_kernel(MlpPrepParams);
 template <int BN, bool LAST>
 __global__ void dm_mlp_gemm_kernel(MlpGemmParams);
+__global__ void dm_mlp_gated_gemm_kernel(MlpGemmParams);
 int dm_mlp_smem_bytes(int bn);
+constexpr int kMlpATileHalves = 128 * 64;   // one operand tile of activations (kernels/dm_mlp.cu: kMlpATile)
 }  // namespace dmk
 
 extern "C" void dm_set_last_error(const char* msg);
 
 struct dm_mlp {
     int device = 0, in_dim = 0, h0 = 0, h1 = 0, out_dim = 0, max_rows = 0;
-    int K0 = 0, N0 = 0, N1 = 0, N2 = 64;  // padded sizes: K0 = pad64(in), N0 = pad128(h0) = K1, N1 = pad128(h1) = K2, N2 = 64
+    int K0 = 0, N0 = 0, N1 = 0, N2 = 64;  // padded sizes: K0 = pad64(in), N0 = pad128(h0) = K1, N1 = pad128(h1) = K2, N2 = 64 (gated: K0 = pad64(in + goal), pad64(h))
     __half *w[3] = {nullptr, nullptr, nullptr}, *obs_t = nullptr, *act0 = nullptr, *act1 = nullptr;   // activations: operand tiles [m tiles][K / 64][128 x 64]
     float *b[3] = {nullptr, nullptr, nullptr}, *in_mean = nullptr, *in_istd = nullptr, *out_mean = nullptr, *out_std = nullptr;
     float in_clip = 1e30f;
     long long launches = 0;
+    // gated actor (dm_mlp_create_gated) only: gate trunk (goal -> 128), both gate hidden layers as one 128 -> 128 GEMM (layer l in columns
+    // [64 l, 64 l + 64)), per trunk layer the gate's scale and bias weights (64 -> h_l)
+    bool gated = false;
+    int goal_dim = 0;
+    __half *wgc = nullptr, *wgh = nullptr, *wgs[2] = {nullptr, nullptr}, *wgb[2] = {nullptr, nullptr}, *goal_t = nullptr, *gc_t = nullptr, *gh_t = nullptr;
+    float *bgc = nullptr, *bgh = nullptr, *bgs[2] = {nullptr, nullptr}, *bgb[2] = {nullptr, nullptr}, *g_mean = nullptr, *g_istd = nullptr;
+    float g_clip = 1e30f;
 };
 
 namespace {
@@ -64,6 +79,7 @@ bool upload(T** dst, const std::vector<T>& src) {
     return cudaMemcpy(*dst, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice) == cudaSuccess;
 }
 std::vector<float> padded(const float* v, int n, int N, float fill = 0.f) { std::vector<float> o(N, fill); if (v) std::memcpy(o.data(), v, sizeof(float) * n); return o; }
+std::vector<float> inverse_std(const float* std_dev, int n) { std::vector<float> o(n, 1.f); for (int i = 0; i < n; ++i) o[i] = std_dev ? 1.0f / std_dev[i] : 1.f; return o; }
 }  // namespace
 
 extern "C" {
@@ -81,11 +97,9 @@ dm_mlp* dm_mlp_create(int device, int in_dim, int h0, int h1, int out_dim, const
     m->device = device; m->in_dim = in_dim; m->h0 = h0; m->h1 = h1; m->out_dim = out_dim; m->max_rows = pad_to(max_rows, 128);
     m->K0 = pad_to(in_dim, 64); m->N0 = pad_to(h0, 128); m->N1 = pad_to(h1, 128);
     m->in_clip = in_clip > 0.f ? in_clip : 1e30f;
-    std::vector<float> istd(in_dim, 1.f);
-    for (int i = 0; i < in_dim; ++i) istd[i] = in_std ? 1.0f / in_std[i] : 1.f;
     bool ok = upload(&m->w[0], tile_weights(w0, in_dim, h0, m->K0, m->N0, 128)) && upload(&m->w[1], tile_weights(w1, h0, h1, m->N0, m->N1, 128)) &&
               upload(&m->w[2], tile_weights(w2, h1, out_dim, m->N1, m->N2, m->N2)) && upload(&m->b[0], padded(b0, h0, m->N0)) && upload(&m->b[1], padded(b1, h1, m->N1)) &&
-              upload(&m->b[2], padded(b2, out_dim, m->N2)) && upload(&m->in_mean, padded(in_mean, in_dim, in_dim)) && upload(&m->in_istd, istd) &&
+              upload(&m->b[2], padded(b2, out_dim, m->N2)) && upload(&m->in_mean, padded(in_mean, in_dim, in_dim)) && upload(&m->in_istd, inverse_std(in_std, in_dim)) &&
               upload(&m->out_mean, padded(out_mean, out_dim, out_dim)) && upload(&m->out_std, padded(out_std, out_dim, out_dim, 1.f)) &&
               cudaMalloc(&m->obs_t, static_cast<size_t>(m->max_rows) * m->K0 * sizeof(__half)) == cudaSuccess &&
               cudaMalloc(&m->act0, static_cast<size_t>(m->max_rows) * m->N0 * sizeof(__half)) == cudaSuccess &&
@@ -101,6 +115,7 @@ dm_mlp* dm_mlp_create(int device, int in_dim, int h0, int h1, int out_dim, const
 
 int dm_mlp_forward(dm_mlp* m, const float* d_obs, const float* d_noise, float* d_actions, int rows, void* stream) {
     if (!m) return mlp_fail("dm_mlp_forward: null handle");
+    if (m->gated) return mlp_fail("dm_mlp_forward: the handle holds a gated actor (dm_mlp_create_gated); use dm_mlp_forward_gated");
     if (rows <= 0 || rows > m->max_rows) return mlp_fail("dm_mlp_forward: rows out of range");
     if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_mlp_forward: cudaSetDevice failed");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -126,6 +141,100 @@ int dm_mlp_forward(dm_mlp* m, const float* d_obs, const float* d_noise, float* d
     return 0;
 }
 
+dm_mlp* dm_mlp_create_gated(int device, const dm_mlp_gated_weights* g, int max_rows) {
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { mlp_fail("dm_mlp_create_gated: no CUDA device (the policy network has no CPU fallback)"); return nullptr; }
+    if (!g) { mlp_fail("dm_mlp_create_gated: null weights"); return nullptr; }
+    if (g->in_dim <= 0 || g->goal_dim <= 0 || g->goal_dim > 64 || g->h0 <= 0 || g->h1 <= 0 || g->out_dim <= 0 || g->out_dim > 64 || max_rows <= 0) {
+        mlp_fail("dm_mlp_create_gated: bad sizes (goal_dim must be <= 64, out_dim <= 64)"); return nullptr;
+    }
+    if (g->gate_common <= 0 || g->gate_common > 128 || g->gate_hidden <= 0 || g->gate_hidden > 64) {
+        mlp_fail("dm_mlp_create_gated: unsupported gate sizes (gate_common must be <= 128, gate_hidden <= 64)"); return nullptr;
+    }
+    const float* need[] = {g->w0, g->b0, g->w1, g->b1, g->w2, g->b2, g->gc_w, g->gc_b, g->gh_w[0], g->gh_b[0], g->gh_w[1], g->gh_b[1],
+                           g->gs_w[0], g->gs_b[0], g->gs_w[1], g->gs_b[1], g->gb_w[0], g->gb_b[0], g->gb_w[1], g->gb_b[1]};
+    for (const float* p : need)
+        if (!p) { mlp_fail("dm_mlp_create_gated: null weight pointer"); return nullptr; }
+    if (cudaSetDevice(device) != cudaSuccess) { mlp_fail("dm_mlp_create_gated: cudaSetDevice failed"); return nullptr; }
+    cudaDeviceProp prop;
+    cudaGetDeviceProperties(&prop, device);
+    if (prop.major != 9 || prop.minor != 0) { mlp_fail("dm_mlp_create_gated: the wgmma kernels are built for sm_90a (found sm_" + std::to_string(prop.major) + std::to_string(prop.minor) + ")"); return nullptr; }
+    dm_mlp* m = new dm_mlp();
+    m->gated = true;
+    m->device = device; m->in_dim = g->in_dim; m->goal_dim = g->goal_dim; m->h0 = g->h0; m->h1 = g->h1; m->out_dim = g->out_dim; m->max_rows = pad_to(max_rows, 128);
+    const int trunk_in = g->in_dim + g->goal_dim, GC = g->gate_common, GH = g->gate_hidden;
+    m->K0 = pad_to(trunk_in, 64); m->N0 = pad_to(g->h0, 64); m->N1 = pad_to(g->h1, 64);   // the gated layers run on 64-column tiles
+    m->in_clip = g->s_clip > 0.f ? g->s_clip : 1e30f;
+    m->g_clip = g->g_clip > 0.f ? g->g_clip : 1e30f;
+    // both gate hidden layers side by side: layer l's GH units in columns [64 l, 64 l + GH), zero columns (relu(0) = 0) up to 64 l + 64
+    std::vector<float> wgh(static_cast<size_t>(GC) * 128, 0.f), bgh(128, 0.f);
+    for (int l = 0; l < 2; ++l) {
+        for (int k = 0; k < GC; ++k)
+            for (int n = 0; n < GH; ++n) wgh[static_cast<size_t>(k) * 128 + 64 * l + n] = g->gh_w[l][static_cast<size_t>(k) * GH + n];
+        for (int n = 0; n < GH; ++n) bgh[64 * l + n] = g->gh_b[l][n];
+    }
+    const size_t R = m->max_rows;
+    bool ok = upload(&m->w[0], tile_weights(g->w0, trunk_in, g->h0, m->K0, m->N0, 64)) && upload(&m->w[1], tile_weights(g->w1, g->h0, g->h1, m->N0, m->N1, 64)) &&
+              upload(&m->w[2], tile_weights(g->w2, g->h1, g->out_dim, m->N1, m->N2, m->N2)) && upload(&m->b[0], padded(g->b0, g->h0, m->N0)) &&
+              upload(&m->b[1], padded(g->b1, g->h1, m->N1)) && upload(&m->b[2], padded(g->b2, g->out_dim, m->N2)) &&
+              upload(&m->wgc, tile_weights(g->gc_w, g->goal_dim, GC, 64, 128, 128)) && upload(&m->bgc, padded(g->gc_b, GC, 128)) &&
+              upload(&m->wgh, tile_weights(wgh.data(), GC, 128, 128, 128, 128)) && upload(&m->bgh, bgh);
+    const int hl[2] = {g->h0, g->h1}, Nl[2] = {m->N0, m->N1};
+    for (int l = 0; l < 2 && ok; ++l)
+        ok = upload(&m->wgs[l], tile_weights(g->gs_w[l], GH, hl[l], 64, Nl[l], 64)) && upload(&m->bgs[l], padded(g->gs_b[l], hl[l], Nl[l])) &&
+             upload(&m->wgb[l], tile_weights(g->gb_w[l], GH, hl[l], 64, Nl[l], 64)) && upload(&m->bgb[l], padded(g->gb_b[l], hl[l], Nl[l]));
+    ok = ok && upload(&m->in_mean, padded(g->s_mean, g->in_dim, g->in_dim)) && upload(&m->in_istd, inverse_std(g->s_std, g->in_dim)) &&
+         upload(&m->g_mean, padded(g->g_mean, g->goal_dim, g->goal_dim)) && upload(&m->g_istd, inverse_std(g->g_std, g->goal_dim)) &&
+         upload(&m->out_mean, padded(g->a_mean, g->out_dim, g->out_dim)) && upload(&m->out_std, padded(g->a_std, g->out_dim, g->out_dim, 1.f)) &&
+         cudaMalloc(&m->obs_t, R * m->K0 * sizeof(__half)) == cudaSuccess && cudaMalloc(&m->goal_t, R * 64 * sizeof(__half)) == cudaSuccess &&
+         cudaMalloc(&m->gc_t, R * 128 * sizeof(__half)) == cudaSuccess && cudaMalloc(&m->gh_t, R * 128 * sizeof(__half)) == cudaSuccess &&
+         cudaMalloc(&m->act0, R * m->N0 * sizeof(__half)) == cudaSuccess && cudaMalloc(&m->act1, R * m->N1 * sizeof(__half)) == cudaSuccess;
+    if (ok) {
+        ok = cudaFuncSetAttribute(dmk::dm_mlp_gemm_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
+             cudaFuncSetAttribute(dmk::dm_mlp_gated_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess &&
+             cudaFuncSetAttribute(dmk::dm_mlp_gemm_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess;
+    }
+    if (!ok) { mlp_fail(std::string("dm_mlp_create_gated: ") + cudaGetErrorString(cudaGetLastError())); dm_mlp_destroy(m); return nullptr; }
+    return m;
+}
+
+int dm_mlp_forward_gated(dm_mlp* m, const float* d_obs, const float* d_goal, const float* d_noise, float* d_actions, int rows, void* stream) {
+    if (!m) return mlp_fail("dm_mlp_forward_gated: null handle");
+    if (!m->gated) return mlp_fail("dm_mlp_forward_gated: the handle holds a plain actor (dm_mlp_create); use dm_mlp_forward");
+    if (!d_obs || !d_goal || !d_actions) return mlp_fail("dm_mlp_forward_gated: null observation, goal or action pointer");
+    if (rows <= 0 || rows > m->max_rows) return mlp_fail("dm_mlp_forward_gated: rows out of range");
+    if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_mlp_forward_gated: cudaSetDevice failed");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int mt = (rows + 127) / 128;
+    // [state | goal] -> normalised fp16 trunk tiles; the normalised goal alone -> the gate trunk's tile (the extra chunk of the grid)
+    dmk::MlpPrepParams Q{d_obs, m->in_mean, m->in_istd, m->in_clip, m->in_dim, rows, m->K0 / 64, m->obs_t, d_goal, m->g_mean, m->g_istd, m->g_clip, m->goal_dim, m->goal_t};
+    dmk::dm_mlp_gated_prep_kernel<<<dim3(mt, m->K0 / 64 + 1), 128, 0, st>>>(Q);
+    dmk::MlpGemmParams P{};
+    P.M = rows;
+    // gate trunk: goal -> 128 + ReLU
+    P.a_tiles = m->goal_t; P.w_tiles = m->wgc; P.bias = m->bgc; P.out_tiles = m->gc_t; P.K = 64; P.N = 128;
+    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
+    // both gate hidden layers: 128 -> 2 x 64 + ReLU; K-chunk l of the output is layer l's gate in operand layout
+    P.a_tiles = m->gc_t; P.w_tiles = m->wgh; P.bias = m->bgh; P.out_tiles = m->gh_t; P.K = 128; P.N = 128;
+    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
+    // gated trunk layers: 229 -> 1024, 1024 -> 512, each scaled and shifted by its gate
+    P.gate_stride = 2 * dmk::kMlpATileHalves;
+    P.a_tiles = m->obs_t; P.w_tiles = m->w[0]; P.bias = m->b[0]; P.out_tiles = m->act0; P.K = m->K0; P.N = m->N0;
+    P.gate_tiles = m->gh_t; P.ws_tiles = m->wgs[0]; P.wb_tiles = m->wgb[0]; P.bias_s = m->bgs[0]; P.bias_b = m->bgb[0];
+    dmk::dm_mlp_gated_gemm_kernel<<<dim3(mt, m->N0 / 64), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P);
+    P.a_tiles = m->act0; P.w_tiles = m->w[1]; P.bias = m->b[1]; P.out_tiles = m->act1; P.K = m->N0; P.N = m->N1;
+    P.gate_tiles = m->gh_t + dmk::kMlpATileHalves; P.ws_tiles = m->wgs[1]; P.wb_tiles = m->wgb[1]; P.bias_s = m->bgs[1]; P.bias_b = m->bgb[1];
+    dmk::dm_mlp_gated_gemm_kernel<<<dim3(mt, m->N1 / 64), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P);
+    // output layer: 512 -> actions, un-normalised
+    P.a_tiles = m->act1; P.w_tiles = m->w[2]; P.bias = m->b[2]; P.out_tiles = nullptr; P.actions = d_actions; P.out_mean = m->out_mean; P.out_std = m->out_std; P.noise = d_noise;
+    P.out_dim = m->out_dim; P.K = m->N1; P.N = m->N2;
+    dmk::dm_mlp_gemm_kernel<64, true><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return mlp_fail(std::string("dm_mlp_forward_gated: ") + cudaGetErrorString(e));
+    m->launches += 6;
+    return 0;
+}
+
 long long dm_mlp_launches(dm_mlp* m) { return m ? m->launches : 0; }
 
 void dm_mlp_destroy(dm_mlp* m) {
@@ -134,6 +243,8 @@ void dm_mlp_destroy(dm_mlp* m) {
     for (auto& p : m->w) cudaFree(p);
     for (auto& p : m->b) cudaFree(p);
     cudaFree(m->obs_t); cudaFree(m->act0); cudaFree(m->act1); cudaFree(m->in_mean); cudaFree(m->in_istd); cudaFree(m->out_mean); cudaFree(m->out_std);
+    for (int l = 0; l < 2; ++l) { cudaFree(m->wgs[l]); cudaFree(m->wgb[l]); cudaFree(m->bgs[l]); cudaFree(m->bgb[l]); }
+    cudaFree(m->wgc); cudaFree(m->wgh); cudaFree(m->bgc); cudaFree(m->bgh); cudaFree(m->goal_t); cudaFree(m->gc_t); cudaFree(m->gh_t); cudaFree(m->g_mean); cudaFree(m->g_istd);
     delete m;
 }
 

@@ -8,7 +8,8 @@ N environments of a rank at once with observations, actions and rewards staying 
   BatchedRollout     record_state -> normalise -> actor -> un-normalise -> set_action -> 20 x update -> reward / flags -> masked reset,
                      collecting [T, N, .] trajectory tensors for a learner
 
-The MLP runs as plain torch matmuls (cuBLAS): a library GEMM, not part of the hand-written hot path.  The reference's TF1 checkpoints
+With backend "torch" the MLP runs as plain torch matmuls (cuBLAS); with backend "tensor_core" the actor's inference (plain or gated) runs on
+the library's own wgmma kernels (kernels/dm_mlp.cu).  The reference's TF1 checkpoints
 are read by deepmimic_b200/tf_checkpoint.py (TensorBundle reader, no TensorFlow) and loaded with load_actor_weights; without a
 checkpoint the weights are random-initialised the way the reference initialises them."""
 import math
@@ -193,10 +194,12 @@ class _nullcontext:
 
 
 class BatchedRollout:
-    """backend "torch": the policy is a torch module (cuBLAS GEMMs, eager normalisers) -- needed for training and for the gated task actor.
-    backend "tensor_core": inference of the plain 2-layer actor on the library's own tensor-core kernels (dm_mlp_*, kernels/dm_mlp.cu): normaliser,
-    three GEMMs, bias / ReLU and the action un-normalisation in four launches (operand preparation + one per layer) on the environment's stream; the weights and the normaliser
-    statistics are snapshotted by refresh_tensor_core_policy() (call it again after a learner update)."""
+    """backend "torch": the policy is a torch module (cuBLAS GEMMs, eager normalisers) -- needed for training.
+    backend "tensor_core": inference of the actor on the library's own tensor-core kernels (dm_mlp_*, kernels/dm_mlp.cu) on the environment's
+    stream.  The plain 2-layer actor: normaliser, three GEMMs, bias / ReLU and the action un-normalisation in four launches (operand preparation
+    + one per layer).  The gated actor of the goal-conditioned task scenes: six launches (operand preparation of [state | goal], gate trunk, both
+    gate hidden layers, the two gated trunk layers, output layer).  The weights and the normaliser statistics are snapshotted by
+    refresh_tensor_core_policy() (call it again after a learner update)."""
 
     def __init__(self, env, policy=None, exp_rate=1.0, noise=0.05, seed=0, backend="torch"):
         import torch
@@ -218,26 +221,33 @@ class BatchedRollout:
         self.backend, self._tc = backend, None
         if backend not in ("torch", "tensor_core"):
             raise ValueError("backend must be 'torch' or 'tensor_core'")
-        if backend == "tensor_core" and G > 0:
-            raise ValueError("the tensor_core backend implements the plain 2-layer actor; goal-conditioned (gated) actors run on the torch backend")
 
     def refresh_tensor_core_policy(self):
         """(re)builds the dm_mlp handle from the current torch policy and normalisers"""
-        from .capi import TensorCoreMLP
+        from .capi import TensorCoreGatedMLP, TensorCoreMLP
         pol, env = self.policy, self.env
         if len(pol.hidden) != 2:
             raise ValueError("the tensor_core backend implements exactly two hidden layers")
         g = lambda t: t.detach().float().cpu().numpy()
         if self._tc is not None:
             self._tc.close()
-        self._tc = TensorCoreMLP(g(pol.hidden[0].weight).T, g(pol.hidden[0].bias), g(pol.hidden[1].weight).T, g(pol.hidden[1].bias), g(pol.mean.weight).T, g(pol.mean.bias),
-                                 in_mean=g(self.s_norm.mean), in_std=g(self.s_norm.std), in_clip=self.s_norm.clip, out_mean=g(self.a_norm.mean), out_std=g(self.a_norm.std),
-                                 max_rows=env.num_envs, device=env.device.index or 0)
+        if self.goal_size > 0:
+            wb = lambda l: (g(l.weight).T, g(l.bias))
+            actor = dict(hidden=[wb(l) for l in pol.hidden], mean=wb(pol.mean), gate_common=wb(pol.gate_common),
+                         gates=[dict(hidden=wb(h), scale=wb(sc), bias=wb(b)) for h, sc, b in zip(pol.gate_hidden, pol.gate_scale, pol.gate_bias)])
+            self._tc = TensorCoreGatedMLP(actor, s_mean=g(self.s_norm.mean), s_std=g(self.s_norm.std), s_clip=self.s_norm.clip, g_mean=g(self.g_norm.mean),
+                                          g_std=g(self.g_norm.std), g_clip=self.g_norm.clip, a_mean=g(self.a_norm.mean), a_std=g(self.a_norm.std),
+                                          max_rows=env.num_envs, device=env.device.index or 0)
+        else:
+            self._tc = TensorCoreMLP(g(pol.hidden[0].weight).T, g(pol.hidden[0].bias), g(pol.hidden[1].weight).T, g(pol.hidden[1].bias), g(pol.mean.weight).T, g(pol.mean.bias),
+                                     in_mean=g(self.s_norm.mean), in_std=g(self.s_norm.std), in_clip=self.s_norm.clip, out_mean=g(self.a_norm.mean), out_std=g(self.a_norm.std),
+                                     max_rows=env.num_envs, device=env.device.index or 0)
         self._tc_act = self.torch.empty(env.num_envs, env.get_action_size(), device=env.device)
         return self._tc
 
-    def _act_tensor_core(self, s, explore):
-        """un-normalised actions and log-probabilities from the tensor-core actor (exploration noise is drawn in torch, added in the kernel's epilogue)"""
+    def _act_tensor_core(self, s, explore, g=None):
+        """un-normalised actions and log-probabilities from the tensor-core actor (exploration noise is drawn in torch, added in the kernel's epilogue);
+        g: the goals, for the gated actor of the goal-conditioned scenes"""
         t = self.torch
         if self._tc is None:
             self.refresh_tensor_core_policy()
@@ -245,7 +255,10 @@ class BatchedRollout:
         eps = t.randn(s.shape[0], std.shape[0], device=s.device, generator=self.gen) * explore[:, None].to(s.dtype)
         noise = (std * eps).contiguous()
         cur = t.cuda.current_stream(s.device)
-        self._tc.forward(s.contiguous(), self._tc_act, noise=noise, stream=cur.cuda_stream)
+        if g is None:
+            self._tc.forward(s.contiguous(), self._tc_act, noise=noise, stream=cur.cuda_stream)
+        else:
+            self._tc.forward(s.contiguous(), g.contiguous(), self._tc_act, noise=noise, stream=cur.cuda_stream)
         logp = (-0.5 * eps * eps - self.policy.logstd.detach() - 0.5 * math.log(2 * math.pi)).sum(dim=-1)
         return self._tc_act, logp
 
@@ -280,12 +293,13 @@ class BatchedRollout:
                     out["goals"][k] = g
                     if record_stats:
                         self.g_norm.record(g)
+                if self.backend == "tensor_core":
+                    a, logp = self._act_tensor_core(s, explore, g if G > 0 else None)
+                elif G > 0:
                     na, logp = self.policy.sample(self.s_norm.normalize(s), self.g_norm.normalize(g), explore, self.gen)
-                elif self.backend == "tensor_core":
-                    a, logp = self._act_tensor_core(s, explore)
                 else:
                     na, logp = self.policy.sample(self.s_norm.normalize(s), explore, self.gen)
-                if not (G == 0 and self.backend == "tensor_core"):
+                if self.backend != "tensor_core":
                     a = self.a_norm.unnormalize(na).contiguous()
                 s, r, done, term = env.step(a)
                 out["actions"][k] = a; out["logps"][k] = logp; out["rewards"][k] = r; out["dones"][k] = done; out["terminate"][k] = term

@@ -172,7 +172,26 @@ dm_mlp* dm_mlp_create(int device, int in_dim, int h0, int h1, int out_dim, const
                       const float* h_w2, const float* h_b2, const float* h_in_mean, const float* h_in_std, float in_clip, const float* h_out_mean,
                       const float* h_out_std, int max_rows);
 int dm_mlp_forward(dm_mlp* m, const float* d_obs, const float* d_noise, float* d_actions, int rows, void* stream);
-long long dm_mlp_launches(dm_mlp* m);
+/* The goal-conditioned actor of the AMP task scenes (R/learning/nets/fc_2layers_gated_1024units.py:6-58, R/learning/amp_agent.py): with
+ * ns = clip((s - s_mean) / s_std), ng = clip((g - g_mean) / g_std), gc = relu(ng Wgc + bgc) and per hidden layer l
+ *   gh_l = relu(gc Wgh_l + bgh_l),  h = relu(2 sigmoid(gh_l Wgs_l + bgs_l) * (h W_l + b_l) + gh_l Wgb_l + bgb_l),  h starting as [ns, ng],
+ * actions = a_mean + a_std * (h W2 + b2 [+ noise]).  Exactly two hidden layers; gate_common <= 128, gate_hidden <= 64, goal_dim <= 64,
+ * out_dim <= 64.  Same weight layout and tiling as dm_mlp_create; the std / mean pointers may be NULL (identity), a clip <= 0 means none. */
+typedef struct dm_mlp_gated_weights {
+    int in_dim, goal_dim, h0, h1, out_dim, gate_common, gate_hidden;
+    const float *w0, *b0, *w1, *b1, *w2, *b2;  /* trunk: [in_dim + goal_dim x h0], [h0 x h1], output layer [h1 x out_dim] */
+    const float *gc_w, *gc_b;                  /* gate trunk [goal_dim x gate_common] */
+    const float *gh_w[2], *gh_b[2];            /* gate hidden layer l [gate_common x gate_hidden] */
+    const float *gs_w[2], *gs_b[2];            /* gate scale of layer l [gate_hidden x h_l] */
+    const float *gb_w[2], *gb_b[2];            /* gate bias of layer l [gate_hidden x h_l] */
+    const float *s_mean, *s_std, *g_mean, *g_std, *a_mean, *a_std;
+    float s_clip, g_clip;
+} dm_mlp_gated_weights;
+dm_mlp* dm_mlp_create_gated(int device, const dm_mlp_gated_weights* h_weights, int max_rows);
+/* d_obs [rows x in_dim], d_goal [rows x goal_dim], d_noise [rows x out_dim] or NULL, d_actions [rows x out_dim]: fp32 device pointers.
+ * dm_mlp_forward refuses a gated handle and dm_mlp_forward_gated a plain one. */
+int dm_mlp_forward_gated(dm_mlp* m, const float* d_obs, const float* d_goal, const float* d_noise, float* d_actions, int rows, void* stream);
+long long dm_mlp_launches(dm_mlp* m);   /* kernel launches so far: 4 per plain forward, 6 per gated forward */
 void dm_mlp_destroy(dm_mlp* m);
 
 /* ---- test hooks: raw per-env simulator state, layout shared with the CPU oracle (doubles):

@@ -1,10 +1,11 @@
-"""Times the policy network alone (4096 x 227 -> 1024 -> 512 -> 28): dm_mlp_forward (wgmma kernels) against the fp32 torch actor, CUDA events."""
+"""Times the policy networks alone, CUDA events: the plain actor (4096 x 227 -> 1024 -> 512 -> 28, dm_mlp_forward) and the gated task actor
+(4096 x (226 + 3) -> 1024 -> 512 -> 28 with its gates, dm_mlp_forward_gated) on the wgmma kernels, each against the fp32 torch network."""
 import os, sys
 import numpy as np
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 import torch
-from deepmimic_b200.capi import TensorCoreMLP
+from deepmimic_b200.capi import TensorCoreGatedMLP, TensorCoreMLP
 rows, din, h0, h1, dout = int(os.environ.get("MLP_ROWS", "4096")), 227, 1024, 512, 28
 rng = np.random.default_rng(0)
 w0 = (rng.standard_normal((din, h0)) / np.sqrt(din)).astype(np.float32); w1 = (rng.standard_normal((h0, h1)) / np.sqrt(h0)).astype(np.float32); w2 = (rng.standard_normal((h1, dout)) / np.sqrt(h1)).astype(np.float32)
@@ -29,3 +30,27 @@ t_tc = timeit(lambda: mlp.forward(x, out, noise=noise, stream=st.cuda_stream))
 t_th = timeit(torch_actor)
 ref = torch_actor(); torch.cuda.synchronize()
 print("policy network, %d rows: wgmma kernels %.1f us per forward, fp32 torch actor %.1f us; max |diff| %.2e" % (rows, t_tc, t_th, (out - ref).abs().max().item()))
+
+# the gated actor of the task scenes: goal 3, gate trunk 128, gate hidden 64
+G, ds = 3, din - 1
+lin = lambda a, b: ((rng.standard_normal((a, b)) / np.sqrt(a)).astype(np.float32), (rng.standard_normal(b) * 0.1).astype(np.float32))
+actor = dict(hidden=[lin(ds + G, h0), lin(h0, h1)], mean=lin(h1, dout), gate_common=lin(G, 128),
+             gates=[dict(hidden=lin(128, 64), scale=lin(64, h), bias=lin(64, h)) for h in (h0, h1)])
+g_mean, g_std = rng.standard_normal(G).astype(np.float32), (0.5 + rng.random(G)).astype(np.float32)
+gmlp = TensorCoreGatedMLP(actor, s_mean=mean[:ds], s_std=std[:ds], s_clip=5.0, g_mean=g_mean, g_std=g_std, g_clip=5.0, max_rows=rows)
+xs, xg = x[:, :ds].contiguous(), torch.randn(rows, G, device="cuda")
+T = lambda a: torch.tensor(a, device="cuda")
+ta = {k: tuple(T(a) for a in v) for k, v in (("h0", actor["hidden"][0]), ("h1", actor["hidden"][1]), ("m", actor["mean"]), ("gc", actor["gate_common"]))}
+tg = [{k: tuple(T(a) for a in g[k]) for k in ("hidden", "scale", "bias")} for g in actor["gates"]]
+tn = [T(a) for a in (mean[:ds], std[:ds], g_mean, g_std)]
+def torch_gated_actor():
+    L = lambda v, wb: v @ wb[0] + wb[1]
+    ns, ng = torch.clamp((xs - tn[0]) / tn[1], -5, 5), torch.clamp((xg - tn[2]) / tn[3], -5, 5)
+    gc = torch.relu(L(ng, ta["gc"])); h = torch.cat([ns, ng], dim=-1)
+    for w, g in zip((ta["h0"], ta["h1"]), tg):
+        gh = torch.relu(L(gc, g["hidden"])); h = torch.relu(2.0 * torch.sigmoid(L(gh, g["scale"])) * L(h, w) + L(gh, g["bias"]))
+    return L(h, ta["m"])
+t_gtc = timeit(lambda: gmlp.forward(xs, xg, out, noise=noise, stream=st.cuda_stream))
+t_gth = timeit(torch_gated_actor)
+ref = torch_gated_actor(); torch.cuda.synchronize()
+print("gated policy network, %d rows: wgmma kernels %.1f us per forward, fp32 torch actor %.1f us; max |diff| %.2e" % (rows, t_gtc, t_gth, (out - ref).abs().max().item()))

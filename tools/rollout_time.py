@@ -1,5 +1,6 @@
 """Where does a device-resident rollout step spend its time?  CUDA events around the actor and around the environment step, host time per step,
-for both actor backends (diagnosis tool for tests/test_mlp_gpu.py's rollout rates)."""
+for both actor backends (diagnosis tool for the rollout rates of tests/test_mlp_gpu.py and tests/test_mlp_gated_gpu.py): the spin-kick imitation
+scene with the plain actor, then the target_amp task scene with the gated actor."""
 import os, sys, time
 import numpy as np
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -7,15 +8,25 @@ sys.path.insert(0, REPO)
 import torch
 from deepmimic_b200.assets import asset_root
 from deepmimic_b200.env import DeepMimicBatchEnv
-from deepmimic_b200.rollout import BatchedRollout, build_policy, load_actor_weights
+from deepmimic_b200.rollout import BatchedRollout, build_gated_policy, build_policy, load_actor_weights
+sys.path.insert(0, os.path.join(REPO, "tests"))
+from test_task_scenes_cpu import fixture_task_actor
 f = np.load(os.path.join(REPO, "tests", "golden", "policy_humanoid3d_spinkick_fp16.npz"))
 a = {k: f[k].astype(np.float64) for k in f.files}
 root = asset_root(True)
-for backend in ("tensor_core", "torch", "tensor_core"):
-    env = DeepMimicBatchEnv(["--arg_file", "args/train_humanoid3d_spinkick_args.txt"], num_envs=4096, asset_root=root, seed=4)
-    env._core.set_episode_limit(20.0); env.reset(True)
-    ro = BatchedRollout(env, policy=load_actor_weights(build_policy(227, 28), a), exp_rate=1.0, backend=backend)
-    ro.s_norm.set_mean_std(a["s_mean"], a["s_std"]); ro.a_norm.set_mean_std(a["a_mean"], a["a_std"])
+at = fixture_task_actor("target")
+TARGET = ["--motion_file", "data/datasets/test_clips_mini.txt", "--arg_file", "args/train_amp_target_humanoid3d_locomotion_args.txt"]
+for scene, backend in [("spinkick", "tensor_core"), ("spinkick", "torch"), ("spinkick", "tensor_core"), ("target", "tensor_core"), ("target", "torch"), ("target", "tensor_core")]:
+    if scene == "spinkick":
+        env = DeepMimicBatchEnv(["--arg_file", "args/train_humanoid3d_spinkick_args.txt"], num_envs=4096, asset_root=root, seed=4)
+        env._core.set_episode_limit(20.0); env.reset(True)
+        ro = BatchedRollout(env, policy=load_actor_weights(build_policy(227, 28), a), exp_rate=1.0, backend=backend)
+        ro.s_norm.set_mean_std(a["s_mean"], a["s_std"]); ro.a_norm.set_mean_std(a["a_mean"], a["a_std"])
+    else:
+        env = DeepMimicBatchEnv(TARGET, num_envs=4096, asset_root=root, seed=4)
+        env.reset(True)
+        ro = BatchedRollout(env, policy=load_actor_weights(build_gated_policy(226, 3, 28), at), exp_rate=1.0, backend=backend)
+        ro.s_norm.set_mean_std(at["s_norm_mean"], at["s_norm_std"]); ro.g_norm.set_mean_std(at["g_norm_mean"], at["g_norm_std"]); ro.a_norm.set_mean_std(at["a_norm_mean"], at["a_norm_std"])
     ro.collect(8, record_stats=False); torch.cuda.synchronize()
     t0 = time.perf_counter(); ro.collect(48, record_stats=False); torch.cuda.synchronize(); dt = time.perf_counter() - t0
     # manual loop with events
@@ -24,9 +35,12 @@ for backend in ("tensor_core", "torch", "tensor_core"):
     for k in range(32):
         e = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
         explore = torch.rand(4096, device="cuda") < 1.0
+        g = env.record_goal() if scene == "target" else None
         e[0].record()
         if backend == "tensor_core":
-            act, logp = ro._act_tensor_core(s, explore)
+            act, logp = ro._act_tensor_core(s, explore, g)
+        elif g is not None:
+            na, logp = ro.policy.sample(ro.s_norm.normalize(s), ro.g_norm.normalize(g), explore, ro.gen); act = ro.a_norm.unnormalize(na).contiguous()
         else:
             na, logp = ro.policy.sample(ro.s_norm.normalize(s), explore, ro.gen); act = ro.a_norm.unnormalize(na).contiguous()
         e[1].record()
@@ -39,5 +53,5 @@ for backend in ("tensor_core", "torch", "tensor_core"):
     torch.cuda.synchronize()
     wall = time.perf_counter() - th
     g = lambda i, j: np.median([x[i].elapsed_time(x[j]) for x in ev])
-    print("%-8s collect(48): %.0f steps/s | manual loop: actor %.3f ms, env.step %.3f ms, reset+observe %.3f ms (GPU, median) ; host enqueue %.3f ms/step, wall %.3f ms/step"
-          % (backend, 4096 * 48 / dt, g(0, 1), g(1, 2), g(2, 3), 1e3 * host / 32, 1e3 * wall / 32))
+    print("%-8s %-11s collect(48): %.0f steps/s | manual loop: actor %.3f ms, env.step %.3f ms, reset+observe %.3f ms (GPU, median) ; host enqueue %.3f ms/step, wall %.3f ms/step"
+          % (scene, backend, 4096 * 48 / dt, g(0, 1), g(1, 2), g(2, 3), 1e3 * host / 32, 1e3 * wall / 32))
