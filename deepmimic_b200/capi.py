@@ -31,7 +31,7 @@ DM_STATE_OFFSET, DM_STATE_SCALE, DM_ACTION_OFFSET, DM_ACTION_SCALE, DM_ACTION_BO
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
            "dm_update", "dm_record_state", "dm_record_goal", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
            "dm_set_snapshot", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
-           "dm_mlp_launches", "dm_mlp_destroy"]
+           "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy"]
 
 
 def lib():
@@ -102,6 +102,7 @@ def lib():
         L.dm_mlp_create_gated.restype = vp
         L.dm_mlp_create_gated.argtypes = [C.c_int, C.POINTER(DmMlpGatedWeights), C.c_int]
         L.dm_mlp_forward_gated.argtypes = [vp, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+        L.dm_mlp_forward_style_reward.argtypes = [vp, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.dm_mlp_launches.restype = C.c_longlong
         L.dm_mlp_launches.argtypes = [vp]
         L.dm_mlp_destroy.argtypes = [vp]
@@ -394,7 +395,8 @@ class HostModel:
 
 class TensorCoreMLP:
     """dm_mlp_* handle: the actor network (normalise -> 2 hidden ReLU layers -> linear -> un-normalise) on the tensor cores (wgmma).
-    weights: the reference's dense kernels, [inputs x units] float arrays (deepmimic_b200.tf_checkpoint.load_actor / the fixture files)."""
+    weights: the reference's dense kernels, [inputs x units] float arrays (deepmimic_b200.tf_checkpoint.load_actor / the fixture files).
+    With one output unit and no output normaliser the handle is an AMP discriminator: style_reward() runs it with the reward epilogue."""
 
     def __init__(self, w0, b0, w1, b1, w2, b2, in_mean=None, in_std=None, in_clip=float("inf"), out_mean=None, out_std=None, max_rows=4096, device=0):
         L = lib()
@@ -419,6 +421,17 @@ class TensorCoreMLP:
         if rc != 0:
             raise RuntimeError("dm_mlp_forward: %s" % lib().dm_last_error().decode())
         return actions
+
+    def style_reward(self, amp_obs, reward, task_reward=None, task_lerp=0.0, logit=None, style=None, stream=None):
+        """dm_mlp_forward_style_reward: the discriminator's logit d on amp_obs [rows, in_dim], style = max(0, 1 - 0.25 (1 - d)^2) and
+        reward [rows] (written) = (1 - task_lerp) style + task_lerp task_reward, or style without task_reward.  logit / style [rows] are
+        written when given.  Contiguous float32 CUDA tensors; stream: cudaStream_t handle (int) or None"""
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+        rc = lib().dm_mlp_forward_style_reward(self.h, ptr(amp_obs), ptr(task_reward), float(task_lerp), ptr(logit), ptr(style), ptr(reward), amp_obs.shape[0],
+                                               C.c_void_p(stream) if stream else None)
+        if rc != 0:
+            raise RuntimeError("dm_mlp_forward_style_reward: %s" % lib().dm_last_error().decode())
+        return reward
 
     def launches(self):
         return int(lib().dm_mlp_launches(self.h))

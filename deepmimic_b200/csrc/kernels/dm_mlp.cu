@@ -69,6 +69,17 @@ struct MlpGemmParams {
     const float* bias_b;
     int gate_stride;           // halves
 };
+// The discriminator head's outputs, a kernel parameter of its own: MlpGemmParams stays at 128 bytes (nvcc 12.9 compiles every GEMM
+// instantiation differently once that struct grows past 128 bytes, even with the new fields unused).  Column 0 of the head is the logit
+// d = acc + bias (no un-normalisation); per row r < M, style = max(0, 1 - 0.25 (1 - d)^2) and
+// reward = (1 - task_lerp) style + task_lerp task_reward[r], or style without a task reward.
+struct MlpStyleParams {
+    const float* task_reward;  // [M] or null
+    float* logit;              // [M] or null
+    float* style;              // [M] or null
+    float* reward;             // [M]
+    float task_lerp;
+};
 
 namespace {
 
@@ -149,14 +160,16 @@ __global__ void __launch_bounds__(kMlpThreads) dm_mlp_gated_prep_kernel(MlpPrepP
 // dynamic shared memory = 2 stages x (A 16 KB + W hi/lo 2 x BN x 128 B) + 1 KB (barriers).
 // GATED (a hidden layer of the gated actor): two more pipeline chunks after the K loop (MlpGemmParams::gate_tiles) accumulate the gate's scale
 // and bias pre-activations in registers of their own; with BN = 64 that is 3 x 32 accumulator registers per thread.
-template <int BN, bool LAST, bool GATED>
-__device__ __forceinline__ void mlp_gemm(const MlpGemmParams& P) {
+// STYLE (the discriminator's one-unit logit head): the last layer's epilogue writes the style reward instead of actions.
+template <int BN, bool LAST, bool GATED, bool STYLE = false>
+__device__ __forceinline__ void mlp_gemm(const MlpGemmParams& P, const MlpStyleParams* S = nullptr) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     constexpr int kABytes = kMlpATile * 2;               // 16 KB
     constexpr int kWBytes = 2 * BN * kMlpBK * 2;         // hi + lo
     constexpr int kStage = kABytes + kWBytes;
     constexpr int NH = BN / 64;                          // 64-column accumulators per warpgroup
     static_assert(!GATED || (!LAST && NH == 1), "the gated epilogue is written for one 64-column accumulator of a hidden layer");
+    static_assert(!STYLE || (LAST && !GATED && NH == 1), "the style-reward epilogue is written for one 64-column accumulator of the last layer");
     uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem_raw + kMlpStages * kStage);   // [stages] both operands of the stage have landed
     uint64_t* bar_empty = bar_full + kMlpStages;                                         // [stages] every thread's MMAs reading the stage have completed
     const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127;
@@ -245,7 +258,16 @@ __device__ __forceinline__ void mlp_gemm(const MlpGemmParams& P) {
             const int n = n0 + h * 64 + 8 * (q >> 1) + 2 * (lane & 3);
             const int i0 = 4 * (q >> 1) + 2 * (q & 1);
             const float v0 = acc[h][i0], v1 = acc[h][i0 + 1];
-            if constexpr (LAST) {
+            if constexpr (STYLE) {
+                // the logit is column 0 (the tile's other 63 columns are padding): one thread per row holds it and writes every output of that row
+                if (row < P.M && n == 0) {
+                    const float d = v0 + P.bias[0], e = 1.f - d;
+                    const float style = fmaxf(0.f, 1.f - 0.25f * e * e);
+                    S->reward[row] = S->task_reward ? (1.f - S->task_lerp) * style + S->task_lerp * S->task_reward[row] : style;
+                    if (S->logit) S->logit[row] = d;
+                    if (S->style) S->style[row] = style;
+                }
+            } else if constexpr (LAST) {
                 if (row < P.M) {
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
@@ -280,6 +302,8 @@ template <int BN, bool LAST>
 __global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_gemm_kernel(MlpGemmParams P) { mlp_gemm<BN, LAST, false>(P); }
 // a hidden layer of the gated actor, 64-column tiles
 __global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_gated_gemm_kernel(MlpGemmParams P) { mlp_gemm<64, false, true>(P); }
+// the discriminator's logit head with the style-reward epilogue (AMP, Peng et al. 2021, eq. 7), 64-column tile
+__global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_style_reward_kernel(MlpGemmParams P, MlpStyleParams S) { mlp_gemm<64, true, false, true>(P, &S); }
 
 int dm_mlp_smem_bytes(int bn) { return kMlpStages * (kMlpATile * 2 + 2 * bn * kMlpBK * 2) + 1024; }
 

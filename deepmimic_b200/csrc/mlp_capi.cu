@@ -1,6 +1,7 @@
 // C ABI of the tensor-core policy network (include/deepmimic_b200.h, dm_mlp_*): host-side weight tiling + the launches of kernels/dm_mlp.cu: four for
 // the plain actor (operand preparation, three GEMMs), six for the gated one (operand preparation, gate trunk, both gate hidden layers, two gated
-// trunk layers, output layer).  Same library, same rules: no CPU fallback, errors through dm_last_error.
+// trunk layers, output layer), four for the AMP discriminator's style reward (operand preparation, two GEMMs, the logit head with the reward
+// epilogue).  Same library, same rules: no CPU fallback, errors through dm_last_error.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
@@ -22,11 +23,13 @@ struct MlpGemmParams {
     int out_dim; int M, K, N;
     const __half* gate_tiles; const __half* ws_tiles; const __half* wb_tiles; const float* bias_s; const float* bias_b; int gate_stride;
 };
+struct MlpStyleParams { const float* task_reward; float* logit; float* style; float* reward; float task_lerp; };
 __global__ void dm_mlp_prep_kernel(MlpPrepParams);
 __global__ void dm_mlp_gated_prep_kernel(MlpPrepParams);
 template <int BN, bool LAST>
 __global__ void dm_mlp_gemm_kernel(MlpGemmParams);
 __global__ void dm_mlp_gated_gemm_kernel(MlpGemmParams);
+__global__ void dm_mlp_style_reward_kernel(MlpGemmParams, MlpStyleParams);
 int dm_mlp_smem_bytes(int bn);
 constexpr int kMlpATileHalves = 128 * 64;   // one operand tile of activations (kernels/dm_mlp.cu: kMlpATile)
 }  // namespace dmk
@@ -80,6 +83,25 @@ bool upload(T** dst, const std::vector<T>& src) {
 }
 std::vector<float> padded(const float* v, int n, int N, float fill = 0.f) { std::vector<float> o(N, fill); if (v) std::memcpy(o.data(), v, sizeof(float) * n); return o; }
 std::vector<float> inverse_std(const float* std_dev, int n) { std::vector<float> o(n, 1.f); for (int i = 0; i < n; ++i) o[i] = std_dev ? 1.0f / std_dev[i] : 1.f; return o; }
+// the plain network's operand preparation and two hidden layers (three launches); the caller sets the output layer's fields of the returned
+// parameters and launches it
+dmk::MlpGemmParams plain_trunk(dm_mlp* m, const float* d_obs, int rows, cudaStream_t st) {
+    const int mt = (rows + 127) / 128;
+    // observations -> normalised fp16 operand tiles
+    dmk::MlpPrepParams Q{d_obs, m->in_mean, m->in_istd, m->in_clip, m->in_dim, rows, m->K0 / 64, m->obs_t};
+    dmk::dm_mlp_prep_kernel<<<dim3(mt, m->K0 / 64), 128, 0, st>>>(Q);
+    dmk::MlpGemmParams P{};
+    P.M = rows;
+    // layer 0: 227 -> 1024 + ReLU
+    P.a_tiles = m->obs_t; P.w_tiles = m->w[0]; P.bias = m->b[0]; P.out_tiles = m->act0; P.K = m->K0; P.N = m->N0;
+    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, m->N0 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
+    // layer 1: 1024 -> 512 + ReLU
+    P.a_tiles = m->act0; P.w_tiles = m->w[1]; P.bias = m->b[1]; P.out_tiles = m->act1; P.K = m->N0; P.N = m->N1;
+    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, m->N1 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
+    // the output layer reads layer 1's tiles
+    P.a_tiles = m->act1; P.w_tiles = m->w[2]; P.bias = m->b[2]; P.out_tiles = nullptr; P.K = m->N1; P.N = m->N2;
+    return P;
+}
 }  // namespace
 
 extern "C" {
@@ -109,6 +131,8 @@ dm_mlp* dm_mlp_create(int device, int in_dim, int h0, int h1, int out_dim, const
         ok = cudaFuncSetAttribute(dmk::dm_mlp_gemm_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
              cudaFuncSetAttribute(dmk::dm_mlp_gemm_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess;
     }
+    if (ok && out_dim == 1)   // a one-unit head can be a discriminator (dm_mlp_forward_style_reward)
+        ok = cudaFuncSetAttribute(dmk::dm_mlp_style_reward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess;
     if (!ok) { mlp_fail(std::string("dm_mlp_create: ") + cudaGetErrorString(cudaGetLastError())); dm_mlp_destroy(m); return nullptr; }
     return m;
 }
@@ -119,22 +143,10 @@ int dm_mlp_forward(dm_mlp* m, const float* d_obs, const float* d_noise, float* d
     if (rows <= 0 || rows > m->max_rows) return mlp_fail("dm_mlp_forward: rows out of range");
     if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_mlp_forward: cudaSetDevice failed");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int mt = (rows + 127) / 128;
-    // observations -> normalised fp16 operand tiles
-    dmk::MlpPrepParams Q{d_obs, m->in_mean, m->in_istd, m->in_clip, m->in_dim, rows, m->K0 / 64, m->obs_t};
-    dmk::dm_mlp_prep_kernel<<<dim3(mt, m->K0 / 64), 128, 0, st>>>(Q);
-    dmk::MlpGemmParams P{};
-    P.M = rows;
-    // layer 0: 227 -> 1024 + ReLU
-    P.a_tiles = m->obs_t; P.w_tiles = m->w[0]; P.bias = m->b[0]; P.out_tiles = m->act0; P.K = m->K0; P.N = m->N0;
-    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, m->N0 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
-    // layer 1: 1024 -> 512 + ReLU
-    P.a_tiles = m->act0; P.w_tiles = m->w[1]; P.bias = m->b[1]; P.out_tiles = m->act1; P.K = m->N0; P.N = m->N1;
-    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, m->N1 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
+    dmk::MlpGemmParams P = plain_trunk(m, d_obs, rows, st);
     // layer 2: 512 -> actions, un-normalised
-    P.a_tiles = m->act1; P.w_tiles = m->w[2]; P.bias = m->b[2]; P.out_tiles = nullptr; P.actions = d_actions; P.out_mean = m->out_mean; P.out_std = m->out_std; P.noise = d_noise;
-    P.out_dim = m->out_dim; P.K = m->N1; P.N = m->N2;
-    dmk::dm_mlp_gemm_kernel<64, true><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P);
+    P.actions = d_actions; P.out_mean = m->out_mean; P.out_std = m->out_std; P.noise = d_noise; P.out_dim = m->out_dim;
+    dmk::dm_mlp_gemm_kernel<64, true><<<dim3((rows + 127) / 128, 1), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return mlp_fail(std::string("dm_mlp_forward: ") + cudaGetErrorString(e));
     m->launches += 4;
@@ -232,6 +244,26 @@ int dm_mlp_forward_gated(dm_mlp* m, const float* d_obs, const float* d_goal, con
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return mlp_fail(std::string("dm_mlp_forward_gated: ") + cudaGetErrorString(e));
     m->launches += 6;
+    return 0;
+}
+
+int dm_mlp_forward_style_reward(dm_mlp* m, const float* d_amp_obs, const float* d_task_reward, float task_lerp, float* d_logit, float* d_style, float* d_reward,
+                                int rows, void* stream) {
+    if (!m) return mlp_fail("dm_mlp_forward_style_reward: null handle");
+    if (m->gated) return mlp_fail("dm_mlp_forward_style_reward: the handle holds a gated actor (dm_mlp_create_gated); a discriminator is a plain handle");
+    if (m->out_dim != 1) return mlp_fail("dm_mlp_forward_style_reward: a discriminator has one output (out_dim " + std::to_string(m->out_dim) + ")");
+    if (!(task_lerp >= 0.f && task_lerp <= 1.f)) return mlp_fail("dm_mlp_forward_style_reward: task_lerp must be in [0, 1]");
+    if (rows <= 0 || rows > m->max_rows) return mlp_fail("dm_mlp_forward_style_reward: rows out of range");
+    if (!d_amp_obs || !d_reward) return mlp_fail("dm_mlp_forward_style_reward: null AMP observation or reward pointer");
+    if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_mlp_forward_style_reward: cudaSetDevice failed");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    dmk::MlpGemmParams P = plain_trunk(m, d_amp_obs, rows, st);
+    // logit head: 512 -> 1, then the style reward and its blend with the task reward
+    const dmk::MlpStyleParams S{d_task_reward, d_logit, d_style, d_reward, task_lerp};
+    dmk::dm_mlp_style_reward_kernel<<<dim3((rows + 127) / 128, 1), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P, S);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return mlp_fail(std::string("dm_mlp_forward_style_reward: ") + cudaGetErrorString(e));
+    m->launches += 4;
     return 0;
 }
 

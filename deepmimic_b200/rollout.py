@@ -5,11 +5,14 @@ N environments of a rank at once with observations, actions and rewards staying 
   DeviceNormalizer   R/learning/normalizer.py (mean / std / clip, group-wise running statistics), torch tensors
   GaussianMLPPolicy  actor of PPOAgent: fc_2layers_1024units -> Gaussian mean (+ state-independent log-std bias = log(noise))
                      (R/learning/ppo_agent.py:52-90, pg_agent.py:140-160, nets/fc_2layers_1024units.py, tf_util.py:27-39)
+  Discriminator      the AMP agent's discriminator (R/learning/amp_agent.py): fc_2layers_1024units over the normalised AMP observation, one-unit
+                     logit; its style reward max(0, 1 - 0.25 (1 - d)^2) is the AMP paper's least-squares reward (Peng et al. 2021, eq. 7)
   BatchedRollout     record_state -> normalise -> actor -> un-normalise -> set_action -> 20 x update -> reward / flags -> masked reset,
-                     collecting [T, N, .] trajectory tensors for a learner
+                     collecting [T, N, .] trajectory tensors for a learner; with a discriminator also the agent's AMP observation of every
+                     transition and the style reward (blended with the task reward in the AMP task scenes) that an AMP learner trains on
 
-With backend "torch" the MLP runs as plain torch matmuls (cuBLAS); with backend "tensor_core" the actor's inference (plain or gated) runs on
-the library's own wgmma kernels (kernels/dm_mlp.cu).  The reference's TF1 checkpoints
+With backend "torch" the MLPs run as plain torch matmuls (cuBLAS); with backend "tensor_core" the actor's inference (plain or gated) and the
+discriminator's reward run on the library's own wgmma kernels (kernels/dm_mlp.cu).  The reference's TF1 checkpoints
 are read by deepmimic_b200/tf_checkpoint.py (TensorBundle reader, no TensorFlow) and loaded with load_actor_weights; without a
 checkpoint the weights are random-initialised the way the reference initialises them."""
 import math
@@ -164,6 +167,51 @@ def build_gated_policy(state_size, goal_size, action_size, init_output_scale=0.0
     return GatedGaussianMLPPolicy()
 
 
+def build_discriminator(amp_obs_size, hidden=(1024, 512), init_output_scale=1.0):
+    """The AMP agent's discriminator (R/learning/amp_agent.py): the fc_2layers_1024units ReLU trunk (xavier-uniform weights, zero biases) over
+    the normalised AMP observation and a one-unit linear logit whose weights are uniform in [-init_output_scale, init_output_scale].
+    forward(norm_amp_obs) returns the logits [rows, 1]."""
+    import torch
+
+    class Discriminator(torch.nn.Module):
+        def __init__(self):
+            super().__init__()
+            dims = [amp_obs_size] + list(hidden)
+            self.hidden = torch.nn.ModuleList([torch.nn.Linear(a, b) for a, b in zip(dims[:-1], dims[1:])])
+            for l in self.hidden:
+                torch.nn.init.xavier_uniform_(l.weight); torch.nn.init.zeros_(l.bias)
+            self.logit = torch.nn.Linear(dims[-1], 1)
+            torch.nn.init.uniform_(self.logit.weight, -init_output_scale, init_output_scale); torch.nn.init.zeros_(self.logit.bias)
+
+        def forward(self, norm_amp_obs):
+            h = norm_amp_obs
+            for l in self.hidden:
+                h = torch.relu(l(h))
+            return self.logit(h)
+
+    return Discriminator()
+
+
+def amp_rewards(logits, task_reward=None, task_lerp=0.0):
+    """(style, reward) from discriminator logits d: style = max(0, 1 - 0.25 (1 - d)^2) (Peng et al. 2021, eq. 7) and the reward an AMP
+    learner trains on, (1 - task_lerp) style + task_lerp task_reward, or style without a task reward."""
+    style = (1.0 - 0.25 * (1.0 - logits) ** 2).clamp_min(0.0)
+    return style, (style if task_reward is None else (1.0 - task_lerp) * style + task_lerp * task_reward)
+
+
+def load_disc_weights(disc, d):
+    """Copies discriminator weights {"hidden": [(w, b), ...], "logit": (w, b)} into a Discriminator (build_discriminator).  TF dense kernels are
+    [in, out]; torch Linear weights are [out, in]."""
+    import torch
+    if len(d["hidden"]) != len(disc.hidden):
+        raise ValueError("the discriminator has %d hidden layers, the weights %d" % (len(disc.hidden), len(d["hidden"])))
+    f = lambda a: torch.as_tensor(np.asarray(a, dtype=np.float32))
+    with torch.no_grad():
+        for layer, (w, b) in zip(list(disc.hidden) + [disc.logit], list(d["hidden"]) + [d["logit"]]):
+            layer.weight.copy_(f(w).reshape(layer.weight.shape[::-1]).t()); layer.bias.copy_(f(b).reshape(layer.bias.shape))
+    return disc
+
+
 def load_actor_weights(policy, actor):
     """Copies a reference actor (deepmimic_b200.tf_checkpoint.load_actor, or the tests/golden fixture keys w0 b0 w1 b1 wm bm logstd) into a
     GaussianMLPPolicy.  TF dense kernels are [in, out]; torch Linear weights are [out, in]."""
@@ -199,9 +247,15 @@ class BatchedRollout:
     stream.  The plain 2-layer actor: normaliser, three GEMMs, bias / ReLU and the action un-normalisation in four launches (operand preparation
     + one per layer).  The gated actor of the goal-conditioned task scenes: six launches (operand preparation of [state | goal], gate trunk, both
     gate hidden layers, the two gated trunk layers, output layer).  The weights and the normaliser statistics are snapshotted by
-    refresh_tensor_core_policy() (call it again after a learner update)."""
+    refresh_tensor_core_policy() (call it again after a learner update).
 
-    def __init__(self, env, policy=None, exp_rate=1.0, noise=0.05, seed=0, backend="torch"):
+    disc (AMP scenes only): a Discriminator (build_discriminator) over the normalised agent AMP observation (normaliser amp_norm).  collect()
+    then also returns the agent's AMP observation of every transition and the discriminator's logits, style rewards and amp_rewards, the reward
+    an AMP learner trains on: the style reward in imitate_amp (the scene's own reward is not used there), (1 - task_reward_lerp) style +
+    task_reward_lerp task reward in the task scenes, which need task_reward_lerp.  On the tensor_core backend the discriminator's reward runs in
+    four launches (operand preparation, two hidden layers, the logit head with the reward epilogue)."""
+
+    def __init__(self, env, policy=None, exp_rate=1.0, noise=0.05, seed=0, backend="torch", disc=None, task_reward_lerp=None):
         import torch
         self.torch, self.env = torch, env
         dev = env.device
@@ -221,9 +275,27 @@ class BatchedRollout:
         self.backend, self._tc = backend, None
         if backend not in ("torch", "tensor_core"):
             raise ValueError("backend must be 'torch' or 'tensor_core'")
+        self.disc, self._tc_disc = None, None
+        if disc is not None:
+            if "AMP" not in env.get_name():
+                raise ValueError("a discriminator needs an AMP scene (this one is %r)" % env.get_name())
+            self._amp_task_reward = env.enable_amp_task_reward()
+            if self._amp_task_reward:
+                # the reference reads TaskRewardLerp from the agent file; there is no default to fall back on
+                if task_reward_lerp is None or not 0.0 <= float(task_reward_lerp) <= 1.0:
+                    raise ValueError("scene %r blends style and task rewards: task_reward_lerp in [0, 1] is required" % env.get_name())
+                self.task_reward_lerp = float(task_reward_lerp)
+            elif task_reward_lerp:
+                raise ValueError("scene %r has no AMP task reward: task_reward_lerp must be 0 or None" % env.get_name())
+            else:
+                self.task_reward_lerp = 0.0
+            self.disc = disc.to(dev)
+            M = env.get_amp_obs_size()
+            self.amp_norm = DeviceNormalizer(M, env.get_amp_obs_norm_group(), device=dev)
+            self.amp_norm.set_mean_std(-env.get_amp_obs_offset(), 1.0 / env.get_amp_obs_scale())
 
     def refresh_tensor_core_policy(self):
-        """(re)builds the dm_mlp handle from the current torch policy and normalisers"""
+        """(re)builds the dm_mlp handles from the current torch policy, discriminator and normalisers"""
         from .capi import TensorCoreGatedMLP, TensorCoreMLP
         pol, env = self.policy, self.env
         if len(pol.hidden) != 2:
@@ -243,6 +315,15 @@ class BatchedRollout:
                                      in_mean=g(self.s_norm.mean), in_std=g(self.s_norm.std), in_clip=self.s_norm.clip, out_mean=g(self.a_norm.mean), out_std=g(self.a_norm.std),
                                      max_rows=env.num_envs, device=env.device.index or 0)
         self._tc_act = self.torch.empty(env.num_envs, env.get_action_size(), device=env.device)
+        if self.disc is not None:
+            d = self.disc
+            if len(d.hidden) != 2:
+                raise ValueError("the tensor_core backend implements exactly two hidden layers")
+            if self._tc_disc is not None:
+                self._tc_disc.close()
+            self._tc_disc = TensorCoreMLP(g(d.hidden[0].weight).T, g(d.hidden[0].bias), g(d.hidden[1].weight).T, g(d.hidden[1].bias), g(d.logit.weight).T, g(d.logit.bias),
+                                          in_mean=g(self.amp_norm.mean), in_std=g(self.amp_norm.std), in_clip=self.amp_norm.clip, max_rows=env.num_envs,
+                                          device=env.device.index or 0)
         return self._tc
 
     def _act_tensor_core(self, s, explore, g=None):
@@ -262,12 +343,25 @@ class BatchedRollout:
         logp = (-0.5 * eps * eps - self.policy.logstd.detach() - 0.5 * math.log(2 * math.pi)).sum(dim=-1)
         return self._tc_act, logp
 
+    def _disc_rewards(self, amp, r, out, k):
+        """the discriminator's logits, style rewards and amp_rewards of step k from the agent AMP observations amp and the env rewards r"""
+        task = r if self._amp_task_reward else None
+        logit, style, reward = out["disc_logits"][k], out["style_rewards"][k], out["amp_rewards"][k]
+        if self.backend == "tensor_core":
+            self._tc_disc.style_reward(amp, reward, task_reward=task, task_lerp=self.task_reward_lerp, logit=logit, style=style,
+                                       stream=self.torch.cuda.current_stream(amp.device).cuda_stream)
+        else:
+            d = self.disc(self.amp_norm.normalize(amp))[:, 0]
+            st, rw = amp_rewards(d, task, self.task_reward_lerp)
+            logit.copy_(d); style.copy_(st); reward.copy_(rw)
+
     @property
     def stream(self):
         return self.env.stream
 
     def collect(self, num_steps, record_stats=True):
-        """num_steps policy steps of all environments; returns dict of [T, N, .] tensors (states, actions, logps, rewards, dones)."""
+        """num_steps policy steps of all environments; returns dict of [T, N, .] tensors (states, actions, logps, rewards, dones, terminate; goals
+        in the goal-conditioned scenes; with a discriminator amp_obs, disc_logits, style_rewards, amp_rewards).  rewards is the env's reward."""
         t, env = self.torch, self.env
         N, S, A = env.num_envs, env.get_state_size(), env.get_action_size()
         out = dict(states=t.empty(num_steps, N, S, device=env.device), actions=t.empty(num_steps, N, A, device=env.device),
@@ -276,6 +370,10 @@ class BatchedRollout:
         G = self.goal_size
         if G > 0:
             out["goals"] = t.empty(num_steps, N, G, device=env.device)
+        if self.disc is not None:
+            out["amp_obs"] = t.empty(num_steps, N, env.get_amp_obs_size(), device=env.device)
+            for key in ("disc_logits", "style_rewards", "amp_rewards"):
+                out[key] = t.empty(num_steps, N, device=env.device)
         # the whole loop runs on the environment's stream: with the actor and the bookkeeping on another stream every env call is a pair of
         # cross-stream event waits (measured: 0.4 ms of bubbles per policy step); the caller's stream waits for the trajectory at the end
         caller = t.cuda.current_stream(env.device) if env.device.type == "cuda" else None
@@ -303,6 +401,13 @@ class BatchedRollout:
                     a = self.a_norm.unnormalize(na).contiguous()
                 s, r, done, term = env.step(a)
                 out["actions"][k] = a; out["logps"][k] = logp; out["rewards"][k] = r; out["dones"][k] = done; out["terminate"][k] = term
+                if self.disc is not None:
+                    # before the reset: the last transition of a finished episode is the agent's own motion, not the restarted state
+                    amp = env.record_amp_obs_agent()
+                    out["amp_obs"][k] = amp
+                    if record_stats:
+                        self.amp_norm.record(amp)
+                    self._disc_rewards(out["amp_obs"][k], out["rewards"][k], out, k)
                 env.reset()                # restarts exactly the finished episodes
                 # the restarted environments need the observation of their new state.  Unconditional (one more ~10 us observation kernel) instead of
                 # `if done.any()`: that test is a host synchronisation per policy step, which leaves the GPU idle while the host launches the

@@ -191,7 +191,16 @@ dm_mlp* dm_mlp_create_gated(int device, const dm_mlp_gated_weights* h_weights, i
 /* d_obs [rows x in_dim], d_goal [rows x goal_dim], d_noise [rows x out_dim] or NULL, d_actions [rows x out_dim]: fp32 device pointers.
  * dm_mlp_forward refuses a gated handle and dm_mlp_forward_gated a plain one. */
 int dm_mlp_forward_gated(dm_mlp* m, const float* d_obs, const float* d_goal, const float* d_noise, float* d_actions, int rows, void* stream);
-long long dm_mlp_launches(dm_mlp* m);   /* kernel launches so far: 4 per plain forward, 6 per gated forward */
+/* The style reward of an AMP agent (Peng et al. 2021, "AMP: Adversarial Motion Priors", eq. 7; R/learning/amp_agent.py): the discriminator is a plain
+ * handle from dm_mlp_create with out_dim == 1, the AMP-observation normaliser as its input normaliser and h_out_mean / h_out_std NULL.  Per row r,
+ *   d      = W2^T relu(W1^T relu(W0^T clip((x_r - x_mean) / x_std) + b0) + b1) + b2     (the logit, not un-normalised)
+ *   style  = max(0, 1 - 0.25 (1 - d)^2)
+ *   reward = (1 - task_lerp) style + task_lerp d_task_reward[r],  or style when d_task_reward is NULL.
+ * d_amp_obs [rows x in_dim], d_task_reward / d_logit / d_style / d_reward [rows]: fp32 device pointers; d_task_reward, d_logit and d_style may be
+ * NULL.  Refused: a gated handle, out_dim != 1, task_lerp outside [0, 1] (or NaN), rows out of range, a NULL d_amp_obs or d_reward. */
+int dm_mlp_forward_style_reward(dm_mlp* m, const float* d_amp_obs, const float* d_task_reward, float task_lerp, float* d_logit, float* d_style, float* d_reward,
+                                int rows, void* stream);
+long long dm_mlp_launches(dm_mlp* m);   /* kernel launches so far: 4 per plain forward, 6 per gated forward, 4 per style-reward forward */
 void dm_mlp_destroy(dm_mlp* m);
 
 /* ---- test hooks: raw per-env simulator state, layout shared with the CPU oracle (doubles):

@@ -1,5 +1,6 @@
-"""Times the policy networks alone, CUDA events: the plain actor (4096 x 227 -> 1024 -> 512 -> 28, dm_mlp_forward) and the gated task actor
-(4096 x (226 + 3) -> 1024 -> 512 -> 28 with its gates, dm_mlp_forward_gated) on the wgmma kernels, each against the fp32 torch network."""
+"""Times the networks alone, CUDA events: the plain actor (4096 x 227 -> 1024 -> 512 -> 28, dm_mlp_forward), the gated task actor
+(4096 x (226 + 3) -> 1024 -> 512 -> 28 with its gates, dm_mlp_forward_gated) and the AMP discriminator's reward (4096 x 226 -> 1024 -> 512 -> 1,
+style reward and its blend with a task reward, dm_mlp_forward_style_reward) on the wgmma kernels, each against the fp32 torch network."""
 import os, sys
 import numpy as np
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -54,3 +55,21 @@ t_gtc = timeit(lambda: gmlp.forward(xs, xg, out, noise=noise, stream=st.cuda_str
 t_gth = timeit(torch_gated_actor)
 ref = torch_gated_actor(); torch.cuda.synchronize()
 print("gated policy network, %d rows: wgmma kernels %.1f us per forward, fp32 torch actor %.1f us; max |diff| %.2e" % (rows, t_gtc, t_gth, (out - ref).abs().max().item()))
+
+# the AMP discriminator's reward: normalise, 226 -> 1024 -> 512 -> 1 logit, style reward max(0, 1 - 0.25 (1 - d)^2), blend with a task reward
+da = 226
+disc = dict(hidden=[lin(da, h0), lin(h0, h1)], logit=lin(h1, 1))
+dmlp = TensorCoreMLP(*disc["hidden"][0], *disc["hidden"][1], *disc["logit"], in_mean=mean[:da], in_std=std[:da], in_clip=5.0, max_rows=rows)
+xa, task = x[:, :da].contiguous(), torch.rand(rows, device="cuda")
+logit, style, reward = (torch.zeros(rows, device="cuda") for _ in range(3))
+td = [T(a) for a in (*disc["hidden"][0], *disc["hidden"][1], *disc["logit"])]
+def torch_disc_reward():
+    h = torch.clamp((xa - tn[0]) / tn[1], -5, 5)
+    h = torch.relu(h @ td[0] + td[1]); h = torch.relu(h @ td[2] + td[3]); d = (h @ td[4] + td[5])[:, 0]
+    s = (1.0 - 0.25 * (1.0 - d) ** 2).clamp_min(0.0)
+    return d, 0.5 * s + 0.5 * task
+t_dtc = timeit(lambda: dmlp.style_reward(xa, reward, task_reward=task, task_lerp=0.5, logit=logit, style=style, stream=st.cuda_stream))
+t_dth = timeit(torch_disc_reward)
+ref_d, ref_r = torch_disc_reward(); torch.cuda.synchronize()
+print("discriminator reward, %d rows: wgmma kernels %.1f us per forward, fp32 torch discriminator + reward ops %.1f us; max |logit diff| %.2e, max |reward diff| %.2e"
+      % (rows, t_dtc, t_dth, (logit - ref_d).abs().max().item(), (reward - ref_r).abs().max().item()))

@@ -1,6 +1,7 @@
 """Where does a device-resident rollout step spend its time?  CUDA events around the actor and around the environment step, host time per step,
 for both actor backends (diagnosis tool for the rollout rates of tests/test_mlp_gpu.py and tests/test_mlp_gated_gpu.py): the spin-kick imitation
-scene with the plain actor, then the target_amp task scene with the gated actor."""
+scene with the plain actor, then the target_amp task scene with the gated actor; then the target_amp rollout rate without and with the AMP
+discriminator (agent AMP observations and amp_rewards recorded every step, tests/test_amp_reward_gpu.py) on both backends."""
 import os, sys, time
 import numpy as np
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -8,7 +9,7 @@ sys.path.insert(0, REPO)
 import torch
 from deepmimic_b200.assets import asset_root
 from deepmimic_b200.env import DeepMimicBatchEnv
-from deepmimic_b200.rollout import BatchedRollout, build_gated_policy, build_policy, load_actor_weights
+from deepmimic_b200.rollout import BatchedRollout, build_discriminator, build_gated_policy, build_policy, load_actor_weights
 sys.path.insert(0, os.path.join(REPO, "tests"))
 from test_task_scenes_cpu import fixture_task_actor
 f = np.load(os.path.join(REPO, "tests", "golden", "policy_humanoid3d_spinkick_fp16.npz"))
@@ -55,3 +56,21 @@ for scene, backend in [("spinkick", "tensor_core"), ("spinkick", "torch"), ("spi
     g = lambda i, j: np.median([x[i].elapsed_time(x[j]) for x in ev])
     print("%-8s %-11s collect(48): %.0f steps/s | manual loop: actor %.3f ms, env.step %.3f ms, reset+observe %.3f ms (GPU, median) ; host enqueue %.3f ms/step, wall %.3f ms/step"
           % (scene, backend, 4096 * 48 / dt, g(0, 1), g(1, 2), g(2, 3), 1e3 * host / 32, 1e3 * wall / 32))
+
+# target_amp collect() rate with and without the discriminator, alternating; best of two 48-step windows each
+for backend in ("tensor_core", "torch"):
+    rates = {}
+    for with_disc in (False, True, False, True):
+        env = DeepMimicBatchEnv(TARGET, num_envs=4096, asset_root=root, seed=4)
+        env.reset(True)
+        torch.manual_seed(0)
+        extra = dict(disc=build_discriminator(env.get_amp_obs_size()), task_reward_lerp=0.5) if with_disc else {}
+        ro = BatchedRollout(env, policy=load_actor_weights(build_gated_policy(226, 3, 28), at), exp_rate=1.0, backend=backend, **extra)
+        ro.s_norm.set_mean_std(at["s_norm_mean"], at["s_norm_std"]); ro.g_norm.set_mean_std(at["g_norm_mean"], at["g_norm_std"]); ro.a_norm.set_mean_std(at["a_norm_mean"], at["a_norm_std"])
+        ro.collect(8, record_stats=False); torch.cuda.synchronize()
+        for _ in range(2):
+            t0 = time.perf_counter(); ro.collect(48, record_stats=False); torch.cuda.synchronize()
+            rates[with_disc] = max(rates.get(with_disc, 0.0), 4096 * 48 / (time.perf_counter() - t0))
+        assert env.counters()[1] == 0
+        del ro, env
+    print("target_amp %-11s collect(48): %.0f steps/s without the discriminator, %.0f with it" % (backend, rates[False], rates[True]))
