@@ -31,7 +31,7 @@ DM_STATE_OFFSET, DM_STATE_SCALE, DM_ACTION_OFFSET, DM_ACTION_SCALE, DM_ACTION_BO
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
            "dm_update", "dm_record_state", "dm_record_goal", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
            "dm_set_snapshot", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
-           "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy"]
+           "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy", "dm_td_lambda_returns"]
 
 
 def lib():
@@ -106,12 +106,30 @@ def lib():
         L.dm_mlp_launches.restype = C.c_longlong
         L.dm_mlp_launches.argtypes = [vp]
         L.dm_mlp_destroy.argtypes = [vp]
+        L.dm_td_lambda_returns.argtypes = [vp] * 5 + [C.c_int, C.c_int] + [C.c_float] * 4 + [vp, vp, vp]
         _lib = L
     return _lib
 
 
 def _dptr(a):
     return a.ctypes.data_as(C.POINTER(C.c_double)) if a is not None else None
+
+
+def td_lambda_returns(rewards, values, end_values, done, terminate, discount, td_lambda, val_fail, val_succ, returns, advantages, stream=None):
+    """dm_td_lambda_returns: TD(lambda) returns and advantages of a [T, N] rollout window on the device.  rewards, values, end_values, returns,
+    advantages: contiguous float32 CUDA tensors [T, N]; done: bool (or uint8) [T, N]; terminate: int32 [T, N]; stream: cudaStream_t handle (int)
+    or None.  returns and advantages are written."""
+    T, N = rewards.shape
+    for name, x, dt in (("rewards", rewards, "float32"), ("values", values, "float32"), ("end_values", end_values, "float32"), ("returns", returns, "float32"),
+                        ("advantages", advantages, "float32"), ("done", done, ("bool", "uint8")), ("terminate", terminate, "int32")):
+        if tuple(x.shape) != (T, N) or not x.is_contiguous() or not x.is_cuda or str(x.dtype).replace("torch.", "") not in (dt if isinstance(dt, tuple) else (dt,)):
+            raise ValueError("td_lambda_returns: %s must be a contiguous %s CUDA tensor [%d, %d]" % (name, dt, T, N))
+    ptr = lambda t: C.c_void_p(t.data_ptr())
+    rc = lib().dm_td_lambda_returns(ptr(rewards), ptr(values), ptr(end_values), ptr(done), ptr(terminate), T, N, float(discount), float(td_lambda),
+                                    float(val_fail), float(val_succ), ptr(returns), ptr(advantages), C.c_void_p(stream) if stream else None)
+    if rc != 0:
+        raise RuntimeError("dm_td_lambda_returns: %s" % lib().dm_last_error().decode())
+    return returns, advantages
 
 
 class BatchedCore:

@@ -1,7 +1,8 @@
 // C ABI of the tensor-core policy network (include/deepmimic_b200.h, dm_mlp_*): host-side weight tiling + the launches of kernels/dm_mlp.cu: four for
 // the plain actor (operand preparation, three GEMMs), six for the gated one (operand preparation, gate trunk, both gate hidden layers, two gated
 // trunk layers, output layer), four for the AMP discriminator's style reward (operand preparation, two GEMMs, the logit head with the reward
-// epilogue).  Same library, same rules: no CPU fallback, errors through dm_last_error.
+// epilogue); and the learner-side TD(lambda) return scan of a rollout window (kernels/dm_returns.cu, one launch).  Same library, same rules: no
+// CPU fallback, errors through dm_last_error.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
@@ -30,6 +31,7 @@ template <int BN, bool LAST>
 __global__ void dm_mlp_gemm_kernel(MlpGemmParams);
 __global__ void dm_mlp_gated_gemm_kernel(MlpGemmParams);
 __global__ void dm_mlp_style_reward_kernel(MlpGemmParams, MlpStyleParams);
+__global__ void dm_td_lambda_kernel(const float*, const float*, const float*, const uint8_t*, const int32_t*, int, int, float, float, float, float, float*, float*);
 int dm_mlp_smem_bytes(int bn);
 constexpr int kMlpATileHalves = 128 * 64;   // one operand tile of activations (kernels/dm_mlp.cu: kMlpATile)
 }  // namespace dmk
@@ -264,6 +266,20 @@ int dm_mlp_forward_style_reward(dm_mlp* m, const float* d_amp_obs, const float* 
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return mlp_fail(std::string("dm_mlp_forward_style_reward: ") + cudaGetErrorString(e));
     m->launches += 4;
+    return 0;
+}
+
+int dm_td_lambda_returns(const float* d_rewards, const float* d_values, const float* d_end_values, const uint8_t* d_done, const int32_t* d_terminate, int T, int N,
+                         float discount, float td_lambda, float val_fail, float val_succ, float* d_returns, float* d_advantages, void* stream) {
+    if (T <= 0 || N <= 0) return mlp_fail("dm_td_lambda_returns: T and N must be positive");
+    if (!(discount >= 0.f && discount < 1.f)) return mlp_fail("dm_td_lambda_returns: discount must be in [0, 1)");
+    if (!(td_lambda >= 0.f && td_lambda <= 1.f)) return mlp_fail("dm_td_lambda_returns: td_lambda must be in [0, 1]");
+    if (!d_rewards || !d_values || !d_end_values || !d_done || !d_terminate || !d_returns || !d_advantages) return mlp_fail("dm_td_lambda_returns: null pointer");
+    constexpr int kThreads = 64;   // N = 4096 environments -> 64 CTAs on 64 SMs: the scan is latency-bound, more SMs keep more loads in flight
+    dmk::dm_td_lambda_kernel<<<(N + kThreads - 1) / kThreads, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+        d_rewards, d_values, d_end_values, d_done, d_terminate, T, N, discount, td_lambda, val_fail, val_succ, d_returns, d_advantages);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return mlp_fail(std::string("dm_td_lambda_returns: ") + cudaGetErrorString(e));
     return 0;
 }
 

@@ -7,12 +7,16 @@ N environments of a rank at once with observations, actions and rewards staying 
                      (R/learning/ppo_agent.py:52-90, pg_agent.py:140-160, nets/fc_2layers_1024units.py, tf_util.py:27-39)
   Discriminator      the AMP agent's discriminator (R/learning/amp_agent.py): fc_2layers_1024units over the normalised AMP observation, one-unit
                      logit; its style reward max(0, 1 - 0.25 (1 - d)^2) is the AMP paper's least-squares reward (Peng et al. 2021, eq. 7)
+  Critic             the PPO critic (R/learning/ppo_agent.py: _build_net_critic): the actor's trunk over the actor's normalised inputs, a
+                     one-unit output un-normalised by the value normaliser (val_norm_from_rewards; terminal_values gives val_fail / val_succ)
   BatchedRollout     record_state -> normalise -> actor -> un-normalise -> set_action -> 20 x update -> reward / flags -> masked reset,
                      collecting [T, N, .] trajectory tensors for a learner; with a discriminator also the agent's AMP observation of every
-                     transition and the style reward (blended with the task reward in the AMP task scenes) that an AMP learner trains on
+                     transition and the style reward (blended with the task reward in the AMP task scenes) that an AMP learner trains on;
+                     with a critic also the values of every state and of every step's pre-reset end state, and the TD(lambda) returns and
+                     advantages of the window (R/learning/rl_util.py: compute_return), scanned on the device (kernels/dm_returns.cu)
 
-With backend "torch" the MLPs run as plain torch matmuls (cuBLAS); with backend "tensor_core" the actor's inference (plain or gated) and the
-discriminator's reward run on the library's own wgmma kernels (kernels/dm_mlp.cu).  The reference's TF1 checkpoints
+With backend "torch" the MLPs run as plain torch matmuls (cuBLAS); with backend "tensor_core" the actor's inference (plain or gated), the
+discriminator's reward and the critic's values run on the library's own wgmma kernels (kernels/dm_mlp.cu).  The reference's TF1 checkpoints
 are read by deepmimic_b200/tf_checkpoint.py (TensorBundle reader, no TensorFlow) and loaded with load_actor_weights; without a
 checkpoint the weights are random-initialised the way the reference initialises them."""
 import math
@@ -147,12 +151,7 @@ def build_gated_policy(state_size, goal_size, action_size, init_output_scale=0.0
             self.logstd = torch.nn.Parameter(torch.full((action_size,), math.log(noise)))
 
         def forward(self, norm_s, norm_g):
-            gc = torch.relu(self.gate_common(norm_g))
-            h = torch.cat([norm_s, norm_g], dim=-1)
-            for l, gh, gb, gs in zip(self.hidden, self.gate_hidden, self.gate_bias, self.gate_scale):
-                gate = torch.relu(gh(gc))
-                h = torch.relu(2.0 * torch.sigmoid(gs(gate)) * l(h) + gb(gate))
-            return self.mean(h)
+            return self.mean(_gated_trunk(self, norm_s, norm_g))
 
         def sample(self, norm_s, norm_g, explore_mask=None, generator=None):
             mu = self.forward(norm_s, norm_g)
@@ -165,6 +164,71 @@ def build_gated_policy(state_size, goal_size, action_size, init_output_scale=0.0
             return a, logp
 
     return GatedGaussianMLPPolicy()
+
+
+def _gated_trunk(net, norm_s, norm_g):
+    """the hidden layers of fc_2layers_gated_1024units (net: hidden, gate_common, gate_hidden, gate_bias, gate_scale)"""
+    import torch
+    gc = torch.relu(net.gate_common(norm_g))
+    h = torch.cat([norm_s, norm_g], dim=-1)
+    for l, gh, gb, gs in zip(net.hidden, net.gate_hidden, net.gate_bias, net.gate_scale):
+        gate = torch.relu(gh(gc))
+        h = torch.relu(2.0 * torch.sigmoid(gs(gate)) * l(h) + gb(gate))
+    return h
+
+
+def build_critic(state_size, goal_size=0, hidden=(1024, 512), gate_common=128, gate_hidden=64):
+    """The PPO critic (PPOAgent._build_net_critic, R/learning/ppo_agent.py): a trunk over the actor's own normalised inputs, then a one-unit
+    linear output, the normalised value; V = val_norm.unnormalize(output).  The trunk is the one this rollout builds for the actor: the plain
+    fc_2layers_1024units over norm_s when goal_size is 0, the gated fc_2layers_gated_1024units over (norm_s, norm_g) otherwise.  The reference
+    names the critic's network in an agent file, and the asset archive has no agent files.  Xavier-uniform weights and zero biases everywhere,
+    the output layer included (tf.contrib.layers.xavier_initializer).  forward(norm_s[, norm_g]) returns [rows, 1]."""
+    import torch
+
+    class Critic(torch.nn.Module):
+        def __init__(self):
+            super().__init__()
+            lin = torch.nn.Linear
+            dims = [state_size + goal_size] + list(hidden)
+            self.goal_size = goal_size
+            self.hidden = torch.nn.ModuleList([lin(a, b) for a, b in zip(dims[:-1], dims[1:])])
+            layers = list(self.hidden)
+            if goal_size > 0:
+                self.gate_common = lin(goal_size, gate_common)
+                self.gate_hidden = torch.nn.ModuleList([lin(gate_common, gate_hidden) for _ in hidden])
+                self.gate_bias = torch.nn.ModuleList([lin(gate_hidden, h) for h in hidden])
+                self.gate_scale = torch.nn.ModuleList([lin(gate_hidden, h) for h in hidden])
+                layers += [self.gate_common] + list(self.gate_hidden) + list(self.gate_bias) + list(self.gate_scale)
+            self.out = lin(dims[-1], 1)
+            for l in layers + [self.out]:
+                torch.nn.init.xavier_uniform_(l.weight); torch.nn.init.zeros_(l.bias)
+
+        def forward(self, norm_s, norm_g=None):
+            if self.goal_size > 0:
+                return self.out(_gated_trunk(self, norm_s, norm_g))
+            h = norm_s
+            for l in self.hidden:
+                h = torch.relu(l(h))
+            return self.out(h)
+
+    return Critic()
+
+
+def val_norm_from_rewards(env, discount, device="cpu"):
+    """The value normaliser of PGAgent (_calc_val_bounds, _calc_val_offset_scale): values lie in [r_min, r_max] / (1 - discount), so
+    mean = (val_max + val_min) / 2 and std = (val_max - val_min) / 2 (mean 10, std 10 for rewards in [0, 1] at discount 0.95)."""
+    val_min, val_max = env.get_reward_min() / (1.0 - discount), env.get_reward_max() / (1.0 - discount)
+    n = DeviceNormalizer(1, device=device)
+    n.set_mean_std([0.5 * (val_max + val_min)], [0.5 * (val_max - val_min)])
+    return n
+
+
+def terminal_values(env, discount):
+    """(val_fail, val_succ) of RLAgent._calc_term_vals: the value of a failed / succeeded episode's terminal state, r / (1 - discount), 0 at
+    discount 0"""
+    if discount == 0:
+        return 0.0, 0.0
+    return env.get_reward_fail() / (1.0 - discount), env.get_reward_succ() / (1.0 - discount)
 
 
 def build_discriminator(amp_obs_size, hidden=(1024, 512), init_output_scale=1.0):
@@ -212,6 +276,26 @@ def load_disc_weights(disc, d):
     return disc
 
 
+def load_critic_weights(critic, d):
+    """Copies critic weights (deepmimic_b200.tf_checkpoint.load_critic: {"hidden": [(w, b), ...], "out": (w, b)}, and "gate_common" / "gates"
+    for the gated trunk) into a Critic (build_critic).  TF dense kernels are [in, out]; torch Linear weights are [out, in]."""
+    import torch
+    if len(d["hidden"]) != len(critic.hidden):
+        raise ValueError("the critic has %d hidden layers, the weights %d" % (len(critic.hidden), len(d["hidden"])))
+    if ("gate_common" in d) != (critic.goal_size > 0):
+        raise ValueError("gated weights need a goal-conditioned critic and plain weights a plain one")
+    f = lambda a: torch.as_tensor(np.asarray(a, dtype=np.float32))
+    pairs = list(zip(critic.hidden, d["hidden"])) + [(critic.out, d["out"])]
+    if critic.goal_size > 0:
+        pairs.append((critic.gate_common, d["gate_common"]))
+        for i, g in enumerate(d["gates"]):
+            pairs += [(critic.gate_hidden[i], g["hidden"]), (critic.gate_bias[i], g["bias"]), (critic.gate_scale[i], g["scale"])]
+    with torch.no_grad():
+        for layer, (w, b) in pairs:
+            layer.weight.copy_(f(w).reshape(layer.weight.shape[::-1]).t()); layer.bias.copy_(f(b).reshape(layer.bias.shape))
+    return critic
+
+
 def load_actor_weights(policy, actor):
     """Copies a reference actor (deepmimic_b200.tf_checkpoint.load_actor, or the tests/golden fixture keys w0 b0 w1 b1 wm bm logstd) into a
     GaussianMLPPolicy.  TF dense kernels are [in, out]; torch Linear weights are [out, in]."""
@@ -231,6 +315,20 @@ def load_actor_weights(policy, actor):
             for i, g in enumerate(actor["gates"]):
                 put(policy.gate_hidden[i], g["hidden"]); put(policy.gate_bias[i], g["bias"]); put(policy.gate_scale[i], g["scale"])
     return policy
+
+
+def td_lambda_returns_host(rewards, values, end_values, done, terminate, discount, td_lambda, val_fail, val_succ, returns, advantages):
+    """dm_td_lambda_returns's rule as torch ops on CPU tensors [T, N] (a CPU device has no kernel; on a CUDA device collect() always runs the
+    kernel, capi.td_lambda_returns): returns and advantages are written."""
+    import torch as t
+    v_next = t.where(done & (terminate == 1), t.full_like(end_values, val_fail), end_values)
+    v_next = t.where(done & (terminate == 2), t.full_like(end_values, val_succ), v_next)
+    T = rewards.shape[0]
+    for k in range(T - 1, -1, -1):
+        g_next = v_next[k] if k == T - 1 else t.where(done[k], v_next[k], returns[k + 1])
+        returns[k] = rewards[k] + discount * ((1.0 - td_lambda) * v_next[k] + td_lambda * g_next)
+    advantages.copy_(returns - values)
+    return returns, advantages
 
 
 class _nullcontext:
@@ -253,9 +351,16 @@ class BatchedRollout:
     then also returns the agent's AMP observation of every transition and the discriminator's logits, style rewards and amp_rewards, the reward
     an AMP learner trains on: the style reward in imitate_amp (the scene's own reward is not used there), (1 - task_reward_lerp) style +
     task_reward_lerp task reward in the task scenes, which need task_reward_lerp.  On the tensor_core backend the discriminator's reward runs in
-    four launches (operand preparation, two hidden layers, the logit head with the reward epilogue)."""
+    four launches (operand preparation, two hidden layers, the logit head with the reward epilogue).
 
-    def __init__(self, env, policy=None, exp_rate=1.0, noise=0.05, seed=0, backend="torch", disc=None, task_reward_lerp=None):
+    critic: a Critic (build_critic) with discount and td_lambda, which the reference reads from the agent file (Discount, TDLambda; there is no
+    default).  val_norm is built from the env's reward bounds (val_norm_from_rewards).  collect() then also evaluates the critic on every
+    state s_k and on the state s'_k each step ends in, before the reset (the terminal state of a finished episode, which RLAgent._end_path
+    keeps), and runs the TD(lambda) return scan of rl_util.compute_return on the device (dm_td_lambda_returns, on either backend).  On the
+    tensor_core backend the critic runs as one forward over the 2N rows [s_k; s'_k] on the plain or gated dm_mlp kernels."""
+
+    def __init__(self, env, policy=None, exp_rate=1.0, noise=0.05, seed=0, backend="torch", disc=None, task_reward_lerp=None, critic=None,
+                 discount=None, td_lambda=None):
         import torch
         self.torch, self.env = torch, env
         dev = env.device
@@ -293,9 +398,25 @@ class BatchedRollout:
             M = env.get_amp_obs_size()
             self.amp_norm = DeviceNormalizer(M, env.get_amp_obs_norm_group(), device=dev)
             self.amp_norm.set_mean_std(-env.get_amp_obs_offset(), 1.0 / env.get_amp_obs_scale())
+        self.critic, self._tc_critic = None, None
+        if critic is None:
+            if discount is not None or td_lambda is not None:
+                raise ValueError("discount and td_lambda are the critic's: they need a critic")
+        else:
+            # the reference reads Discount and TDLambda from the agent file; there is no default to fall back on
+            if discount is None or not 0.0 <= float(discount) < 1.0:
+                raise ValueError("a critic needs a discount in [0, 1)")
+            if td_lambda is None or not 0.0 <= float(td_lambda) <= 1.0:
+                raise ValueError("a critic needs a td_lambda in [0, 1]")
+            if getattr(critic, "goal_size", 0) != G:
+                raise ValueError("the critic sees %d goal values, the scene has %d" % (getattr(critic, "goal_size", 0), G))
+            self.critic = critic.to(dev)
+            self.discount, self.td_lambda = float(discount), float(td_lambda)
+            self.val_norm = val_norm_from_rewards(env, self.discount, device=dev)
+            self.val_fail, self.val_succ = terminal_values(env, self.discount)
 
     def refresh_tensor_core_policy(self):
-        """(re)builds the dm_mlp handles from the current torch policy, discriminator and normalisers"""
+        """(re)builds the dm_mlp handles from the current torch policy, discriminator, critic and normalisers"""
         from .capi import TensorCoreGatedMLP, TensorCoreMLP
         pol, env = self.policy, self.env
         if len(pol.hidden) != 2:
@@ -303,11 +424,11 @@ class BatchedRollout:
         g = lambda t: t.detach().float().cpu().numpy()
         if self._tc is not None:
             self._tc.close()
+        wb = lambda l: (g(l.weight).T, g(l.bias))
+        gated = lambda net, head: dict(hidden=[wb(l) for l in net.hidden], mean=wb(head), gate_common=wb(net.gate_common),
+                                       gates=[dict(hidden=wb(h), scale=wb(sc), bias=wb(b)) for h, sc, b in zip(net.gate_hidden, net.gate_scale, net.gate_bias)])
         if self.goal_size > 0:
-            wb = lambda l: (g(l.weight).T, g(l.bias))
-            actor = dict(hidden=[wb(l) for l in pol.hidden], mean=wb(pol.mean), gate_common=wb(pol.gate_common),
-                         gates=[dict(hidden=wb(h), scale=wb(sc), bias=wb(b)) for h, sc, b in zip(pol.gate_hidden, pol.gate_scale, pol.gate_bias)])
-            self._tc = TensorCoreGatedMLP(actor, s_mean=g(self.s_norm.mean), s_std=g(self.s_norm.std), s_clip=self.s_norm.clip, g_mean=g(self.g_norm.mean),
+            self._tc = TensorCoreGatedMLP(gated(pol, pol.mean), s_mean=g(self.s_norm.mean), s_std=g(self.s_norm.std), s_clip=self.s_norm.clip, g_mean=g(self.g_norm.mean),
                                           g_std=g(self.g_norm.std), g_clip=self.g_norm.clip, a_mean=g(self.a_norm.mean), a_std=g(self.a_norm.std),
                                           max_rows=env.num_envs, device=env.device.index or 0)
         else:
@@ -324,6 +445,21 @@ class BatchedRollout:
             self._tc_disc = TensorCoreMLP(g(d.hidden[0].weight).T, g(d.hidden[0].bias), g(d.hidden[1].weight).T, g(d.hidden[1].bias), g(d.logit.weight).T, g(d.logit.bias),
                                           in_mean=g(self.amp_norm.mean), in_std=g(self.amp_norm.std), in_clip=self.amp_norm.clip, max_rows=env.num_envs,
                                           device=env.device.index or 0)
+        if self.critic is not None:
+            c = self.critic
+            if len(c.hidden) != 2:
+                raise ValueError("the tensor_core backend implements exactly two hidden layers")
+            if self._tc_critic is not None:
+                self._tc_critic.close()
+            # one output unit un-normalised by val_norm; 2N rows: [s_k; s'_k] in one forward
+            vm, vs = g(self.val_norm.mean), g(self.val_norm.std)
+            if self.goal_size > 0:
+                self._tc_critic = TensorCoreGatedMLP(gated(c, c.out), s_mean=g(self.s_norm.mean), s_std=g(self.s_norm.std), s_clip=self.s_norm.clip,
+                                                     g_mean=g(self.g_norm.mean), g_std=g(self.g_norm.std), g_clip=self.g_norm.clip, a_mean=vm, a_std=vs,
+                                                     max_rows=2 * env.num_envs, device=env.device.index or 0)
+            else:
+                self._tc_critic = TensorCoreMLP(*wb(c.hidden[0]), *wb(c.hidden[1]), *wb(c.out), in_mean=g(self.s_norm.mean), in_std=g(self.s_norm.std),
+                                                in_clip=self.s_norm.clip, out_mean=vm, out_std=vs, max_rows=2 * env.num_envs, device=env.device.index or 0)
         return self._tc
 
     def _act_tensor_core(self, s, explore, g=None):
@@ -355,13 +491,41 @@ class BatchedRollout:
             st, rw = amp_rewards(d, task, self.task_reward_lerp)
             logit.copy_(d); style.copy_(st); reward.copy_(rw)
 
+    def _critic_values(self, x, g, v):
+        """V (un-normalised) of the rows x [2N, S] (and goals g [2N, G] in the goal-conditioned scenes) into v [2N]"""
+        if self.backend == "tensor_core":
+            st = self.torch.cuda.current_stream(x.device).cuda_stream
+            if g is None:
+                self._tc_critic.forward(x, v[:, None], stream=st)
+            else:
+                self._tc_critic.forward(x, g, v[:, None], stream=st)
+        else:
+            ns = self.s_norm.normalize(x)
+            out = self.critic(ns) if g is None else self.critic(ns, self.g_norm.normalize(g))
+            v.copy_(self.val_norm.unnormalize(out)[:, 0])
+
+    def _returns(self, out):
+        """TD(lambda) returns and advantages of the window over amp_rewards (with a discriminator: AMPAgent trains on them) or rewards"""
+        t = self.torch
+        r = out["amp_rewards"] if self.disc is not None else out["rewards"]
+        args = (r, out["values"], out["end_values"], out["dones"], out["terminate"], self.discount, self.td_lambda, self.val_fail, self.val_succ,
+                out["returns"], out["advantages"])
+        if r.is_cuda:
+            from .capi import td_lambda_returns
+            td_lambda_returns(*args, stream=t.cuda.current_stream(r.device).cuda_stream)
+        else:
+            td_lambda_returns_host(*args)
+
     @property
     def stream(self):
         return self.env.stream
 
     def collect(self, num_steps, record_stats=True):
         """num_steps policy steps of all environments; returns dict of [T, N, .] tensors (states, actions, logps, rewards, dones, terminate; goals
-        in the goal-conditioned scenes; with a discriminator amp_obs, disc_logits, style_rewards, amp_rewards).  rewards is the env's reward."""
+        in the goal-conditioned scenes; with a discriminator amp_obs, disc_logits, style_rewards, amp_rewards; with a critic values = V(s_k),
+        end_values = V(s'_k) of the state step k ended in (before the reset), returns and advantages = returns - values).  rewards is the env's
+        reward.  A path still running at the last step is bootstrapped with its end value, as the reference bootstraps a path that ends by time
+        limit (a deviation: the reference stores only complete paths)."""
         t, env = self.torch, self.env
         N, S, A = env.num_envs, env.get_state_size(), env.get_action_size()
         out = dict(states=t.empty(num_steps, N, S, device=env.device), actions=t.empty(num_steps, N, A, device=env.device),
@@ -374,6 +538,13 @@ class BatchedRollout:
             out["amp_obs"] = t.empty(num_steps, N, env.get_amp_obs_size(), device=env.device)
             for key in ("disc_logits", "style_rewards", "amp_rewards"):
                 out[key] = t.empty(num_steps, N, device=env.device)
+        crit = self.critic is not None
+        if crit:
+            for key in ("values", "end_values", "returns", "advantages"):
+                out[key] = t.empty(num_steps, N, device=env.device)
+            # critic inputs [s_k; s'_k] (and goals) and its outputs [V(s_k) | V(s'_k)] per step
+            x2, v2 = t.empty(2 * N, S, device=env.device), t.empty(num_steps, 2 * N, device=env.device)
+            g2 = t.empty(2 * N, G, device=env.device) if G > 0 else None
         # the whole loop runs on the environment's stream: with the actor and the bookkeeping on another stream every env call is a pair of
         # cross-stream event waits (measured: 0.4 ms of bubbles per policy step); the caller's stream waits for the trajectory at the end
         caller = t.cuda.current_stream(env.device) if env.device.type == "cuda" else None
@@ -383,12 +554,16 @@ class BatchedRollout:
             s = env.record_state()
             for k in range(num_steps):
                 out["states"][k] = s
+                if crit:
+                    x2[:N] = s
                 if record_stats:
                     self.s_norm.record(s)
                 explore = t.rand(N, device=env.device, generator=self.gen) < self.exp_rate
                 if G > 0:   # RLAgent._update_new_action records the goal next to the state (R/learning/rl_agent.py:319-343)
                     g = env.record_goal()
                     out["goals"][k] = g
+                    if crit:
+                        g2[:N] = g
                     if record_stats:
                         self.g_norm.record(g)
                 if self.backend == "tensor_core":
@@ -408,11 +583,20 @@ class BatchedRollout:
                     if record_stats:
                         self.amp_norm.record(amp)
                     self._disc_rewards(out["amp_obs"][k], out["rewards"][k], out, k)
+                if crit:
+                    # before the reset: s'_k of a finished episode is its terminal state (and goal), not the restarted one
+                    x2[N:] = s
+                    if G > 0:
+                        g2[N:] = env.record_goal()
+                    self._critic_values(x2, g2, v2[k])
                 env.reset()                # restarts exactly the finished episodes
                 # the restarted environments need the observation of their new state.  Unconditional (one more ~10 us observation kernel) instead of
                 # `if done.any()`: that test is a host synchronisation per policy step, which leaves the GPU idle while the host launches the
                 # next step's small kernels (measured: 1.52 M -> see tests/test_mlp_gpu.py for the current rates)
                 s = env.record_state()
+            if crit:
+                out["values"].copy_(v2[:, :N]); out["end_values"].copy_(v2[:, N:])
+                self._returns(out)
         if caller is not None:
             caller.wait_stream(env.stream)
         return out

@@ -130,9 +130,32 @@ def load_actor(prefix):
         g = lambda name: (t[a + name + "/kernel"], t[a + name + "/bias"])
         out["gate_common"] = g("gate_common/0/dense")
         out["gates"] = [dict(hidden=g("gate%d/0/dense" % i), bias=g("gate%d/dense" % i), scale=g("gate%d/dense_1" % i)) for i in range(len(hidden))]
-    for nm in ("s_norm", "g_norm", "a_norm"):
+    _add_norms(out, t, ("s_norm", "g_norm", "a_norm"))
+    return out
+
+
+def load_critic(prefix):
+    """The PPO critic of a reference checkpoint (PPOAgent._build_net_critic, R/learning/ppo_agent.py): the hidden layers under
+    agent/main/critic/<i>/dense, the one-unit output layer agent/main/critic/dense, the gate layers of fc_2layers_gated_1024units named as in
+    load_actor, and the value normaliser agent/resource/val_norm (plus s_norm / g_norm, which the critic shares with the actor) when present.
+    These names follow the actor's scopes; they have not been checked against a checkpoint the reference wrote with its critic."""
+    t = load_checkpoint(prefix)
+    c = "agent/main/critic/"
+    g = lambda name: (t[c + name + "/kernel"], t[c + name + "/bias"])
+    hidden = []
+    while c + "%d/dense/kernel" % len(hidden) in t:
+        hidden.append(g("%d/dense" % len(hidden)))
+    out = dict(hidden=hidden, out=g("dense"))
+    if c + "gate_common/0/dense/kernel" in t:
+        out["gate_common"] = g("gate_common/0/dense")
+        out["gates"] = [dict(hidden=g("gate%d/0/dense" % i), bias=g("gate%d/dense" % i), scale=g("gate%d/dense_1" % i)) for i in range(len(hidden))]
+    _add_norms(out, t, ("s_norm", "g_norm", "val_norm"))
+    return out
+
+
+def _add_norms(out, t, names):
+    for nm in names:
         for st in ("mean", "std"):
             key = "agent/resource/%s/%s" % (nm, st)
             if key in t:
                 out["%s_%s" % (nm, st)] = t[key]
-    return out

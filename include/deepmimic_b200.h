@@ -202,6 +202,17 @@ int dm_mlp_forward_style_reward(dm_mlp* m, const float* d_amp_obs, const float* 
                                 int rows, void* stream);
 long long dm_mlp_launches(dm_mlp* m);   /* kernel launches so far: 4 per plain forward, 6 per gated forward, 4 per style-reward forward */
 void dm_mlp_destroy(dm_mlp* m);
+/* PPO value targets of a rollout window (R/learning/rl_util.py: compute_return, R/learning/ppo_agent.py: _compute_batch_vals), one launch.
+ * The critic is a dm_mlp handle with out_dim == 1 and the value normaliser as its output normaliser (plain: dm_mlp_create; goal-conditioned:
+ * dm_mlp_create_gated).  Inputs [T x N] row major (step k, environment n at k N + n): d_rewards, d_values = V(s_k), d_end_values = V(s'_k) with
+ * s'_k the state after step k before the reset, d_done (0 / 1 bytes), d_terminate (0 null, 1 fail, 2 succ).  Per environment, k = T - 1 .. 0:
+ *   v_next = done[k] ? (terminate[k] == 1 ? val_fail : terminate[k] == 2 ? val_succ : end_values[k]) : end_values[k]
+ *   G_next = (done[k] || k == T - 1) ? v_next : returns[k + 1]
+ *   returns[k] = rewards[k] + discount ((1 - td_lambda) v_next + td_lambda G_next),   advantages[k] = returns[k] - values[k]   (fp32)
+ * A path still running at step T - 1 is bootstrapped with V(s'_{T-1}), as a null end is.  Refused: T or N <= 0, discount outside [0, 1),
+ * td_lambda outside [0, 1] (either NaN), a NULL pointer. */
+int dm_td_lambda_returns(const float* d_rewards, const float* d_values, const float* d_end_values, const uint8_t* d_done, const int32_t* d_terminate, int T, int N,
+                         float discount, float td_lambda, float val_fail, float val_succ, float* d_returns, float* d_advantages, void* stream);
 
 /* ---- test hooks: raw per-env simulator state, layout shared with the CPU oracle (doubles):
  *  [0..2] basePos(scaled) [3..6] baseQuat world->base (x,y,z,w) [7..9] baseOmega [10..12] baseVel(scaled)

@@ -1,6 +1,8 @@
 """Times the networks alone, CUDA events: the plain actor (4096 x 227 -> 1024 -> 512 -> 28, dm_mlp_forward), the gated task actor
 (4096 x (226 + 3) -> 1024 -> 512 -> 28 with its gates, dm_mlp_forward_gated) and the AMP discriminator's reward (4096 x 226 -> 1024 -> 512 -> 1,
-style reward and its blend with a task reward, dm_mlp_forward_style_reward) on the wgmma kernels, each against the fp32 torch network."""
+style reward and its blend with a task reward, dm_mlp_forward_style_reward) on the wgmma kernels, each against the fp32 torch network; then the
+PPO critic of a rollout step (2 x 4096 rows [s_k; s'_k] x 227 -> 1024 -> 512 -> 1, un-normalised by the value normaliser) against the fp32 torch
+critic, and the TD(lambda) return scan of a 600 x 4096 window (dm_td_lambda_returns) against a torch loop over the steps."""
 import os, sys
 import numpy as np
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -73,3 +75,30 @@ t_dth = timeit(torch_disc_reward)
 ref_d, ref_r = torch_disc_reward(); torch.cuda.synchronize()
 print("discriminator reward, %d rows: wgmma kernels %.1f us per forward, fp32 torch discriminator + reward ops %.1f us; max |logit diff| %.2e, max |reward diff| %.2e"
       % (rows, t_dtc, t_dth, (logit - ref_d).abs().max().item(), (reward - ref_r).abs().max().item()))
+
+# the PPO critic of one rollout step: 2 x rows states [s_k; s'_k] -> 1024 -> 512 -> 1, value = 10 + 10 out (discount 0.95, rewards in [0, 1])
+crit = dict(hidden=[lin(din, h0), lin(h0, h1)], out=lin(h1, 1))
+cmlp = TensorCoreMLP(*crit["hidden"][0], *crit["hidden"][1], *crit["out"], in_mean=mean, in_std=std, in_clip=5.0, out_mean=[10.0], out_std=[10.0], max_rows=2 * rows)
+x2, v2 = torch.randn(2 * rows, din, device="cuda"), torch.zeros(2 * rows, 1, device="cuda")
+tcr = [T(a) for a in (*crit["hidden"][0], *crit["hidden"][1], *crit["out"])]
+def torch_critic():
+    h = torch.clamp((x2 - tw[6]) / tw[7], -5, 5)
+    h = torch.relu(h @ tcr[0] + tcr[1]); h = torch.relu(h @ tcr[2] + tcr[3]); return 10.0 + 10.0 * (h @ tcr[4] + tcr[5])
+t_ctc = timeit(lambda: cmlp.forward(x2, v2, stream=st.cuda_stream))
+t_cth = timeit(torch_critic)
+ref_v = torch_critic(); torch.cuda.synchronize()
+print("critic, %d rows: wgmma kernels %.1f us per forward, fp32 torch critic %.1f us; max |value diff| %.2e" % (2 * rows, t_ctc, t_cth, (v2 - ref_v).abs().max().item()))
+
+# the TD(lambda) return scan over a 600-step window
+from deepmimic_b200.capi import td_lambda_returns
+from deepmimic_b200.rollout import td_lambda_returns_host
+sys.path.insert(0, os.path.join(REPO, "tests"))
+from test_value_targets_cpu import synthetic_window
+steps = 600
+win = [torch.as_tensor(a).cuda() for a in synthetic_window(rng, steps, rows)]
+ret, adv = torch.empty(steps, rows, device="cuda"), torch.empty(steps, rows, device="cuda")
+ret2, adv2 = torch.empty_like(ret), torch.empty_like(adv)
+t_k = timeit(lambda: td_lambda_returns(*win, 0.95, 0.95, 0.0, 20.0, ret, adv, stream=st.cuda_stream))
+t_loop = timeit(lambda: td_lambda_returns_host(*win, 0.95, 0.95, 0.0, 20.0, ret2, adv2), n=5)
+torch.cuda.synchronize()
+print("TD(lambda) returns, %d x %d: return kernel %.1f us, torch loop over the steps %.1f us; max |return diff| %.2e" % (steps, rows, t_k, t_loop, (ret - ret2).abs().max().item()))
