@@ -319,10 +319,10 @@ class BatchedCore:
         return int(out[0]), int(out[1])
 
     def section_profile(self):
-        """profile build only: [blocks, warps per block, 16] uint32 section cycle counters of the last update launch"""
+        """profile build only: [blocks, warps per block, 18] uint32 section cycle counters of the last update launch"""
         nb, nw = C.c_int(0), C.c_int(0)
         self._chk(lib().dm_get_section_profile(self.h, None, C.byref(nb), C.byref(nw)))
-        out = np.zeros((nb.value, nw.value, 16), dtype=np.uint32)
+        out = np.zeros((nb.value, nw.value, 18), dtype=np.uint32)
         self._chk(lib().dm_get_section_profile(self.h, C.c_void_p(out.ctypes.data), None, None))
         return out
 

@@ -23,7 +23,7 @@ constexpr int kMaxChildren = 4;
 constexpr int kStepMaxThreads = 448;    // dm_step_kernel: 28 (W=16) / 14 (W=32) environments per block (14 warps)
 constexpr int kStepRegs = 128;          // registers per thread ptxas allocates for every dm_step_kernel instantiation (host-only launch plans; dm_create reads the real count)
 constexpr int kManifoldFloats = 48;  // per link: 4 points x 12 floats
-constexpr int kProfCounters = 16;    // DM_PROFILE builds: section cycle counters per warp of dm_step_kernel
+constexpr int kProfCounters = 18;    // DM_PROFILE builds: section cycle counters per warp of dm_step_kernel (14 warps x 18 fit the launch's 1 KiB of spare shared memory)
 
 enum DevJointType { kJRevolute = 0, kJSpherical = 1, kJFixed = 2 };
 enum DevShape { kSBox = 1, kSCapsule = 2, kSSphere = 3 };

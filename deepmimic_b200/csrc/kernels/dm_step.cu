@@ -156,6 +156,7 @@ int dm_step_layout(int nl, int n, int chain_len, int maxrows, int W, StepLayout*
 }
 int dm_step_smem_bytes(const StepLayout& L, int tiles) { return (L.hot_floats + L.env_floats * tiles) * static_cast<int>(sizeof(float)); }
 
+constexpr int kSubstepBarriers = 2;   // block barriers inside a Bullet sub-step stage (dm_step_kernel's main loop)
 constexpr int kPgsBlock = 2;   // solver steps evaluated per block of the projected Gauss-Seidel sweeps (chosen by measuring 1, 2, 4 and 8; 2 was the fastest)
 // Projected Gauss-Seidel in impulse space, 10 sweeps in btMultiBodyConstraintSolver::solveSingleIteration's row order (joint limits in
 // alternating order, contact normals, friction pairs).  Lanes = rows for the state that is wide: every lane keeps w = (A lambda)_row of ITS rows in
@@ -1380,10 +1381,17 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
         PROF(1);
         if (stage == total_stages) break;
         // a block barrier after every stage keeps the warps in lockstep: warps that drift apart thrash the instruction cache (measured throughput:
-        // 2.12 M with this barrier, 2.11 M with one per update, 1.94 / 1.89 / 1.78 M with one every 2 / 4 updates / none)
+        // 2.12 M with this barrier, 2.11 M with one per update, 1.94 / 1.89 / 1.78 M with one every 2 / 4 updates / none).  A Bullet sub-step
+        // has two more (kSubstepBarriers, after the unconstrained solve and after the constraint solve), so that the warps of a block also run
+        // its routines together (spin kick on an H100 at a 400 W limit: 2.37-2.39 M policy steps/s with the stage barriers alone, 2.47-2.50 M
+        // with these two, 2.38 M / 2.43-2.44 M with only the first / only the second; dropping stage barriers instead lost 1-8 %)
         if (__syncthreads_and(!alive)) break;
         PROF(2);
-        if (__ballot_sync(0xffffffffu, alive) == 0u) continue;   // both environments of this warp are frozen
+        if (__ballot_sync(0xffffffffu, alive) == 0u) {   // both environments of this warp are frozen: it still meets the sub-step's barriers
+            if ((stage % stages_per_upd) != 0)
+                for (int k = 0; k < kSubstepBarriers; ++k) __syncthreads();
+            continue;
+        }
         const int ph = stage % stages_per_upd;      // 0: Stable-PD stage, 1..sim_substeps: Bullet sub-steps
         if (ph == 0) {
             // ---------------- clocks: cScene::Update, cSceneImitate::UpdateKinChar, cDeepMimicCharController::UpdateCalcTau
@@ -1477,7 +1485,9 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
                 vel_pass<W>(jv.x, jv.y, jv.z, hseg != 0u);
             }
         }
-        PROF(4);
+        PROF(ph == 1 ? 16 : 17);   // the Stable-PD stage's solve is section 4
+        __syncthreads();   // sub-step barrier 1 of kSubstepBarriers: every warp of the block, frozen ones included, passes it
+        PROF(2);
         // ---- joint-limit rows (btMultiBodyJointLimitConstraint): a lane owns at most one active row
         int lim_dir = 0; float lim_pen = 0.f;
         if (act && has_limit && alive) {
@@ -1511,6 +1521,8 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
             }
             PROF(11);
         }
+        __syncthreads();   // sub-step barrier 2 of kSubstepBarriers
+        PROF(2);
         // ---- integrate positions (btMultiBody::stepPositionsMultiDof)
         if (lane == 0) {
             sB[0] += h * sB[10]; sB[1] += h * sB[11]; sB[2] += h * sB[12];

@@ -223,7 +223,7 @@ int dm_td_lambda_returns(const float* d_rewards, const float* d_values, const fl
 int dm_get_snapshot(dm_handle* h, int env, double* h_out);
 int dm_set_snapshot(dm_handle* h, int env, const double* h_in);
 /* profile build only (DM_PROFILE, `make -C deepmimic_b200/csrc profile`; fails in a normal build): per-warp cycle counters by code section of the
- * last dm_update's step kernel, 16 uint32 per warp, block-major ([num_blocks][warps_per_block][16], tools/section_profile.py names them).
+ * last dm_update's step kernel, 18 uint32 per warp, block-major ([num_blocks][warps_per_block][18], tools/section_profile.py names them).
  * h_out may be NULL to query the two sizes only. */
 int dm_get_section_profile(dm_handle* h, uint32_t* h_out, int* num_blocks, int* warps_per_block);
 int dm_get_counters(dm_handle* h, int64_t* h_out);           /* {kernel launches so far, row-capacity overflows seen (must stay 0)} */

@@ -24,19 +24,22 @@ with torch.cuda.stream(stream):
     a = torch.clamp(-off + 0.25 / scl * torch.randn(N, A, device="cuda", generator=g), lo, hi).contiguous()
     core.set_action(a); core.update(1 / 600., 20)
 core.sync()
-d = core.section_profile().astype(np.float64)   # [blocks, warps per block, 16] counters of the last launch
+d = core.section_profile().astype(np.float64)   # [blocks, warps per block, 18] counters of the last launch
 nblocks, warps_per_block = d.shape[:2]
 print("%d blocks of %d warps" % (nblocks, warps_per_block))
-names = ["kin", "flags", "sync", "clock/collide", "ab+up", "base", "descend(+torque/vel)", "limits+publish", "rows", "Abuild", "warm+PGS", "z+down", "integrate"]
-tot = d[:, :, :13].sum(axis=2)
+# counter index -> section (dm_step_kernel's PROF / solve_rows' SPROF points).  7-9 are parts of solve_rows and already inside 10; 13-15 count rows.
+names = {0: "kin", 1: "flags", 2: "sync (barriers)", 3: "clock/collide", 4: "PD solve+torque", 16: "sub-step 1 solve", 17: "sub-step 2 solve",
+         5: "limit rows", 10: "solve_rows+z", 7: "  rows", 8: "  Abuild", 9: "  warm+PGS", 11: "dv_pass", 12: "integrate"}
+timed = [0, 1, 2, 3, 4, 16, 17, 5, 10, 11, 12]
+tot = d[:, :, timed].sum(axis=2)
 print("cycles per launch (20 updates): mean warp %.0f, mean of slowest warp per block %.0f, max %.0f" % (tot.mean(), tot.max(axis=1).mean(), tot.max()))
-slow = d[np.arange(nblocks), tot.argmax(axis=1)]
 wosync = tot - d[:, :, 2]
 print("without barrier wait: mean warp %.0f, slowest per block %.0f" % (wosync.mean(), wosync.max(axis=1).mean()))
 slow2 = d[np.arange(nblocks), wosync.argmax(axis=1)]
-print("%-22s %12s %12s" % ("section", "mean warp", "busiest warp/block"))
-for k, nme in enumerate(names):
-    print("%-22s %12.0f %12.0f" % (nme, d[:, :, k].mean(), slow2[:, k].mean()))
+busy_tot = wosync.max(axis=1).mean()
+print("%-22s %12s %12s %8s" % ("section", "mean warp", "busiest warp/block", "share"))
+for k in timed[:8] + [7, 8, 9] + timed[8:]:
+    print("%-22s %12.0f %12.0f %7.1f%%" % (names[k], d[:, :, k].mean(), slow2[:, k].mean(), 100.0 * slow2[:, k].mean() / busy_tot if k != 2 else 0.0))
 
 nr_sum, nr_cnt = d[:, :, 13], d[:, :, 14]
 busy = wosync.argmax(axis=1)
@@ -58,7 +61,7 @@ for b in list(order[:6]) + list(order[len(order) // 2: len(order) // 2 + 3]):
     w = wosync[b].argmax()
     print("  block %3d time %9.0f busiest work %9.0f substeps %2d rows %.1f general %2d block work %10.0f | busiest warp sections: %s" % (
         b, bt[b], wosync[b, w], nr_cnt[b, w], nr_sum[b, w] / max(1, nr_cnt[b, w]), gen[b].sum(), wosync[b].sum(),
-        " ".join("%s=%.0f" % (names[k].split()[0][:6], d[b, w, k]) for k in (0, 3, 4, 8, 9, 10, 11, 12))))
+        " ".join("%s=%.0f" % (names[k].strip().replace(" ", "_"), d[b, w, k]) for k in (0, 3, 4, 16, 17, 7, 8, 9, 10, 11, 12))))
 c = np.corrcoef(bt, gen.sum(axis=1))[0, 1] if gen.sum() > 0 else 0.0
 c2 = np.corrcoef(bt, nr_sum.sum(axis=1))[0, 1]
 c3 = np.corrcoef(bt, wosync.max(axis=1))[0, 1]
