@@ -26,12 +26,26 @@ class DmMlpGatedWeights(C.Structure):
                 + [(n, _fp) for n in ("s_mean", "s_std", "g_mean", "g_std", "a_mean", "a_std")] + [("s_clip", C.c_float), ("g_clip", C.c_float)])
 
 
+class DmLearnNet(C.Structure):
+    """dm_learn_net of include/deepmimic_b200.h"""
+    _fields_ = [(n, C.c_void_p * 3) for n in ("w", "b", "acc_w", "acc_b")]
+
+
+class DmLearnBatch(C.Structure):
+    """dm_learn_batch of include/deepmimic_b200.h"""
+    _fields_ = ([("states", C.c_void_p), ("idx", C.c_void_p), ("rows", C.c_int), ("in_mean", C.c_void_p), ("in_istd", C.c_void_p), ("in_clip", C.c_float)]
+                + [(n, C.c_void_p) for n in ("norm_actions", "old_logp", "adv", "logstd", "bound_min", "bound_max")]
+                + [("ratio_clip", C.c_float), ("ratio", C.c_void_p), ("norm_targets", C.c_void_p)]
+                + [(n, C.c_float) for n in ("stepsize", "momentum", "weight_decay")] + [("stats", C.c_void_p)])
+
+
 DM_STATE_OFFSET, DM_STATE_SCALE, DM_ACTION_OFFSET, DM_ACTION_SCALE, DM_ACTION_BOUND_MIN, DM_ACTION_BOUND_MAX, DM_STATE_NORM_GROUPS = range(7)
 
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
            "dm_update", "dm_record_state", "dm_record_goal", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
            "dm_set_snapshot", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
-           "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy", "dm_td_lambda_returns"]
+           "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy", "dm_td_lambda_returns", "dm_mlp_set_weights_device", "dm_learn_create",
+           "dm_mlp_set_normalizers_device", "dm_learn_set_weights", "dm_learn_step", "dm_learn_destroy"]
 
 
 def lib():
@@ -107,8 +121,25 @@ def lib():
         L.dm_mlp_launches.argtypes = [vp]
         L.dm_mlp_destroy.argtypes = [vp]
         L.dm_td_lambda_returns.argtypes = [vp] * 5 + [C.c_int, C.c_int] + [C.c_float] * 4 + [vp, vp, vp]
+        L.dm_mlp_set_weights_device.argtypes = [vp] * 8
+        L.dm_mlp_set_normalizers_device.argtypes = [vp] * 6
+        L.dm_learn_create.restype = vp
+        L.dm_learn_create.argtypes = [C.c_int] * 7
+        L.dm_learn_set_weights.argtypes = [vp, C.POINTER(DmLearnNet), vp]
+        L.dm_learn_step.argtypes = [vp, C.POINTER(DmLearnNet), C.POINTER(DmLearnBatch), vp]
+        L.dm_learn_destroy.argtypes = [vp]
         _lib = L
     return _lib
+
+
+def _check_device_f32(t, what, shape=None, device=None):
+    """a contiguous float32 CUDA tensor (of the given shape, on the given device): what the C ABI's raw device pointers require"""
+    import torch
+    if (not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32 or not t.is_contiguous()
+            or (shape is not None and tuple(t.shape) != tuple(shape)) or (device is not None and t.device != device)):
+        raise ValueError("%s: need a contiguous float32 CUDA tensor%s%s (got %s)" % (what, "" if shape is None else " of shape %s" % (tuple(shape),),
+                         "" if device is None else " on %s" % device, "a %s" % type(t).__name__ if not isinstance(t, torch.Tensor)
+                         else "%s %s on %s%s" % (t.dtype, tuple(t.shape), t.device, "" if t.is_contiguous() else ", not contiguous")))
 
 
 def _dptr(a):
@@ -440,6 +471,28 @@ class TensorCoreMLP:
             raise RuntimeError("dm_mlp_forward: %s" % lib().dm_last_error().decode())
         return actions
 
+    def set_weights_device(self, layers, stream=None):
+        """dm_mlp_set_weights_device: re-tiles the handle on the device from three torch Linear layers with fp32 CUDA parameters (the two hidden
+        layers and the output layer; [out, in] weights); the normalisers are kept"""
+        shapes = [(self.h0, self.in_dim), (self.h0,), (self.h1, self.h0), (self.h1,), (self.out_dim, self.h1), (self.out_dim,)]
+        tensors = [t for l in layers for t in (l.weight, l.bias)]
+        for t, shape in zip(tensors, shapes):
+            _check_device_f32(t, "set_weights_device", shape)
+        ptrs = [C.c_void_p(t.data_ptr()) for t in tensors]
+        rc = lib().dm_mlp_set_weights_device(self.h, *ptrs, C.c_void_p(stream) if stream else None)
+        if rc != 0:
+            raise RuntimeError("dm_mlp_set_weights_device: %s" % lib().dm_last_error().decode())
+
+    def set_normalizers_device(self, in_mean, in_std, out_mean, out_std, stream=None):
+        """dm_mlp_set_normalizers_device: the input and output normalisers from contiguous float32 CUDA tensors ([in_dim], [out_dim]) on the
+        device, the values dm_mlp_create would store"""
+        for name, t, n in (("in_mean", in_mean, self.in_dim), ("in_std", in_std, self.in_dim), ("out_mean", out_mean, self.out_dim), ("out_std", out_std, self.out_dim)):
+            _check_device_f32(t, "set_normalizers_device: " + name, (n,))
+        rc = lib().dm_mlp_set_normalizers_device(self.h, *[C.c_void_p(t.data_ptr()) for t in (in_mean, in_std, out_mean, out_std)],
+                                                 C.c_void_p(stream) if stream else None)
+        if rc != 0:
+            raise RuntimeError("dm_mlp_set_normalizers_device: %s" % lib().dm_last_error().decode())
+
     def style_reward(self, amp_obs, reward, task_reward=None, task_lerp=0.0, logit=None, style=None, stream=None):
         """dm_mlp_forward_style_reward: the discriminator's logit d on amp_obs [rows, in_dim], style = max(0, 1 - 0.25 (1 - d)^2) and
         reward [rows] (written) = (1 - task_lerp) style + task_lerp task_reward, or style without task_reward.  logit / style [rows] are
@@ -512,6 +565,63 @@ class TensorCoreGatedMLP:
     def close(self):
         if self.h:
             lib().dm_mlp_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class TensorCoreLearner:
+    """dm_learn_* workspace: PPO minibatch steps of a plain 2-layer torch network (build_policy: kind "actor", build_critic: kind "critic") on the
+    tensor cores.  The network's parameters and the momentum accumulators `acc` ({parameter: tensor}) are updated in place; both must be
+    contiguous float32 CUDA tensors on the workspace's device.  Their device pointers are read again (and checked) by every set_weights(), so a
+    network moved after construction is picked up there, or refused."""
+
+    def __init__(self, net, acc, kind, max_rows, device=0):
+        if getattr(net, "goal_size", 0) or hasattr(net, "gate_common") or len(net.hidden) != 2:
+            raise ValueError("the tensor-core learner implements the plain network with exactly two hidden layers (the gated backward is not built)")
+        self.layers = list(net.hidden) + [net.mean if kind == "actor" else net.out]
+        self.acc, self.device = acc, device
+        ins, outs = [l.weight.shape[1] for l in self.layers], [l.weight.shape[0] for l in self.layers]
+        L = lib()
+        self.h = L.dm_learn_create(device, 0 if kind == "actor" else 1, ins[0], outs[0], outs[1], outs[2], max_rows)
+        if not self.h:
+            raise RuntimeError("dm_learn_create failed: %s" % L.dm_last_error().decode())
+        self.h = C.c_void_p(self.h)
+        self.net = None
+        self._bind()
+
+    def _bind(self):
+        import torch
+        dev = torch.device("cuda", self.device)
+        for l in self.layers:
+            for p in (l.weight, l.bias):
+                if p not in self.acc:
+                    raise ValueError("TensorCoreLearner: a parameter has no momentum accumulator (the network's parameters were replaced)")
+                _check_device_f32(p, "TensorCoreLearner parameter", None, dev)
+                _check_device_f32(self.acc[p], "TensorCoreLearner accumulator", tuple(p.shape), dev)
+        p = lambda t: C.c_void_p(t.data_ptr())
+        arr = lambda ts: (C.c_void_p * 3)(*[p(t) for t in ts])
+        self.net = DmLearnNet(arr([l.weight for l in self.layers]), arr([l.bias for l in self.layers]),
+                              arr([self.acc[l.weight] for l in self.layers]), arr([self.acc[l.bias] for l in self.layers]))
+
+    def set_weights(self, stream=None):
+        """binds the parameters' current storage (checked) and loads their values into the workspace's tiles"""
+        self._bind()
+        if lib().dm_learn_set_weights(self.h, C.byref(self.net), C.c_void_p(stream) if stream else None) != 0:
+            raise RuntimeError("dm_learn_set_weights: %s" % lib().dm_last_error().decode())
+
+    def step(self, batch, stream=None):
+        """batch: a DmLearnBatch"""
+        if lib().dm_learn_step(self.h, C.byref(self.net), C.byref(batch), C.c_void_p(stream) if stream else None) != 0:
+            raise RuntimeError("dm_learn_step: %s" % lib().dm_last_error().decode())
+
+    def close(self):
+        if self.h:
+            lib().dm_learn_destroy(self.h)
             self.h = None
 
     def __del__(self):

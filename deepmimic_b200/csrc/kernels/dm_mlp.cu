@@ -80,6 +80,23 @@ struct MlpStyleParams {
     float* reward;             // [M]
     float task_lerp;
 };
+// The backward GEMMs of the PPO learner (kernels/dm_learn.cu, mlp_capi.cu: dm_learn_step), also a parameter struct of their own.  Same pipeline,
+// other operands and epilogues:
+//   GRAD_X  dH = (dY W^T) * 1[H > 0]: A = dY in operand layout as hi + lo chunks (K = twice this layer's padded outputs), B = W^T as hi + lo
+//           tiles (N = its padded inputs), so both operands are exact to fp32 level (a minibatch's gradient is a sum of per-row terms that
+//           largely cancel, which magnifies fp16 rounding of dY); the epilogue masks with the saved forward activation tile and writes dH as the
+//           next dX GEMM's A operand and, as hi + lo, as the dW GEMM's B operand
+//   GRAD_W  dW = X^T dY: A = the layer's input activations transposed (M = padded inputs + the ones feature whose dW row is db), B = dY as
+//           hi + lo (K = minibatch rows); K is split over row-chunk ranges (blockIdx.z) and each split writes its fp32 partial product
+enum { kGradNone = 0, kGradX = 1, kGradW = 2 };
+struct MlpGradParams {
+    const __half* mask_tiles;  // GRAD_X: the layer's input activations, [m tiles][N / 64][kMlpATile]
+    __half* dy_a;              // GRAD_X: dH in operand layout [m tiles][hi: N / 64, lo: N / 64][kMlpATile], or null
+    __half* dy_b;              // GRAD_X: dH as B of the dW GEMM, [N / 128][row_chunks][hi | lo][128 x 64]
+    float* partial;            // GRAD_W: [splits][N][M] (the parameter's [out x in] order)
+    int row_chunks;            // minibatch rows / 64 (padded)
+    int chunks_per_split;      // GRAD_W
+};
 
 namespace {
 
@@ -161,8 +178,9 @@ __global__ void __launch_bounds__(kMlpThreads) dm_mlp_gated_prep_kernel(MlpPrepP
 // GATED (a hidden layer of the gated actor): two more pipeline chunks after the K loop (MlpGemmParams::gate_tiles) accumulate the gate's scale
 // and bias pre-activations in registers of their own; with BN = 64 that is 3 x 32 accumulator registers per thread.
 // STYLE (the discriminator's one-unit logit head): the last layer's epilogue writes the style reward instead of actions.
-template <int BN, bool LAST, bool GATED, bool STYLE = false>
-__device__ __forceinline__ void mlp_gemm(const MlpGemmParams& P, const MlpStyleParams* S = nullptr) {
+// GRAD (the learner's backward GEMMs, MlpGradParams): kGradX / kGradW epilogues; kGradW also takes its K range from blockIdx.z.
+template <int BN, bool LAST, bool GATED, bool STYLE = false, int GRAD = kGradNone>
+__device__ __forceinline__ void mlp_gemm(const MlpGemmParams& P, const MlpStyleParams* S = nullptr, const MlpGradParams* G = nullptr) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     constexpr int kABytes = kMlpATile * 2;               // 16 KB
     constexpr int kWBytes = 2 * BN * kMlpBK * 2;         // hi + lo
@@ -174,10 +192,16 @@ __device__ __forceinline__ void mlp_gemm(const MlpGemmParams& P, const MlpStyleP
     uint64_t* bar_empty = bar_full + kMlpStages;                                         // [stages] every thread's MMAs reading the stage have completed
     const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127;
     const int mt = blockIdx.x, m0 = mt * kMlpBM, nt = blockIdx.y, n0 = nt * BN;
-    const int NC = P.K / kMlpBK;
+    static_assert(GRAD == kGradNone || (!LAST && !GATED && !STYLE), "the gradient epilogues replace the hidden-layer epilogue");
+    // kGradW: this split's row chunks [c0, c0 + NC) of the KC chunks every m / n tile holds
+    // kGradX: A is dY as hi chunks then lo chunks (2 K / 64 chunks per m tile), each against the same W^T chunk: dY exact to fp32 level
+    const int KW = GRAD == kGradW ? G->row_chunks : P.K / kMlpBK;   // K chunks per n tile of B
+    const int KC = GRAD == kGradX ? 2 * KW : KW;                    // K chunks per m tile of A
+    const int c0 = GRAD == kGradW ? static_cast<int>(blockIdx.z) * G->chunks_per_split : 0;
+    const int NC = GRAD == kGradW ? min(G->chunks_per_split, KC - c0) : KC;
     const int NT = GATED ? NC + 2 : NC;                  // pipeline chunks: the K loop, then the gate's scale and bias chunks
-    const __half* a_src = P.a_tiles + static_cast<size_t>(mt) * NC * kMlpATile;
-    const __half* w_src = P.w_tiles + static_cast<size_t>(nt) * NC * (kWBytes / 2);
+    const __half* a_src = P.a_tiles + (static_cast<size_t>(mt) * KC + c0) * kMlpATile;
+    const __half* w_src = P.w_tiles + (static_cast<size_t>(nt) * KW + c0) * (kWBytes / 2);
     // one bulk copy per operand and K-chunk (both are contiguous blocks in operand layout)
     auto load = [&](int c) {
         const int s = c % kMlpStages;
@@ -189,7 +213,7 @@ __device__ __forceinline__ void mlp_gemm(const MlpGemmParams& P, const MlpStyleP
             return;
         }
         bulk_g2s(sA, a_src + static_cast<size_t>(c) * kMlpATile, kABytes, &bar_full[s]);
-        bulk_g2s(sA + kABytes, w_src + static_cast<size_t>(c) * (kWBytes / 2), kWBytes, &bar_full[s]);
+        bulk_g2s(sA + kABytes, w_src + static_cast<size_t>(GRAD == kGradX ? c % KW : c) * (kWBytes / 2), kWBytes, &bar_full[s]);
     };
 
     if (tid == 0) {
@@ -258,7 +282,35 @@ __device__ __forceinline__ void mlp_gemm(const MlpGemmParams& P, const MlpStyleP
             const int n = n0 + h * 64 + 8 * (q >> 1) + 2 * (lane & 3);
             const int i0 = 4 * (q >> 1) + 2 * (q & 1);
             const float v0 = acc[h][i0], v1 = acc[h][i0 + 1];
-            if constexpr (STYLE) {
+            if constexpr (GRAD == kGradW) {
+                // row = input feature, n = output unit: the partial sum of this split in the parameter's [out x in] order (every row of the
+                // padded M is written; the optimiser reads the real ones)
+                float* out = G->partial + static_cast<size_t>(blockIdx.z) * P.N * P.M;
+                out[static_cast<size_t>(n) * P.M + row] = v0;
+                out[static_cast<size_t>(n + 1) * P.M + row] = v1;
+            } else if constexpr (GRAD == kGradX) {
+                // ReLU mask from the saved fp16 activation: a pre-activation in (0, 2^-25) rounded to 0 there and is masked (within tolerance)
+                const size_t in_tile = (((n & 63) >> 3) * (kMlpBM / 8) + (r >> 3)) * 64 + (r & 7) * 8 + (n & 7);
+                const __half2 hact = *reinterpret_cast<const __half2*>(G->mask_tiles + (static_cast<size_t>(mt) * (P.N >> 6) + (n >> 6)) * kMlpATile + in_tile);
+                const float d0 = __low2float(hact) > 0.f ? v0 : 0.f, d1 = __high2float(hact) > 0.f ? v1 : 0.f;
+                if (G->dy_a) {
+                    // the next dX GEMM's A: hi in chunk n / 64, lo in chunk N / 64 + n / 64 of the m tile's 2 N / 64 chunks
+                    __half* t = G->dy_a + (static_cast<size_t>(mt) * 2 * (P.N >> 6) + (n >> 6)) * kMlpATile + in_tile;
+                    const __half2 hi = __floats2half2_rn(d0, d1);
+                    *reinterpret_cast<__half2*>(t) = hi;
+                    *reinterpret_cast<__half2*>(t + static_cast<size_t>(P.N >> 6) * kMlpATile) = __floats2half2_rn(d0 - __low2float(hi), d1 - __high2float(hi));
+                }
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int ne = n + e, k = row & 63;
+                    const float d = e ? d1 : d0;
+                    const __half hi = __float2half_rn(d);
+                    __half* t = G->dy_b + (static_cast<size_t>(ne >> 7) * G->row_chunks + (row >> 6)) * 2 * 128 * kMlpBK +
+                                (((k >> 3) * 16 + ((ne & 127) >> 3)) * 64 + (ne & 7) * 8 + (k & 7));
+                    t[0] = hi;
+                    t[128 * kMlpBK] = __float2half_rn(d - __half2float(hi));
+                }
+            } else if constexpr (STYLE) {
                 // the logit is column 0 (the tile's other 63 columns are padding): one thread per row holds it and writes every output of that row
                 if (row < P.M && n == 0) {
                     const float d = v0 + P.bias[0], e = 1.f - d;
@@ -304,6 +356,14 @@ __global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_gemm_kernel(MlpGemm
 __global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_gated_gemm_kernel(MlpGemmParams P) { mlp_gemm<64, false, true>(P); }
 // the discriminator's logit head with the style-reward epilogue (AMP, Peng et al. 2021, eq. 7), 64-column tile
 __global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_style_reward_kernel(MlpGemmParams P, MlpStyleParams S) { mlp_gemm<64, true, false, true>(P, &S); }
+
+// the PPO learner's backward GEMMs (MlpGradParams): dX of a hidden layer (128-column tiles) and the split-K dW (BN = 128, or 64 for an output
+// layer of up to 64 units)
+__global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_grad_x_kernel(MlpGemmParams P, MlpGradParams G) { mlp_gemm<128, false, false, false, kGradX>(P, nullptr, &G); }
+template <int BN>
+__global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_grad_w_kernel(MlpGemmParams P, MlpGradParams G) { mlp_gemm<BN, false, false, false, kGradW>(P, nullptr, &G); }
+template __global__ void dm_mlp_grad_w_kernel<128>(MlpGemmParams, MlpGradParams);
+template __global__ void dm_mlp_grad_w_kernel<64>(MlpGemmParams, MlpGradParams);
 
 int dm_mlp_smem_bytes(int bn) { return kMlpStages * (kMlpATile * 2 + 2 * bn * kMlpBK * 2) + 1024; }
 

@@ -1,11 +1,13 @@
 // C ABI of the tensor-core policy network (include/deepmimic_b200.h, dm_mlp_*): host-side weight tiling + the launches of kernels/dm_mlp.cu: four for
 // the plain actor (operand preparation, three GEMMs), six for the gated one (operand preparation, gate trunk, both gate hidden layers, two gated
 // trunk layers, output layer), four for the AMP discriminator's style reward (operand preparation, two GEMMs, the logit head with the reward
-// epilogue); and the learner-side TD(lambda) return scan of a rollout window (kernels/dm_returns.cu, one launch).  Same library, same rules: no
-// CPU fallback, errors through dm_last_error.
+// epilogue); the learner-side TD(lambda) return scan of a rollout window (kernels/dm_returns.cu, one launch); and the PPO learner's minibatch
+// step (dm_learn_*: kernels/dm_learn.cu and the backward GEMMs of kernels/dm_mlp.cu, 15 launches) with the device-side re-tiling of a plain
+// handle (dm_mlp_set_weights_device).  Same library, same rules: no CPU fallback, errors through dm_last_error.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -34,6 +36,29 @@ __global__ void dm_mlp_style_reward_kernel(MlpGemmParams, MlpStyleParams);
 __global__ void dm_td_lambda_kernel(const float*, const float*, const float*, const uint8_t*, const int32_t*, int, int, float, float, float, float, float*, float*);
 int dm_mlp_smem_bytes(int bn);
 constexpr int kMlpATileHalves = 128 * 64;   // one operand tile of activations (kernels/dm_mlp.cu: kMlpATile)
+// the PPO learner (kernels/dm_mlp.cu: MlpGradParams and the backward GEMMs; kernels/dm_learn.cu)
+struct MlpGradParams { const __half* mask_tiles; __half* dy_a; __half* dy_b; float* partial; int row_chunks; int chunks_per_split; };
+struct LearnPrepParams { const float* x; const int64_t* idx; const float* mean; const float* istd; float clip; int in_dim, M, NC; __half* tiles; };
+struct LearnTransposeParams { const __half* src[3]; __half* dst[3]; int src_nc[3]; int ones[3]; int F[3]; int row_chunks; };
+struct LearnHeadParams {
+    const float* out; const int64_t* idx; int M, out_dim; __half* dy_a; __half* dy_b; float* partials;
+    const float* actions; const float* old_logp; const float* adv; const float* logstd; const float* bound_min; const float* bound_max; float ratio_clip; float* ratio;
+    const float* targets;
+};
+struct LearnLayerParams {
+    float* w; float* b; float* acc_w; float* acc_b; const float* partial; int splits, Npad, F; float inv_rows, lr, mom, wd; int in_dim, out_dim;
+    __half* tiles; float* bias_pad; int NC, BN; __half* t_tiles; int t_NC;
+};
+__global__ void dm_mlp_grad_x_kernel(MlpGemmParams, MlpGradParams);
+template <int BN>
+__global__ void dm_mlp_grad_w_kernel(MlpGemmParams, MlpGradParams);
+__global__ void dm_learn_prep_kernel(LearnPrepParams);
+__global__ void dm_learn_transpose_kernel(LearnTransposeParams);
+__global__ void dm_learn_actor_head_kernel(LearnHeadParams);
+__global__ void dm_learn_critic_head_kernel(LearnHeadParams);
+__global__ void dm_learn_stats_kernel(const float*, int, float, int, float*);
+__global__ void dm_learn_layer_kernel(LearnLayerParams);
+__global__ void dm_learn_norm_kernel(const float*, const float*, int, float*, float*, int);
 }  // namespace dmk
 
 extern "C" void dm_set_last_error(const char* msg);
@@ -103,6 +128,41 @@ dmk::MlpGemmParams plain_trunk(dm_mlp* m, const float* d_obs, int rows, cudaStre
     // the output layer reads layer 1's tiles
     P.a_tiles = m->act1; P.w_tiles = m->w[2]; P.bias = m->b[2]; P.out_tiles = nullptr; P.K = m->N1; P.N = m->N2;
     return P;
+}
+// the layer pass of kernels/dm_learn.cu for layer l of a plain handle: tiles of w[l] / b[l] from the fp32 [units x inputs] weights; the caller
+// adds the optimiser's and the transposed tiles' fields
+dmk::LearnLayerParams layer_params(dm_mlp* m, int l, const float* w, const float* b) {
+    const int in[3] = {m->in_dim, m->h0, m->h1}, out[3] = {m->h0, m->h1, m->out_dim}, K[3] = {m->K0, m->N0, m->N1};
+    dmk::LearnLayerParams L{};
+    L.w = const_cast<float*>(w); L.b = const_cast<float*>(b); L.in_dim = in[l]; L.out_dim = out[l];
+    L.tiles = m->w[l]; L.bias_pad = m->b[l]; L.NC = K[l] / 64; L.BN = l == 2 ? m->N2 : 128;
+    return L;
+}
+void launch_layer(const dmk::LearnLayerParams& L, cudaStream_t st) {
+    dmk::dm_learn_layer_kernel<<<dim3((L.in_dim + 1 + 255) / 256, L.out_dim), 256, 0, st>>>(L);
+}
+}  // namespace
+
+// PPO learner workspace (include/deepmimic_b200.h: dm_learn_*).  Layer l = 0, 1, 2 has F[l] = pad128(inputs + 1) transposed-input features (the
+// ones feature at index `inputs` makes row `inputs` of dW the bias gradient) and Nout[l] padded outputs (N0, N1, N2 of the handle).
+struct dm_learn {
+    dm_mlp* m = nullptr;
+    bool actor = true;
+    int max_rows = 0, F[3] = {0, 0, 0}, Nout[3] = {0, 0, 0}, max_splits[3] = {0, 0, 0};
+    float* out = nullptr;                                    // [max_rows x out_dim] normalised network output
+    __half *xt[3] = {nullptr, nullptr, nullptr};             // transposed saved activations: A of the dW GEMMs
+    __half *dy_a[3] = {nullptr, nullptr, nullptr};           // dY of layers 1, 2 in operand layout, hi + lo chunks: A of the dX GEMMs (layer 0 needs none)
+    __half *dy_b[3] = {nullptr, nullptr, nullptr};           // dY of every layer as hi + lo: B of the dW GEMMs
+    __half *wt[3] = {nullptr, nullptr, nullptr};             // W1^T, W2^T as hi + lo: B of the dX GEMMs
+    float *partial[3] = {nullptr, nullptr, nullptr}, *head_partials = nullptr;
+};
+
+namespace {
+// split-K of a dW GEMM: about two CTAs per SM of an H100 (132 SMs) over the (F / 128) x (Nout / BN) output tiles
+void dw_split(int tiles, int chunks, int* splits, int* cps) {
+    int s = std::max(1, std::min(chunks, (264 + tiles - 1) / tiles));
+    *cps = (chunks + s - 1) / s;
+    *splits = (chunks + *cps - 1) / *cps;
 }
 }  // namespace
 
@@ -281,6 +341,183 @@ int dm_td_lambda_returns(const float* d_rewards, const float* d_values, const fl
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return mlp_fail(std::string("dm_td_lambda_returns: ") + cudaGetErrorString(e));
     return 0;
+}
+
+int dm_mlp_set_weights_device(dm_mlp* m, const float* d_w0, const float* d_b0, const float* d_w1, const float* d_b1, const float* d_w2, const float* d_b2,
+                              void* stream) {
+    if (!m) return mlp_fail("dm_mlp_set_weights_device: null handle");
+    if (m->gated) return mlp_fail("dm_mlp_set_weights_device: the handle holds a gated actor; only plain handles are re-tiled on the device");
+    const float* p[6] = {d_w0, d_b0, d_w1, d_b1, d_w2, d_b2};
+    for (const float* q : p)
+        if (!q) return mlp_fail("dm_mlp_set_weights_device: null weight pointer");
+    if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_mlp_set_weights_device: cudaSetDevice failed");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    for (int l = 0; l < 3; ++l) launch_layer(layer_params(m, l, p[2 * l], p[2 * l + 1]), st);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return mlp_fail(std::string("dm_mlp_set_weights_device: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+int dm_mlp_set_normalizers_device(dm_mlp* m, const float* d_in_mean, const float* d_in_std, const float* d_out_mean, const float* d_out_std, void* stream) {
+    if (!m) return mlp_fail("dm_mlp_set_normalizers_device: null handle");
+    if (m->gated) return mlp_fail("dm_mlp_set_normalizers_device: the handle holds a gated actor; only plain handles are refreshed on the device");
+    if (!d_in_mean || !d_in_std || !d_out_mean || !d_out_std) return mlp_fail("dm_mlp_set_normalizers_device: null normaliser pointer");
+    if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_mlp_set_normalizers_device: cudaSetDevice failed");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    dmk::dm_learn_norm_kernel<<<(m->in_dim + 255) / 256, 256, 0, st>>>(d_in_mean, d_in_std, m->in_dim, m->in_mean, m->in_istd, 1);
+    dmk::dm_learn_norm_kernel<<<(m->out_dim + 255) / 256, 256, 0, st>>>(d_out_mean, d_out_std, m->out_dim, m->out_mean, m->out_std, 0);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return mlp_fail(std::string("dm_mlp_set_normalizers_device: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+dm_learn* dm_learn_create(int device, int kind, int in_dim, int h0, int h1, int out_dim, int max_rows) {
+    if (kind != 0 && kind != 1) { mlp_fail("dm_learn_create: kind must be 0 (actor) or 1 (critic)"); return nullptr; }
+    if (kind == 1 && out_dim != 1) { mlp_fail("dm_learn_create: a critic has one output"); return nullptr; }
+    if (in_dim <= 0 || h0 <= 0 || h1 <= 0 || out_dim <= 0 || out_dim > 64 || max_rows <= 0) { mlp_fail("dm_learn_create: bad sizes (out_dim must be <= 64)"); return nullptr; }
+    // zero weights and an identity output normaliser: dm_learn_set_weights loads the parameters, the output stays normalised
+    std::vector<float> w0(static_cast<size_t>(in_dim) * h0), w1(static_cast<size_t>(h0) * h1), w2(static_cast<size_t>(h1) * out_dim), b0(h0), b1(h1), b2(out_dim);
+    dm_mlp* m = dm_mlp_create(device, in_dim, h0, h1, out_dim, w0.data(), b0.data(), w1.data(), b1.data(), w2.data(), b2.data(), nullptr, nullptr, 0.f, nullptr, nullptr, max_rows);
+    if (!m) return nullptr;   // dm_last_error is set
+    dm_learn* l = new dm_learn();
+    l->m = m; l->actor = kind == 0; l->max_rows = m->max_rows;
+    const int in[3] = {in_dim, h0, h1}, BN[3] = {128, 128, m->N2}, chunks = m->max_rows / 64;
+    l->Nout[0] = m->N0; l->Nout[1] = m->N1; l->Nout[2] = m->N2;
+    const size_t R = m->max_rows;
+    bool ok = cudaMalloc(&l->out, R * out_dim * sizeof(float)) == cudaSuccess && cudaMalloc(&l->head_partials, R / 128 * 3 * sizeof(float)) == cudaSuccess;
+    for (int i = 0; i < 3 && ok; ++i) {
+        l->F[i] = pad_to(in[i] + 1, 128);
+        // the split count is not monotonic in the row count (ceil(c / ceil(c / s))): size the partials for the largest over every minibatch
+        // a step may take (rows in [1, max_rows]: an even chunk count up to max_rows / 64)
+        for (int c = 2; c <= chunks; c += 2) {
+            int s = 0, cps = 0;
+            dw_split((l->F[i] / 128) * (l->Nout[i] / BN[i]), c, &s, &cps);
+            l->max_splits[i] = std::max(l->max_splits[i], s);
+        }
+        ok = cudaMalloc(&l->xt[i], R * l->F[i] * sizeof(__half)) == cudaSuccess && cudaMalloc(&l->dy_b[i], 2 * R * l->Nout[i] * sizeof(__half)) == cudaSuccess &&
+             cudaMalloc(&l->partial[i], static_cast<size_t>(l->max_splits[i]) * l->Nout[i] * l->F[i] * sizeof(float)) == cudaSuccess;
+        // W_i^T as B of the dX GEMM: K = Nout[i], N = Nout[i - 1] (zero padding written once)
+        if (ok && i > 0) {
+            const size_t n = 2 * static_cast<size_t>(l->Nout[i]) * l->Nout[i - 1];
+            ok = cudaMalloc(&l->dy_a[i], 2 * R * l->Nout[i] * sizeof(__half)) == cudaSuccess && cudaMalloc(&l->wt[i], n * sizeof(__half)) == cudaSuccess &&
+                 cudaMemset(l->wt[i], 0, n * sizeof(__half)) == cudaSuccess;
+        }
+    }
+    if (ok) {
+        ok = cudaFuncSetAttribute(dmk::dm_mlp_grad_x_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
+             cudaFuncSetAttribute(dmk::dm_mlp_grad_w_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
+             cudaFuncSetAttribute(dmk::dm_mlp_grad_w_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess;
+    }
+    if (!ok) { mlp_fail(std::string("dm_learn_create: ") + cudaGetErrorString(cudaGetLastError())); dm_learn_destroy(l); return nullptr; }
+    return l;
+}
+
+namespace {
+int learn_net_check(const dm_learn_net* net, const char* fn) {
+    if (!net) return mlp_fail(std::string(fn) + ": null parameters");
+    for (int i = 0; i < 3; ++i)
+        if (!net->w[i] || !net->b[i] || !net->acc_w[i] || !net->acc_b[i]) return mlp_fail(std::string(fn) + ": null parameter or accumulator pointer");
+    return 0;
+}
+// the forward tiles of the learner's handle and the transposed tiles of the dX GEMMs; with `step` also the optimiser step before the re-tiling
+void learn_layers(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, int rows, const int* splits, cudaStream_t st) {
+    for (int i = 0; i < 3; ++i) {
+        dmk::LearnLayerParams L = layer_params(l->m, i, net->w[i], net->b[i]);
+        if (i > 0) { L.t_tiles = l->wt[i]; L.t_NC = l->Nout[i] / 64; }
+        if (b) {
+            L.acc_w = net->acc_w[i]; L.acc_b = net->acc_b[i]; L.partial = l->partial[i]; L.splits = splits[i]; L.Npad = l->Nout[i]; L.F = l->F[i];
+            L.inv_rows = 1.f / rows; L.lr = b->stepsize; L.mom = b->momentum; L.wd = b->weight_decay;
+        }
+        launch_layer(L, st);
+    }
+}
+}  // namespace
+
+int dm_learn_set_weights(dm_learn* l, const dm_learn_net* net, void* stream) {
+    if (!l) return mlp_fail("dm_learn_set_weights: null handle");
+    if (learn_net_check(net, "dm_learn_set_weights")) return 1;
+    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_set_weights: cudaSetDevice failed");
+    learn_layers(l, net, nullptr, 0, nullptr, static_cast<cudaStream_t>(stream));
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return mlp_fail(std::string("dm_learn_set_weights: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+int dm_learn_step(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, void* stream) {
+    if (!l) return mlp_fail("dm_learn_step: null handle");
+    if (learn_net_check(net, "dm_learn_step")) return 1;
+    if (!b) return mlp_fail("dm_learn_step: null batch");
+    if (b->rows <= 0 || b->rows > l->max_rows) return mlp_fail("dm_learn_step: rows out of range");
+    if (!b->states || !b->idx || !b->in_mean || !b->in_istd || !b->stats) return mlp_fail("dm_learn_step: null state, index, normaliser or statistics pointer");
+    if (l->actor && (!b->norm_actions || !b->old_logp || !b->adv || !b->logstd || !b->bound_min || !b->bound_max))
+        return mlp_fail("dm_learn_step: null action, log-probability, advantage, log-std or bound pointer");
+    if (!l->actor && !b->norm_targets) return mlp_fail("dm_learn_step: null target pointer");
+    if (l->actor && !(b->ratio_clip > 0.f)) return mlp_fail("dm_learn_step: ratio_clip must be positive");
+    if (!(b->stepsize >= 0.f) || !(b->momentum >= 0.f) || !(b->weight_decay >= 0.f)) return mlp_fail("dm_learn_step: stepsize, momentum and weight_decay must be >= 0");
+    dm_mlp* m = l->m;
+    if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_learn_step: cudaSetDevice failed");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int rows = b->rows, mt = (rows + 127) / 128, chunks = 2 * mt;
+    // split-K of the three dW GEMMs for this row count (the workspace holds the largest over every row count, dm_learn_create)
+    int splits[3], cps[3];
+    for (int i = 0; i < 3; ++i) {
+        dw_split((l->F[i] / 128) * (l->Nout[i] / (i == 2 ? m->N2 : 128)), chunks, &splits[i], &cps[i]);
+        if (splits[i] > l->max_splits[i]) return mlp_fail("dm_learn_step: internal error: dW split count exceeds the workspace");
+    }
+    // forward: gathered rows -> the plain trunk -> the normalised output (identity output normaliser)
+    dmk::LearnPrepParams Q{b->states, b->idx, b->in_mean, b->in_istd, b->in_clip > 0.f ? b->in_clip : 1e30f, m->in_dim, rows, m->K0 / 64, m->obs_t};
+    dmk::dm_learn_prep_kernel<<<dim3(mt, m->K0 / 64), 128, 0, st>>>(Q);
+    dmk::MlpGemmParams P{};
+    P.M = rows;
+    P.a_tiles = m->obs_t; P.w_tiles = m->w[0]; P.bias = m->b[0]; P.out_tiles = m->act0; P.K = m->K0; P.N = m->N0;
+    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, m->N0 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
+    P.a_tiles = m->act0; P.w_tiles = m->w[1]; P.bias = m->b[1]; P.out_tiles = m->act1; P.K = m->N0; P.N = m->N1;
+    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, m->N1 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
+    P.a_tiles = m->act1; P.w_tiles = m->w[2]; P.bias = m->b[2]; P.out_tiles = nullptr; P.K = m->N1; P.N = m->N2;
+    P.actions = l->out; P.out_mean = m->out_mean; P.out_std = m->out_std; P.noise = nullptr; P.out_dim = m->out_dim;
+    dmk::dm_mlp_gemm_kernel<64, true><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P);
+    // the saved activations transposed for the dW GEMMs
+    dmk::LearnTransposeParams T{{m->obs_t, m->act0, m->act1}, {l->xt[0], l->xt[1], l->xt[2]}, {m->K0 / 64, m->N0 / 64, m->N1 / 64},
+                                {m->in_dim, m->h0, m->h1}, {l->F[0], l->F[1], l->F[2]}, chunks};
+    dmk::dm_learn_transpose_kernel<<<dim3(std::max(l->F[0], std::max(l->F[1], l->F[2])) / 128, chunks, 3), 256, 0, st>>>(T);
+    // loss head: dY of the output layer, the loss partials, the statistics
+    dmk::LearnHeadParams H{l->out, b->idx, rows, m->out_dim, l->dy_a[2], l->dy_b[2], l->head_partials, b->norm_actions, b->old_logp, b->adv, b->logstd,
+                           b->bound_min, b->bound_max, b->ratio_clip, b->ratio, b->norm_targets};
+    if (l->actor) dmk::dm_learn_actor_head_kernel<<<mt, 128, 0, st>>>(H);
+    else dmk::dm_learn_critic_head_kernel<<<mt, 128, 0, st>>>(H);
+    dmk::dm_learn_stats_kernel<<<1, 1, 0, st>>>(l->head_partials, mt, 1.f / rows, l->actor ? 1 : 0, b->stats);
+    // backward, output layer first: dW_i = X_i^T dY_i (split K), dY_{i-1} = (dY_i W_i^T) * 1[X_i > 0]
+    const __half* act[3] = {m->obs_t, m->act0, m->act1};
+    for (int i = 2; i >= 0; --i) {
+        const int BN = i == 2 ? m->N2 : 128;
+        dmk::MlpGemmParams W{};
+        W.a_tiles = l->xt[i]; W.w_tiles = l->dy_b[i]; W.M = l->F[i]; W.N = l->Nout[i];
+        const dmk::MlpGradParams GW{nullptr, nullptr, nullptr, l->partial[i], chunks, cps[i]};
+        const dim3 gw(l->F[i] / 128, l->Nout[i] / BN, splits[i]);
+        if (i == 2) dmk::dm_mlp_grad_w_kernel<64><<<gw, 256, dmk::dm_mlp_smem_bytes(64), st>>>(W, GW);
+        else dmk::dm_mlp_grad_w_kernel<128><<<gw, 256, dmk::dm_mlp_smem_bytes(128), st>>>(W, GW);
+        if (i == 0) break;
+        dmk::MlpGemmParams X{};
+        X.a_tiles = l->dy_a[i]; X.w_tiles = l->wt[i]; X.M = rows; X.K = l->Nout[i]; X.N = l->Nout[i - 1];
+        const dmk::MlpGradParams GX{act[i], i > 1 ? l->dy_a[i - 1] : nullptr, l->dy_b[i - 1], nullptr, chunks, 0};
+        dmk::dm_mlp_grad_x_kernel<<<dim3(mt, l->Nout[i - 1] / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(X, GX);
+    }
+    // optimiser step and re-tiling, after every GEMM that read the old weights
+    learn_layers(l, net, b, rows, splits, st);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return mlp_fail(std::string("dm_learn_step: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+void dm_learn_destroy(dm_learn* l) {
+    if (!l) return;
+    if (l->m) {
+        cudaSetDevice(l->m->device);
+        dm_mlp_destroy(l->m);
+    }
+    cudaFree(l->out); cudaFree(l->head_partials);
+    for (int i = 0; i < 3; ++i) { cudaFree(l->xt[i]); cudaFree(l->dy_a[i]); cudaFree(l->dy_b[i]); cudaFree(l->wt[i]); cudaFree(l->partial[i]); }
+    delete l;
 }
 
 long long dm_mlp_launches(dm_mlp* m) { return m ? m->launches : 0; }

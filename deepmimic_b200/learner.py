@@ -1,0 +1,299 @@
+"""The PPO learner: one PPOAgent._update over a window collected by BatchedRollout(critic=...) (R/learning/ppo_agent.py: _update,
+_update_actor, _update_critic, _build_losses; pg_agent.py; tf_util.py: calc_bound_loss; solvers/mpi_solver.py wrapping TF's MomentumOptimizer).
+
+The reference tree is not vendored here; its rules are restated below, one function per rule, and the CPU tests pin them there
+(tests/test_learner_cpu.py).  Where a restatement and the reference disagree, the reference is right.
+
+  PPOLearner(rollout, ...).update(traj)   one epoch loop over the window: per minibatch one critic step, then one actor step
+    backend "torch"        autograd over the rollout's torch modules (plain or gated networks, CPU or CUDA tensors): the reference the
+                           tensor-core backend is tested against
+    backend "tensor_core"  the plain networks' minibatch steps on the library's own sm_90a kernels (dm_learn_step: kernels/dm_learn.cu and the
+                           backward GEMMs of kernels/dm_mlp.cu); the gated networks of the task scenes are refused (their backward is not built)
+
+Documented deviations: minibatches are shuffled by a seeded torch.Generator on the window's device, not the reference's numpy stream; the
+statistics leave out the weight-decay term of the losses (the reference's logged losses include it); the normalisers are not updated here
+(DeviceNormalizer.update stays the caller's call, as the reference's normaliser schedule is).  Not done: the gated tensor-core backward, the AMP
+discriminator's training step, a multi-GPU gradient all-reduce, TarClipFrac stepsize decay, checkpoint writing."""
+import math
+
+ADV_EPS = 1e-5   # PPOAgent.ADV_EPS
+
+
+def clipped_value_targets(returns, val_min, val_max):
+    """The critic's targets: the TD(lambda) returns clipped to the value bounds [r_min, r_max] / (1 - discount) (PPOAgent._update clips new_vals
+    to val_min / val_max after the advantages are taken from the unclipped returns)."""
+    return returns.clamp(val_min, val_max)
+
+
+def normalized_advantages(returns, values, exp_idx, norm_adv_clip):
+    """PPOAgent._update: adv = new_vals - vals over the explored samples only (exp_idx), normalised with their mean and their (population,
+    np.std) std plus ADV_EPS, then clipped to +-norm_adv_clip.  Returns (adv of the explored samples in exp_idx's order, mean, std)."""
+    adv = (returns - values)[exp_idx]
+    mean, std = adv.mean(), adv.std(unbiased=False)
+    return ((adv - mean) / (std + ADV_EPS)).clamp(-norm_adv_clip, norm_adv_clip), mean, std
+
+
+def critic_loss(norm_out, norm_targets):
+    """PPOAgent._build_losses: 0.5 mean((norm(target) - norm(V))^2) in the value normaliser's space"""
+    return 0.5 * (norm_targets - norm_out).square().mean()
+
+
+def gaussian_log_prob(norm_a, mu, logstd):
+    """log N(norm_a; mu, exp(logstd)) summed over the action (PGAgent's logp of the normalised action; sigma is the constant norm_a_std_tf)"""
+    return (-0.5 * ((norm_a - mu) / logstd.exp()).square() - logstd - 0.5 * math.log(2.0 * math.pi)).sum(dim=-1)
+
+
+def clipped_surrogate(adv, ratio, ratio_clip):
+    """PPOAgent._build_losses: min(adv ratio, adv clip(ratio, 1 - eps, 1 + eps)) per row, with the gradient TF gives it: tf.minimum passes the
+    gradient to its first argument on ties, tf.clip_by_value passes it inside the clip range, bounds included.  A row therefore contributes
+    adv ratio dlogp when the unclipped term is the minimum or the ratio lies inside the range, and nothing otherwise."""
+    l0 = adv * ratio
+    l1 = adv * ratio.clamp(1.0 - ratio_clip, 1.0 + ratio_clip)
+    return l0.where(l0 <= l1, l1)
+
+
+def clip_fraction(ratio, ratio_clip):
+    """PPOAgent.clip_frac_tf: the fraction of rows with |ratio - 1| > eps"""
+    return ((ratio - 1.0).abs() > ratio_clip).float().mean()
+
+
+def bound_loss(mu, bound_min, bound_max):
+    """TFUtil.calc_bound_loss on the normalised action mean: 0.5 mean_rows sum_j (min(mu - lo, 0)^2 + max(mu - hi, 0)^2), lo / hi the normalised
+    action bounds"""
+    vmin, vmax = (mu - bound_min).clamp(max=0.0), (mu - bound_max).clamp(min=0.0)
+    return 0.5 * (vmin.square().sum(dim=-1) + vmax.square().sum(dim=-1)).mean()
+
+
+def weight_decay_loss(net):
+    """PPOAgent._weight_decay_loss: sum ||W||^2 / 2 (tf.nn.l2_loss) over the network's weight matrices; variables named bias are skipped, and the
+    actor's log-std is a constant, not a variable"""
+    return sum(0.5 * p.square().sum() for n, p in net.named_parameters() if n.endswith("weight"))
+
+
+def trained_parameters(net):
+    """the optimiser's variables: every parameter but the actor's log-std (norm_a_std_tf is a constant in the reference)"""
+    return [p for n, p in net.named_parameters() if n != "logstd"]
+
+
+def minibatch_schedule(num_critic, num_actor, minibatch_size, epochs, generator, device="cpu"):
+    """PPOAgent._update's loop: ceil(num_critic / B) minibatches per epoch, each of exactly B rows; minibatch b takes the positions b B .. b B + B - 1
+    modulo each set's size from that set's shuffled order (critic: every sample, actor: the explored ones).  Both orders are reshuffled at every
+    epoch, and the actor's also right after a minibatch whose positions wrapped or reached its last entry (shuffle_actor).  Yields
+    (critic positions, actor positions), int64 tensors of B entries on `device`.  The shuffles draw from `generator` (a documented deviation
+    from the reference's numpy stream); no host synchronisation."""
+    import torch
+    B = minibatch_size
+    for _ in range(epochs):
+        cperm = torch.randperm(num_critic, generator=generator, device=device)
+        aperm = torch.randperm(num_actor, generator=generator, device=device)
+        for b in range(-(-num_critic // B)):
+            pos = torch.arange(b * B, (b + 1) * B, device=device)
+            yield cperm[pos % num_critic], aperm[pos % num_actor]
+            first, last = (b * B) % num_actor, ((b + 1) * B - 1) % num_actor
+            if last < first or last == num_actor - 1:
+                aperm = torch.randperm(num_actor, generator=generator, device=device)
+
+
+def momentum_step(params, accs, grads, stepsize, momentum):
+    """TF MomentumOptimizer (what MPISolver wraps): acc = momentum acc + g; w -= stepsize acc"""
+    for p, a, g in zip(params, accs, grads):
+        a.mul_(momentum).add_(g)
+        p.sub_(stepsize * a)
+
+
+def _check(name, v, lo, hi, lo_open=False, hi_open=False):
+    bad = v is None or not (isinstance(v, (int, float)) and math.isfinite(float(v)))
+    if not bad:
+        v = float(v)
+        bad = v < lo or v > hi or (lo_open and v == lo) or (hi_open and v == hi)
+    if bad:
+        raise ValueError("%s must be in %s%s, %s%s (got %r)" % (name, "(" if lo_open else "[", lo, hi, ")" if hi_open else "]", v))
+    return float(v)
+
+
+class PPOLearner:
+    """One PPOAgent._update per update(traj) over a window of BatchedRollout(critic=...).collect(): the rollout's policy, critic and normalisers
+    (s_norm, g_norm, a_norm, val_norm).  Every hyperparameter is required (the reference reads them from an agent file; the asset archive has none).
+    The momentum accumulators are the learner's; after update() the torch modules hold the new weights and the rollout's tensor-core actor and
+    critic, where they exist, hold those weights and the normalisers' statistics that the update trained with.  A normaliser updated after
+    update() reaches those handles with the next update() or with rollout.refresh_tensor_core_policy()."""
+
+    def __init__(self, rollout, *, actor_stepsize=None, actor_momentum=None, actor_weight_decay=None, critic_stepsize=None, critic_momentum=None,
+                 critic_weight_decay=None, ratio_clip=None, norm_adv_clip=None, minibatch_size=None, epochs=None, backend="torch", seed=0):
+        import torch
+        self.torch, self.ro = torch, rollout
+        if rollout.critic is None:
+            raise ValueError("the PPO learner needs a rollout with a critic (BatchedRollout(critic=..., discount=..., td_lambda=...))")
+        inf = float("inf")
+        self.actor_stepsize = _check("actor_stepsize", actor_stepsize, 0.0, inf, lo_open=True, hi_open=True)
+        self.actor_momentum = _check("actor_momentum", actor_momentum, 0.0, 1.0, hi_open=True)
+        self.actor_weight_decay = _check("actor_weight_decay", actor_weight_decay, 0.0, inf, hi_open=True)
+        self.critic_stepsize = _check("critic_stepsize", critic_stepsize, 0.0, inf, lo_open=True, hi_open=True)
+        self.critic_momentum = _check("critic_momentum", critic_momentum, 0.0, 1.0, hi_open=True)
+        self.critic_weight_decay = _check("critic_weight_decay", critic_weight_decay, 0.0, inf, hi_open=True)
+        self.ratio_clip = _check("ratio_clip", ratio_clip, 0.0, 1.0, lo_open=True, hi_open=True)
+        self.norm_adv_clip = _check("norm_adv_clip", norm_adv_clip, 0.0, inf, lo_open=True, hi_open=True)
+        for name, v in (("minibatch_size", minibatch_size), ("epochs", epochs)):
+            if not isinstance(v, int) or isinstance(v, bool) or v < 1:
+                raise ValueError("%s must be a positive int (got %r)" % (name, v))
+        self.minibatch_size, self.epochs = minibatch_size, epochs
+        if backend not in ("torch", "tensor_core"):
+            raise ValueError("backend must be 'torch' or 'tensor_core'")
+        self.backend = backend
+        env, dev = rollout.env, rollout.env.device
+        self.device = dev
+        self.policy, self.critic = rollout.policy, rollout.critic
+        self.val_min = env.get_reward_min() / (1.0 - rollout.discount)
+        self.val_max = env.get_reward_max() / (1.0 - rollout.discount)
+        f = lambda a: torch.as_tensor(a, dtype=torch.float32, device=dev)
+        self.bound_min = rollout.a_norm.normalize(f(env.build_action_bound_min()))
+        self.bound_max = rollout.a_norm.normalize(f(env.build_action_bound_max()))
+        self.actor_params, self.critic_params = trained_parameters(self.policy), trained_parameters(self.critic)
+        self.acc = {p: torch.zeros_like(p, memory_format=torch.contiguous_format) for p in self.actor_params + self.critic_params}
+        self.gen = torch.Generator(device=dev)
+        self.gen.manual_seed(seed)
+        if backend == "tensor_core":
+            if rollout.goal_size > 0:
+                raise ValueError("the tensor_core learner implements the plain networks; the gated networks of the goal-conditioned scenes need "
+                                 "backend='torch'")
+            if dev.type != "cuda":
+                raise ValueError("the tensor_core learner needs a CUDA device")
+            from .capi import TensorCoreLearner
+            di = dev.index or 0
+            self._tc_actor = TensorCoreLearner(self.policy, self.acc, "actor", minibatch_size, device=di)
+            self._tc_critic = TensorCoreLearner(self.critic, self.acc, "critic", minibatch_size, device=di)
+
+    # ---- the window: everything a minibatch step reads, computed once per update
+    def window(self, traj):
+        """flattened [T N] views of the window and the per-sample tensors of the rules above; the one host synchronisation of update() sizes the
+        explored set"""
+        t, ro = self.torch, self.ro
+        for key in ("states", "actions", "logps", "returns", "values", "explore") + (("goals",) if ro.goal_size else ()):
+            if key not in traj:
+                raise ValueError("traj has no %r: collect() with a critic returns it" % key)
+        R = traj["returns"].numel()
+        w = dict(R=R, states=traj["states"].reshape(R, -1), norm_a=ro.a_norm.normalize(traj["actions"].reshape(R, -1)),
+                 old_logp=traj["logps"].reshape(R))
+        if ro.goal_size:
+            w["goals"] = traj["goals"].reshape(R, -1)
+        ret, val = traj["returns"].reshape(R), traj["values"].reshape(R)
+        exp_idx = traj["explore"].reshape(R).nonzero()[:, 0]
+        if exp_idx.numel() == 0:
+            raise ValueError("the window has no explored sample: the actor trains on explored actions only (exp_rate > 0)")
+        adv, w["adv_mean"], w["adv_std"] = normalized_advantages(ret, val, exp_idx, self.norm_adv_clip)
+        w["adv"] = t.zeros(R, device=ret.device)
+        w["adv"][exp_idx] = adv
+        w["exp_idx"] = exp_idx
+        w["norm_tar"] = ro.val_norm.normalize(clipped_value_targets(ret, self.val_min, self.val_max))
+        return w
+
+    def _inputs(self, w, idx):
+        ro = self.ro
+        ns = ro.s_norm.normalize(w["states"][idx])
+        return (ns,) if not ro.goal_size else (ns, ro.g_norm.normalize(w["goals"][idx]))
+
+    def critic_loss(self, w, idx):
+        """(loss with weight decay, loss) of the critic on the window samples idx (torch autograd)"""
+        loss = critic_loss(self.critic(*self._inputs(w, idx))[:, 0], w["norm_tar"][idx])
+        return loss + self.critic_weight_decay * weight_decay_loss(self.critic), loss
+
+    def actor_loss(self, w, idx):
+        """(loss with weight decay, surrogate + bound loss, ratio) of the actor on the explored window samples idx (torch autograd)"""
+        mu = self.policy(*self._inputs(w, idx))
+        ratio = (gaussian_log_prob(w["norm_a"][idx], mu, self.policy.logstd.detach()) - w["old_logp"][idx]).exp()
+        loss = -clipped_surrogate(w["adv"][idx], ratio, self.ratio_clip).mean() + bound_loss(mu, self.bound_min, self.bound_max)
+        return loss + self.actor_weight_decay * weight_decay_loss(self.policy), loss, ratio
+
+    # ---- one minibatch: a critic step, then an actor step
+    def _tc_batch(self, w, ratio=None):
+        """the dm_learn_batch of the actor and of the critic over the window w (and the tensors they point into); ratio: an optional float32
+        CUDA tensor [minibatch_size] that receives the actor's per-row probability ratios of the last step"""
+        from .capi import DmLearnBatch
+        t, ro = self.torch, self.ro
+        keep = dict(istd=(1.0 / ro.s_norm.std).contiguous(), mean=ro.s_norm.mean.contiguous(), old=w["old_logp"].contiguous(),
+                    logstd=self.policy.logstd.detach().contiguous(), states=w["states"].contiguous(), norm_a=w["norm_a"].contiguous(),
+                    lo=self.bound_min.contiguous(), hi=self.bound_max.contiguous(), adv=w["adv"].contiguous(), tar=w["norm_tar"].contiguous(),
+                    stats_a=t.zeros(2, device=self.device), stats_c=t.zeros(1, device=self.device))
+        p = lambda x: x.data_ptr()
+        clip = 0.0 if math.isinf(ro.s_norm.clip) else float(ro.s_norm.clip)
+        common = dict(states=p(keep["states"]), rows=self.minibatch_size, in_mean=p(keep["mean"]), in_istd=p(keep["istd"]), in_clip=clip)
+        actor = DmLearnBatch(**common, norm_actions=p(keep["norm_a"]), old_logp=p(keep["old"]), adv=p(keep["adv"]), logstd=p(keep["logstd"]),
+                             bound_min=p(keep["lo"]), bound_max=p(keep["hi"]), ratio_clip=self.ratio_clip, ratio=None if ratio is None else p(ratio),
+                             stepsize=self.actor_stepsize,
+                             momentum=self.actor_momentum, weight_decay=self.actor_weight_decay, stats=p(keep["stats_a"]))
+        critic = DmLearnBatch(**common, norm_targets=p(keep["tar"]), stepsize=self.critic_stepsize, momentum=self.critic_momentum,
+                              weight_decay=self.critic_weight_decay, stats=p(keep["stats_c"]))
+        return keep, actor, critic
+
+    def minibatch_step(self, w, critic_idx, actor_idx, stats, tc=None):
+        """one critic step on the window samples critic_idx, then one actor step on the samples actor_idx; stats (3 zero-d tensors: actor loss,
+        critic loss, clip fraction) accumulate"""
+        if self.backend == "tensor_core":
+            keep, actor, critic = tc
+            for name, idx, batch in (("critic_idx", critic_idx, critic), ("actor_idx", actor_idx, actor)):
+                if idx.dtype != self.torch.int64 or not idx.is_contiguous() or idx.device != self.device or idx.numel() != batch.rows:
+                    raise ValueError("%s must be a contiguous int64 tensor of %d entries on %s" % (name, batch.rows, self.device))
+            st = self.torch.cuda.current_stream(self.device).cuda_stream
+            critic.idx = critic_idx.data_ptr()
+            self._tc_critic.step(critic, stream=st)
+            actor.idx = actor_idx.data_ptr()
+            self._tc_actor.step(actor, stream=st)
+            return
+        t = self.torch
+        total, loss = self.critic_loss(w, critic_idx)
+        grads = t.autograd.grad(total, self.critic_params)
+        with t.no_grad():
+            momentum_step(self.critic_params, [self.acc[p] for p in self.critic_params], grads, self.critic_stepsize, self.critic_momentum)
+            stats[1] += loss.detach()
+        total, loss, ratio = self.actor_loss(w, actor_idx)
+        grads = t.autograd.grad(total, self.actor_params)
+        with t.no_grad():
+            momentum_step(self.actor_params, [self.acc[p] for p in self.actor_params], grads, self.actor_stepsize, self.actor_momentum)
+            stats[0] += loss.detach().abs()      # PPOAgent._update logs the mean of |actor loss| over the minibatches
+            stats[2] += clip_fraction(ratio.detach(), self.ratio_clip)
+
+    def update(self, traj):
+        """one PPOAgent._update over the window traj (collect() with a critic); returns 0-d device tensors: actor_loss, critic_loss, clip_frac
+        (means over the minibatch steps), adv_mean, adv_std, exp_samples"""
+        t = self.torch
+        same = lambda now, then: len(now) == len(then) and all(x is y for x, y in zip(now, then))
+        if not same(trained_parameters(self.policy), self.actor_params) or not same(trained_parameters(self.critic), self.critic_params):
+            raise ValueError("the policy's or the critic's parameters were replaced after the learner was built: build a new PPOLearner")
+        w = self.window(traj)
+        n_exp = w["exp_idx"].numel()
+        stats = [t.zeros((), device=self.device) for _ in range(3)]
+        tc = None
+        if self.backend == "tensor_core":
+            st = t.cuda.current_stream(self.device).cuda_stream
+            self._tc_critic.set_weights(stream=st)
+            self._tc_actor.set_weights(stream=st)
+            tc = self._tc_batch(w)
+        steps = 0
+        for c, a in minibatch_schedule(w["R"], n_exp, self.minibatch_size, self.epochs, self.gen, self.device):
+            self.minibatch_step(w, c, w["exp_idx"][a], stats, tc)
+            steps += 1
+        if tc is not None:
+            keep = tc[0]
+            stats = [keep["stats_a"][0], keep["stats_c"][0], keep["stats_a"][1]]
+        self._refresh_rollout()
+        return dict(actor_loss=stats[0] / steps, critic_loss=stats[1] / steps, clip_frac=stats[2] / steps, adv_mean=w["adv_mean"],
+                    adv_std=w["adv_std"], exp_samples=t.tensor(n_exp, device=self.device))
+
+    def _refresh_rollout(self):
+        """the rollout's tensor-core actor and critic take the new weights and the normalisers' current statistics, the ones this update trained
+        with: re-tiled and copied on the device for plain handles; the gated handles of the goal-conditioned scenes are rebuilt
+        (refresh_tensor_core_policy, a host round trip)"""
+        ro = self.ro
+        if ro._tc is None and ro._tc_critic is None:
+            return
+        if ro.goal_size > 0:
+            ro.refresh_tensor_core_policy()
+            return
+        st = self.torch.cuda.current_stream(self.device).cuda_stream
+        c = lambda n: (n.mean.contiguous(), n.std.contiguous())
+        if ro._tc is not None:
+            ro._tc.set_weights_device(list(self.policy.hidden) + [self.policy.mean], stream=st)
+            ro._tc.set_normalizers_device(*c(ro.s_norm), *c(ro.a_norm), stream=st)
+        if ro._tc_critic is not None:
+            ro._tc_critic.set_weights_device(list(self.critic.hidden) + [self.critic.out], stream=st)
+            ro._tc_critic.set_normalizers_device(*c(ro.s_norm), *c(ro.val_norm), stream=st)

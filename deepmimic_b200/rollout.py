@@ -521,7 +521,8 @@ class BatchedRollout:
         return self.env.stream
 
     def collect(self, num_steps, record_stats=True):
-        """num_steps policy steps of all environments; returns dict of [T, N, .] tensors (states, actions, logps, rewards, dones, terminate; goals
+        """num_steps policy steps of all environments; returns dict of [T, N, .] tensors (states, actions, logps, rewards, dones, terminate,
+        explore = the exploration draw of each step (True: the action was sampled, False: the mode was taken); goals
         in the goal-conditioned scenes; with a discriminator amp_obs, disc_logits, style_rewards, amp_rewards; with a critic values = V(s_k),
         end_values = V(s'_k) of the state step k ended in (before the reset), returns and advantages = returns - values).  rewards is the env's
         reward.  A path still running at the last step is bootstrapped with its end value, as the reference bootstraps a path that ends by time
@@ -530,7 +531,8 @@ class BatchedRollout:
         N, S, A = env.num_envs, env.get_state_size(), env.get_action_size()
         out = dict(states=t.empty(num_steps, N, S, device=env.device), actions=t.empty(num_steps, N, A, device=env.device),
                    logps=t.empty(num_steps, N, device=env.device), rewards=t.empty(num_steps, N, device=env.device),
-                   dones=t.empty(num_steps, N, dtype=t.bool, device=env.device), terminate=t.empty(num_steps, N, dtype=t.int32, device=env.device))
+                   dones=t.empty(num_steps, N, dtype=t.bool, device=env.device), terminate=t.empty(num_steps, N, dtype=t.int32, device=env.device),
+                   explore=t.empty(num_steps, N, dtype=t.bool, device=env.device))
         G = self.goal_size
         if G > 0:
             out["goals"] = t.empty(num_steps, N, G, device=env.device)
@@ -559,6 +561,7 @@ class BatchedRollout:
                 if record_stats:
                     self.s_norm.record(s)
                 explore = t.rand(N, device=env.device, generator=self.gen) < self.exp_rate
+                out["explore"][k] = explore   # RLAgent's EXP_ACTION_FLAG: PPOAgent._update trains the actor on these samples only
                 if G > 0:   # RLAgent._update_new_action records the goal next to the state (R/learning/rl_agent.py:319-343)
                     g = env.record_goal()
                     out["goals"][k] = g

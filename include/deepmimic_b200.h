@@ -213,6 +213,59 @@ void dm_mlp_destroy(dm_mlp* m);
  * td_lambda outside [0, 1] (either NaN), a NULL pointer. */
 int dm_td_lambda_returns(const float* d_rewards, const float* d_values, const float* d_end_values, const uint8_t* d_done, const int32_t* d_terminate, int T, int N,
                          float discount, float td_lambda, float val_fail, float val_succ, float* d_returns, float* d_advantages, void* stream);
+/* Re-tiles a plain handle's weights from fp32 DEVICE memory, [units x inputs] row major (the transpose of dm_mlp_create's layout: d_w0 [h0 x in_dim], d_w1 [h1 x h0],
+ * d_w2 [out_dim x h1], biases [units]) on `stream`, without a host round trip: the same tiles dm_mlp_create builds from the transposed weights.
+ * The normalisers are kept.  Refused: a NULL handle or pointer, a gated handle. */
+int dm_mlp_set_weights_device(dm_mlp* m, const float* d_w0, const float* d_b0, const float* d_w1, const float* d_b1, const float* d_w2, const float* d_b2,
+                              void* stream);
+
+/* Refreshes a plain handle's normalisers from fp32 DEVICE statistics on `stream`: d_in_mean / d_in_std [in_dim] (the handle keeps 1 / std, as
+ * dm_mlp_create does), d_out_mean / d_out_std [out_dim].  The same values dm_mlp_create would store.  Refused: a NULL handle or pointer, a gated
+ * handle. */
+int dm_mlp_set_normalizers_device(dm_mlp* m, const float* d_in_mean, const float* d_in_std, const float* d_out_mean, const float* d_out_std, void* stream);
+
+/* ---- PPO minibatch step of a plain 2-layer network on the Hopper tensor cores (R/learning/ppo_agent.py: PPOAgent._update_actor /
+ * _update_critic; solvers/mpi_solver.py wrapping TF's MomentumOptimizer).  A dm_learn workspace holds a learner-owned dm_mlp handle of
+ * max_rows rows (the forward's saved activations), the backward operand tiles and the dW partials.  kind 0: the PPO actor (out_dim <= 64
+ * normalised action means), kind 1: the critic (out_dim 1, the normalised value).  The parameters are the caller's fp32 device tensors in
+ * [units x inputs] layout of dm_mlp_set_weights_device and are updated in place, with the caller's momentum accumulators of the same shapes. */
+typedef struct dm_learn dm_learn;
+typedef struct dm_learn_net {
+    float *w[3], *b[3];            /* parameters: w[l] [units x inputs], b[l] [units] */
+    float *acc_w[3], *acc_b[3];    /* momentum accumulators, same shapes */
+} dm_learn_net;
+/* One minibatch of `rows` rows of a window of samples.  Per row r with sample s = idx[r]:
+ *   x = clip((states[s] - in_mean) * in_istd, +-in_clip) through the network: y = the normalised output.
+ *   actor:  logp = sum_j (-0.5 ((norm_actions[s][j] - y_j) / sigma_j)^2 - logstd[j] - 0.5 log(2 pi)),  sigma = exp(logstd),
+ *           ratio = exp(logp - old_logp[s]) (written to ratio[r] when ratio is not NULL),  A = adv[s],
+ *           loss = -mean_r min(A ratio, A clip(ratio, 1 +- ratio_clip)) + 0.5 mean_r sum_j (min(y_j - bound_min_j, 0)^2 + max(y_j - bound_max_j, 0)^2);
+ *           the surrogate's gradient flows where the unclipped term is the minimum (ties included) or the ratio lies inside the clip range.
+ *           stats[0] += |loss|, stats[1] += the fraction of rows with |ratio - 1| > ratio_clip.
+ *   critic: loss = 0.5 mean_r (norm_targets[s] - y)^2;  stats[0] += loss.
+ * Then per parameter g = dloss/dw + weight_decay w (weights only), acc = momentum acc + g, w -= stepsize acc.  The step is bit-reproducible
+ * (fixed-order reductions).  fp32 device pointers except idx (int64); the actor-only pointers may be NULL for the critic and targets for the
+ * actor. */
+typedef struct dm_learn_batch {
+    const float* states;           /* [samples x in_dim] */
+    const int64_t* idx;            /* [rows] */
+    int rows;
+    const float *in_mean, *in_istd;
+    float in_clip;                 /* <= 0: none */
+    const float *norm_actions, *old_logp, *adv, *logstd, *bound_min, *bound_max;   /* actor: [samples x out_dim], [samples], [samples], [out_dim] x 3 */
+    float ratio_clip;
+    float* ratio;                  /* actor, optional: [rows] the probability ratio of every row */
+    const float* norm_targets;     /* critic: [samples] */
+    float stepsize, momentum, weight_decay;
+    float* stats;                  /* actor: 2 floats, critic: 1 */
+} dm_learn_batch;
+/* Refused: no CUDA device or not sm_90a, bad sizes (out_dim <= 64, kind 1 needs out_dim 1), max_rows <= 0. */
+dm_learn* dm_learn_create(int device, int kind, int in_dim, int h0, int h1, int out_dim, int max_rows);
+/* Loads the parameters' current values into the workspace's tiles (call before the first step and whenever they changed elsewhere). */
+int dm_learn_set_weights(dm_learn* l, const dm_learn_net* net, void* stream);
+/* One minibatch step, 15 launches on `stream`.  Refused: a NULL handle or pointer, rows outside [1, max_rows], ratio_clip <= 0, a negative
+ * stepsize, momentum or weight_decay (or NaN). */
+int dm_learn_step(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* batch, void* stream);
+void dm_learn_destroy(dm_learn* l);
 
 /* ---- test hooks: raw per-env simulator state, layout shared with the CPU oracle (doubles):
  *  [0..2] basePos(scaled) [3..6] baseQuat world->base (x,y,z,w) [7..9] baseOmega [10..12] baseVel(scaled)
