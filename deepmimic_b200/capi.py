@@ -39,13 +39,20 @@ class DmLearnBatch(C.Structure):
                 + [(n, C.c_float) for n in ("stepsize", "momentum", "weight_decay")] + [("stats", C.c_void_p)])
 
 
+class DmLearnDiscBatch(C.Structure):
+    """dm_learn_disc_batch of include/deepmimic_b200.h"""
+    _fields_ = ([(n, C.c_void_p) for n in ("agent", "expert", "agent_idx", "expert_idx")] + [("rows", C.c_int), ("in_mean", C.c_void_p),
+                ("in_istd", C.c_void_p), ("in_clip", C.c_float)]
+                + [(n, C.c_float) for n in ("stepsize", "momentum", "weight_decay", "logit_reg_weight", "grad_penalty_weight")] + [("stats", C.c_void_p)])
+
+
 DM_STATE_OFFSET, DM_STATE_SCALE, DM_ACTION_OFFSET, DM_ACTION_SCALE, DM_ACTION_BOUND_MIN, DM_ACTION_BOUND_MAX, DM_STATE_NORM_GROUPS = range(7)
 
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
            "dm_update", "dm_record_state", "dm_record_goal", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
            "dm_set_snapshot", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
            "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy", "dm_td_lambda_returns", "dm_mlp_set_weights_device", "dm_learn_create",
-           "dm_mlp_set_normalizers_device", "dm_learn_set_weights", "dm_learn_step", "dm_learn_destroy"]
+           "dm_mlp_set_normalizers_device", "dm_learn_set_weights", "dm_learn_step", "dm_learn_disc_step", "dm_learn_destroy"]
 
 
 def lib():
@@ -127,6 +134,7 @@ def lib():
         L.dm_learn_create.argtypes = [C.c_int] * 7
         L.dm_learn_set_weights.argtypes = [vp, C.POINTER(DmLearnNet), vp]
         L.dm_learn_step.argtypes = [vp, C.POINTER(DmLearnNet), C.POINTER(DmLearnBatch), vp]
+        L.dm_learn_disc_step.argtypes = [vp, C.POINTER(DmLearnNet), C.POINTER(DmLearnDiscBatch), vp]
         L.dm_learn_destroy.argtypes = [vp]
         _lib = L
     return _lib
@@ -575,19 +583,24 @@ class TensorCoreGatedMLP:
 
 
 class TensorCoreLearner:
-    """dm_learn_* workspace: PPO minibatch steps of a plain 2-layer torch network (build_policy: kind "actor", build_critic: kind "critic") on the
-    tensor cores.  The network's parameters and the momentum accumulators `acc` ({parameter: tensor}) are updated in place; both must be
-    contiguous float32 CUDA tensors on the workspace's device.  Their device pointers are read again (and checked) by every set_weights(), so a
-    network moved after construction is picked up there, or refused."""
+    """dm_learn_* workspace: minibatch steps of a plain 2-layer torch network on the tensor cores: PPO steps of build_policy (kind "actor") and
+    build_critic (kind "critic"), AMP discriminator steps of build_discriminator (kind "disc", max_rows = agent + expert rows of a step).  The
+    network's parameters and the momentum accumulators `acc` ({parameter: tensor}) are updated in place; both must be contiguous float32 CUDA
+    tensors on the workspace's device.  Their device pointers are read again (and checked) by every set_weights(), so a network moved after
+    construction is picked up there, or refused."""
+    KINDS = dict(actor=0, critic=1, disc=2)
 
     def __init__(self, net, acc, kind, max_rows, device=0):
+        if kind not in self.KINDS:
+            raise ValueError("kind must be 'actor', 'critic' or 'disc' (got %r)" % (kind,))
         if getattr(net, "goal_size", 0) or hasattr(net, "gate_common") or len(net.hidden) != 2:
             raise ValueError("the tensor-core learner implements the plain network with exactly two hidden layers (the gated backward is not built)")
-        self.layers = list(net.hidden) + [net.mean if kind == "actor" else net.out]
+        self.kind = kind
+        self.layers = list(net.hidden) + [dict(actor=getattr(net, "mean", None), critic=getattr(net, "out", None), disc=getattr(net, "logit", None))[kind]]
         self.acc, self.device = acc, device
         ins, outs = [l.weight.shape[1] for l in self.layers], [l.weight.shape[0] for l in self.layers]
         L = lib()
-        self.h = L.dm_learn_create(device, 0 if kind == "actor" else 1, ins[0], outs[0], outs[1], outs[2], max_rows)
+        self.h = L.dm_learn_create(device, self.KINDS[kind], ins[0], outs[0], outs[1], outs[2], max_rows)
         if not self.h:
             raise RuntimeError("dm_learn_create failed: %s" % L.dm_last_error().decode())
         self.h = C.c_void_p(self.h)
@@ -615,9 +628,10 @@ class TensorCoreLearner:
             raise RuntimeError("dm_learn_set_weights: %s" % lib().dm_last_error().decode())
 
     def step(self, batch, stream=None):
-        """batch: a DmLearnBatch"""
-        if lib().dm_learn_step(self.h, C.byref(self.net), C.byref(batch), C.c_void_p(stream) if stream else None) != 0:
-            raise RuntimeError("dm_learn_step: %s" % lib().dm_last_error().decode())
+        """batch: a DmLearnBatch (kinds "actor", "critic") or a DmLearnDiscBatch (kind "disc")"""
+        fn = "dm_learn_disc_step" if self.kind == "disc" else "dm_learn_step"
+        if getattr(lib(), fn)(self.h, C.byref(self.net), C.byref(batch), C.c_void_p(stream) if stream else None) != 0:
+            raise RuntimeError("%s: %s" % (fn, lib().dm_last_error().decode()))
 
     def close(self):
         if self.h:

@@ -12,6 +12,9 @@
 //     acc = m acc + g, w -= lr acc (TF MomentumOptimizer) on the fp32 torch parameters, and the re-tiling of the new weights into the forward
 //     hi + lo tiles and the transposed tiles of the next dX GEMM.  Without an optimiser step the same pass re-tiles fp32 device weights into a
 //     dm_mlp handle (dm_mlp_set_weights_device).
+// The AMP discriminator's step (dm_learn_disc_step) reuses the preparation, transposition and backward GEMMs and adds its least-squares head
+// (which also seeds dd/dd = 1 on the expert rows for the gradient penalty), the per-row ||dd/dx||^2 partials, its statistics and a layer pass
+// that adds the penalty's weight gradients and the logit regulariser.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
@@ -252,6 +255,155 @@ __global__ void __launch_bounds__(256) dm_learn_norm_kernel(const float* mean, c
     if (i >= n) return;
     d_mean[i] = mean[i];
     d_std[i] = invert ? __frcp_rn(std_dev[i]) : std_dev[i];
+}
+
+// ---- the AMP discriminator's minibatch step (R/learning/amp_agent.py: AMPAgent._build_losses, _disc_grad_penalty_loss; mlp_capi.cu:
+// dm_learn_disc_step).  A step of `rows` agent and `rows` expert rows puts the agent rows at [0, rows) and the expert rows at [E, E + rows),
+// E = pad128(rows), so every m tile holds one side only and the penalty's GEMMs address the expert tiles from tile E / 128 on.
+struct LearnDiscHeadParams {
+    const float* out;          // [2E] logits
+    int rows, E;
+    __half* dy_a;              // dY of the logit layer over all 2E rows, as LearnHeadParams::dy_a / dy_b
+    __half* dy_b;
+    __half* seed_a;            // dd / dd = 1 on the real expert rows (0 on their padding), over the E expert rows: A of the penalty's first dX
+    __half* seed_b;            // GEMM, and B of its logit-weight dW GEMM
+    float* partials;           // [2E / 128][3]: sum of (d -+ 1)^2, rows on the right side of 0, sum of d
+};
+
+// one thread per row, grid = 2E / 128.  Least-squares loss (Peng et al. 2021, eq. 8): 0.5 (0.5 mean (d_e - 1)^2 + 0.5 mean (d_a + 1)^2), so the
+// gradient of the SUM over rows is 0.5 (d - 1) on an expert row and 0.5 (d + 1) on an agent row (1 / rows is applied by the optimiser)
+__global__ void __launch_bounds__(kLearnRows) dm_learn_disc_head_kernel(LearnDiscHeadParams P) {
+    __shared__ float red[3][kLearnRows];
+    const int tid = threadIdx.x, row = blockIdx.x * kLearnRows + tid;
+    const bool expert = row >= P.E;
+    const int r = expert ? row - P.E : row;
+    const bool real = r < P.rows;
+    float g = 0.f, part[3] = {0.f, 0.f, 0.f};
+    if (real) {
+        const float d = P.out[row], e = d - (expert ? 1.f : -1.f);
+        g = 0.5f * e;
+        part[0] = e * e;
+        part[1] = (expert ? d > 0.f : d < 0.f) ? 1.f : 0.f;
+        part[2] = d;
+    }
+    __half* dya = P.dy_a + static_cast<size_t>(blockIdx.x) * 2 * kLearnTile;
+    __half* dyb = P.dy_b + static_cast<size_t>(row >> 6) * 2 * 64 * 64;
+    __half* sa = expert ? P.seed_a + static_cast<size_t>(blockIdx.x - P.E / kLearnRows) * 2 * kLearnTile : nullptr;
+    __half* sb = expert ? P.seed_b + static_cast<size_t>(r >> 6) * 2 * 64 * 64 : nullptr;
+    const int k = row & 63;
+    const __half zero = __float2half_rn(0.f);
+    for (int j = 0; j < 64; ++j) {
+        const float v = j == 0 ? g : 0.f;
+        const __half hi = __float2half_rn(v), lo = __float2half_rn(v - __half2float(hi));
+        const int oa = ((j >> 3) * 16 + (tid >> 3)) * 64 + (tid & 7) * 8 + (j & 7);
+        const int o = ((k >> 3) * 8 + (j >> 3)) * 64 + (j & 7) * 8 + (k & 7);
+        dya[oa] = hi;
+        dya[oa + kLearnTile] = lo;
+        dyb[o] = hi;
+        dyb[o + 64 * 64] = lo;
+        if (expert) {
+            sa[oa] = sb[o] = __float2half_rn(j == 0 && real ? 1.f : 0.f);
+            sa[oa + kLearnTile] = sb[o + 64 * 64] = zero;
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < 3; ++i) red[i][tid] = part[i];
+    __syncthreads();
+    for (int w = kLearnRows / 2; w > 0; w >>= 1) {
+        if (tid < w)
+#pragma unroll
+            for (int i = 0; i < 3; ++i) red[i][tid] += red[i][tid + w];
+        __syncthreads();
+    }
+    if (tid < 3) P.partials[blockIdx.x * 3 + tid] = red[tid][0];
+}
+
+// ||g||^2 of every expert row, g = dd / dx the input gradient held as hi + lo operand tiles [E / 128][hi: NC, lo: NC][kLearnTile]; one thread
+// per row (a thread reads 16-byte core-matrix rows: 8 consecutive inputs of its row), the CTA's sum in a fixed tree.  grid = E / 128
+__global__ void __launch_bounds__(kLearnRows) dm_learn_disc_gp_kernel(const __half* g, int NC, float* partials) {
+    __shared__ float red[kLearnRows];
+    const int tid = threadIdx.x;
+    const __half* base = g + static_cast<size_t>(blockIdx.x) * 2 * NC * kLearnTile;
+    float s = 0.f;
+    for (int c = 0; c < NC; ++c)
+        for (int k8 = 0; k8 < 8; ++k8) {
+            const size_t o = static_cast<size_t>(c) * kLearnTile + (k8 * 16 + (tid >> 3)) * 64 + (tid & 7) * 8;
+            __align__(16) __half hi[8], lo[8];
+            *reinterpret_cast<uint4*>(hi) = *reinterpret_cast<const uint4*>(base + o);
+            *reinterpret_cast<uint4*>(lo) = *reinterpret_cast<const uint4*>(base + o + static_cast<size_t>(NC) * kLearnTile);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                const float v = __half2float(hi[e]) + __half2float(lo[e]);
+                s += v * v;
+            }
+        }
+    red[tid] = s;
+    __syncthreads();
+    for (int w = kLearnRows / 2; w > 0; w >>= 1) {
+        if (tid < w) red[tid] += red[tid + w];
+        __syncthreads();
+    }
+    if (tid == 0) partials[blockIdx.x] = red[0];
+}
+
+// one thread: the CTA partials in a fixed order (head CTAs [0, ctas / 2) hold agent rows, the rest expert rows), added to the running statistics:
+// stats[0] += the least-squares loss, [1] += 0.5 mean ||g||^2 (unweighted), [2] += mean(d_e > 0), [3] += mean(d_a < 0), [4] += mean d_e,
+// [5] += mean d_a
+__global__ void dm_learn_disc_stats_kernel(const float* head, int ctas, const float* gp, int gp_ctas, float inv_rows, float* stats) {
+    float a[3] = {0.f, 0.f, 0.f}, e[3] = {0.f, 0.f, 0.f}, q = 0.f;
+    for (int c = 0; c < ctas; ++c)
+        for (int i = 0; i < 3; ++i) (c < ctas / 2 ? a : e)[i] += head[c * 3 + i];
+    for (int c = 0; c < gp_ctas; ++c) q += gp[c];
+    stats[0] += 0.25f * (e[0] + a[0]) * inv_rows;
+    stats[1] += 0.5f * q * inv_rows;
+    stats[2] += e[1] * inv_rows;
+    stats[3] += a[1] * inv_rows;
+    stats[4] += e[2] * inv_rows;
+    stats[5] += a[2] * inv_rows;
+}
+
+struct LearnDiscLayerParams {
+    LearnLayerParams L;        // as dm_learn_layer_kernel; t_tiles for every layer (layer 0's W0^T feeds the penalty's input-gradient GEMM)
+    const float* pen;          // [pen_splits][L.Npad][pen_F] dW partials of 0.5 sum ||g||^2 (no bias term), or null: no penalty
+    int pen_splits, pen_F;
+    float gp_w;                // the penalty's weight
+    float reg;                 // weight decay on top of L.wd for this layer's weights (the logit layer: logit_reg_weight)
+    __half* p_tiles;           // layer 0, or null: W0's forward tiles with K padded to p_NC * 64 (B of the penalty's W0 e GEMM)
+    int p_NC;
+};
+
+// dm_learn_layer_kernel with the penalty's partials and the logit regulariser: g = (sum dW + gp_w sum dW_pen) / rows + (wd + reg) w on the
+// weights, (sum db) / rows on the biases; then the momentum step and the re-tiling
+__global__ void __launch_bounds__(256) dm_learn_disc_layer_kernel(LearnDiscLayerParams D) {
+    const LearnLayerParams& L = D.L;
+    const int k = blockIdx.x * 256 + threadIdx.x, n = blockIdx.y;
+    if (k > L.in_dim) return;
+    const bool bias = k == L.in_dim;
+    float* p = bias ? L.b + n : L.w + static_cast<size_t>(n) * L.in_dim + k;
+    float w = *p;
+    if (L.acc_w) {
+        float g = 0.f;
+        for (int z = 0; z < L.splits; ++z) g += L.partial[(static_cast<size_t>(z) * L.Npad + n) * L.F + k];
+        if (!bias && D.pen) {
+            float q = 0.f;
+            for (int z = 0; z < D.pen_splits; ++z) q += D.pen[(static_cast<size_t>(z) * L.Npad + n) * D.pen_F + k];
+            g += D.gp_w * q;
+        }
+        g *= L.inv_rows;
+        if (!bias) g += (L.wd + D.reg) * w;
+        float* a = bias ? L.acc_b + n : L.acc_w + static_cast<size_t>(n) * L.in_dim + k;
+        const float acc = L.mom * *a + g;
+        *a = acc;
+        w -= L.lr * acc;
+        *p = w;
+    }
+    if (bias) {
+        L.bias_pad[n] = w;
+        return;
+    }
+    learn_put(L.tiles, learn_tile_off(k, n, L.NC, L.BN), L.BN, w);
+    if (L.t_tiles) learn_put(L.t_tiles, learn_tile_off(n, k, L.t_NC, 128), 128, w);
+    if (D.p_tiles) learn_put(D.p_tiles, learn_tile_off(k, n, D.p_NC, 128), 128, w);
 }
 
 }  // namespace dmk

@@ -88,9 +88,11 @@ struct MlpStyleParams {
 //           next dX GEMM's A operand and, as hi + lo, as the dW GEMM's B operand
 //   GRAD_W  dW = X^T dY: A = the layer's input activations transposed (M = padded inputs + the ones feature whose dW row is db), B = dY as
 //           hi + lo (K = minibatch rows); K is split over row-chunk ranges (blockIdx.z) and each split writes its fp32 partial product
-enum { kGradNone = 0, kGradX = 1, kGradW = 2 };
+//   GRAD_XA the AMP discriminator's gradient-penalty chain: the GRAD_X pipeline (B = W^T, or a layer's forward tiles for a product W x), the
+//           mask only where mask_tiles is given, and dH written as the next GEMM's A operand only (dy_a), never as a dW operand
+enum { kGradNone = 0, kGradX = 1, kGradW = 2, kGradXA = 3 };
 struct MlpGradParams {
-    const __half* mask_tiles;  // GRAD_X: the layer's input activations, [m tiles][N / 64][kMlpATile]
+    const __half* mask_tiles;  // GRAD_X: the layer's input activations, [m tiles][N / 64][kMlpATile] (GRAD_XA: or null, no mask)
     __half* dy_a;              // GRAD_X: dH in operand layout [m tiles][hi: N / 64, lo: N / 64][kMlpATile], or null
     __half* dy_b;              // GRAD_X: dH as B of the dW GEMM, [N / 128][row_chunks][hi | lo][128 x 64]
     float* partial;            // GRAD_W: [splits][N][M] (the parameter's [out x in] order)
@@ -195,8 +197,9 @@ __device__ __forceinline__ void mlp_gemm(const MlpGemmParams& P, const MlpStyleP
     static_assert(GRAD == kGradNone || (!LAST && !GATED && !STYLE), "the gradient epilogues replace the hidden-layer epilogue");
     // kGradW: this split's row chunks [c0, c0 + NC) of the KC chunks every m / n tile holds
     // kGradX: A is dY as hi chunks then lo chunks (2 K / 64 chunks per m tile), each against the same W^T chunk: dY exact to fp32 level
+    constexpr bool kDyHiLo = GRAD == kGradX || GRAD == kGradXA;
     const int KW = GRAD == kGradW ? G->row_chunks : P.K / kMlpBK;   // K chunks per n tile of B
-    const int KC = GRAD == kGradX ? 2 * KW : KW;                    // K chunks per m tile of A
+    const int KC = kDyHiLo ? 2 * KW : KW;                           // K chunks per m tile of A
     const int c0 = GRAD == kGradW ? static_cast<int>(blockIdx.z) * G->chunks_per_split : 0;
     const int NC = GRAD == kGradW ? min(G->chunks_per_split, KC - c0) : KC;
     const int NT = GATED ? NC + 2 : NC;                  // pipeline chunks: the K loop, then the gate's scale and bias chunks
@@ -213,7 +216,7 @@ __device__ __forceinline__ void mlp_gemm(const MlpGemmParams& P, const MlpStyleP
             return;
         }
         bulk_g2s(sA, a_src + static_cast<size_t>(c) * kMlpATile, kABytes, &bar_full[s]);
-        bulk_g2s(sA + kABytes, w_src + static_cast<size_t>(GRAD == kGradX ? c % KW : c) * (kWBytes / 2), kWBytes, &bar_full[s]);
+        bulk_g2s(sA + kABytes, w_src + static_cast<size_t>(kDyHiLo ? c % KW : c) * (kWBytes / 2), kWBytes, &bar_full[s]);
     };
 
     if (tid == 0) {
@@ -310,6 +313,18 @@ __device__ __forceinline__ void mlp_gemm(const MlpGemmParams& P, const MlpStyleP
                     t[0] = hi;
                     t[128 * kMlpBK] = __float2half_rn(d - __half2float(hi));
                 }
+            } else if constexpr (GRAD == kGradXA) {
+                const size_t in_tile = (((n & 63) >> 3) * (kMlpBM / 8) + (r >> 3)) * 64 + (r & 7) * 8 + (n & 7);
+                float d0 = v0, d1 = v1;
+                if (G->mask_tiles) {
+                    const __half2 hact = *reinterpret_cast<const __half2*>(G->mask_tiles + (static_cast<size_t>(mt) * (P.N >> 6) + (n >> 6)) * kMlpATile + in_tile);
+                    d0 = __low2float(hact) > 0.f ? v0 : 0.f;
+                    d1 = __high2float(hact) > 0.f ? v1 : 0.f;
+                }
+                __half* t = G->dy_a + (static_cast<size_t>(mt) * 2 * (P.N >> 6) + (n >> 6)) * kMlpATile + in_tile;
+                const __half2 hi = __floats2half2_rn(d0, d1);
+                *reinterpret_cast<__half2*>(t) = hi;
+                *reinterpret_cast<__half2*>(t + static_cast<size_t>(P.N >> 6) * kMlpATile) = __floats2half2_rn(d0 - __low2float(hi), d1 - __high2float(hi));
             } else if constexpr (STYLE) {
                 // the logit is column 0 (the tile's other 63 columns are padding): one thread per row holds it and writes every output of that row
                 if (row < P.M && n == 0) {
@@ -364,6 +379,8 @@ template <int BN>
 __global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_grad_w_kernel(MlpGemmParams P, MlpGradParams G) { mlp_gemm<BN, false, false, false, kGradW>(P, nullptr, &G); }
 template __global__ void dm_mlp_grad_w_kernel<128>(MlpGemmParams, MlpGradParams);
 template __global__ void dm_mlp_grad_w_kernel<64>(MlpGemmParams, MlpGradParams);
+// the AMP discriminator's gradient-penalty products (GRAD_XA, mlp_capi.cu: dm_learn_disc_step), 128-column tiles
+__global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_grad_xa_kernel(MlpGemmParams P, MlpGradParams G) { mlp_gemm<128, false, false, false, kGradXA>(P, nullptr, &G); }
 
 int dm_mlp_smem_bytes(int bn) { return kMlpStages * (kMlpATile * 2 + 2 * bn * kMlpBK * 2) + 1024; }
 

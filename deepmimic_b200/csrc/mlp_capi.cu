@@ -59,6 +59,14 @@ __global__ void dm_learn_critic_head_kernel(LearnHeadParams);
 __global__ void dm_learn_stats_kernel(const float*, int, float, int, float*);
 __global__ void dm_learn_layer_kernel(LearnLayerParams);
 __global__ void dm_learn_norm_kernel(const float*, const float*, int, float*, float*, int);
+// the AMP discriminator's step (kernels/dm_learn.cu, kernels/dm_mlp.cu: dm_mlp_grad_xa_kernel)
+struct LearnDiscHeadParams { const float* out; int rows, E; __half* dy_a; __half* dy_b; __half* seed_a; __half* seed_b; float* partials; };
+struct LearnDiscLayerParams { LearnLayerParams L; const float* pen; int pen_splits, pen_F; float gp_w, reg; __half* p_tiles; int p_NC; };
+__global__ void dm_mlp_grad_xa_kernel(MlpGemmParams, MlpGradParams);
+__global__ void dm_learn_disc_head_kernel(LearnDiscHeadParams);
+__global__ void dm_learn_disc_gp_kernel(const __half*, int, float*);
+__global__ void dm_learn_disc_stats_kernel(const float*, int, const float*, int, float, float*);
+__global__ void dm_learn_disc_layer_kernel(LearnDiscLayerParams);
 }  // namespace dmk
 
 extern "C" void dm_set_last_error(const char* msg);
@@ -148,13 +156,24 @@ void launch_layer(const dmk::LearnLayerParams& L, cudaStream_t st) {
 struct dm_learn {
     dm_mlp* m = nullptr;
     bool actor = true;
+    int kind = 0;
     int max_rows = 0, F[3] = {0, 0, 0}, Nout[3] = {0, 0, 0}, max_splits[3] = {0, 0, 0};
     float* out = nullptr;                                    // [max_rows x out_dim] normalised network output
     __half *xt[3] = {nullptr, nullptr, nullptr};             // transposed saved activations: A of the dW GEMMs
     __half *dy_a[3] = {nullptr, nullptr, nullptr};           // dY of layers 1, 2 in operand layout, hi + lo chunks: A of the dX GEMMs (layer 0 needs none)
     __half *dy_b[3] = {nullptr, nullptr, nullptr};           // dY of every layer as hi + lo: B of the dW GEMMs
-    __half *wt[3] = {nullptr, nullptr, nullptr};             // W1^T, W2^T as hi + lo: B of the dX GEMMs
+    __half *wt[3] = {nullptr, nullptr, nullptr};             // W1^T, W2^T as hi + lo: B of the dX GEMMs (kind 2: also W0^T)
     float *partial[3] = {nullptr, nullptr, nullptr}, *head_partials = nullptr;
+    // kind 2, the discriminator's gradient penalty over the expert rows (at most E = pad128(max_rows / 2)), with the masks m_l = 1[a_l > 0]:
+    //   u1 = m1 w2, u0 = m0 (W1^T u1), e = g = W0^T u0, q0 = m0 (W0 e), q1 = m1 (W1 q0);
+    //   d(0.5 sum ||g||^2)/dW0 = sum u0 e^T, /dW1 = sum u1 q0^T, /dw2 = sum q1 (A of those dW GEMMs: e, q0, q1 transposed; B: u0, u1, the seed)
+    int side_rows = 0, E = 0, Ng = 0, pen_F[3] = {0, 0, 0}, pen_max_splits[3] = {0, 0, 0};   // Ng = pad128(in_dim)
+    __half *seed_a = nullptr, *seed_b = nullptr;             // dd/dd = 1 on the expert rows, A and B layouts of the logit layer's dY
+    __half *u_a[2] = {nullptr, nullptr}, *u_b[2] = {nullptr, nullptr};   // u0, u1 as hi + lo A (next dX GEMM) and B (dW GEMM) operands
+    __half *e_a = nullptr, *q_a[2] = {nullptr, nullptr};     // e, q0, q1 as hi + lo A operands
+    __half *pt[3] = {nullptr, nullptr, nullptr};             // e, q0, q1 transposed: A of the penalty's dW GEMMs
+    __half* w0p = nullptr;                                   // W0's forward tiles with K padded to Ng: B of the W0 e GEMM
+    float *pen[3] = {nullptr, nullptr, nullptr}, *gp_partials = nullptr;
 };
 
 namespace {
@@ -372,15 +391,19 @@ int dm_mlp_set_normalizers_device(dm_mlp* m, const float* d_in_mean, const float
 }
 
 dm_learn* dm_learn_create(int device, int kind, int in_dim, int h0, int h1, int out_dim, int max_rows) {
-    if (kind != 0 && kind != 1) { mlp_fail("dm_learn_create: kind must be 0 (actor) or 1 (critic)"); return nullptr; }
+    if (kind != 0 && kind != 1 && kind != 2) { mlp_fail("dm_learn_create: kind must be 0 (actor), 1 (critic) or 2 (discriminator)"); return nullptr; }
     if (kind == 1 && out_dim != 1) { mlp_fail("dm_learn_create: a critic has one output"); return nullptr; }
+    if (kind == 2 && out_dim != 1) { mlp_fail("dm_learn_create: a discriminator has one output"); return nullptr; }
+    if (kind == 2 && max_rows == 1) { mlp_fail("dm_learn_create: a discriminator step needs max_rows >= 2 (one agent and one expert row)"); return nullptr; }
     if (in_dim <= 0 || h0 <= 0 || h1 <= 0 || out_dim <= 0 || out_dim > 64 || max_rows <= 0) { mlp_fail("dm_learn_create: bad sizes (out_dim must be <= 64)"); return nullptr; }
+    // a discriminator's rows: the agent side in [0, E), the expert side in [E, 2 E), E = pad128(max_rows / 2)
+    const int side = max_rows / 2, E = pad_to(side, 128), rows = kind == 2 ? 2 * E : max_rows;
     // zero weights and an identity output normaliser: dm_learn_set_weights loads the parameters, the output stays normalised
     std::vector<float> w0(static_cast<size_t>(in_dim) * h0), w1(static_cast<size_t>(h0) * h1), w2(static_cast<size_t>(h1) * out_dim), b0(h0), b1(h1), b2(out_dim);
-    dm_mlp* m = dm_mlp_create(device, in_dim, h0, h1, out_dim, w0.data(), b0.data(), w1.data(), b1.data(), w2.data(), b2.data(), nullptr, nullptr, 0.f, nullptr, nullptr, max_rows);
+    dm_mlp* m = dm_mlp_create(device, in_dim, h0, h1, out_dim, w0.data(), b0.data(), w1.data(), b1.data(), w2.data(), b2.data(), nullptr, nullptr, 0.f, nullptr, nullptr, rows);
     if (!m) return nullptr;   // dm_last_error is set
     dm_learn* l = new dm_learn();
-    l->m = m; l->actor = kind == 0; l->max_rows = m->max_rows;
+    l->m = m; l->actor = kind == 0; l->kind = kind; l->max_rows = m->max_rows;
     const int in[3] = {in_dim, h0, h1}, BN[3] = {128, 128, m->N2}, chunks = m->max_rows / 64;
     l->Nout[0] = m->N0; l->Nout[1] = m->N1; l->Nout[2] = m->N2;
     const size_t R = m->max_rows;
@@ -402,6 +425,29 @@ dm_learn* dm_learn_create(int device, int kind, int in_dim, int h0, int h1, int 
             ok = cudaMalloc(&l->dy_a[i], 2 * R * l->Nout[i] * sizeof(__half)) == cudaSuccess && cudaMalloc(&l->wt[i], n * sizeof(__half)) == cudaSuccess &&
                  cudaMemset(l->wt[i], 0, n * sizeof(__half)) == cudaSuccess;
         }
+    }
+    if (ok && kind == 2) {
+        l->side_rows = side; l->E = E; l->Ng = pad_to(in_dim, 128);
+        const int Ng = l->Ng, N0 = m->N0, N1 = m->N1;
+        l->pen_F[0] = Ng; l->pen_F[1] = N0; l->pen_F[2] = N1;
+        for (int i = 0; i < 3; ++i)
+            for (int c = 2; c <= E / 64; c += 2) {
+                int s = 0, cps = 0;
+                dw_split((l->pen_F[i] / 128) * (l->Nout[i] / BN[i]), c, &s, &cps);
+                l->pen_max_splits[i] = std::max(l->pen_max_splits[i], s);
+            }
+        const size_t e = E, h = sizeof(__half), tw = 2 * static_cast<size_t>(N0) * Ng;   // halves of W0^T / W0 as hi + lo tiles
+        ok = cudaMalloc(&l->seed_a, 2 * e * 64 * h) == cudaSuccess && cudaMalloc(&l->seed_b, 2 * e * 64 * h) == cudaSuccess &&
+             cudaMalloc(&l->u_a[0], 2 * e * N0 * h) == cudaSuccess && cudaMalloc(&l->u_b[0], 2 * e * N0 * h) == cudaSuccess &&
+             cudaMalloc(&l->u_a[1], 2 * e * N1 * h) == cudaSuccess && cudaMalloc(&l->u_b[1], 2 * e * N1 * h) == cudaSuccess &&
+             cudaMalloc(&l->e_a, 2 * e * Ng * h) == cudaSuccess && cudaMalloc(&l->q_a[0], 2 * e * N0 * h) == cudaSuccess &&
+             cudaMalloc(&l->q_a[1], 2 * e * N1 * h) == cudaSuccess && cudaMalloc(&l->gp_partials, e / 128 * sizeof(float)) == cudaSuccess &&
+             cudaMalloc(&l->wt[0], tw * h) == cudaSuccess && cudaMemset(l->wt[0], 0, tw * h) == cudaSuccess &&
+             cudaMalloc(&l->w0p, tw * h) == cudaSuccess && cudaMemset(l->w0p, 0, tw * h) == cudaSuccess;
+        for (int i = 0; i < 3 && ok; ++i)
+            ok = cudaMalloc(&l->pt[i], e * l->pen_F[i] * h) == cudaSuccess &&
+                 cudaMalloc(&l->pen[i], static_cast<size_t>(l->pen_max_splits[i]) * l->Nout[i] * l->pen_F[i] * sizeof(float)) == cudaSuccess;
+        ok = ok && cudaFuncSetAttribute(dmk::dm_mlp_grad_xa_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess;
     }
     if (ok) {
         ok = cudaFuncSetAttribute(dmk::dm_mlp_grad_x_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
@@ -431,13 +477,68 @@ void learn_layers(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b,
         launch_layer(L, st);
     }
 }
+// the discriminator's layer passes (kind 2): W0^T and W0's K-padded tiles for the penalty as well; with `b` also the optimiser step with the
+// penalty's partials (psplits of them) and the logit regulariser
+void learn_disc_layers(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* b, const int* splits, const int* psplits, cudaStream_t st) {
+    for (int i = 0; i < 3; ++i) {
+        dmk::LearnDiscLayerParams D{};
+        D.L = layer_params(l->m, i, net->w[i], net->b[i]);
+        D.L.t_tiles = l->wt[i]; D.L.t_NC = l->Nout[i] / 64;
+        if (i == 0) { D.p_tiles = l->w0p; D.p_NC = l->Ng / 64; }
+        if (b) {
+            D.L.acc_w = net->acc_w[i]; D.L.acc_b = net->acc_b[i]; D.L.partial = l->partial[i]; D.L.splits = splits[i]; D.L.Npad = l->Nout[i]; D.L.F = l->F[i];
+            D.L.inv_rows = 1.f / b->rows; D.L.lr = b->stepsize; D.L.mom = b->momentum; D.L.wd = b->weight_decay;
+            D.pen = l->pen[i]; D.pen_splits = psplits[i]; D.pen_F = l->pen_F[i]; D.gp_w = b->grad_penalty_weight; D.reg = i == 2 ? b->logit_reg_weight : 0.f;
+        }
+        dmk::dm_learn_disc_layer_kernel<<<dim3((D.L.in_dim + 1 + 255) / 256, D.L.out_dim), 256, 0, st>>>(D);
+    }
+}
+// the forward over the mt m tiles prepared in the handle's obs_t (the output layer writes `rows` rows of l->out) and the transposition of the
+// saved activations into the dW GEMMs' A operands
+void learn_forward(dm_learn* l, int rows, int mt, cudaStream_t st) {
+    dm_mlp* m = l->m;
+    dmk::MlpGemmParams P{};
+    P.M = rows;
+    P.a_tiles = m->obs_t; P.w_tiles = m->w[0]; P.bias = m->b[0]; P.out_tiles = m->act0; P.K = m->K0; P.N = m->N0;
+    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, m->N0 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
+    P.a_tiles = m->act0; P.w_tiles = m->w[1]; P.bias = m->b[1]; P.out_tiles = m->act1; P.K = m->N0; P.N = m->N1;
+    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, m->N1 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
+    P.a_tiles = m->act1; P.w_tiles = m->w[2]; P.bias = m->b[2]; P.out_tiles = nullptr; P.K = m->N1; P.N = m->N2;
+    P.actions = l->out; P.out_mean = m->out_mean; P.out_std = m->out_std; P.noise = nullptr; P.out_dim = m->out_dim;
+    dmk::dm_mlp_gemm_kernel<64, true><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P);
+    const int chunks = 2 * mt;
+    dmk::LearnTransposeParams T{{m->obs_t, m->act0, m->act1}, {l->xt[0], l->xt[1], l->xt[2]}, {m->K0 / 64, m->N0 / 64, m->N1 / 64},
+                                {m->in_dim, m->h0, m->h1}, {l->F[0], l->F[1], l->F[2]}, chunks};
+    dmk::dm_learn_transpose_kernel<<<dim3(std::max(l->F[0], std::max(l->F[1], l->F[2])) / 128, chunks, 3), 256, 0, st>>>(T);
+}
+// backward of the dY a head wrote into dy_a[2] / dy_b[2], output layer first: dW_i = X_i^T dY_i (split K), dY_{i-1} = (dY_i W_i^T) * 1[X_i > 0]
+void learn_backward(dm_learn* l, int rows, int mt, const int* splits, const int* cps, cudaStream_t st) {
+    dm_mlp* m = l->m;
+    const int chunks = 2 * mt;
+    const __half* act[3] = {m->obs_t, m->act0, m->act1};
+    for (int i = 2; i >= 0; --i) {
+        const int BN = i == 2 ? m->N2 : 128;
+        dmk::MlpGemmParams W{};
+        W.a_tiles = l->xt[i]; W.w_tiles = l->dy_b[i]; W.M = l->F[i]; W.N = l->Nout[i];
+        const dmk::MlpGradParams GW{nullptr, nullptr, nullptr, l->partial[i], chunks, cps[i]};
+        const dim3 gw(l->F[i] / 128, l->Nout[i] / BN, splits[i]);
+        if (i == 2) dmk::dm_mlp_grad_w_kernel<64><<<gw, 256, dmk::dm_mlp_smem_bytes(64), st>>>(W, GW);
+        else dmk::dm_mlp_grad_w_kernel<128><<<gw, 256, dmk::dm_mlp_smem_bytes(128), st>>>(W, GW);
+        if (i == 0) break;
+        dmk::MlpGemmParams X{};
+        X.a_tiles = l->dy_a[i]; X.w_tiles = l->wt[i]; X.M = rows; X.K = l->Nout[i]; X.N = l->Nout[i - 1];
+        const dmk::MlpGradParams GX{act[i], i > 1 ? l->dy_a[i - 1] : nullptr, l->dy_b[i - 1], nullptr, chunks, 0};
+        dmk::dm_mlp_grad_x_kernel<<<dim3(mt, l->Nout[i - 1] / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(X, GX);
+    }
+}
 }  // namespace
 
 int dm_learn_set_weights(dm_learn* l, const dm_learn_net* net, void* stream) {
     if (!l) return mlp_fail("dm_learn_set_weights: null handle");
     if (learn_net_check(net, "dm_learn_set_weights")) return 1;
     if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_set_weights: cudaSetDevice failed");
-    learn_layers(l, net, nullptr, 0, nullptr, static_cast<cudaStream_t>(stream));
+    if (l->kind == 2) learn_disc_layers(l, net, nullptr, nullptr, nullptr, static_cast<cudaStream_t>(stream));
+    else learn_layers(l, net, nullptr, 0, nullptr, static_cast<cudaStream_t>(stream));
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return mlp_fail(std::string("dm_learn_set_weights: ") + cudaGetErrorString(e));
     return 0;
@@ -445,6 +546,7 @@ int dm_learn_set_weights(dm_learn* l, const dm_learn_net* net, void* stream) {
 
 int dm_learn_step(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, void* stream) {
     if (!l) return mlp_fail("dm_learn_step: null handle");
+    if (l->kind == 2) return mlp_fail("dm_learn_step: the workspace is a discriminator's (kind 2); use dm_learn_disc_step");
     if (learn_net_check(net, "dm_learn_step")) return 1;
     if (!b) return mlp_fail("dm_learn_step: null batch");
     if (b->rows <= 0 || b->rows > l->max_rows) return mlp_fail("dm_learn_step: rows out of range");
@@ -467,45 +569,91 @@ int dm_learn_step(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b,
     // forward: gathered rows -> the plain trunk -> the normalised output (identity output normaliser)
     dmk::LearnPrepParams Q{b->states, b->idx, b->in_mean, b->in_istd, b->in_clip > 0.f ? b->in_clip : 1e30f, m->in_dim, rows, m->K0 / 64, m->obs_t};
     dmk::dm_learn_prep_kernel<<<dim3(mt, m->K0 / 64), 128, 0, st>>>(Q);
-    dmk::MlpGemmParams P{};
-    P.M = rows;
-    P.a_tiles = m->obs_t; P.w_tiles = m->w[0]; P.bias = m->b[0]; P.out_tiles = m->act0; P.K = m->K0; P.N = m->N0;
-    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, m->N0 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
-    P.a_tiles = m->act0; P.w_tiles = m->w[1]; P.bias = m->b[1]; P.out_tiles = m->act1; P.K = m->N0; P.N = m->N1;
-    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, m->N1 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
-    P.a_tiles = m->act1; P.w_tiles = m->w[2]; P.bias = m->b[2]; P.out_tiles = nullptr; P.K = m->N1; P.N = m->N2;
-    P.actions = l->out; P.out_mean = m->out_mean; P.out_std = m->out_std; P.noise = nullptr; P.out_dim = m->out_dim;
-    dmk::dm_mlp_gemm_kernel<64, true><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P);
-    // the saved activations transposed for the dW GEMMs
-    dmk::LearnTransposeParams T{{m->obs_t, m->act0, m->act1}, {l->xt[0], l->xt[1], l->xt[2]}, {m->K0 / 64, m->N0 / 64, m->N1 / 64},
-                                {m->in_dim, m->h0, m->h1}, {l->F[0], l->F[1], l->F[2]}, chunks};
-    dmk::dm_learn_transpose_kernel<<<dim3(std::max(l->F[0], std::max(l->F[1], l->F[2])) / 128, chunks, 3), 256, 0, st>>>(T);
+    learn_forward(l, rows, mt, st);
     // loss head: dY of the output layer, the loss partials, the statistics
     dmk::LearnHeadParams H{l->out, b->idx, rows, m->out_dim, l->dy_a[2], l->dy_b[2], l->head_partials, b->norm_actions, b->old_logp, b->adv, b->logstd,
                            b->bound_min, b->bound_max, b->ratio_clip, b->ratio, b->norm_targets};
     if (l->actor) dmk::dm_learn_actor_head_kernel<<<mt, 128, 0, st>>>(H);
     else dmk::dm_learn_critic_head_kernel<<<mt, 128, 0, st>>>(H);
     dmk::dm_learn_stats_kernel<<<1, 1, 0, st>>>(l->head_partials, mt, 1.f / rows, l->actor ? 1 : 0, b->stats);
-    // backward, output layer first: dW_i = X_i^T dY_i (split K), dY_{i-1} = (dY_i W_i^T) * 1[X_i > 0]
-    const __half* act[3] = {m->obs_t, m->act0, m->act1};
-    for (int i = 2; i >= 0; --i) {
-        const int BN = i == 2 ? m->N2 : 128;
-        dmk::MlpGemmParams W{};
-        W.a_tiles = l->xt[i]; W.w_tiles = l->dy_b[i]; W.M = l->F[i]; W.N = l->Nout[i];
-        const dmk::MlpGradParams GW{nullptr, nullptr, nullptr, l->partial[i], chunks, cps[i]};
-        const dim3 gw(l->F[i] / 128, l->Nout[i] / BN, splits[i]);
-        if (i == 2) dmk::dm_mlp_grad_w_kernel<64><<<gw, 256, dmk::dm_mlp_smem_bytes(64), st>>>(W, GW);
-        else dmk::dm_mlp_grad_w_kernel<128><<<gw, 256, dmk::dm_mlp_smem_bytes(128), st>>>(W, GW);
-        if (i == 0) break;
-        dmk::MlpGemmParams X{};
-        X.a_tiles = l->dy_a[i]; X.w_tiles = l->wt[i]; X.M = rows; X.K = l->Nout[i]; X.N = l->Nout[i - 1];
-        const dmk::MlpGradParams GX{act[i], i > 1 ? l->dy_a[i - 1] : nullptr, l->dy_b[i - 1], nullptr, chunks, 0};
-        dmk::dm_mlp_grad_x_kernel<<<dim3(mt, l->Nout[i - 1] / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(X, GX);
-    }
+    learn_backward(l, rows, mt, splits, cps, st);
     // optimiser step and re-tiling, after every GEMM that read the old weights
     learn_layers(l, net, b, rows, splits, st);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return mlp_fail(std::string("dm_learn_step: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+int dm_learn_disc_step(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* b, void* stream) {
+    if (!l) return mlp_fail("dm_learn_disc_step: null handle");
+    if (l->kind != 2) return mlp_fail("dm_learn_disc_step: the workspace is a PPO actor's or critic's (kind 0 or 1); a discriminator step needs kind 2");
+    if (learn_net_check(net, "dm_learn_disc_step")) return 1;
+    if (!b) return mlp_fail("dm_learn_disc_step: null batch");
+    if (b->rows <= 0 || b->rows > l->side_rows) return mlp_fail("dm_learn_disc_step: rows out of range (1 to max_rows / 2 per side)");
+    if (!b->agent || !b->expert || !b->agent_idx || !b->expert_idx || !b->in_mean || !b->in_istd || !b->stats)
+        return mlp_fail("dm_learn_disc_step: null observation, index, normaliser or statistics pointer");
+    if (!(b->stepsize >= 0.f) || !(b->momentum >= 0.f) || !(b->weight_decay >= 0.f) || !(b->logit_reg_weight >= 0.f) || !(b->grad_penalty_weight >= 0.f))
+        return mlp_fail("dm_learn_disc_step: stepsize, momentum, weight_decay, logit_reg_weight and grad_penalty_weight must be >= 0");
+    dm_mlp* m = l->m;
+    if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_learn_disc_step: cudaSetDevice failed");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    // agent rows in m tiles [0, et), expert rows in [et, 2 et)
+    const int rows = b->rows, E = pad_to(rows, 128), et = E / 128, mt = 2 * et, chunks = 2 * mt, echunks = 2 * et;
+    const int BN[3] = {128, 128, m->N2};
+    int splits[3], cps[3], psplits[3], pcps[3];
+    for (int i = 0; i < 3; ++i) {
+        dw_split((l->F[i] / 128) * (l->Nout[i] / BN[i]), chunks, &splits[i], &cps[i]);
+        dw_split((l->pen_F[i] / 128) * (l->Nout[i] / BN[i]), echunks, &psplits[i], &pcps[i]);
+        if (splits[i] > l->max_splits[i] || psplits[i] > l->pen_max_splits[i]) return mlp_fail("dm_learn_disc_step: internal error: dW split count exceeds the workspace");
+    }
+    // forward over both sides: each gathered into its own m tiles
+    const int NC0 = m->K0 / 64;
+    dmk::LearnPrepParams Q{b->agent, b->agent_idx, b->in_mean, b->in_istd, b->in_clip > 0.f ? b->in_clip : 1e30f, m->in_dim, rows, NC0, m->obs_t};
+    dmk::dm_learn_prep_kernel<<<dim3(et, NC0), 128, 0, st>>>(Q);
+    Q.x = b->expert; Q.idx = b->expert_idx; Q.tiles = m->obs_t + static_cast<size_t>(et) * NC0 * dmk::kMlpATileHalves;
+    dmk::dm_learn_prep_kernel<<<dim3(et, NC0), 128, 0, st>>>(Q);
+    learn_forward(l, 2 * E, mt, st);
+    // least-squares head: dY of the logit over both sides, the penalty's seed over the expert rows, the partials
+    const dmk::LearnDiscHeadParams H{l->out, rows, E, l->dy_a[2], l->dy_b[2], l->seed_a, l->seed_b, l->head_partials};
+    dmk::dm_learn_disc_head_kernel<<<mt, 128, 0, st>>>(H);
+    learn_backward(l, 2 * E, mt, splits, cps, st);
+    // the gradient penalty on the expert tiles, with the forward's masks: u1 = m1 w2, u0 = m0 (W1^T u1) (hi + lo A and B operands) ...
+    const size_t tile = dmk::kMlpATileHalves;
+    const __half* act0e = m->act0 + static_cast<size_t>(et) * (m->N0 / 64) * tile;
+    const __half* act1e = m->act1 + static_cast<size_t>(et) * (m->N1 / 64) * tile;
+    dmk::MlpGemmParams X{};
+    X.M = E;
+    X.a_tiles = l->seed_a; X.w_tiles = l->wt[2]; X.K = m->N2; X.N = m->N1;
+    dmk::dm_mlp_grad_x_kernel<<<dim3(et, m->N1 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(X, dmk::MlpGradParams{act1e, l->u_a[1], l->u_b[1], nullptr, echunks, 0});
+    X.a_tiles = l->u_a[1]; X.w_tiles = l->wt[1]; X.K = m->N1; X.N = m->N0;
+    dmk::dm_mlp_grad_x_kernel<<<dim3(et, m->N0 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(X, dmk::MlpGradParams{act0e, l->u_a[0], l->u_b[0], nullptr, echunks, 0});
+    // ... e = g = W0^T u0 (no mask), q0 = m0 (W0 e), q1 = m1 (W1 q0): hi + lo A operands only
+    X.a_tiles = l->u_a[0]; X.w_tiles = l->wt[0]; X.K = m->N0; X.N = l->Ng;
+    dmk::dm_mlp_grad_xa_kernel<<<dim3(et, l->Ng / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(X, dmk::MlpGradParams{nullptr, l->e_a, nullptr, nullptr, echunks, 0});
+    X.a_tiles = l->e_a; X.w_tiles = l->w0p; X.K = l->Ng; X.N = m->N0;
+    dmk::dm_mlp_grad_xa_kernel<<<dim3(et, m->N0 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(X, dmk::MlpGradParams{act0e, l->q_a[0], nullptr, nullptr, echunks, 0});
+    X.a_tiles = l->q_a[0]; X.w_tiles = m->w[1]; X.K = m->N0; X.N = m->N1;
+    dmk::dm_mlp_grad_xa_kernel<<<dim3(et, m->N1 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(X, dmk::MlpGradParams{act1e, l->q_a[1], nullptr, nullptr, echunks, 0});
+    dmk::dm_learn_disc_gp_kernel<<<et, 128, 0, st>>>(l->e_a, l->Ng / 64, l->gp_partials);
+    // e, q0, q1 transposed (their hi chunks; no ones feature: the penalty has no bias gradient), then d(0.5 sum ||g||^2)/dW: sum u0 e^T,
+    // sum u1 q0^T, sum q1 (B = the seed)
+    const dmk::LearnTransposeParams T{{l->e_a, l->q_a[0], l->q_a[1]}, {l->pt[0], l->pt[1], l->pt[2]}, {2 * l->Ng / 64, 2 * m->N0 / 64, 2 * m->N1 / 64},
+                                      {-1, -1, -1}, {l->pen_F[0], l->pen_F[1], l->pen_F[2]}, echunks};
+    dmk::dm_learn_transpose_kernel<<<dim3(std::max(l->pen_F[0], std::max(l->pen_F[1], l->pen_F[2])) / 128, echunks, 3), 256, 0, st>>>(T);
+    const __half* pen_b[3] = {l->u_b[0], l->u_b[1], l->seed_b};
+    for (int i = 0; i < 3; ++i) {
+        dmk::MlpGemmParams W{};
+        W.a_tiles = l->pt[i]; W.w_tiles = pen_b[i]; W.M = l->pen_F[i]; W.N = l->Nout[i];
+        const dmk::MlpGradParams GW{nullptr, nullptr, nullptr, l->pen[i], echunks, pcps[i]};
+        const dim3 gw(l->pen_F[i] / 128, l->Nout[i] / BN[i], psplits[i]);
+        if (i == 2) dmk::dm_mlp_grad_w_kernel<64><<<gw, 256, dmk::dm_mlp_smem_bytes(64), st>>>(W, GW);
+        else dmk::dm_mlp_grad_w_kernel<128><<<gw, 256, dmk::dm_mlp_smem_bytes(128), st>>>(W, GW);
+    }
+    dmk::dm_learn_disc_stats_kernel<<<1, 1, 0, st>>>(l->head_partials, mt, l->gp_partials, et, 1.f / rows, b->stats);
+    // optimiser step and re-tiling, after every GEMM that read the old weights
+    learn_disc_layers(l, net, b, splits, psplits, st);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return mlp_fail(std::string("dm_learn_disc_step: ") + cudaGetErrorString(e));
     return 0;
 }
 
@@ -516,7 +664,9 @@ void dm_learn_destroy(dm_learn* l) {
         dm_mlp_destroy(l->m);
     }
     cudaFree(l->out); cudaFree(l->head_partials);
-    for (int i = 0; i < 3; ++i) { cudaFree(l->xt[i]); cudaFree(l->dy_a[i]); cudaFree(l->dy_b[i]); cudaFree(l->wt[i]); cudaFree(l->partial[i]); }
+    for (int i = 0; i < 3; ++i) { cudaFree(l->xt[i]); cudaFree(l->dy_a[i]); cudaFree(l->dy_b[i]); cudaFree(l->wt[i]); cudaFree(l->partial[i]); cudaFree(l->pt[i]); cudaFree(l->pen[i]); }
+    for (int i = 0; i < 2; ++i) { cudaFree(l->u_a[i]); cudaFree(l->u_b[i]); cudaFree(l->q_a[i]); }
+    cudaFree(l->seed_a); cudaFree(l->seed_b); cudaFree(l->e_a); cudaFree(l->w0p); cudaFree(l->gp_partials);
     delete l;
 }
 

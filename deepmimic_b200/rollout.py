@@ -351,7 +351,8 @@ class BatchedRollout:
     then also returns the agent's AMP observation of every transition and the discriminator's logits, style rewards and amp_rewards, the reward
     an AMP learner trains on: the style reward in imitate_amp (the scene's own reward is not used there), (1 - task_reward_lerp) style +
     task_reward_lerp task reward in the task scenes, which need task_reward_lerp.  On the tensor_core backend the discriminator's reward runs in
-    four launches (operand preparation, two hidden layers, the logit head with the reward epilogue).
+    four launches (operand preparation, two hidden layers, the logit head with the reward epilogue).  learner.AMPDiscLearner trains the
+    discriminator and refreshes its tensor-core handle (weights and amp_norm) on the device after every update().
 
     critic: a Critic (build_critic) with discount and td_lambda, which the reference reads from the agent file (Discount, TDLambda; there is no
     default).  val_norm is built from the env's reward bounds (val_norm_from_rewards).  collect() then also evaluates the critic on every

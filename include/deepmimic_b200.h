@@ -258,13 +258,36 @@ typedef struct dm_learn_batch {
     float stepsize, momentum, weight_decay;
     float* stats;                  /* actor: 2 floats, critic: 1 */
 } dm_learn_batch;
-/* Refused: no CUDA device or not sm_90a, bad sizes (out_dim <= 64, kind 1 needs out_dim 1), max_rows <= 0. */
+/* kind 2: the AMP discriminator (R/learning/amp_agent.py: AMPAgent._build_losses, _disc_grad_penalty_loss, _disc_weight_decay_loss,
+ * _disc_logit_reg_loss, _update_disc), out_dim 1, stepped by dm_learn_disc_step; max_rows counts the rows of one step, agent and expert
+ * together (up to max_rows / 2 per side).  One step of `rows` agent rows a_r = agent[agent_idx[r]] and `rows` expert rows
+ * e_r = expert[expert_idx[r]], each normalised and clipped as x = clip((. - in_mean) * in_istd, +-in_clip), logits d = D(x):
+ *   disc_loss    = 0.5 (0.5 mean_r (d(e_r) - 1)^2 + 0.5 mean_r (d(a_r) + 1)^2)              (least squares, Peng et al. 2021, eq. 8)
+ *   grad_penalty = 0.5 mean_r ||dd/dx (e_r)||^2                                                (the ReLU masks held constant)
+ *   loss = disc_loss + grad_penalty_weight grad_penalty + weight_decay sum_l ||W_l||^2 / 2 (the logit layer included, biases not)
+ *          + logit_reg_weight ||W_logit||^2 / 2
+ * then acc = momentum acc + dloss/dw, w -= stepsize acc.  stats (6 floats) += {disc_loss, grad_penalty, mean(d_e > 0), mean(d_a < 0), mean d_e,
+ * mean d_a}.  Bit-reproducible (fixed-order reductions).  fp32 device pointers except the int64 indices. */
+typedef struct dm_learn_disc_batch {
+    const float *agent, *expert;   /* [agent samples x in_dim], [expert samples x in_dim] */
+    const int64_t *agent_idx, *expert_idx;   /* [rows] each */
+    int rows;                      /* per side */
+    const float *in_mean, *in_istd;
+    float in_clip;                 /* <= 0: none */
+    float stepsize, momentum, weight_decay, logit_reg_weight, grad_penalty_weight;
+    float* stats;                  /* 6 floats */
+} dm_learn_disc_batch;
+/* Refused: no CUDA device or not sm_90a, a kind other than 0, 1, 2, bad sizes (out_dim <= 64, kinds 1 and 2 need out_dim 1), max_rows <= 0
+ * (kind 2: < 2). */
 dm_learn* dm_learn_create(int device, int kind, int in_dim, int h0, int h1, int out_dim, int max_rows);
 /* Loads the parameters' current values into the workspace's tiles (call before the first step and whenever they changed elsewhere). */
 int dm_learn_set_weights(dm_learn* l, const dm_learn_net* net, void* stream);
-/* One minibatch step, 15 launches on `stream`.  Refused: a NULL handle or pointer, rows outside [1, max_rows], ratio_clip <= 0, a negative
- * stepsize, momentum or weight_decay (or NaN). */
+/* One PPO minibatch step (kinds 0 and 1), 15 launches on `stream`.  Refused: a NULL handle or pointer, a kind 2 workspace, rows outside
+ * [1, max_rows], ratio_clip <= 0, a negative stepsize, momentum or weight_decay (or NaN). */
 int dm_learn_step(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* batch, void* stream);
+/* One discriminator step (kind 2), 26 launches on `stream`.  Refused: a NULL handle or pointer, a kind 0 or 1 workspace, rows outside
+ * [1, max_rows / 2], a negative (or NaN) stepsize, momentum, weight_decay, logit_reg_weight or grad_penalty_weight. */
+int dm_learn_disc_step(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* batch, void* stream);
 void dm_learn_destroy(dm_learn* l);
 
 /* ---- test hooks: raw per-env simulator state, layout shared with the CPU oracle (doubles):
