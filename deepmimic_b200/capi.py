@@ -46,13 +46,25 @@ class DmLearnDiscBatch(C.Structure):
                 + [(n, C.c_float) for n in ("stepsize", "momentum", "weight_decay", "logit_reg_weight", "grad_penalty_weight")] + [("stats", C.c_void_p)])
 
 
+class DmLearnGatedNet(C.Structure):
+    """dm_learn_gated_net of include/deepmimic_b200.h"""
+    _fields_ = [(n, C.c_void_p * 10) for n in ("w", "b", "acc_w", "acc_b")]
+
+
+class DmLearnGatedBatch(C.Structure):
+    """dm_learn_gated_batch of include/deepmimic_b200.h; the dm_learn_batch fields read and write through it"""
+    _anonymous_ = ("batch",)
+    _fields_ = [("batch", DmLearnBatch), ("goals", C.c_void_p), ("g_mean", C.c_void_p), ("g_istd", C.c_void_p), ("g_clip", C.c_float)]
+
+
 DM_STATE_OFFSET, DM_STATE_SCALE, DM_ACTION_OFFSET, DM_ACTION_SCALE, DM_ACTION_BOUND_MIN, DM_ACTION_BOUND_MAX, DM_STATE_NORM_GROUPS = range(7)
 
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
            "dm_update", "dm_record_state", "dm_record_goal", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
            "dm_set_snapshot", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
            "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy", "dm_td_lambda_returns", "dm_mlp_set_weights_device", "dm_learn_create",
-           "dm_mlp_set_normalizers_device", "dm_learn_set_weights", "dm_learn_step", "dm_learn_disc_step", "dm_learn_destroy"]
+           "dm_mlp_set_normalizers_device", "dm_learn_set_weights", "dm_learn_step", "dm_learn_disc_step", "dm_learn_destroy",
+           "dm_learn_create_gated", "dm_learn_set_gated_weights", "dm_learn_gated_step", "dm_mlp_set_gated_weights_device", "dm_mlp_set_gated_normalizers_device"]
 
 
 def lib():
@@ -136,6 +148,12 @@ def lib():
         L.dm_learn_step.argtypes = [vp, C.POINTER(DmLearnNet), C.POINTER(DmLearnBatch), vp]
         L.dm_learn_disc_step.argtypes = [vp, C.POINTER(DmLearnNet), C.POINTER(DmLearnDiscBatch), vp]
         L.dm_learn_destroy.argtypes = [vp]
+        L.dm_learn_create_gated.restype = vp
+        L.dm_learn_create_gated.argtypes = [C.c_int] * 10
+        L.dm_learn_set_gated_weights.argtypes = [vp, C.POINTER(DmLearnGatedNet), vp]
+        L.dm_learn_gated_step.argtypes = [vp, C.POINTER(DmLearnGatedNet), C.POINTER(DmLearnGatedBatch), vp]
+        L.dm_mlp_set_gated_weights_device.argtypes = [vp, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), vp]
+        L.dm_mlp_set_gated_normalizers_device.argtypes = [vp] * 8
         _lib = L
     return _lib
 
@@ -545,6 +563,7 @@ class TensorCoreGatedMLP:
         self.goal_dim, gate_common = gcw.shape
         self.in_dim, self.out_dim = w0.shape[0] - self.goal_dim, w2.shape[1]
         gate_hidden = gh[0][0].shape[1]
+        self.h0, self.h1, self.gate_common, self.gate_hidden = w0.shape[1], w1.shape[1], gate_common, gate_hidden
         p = lambda a: None if a is None else a.ctypes.data_as(_fp)
         pair = lambda ab, i: (_fp * 2)(p(ab[0][i]), p(ab[1][i]))
         W = DmMlpGatedWeights(self.in_dim, self.goal_dim, w0.shape[1], w1.shape[1], self.out_dim, gate_common, gate_hidden,
@@ -566,6 +585,31 @@ class TensorCoreGatedMLP:
         if rc != 0:
             raise RuntimeError("dm_mlp_forward_gated: %s" % lib().dm_last_error().decode())
         return actions
+
+    def set_weights_device(self, layers, stream=None):
+        """dm_mlp_set_gated_weights_device: re-tiles the handle on the device from the ten torch Linear layers of gated_layers(net, head)
+        with fp32 CUDA parameters ([out, in] weights); the normalisers are kept"""
+        S, G, h0, h1, A, GC, GH = self.in_dim, self.goal_dim, self.h0, self.h1, self.out_dim, self.gate_common, self.gate_hidden
+        shapes = _gated_shapes(S, G, h0, h1, A, GC, GH)
+        if len(layers) != 10:
+            raise ValueError("set_weights_device: need the ten layers of gated_layers() (got %d)" % len(layers))
+        for l, shape in zip(layers, shapes):
+            _check_device_f32(l.weight, "set_weights_device", shape)
+            _check_device_f32(l.bias, "set_weights_device", shape[:1])
+        w = (C.c_void_p * 10)(*[l.weight.data_ptr() for l in layers])
+        b = (C.c_void_p * 10)(*[l.bias.data_ptr() for l in layers])
+        if lib().dm_mlp_set_gated_weights_device(self.h, w, b, C.c_void_p(stream) if stream else None) != 0:
+            raise RuntimeError("dm_mlp_set_gated_weights_device: %s" % lib().dm_last_error().decode())
+
+    def set_normalizers_device(self, s_mean, s_std, g_mean, g_std, out_mean, out_std, stream=None):
+        """dm_mlp_set_gated_normalizers_device: the state, goal and output normalisers from contiguous float32 CUDA tensors ([in_dim],
+        [goal_dim], [out_dim]) on the device, the values dm_mlp_create_gated would store"""
+        ts = (("s_mean", s_mean, self.in_dim), ("s_std", s_std, self.in_dim), ("g_mean", g_mean, self.goal_dim), ("g_std", g_std, self.goal_dim),
+              ("out_mean", out_mean, self.out_dim), ("out_std", out_std, self.out_dim))
+        for name, t, n in ts:
+            _check_device_f32(t, "set_normalizers_device: " + name, (n,))
+        if lib().dm_mlp_set_gated_normalizers_device(self.h, *[C.c_void_p(t.data_ptr()) for _, t, _ in ts], C.c_void_p(stream) if stream else None) != 0:
+            raise RuntimeError("dm_mlp_set_gated_normalizers_device: %s" % lib().dm_last_error().decode())
 
     def launches(self):
         return int(lib().dm_mlp_launches(self.h))
@@ -589,12 +633,14 @@ class TensorCoreLearner:
     tensors on the workspace's device.  Their device pointers are read again (and checked) by every set_weights(), so a network moved after
     construction is picked up there, or refused."""
     KINDS = dict(actor=0, critic=1, disc=2)
+    _NET, _SET = DmLearnNet, "dm_learn_set_weights"
 
     def __init__(self, net, acc, kind, max_rows, device=0):
         if kind not in self.KINDS:
             raise ValueError("kind must be 'actor', 'critic' or 'disc' (got %r)" % (kind,))
         if getattr(net, "goal_size", 0) or hasattr(net, "gate_common") or len(net.hidden) != 2:
-            raise ValueError("the tensor-core learner implements the plain network with exactly two hidden layers (the gated backward is not built)")
+            raise ValueError("the tensor-core learner implements the plain network with exactly two hidden layers (gated networks: "
+                             "TensorCoreGatedLearner)")
         self.kind = kind
         self.layers = list(net.hidden) + [dict(actor=getattr(net, "mean", None), critic=getattr(net, "out", None), disc=getattr(net, "logit", None))[kind]]
         self.acc, self.device = acc, device
@@ -617,19 +663,22 @@ class TensorCoreLearner:
                 _check_device_f32(p, "TensorCoreLearner parameter", None, dev)
                 _check_device_f32(self.acc[p], "TensorCoreLearner accumulator", tuple(p.shape), dev)
         p = lambda t: C.c_void_p(t.data_ptr())
-        arr = lambda ts: (C.c_void_p * 3)(*[p(t) for t in ts])
-        self.net = DmLearnNet(arr([l.weight for l in self.layers]), arr([l.bias for l in self.layers]),
-                              arr([self.acc[l.weight] for l in self.layers]), arr([self.acc[l.bias] for l in self.layers]))
+        arr = lambda ts: (C.c_void_p * len(ts))(*[p(t) for t in ts])
+        self.net = self._NET(arr([l.weight for l in self.layers]), arr([l.bias for l in self.layers]),
+                             arr([self.acc[l.weight] for l in self.layers]), arr([self.acc[l.bias] for l in self.layers]))
 
     def set_weights(self, stream=None):
         """binds the parameters' current storage (checked) and loads their values into the workspace's tiles"""
         self._bind()
-        if lib().dm_learn_set_weights(self.h, C.byref(self.net), C.c_void_p(stream) if stream else None) != 0:
-            raise RuntimeError("dm_learn_set_weights: %s" % lib().dm_last_error().decode())
+        if getattr(lib(), self._SET)(self.h, C.byref(self.net), C.c_void_p(stream) if stream else None) != 0:
+            raise RuntimeError("%s: %s" % (self._SET, lib().dm_last_error().decode()))
+
+    def _step_fn(self):
+        return "dm_learn_disc_step" if self.kind == "disc" else "dm_learn_step"
 
     def step(self, batch, stream=None):
-        """batch: a DmLearnBatch (kinds "actor", "critic") or a DmLearnDiscBatch (kind "disc")"""
-        fn = "dm_learn_disc_step" if self.kind == "disc" else "dm_learn_step"
+        """batch: a DmLearnBatch (kinds "actor", "critic"), a DmLearnDiscBatch (kind "disc") or a DmLearnGatedBatch (TensorCoreGatedLearner)"""
+        fn = self._step_fn()
         if getattr(lib(), fn)(self.h, C.byref(self.net), C.byref(batch), C.c_void_p(stream) if stream else None) != 0:
             raise RuntimeError("%s: %s" % (fn, lib().dm_last_error().decode()))
 
@@ -643,3 +692,53 @@ class TensorCoreLearner:
             self.close()
         except Exception:
             pass
+
+
+def gated_layers(net, head):
+    """the ten Linear layers of a gated network (build_gated_policy, or build_critic with a goal) in dm_learn_gated_net's order: hidden[0],
+    hidden[1], the output layer `head`, gate_common, gate_hidden[0], gate_hidden[1], gate_scale[0], gate_scale[1], gate_bias[0], gate_bias[1]"""
+    return (list(net.hidden) + [head, net.gate_common] + list(net.gate_hidden) + list(net.gate_scale) + list(net.gate_bias))
+
+
+def _gated_shapes(S, G, h0, h1, A, GC, GH):
+    """the [out, in] weight shapes of gated_layers() for state size S, goal size G, hidden (h0, h1), A outputs and gate sizes GC, GH"""
+    return [(h0, S + G), (h1, h0), (A, h1), (GC, G), (GH, GC), (GH, GC), (h0, GH), (h1, GH), (h0, GH), (h1, GH)]
+
+
+class TensorCoreGatedLearner(TensorCoreLearner):
+    """dm_learn_*_gated workspace: PPO minibatch steps of the gated actor (build_gated_policy, kind "actor") or the gated critic (build_critic
+    with a goal, kind "critic") of the AMP task scenes, as TensorCoreLearner does for the plain networks (same contract for the parameters and
+    accumulators; the ten parameter pairs of gated_layers()).  The sizes dm_mlp_create_gated accepts: two hidden layers, goal size <= 64,
+    gate_common <= 128, gate_hidden <= 64, at most 64 outputs."""
+    KINDS = dict(actor=0, critic=1)
+    _NET, _SET = DmLearnGatedNet, "dm_learn_set_gated_weights"
+
+    def __init__(self, net, acc, kind, max_rows, device=0):
+        if kind not in self.KINDS:
+            raise ValueError("kind must be 'actor' or 'critic' (got %r)" % (kind,))
+        G = getattr(net, "goal_size", 0)
+        if not G or not hasattr(net, "gate_common") or len(net.hidden) != 2 or len(net.gate_hidden) != 2:
+            raise ValueError("the gated tensor-core learner implements the gated network with exactly two hidden layers (plain networks: "
+                             "TensorCoreLearner)")
+        self.kind = kind
+        self.layers = gated_layers(net, net.mean if kind == "actor" else net.out)
+        h0, h1, A = (l.weight.shape[0] for l in self.layers[:3])
+        S = self.layers[0].weight.shape[1] - G
+        GC, GH = net.gate_common.weight.shape[0], net.gate_hidden[0].weight.shape[0]
+        for name, v, hi in (("goal size", G, 64), ("gate_common", GC, 128), ("gate_hidden", GH, 64), ("outputs", A, 64)):
+            if v > hi:
+                raise ValueError("the gated tensor-core learner supports %s <= %d (got %d)" % (name, hi, v))
+        for l, shape in zip(self.layers, _gated_shapes(S, G, h0, h1, A, GC, GH)):
+            if tuple(l.weight.shape) != shape or tuple(l.bias.shape) != shape[:1]:
+                raise ValueError("the gated network's layers do not have the shapes of one gated network: %s against %s" % (tuple(l.weight.shape), shape))
+        self.acc, self.device = acc, device
+        L = lib()
+        self.h = L.dm_learn_create_gated(device, self.KINDS[kind], S, G, h0, h1, A, GC, GH, max_rows)
+        if not self.h:
+            raise RuntimeError("dm_learn_create_gated failed: %s" % L.dm_last_error().decode())
+        self.h = C.c_void_p(self.h)
+        self.net = None
+        self._bind()
+
+    def _step_fn(self):
+        return "dm_learn_gated_step"

@@ -14,7 +14,8 @@
 //     dm_mlp handle (dm_mlp_set_weights_device).
 // The AMP discriminator's step (dm_learn_disc_step) reuses the preparation, transposition and backward GEMMs and adds its least-squares head
 // (which also seeds dd/dd = 1 on the expert rows for the gradient penalty), the per-row ||dd/dx||^2 partials, its statistics and a layer pass
-// that adds the penalty's weight gradients and the logit regulariser.
+// that adds the penalty's weight gradients and the logit regulariser.  The gated networks' step (dm_learn_gated_step) adds a preparation that
+// also writes the goal's tile and reuses the rest; its gated backward epilogue is in kernels/dm_mlp.cu (GRAD_XG).
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
@@ -78,6 +79,16 @@ struct LearnLayerParams {
     int t_NC;
 };
 
+// the gated networks' goal (dm_learn_gated_step): [goal samples x goal_dim] fp32 window, normalised and clipped with its own statistics
+struct LearnGoalParams {
+    const float* goal;
+    const float* g_mean;
+    const float* g_istd;
+    float g_clip;
+    int goal_dim;
+    __half* g_tiles;           // [m tiles][kLearnTile]: the normalised goal alone, the gate trunk's operand
+};
+
 // minibatch rows gathered from the window -> normalised, clipped fp16 operand tiles (dm_mlp_prep_kernel with a row index)
 __global__ void __launch_bounds__(kLearnRows) dm_learn_prep_kernel(LearnPrepParams P) {
     const int m0 = blockIdx.x * kLearnRows, c = blockIdx.y;
@@ -92,6 +103,35 @@ __global__ void __launch_bounds__(kLearnRows) dm_learn_prep_kernel(LearnPrepPara
         for (int e = 0; e < 8; ++e) {
             float x = 0.f;
             if (src && k + e < P.in_dim) x = fminf(fmaxf((src[k + e] - P.mean[k + e]) * P.istd[k + e], -P.clip), P.clip);
+            h[e] = __float2half_rn(x);
+        }
+        *reinterpret_cast<uint4*>(tile + ((k8 * (kLearnRows / 8) + (row >> 3)) * 64 + (row & 7) * 8)) = *reinterpret_cast<const uint4*>(h);
+    }
+}
+
+// dm_learn_prep_kernel for the gated networks: the trunk tiles hold [state | goal] and the extra chunk blockIdx.y == NC writes the normalised
+// goal's own tile, as dm_mlp_gated_prep_kernel does.  (A kernel of its own: sharing the body changes dm_learn_prep_kernel's code.)
+// grid = (m tiles, NC + 1)
+__global__ void __launch_bounds__(kLearnRows) dm_learn_gated_prep_kernel(LearnPrepParams P, LearnGoalParams Q) {
+    const int m0 = blockIdx.x * kLearnRows;
+    const bool gate = static_cast<int>(blockIdx.y) == P.NC;
+    const int c = gate ? 0 : blockIdx.y;
+    __half* tile = gate ? Q.g_tiles + static_cast<size_t>(blockIdx.x) * kLearnTile : P.tiles + (static_cast<size_t>(blockIdx.x) * P.NC + c) * kLearnTile;
+#pragma unroll
+    for (int i = 0; i < (kLearnRows * 8) / kLearnRows; ++i) {
+        const int u = threadIdx.x + i * kLearnRows, row = u >> 3, k8 = u & 7;
+        const int grow = m0 + row, k = c * 64 + k8 * 8;
+        const int64_t s = grow < P.M ? P.idx[grow] : -1;
+        __align__(16) __half h[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+            float x = 0.f;
+            if (s >= 0 && !gate && k + e < P.in_dim) {
+                x = fminf(fmaxf((P.x[s * P.in_dim + k + e] - P.mean[k + e]) * P.istd[k + e], -P.clip), P.clip);
+            } else if (s >= 0) {
+                const int j = gate ? k + e : k + e - P.in_dim;
+                if (j < Q.goal_dim) x = fminf(fmaxf((Q.goal[s * Q.goal_dim + j] - Q.g_mean[j]) * Q.g_istd[j], -Q.g_clip), Q.g_clip);
+            }
             h[e] = __float2half_rn(x);
         }
         *reinterpret_cast<uint4*>(tile + ((k8 * (kLearnRows / 8) + (row >> 3)) * 64 + (row & 7) * 8)) = *reinterpret_cast<const uint4*>(h);

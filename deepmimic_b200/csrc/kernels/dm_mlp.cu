@@ -90,7 +90,11 @@ struct MlpStyleParams {
 //           hi + lo (K = minibatch rows); K is split over row-chunk ranges (blockIdx.z) and each split writes its fp32 partial product
 //   GRAD_XA the AMP discriminator's gradient-penalty chain: the GRAD_X pipeline (B = W^T, or a layer's forward tiles for a product W x), the
 //           mask only where mask_tiles is given, and dH written as the next GEMM's A operand only (dy_a), never as a dW operand
-enum { kGradNone = 0, kGradX = 1, kGradW = 2, kGradXA = 3 };
+//   GRAD_XG the dX GEMM into a gated layer's output h (dm_learn_gated_step): p = dh 1[h > 0], then dz = a p written as GRAD_X writes dH, and
+//           ds = b p, dt = p (MlpGateParams) as hi + lo A operands of the gate's dX GEMM and B operands of the gate's dW GEMM
+//   SAVE    not a backward GEMM: the gated forward epilogue of the learner, which also writes the factors a = 2 sigmoid(s) and
+//           b = 2 sigmoid(s) (1 - sigmoid(s)) z (z = acc + bias) of every row and unit, so that the backward uses the forward's own sigmoid
+enum { kGradNone = 0, kGradX = 1, kGradW = 2, kGradXA = 3, kGradXG = 4, kGradSave = 5 };
 struct MlpGradParams {
     const __half* mask_tiles;  // GRAD_X: the layer's input activations, [m tiles][N / 64][kMlpATile] (GRAD_XA: or null, no mask)
     __half* dy_a;              // GRAD_X: dH in operand layout [m tiles][hi: N / 64, lo: N / 64][kMlpATile], or null
@@ -98,6 +102,14 @@ struct MlpGradParams {
     float* partial;            // GRAD_W: [splits][N][M] (the parameter's [out x in] order)
     int row_chunks;            // minibatch rows / 64 (padded)
     int chunks_per_split;      // GRAD_W
+};
+// The gated layers' factors and gate operands (GRAD_XG, SAVE), a parameter struct of their own for the reason MlpStyleParams is
+struct MlpGateParams {
+    float* fa;                 // [M padded][N] fp32: 2 sigmoid(s)
+    float* fb;                 // [M padded][N] fp32: 2 sigmoid(s) (1 - sigmoid(s)) z
+    __half* st_a;              // GRAD_XG: A of the gate's dX GEMM, [m tiles][hi: st_nc, lo: st_nc][kMlpATile]; ds_l in chunks s_chunk + n / 64,
+    int st_nc, s_chunk, t_chunk;   // dt_l in chunks t_chunk + n / 64
+    __half* st_b;              // GRAD_XG: [2 N / 128][row_chunks][hi | lo][128 x 64], ds_l in n tiles [0, N / 128), dt_l in [N / 128, 2 N / 128)
 };
 
 namespace {
@@ -181,8 +193,10 @@ __global__ void __launch_bounds__(kMlpThreads) dm_mlp_gated_prep_kernel(MlpPrepP
 // and bias pre-activations in registers of their own; with BN = 64 that is 3 x 32 accumulator registers per thread.
 // STYLE (the discriminator's one-unit logit head): the last layer's epilogue writes the style reward instead of actions.
 // GRAD (the learner's backward GEMMs, MlpGradParams): kGradX / kGradW epilogues; kGradW also takes its K range from blockIdx.z.
+// Q (MlpGateParams): kGradXG, and kGradSave on a GATED layer.
 template <int BN, bool LAST, bool GATED, bool STYLE = false, int GRAD = kGradNone>
-__device__ __forceinline__ void mlp_gemm(const MlpGemmParams& P, const MlpStyleParams* S = nullptr, const MlpGradParams* G = nullptr) {
+__device__ __forceinline__ void mlp_gemm(const MlpGemmParams& P, const MlpStyleParams* S = nullptr, const MlpGradParams* G = nullptr,
+                                         const MlpGateParams* Q = nullptr) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     constexpr int kABytes = kMlpATile * 2;               // 16 KB
     constexpr int kWBytes = 2 * BN * kMlpBK * 2;         // hi + lo
@@ -194,10 +208,10 @@ __device__ __forceinline__ void mlp_gemm(const MlpGemmParams& P, const MlpStyleP
     uint64_t* bar_empty = bar_full + kMlpStages;                                         // [stages] every thread's MMAs reading the stage have completed
     const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127;
     const int mt = blockIdx.x, m0 = mt * kMlpBM, nt = blockIdx.y, n0 = nt * BN;
-    static_assert(GRAD == kGradNone || (!LAST && !GATED && !STYLE), "the gradient epilogues replace the hidden-layer epilogue");
+    static_assert(GRAD == kGradNone || (!LAST && GATED == (GRAD == kGradSave) && !STYLE), "the gradient epilogues replace the hidden-layer epilogue");
     // kGradW: this split's row chunks [c0, c0 + NC) of the KC chunks every m / n tile holds
     // kGradX: A is dY as hi chunks then lo chunks (2 K / 64 chunks per m tile), each against the same W^T chunk: dY exact to fp32 level
-    constexpr bool kDyHiLo = GRAD == kGradX || GRAD == kGradXA;
+    constexpr bool kDyHiLo = GRAD == kGradX || GRAD == kGradXA || GRAD == kGradXG;
     const int KW = GRAD == kGradW ? G->row_chunks : P.K / kMlpBK;   // K chunks per n tile of B
     const int KC = kDyHiLo ? 2 * KW : KW;                           // K chunks per m tile of A
     const int c0 = GRAD == kGradW ? static_cast<int>(blockIdx.z) * G->chunks_per_split : 0;
@@ -325,6 +339,38 @@ __device__ __forceinline__ void mlp_gemm(const MlpGemmParams& P, const MlpStyleP
                 const __half2 hi = __floats2half2_rn(d0, d1);
                 *reinterpret_cast<__half2*>(t) = hi;
                 *reinterpret_cast<__half2*>(t + static_cast<size_t>(P.N >> 6) * kMlpATile) = __floats2half2_rn(d0 - __low2float(hi), d1 - __high2float(hi));
+            } else if constexpr (GRAD == kGradXG) {
+                const size_t in_tile = (((n & 63) >> 3) * (kMlpBM / 8) + (r >> 3)) * 64 + (r & 7) * 8 + (n & 7);
+                const __half2 hact = *reinterpret_cast<const __half2*>(G->mask_tiles + (static_cast<size_t>(mt) * (P.N >> 6) + (n >> 6)) * kMlpATile + in_tile);
+                const float p0 = __low2float(hact) > 0.f ? v0 : 0.f, p1 = __high2float(hact) > 0.f ? v1 : 0.f;
+                const size_t o = static_cast<size_t>(row) * P.N + n;
+                const float2 fa = *reinterpret_cast<const float2*>(Q->fa + o), fb = *reinterpret_cast<const float2*>(Q->fb + o);
+                const float dz[2] = {fa.x * p0, fa.y * p1}, ds[2] = {fb.x * p0, fb.y * p1}, dt[2] = {p0, p1};
+                // hi at t, lo `lo` halves further
+                auto put_a = [&](__half* t, const float* d, size_t lo) {
+                    const __half2 hi = __floats2half2_rn(d[0], d[1]);
+                    *reinterpret_cast<__half2*>(t) = hi;
+                    *reinterpret_cast<__half2*>(t + lo) = __floats2half2_rn(d[0] - __low2float(hi), d[1] - __high2float(hi));
+                };
+                // element (row, ne) of a dW GEMM's B operand [N' / 128][row_chunks][hi | lo][128 x 64]
+                auto put_b = [&](__half* base, int ne, float d) {
+                    const int k = row & 63;
+                    const __half hi = __float2half_rn(d);
+                    __half* t = base + (static_cast<size_t>(ne >> 7) * G->row_chunks + (row >> 6)) * 2 * 128 * kMlpBK +
+                                (((k >> 3) * 16 + ((ne & 127) >> 3)) * 64 + (ne & 7) * 8 + (k & 7));
+                    t[0] = hi;
+                    t[128 * kMlpBK] = __float2half_rn(d - __half2float(hi));
+                };
+                if (G->dy_a) put_a(G->dy_a + (static_cast<size_t>(mt) * 2 * (P.N >> 6) + (n >> 6)) * kMlpATile + in_tile, dz, static_cast<size_t>(P.N >> 6) * kMlpATile);
+                __half* sa = Q->st_a + (static_cast<size_t>(mt) * 2 * Q->st_nc + (n >> 6)) * kMlpATile + in_tile;
+                put_a(sa + static_cast<size_t>(Q->s_chunk) * kMlpATile, ds, static_cast<size_t>(Q->st_nc) * kMlpATile);
+                put_a(sa + static_cast<size_t>(Q->t_chunk) * kMlpATile, dt, static_cast<size_t>(Q->st_nc) * kMlpATile);
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    put_b(G->dy_b, n + e, dz[e]);
+                    put_b(Q->st_b, n + e, ds[e]);
+                    put_b(Q->st_b, P.N + n + e, dt[e]);
+                }
             } else if constexpr (STYLE) {
                 // the logit is column 0 (the tile's other 63 columns are padding): one thread per row holds it and writes every output of that row
                 if (row < P.M && n == 0) {
@@ -350,11 +396,20 @@ __device__ __forceinline__ void mlp_gemm(const MlpGemmParams& P, const MlpStyleP
                 // next layer's operand tiles: K index = this layer's column; rows past M carry relu(bias) (never read back as results)
                 __half2 hv;
                 if constexpr (GATED) {
-                    auto gated = [&](float v, int i, int ne) {
+                    float fa[2], fb[2];   // kGradSave: the backward's factors
+                    auto gated = [&](float v, int i, int ne, int e) {
                         const float scale = 2.f / (1.f + __expf(-(acc_s[h][i] + P.bias_s[ne])));
-                        return fmaxf(scale * (v + P.bias[ne]) + acc_b[h][i] + P.bias_b[ne], 0.f);
+                        const float z = v + P.bias[ne];
+                        fa[e] = scale;
+                        fb[e] = scale * (1.f - 0.5f * scale) * z;
+                        return fmaxf(scale * z + acc_b[h][i] + P.bias_b[ne], 0.f);
                     };
-                    hv = __floats2half2_rn(gated(v0, i0, n), gated(v1, i0 + 1, n + 1));
+                    hv = __floats2half2_rn(gated(v0, i0, n, 0), gated(v1, i0 + 1, n + 1, 1));
+                    if constexpr (GRAD == kGradSave) {
+                        const size_t o = static_cast<size_t>(row) * P.N + n;
+                        *reinterpret_cast<float2*>(Q->fa + o) = make_float2(fa[0], fa[1]);
+                        *reinterpret_cast<float2*>(Q->fb + o) = make_float2(fb[0], fb[1]);
+                    }
                 } else {
                     hv = __floats2half2_rn(fmaxf(v0 + P.bias[n], 0.f), fmaxf(v1 + P.bias[n + 1], 0.f));
                 }
@@ -381,6 +436,10 @@ template __global__ void dm_mlp_grad_w_kernel<128>(MlpGemmParams, MlpGradParams)
 template __global__ void dm_mlp_grad_w_kernel<64>(MlpGemmParams, MlpGradParams);
 // the AMP discriminator's gradient-penalty products (GRAD_XA, mlp_capi.cu: dm_learn_disc_step), 128-column tiles
 __global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_grad_xa_kernel(MlpGemmParams P, MlpGradParams G) { mlp_gemm<128, false, false, false, kGradXA>(P, nullptr, &G); }
+// the gated PPO learner (mlp_capi.cu: dm_learn_gated_step): a gated trunk layer's forward that saves the backward's factors (64-column tiles,
+// as dm_mlp_gated_gemm_kernel), and the dX GEMM into a gated layer's output (GRAD_XG, 128-column tiles)
+__global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_gated_save_kernel(MlpGemmParams P, MlpGateParams Q) { mlp_gemm<64, false, true, false, kGradSave>(P, nullptr, nullptr, &Q); }
+__global__ void __launch_bounds__(kMlpGemmThreads, 2) dm_mlp_grad_xg_kernel(MlpGemmParams P, MlpGradParams G, MlpGateParams Q) { mlp_gemm<128, false, false, false, kGradXG>(P, nullptr, &G, &Q); }
 
 int dm_mlp_smem_bytes(int bn) { return kMlpStages * (kMlpATile * 2 + 2 * bn * kMlpBK * 2) + 1024; }
 

@@ -2,8 +2,9 @@
 // the plain actor (operand preparation, three GEMMs), six for the gated one (operand preparation, gate trunk, both gate hidden layers, two gated
 // trunk layers, output layer), four for the AMP discriminator's style reward (operand preparation, two GEMMs, the logit head with the reward
 // epilogue); the learner-side TD(lambda) return scan of a rollout window (kernels/dm_returns.cu, one launch); and the PPO learner's minibatch
-// step (dm_learn_*: kernels/dm_learn.cu and the backward GEMMs of kernels/dm_mlp.cu, 15 launches) with the device-side re-tiling of a plain
-// handle (dm_mlp_set_weights_device).  Same library, same rules: no CPU fallback, errors through dm_last_error.
+// step (dm_learn_*: kernels/dm_learn.cu and the backward GEMMs of kernels/dm_mlp.cu, 15 launches; 32 for the gated networks,
+// dm_learn_gated_step) with the device-side re-tiling of plain and gated handles (dm_mlp_set_weights_device, dm_mlp_set_gated_weights_device).
+// Same library, same rules: no CPU fallback, errors through dm_last_error.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
@@ -67,6 +68,12 @@ __global__ void dm_learn_disc_head_kernel(LearnDiscHeadParams);
 __global__ void dm_learn_disc_gp_kernel(const __half*, int, float*);
 __global__ void dm_learn_disc_stats_kernel(const float*, int, const float*, int, float, float*);
 __global__ void dm_learn_disc_layer_kernel(LearnDiscLayerParams);
+// the gated networks' step (kernels/dm_learn.cu, kernels/dm_mlp.cu: MlpGateParams)
+struct MlpGateParams { float* fa; float* fb; __half* st_a; int st_nc, s_chunk, t_chunk; __half* st_b; };
+struct LearnGoalParams { const float* goal; const float* g_mean; const float* g_istd; float g_clip; int goal_dim; __half* g_tiles; };
+__global__ void dm_mlp_gated_save_kernel(MlpGemmParams, MlpGateParams);
+__global__ void dm_mlp_grad_xg_kernel(MlpGemmParams, MlpGradParams, MlpGateParams);
+__global__ void dm_learn_gated_prep_kernel(LearnPrepParams, LearnGoalParams);
 }  // namespace dmk
 
 extern "C" void dm_set_last_error(const char* msg);
@@ -81,7 +88,7 @@ struct dm_mlp {
     // gated actor (dm_mlp_create_gated) only: gate trunk (goal -> 128), both gate hidden layers as one 128 -> 128 GEMM (layer l in columns
     // [64 l, 64 l + 64)), per trunk layer the gate's scale and bias weights (64 -> h_l)
     bool gated = false;
-    int goal_dim = 0;
+    int goal_dim = 0, gate_common = 0, gate_hidden = 0;
     __half *wgc = nullptr, *wgh = nullptr, *wgs[2] = {nullptr, nullptr}, *wgb[2] = {nullptr, nullptr}, *goal_t = nullptr, *gc_t = nullptr, *gh_t = nullptr;
     float *bgc = nullptr, *bgh = nullptr, *bgs[2] = {nullptr, nullptr}, *bgb[2] = {nullptr, nullptr}, *g_mean = nullptr, *g_istd = nullptr;
     float g_clip = 1e30f;
@@ -149,6 +156,26 @@ dmk::LearnLayerParams layer_params(dm_mlp* m, int l, const float* w, const float
 void launch_layer(const dmk::LearnLayerParams& L, cudaStream_t st) {
     dmk::dm_learn_layer_kernel<<<dim3((L.in_dim + 1 + 255) / 256, L.out_dim), 256, 0, st>>>(L);
 }
+// parameter pair i of a gated handle, in dm_learn_gated_net's order W0, W1, W2, Wgc, Wgh_0, Wgh_1, Ws_0, Ws_1, Wt_0, Wt_1: the layer pass's fields
+// for the forward tiles.  Both gate hidden layers share one 128-column matrix, layer l in columns [64 l, 64 l + GH): within a 128-wide tile,
+// column 64 l + j sits 512 halves after column j, so the pass writes Wgh_l through shifted tile and bias pointers
+dmk::LearnLayerParams gated_layer_params(dm_mlp* m, int i, const float* w, const float* b) {
+    dmk::LearnLayerParams L{};
+    L.w = const_cast<float*>(w); L.b = const_cast<float*>(b);
+    const int GC = m->gate_common, GH = m->gate_hidden, l = i & 1;
+    if (i < 3) {
+        const int in[3] = {m->in_dim + m->goal_dim, m->h0, m->h1}, out[3] = {m->h0, m->h1, m->out_dim}, K[3] = {m->K0, m->N0, m->N1};
+        L.in_dim = in[i]; L.out_dim = out[i]; L.tiles = m->w[i]; L.bias_pad = m->b[i]; L.NC = K[i] / 64; L.BN = 64;
+    } else if (i == 3) {
+        L.in_dim = m->goal_dim; L.out_dim = GC; L.tiles = m->wgc; L.bias_pad = m->bgc; L.NC = 1; L.BN = 128;
+    } else if (i < 6) {
+        L.in_dim = GC; L.out_dim = GH; L.tiles = m->wgh + 512 * l; L.bias_pad = m->bgh + 64 * l; L.NC = 2; L.BN = 128;
+    } else {
+        const bool scale = i < 8;
+        L.in_dim = GH; L.out_dim = l ? m->h1 : m->h0; L.tiles = scale ? m->wgs[l] : m->wgb[l]; L.bias_pad = scale ? m->bgs[l] : m->bgb[l]; L.NC = 1; L.BN = 64;
+    }
+    return L;
+}
 }  // namespace
 
 // PPO learner workspace (include/deepmimic_b200.h: dm_learn_*).  Layer l = 0, 1, 2 has F[l] = pad128(inputs + 1) transposed-input features (the
@@ -174,9 +201,83 @@ struct dm_learn {
     __half *pt[3] = {nullptr, nullptr, nullptr};             // e, q0, q1 transposed: A of the penalty's dW GEMMs
     __half* w0p = nullptr;                                   // W0's forward tiles with K padded to Ng: B of the W0 e GEMM
     float *pen[3] = {nullptr, nullptr, nullptr}, *gp_partials = nullptr;
+    // gated networks (dm_learn_create_gated): the trunk uses the fields of layers 0..2 above (dy_a[1] = dz_1); the handle pads the trunk to 128.
+    // The gate's dW GEMMs j = 0..3: [Ws_0 | Wt_0] and [Ws_1 | Wt_1] (A = g_l transposed, B = [ds_l | dt_l]), [Wgh_0 | Wgh_1] (A = gc, B =
+    // [dg_0 | dg_1]), Wgc (A = ng, B = dgc), each with gF[j] = pad128(inputs + 1) features and gN[j] outputs
+    bool gated = false;
+    int gF[4] = {0, 0, 0, 0}, gN[4] = {0, 0, 0, 0}, g_max_splits[4] = {0, 0, 0, 0};
+    __half *gxt[4] = {nullptr, nullptr, nullptr, nullptr}, *gdy_b[4] = {nullptr, nullptr, nullptr, nullptr};
+    float* gpartial[4] = {nullptr, nullptr, nullptr, nullptr};
+    float *fa[2] = {nullptr, nullptr}, *fb[2] = {nullptr, nullptr};   // the gated layers' saved factors 2 sigma(s), 2 sigma(s) (1 - sigma(s)) z
+    int KS = 0;                                              // chunks of [ds_0 | dt_0 | ds_1 | dt_1]: (2 N0 + 2 N1) / 64
+    __half* st_a = nullptr;                                  // [ds_0 | dt_0 | ds_1 | dt_1] as hi + lo A of the dg GEMM
+    __half* wst = nullptr;                                   // its B: Ws_l^T, Wt_l^T block-diagonal (layer l in columns [64 l, 64 l + GH))
+    __half *dg_a = nullptr, *wght = nullptr;                 // [dg_0 | dg_1] as hi + lo A of the dgc GEMM, and its B: [Wgh_0 | Wgh_1]^T
 };
 
 namespace {
+// dm_mlp_create_gated with the trunk's widths padded to trunk_pad (64 for inference; the learner's own handle pads to 128, the width of the
+// backward's tiles; the padding columns are zero and change no row's values).  fn names the caller in error messages
+dm_mlp* create_gated(const char* fn, int device, const dm_mlp_gated_weights* g, int max_rows, int trunk_pad) {
+    const std::string f(fn);
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { mlp_fail(f + ": no CUDA device (the policy network has no CPU fallback)"); return nullptr; }
+    if (!g) { mlp_fail(f + ": null weights"); return nullptr; }
+    if (g->in_dim <= 0 || g->goal_dim <= 0 || g->goal_dim > 64 || g->h0 <= 0 || g->h1 <= 0 || g->out_dim <= 0 || g->out_dim > 64 || max_rows <= 0) {
+        mlp_fail(f + ": bad sizes (goal_dim must be <= 64, out_dim <= 64)"); return nullptr;
+    }
+    if (g->gate_common <= 0 || g->gate_common > 128 || g->gate_hidden <= 0 || g->gate_hidden > 64) {
+        mlp_fail(f + ": unsupported gate sizes (gate_common must be <= 128, gate_hidden <= 64)"); return nullptr;
+    }
+    const float* need[] = {g->w0, g->b0, g->w1, g->b1, g->w2, g->b2, g->gc_w, g->gc_b, g->gh_w[0], g->gh_b[0], g->gh_w[1], g->gh_b[1],
+                           g->gs_w[0], g->gs_b[0], g->gs_w[1], g->gs_b[1], g->gb_w[0], g->gb_b[0], g->gb_w[1], g->gb_b[1]};
+    for (const float* p : need)
+        if (!p) { mlp_fail(f + ": null weight pointer"); return nullptr; }
+    if (cudaSetDevice(device) != cudaSuccess) { mlp_fail(f + ": cudaSetDevice failed"); return nullptr; }
+    cudaDeviceProp prop;
+    cudaGetDeviceProperties(&prop, device);
+    if (prop.major != 9 || prop.minor != 0) { mlp_fail(f + ": the wgmma kernels are built for sm_90a (found sm_" + std::to_string(prop.major) + std::to_string(prop.minor) + ")"); return nullptr; }
+    dm_mlp* m = new dm_mlp();
+    m->gated = true;
+    m->device = device; m->in_dim = g->in_dim; m->goal_dim = g->goal_dim; m->gate_common = g->gate_common; m->gate_hidden = g->gate_hidden; m->h0 = g->h0; m->h1 = g->h1; m->out_dim = g->out_dim; m->max_rows = pad_to(max_rows, 128);
+    const int trunk_in = g->in_dim + g->goal_dim, GC = g->gate_common, GH = g->gate_hidden;
+    m->K0 = pad_to(trunk_in, 64); m->N0 = pad_to(g->h0, trunk_pad); m->N1 = pad_to(g->h1, trunk_pad);   // the gated layers run on 64-column tiles
+    m->in_clip = g->s_clip > 0.f ? g->s_clip : 1e30f;
+    m->g_clip = g->g_clip > 0.f ? g->g_clip : 1e30f;
+    // both gate hidden layers side by side: layer l's GH units in columns [64 l, 64 l + GH), zero columns (relu(0) = 0) up to 64 l + 64
+    std::vector<float> wgh(static_cast<size_t>(GC) * 128, 0.f), bgh(128, 0.f);
+    for (int l = 0; l < 2; ++l) {
+        for (int k = 0; k < GC; ++k)
+            for (int n = 0; n < GH; ++n) wgh[static_cast<size_t>(k) * 128 + 64 * l + n] = g->gh_w[l][static_cast<size_t>(k) * GH + n];
+        for (int n = 0; n < GH; ++n) bgh[64 * l + n] = g->gh_b[l][n];
+    }
+    const size_t R = m->max_rows;
+    bool ok = upload(&m->w[0], tile_weights(g->w0, trunk_in, g->h0, m->K0, m->N0, 64)) && upload(&m->w[1], tile_weights(g->w1, g->h0, g->h1, m->N0, m->N1, 64)) &&
+              upload(&m->w[2], tile_weights(g->w2, g->h1, g->out_dim, m->N1, m->N2, m->N2)) && upload(&m->b[0], padded(g->b0, g->h0, m->N0)) &&
+              upload(&m->b[1], padded(g->b1, g->h1, m->N1)) && upload(&m->b[2], padded(g->b2, g->out_dim, m->N2)) &&
+              upload(&m->wgc, tile_weights(g->gc_w, g->goal_dim, GC, 64, 128, 128)) && upload(&m->bgc, padded(g->gc_b, GC, 128)) &&
+              upload(&m->wgh, tile_weights(wgh.data(), GC, 128, 128, 128, 128)) && upload(&m->bgh, bgh);
+    const int hl[2] = {g->h0, g->h1}, Nl[2] = {m->N0, m->N1};
+    for (int l = 0; l < 2 && ok; ++l)
+        ok = upload(&m->wgs[l], tile_weights(g->gs_w[l], GH, hl[l], 64, Nl[l], 64)) && upload(&m->bgs[l], padded(g->gs_b[l], hl[l], Nl[l])) &&
+             upload(&m->wgb[l], tile_weights(g->gb_w[l], GH, hl[l], 64, Nl[l], 64)) && upload(&m->bgb[l], padded(g->gb_b[l], hl[l], Nl[l]));
+    // gh_t has one tile more than its rows need: the learner transposes layer 1's gate (chunk 1 of every m tile) as a two-chunk source, which
+    // also reads the chunk after it (learn_gated_forward)
+    ok = ok && upload(&m->in_mean, padded(g->s_mean, g->in_dim, g->in_dim)) && upload(&m->in_istd, inverse_std(g->s_std, g->in_dim)) &&
+         upload(&m->g_mean, padded(g->g_mean, g->goal_dim, g->goal_dim)) && upload(&m->g_istd, inverse_std(g->g_std, g->goal_dim)) &&
+         upload(&m->out_mean, padded(g->a_mean, g->out_dim, g->out_dim)) && upload(&m->out_std, padded(g->a_std, g->out_dim, g->out_dim, 1.f)) &&
+         cudaMalloc(&m->obs_t, R * m->K0 * sizeof(__half)) == cudaSuccess && cudaMalloc(&m->goal_t, R * 64 * sizeof(__half)) == cudaSuccess &&
+         cudaMalloc(&m->gc_t, R * 128 * sizeof(__half)) == cudaSuccess && cudaMalloc(&m->gh_t, (R * 128 + dmk::kMlpATileHalves) * sizeof(__half)) == cudaSuccess &&
+         cudaMalloc(&m->act0, R * m->N0 * sizeof(__half)) == cudaSuccess && cudaMalloc(&m->act1, R * m->N1 * sizeof(__half)) == cudaSuccess;
+    if (ok) {
+        ok = cudaFuncSetAttribute(dmk::dm_mlp_gemm_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
+             cudaFuncSetAttribute(dmk::dm_mlp_gated_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess &&
+             cudaFuncSetAttribute(dmk::dm_mlp_gemm_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess;
+    }
+    if (!ok) { mlp_fail(f + ": " + cudaGetErrorString(cudaGetLastError())); dm_mlp_destroy(m); return nullptr; }
+    return m;
+}
+
 // split-K of a dW GEMM: about two CTAs per SM of an H100 (132 SMs) over the (F / 128) x (Nout / BN) output tiles
 void dw_split(int tiles, int chunks, int* splits, int* cps) {
     int s = std::max(1, std::min(chunks, (264 + tiles - 1) / tiles));
@@ -235,60 +336,7 @@ int dm_mlp_forward(dm_mlp* m, const float* d_obs, const float* d_noise, float* d
 }
 
 dm_mlp* dm_mlp_create_gated(int device, const dm_mlp_gated_weights* g, int max_rows) {
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { mlp_fail("dm_mlp_create_gated: no CUDA device (the policy network has no CPU fallback)"); return nullptr; }
-    if (!g) { mlp_fail("dm_mlp_create_gated: null weights"); return nullptr; }
-    if (g->in_dim <= 0 || g->goal_dim <= 0 || g->goal_dim > 64 || g->h0 <= 0 || g->h1 <= 0 || g->out_dim <= 0 || g->out_dim > 64 || max_rows <= 0) {
-        mlp_fail("dm_mlp_create_gated: bad sizes (goal_dim must be <= 64, out_dim <= 64)"); return nullptr;
-    }
-    if (g->gate_common <= 0 || g->gate_common > 128 || g->gate_hidden <= 0 || g->gate_hidden > 64) {
-        mlp_fail("dm_mlp_create_gated: unsupported gate sizes (gate_common must be <= 128, gate_hidden <= 64)"); return nullptr;
-    }
-    const float* need[] = {g->w0, g->b0, g->w1, g->b1, g->w2, g->b2, g->gc_w, g->gc_b, g->gh_w[0], g->gh_b[0], g->gh_w[1], g->gh_b[1],
-                           g->gs_w[0], g->gs_b[0], g->gs_w[1], g->gs_b[1], g->gb_w[0], g->gb_b[0], g->gb_w[1], g->gb_b[1]};
-    for (const float* p : need)
-        if (!p) { mlp_fail("dm_mlp_create_gated: null weight pointer"); return nullptr; }
-    if (cudaSetDevice(device) != cudaSuccess) { mlp_fail("dm_mlp_create_gated: cudaSetDevice failed"); return nullptr; }
-    cudaDeviceProp prop;
-    cudaGetDeviceProperties(&prop, device);
-    if (prop.major != 9 || prop.minor != 0) { mlp_fail("dm_mlp_create_gated: the wgmma kernels are built for sm_90a (found sm_" + std::to_string(prop.major) + std::to_string(prop.minor) + ")"); return nullptr; }
-    dm_mlp* m = new dm_mlp();
-    m->gated = true;
-    m->device = device; m->in_dim = g->in_dim; m->goal_dim = g->goal_dim; m->h0 = g->h0; m->h1 = g->h1; m->out_dim = g->out_dim; m->max_rows = pad_to(max_rows, 128);
-    const int trunk_in = g->in_dim + g->goal_dim, GC = g->gate_common, GH = g->gate_hidden;
-    m->K0 = pad_to(trunk_in, 64); m->N0 = pad_to(g->h0, 64); m->N1 = pad_to(g->h1, 64);   // the gated layers run on 64-column tiles
-    m->in_clip = g->s_clip > 0.f ? g->s_clip : 1e30f;
-    m->g_clip = g->g_clip > 0.f ? g->g_clip : 1e30f;
-    // both gate hidden layers side by side: layer l's GH units in columns [64 l, 64 l + GH), zero columns (relu(0) = 0) up to 64 l + 64
-    std::vector<float> wgh(static_cast<size_t>(GC) * 128, 0.f), bgh(128, 0.f);
-    for (int l = 0; l < 2; ++l) {
-        for (int k = 0; k < GC; ++k)
-            for (int n = 0; n < GH; ++n) wgh[static_cast<size_t>(k) * 128 + 64 * l + n] = g->gh_w[l][static_cast<size_t>(k) * GH + n];
-        for (int n = 0; n < GH; ++n) bgh[64 * l + n] = g->gh_b[l][n];
-    }
-    const size_t R = m->max_rows;
-    bool ok = upload(&m->w[0], tile_weights(g->w0, trunk_in, g->h0, m->K0, m->N0, 64)) && upload(&m->w[1], tile_weights(g->w1, g->h0, g->h1, m->N0, m->N1, 64)) &&
-              upload(&m->w[2], tile_weights(g->w2, g->h1, g->out_dim, m->N1, m->N2, m->N2)) && upload(&m->b[0], padded(g->b0, g->h0, m->N0)) &&
-              upload(&m->b[1], padded(g->b1, g->h1, m->N1)) && upload(&m->b[2], padded(g->b2, g->out_dim, m->N2)) &&
-              upload(&m->wgc, tile_weights(g->gc_w, g->goal_dim, GC, 64, 128, 128)) && upload(&m->bgc, padded(g->gc_b, GC, 128)) &&
-              upload(&m->wgh, tile_weights(wgh.data(), GC, 128, 128, 128, 128)) && upload(&m->bgh, bgh);
-    const int hl[2] = {g->h0, g->h1}, Nl[2] = {m->N0, m->N1};
-    for (int l = 0; l < 2 && ok; ++l)
-        ok = upload(&m->wgs[l], tile_weights(g->gs_w[l], GH, hl[l], 64, Nl[l], 64)) && upload(&m->bgs[l], padded(g->gs_b[l], hl[l], Nl[l])) &&
-             upload(&m->wgb[l], tile_weights(g->gb_w[l], GH, hl[l], 64, Nl[l], 64)) && upload(&m->bgb[l], padded(g->gb_b[l], hl[l], Nl[l]));
-    ok = ok && upload(&m->in_mean, padded(g->s_mean, g->in_dim, g->in_dim)) && upload(&m->in_istd, inverse_std(g->s_std, g->in_dim)) &&
-         upload(&m->g_mean, padded(g->g_mean, g->goal_dim, g->goal_dim)) && upload(&m->g_istd, inverse_std(g->g_std, g->goal_dim)) &&
-         upload(&m->out_mean, padded(g->a_mean, g->out_dim, g->out_dim)) && upload(&m->out_std, padded(g->a_std, g->out_dim, g->out_dim, 1.f)) &&
-         cudaMalloc(&m->obs_t, R * m->K0 * sizeof(__half)) == cudaSuccess && cudaMalloc(&m->goal_t, R * 64 * sizeof(__half)) == cudaSuccess &&
-         cudaMalloc(&m->gc_t, R * 128 * sizeof(__half)) == cudaSuccess && cudaMalloc(&m->gh_t, R * 128 * sizeof(__half)) == cudaSuccess &&
-         cudaMalloc(&m->act0, R * m->N0 * sizeof(__half)) == cudaSuccess && cudaMalloc(&m->act1, R * m->N1 * sizeof(__half)) == cudaSuccess;
-    if (ok) {
-        ok = cudaFuncSetAttribute(dmk::dm_mlp_gemm_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
-             cudaFuncSetAttribute(dmk::dm_mlp_gated_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess &&
-             cudaFuncSetAttribute(dmk::dm_mlp_gemm_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess;
-    }
-    if (!ok) { mlp_fail(std::string("dm_mlp_create_gated: ") + cudaGetErrorString(cudaGetLastError())); dm_mlp_destroy(m); return nullptr; }
-    return m;
+    return create_gated("dm_mlp_create_gated", device, g, max_rows, 64);
 }
 
 int dm_mlp_forward_gated(dm_mlp* m, const float* d_obs, const float* d_goal, const float* d_noise, float* d_actions, int rows, void* stream) {
@@ -535,6 +583,7 @@ void learn_backward(dm_learn* l, int rows, int mt, const int* splits, const int*
 
 int dm_learn_set_weights(dm_learn* l, const dm_learn_net* net, void* stream) {
     if (!l) return mlp_fail("dm_learn_set_weights: null handle");
+    if (l->gated) return mlp_fail("dm_learn_set_weights: the workspace holds a gated network (dm_learn_create_gated); use dm_learn_set_gated_weights");
     if (learn_net_check(net, "dm_learn_set_weights")) return 1;
     if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_set_weights: cudaSetDevice failed");
     if (l->kind == 2) learn_disc_layers(l, net, nullptr, nullptr, nullptr, static_cast<cudaStream_t>(stream));
@@ -546,6 +595,7 @@ int dm_learn_set_weights(dm_learn* l, const dm_learn_net* net, void* stream) {
 
 int dm_learn_step(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, void* stream) {
     if (!l) return mlp_fail("dm_learn_step: null handle");
+    if (l->gated) return mlp_fail("dm_learn_step: the workspace holds a gated network (dm_learn_create_gated); use dm_learn_gated_step");
     if (l->kind == 2) return mlp_fail("dm_learn_step: the workspace is a discriminator's (kind 2); use dm_learn_disc_step");
     if (learn_net_check(net, "dm_learn_step")) return 1;
     if (!b) return mlp_fail("dm_learn_step: null batch");
@@ -586,6 +636,7 @@ int dm_learn_step(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b,
 
 int dm_learn_disc_step(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* b, void* stream) {
     if (!l) return mlp_fail("dm_learn_disc_step: null handle");
+    if (l->gated) return mlp_fail("dm_learn_disc_step: the workspace holds a gated network (dm_learn_create_gated); a discriminator step needs kind 2");
     if (l->kind != 2) return mlp_fail("dm_learn_disc_step: the workspace is a PPO actor's or critic's (kind 0 or 1); a discriminator step needs kind 2");
     if (learn_net_check(net, "dm_learn_disc_step")) return 1;
     if (!b) return mlp_fail("dm_learn_disc_step: null batch");
@@ -657,6 +708,275 @@ int dm_learn_disc_step(dm_learn* l, const dm_learn_net* net, const dm_learn_disc
     return 0;
 }
 
+dm_learn* dm_learn_create_gated(int device, int kind, int in_dim, int goal_dim, int h0, int h1, int out_dim, int gate_common, int gate_hidden, int max_rows) {
+    if (kind != 0 && kind != 1) { mlp_fail("dm_learn_create_gated: kind must be 0 (actor) or 1 (critic)"); return nullptr; }
+    if (kind == 1 && out_dim != 1) { mlp_fail("dm_learn_create_gated: a critic has one output"); return nullptr; }
+    if (in_dim <= 0 || goal_dim <= 0 || goal_dim > 64 || h0 <= 0 || h1 <= 0 || out_dim <= 0 || out_dim > 64 || max_rows <= 0) {
+        mlp_fail("dm_learn_create_gated: bad sizes (goal_dim must be <= 64, out_dim <= 64)"); return nullptr;
+    }
+    if (gate_common <= 0 || gate_common > 128 || gate_hidden <= 0 || gate_hidden > 64) {
+        mlp_fail("dm_learn_create_gated: unsupported gate sizes (gate_common must be <= 128, gate_hidden <= 64)"); return nullptr;
+    }
+    // zero weights and identity normalisers (dm_learn_set_gated_weights loads the parameters, the output stays normalised); the trunk padded to
+    // 128 columns, the width of the backward's tiles
+    const int GC = gate_common, GH = gate_hidden, trunk_in = in_dim + goal_dim;
+    std::vector<float> w0(static_cast<size_t>(trunk_in) * h0), w1(static_cast<size_t>(h0) * h1), w2(static_cast<size_t>(h1) * out_dim), b0(h0), b1(h1), b2(out_dim),
+        gcw(static_cast<size_t>(goal_dim) * GC), gcb(GC), ghw(static_cast<size_t>(GC) * GH), ghb(GH), gw0(static_cast<size_t>(GH) * h0), gw1(static_cast<size_t>(GH) * h1);
+    dm_mlp_gated_weights g{};
+    g.in_dim = in_dim; g.goal_dim = goal_dim; g.h0 = h0; g.h1 = h1; g.out_dim = out_dim; g.gate_common = GC; g.gate_hidden = GH;
+    g.w0 = w0.data(); g.b0 = b0.data(); g.w1 = w1.data(); g.b1 = b1.data(); g.w2 = w2.data(); g.b2 = b2.data(); g.gc_w = gcw.data(); g.gc_b = gcb.data();
+    for (int i = 0; i < 2; ++i) {
+        g.gh_w[i] = ghw.data(); g.gh_b[i] = ghb.data();
+        g.gs_w[i] = g.gb_w[i] = i ? gw1.data() : gw0.data(); g.gs_b[i] = g.gb_b[i] = i ? b1.data() : b0.data();
+    }
+    dm_mlp* m = create_gated("dm_learn_create_gated", device, &g, max_rows, 128);
+    if (!m) return nullptr;   // dm_last_error is set
+    dm_learn* l = new dm_learn();
+    l->m = m; l->gated = true; l->actor = kind == 0; l->kind = kind; l->max_rows = m->max_rows;
+    const int N0 = m->N0, N1 = m->N1, in[3] = {trunk_in, h0, h1}, chunks = m->max_rows / 64;
+    l->Nout[0] = N0; l->Nout[1] = N1; l->Nout[2] = m->N2;
+    const int gF[4] = {128, 128, pad_to(GC + 1, 128), 128}, gN[4] = {2 * N0, 2 * N1, 128, 128};
+    // the largest split count over every minibatch a step may take (dm_learn_create)
+    auto max_splits = [&](int tiles) {
+        int mx = 0;
+        for (int c = 2; c <= chunks; c += 2) {
+            int s = 0, cps = 0;
+            dw_split(tiles, c, &s, &cps);
+            mx = std::max(mx, s);
+        }
+        return mx;
+    };
+    const size_t R = m->max_rows, h = sizeof(__half);
+    l->KS = (2 * N0 + 2 * N1) / 64;
+    bool ok = cudaMalloc(&l->out, R * out_dim * sizeof(float)) == cudaSuccess && cudaMalloc(&l->head_partials, R / 128 * 3 * sizeof(float)) == cudaSuccess;
+    for (int i = 0; i < 3 && ok; ++i) {
+        l->F[i] = pad_to(in[i] + 1, 128);
+        l->max_splits[i] = max_splits((l->F[i] / 128) * (l->Nout[i] / (i == 2 ? m->N2 : 128)));
+        ok = cudaMalloc(&l->xt[i], R * l->F[i] * h) == cudaSuccess && cudaMalloc(&l->dy_b[i], 2 * R * l->Nout[i] * h) == cudaSuccess &&
+             cudaMalloc(&l->partial[i], static_cast<size_t>(l->max_splits[i]) * l->Nout[i] * l->F[i] * sizeof(float)) == cudaSuccess;
+        if (ok && i > 0) {
+            const size_t n = 2 * static_cast<size_t>(l->Nout[i]) * l->Nout[i - 1];
+            ok = cudaMalloc(&l->dy_a[i], 2 * R * l->Nout[i] * h) == cudaSuccess && cudaMalloc(&l->wt[i], n * h) == cudaSuccess && cudaMemset(l->wt[i], 0, n * h) == cudaSuccess;
+        }
+    }
+    for (int j = 0; j < 4 && ok; ++j) {
+        l->gF[j] = gF[j]; l->gN[j] = gN[j]; l->g_max_splits[j] = max_splits((gF[j] / 128) * (gN[j] / 128));
+        ok = cudaMalloc(&l->gxt[j], R * gF[j] * h) == cudaSuccess && cudaMalloc(&l->gdy_b[j], 2 * R * gN[j] * h) == cudaSuccess &&
+             cudaMalloc(&l->gpartial[j], static_cast<size_t>(l->g_max_splits[j]) * gN[j] * gF[j] * sizeof(float)) == cudaSuccess;
+    }
+    for (int i = 0; i < 2 && ok; ++i) {
+        const size_t n = R * (i ? N1 : N0) * sizeof(float);
+        ok = cudaMalloc(&l->fa[i], n) == cudaSuccess && cudaMalloc(&l->fb[i], n) == cudaSuccess;
+    }
+    // the block-diagonal and transposed B operands keep their zero blocks and padding from here on (the layer passes write the weights only)
+    const size_t wst = 2 * static_cast<size_t>(l->KS) * 64 * 128, wght = 2 * 128 * 128;
+    ok = ok && cudaMalloc(&l->st_a, 2 * R * l->KS * 64 * h) == cudaSuccess && cudaMalloc(&l->wst, wst * h) == cudaSuccess && cudaMemset(l->wst, 0, wst * h) == cudaSuccess &&
+         cudaMalloc(&l->dg_a, 2 * R * 128 * h) == cudaSuccess && cudaMalloc(&l->wght, wght * h) == cudaSuccess && cudaMemset(l->wght, 0, wght * h) == cudaSuccess;
+    if (ok) {
+        ok = cudaFuncSetAttribute(dmk::dm_mlp_gated_save_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess &&
+             cudaFuncSetAttribute(dmk::dm_mlp_grad_xg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
+             cudaFuncSetAttribute(dmk::dm_mlp_grad_x_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
+             cudaFuncSetAttribute(dmk::dm_mlp_grad_w_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
+             cudaFuncSetAttribute(dmk::dm_mlp_grad_w_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess;
+    }
+    if (!ok) { mlp_fail(std::string("dm_learn_create_gated: ") + cudaGetErrorString(cudaGetLastError())); dm_learn_destroy(l); return nullptr; }
+    return l;
+}
+
+namespace {
+int gated_net_check(const dm_learn_gated_net* net, const char* fn) {
+    if (!net) return mlp_fail(std::string(fn) + ": null parameters");
+    for (int i = 0; i < 10; ++i)
+        if (!net->w[i] || !net->b[i] || !net->acc_w[i] || !net->acc_b[i]) return mlp_fail(std::string(fn) + ": null parameter or accumulator pointer");
+    return 0;
+}
+// chunk offsets of ds_l and dt_l in [ds_0 | dt_0 | ds_1 | dt_1]
+int s_chunk(const dm_learn* l, int layer) { return layer ? 2 * l->m->N0 / 64 : 0; }
+int t_chunk(const dm_learn* l, int layer) { return s_chunk(l, layer) + (layer ? l->m->N1 : l->m->N0) / 64; }
+// the ten layer passes of a gated workspace: the forward tiles, and the B operands of the dX GEMMs (W1^T, W2^T, the block-diagonal
+// [Ws_l^T, Wt_l^T], [Wgh_0 | Wgh_1]^T); with `b` also the optimiser step on the dW partials (split counts: splits for the trunk, gsplits
+// for the gate's GEMMs)
+void learn_gated_layers(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_batch* b, int rows, const int* splits, const int* gsplits, cudaStream_t st) {
+    dm_mlp* m = l->m;
+    const size_t tt = 2 * 128 * 64;   // halves of a hi + lo 128 x 64 B tile
+    for (int i = 0; i < 10; ++i) {
+        dmk::LearnLayerParams L = gated_layer_params(m, i, net->w[i], net->b[i]);
+        const int lay = i & 1;
+        int s = 0;
+        if (i < 3) {
+            if (i > 0) { L.t_tiles = l->wt[i]; L.t_NC = l->Nout[i] / 64; }
+            L.partial = l->partial[i]; L.Npad = l->Nout[i]; L.F = l->F[i]; s = b ? splits[i] : 0;
+        } else if (i == 3) {
+            L.partial = l->gpartial[3]; L.Npad = 128; L.F = l->gF[3]; s = b ? gsplits[3] : 0;
+        } else if (i < 6) {
+            L.t_tiles = l->wght + lay * tt; L.t_NC = 2;
+            L.partial = l->gpartial[2] + static_cast<size_t>(64 * lay) * l->gF[2]; L.Npad = 128; L.F = l->gF[2]; s = b ? gsplits[2] : 0;
+        } else {
+            const bool scale = i < 8;
+            const int N = lay ? m->N1 : m->N0;
+            L.t_tiles = l->wst + static_cast<size_t>(scale ? s_chunk(l, lay) : t_chunk(l, lay)) * tt + 512 * lay; L.t_NC = l->KS;
+            L.partial = l->gpartial[lay] + (scale ? 0 : static_cast<size_t>(N) * l->gF[lay]); L.Npad = 2 * N; L.F = l->gF[lay]; s = b ? gsplits[lay] : 0;
+        }
+        if (b) {
+            L.acc_w = net->acc_w[i]; L.acc_b = net->acc_b[i]; L.splits = s;
+            L.inv_rows = 1.f / rows; L.lr = b->stepsize; L.mom = b->momentum; L.wd = b->weight_decay;
+        }
+        launch_layer(L, st);
+    }
+}
+// the gated forward over the mt m tiles prepared in obs_t / goal_t (dm_mlp_forward_gated, with the gated layers saving their factors) and the
+// transposition of the saved activations into the dW GEMMs' A operands
+void learn_gated_forward(dm_learn* l, int rows, int mt, cudaStream_t st) {
+    dm_mlp* m = l->m;
+    const size_t tile = dmk::kMlpATileHalves;
+    dmk::MlpGemmParams P{};
+    P.M = rows;
+    P.a_tiles = m->goal_t; P.w_tiles = m->wgc; P.bias = m->bgc; P.out_tiles = m->gc_t; P.K = 64; P.N = 128;
+    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
+    P.a_tiles = m->gc_t; P.w_tiles = m->wgh; P.bias = m->bgh; P.out_tiles = m->gh_t; P.K = 128; P.N = 128;
+    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
+    P.gate_stride = 2 * tile;
+    P.a_tiles = m->obs_t; P.w_tiles = m->w[0]; P.bias = m->b[0]; P.out_tiles = m->act0; P.K = m->K0; P.N = m->N0;
+    P.gate_tiles = m->gh_t; P.ws_tiles = m->wgs[0]; P.wb_tiles = m->wgb[0]; P.bias_s = m->bgs[0]; P.bias_b = m->bgb[0];
+    dmk::dm_mlp_gated_save_kernel<<<dim3(mt, m->N0 / 64), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P, dmk::MlpGateParams{l->fa[0], l->fb[0], nullptr, 0, 0, 0, nullptr});
+    P.a_tiles = m->act0; P.w_tiles = m->w[1]; P.bias = m->b[1]; P.out_tiles = m->act1; P.K = m->N0; P.N = m->N1;
+    P.gate_tiles = m->gh_t + tile; P.ws_tiles = m->wgs[1]; P.wb_tiles = m->wgb[1]; P.bias_s = m->bgs[1]; P.bias_b = m->bgb[1];
+    dmk::dm_mlp_gated_save_kernel<<<dim3(mt, m->N1 / 64), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P, dmk::MlpGateParams{l->fa[1], l->fb[1], nullptr, 0, 0, 0, nullptr});
+    P.a_tiles = m->act1; P.w_tiles = m->w[2]; P.bias = m->b[2]; P.out_tiles = nullptr; P.K = m->N1; P.N = m->N2;
+    P.actions = l->out; P.out_mean = m->out_mean; P.out_std = m->out_std; P.noise = nullptr; P.out_dim = m->out_dim;
+    dmk::dm_mlp_gemm_kernel<64, true><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P);
+    // [ns | ng], h_0, h_1; then ng, gc, g_0 (chunk 0 of gh_t) and g_1 (chunk 1: a two-chunk source whose second chunk is never used, hence
+    // gh_t's spare tile), each with its ones feature
+    const int chunks = 2 * mt;
+    const dmk::LearnTransposeParams T{{m->obs_t, m->act0, m->act1}, {l->xt[0], l->xt[1], l->xt[2]}, {m->K0 / 64, m->N0 / 64, m->N1 / 64},
+                                      {m->in_dim + m->goal_dim, m->h0, m->h1}, {l->F[0], l->F[1], l->F[2]}, chunks};
+    dmk::dm_learn_transpose_kernel<<<dim3(std::max(l->F[0], std::max(l->F[1], l->F[2])) / 128, chunks, 3), 256, 0, st>>>(T);
+    const dmk::LearnTransposeParams G{{m->goal_t, m->gc_t, m->gh_t}, {l->gxt[3], l->gxt[2], l->gxt[0]}, {1, 2, 2}, {m->goal_dim, m->gate_common, m->gate_hidden},
+                                      {l->gF[3], l->gF[2], l->gF[0]}, chunks};
+    dmk::dm_learn_transpose_kernel<<<dim3(l->gF[2] / 128, chunks, 3), 256, 0, st>>>(G);
+    const dmk::LearnTransposeParams G1{{m->gh_t + tile, nullptr, nullptr}, {l->gxt[1], nullptr, nullptr}, {2, 0, 0}, {m->gate_hidden, 0, 0}, {l->gF[1], 0, 0}, chunks};
+    dmk::dm_learn_transpose_kernel<<<dim3(1, chunks, 1), 256, 0, st>>>(G1);
+}
+// the gated backward of the dY a head wrote into dy_a[2] / dy_b[2] (DESIGN.md section 8): dX GEMMs output -> h_1 -> h_0 with the gated
+// epilogue (dz, ds, dt), the gate's dg and dgc GEMMs, and the seven split-K dW GEMMs
+void learn_gated_backward(dm_learn* l, int mt, const int* splits, const int* cps, const int* gsplits, const int* gcps, cudaStream_t st) {
+    dm_mlp* m = l->m;
+    const int chunks = 2 * mt, N0 = m->N0, N1 = m->N1;
+    auto dw = [&](const __half* a, const __half* b, float* part, int F, int N, int BN, int s, int c) {
+        dmk::MlpGemmParams W{};
+        W.a_tiles = a; W.w_tiles = b; W.M = F; W.N = N;
+        const dmk::MlpGradParams GW{nullptr, nullptr, nullptr, part, chunks, c};
+        if (BN == 64) dmk::dm_mlp_grad_w_kernel<64><<<dim3(F / 128, N / 64, s), 256, dmk::dm_mlp_smem_bytes(64), st>>>(W, GW);
+        else dmk::dm_mlp_grad_w_kernel<128><<<dim3(F / 128, N / 128, s), 256, dmk::dm_mlp_smem_bytes(128), st>>>(W, GW);
+    };
+    dw(l->xt[2], l->dy_b[2], l->partial[2], l->F[2], m->N2, m->N2, splits[2], cps[2]);
+    dmk::MlpGemmParams X{};
+    X.a_tiles = l->dy_a[2]; X.w_tiles = l->wt[2]; X.K = m->N2; X.N = N1;
+    dmk::dm_mlp_grad_xg_kernel<<<dim3(mt, N1 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(
+        X, dmk::MlpGradParams{m->act1, l->dy_a[1], l->dy_b[1], nullptr, chunks, 0}, dmk::MlpGateParams{l->fa[1], l->fb[1], l->st_a, l->KS, s_chunk(l, 1), t_chunk(l, 1), l->gdy_b[1]});
+    dw(l->xt[1], l->dy_b[1], l->partial[1], l->F[1], N1, 128, splits[1], cps[1]);
+    dw(l->gxt[1], l->gdy_b[1], l->gpartial[1], l->gF[1], l->gN[1], 128, gsplits[1], gcps[1]);
+    X.a_tiles = l->dy_a[1]; X.w_tiles = l->wt[1]; X.K = N1; X.N = N0;
+    dmk::dm_mlp_grad_xg_kernel<<<dim3(mt, N0 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(
+        X, dmk::MlpGradParams{m->act0, nullptr, l->dy_b[0], nullptr, chunks, 0}, dmk::MlpGateParams{l->fa[0], l->fb[0], l->st_a, l->KS, s_chunk(l, 0), t_chunk(l, 0), l->gdy_b[0]});
+    dw(l->xt[0], l->dy_b[0], l->partial[0], l->F[0], N0, 128, splits[0], cps[0]);
+    dw(l->gxt[0], l->gdy_b[0], l->gpartial[0], l->gF[0], l->gN[0], 128, gsplits[0], gcps[0]);
+    // [dg_0 | dg_1] = ([ds_0 | dt_0 | ds_1 | dt_1] x block-diagonal [Ws_l^T; Wt_l^T]) * 1[g > 0], in gh_t's layout; dgc = ([dg_0 | dg_1] Wgh) * 1[gc > 0]
+    X.a_tiles = l->st_a; X.w_tiles = l->wst; X.K = l->KS * 64; X.N = 128;
+    dmk::dm_mlp_grad_x_kernel<<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(128), st>>>(X, dmk::MlpGradParams{m->gh_t, l->dg_a, l->gdy_b[2], nullptr, chunks, 0});
+    dw(l->gxt[2], l->gdy_b[2], l->gpartial[2], l->gF[2], 128, 128, gsplits[2], gcps[2]);
+    X.a_tiles = l->dg_a; X.w_tiles = l->wght; X.K = 128; X.N = 128;
+    dmk::dm_mlp_grad_x_kernel<<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(128), st>>>(X, dmk::MlpGradParams{m->gc_t, nullptr, l->gdy_b[3], nullptr, chunks, 0});
+    dw(l->gxt[3], l->gdy_b[3], l->gpartial[3], l->gF[3], 128, 128, gsplits[3], gcps[3]);
+}
+}  // namespace
+
+int dm_learn_set_gated_weights(dm_learn* l, const dm_learn_gated_net* net, void* stream) {
+    if (!l) return mlp_fail("dm_learn_set_gated_weights: null handle");
+    if (!l->gated) return mlp_fail("dm_learn_set_gated_weights: the workspace holds a plain network (dm_learn_create); use dm_learn_set_weights");
+    if (gated_net_check(net, "dm_learn_set_gated_weights")) return 1;
+    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_set_gated_weights: cudaSetDevice failed");
+    learn_gated_layers(l, net, nullptr, 0, nullptr, nullptr, static_cast<cudaStream_t>(stream));
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return mlp_fail(std::string("dm_learn_set_gated_weights: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+int dm_learn_gated_step(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_gated_batch* gb, void* stream) {
+    if (!l) return mlp_fail("dm_learn_gated_step: null handle");
+    if (!l->gated) return mlp_fail("dm_learn_gated_step: the workspace holds a plain network (dm_learn_create); use dm_learn_step");
+    if (gated_net_check(net, "dm_learn_gated_step")) return 1;
+    if (!gb) return mlp_fail("dm_learn_gated_step: null batch");
+    const dm_learn_batch* b = &gb->batch;
+    if (b->rows <= 0 || b->rows > l->max_rows) return mlp_fail("dm_learn_gated_step: rows out of range");
+    if (!b->states || !b->idx || !b->in_mean || !b->in_istd || !b->stats || !gb->goals || !gb->g_mean || !gb->g_istd)
+        return mlp_fail("dm_learn_gated_step: null state, goal, index, normaliser or statistics pointer");
+    if (l->actor && (!b->norm_actions || !b->old_logp || !b->adv || !b->logstd || !b->bound_min || !b->bound_max))
+        return mlp_fail("dm_learn_gated_step: null action, log-probability, advantage, log-std or bound pointer");
+    if (!l->actor && !b->norm_targets) return mlp_fail("dm_learn_gated_step: null target pointer");
+    if (l->actor && !(b->ratio_clip > 0.f)) return mlp_fail("dm_learn_gated_step: ratio_clip must be positive");
+    if (!(b->stepsize >= 0.f) || !(b->momentum >= 0.f) || !(b->weight_decay >= 0.f)) return mlp_fail("dm_learn_gated_step: stepsize, momentum and weight_decay must be >= 0");
+    dm_mlp* m = l->m;
+    if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_learn_gated_step: cudaSetDevice failed");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int rows = b->rows, mt = (rows + 127) / 128, chunks = 2 * mt;
+    int splits[3], cps[3], gsplits[4], gcps[4];
+    for (int i = 0; i < 3; ++i) {
+        dw_split((l->F[i] / 128) * (l->Nout[i] / (i == 2 ? m->N2 : 128)), chunks, &splits[i], &cps[i]);
+        if (splits[i] > l->max_splits[i]) return mlp_fail("dm_learn_gated_step: internal error: dW split count exceeds the workspace");
+    }
+    for (int j = 0; j < 4; ++j) {
+        dw_split((l->gF[j] / 128) * (l->gN[j] / 128), chunks, &gsplits[j], &gcps[j]);
+        if (gsplits[j] > l->g_max_splits[j]) return mlp_fail("dm_learn_gated_step: internal error: dW split count exceeds the workspace");
+    }
+    // forward: gathered [state | goal] rows and goals -> the gated network -> the normalised output (identity output normaliser)
+    const dmk::LearnPrepParams Q{b->states, b->idx, b->in_mean, b->in_istd, b->in_clip > 0.f ? b->in_clip : 1e30f, m->in_dim, rows, m->K0 / 64, m->obs_t};
+    const dmk::LearnGoalParams Qg{gb->goals, gb->g_mean, gb->g_istd, gb->g_clip > 0.f ? gb->g_clip : 1e30f, m->goal_dim, m->goal_t};
+    dmk::dm_learn_gated_prep_kernel<<<dim3(mt, m->K0 / 64 + 1), 128, 0, st>>>(Q, Qg);
+    learn_gated_forward(l, rows, mt, st);
+    // the loss heads act on the output only: the plain step's
+    dmk::LearnHeadParams H{l->out, b->idx, rows, m->out_dim, l->dy_a[2], l->dy_b[2], l->head_partials, b->norm_actions, b->old_logp, b->adv, b->logstd,
+                           b->bound_min, b->bound_max, b->ratio_clip, b->ratio, b->norm_targets};
+    if (l->actor) dmk::dm_learn_actor_head_kernel<<<mt, 128, 0, st>>>(H);
+    else dmk::dm_learn_critic_head_kernel<<<mt, 128, 0, st>>>(H);
+    dmk::dm_learn_stats_kernel<<<1, 1, 0, st>>>(l->head_partials, mt, 1.f / rows, l->actor ? 1 : 0, b->stats);
+    learn_gated_backward(l, mt, splits, cps, gsplits, gcps, st);
+    // optimiser step and re-tiling, after every GEMM that read the old weights
+    learn_gated_layers(l, net, b, rows, splits, gsplits, st);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return mlp_fail(std::string("dm_learn_gated_step: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+int dm_mlp_set_gated_weights_device(dm_mlp* m, const float* const* d_w, const float* const* d_b, void* stream) {
+    if (!m) return mlp_fail("dm_mlp_set_gated_weights_device: null handle");
+    if (!m->gated) return mlp_fail("dm_mlp_set_gated_weights_device: the handle holds a plain network (dm_mlp_create); use dm_mlp_set_weights_device");
+    if (!d_w || !d_b) return mlp_fail("dm_mlp_set_gated_weights_device: null weight pointer");
+    for (int i = 0; i < 10; ++i)
+        if (!d_w[i] || !d_b[i]) return mlp_fail("dm_mlp_set_gated_weights_device: null weight pointer");
+    if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_mlp_set_gated_weights_device: cudaSetDevice failed");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    for (int i = 0; i < 10; ++i) launch_layer(gated_layer_params(m, i, d_w[i], d_b[i]), st);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return mlp_fail(std::string("dm_mlp_set_gated_weights_device: ") + cudaGetErrorString(e));
+    return 0;
+}
+
+int dm_mlp_set_gated_normalizers_device(dm_mlp* m, const float* d_s_mean, const float* d_s_std, const float* d_g_mean, const float* d_g_std, const float* d_out_mean,
+                                        const float* d_out_std, void* stream) {
+    if (!m) return mlp_fail("dm_mlp_set_gated_normalizers_device: null handle");
+    if (!m->gated) return mlp_fail("dm_mlp_set_gated_normalizers_device: the handle holds a plain network (dm_mlp_create); use dm_mlp_set_normalizers_device");
+    if (!d_s_mean || !d_s_std || !d_g_mean || !d_g_std || !d_out_mean || !d_out_std) return mlp_fail("dm_mlp_set_gated_normalizers_device: null normaliser pointer");
+    if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_mlp_set_gated_normalizers_device: cudaSetDevice failed");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    dmk::dm_learn_norm_kernel<<<(m->in_dim + 255) / 256, 256, 0, st>>>(d_s_mean, d_s_std, m->in_dim, m->in_mean, m->in_istd, 1);
+    dmk::dm_learn_norm_kernel<<<(m->goal_dim + 255) / 256, 256, 0, st>>>(d_g_mean, d_g_std, m->goal_dim, m->g_mean, m->g_istd, 1);
+    dmk::dm_learn_norm_kernel<<<(m->out_dim + 255) / 256, 256, 0, st>>>(d_out_mean, d_out_std, m->out_dim, m->out_mean, m->out_std, 0);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return mlp_fail(std::string("dm_mlp_set_gated_normalizers_device: ") + cudaGetErrorString(e));
+    return 0;
+}
+
 void dm_learn_destroy(dm_learn* l) {
     if (!l) return;
     if (l->m) {
@@ -667,6 +987,9 @@ void dm_learn_destroy(dm_learn* l) {
     for (int i = 0; i < 3; ++i) { cudaFree(l->xt[i]); cudaFree(l->dy_a[i]); cudaFree(l->dy_b[i]); cudaFree(l->wt[i]); cudaFree(l->partial[i]); cudaFree(l->pt[i]); cudaFree(l->pen[i]); }
     for (int i = 0; i < 2; ++i) { cudaFree(l->u_a[i]); cudaFree(l->u_b[i]); cudaFree(l->q_a[i]); }
     cudaFree(l->seed_a); cudaFree(l->seed_b); cudaFree(l->e_a); cudaFree(l->w0p); cudaFree(l->gp_partials);
+    for (int j = 0; j < 4; ++j) { cudaFree(l->gxt[j]); cudaFree(l->gdy_b[j]); cudaFree(l->gpartial[j]); }
+    for (int i = 0; i < 2; ++i) { cudaFree(l->fa[i]); cudaFree(l->fb[i]); }
+    cudaFree(l->st_a); cudaFree(l->wst); cudaFree(l->dg_a); cudaFree(l->wght);
     delete l;
 }
 

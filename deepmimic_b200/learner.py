@@ -9,8 +9,9 @@ The reference tree is not vendored here; its rules are restated below, one funct
   PPOLearner(rollout, ...).update(traj)   one epoch loop over the window: per minibatch one critic step, then one actor step
     backend "torch"        autograd over the rollout's torch modules (plain or gated networks, CPU or CUDA tensors): the reference the
                            tensor-core backend is tested against
-    backend "tensor_core"  the plain networks' minibatch steps on the library's own sm_90a kernels (dm_learn_step: kernels/dm_learn.cu and the
-                           backward GEMMs of kernels/dm_mlp.cu); the gated networks of the task scenes are refused (their backward is not built)
+    backend "tensor_core"  the minibatch steps on the library's own sm_90a kernels (kernels/dm_learn.cu and the backward GEMMs of
+                           kernels/dm_mlp.cu): dm_learn_step for the plain networks, dm_learn_gated_step for the gated networks of the task
+                           scenes (CUDA only)
   AMPDiscLearner(rollout, ...).update(agent_amp_obs, expert_amp_obs)   `steps` discriminator steps on minibatches drawn from the two pools
     backend "torch"        autograd with a double backward for the gradient penalty (CPU or CUDA tensors)
     backend "tensor_core"  dm_learn_disc_step: the penalty's weight gradients as first-order GEMMs (the ReLU masks are constant), every AMP scene
@@ -18,8 +19,7 @@ The reference tree is not vendored here; its rules are restated below, one funct
 Documented deviations: minibatches are shuffled / drawn by a seeded torch.Generator on the data's device, not the reference's numpy stream; the
 statistics leave out the weight-decay (and logit-regulariser) terms of the losses (the reference's logged losses include them); the normalisers
 are not updated here (DeviceNormalizer.update stays the caller's call, as the reference's normaliser schedule is), nor is a replay buffer of
-agent AMP observations kept.  Not done: the gated tensor-core backward, a multi-GPU gradient all-reduce, TarClipFrac stepsize decay,
-checkpoint writing."""
+agent AMP observations kept.  Not done: a multi-GPU gradient all-reduce, TarClipFrac stepsize decay, checkpoint writing."""
 import math
 
 ADV_EPS = 1e-5   # PPOAgent.ADV_EPS
@@ -159,15 +159,13 @@ class PPOLearner:
         self.gen = torch.Generator(device=dev)
         self.gen.manual_seed(seed)
         if backend == "tensor_core":
-            if rollout.goal_size > 0:
-                raise ValueError("the tensor_core learner implements the plain networks; the gated networks of the goal-conditioned scenes need "
-                                 "backend='torch'")
             if dev.type != "cuda":
-                raise ValueError("the tensor_core learner needs a CUDA device")
-            from .capi import TensorCoreLearner
+                raise ValueError("the tensor_core learner needs a CUDA device; on the CPU, plain and gated networks train with backend='torch'")
+            from .capi import TensorCoreGatedLearner, TensorCoreLearner
             di = dev.index or 0
-            self._tc_actor = TensorCoreLearner(self.policy, self.acc, "actor", minibatch_size, device=di)
-            self._tc_critic = TensorCoreLearner(self.critic, self.acc, "critic", minibatch_size, device=di)
+            cls = TensorCoreGatedLearner if rollout.goal_size > 0 else TensorCoreLearner
+            self._tc_actor = cls(self.policy, self.acc, "actor", minibatch_size, device=di)
+            self._tc_critic = cls(self.critic, self.acc, "critic", minibatch_size, device=di)
 
     # ---- the window: everything a minibatch step reads, computed once per update
     def window(self, traj):
@@ -212,9 +210,10 @@ class PPOLearner:
 
     # ---- one minibatch: a critic step, then an actor step
     def _tc_batch(self, w, ratio=None):
-        """the dm_learn_batch of the actor and of the critic over the window w (and the tensors they point into); ratio: an optional float32
-        CUDA tensor [minibatch_size] that receives the actor's per-row probability ratios of the last step"""
-        from .capi import DmLearnBatch
+        """the dm_learn_batch (gated networks: dm_learn_gated_batch) of the actor and of the critic over the window w (and the tensors they
+        point into); ratio: an optional float32 CUDA tensor [minibatch_size] that receives the actor's per-row probability ratios of the last
+        step"""
+        from .capi import DmLearnBatch, DmLearnGatedBatch
         t, ro = self.torch, self.ro
         keep = dict(istd=(1.0 / ro.s_norm.std).contiguous(), mean=ro.s_norm.mean.contiguous(), old=w["old_logp"].contiguous(),
                     logstd=self.policy.logstd.detach().contiguous(), states=w["states"].contiguous(), norm_a=w["norm_a"].contiguous(),
@@ -229,6 +228,11 @@ class PPOLearner:
                              momentum=self.actor_momentum, weight_decay=self.actor_weight_decay, stats=p(keep["stats_a"]))
         critic = DmLearnBatch(**common, norm_targets=p(keep["tar"]), stepsize=self.critic_stepsize, momentum=self.critic_momentum,
                               weight_decay=self.critic_weight_decay, stats=p(keep["stats_c"]))
+        if ro.goal_size:
+            keep.update(goals=w["goals"].contiguous(), g_mean=ro.g_norm.mean.contiguous(), g_istd=(1.0 / ro.g_norm.std).contiguous())
+            g_clip = 0.0 if math.isinf(ro.g_norm.clip) else float(ro.g_norm.clip)
+            goal = dict(goals=p(keep["goals"]), g_mean=p(keep["g_mean"]), g_istd=p(keep["g_istd"]), g_clip=g_clip)
+            actor, critic = DmLearnGatedBatch(batch=actor, **goal), DmLearnGatedBatch(batch=critic, **goal)
         return keep, actor, critic
 
     def minibatch_step(self, w, critic_idx, actor_idx, stats, tc=None):
@@ -287,16 +291,21 @@ class PPOLearner:
 
     def _refresh_rollout(self):
         """the rollout's tensor-core actor and critic take the new weights and the normalisers' current statistics, the ones this update trained
-        with: re-tiled and copied on the device for plain handles; the gated handles of the goal-conditioned scenes are rebuilt
-        (refresh_tensor_core_policy, a host round trip)"""
+        with: re-tiled and copied on the device, plain and gated handles alike"""
         ro = self.ro
         if ro._tc is None and ro._tc_critic is None:
             return
-        if ro.goal_size > 0:
-            ro.refresh_tensor_core_policy()
-            return
         st = self.torch.cuda.current_stream(self.device).cuda_stream
         c = lambda n: (n.mean.contiguous(), n.std.contiguous())
+        if ro.goal_size > 0:
+            from .capi import gated_layers
+            if ro._tc is not None:
+                ro._tc.set_weights_device(gated_layers(self.policy, self.policy.mean), stream=st)
+                ro._tc.set_normalizers_device(*c(ro.s_norm), *c(ro.g_norm), *c(ro.a_norm), stream=st)
+            if ro._tc_critic is not None:
+                ro._tc_critic.set_weights_device(gated_layers(self.critic, self.critic.out), stream=st)
+                ro._tc_critic.set_normalizers_device(*c(ro.s_norm), *c(ro.g_norm), *c(ro.val_norm), stream=st)
+            return
         if ro._tc is not None:
             ro._tc.set_weights_device(list(self.policy.hidden) + [self.policy.mean], stream=st)
             ro._tc.set_normalizers_device(*c(ro.s_norm), *c(ro.a_norm), stream=st)

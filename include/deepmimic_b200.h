@@ -288,6 +288,37 @@ int dm_learn_step(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* ba
 /* One discriminator step (kind 2), 26 launches on `stream`.  Refused: a NULL handle or pointer, a kind 0 or 1 workspace, rows outside
  * [1, max_rows / 2], a negative (or NaN) stepsize, momentum, weight_decay, logit_reg_weight or grad_penalty_weight. */
 int dm_learn_disc_step(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* batch, void* stream);
+/* PPO minibatch steps of the gated networks of the AMP task scenes (fc_2layers_gated_1024units, dm_mlp_create_gated's network): kind 0 the
+ * actor, kind 1 the critic (out_dim 1).  Same rules, losses and statistics as dm_learn_step; the input is [normalised state | normalised goal]
+ * and the goal alone feeds the gates.  Ten parameter pairs in [units x inputs] layout (dm_learn_net's), in this order: the trunk W0 [h0 x (in_dim +
+ * goal_dim)], W1 [h1 x h0], the output layer W2 [out_dim x h1], the gate trunk Wgc [gate_common x goal_dim], the gate hidden layers Wgh_0,
+ * Wgh_1 [gate_hidden x gate_common], the gate scales Ws_0 [h0 x gate_hidden], Ws_1 [h1 x gate_hidden] and the gate biases Wt_0, Wt_1 (same
+ * shapes as the scales); each bias [units]. */
+typedef struct dm_learn_gated_net {
+    float *w[10], *b[10];
+    float *acc_w[10], *acc_b[10];
+} dm_learn_gated_net;
+/* batch: as for dm_learn_step; goals [samples x goal_dim] (row idx[r] of every minibatch row r), normalised as clip((g - g_mean) * g_istd,
+ * +-g_clip) (g_clip <= 0: none). */
+typedef struct dm_learn_gated_batch {
+    dm_learn_batch batch;
+    const float* goals;
+    const float *g_mean, *g_istd;
+    float g_clip;
+} dm_learn_gated_batch;
+/* Refused: no CUDA device or not sm_90a, a kind other than 0, 1, a critic with out_dim != 1, the sizes dm_mlp_create_gated refuses
+ * (goal_dim <= 64, gate_common <= 128, gate_hidden <= 64, out_dim <= 64), max_rows <= 0. */
+dm_learn* dm_learn_create_gated(int device, int kind, int in_dim, int goal_dim, int h0, int h1, int out_dim, int gate_common, int gate_hidden, int max_rows);
+/* dm_learn_set_weights and dm_learn_step of a gated workspace (32 launches per step); each refuses a plain workspace, and the plain functions
+ * refuse a gated one. */
+int dm_learn_set_gated_weights(dm_learn* l, const dm_learn_gated_net* net, void* stream);
+int dm_learn_gated_step(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_gated_batch* batch, void* stream);
+/* Re-tiles a dm_mlp_create_gated handle from fp32 DEVICE weights d_w[10], d_b[10] in dm_learn_gated_net's order and layout, and refreshes its
+ * state, goal and output normalisers from device statistics ([in_dim], [goal_dim], [out_dim]; the handle keeps 1 / std of the first two), on
+ * `stream`: the values dm_mlp_create_gated stores.  Refused: a NULL handle or pointer, a plain handle. */
+int dm_mlp_set_gated_weights_device(dm_mlp* m, const float* const* d_w, const float* const* d_b, void* stream);
+int dm_mlp_set_gated_normalizers_device(dm_mlp* m, const float* d_s_mean, const float* d_s_std, const float* d_g_mean, const float* d_g_std, const float* d_out_mean,
+                                        const float* d_out_std, void* stream);
 void dm_learn_destroy(dm_learn* l);
 
 /* ---- test hooks: raw per-env simulator state, layout shared with the CPU oracle (doubles):
