@@ -172,6 +172,13 @@ def _dptr(a):
     return a.ctypes.data_as(C.POINTER(C.c_double)) if a is not None else None
 
 
+def _call(fn, *args, stream=None):
+    """calls the C function `fn` with args and then the cudaStream_t handle `stream` (int or None); a nonzero return raises
+    RuntimeError("fn: <dm_last_error>")"""
+    if getattr(lib(), fn)(*args, C.c_void_p(stream) if stream else None) != 0:
+        raise RuntimeError("%s: %s" % (fn, lib().dm_last_error().decode()))
+
+
 def td_lambda_returns(rewards, values, end_values, done, terminate, discount, td_lambda, val_fail, val_succ, returns, advantages, stream=None):
     """dm_td_lambda_returns: TD(lambda) returns and advantages of a [T, N] rollout window on the device.  rewards, values, end_values, returns,
     advantages: contiguous float32 CUDA tensors [T, N]; done: bool (or uint8) [T, N]; terminate: int32 [T, N]; stream: cudaStream_t handle (int)
@@ -182,10 +189,8 @@ def td_lambda_returns(rewards, values, end_values, done, terminate, discount, td
         if tuple(x.shape) != (T, N) or not x.is_contiguous() or not x.is_cuda or str(x.dtype).replace("torch.", "") not in (dt if isinstance(dt, tuple) else (dt,)):
             raise ValueError("td_lambda_returns: %s must be a contiguous %s CUDA tensor [%d, %d]" % (name, dt, T, N))
     ptr = lambda t: C.c_void_p(t.data_ptr())
-    rc = lib().dm_td_lambda_returns(ptr(rewards), ptr(values), ptr(end_values), ptr(done), ptr(terminate), T, N, float(discount), float(td_lambda),
-                                    float(val_fail), float(val_succ), ptr(returns), ptr(advantages), C.c_void_p(stream) if stream else None)
-    if rc != 0:
-        raise RuntimeError("dm_td_lambda_returns: %s" % lib().dm_last_error().decode())
+    _call("dm_td_lambda_returns", ptr(rewards), ptr(values), ptr(end_values), ptr(done), ptr(terminate), T, N, float(discount), float(td_lambda),
+          float(val_fail), float(val_succ), ptr(returns), ptr(advantages), stream=stream)
     return returns, advantages
 
 
@@ -468,7 +473,25 @@ class HostModel:
             pass
 
 
-class TensorCoreMLP:
+class _MlpHandle:
+    """a dm_mlp_* handle self.h (plain or gated): its launch count and its release"""
+
+    def launches(self):
+        return int(lib().dm_mlp_launches(self.h))
+
+    def close(self):
+        if self.h:
+            lib().dm_mlp_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class TensorCoreMLP(_MlpHandle):
     """dm_mlp_* handle: the actor network (normalise -> 2 hidden ReLU layers -> linear -> un-normalise) on the tensor cores (wgmma).
     weights: the reference's dense kernels, [inputs x units] float arrays (deepmimic_b200.tf_checkpoint.load_actor / the fixture files).
     With one output unit and no output normaliser the handle is an AMP discriminator: style_reward() runs it with the reward epilogue."""
@@ -491,10 +514,8 @@ class TensorCoreMLP:
     def forward(self, obs, actions, noise=None, stream=None):
         """obs [rows, in_dim], actions [rows, out_dim] (written), noise [rows, out_dim] or None: contiguous float32 CUDA tensors; stream: cudaStream_t handle (int) or None"""
         rows = obs.shape[0]
-        rc = lib().dm_mlp_forward(self.h, C.c_void_p(obs.data_ptr()), C.c_void_p(noise.data_ptr()) if noise is not None else None, C.c_void_p(actions.data_ptr()), rows,
-                                  C.c_void_p(stream) if stream else None)
-        if rc != 0:
-            raise RuntimeError("dm_mlp_forward: %s" % lib().dm_last_error().decode())
+        _call("dm_mlp_forward", self.h, C.c_void_p(obs.data_ptr()), C.c_void_p(noise.data_ptr()) if noise is not None else None, C.c_void_p(actions.data_ptr()),
+              rows, stream=stream)
         return actions
 
     def set_weights_device(self, layers, stream=None):
@@ -505,47 +526,25 @@ class TensorCoreMLP:
         for t, shape in zip(tensors, shapes):
             _check_device_f32(t, "set_weights_device", shape)
         ptrs = [C.c_void_p(t.data_ptr()) for t in tensors]
-        rc = lib().dm_mlp_set_weights_device(self.h, *ptrs, C.c_void_p(stream) if stream else None)
-        if rc != 0:
-            raise RuntimeError("dm_mlp_set_weights_device: %s" % lib().dm_last_error().decode())
+        _call("dm_mlp_set_weights_device", self.h, *ptrs, stream=stream)
 
     def set_normalizers_device(self, in_mean, in_std, out_mean, out_std, stream=None):
         """dm_mlp_set_normalizers_device: the input and output normalisers from contiguous float32 CUDA tensors ([in_dim], [out_dim]) on the
         device, the values dm_mlp_create would store"""
         for name, t, n in (("in_mean", in_mean, self.in_dim), ("in_std", in_std, self.in_dim), ("out_mean", out_mean, self.out_dim), ("out_std", out_std, self.out_dim)):
             _check_device_f32(t, "set_normalizers_device: " + name, (n,))
-        rc = lib().dm_mlp_set_normalizers_device(self.h, *[C.c_void_p(t.data_ptr()) for t in (in_mean, in_std, out_mean, out_std)],
-                                                 C.c_void_p(stream) if stream else None)
-        if rc != 0:
-            raise RuntimeError("dm_mlp_set_normalizers_device: %s" % lib().dm_last_error().decode())
+        _call("dm_mlp_set_normalizers_device", self.h, *[C.c_void_p(t.data_ptr()) for t in (in_mean, in_std, out_mean, out_std)], stream=stream)
 
     def style_reward(self, amp_obs, reward, task_reward=None, task_lerp=0.0, logit=None, style=None, stream=None):
         """dm_mlp_forward_style_reward: the discriminator's logit d on amp_obs [rows, in_dim], style = max(0, 1 - 0.25 (1 - d)^2) and
         reward [rows] (written) = (1 - task_lerp) style + task_lerp task_reward, or style without task_reward.  logit / style [rows] are
         written when given.  Contiguous float32 CUDA tensors; stream: cudaStream_t handle (int) or None"""
         ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
-        rc = lib().dm_mlp_forward_style_reward(self.h, ptr(amp_obs), ptr(task_reward), float(task_lerp), ptr(logit), ptr(style), ptr(reward), amp_obs.shape[0],
-                                               C.c_void_p(stream) if stream else None)
-        if rc != 0:
-            raise RuntimeError("dm_mlp_forward_style_reward: %s" % lib().dm_last_error().decode())
+        _call("dm_mlp_forward_style_reward", self.h, ptr(amp_obs), ptr(task_reward), float(task_lerp), ptr(logit), ptr(style), ptr(reward), amp_obs.shape[0],
+              stream=stream)
         return reward
 
-    def launches(self):
-        return int(lib().dm_mlp_launches(self.h))
-
-    def close(self):
-        if self.h:
-            lib().dm_mlp_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class TensorCoreGatedMLP:
+class TensorCoreGatedMLP(_MlpHandle):
     """dm_mlp_* handle of the gated (goal-conditioned) actor of the AMP task scenes, fc_2layers_gated_1024units, on the tensor cores (wgmma).
     actor: the reference's layout (deepmimic_b200.tf_checkpoint.load_actor, tests.test_task_scenes_cpu.fixture_task_actor): hidden [(w, b)] x 2,
     mean (w, b), gate_common (w, b), gates [dict(hidden=(w, b), scale=(w, b), bias=(w, b))] x 2; dense kernels are [inputs x units] arrays."""
@@ -581,9 +580,7 @@ class TensorCoreGatedMLP:
         tensors; stream: cudaStream_t handle (int) or None"""
         rows = obs.shape[0]
         ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
-        rc = lib().dm_mlp_forward_gated(self.h, ptr(obs), ptr(goal), ptr(noise), ptr(actions), rows, C.c_void_p(stream) if stream else None)
-        if rc != 0:
-            raise RuntimeError("dm_mlp_forward_gated: %s" % lib().dm_last_error().decode())
+        _call("dm_mlp_forward_gated", self.h, ptr(obs), ptr(goal), ptr(noise), ptr(actions), rows, stream=stream)
         return actions
 
     def set_weights_device(self, layers, stream=None):
@@ -598,8 +595,7 @@ class TensorCoreGatedMLP:
             _check_device_f32(l.bias, "set_weights_device", shape[:1])
         w = (C.c_void_p * 10)(*[l.weight.data_ptr() for l in layers])
         b = (C.c_void_p * 10)(*[l.bias.data_ptr() for l in layers])
-        if lib().dm_mlp_set_gated_weights_device(self.h, w, b, C.c_void_p(stream) if stream else None) != 0:
-            raise RuntimeError("dm_mlp_set_gated_weights_device: %s" % lib().dm_last_error().decode())
+        _call("dm_mlp_set_gated_weights_device", self.h, w, b, stream=stream)
 
     def set_normalizers_device(self, s_mean, s_std, g_mean, g_std, out_mean, out_std, stream=None):
         """dm_mlp_set_gated_normalizers_device: the state, goal and output normalisers from contiguous float32 CUDA tensors ([in_dim],
@@ -608,23 +604,7 @@ class TensorCoreGatedMLP:
               ("out_mean", out_mean, self.out_dim), ("out_std", out_std, self.out_dim))
         for name, t, n in ts:
             _check_device_f32(t, "set_normalizers_device: " + name, (n,))
-        if lib().dm_mlp_set_gated_normalizers_device(self.h, *[C.c_void_p(t.data_ptr()) for _, t, _ in ts], C.c_void_p(stream) if stream else None) != 0:
-            raise RuntimeError("dm_mlp_set_gated_normalizers_device: %s" % lib().dm_last_error().decode())
-
-    def launches(self):
-        return int(lib().dm_mlp_launches(self.h))
-
-    def close(self):
-        if self.h:
-            lib().dm_mlp_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
+        _call("dm_mlp_set_gated_normalizers_device", self.h, *[C.c_void_p(t.data_ptr()) for _, t, _ in ts], stream=stream)
 
 class TensorCoreLearner:
     """dm_learn_* workspace: minibatch steps of a plain 2-layer torch network on the tensor cores: PPO steps of build_policy (kind "actor") and
@@ -670,17 +650,14 @@ class TensorCoreLearner:
     def set_weights(self, stream=None):
         """binds the parameters' current storage (checked) and loads their values into the workspace's tiles"""
         self._bind()
-        if getattr(lib(), self._SET)(self.h, C.byref(self.net), C.c_void_p(stream) if stream else None) != 0:
-            raise RuntimeError("%s: %s" % (self._SET, lib().dm_last_error().decode()))
+        _call(self._SET, self.h, C.byref(self.net), stream=stream)
 
     def _step_fn(self):
         return "dm_learn_disc_step" if self.kind == "disc" else "dm_learn_step"
 
     def step(self, batch, stream=None):
         """batch: a DmLearnBatch (kinds "actor", "critic"), a DmLearnDiscBatch (kind "disc") or a DmLearnGatedBatch (TensorCoreGatedLearner)"""
-        fn = self._step_fn()
-        if getattr(lib(), fn)(self.h, C.byref(self.net), C.byref(batch), C.c_void_p(stream) if stream else None) != 0:
-            raise RuntimeError("%s: %s" % (fn, lib().dm_last_error().decode()))
+        _call(self._step_fn(), self.h, C.byref(self.net), C.byref(batch), stream=stream)
 
     def close(self):
         if self.h:

@@ -21,78 +21,16 @@
 
 #include <cstdint>
 
+#include "dm_mlp.cuh"
+
 namespace dmk {
 
 constexpr int kLearnRows = 128;        // rows per CTA of the preparation, transposition and head kernels (one m tile)
-constexpr int kLearnTile = 128 * 64;   // halves per operand tile (kernels/dm_mlp.cu: kMlpATile)
-
-struct LearnPrepParams {
-    const float* x;            // [samples x in_dim] fp32 window
-    const int64_t* idx;        // [M] window sample of each minibatch row
-    const float* mean;
-    const float* istd;
-    float clip;
-    int in_dim, M, NC;         // NC = padded K / 64
-    __half* tiles;             // [m tiles][NC][kLearnTile]
-};
-struct LearnTransposeParams {
-    const __half* src[3];      // forward activations in operand layout [m tiles][src_nc][kLearnTile]
-    __half* dst[3];            // transposed: [F / 128][row_chunks][kLearnTile], M = feature, K = minibatch row
-    int src_nc[3];
-    int ones[3];               // the feature that is 1 on every row (the layer's input size): its dW row is the bias gradient
-    int F[3];                  // padded features (multiple of 128)
-    int row_chunks;
-};
-struct LearnHeadParams {
-    const float* out;          // [M x out_dim] the network's normalised output (mu, or the normalised value)
-    const int64_t* idx;        // [M] window sample of each row
-    int M, out_dim;
-    __half* dy_a;              // [m tiles][hi | lo][kLearnTile]: A of the output layer's dX GEMM
-    __half* dy_b;              // [1][row chunks][hi | lo][64 x 64]: B of the output layer's dW GEMM
-    float* partials;           // [CTAs][3]
-    // actor (PPOAgent._build_losses): normalised actions, old log-probabilities and advantages of the window, log sigma and the normalised
-    // action bounds per action, the ratio clip; ratio: [M] per-row probability ratios, or null
-    const float* actions;
-    const float* old_logp;
-    const float* adv;
-    const float* logstd;
-    const float* bound_min;
-    const float* bound_max;
-    float ratio_clip;
-    float* ratio;
-    // critic: the window's normalised, clipped targets
-    const float* targets;
-};
-struct LearnLayerParams {
-    float* w;                  // [out x in] fp32 (torch layout), updated in place
-    float* b;                  // [out]
-    float* acc_w;              // momentum accumulators, or null: re-tile only
-    float* acc_b;
-    const float* partial;      // [splits][Npad][F] dW partials; row in_dim holds db
-    int splits, Npad, F;
-    float inv_rows, lr, mom, wd;
-    int in_dim, out_dim;
-    __half* tiles;             // forward hi + lo tiles [Npad / BN][NC][2][BN x 64] (dm_mlp w[l])
-    float* bias_pad;           // dm_mlp b[l]
-    int NC, BN;
-    __half* t_tiles;           // W^T hi + lo tiles of the dX GEMM [in tiles of 128][t_NC][2][128 x 64], or null
-    int t_NC;
-};
-
-// the gated networks' goal (dm_learn_gated_step): [goal samples x goal_dim] fp32 window, normalised and clipped with its own statistics
-struct LearnGoalParams {
-    const float* goal;
-    const float* g_mean;
-    const float* g_istd;
-    float g_clip;
-    int goal_dim;
-    __half* g_tiles;           // [m tiles][kLearnTile]: the normalised goal alone, the gate trunk's operand
-};
 
 // minibatch rows gathered from the window -> normalised, clipped fp16 operand tiles (dm_mlp_prep_kernel with a row index)
 __global__ void __launch_bounds__(kLearnRows) dm_learn_prep_kernel(LearnPrepParams P) {
     const int m0 = blockIdx.x * kLearnRows, c = blockIdx.y;
-    __half* tile = P.tiles + (static_cast<size_t>(blockIdx.x) * P.NC + c) * kLearnTile;
+    __half* tile = P.tiles + (static_cast<size_t>(blockIdx.x) * P.NC + c) * kMlpATile;
 #pragma unroll
     for (int i = 0; i < (kLearnRows * 8) / kLearnRows; ++i) {
         const int u = threadIdx.x + i * kLearnRows, row = u >> 3, k8 = u & 7;
@@ -116,7 +54,7 @@ __global__ void __launch_bounds__(kLearnRows) dm_learn_gated_prep_kernel(LearnPr
     const int m0 = blockIdx.x * kLearnRows;
     const bool gate = static_cast<int>(blockIdx.y) == P.NC;
     const int c = gate ? 0 : blockIdx.y;
-    __half* tile = gate ? Q.g_tiles + static_cast<size_t>(blockIdx.x) * kLearnTile : P.tiles + (static_cast<size_t>(blockIdx.x) * P.NC + c) * kLearnTile;
+    __half* tile = gate ? Q.g_tiles + static_cast<size_t>(blockIdx.x) * kMlpATile : P.tiles + (static_cast<size_t>(blockIdx.x) * P.NC + c) * kMlpATile;
 #pragma unroll
     for (int i = 0; i < (kLearnRows * 8) / kLearnRows; ++i) {
         const int u = threadIdx.x + i * kLearnRows, row = u >> 3, k8 = u & 7;
@@ -147,7 +85,7 @@ __global__ void __launch_bounds__(256) dm_learn_transpose_kernel(LearnTransposeP
     const int F = pick(P.F[0], P.F[1], P.F[2]), ones = pick(P.ones[0], P.ones[1], P.ones[2]), src_nc = pick(P.src_nc[0], P.src_nc[1], P.src_nc[2]);
     const __half* src = pick(P.src[0], P.src[1], P.src[2]);
     if (static_cast<int>(blockIdx.x) * 128 >= F) return;
-    __half* dst = pick(P.dst[0], P.dst[1], P.dst[2]) + (static_cast<size_t>(blockIdx.x) * P.row_chunks + blockIdx.y) * kLearnTile;
+    __half* dst = pick(P.dst[0], P.dst[1], P.dst[2]) + (static_cast<size_t>(blockIdx.x) * P.row_chunks + blockIdx.y) * kMlpATile;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
         const int u = threadIdx.x + i * 256, k8 = u >> 7, fl = u & 127;
@@ -157,7 +95,7 @@ __global__ void __launch_bounds__(256) dm_learn_transpose_kernel(LearnTransposeP
 #pragma unroll
             for (int e = 0; e < 8; ++e) h[e] = __float2half_rn(1.f);
         } else if (f < src_nc * 64) {
-            const __half* s = src + (static_cast<size_t>(b0 >> 7) * src_nc + (f >> 6)) * kLearnTile + ((((f & 63) >> 3) * 16 + ((b0 & 127) >> 3)) * 64 + (f & 7));
+            const __half* s = src + (static_cast<size_t>(b0 >> 7) * src_nc + (f >> 6)) * kMlpATile + ((((f & 63) >> 3) * 16 + ((b0 & 127) >> 3)) * 64 + (f & 7));
 #pragma unroll
             for (int e = 0; e < 8; ++e) h[e] = s[e * 8];
         } else {
@@ -173,7 +111,7 @@ template <bool ACTOR>
 __device__ __forceinline__ void learn_head(const LearnHeadParams& P) {
     __shared__ float red[3][kLearnRows];
     const int tid = threadIdx.x, row = blockIdx.x * kLearnRows + tid;
-    __half* dya = P.dy_a + static_cast<size_t>(blockIdx.x) * 2 * kLearnTile;
+    __half* dya = P.dy_a + static_cast<size_t>(blockIdx.x) * 2 * kMlpATile;
     __half* dyb = P.dy_b + static_cast<size_t>(row >> 6) * 2 * 64 * 64;
     const int k = row & 63;
     float part[3] = {0.f, 0.f, 0.f};
@@ -219,7 +157,7 @@ __device__ __forceinline__ void learn_head(const LearnHeadParams& P) {
         const __half hi = __float2half_rn(g), lo = __float2half_rn(g - __half2float(hi));
         const int oa = ((j >> 3) * 16 + (tid >> 3)) * 64 + (tid & 7) * 8 + (j & 7);
         dya[oa] = hi;
-        dya[oa + kLearnTile] = lo;
+        dya[oa + kMlpATile] = lo;
         const int o = ((k >> 3) * 8 + (j >> 3)) * 64 + (j & 7) * 8 + (k & 7);
         dyb[o] = hi;
         dyb[o + 64 * 64] = lo;
@@ -300,15 +238,6 @@ __global__ void __launch_bounds__(256) dm_learn_norm_kernel(const float* mean, c
 // ---- the AMP discriminator's minibatch step (R/learning/amp_agent.py: AMPAgent._build_losses, _disc_grad_penalty_loss; mlp_capi.cu:
 // dm_learn_disc_step).  A step of `rows` agent and `rows` expert rows puts the agent rows at [0, rows) and the expert rows at [E, E + rows),
 // E = pad128(rows), so every m tile holds one side only and the penalty's GEMMs address the expert tiles from tile E / 128 on.
-struct LearnDiscHeadParams {
-    const float* out;          // [2E] logits
-    int rows, E;
-    __half* dy_a;              // dY of the logit layer over all 2E rows, as LearnHeadParams::dy_a / dy_b
-    __half* dy_b;
-    __half* seed_a;            // dd / dd = 1 on the real expert rows (0 on their padding), over the E expert rows: A of the penalty's first dX
-    __half* seed_b;            // GEMM, and B of its logit-weight dW GEMM
-    float* partials;           // [2E / 128][3]: sum of (d -+ 1)^2, rows on the right side of 0, sum of d
-};
 
 // one thread per row, grid = 2E / 128.  Least-squares loss (Peng et al. 2021, eq. 8): 0.5 (0.5 mean (d_e - 1)^2 + 0.5 mean (d_a + 1)^2), so the
 // gradient of the SUM over rows is 0.5 (d - 1) on an expert row and 0.5 (d + 1) on an agent row (1 / rows is applied by the optimiser)
@@ -326,9 +255,9 @@ __global__ void __launch_bounds__(kLearnRows) dm_learn_disc_head_kernel(LearnDis
         part[1] = (expert ? d > 0.f : d < 0.f) ? 1.f : 0.f;
         part[2] = d;
     }
-    __half* dya = P.dy_a + static_cast<size_t>(blockIdx.x) * 2 * kLearnTile;
+    __half* dya = P.dy_a + static_cast<size_t>(blockIdx.x) * 2 * kMlpATile;
     __half* dyb = P.dy_b + static_cast<size_t>(row >> 6) * 2 * 64 * 64;
-    __half* sa = expert ? P.seed_a + static_cast<size_t>(blockIdx.x - P.E / kLearnRows) * 2 * kLearnTile : nullptr;
+    __half* sa = expert ? P.seed_a + static_cast<size_t>(blockIdx.x - P.E / kLearnRows) * 2 * kMlpATile : nullptr;
     __half* sb = expert ? P.seed_b + static_cast<size_t>(r >> 6) * 2 * 64 * 64 : nullptr;
     const int k = row & 63;
     const __half zero = __float2half_rn(0.f);
@@ -338,12 +267,12 @@ __global__ void __launch_bounds__(kLearnRows) dm_learn_disc_head_kernel(LearnDis
         const int oa = ((j >> 3) * 16 + (tid >> 3)) * 64 + (tid & 7) * 8 + (j & 7);
         const int o = ((k >> 3) * 8 + (j >> 3)) * 64 + (j & 7) * 8 + (k & 7);
         dya[oa] = hi;
-        dya[oa + kLearnTile] = lo;
+        dya[oa + kMlpATile] = lo;
         dyb[o] = hi;
         dyb[o + 64 * 64] = lo;
         if (expert) {
             sa[oa] = sb[o] = __float2half_rn(j == 0 && real ? 1.f : 0.f);
-            sa[oa + kLearnTile] = sb[o + 64 * 64] = zero;
+            sa[oa + kMlpATile] = sb[o + 64 * 64] = zero;
         }
     }
 #pragma unroll
@@ -358,19 +287,19 @@ __global__ void __launch_bounds__(kLearnRows) dm_learn_disc_head_kernel(LearnDis
     if (tid < 3) P.partials[blockIdx.x * 3 + tid] = red[tid][0];
 }
 
-// ||g||^2 of every expert row, g = dd / dx the input gradient held as hi + lo operand tiles [E / 128][hi: NC, lo: NC][kLearnTile]; one thread
+// ||g||^2 of every expert row, g = dd / dx the input gradient held as hi + lo operand tiles [E / 128][hi: NC, lo: NC][kMlpATile]; one thread
 // per row (a thread reads 16-byte core-matrix rows: 8 consecutive inputs of its row), the CTA's sum in a fixed tree.  grid = E / 128
 __global__ void __launch_bounds__(kLearnRows) dm_learn_disc_gp_kernel(const __half* g, int NC, float* partials) {
     __shared__ float red[kLearnRows];
     const int tid = threadIdx.x;
-    const __half* base = g + static_cast<size_t>(blockIdx.x) * 2 * NC * kLearnTile;
+    const __half* base = g + static_cast<size_t>(blockIdx.x) * 2 * NC * kMlpATile;
     float s = 0.f;
     for (int c = 0; c < NC; ++c)
         for (int k8 = 0; k8 < 8; ++k8) {
-            const size_t o = static_cast<size_t>(c) * kLearnTile + (k8 * 16 + (tid >> 3)) * 64 + (tid & 7) * 8;
+            const size_t o = static_cast<size_t>(c) * kMlpATile + (k8 * 16 + (tid >> 3)) * 64 + (tid & 7) * 8;
             __align__(16) __half hi[8], lo[8];
             *reinterpret_cast<uint4*>(hi) = *reinterpret_cast<const uint4*>(base + o);
-            *reinterpret_cast<uint4*>(lo) = *reinterpret_cast<const uint4*>(base + o + static_cast<size_t>(NC) * kLearnTile);
+            *reinterpret_cast<uint4*>(lo) = *reinterpret_cast<const uint4*>(base + o + static_cast<size_t>(NC) * kMlpATile);
 #pragma unroll
             for (int e = 0; e < 8; ++e) {
                 const float v = __half2float(hi[e]) + __half2float(lo[e]);
@@ -401,16 +330,6 @@ __global__ void dm_learn_disc_stats_kernel(const float* head, int ctas, const fl
     stats[4] += e[2] * inv_rows;
     stats[5] += a[2] * inv_rows;
 }
-
-struct LearnDiscLayerParams {
-    LearnLayerParams L;        // as dm_learn_layer_kernel; t_tiles for every layer (layer 0's W0^T feeds the penalty's input-gradient GEMM)
-    const float* pen;          // [pen_splits][L.Npad][pen_F] dW partials of 0.5 sum ||g||^2 (no bias term), or null: no penalty
-    int pen_splits, pen_F;
-    float gp_w;                // the penalty's weight
-    float reg;                 // weight decay on top of L.wd for this layer's weights (the logit layer: logit_reg_weight)
-    __half* p_tiles;           // layer 0, or null: W0's forward tiles with K padded to p_NC * 64 (B of the penalty's W0 e GEMM)
-    int p_NC;
-};
 
 // dm_learn_layer_kernel with the penalty's partials and the logit regulariser: g = (sum dW + gp_w sum dW_pen) / rows + (wd + reg) w on the
 // weights, (sum db) / rows on the biases; then the momentum step and the re-tiling

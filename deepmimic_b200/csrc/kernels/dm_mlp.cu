@@ -24,64 +24,15 @@
 
 #include <cstdint>
 
+#include "dm_mlp.cuh"
+
 namespace dmk {
 
-constexpr int kMlpBM = 128;          // environments per CTA
-constexpr int kMlpBK = 64;           // K elements per chunk (8 core matrices of 8 fp16)
 constexpr int kMlpThreads = 128;     // operand-preparation kernel
 constexpr int kMlpGemmThreads = 256; // GEMM kernel: two warpgroups, warpgroup g owns rows [64 g, 64 g + 64) of the CTA tile
 constexpr int kMlpStages = 2;
-constexpr int kMlpATile = kMlpBM * kMlpBK;   // halves per activation tile (16 KB): [k8][row group][row in group][8 halves]
 
-struct MlpPrepParams {
-    const float* obs;          // [M x in_dim] fp32 observations
-    const float* in_mean;      // normaliser mean / 1/std, in_dim entries
-    const float* in_istd;
-    float in_clip;
-    int in_dim, M, NC;         // NC = padded K / 64
-    __half* tiles;             // [m tiles][NC][kMlpATile]
-    // gated actor only: the goal, normalised with its own statistics, fills the trunk columns [in_dim, in_dim + goal_dim) and, alone, the
-    // gate trunk's 64-wide operand tile (written by the extra chunk blockIdx.y == NC)
-    const float* goal;         // [M x goal_dim] fp32
-    const float* g_mean;
-    const float* g_istd;
-    float g_clip;
-    int goal_dim;
-    __half* g_tiles;           // [m tiles][kMlpATile]
-};
-struct MlpGemmParams {
-    const __half* a_tiles;     // [m tiles][K / 64][kMlpATile] fp16 activations in operand layout
-    const __half* w_tiles;     // [n tiles][K / 64][hi | lo][BN x 64] in operand layout
-    const float* bias;         // [N padded]
-    __half* out_tiles;         // !LAST: [m tiles][N / 64][kMlpATile]
-    float* actions;            // LAST: [M x out_dim] fp32
-    const float* out_mean;     // LAST: action un-normalisation a * std + mean
-    const float* out_std;
-    const float* noise;        // LAST, optional: [M x out_dim] added in normalised action space (exploration), may be null
-    int out_dim;
-    int M, K, N;               // rows, padded K (multiple of 64), padded N (multiple of BN)
-    // gated trunk layer only: two more K-chunks after the trunk's, both with this layer's gate-hidden chunk as A, against the gate's scale and
-    // bias weights; the epilogue is relu(2 sigmoid(acc_s + bias_s) (acc + bias) + acc_b + bias_b)
-    const __half* gate_tiles;  // A of the gate chunks: m tile t at gate_tiles + t * gate_stride
-    const __half* ws_tiles;    // [n tiles][1][hi | lo][BN x 64]
-    const __half* wb_tiles;
-    const float* bias_s;       // [N padded]
-    const float* bias_b;
-    int gate_stride;           // halves
-};
-// The discriminator head's outputs, a kernel parameter of its own: MlpGemmParams stays at 128 bytes (nvcc 12.9 compiles every GEMM
-// instantiation differently once that struct grows past 128 bytes, even with the new fields unused).  Column 0 of the head is the logit
-// d = acc + bias (no un-normalisation); per row r < M, style = max(0, 1 - 0.25 (1 - d)^2) and
-// reward = (1 - task_lerp) style + task_lerp task_reward[r], or style without a task reward.
-struct MlpStyleParams {
-    const float* task_reward;  // [M] or null
-    float* logit;              // [M] or null
-    float* style;              // [M] or null
-    float* reward;             // [M]
-    float task_lerp;
-};
-// The backward GEMMs of the PPO learner (kernels/dm_learn.cu, mlp_capi.cu: dm_learn_step), also a parameter struct of their own.  Same pipeline,
-// other operands and epilogues:
+// The modes of the backward GEMMs of the PPO learner (MlpGradParams): same pipeline, other operands and epilogues:
 //   GRAD_X  dH = (dY W^T) * 1[H > 0]: A = dY in operand layout as hi + lo chunks (K = twice this layer's padded outputs), B = W^T as hi + lo
 //           tiles (N = its padded inputs), so both operands are exact to fp32 level (a minibatch's gradient is a sum of per-row terms that
 //           largely cancel, which magnifies fp16 rounding of dY); the epilogue masks with the saved forward activation tile and writes dH as the
@@ -95,22 +46,6 @@ struct MlpStyleParams {
 //   SAVE    not a backward GEMM: the gated forward epilogue of the learner, which also writes the factors a = 2 sigmoid(s) and
 //           b = 2 sigmoid(s) (1 - sigmoid(s)) z (z = acc + bias) of every row and unit, so that the backward uses the forward's own sigmoid
 enum { kGradNone = 0, kGradX = 1, kGradW = 2, kGradXA = 3, kGradXG = 4, kGradSave = 5 };
-struct MlpGradParams {
-    const __half* mask_tiles;  // GRAD_X: the layer's input activations, [m tiles][N / 64][kMlpATile] (GRAD_XA: or null, no mask)
-    __half* dy_a;              // GRAD_X: dH in operand layout [m tiles][hi: N / 64, lo: N / 64][kMlpATile], or null
-    __half* dy_b;              // GRAD_X: dH as B of the dW GEMM, [N / 128][row_chunks][hi | lo][128 x 64]
-    float* partial;            // GRAD_W: [splits][N][M] (the parameter's [out x in] order)
-    int row_chunks;            // minibatch rows / 64 (padded)
-    int chunks_per_split;      // GRAD_W
-};
-// The gated layers' factors and gate operands (GRAD_XG, SAVE), a parameter struct of their own for the reason MlpStyleParams is
-struct MlpGateParams {
-    float* fa;                 // [M padded][N] fp32: 2 sigmoid(s)
-    float* fb;                 // [M padded][N] fp32: 2 sigmoid(s) (1 - sigmoid(s)) z
-    __half* st_a;              // GRAD_XG: A of the gate's dX GEMM, [m tiles][hi: st_nc, lo: st_nc][kMlpATile]; ds_l in chunks s_chunk + n / 64,
-    int st_nc, s_chunk, t_chunk;   // dt_l in chunks t_chunk + n / 64
-    __half* st_b;              // GRAD_XG: [2 N / 128][row_chunks][hi | lo][128 x 64], ds_l in n tiles [0, N / 128), dt_l in [N / 128, 2 N / 128)
-};
 
 namespace {
 

@@ -12,6 +12,8 @@
 
 #include <cstdint>
 
+#include "dm_mlp.cuh"
+
 namespace dmk {
 
 constexpr int kReturnSteps = 16;   // steps whose loads are in flight at once per thread

@@ -4,6 +4,7 @@
 // epilogue); the learner-side TD(lambda) return scan of a rollout window (kernels/dm_returns.cu, one launch); and the PPO learner's minibatch
 // step (dm_learn_*: kernels/dm_learn.cu and the backward GEMMs of kernels/dm_mlp.cu, 15 launches; 32 for the gated networks,
 // dm_learn_gated_step) with the device-side re-tiling of plain and gated handles (dm_mlp_set_weights_device, dm_mlp_set_gated_weights_device).
+// The parameter structs and kernel declarations are kernels/dm_mlp.cuh, shared with the kernels.
 // Same library, same rules: no CPU fallback, errors through dm_last_error.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -16,65 +17,7 @@
 #include <vector>
 
 #include "../../include/deepmimic_b200.h"
-
-namespace dmk {
-struct MlpPrepParams {
-    const float* obs; const float* in_mean; const float* in_istd; float in_clip; int in_dim, M, NC; __half* tiles;
-    const float* goal; const float* g_mean; const float* g_istd; float g_clip; int goal_dim; __half* g_tiles;
-};
-struct MlpGemmParams {
-    const __half* a_tiles; const __half* w_tiles; const float* bias; __half* out_tiles; float* actions; const float* out_mean; const float* out_std; const float* noise;
-    int out_dim; int M, K, N;
-    const __half* gate_tiles; const __half* ws_tiles; const __half* wb_tiles; const float* bias_s; const float* bias_b; int gate_stride;
-};
-struct MlpStyleParams { const float* task_reward; float* logit; float* style; float* reward; float task_lerp; };
-__global__ void dm_mlp_prep_kernel(MlpPrepParams);
-__global__ void dm_mlp_gated_prep_kernel(MlpPrepParams);
-template <int BN, bool LAST>
-__global__ void dm_mlp_gemm_kernel(MlpGemmParams);
-__global__ void dm_mlp_gated_gemm_kernel(MlpGemmParams);
-__global__ void dm_mlp_style_reward_kernel(MlpGemmParams, MlpStyleParams);
-__global__ void dm_td_lambda_kernel(const float*, const float*, const float*, const uint8_t*, const int32_t*, int, int, float, float, float, float, float*, float*);
-int dm_mlp_smem_bytes(int bn);
-constexpr int kMlpATileHalves = 128 * 64;   // one operand tile of activations (kernels/dm_mlp.cu: kMlpATile)
-// the PPO learner (kernels/dm_mlp.cu: MlpGradParams and the backward GEMMs; kernels/dm_learn.cu)
-struct MlpGradParams { const __half* mask_tiles; __half* dy_a; __half* dy_b; float* partial; int row_chunks; int chunks_per_split; };
-struct LearnPrepParams { const float* x; const int64_t* idx; const float* mean; const float* istd; float clip; int in_dim, M, NC; __half* tiles; };
-struct LearnTransposeParams { const __half* src[3]; __half* dst[3]; int src_nc[3]; int ones[3]; int F[3]; int row_chunks; };
-struct LearnHeadParams {
-    const float* out; const int64_t* idx; int M, out_dim; __half* dy_a; __half* dy_b; float* partials;
-    const float* actions; const float* old_logp; const float* adv; const float* logstd; const float* bound_min; const float* bound_max; float ratio_clip; float* ratio;
-    const float* targets;
-};
-struct LearnLayerParams {
-    float* w; float* b; float* acc_w; float* acc_b; const float* partial; int splits, Npad, F; float inv_rows, lr, mom, wd; int in_dim, out_dim;
-    __half* tiles; float* bias_pad; int NC, BN; __half* t_tiles; int t_NC;
-};
-__global__ void dm_mlp_grad_x_kernel(MlpGemmParams, MlpGradParams);
-template <int BN>
-__global__ void dm_mlp_grad_w_kernel(MlpGemmParams, MlpGradParams);
-__global__ void dm_learn_prep_kernel(LearnPrepParams);
-__global__ void dm_learn_transpose_kernel(LearnTransposeParams);
-__global__ void dm_learn_actor_head_kernel(LearnHeadParams);
-__global__ void dm_learn_critic_head_kernel(LearnHeadParams);
-__global__ void dm_learn_stats_kernel(const float*, int, float, int, float*);
-__global__ void dm_learn_layer_kernel(LearnLayerParams);
-__global__ void dm_learn_norm_kernel(const float*, const float*, int, float*, float*, int);
-// the AMP discriminator's step (kernels/dm_learn.cu, kernels/dm_mlp.cu: dm_mlp_grad_xa_kernel)
-struct LearnDiscHeadParams { const float* out; int rows, E; __half* dy_a; __half* dy_b; __half* seed_a; __half* seed_b; float* partials; };
-struct LearnDiscLayerParams { LearnLayerParams L; const float* pen; int pen_splits, pen_F; float gp_w, reg; __half* p_tiles; int p_NC; };
-__global__ void dm_mlp_grad_xa_kernel(MlpGemmParams, MlpGradParams);
-__global__ void dm_learn_disc_head_kernel(LearnDiscHeadParams);
-__global__ void dm_learn_disc_gp_kernel(const __half*, int, float*);
-__global__ void dm_learn_disc_stats_kernel(const float*, int, const float*, int, float, float*);
-__global__ void dm_learn_disc_layer_kernel(LearnDiscLayerParams);
-// the gated networks' step (kernels/dm_learn.cu, kernels/dm_mlp.cu: MlpGateParams)
-struct MlpGateParams { float* fa; float* fb; __half* st_a; int st_nc, s_chunk, t_chunk; __half* st_b; };
-struct LearnGoalParams { const float* goal; const float* g_mean; const float* g_istd; float g_clip; int goal_dim; __half* g_tiles; };
-__global__ void dm_mlp_gated_save_kernel(MlpGemmParams, MlpGateParams);
-__global__ void dm_mlp_grad_xg_kernel(MlpGemmParams, MlpGradParams, MlpGateParams);
-__global__ void dm_learn_gated_prep_kernel(LearnPrepParams, LearnGoalParams);
-}  // namespace dmk
+#include "kernels/dm_mlp.cuh"
 
 extern "C" void dm_set_last_error(const char* msg);
 
@@ -96,6 +39,11 @@ struct dm_mlp {
 
 namespace {
 int mlp_fail(const std::string& m) { dm_set_last_error(m.c_str()); std::fprintf(stderr, "[deepmimic_b200] %s\n", m.c_str()); return 1; }
+// the outcome of the launches `fn` just enqueued: 0, or 1 with the launch error in dm_last_error
+int launch_status(const char* fn) {
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : mlp_fail(std::string(fn) + ": " + cudaGetErrorString(e));
+}
 int pad_to(int v, int q) { return ((v + q - 1) / q) * q; }
 // w: [K_in x N_out] row major (the reference's dense kernels: inputs x units).  Tiles: [n tile][k chunk][hi | lo][k8][row group][row][8 halves]
 std::vector<__half> tile_weights(const float* w, int k_in, int n_out, int K, int N, int BN) {
@@ -125,13 +73,21 @@ bool upload(T** dst, const std::vector<T>& src) {
 }
 std::vector<float> padded(const float* v, int n, int N, float fill = 0.f) { std::vector<float> o(N, fill); if (v) std::memcpy(o.data(), v, sizeof(float) * n); return o; }
 std::vector<float> inverse_std(const float* std_dev, int n) { std::vector<float> o(n, 1.f); for (int i = 0; i < n; ++i) o[i] = std_dev ? 1.0f / std_dev[i] : 1.f; return o; }
-// the plain network's operand preparation and two hidden layers (three launches); the caller sets the output layer's fields of the returned
-// parameters and launches it
-dmk::MlpGemmParams plain_trunk(dm_mlp* m, const float* d_obs, int rows, cudaStream_t st) {
+// the create functions' device checks: a CUDA device is present, `device` can be selected and is an sm_90 part.  fn names the caller in error
+// messages
+bool device_ok(const std::string& fn, int device) {
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { mlp_fail(fn + ": no CUDA device (the policy network has no CPU fallback)"); return false; }
+    if (cudaSetDevice(device) != cudaSuccess) { mlp_fail(fn + ": cudaSetDevice failed"); return false; }
+    cudaDeviceProp prop;
+    cudaGetDeviceProperties(&prop, device);
+    if (prop.major != 9 || prop.minor != 0) { mlp_fail(fn + ": the wgmma kernels are built for sm_90a (found sm_" + std::to_string(prop.major) + std::to_string(prop.minor) + ")"); return false; }
+    return true;
+}
+// the plain network's two hidden layers over the m tiles of `rows` rows prepared in obs_t (two launches); the caller sets the output layer's
+// fields of the returned parameters and launches it
+dmk::MlpGemmParams plain_hidden(const dm_mlp* m, int rows, cudaStream_t st) {
     const int mt = (rows + 127) / 128;
-    // observations -> normalised fp16 operand tiles
-    dmk::MlpPrepParams Q{d_obs, m->in_mean, m->in_istd, m->in_clip, m->in_dim, rows, m->K0 / 64, m->obs_t};
-    dmk::dm_mlp_prep_kernel<<<dim3(mt, m->K0 / 64), 128, 0, st>>>(Q);
     dmk::MlpGemmParams P{};
     P.M = rows;
     // layer 0: 227 -> 1024 + ReLU
@@ -140,6 +96,35 @@ dmk::MlpGemmParams plain_trunk(dm_mlp* m, const float* d_obs, int rows, cudaStre
     // layer 1: 1024 -> 512 + ReLU
     P.a_tiles = m->act0; P.w_tiles = m->w[1]; P.bias = m->b[1]; P.out_tiles = m->act1; P.K = m->N0; P.N = m->N1;
     dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, m->N1 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
+    // the output layer reads layer 1's tiles
+    P.a_tiles = m->act1; P.w_tiles = m->w[2]; P.bias = m->b[2]; P.out_tiles = nullptr; P.K = m->N1; P.N = m->N2;
+    return P;
+}
+// the gated network's gate trunk, both gate hidden layers and two gated trunk layers over the m tiles of `rows` rows prepared in obs_t and
+// goal_t (four launches).  Given the learner's factor buffers (save[l] for trunk layer l) the trunk layers also save their factors
+// (dm_mlp_gated_save_kernel); the caller sets the output layer's fields of the returned parameters and launches it
+dmk::MlpGemmParams gated_hidden(const dm_mlp* m, int rows, const dmk::MlpGateParams* save, cudaStream_t st) {
+    const int mt = (rows + 127) / 128;
+    dmk::MlpGemmParams P{};
+    P.M = rows;
+    // gate trunk: goal -> 128 + ReLU
+    P.a_tiles = m->goal_t; P.w_tiles = m->wgc; P.bias = m->bgc; P.out_tiles = m->gc_t; P.K = 64; P.N = 128;
+    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
+    // both gate hidden layers: 128 -> 2 x 64 + ReLU; K-chunk l of the output is layer l's gate in operand layout
+    P.a_tiles = m->gc_t; P.w_tiles = m->wgh; P.bias = m->bgh; P.out_tiles = m->gh_t; P.K = 128; P.N = 128;
+    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
+    // gated trunk layers: 229 -> 1024, 1024 -> 512, each scaled and shifted by its gate
+    auto gated = [&](int l) {
+        if (save) dmk::dm_mlp_gated_save_kernel<<<dim3(mt, P.N / 64), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P, save[l]);
+        else dmk::dm_mlp_gated_gemm_kernel<<<dim3(mt, P.N / 64), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P);
+    };
+    P.gate_stride = 2 * dmk::kMlpATile;
+    P.a_tiles = m->obs_t; P.w_tiles = m->w[0]; P.bias = m->b[0]; P.out_tiles = m->act0; P.K = m->K0; P.N = m->N0;
+    P.gate_tiles = m->gh_t; P.ws_tiles = m->wgs[0]; P.wb_tiles = m->wgb[0]; P.bias_s = m->bgs[0]; P.bias_b = m->bgb[0];
+    gated(0);
+    P.a_tiles = m->act0; P.w_tiles = m->w[1]; P.bias = m->b[1]; P.out_tiles = m->act1; P.K = m->N0; P.N = m->N1;
+    P.gate_tiles = m->gh_t + dmk::kMlpATile; P.ws_tiles = m->wgs[1]; P.wb_tiles = m->wgb[1]; P.bias_s = m->bgs[1]; P.bias_b = m->bgb[1];
+    gated(1);
     // the output layer reads layer 1's tiles
     P.a_tiles = m->act1; P.w_tiles = m->w[2]; P.bias = m->b[2]; P.out_tiles = nullptr; P.K = m->N1; P.N = m->N2;
     return P;
@@ -176,13 +161,19 @@ dmk::LearnLayerParams gated_layer_params(dm_mlp* m, int i, const float* w, const
     }
     return L;
 }
+// the optimiser step's fields of the layer pass of parameter pair i: its accumulators, the split count of its dW partials and the batch's 1 / rows,
+// stepsize, momentum and weight decay
+template <class Net, class Batch>
+void optimiser_fields(dmk::LearnLayerParams& L, const Net* net, int i, const Batch* b, int splits) {
+    L.acc_w = net->acc_w[i]; L.acc_b = net->acc_b[i]; L.splits = splits;
+    L.inv_rows = 1.f / b->rows; L.lr = b->stepsize; L.mom = b->momentum; L.wd = b->weight_decay;
+}
 }  // namespace
 
 // PPO learner workspace (include/deepmimic_b200.h: dm_learn_*).  Layer l = 0, 1, 2 has F[l] = pad128(inputs + 1) transposed-input features (the
 // ones feature at index `inputs` makes row `inputs` of dW the bias gradient) and Nout[l] padded outputs (N0, N1, N2 of the handle).
 struct dm_learn {
     dm_mlp* m = nullptr;
-    bool actor = true;
     int kind = 0;
     int max_rows = 0, F[3] = {0, 0, 0}, Nout[3] = {0, 0, 0}, max_splits[3] = {0, 0, 0};
     float* out = nullptr;                                    // [max_rows x out_dim] normalised network output
@@ -220,8 +211,7 @@ namespace {
 // backward's tiles; the padding columns are zero and change no row's values).  fn names the caller in error messages
 dm_mlp* create_gated(const char* fn, int device, const dm_mlp_gated_weights* g, int max_rows, int trunk_pad) {
     const std::string f(fn);
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { mlp_fail(f + ": no CUDA device (the policy network has no CPU fallback)"); return nullptr; }
+    if (!device_ok(f, device)) return nullptr;
     if (!g) { mlp_fail(f + ": null weights"); return nullptr; }
     if (g->in_dim <= 0 || g->goal_dim <= 0 || g->goal_dim > 64 || g->h0 <= 0 || g->h1 <= 0 || g->out_dim <= 0 || g->out_dim > 64 || max_rows <= 0) {
         mlp_fail(f + ": bad sizes (goal_dim must be <= 64, out_dim <= 64)"); return nullptr;
@@ -233,10 +223,6 @@ dm_mlp* create_gated(const char* fn, int device, const dm_mlp_gated_weights* g, 
                            g->gs_w[0], g->gs_b[0], g->gs_w[1], g->gs_b[1], g->gb_w[0], g->gb_b[0], g->gb_w[1], g->gb_b[1]};
     for (const float* p : need)
         if (!p) { mlp_fail(f + ": null weight pointer"); return nullptr; }
-    if (cudaSetDevice(device) != cudaSuccess) { mlp_fail(f + ": cudaSetDevice failed"); return nullptr; }
-    cudaDeviceProp prop;
-    cudaGetDeviceProperties(&prop, device);
-    if (prop.major != 9 || prop.minor != 0) { mlp_fail(f + ": the wgmma kernels are built for sm_90a (found sm_" + std::to_string(prop.major) + std::to_string(prop.minor) + ")"); return nullptr; }
     dm_mlp* m = new dm_mlp();
     m->gated = true;
     m->device = device; m->in_dim = g->in_dim; m->goal_dim = g->goal_dim; m->gate_common = g->gate_common; m->gate_hidden = g->gate_hidden; m->h0 = g->h0; m->h1 = g->h1; m->out_dim = g->out_dim; m->max_rows = pad_to(max_rows, 128);
@@ -267,7 +253,7 @@ dm_mlp* create_gated(const char* fn, int device, const dm_mlp_gated_weights* g, 
          upload(&m->g_mean, padded(g->g_mean, g->goal_dim, g->goal_dim)) && upload(&m->g_istd, inverse_std(g->g_std, g->goal_dim)) &&
          upload(&m->out_mean, padded(g->a_mean, g->out_dim, g->out_dim)) && upload(&m->out_std, padded(g->a_std, g->out_dim, g->out_dim, 1.f)) &&
          cudaMalloc(&m->obs_t, R * m->K0 * sizeof(__half)) == cudaSuccess && cudaMalloc(&m->goal_t, R * 64 * sizeof(__half)) == cudaSuccess &&
-         cudaMalloc(&m->gc_t, R * 128 * sizeof(__half)) == cudaSuccess && cudaMalloc(&m->gh_t, (R * 128 + dmk::kMlpATileHalves) * sizeof(__half)) == cudaSuccess &&
+         cudaMalloc(&m->gc_t, R * 128 * sizeof(__half)) == cudaSuccess && cudaMalloc(&m->gh_t, (R * 128 + dmk::kMlpATile) * sizeof(__half)) == cudaSuccess &&
          cudaMalloc(&m->act0, R * m->N0 * sizeof(__half)) == cudaSuccess && cudaMalloc(&m->act1, R * m->N1 * sizeof(__half)) == cudaSuccess;
     if (ok) {
         ok = cudaFuncSetAttribute(dmk::dm_mlp_gemm_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
@@ -278,11 +264,61 @@ dm_mlp* create_gated(const char* fn, int device, const dm_mlp_gated_weights* g, 
     return m;
 }
 
-// split-K of a dW GEMM: about two CTAs per SM of an H100 (132 SMs) over the (F / 128) x (Nout / BN) output tiles
-void dw_split(int tiles, int chunks, int* splits, int* cps) {
+// split-K of a dW GEMM: about two CTAs per SM of an H100 (132 SMs) over the (F / 128) x (N / BN) output tiles
+void dw_split(int F, int N, int BN, int chunks, int* splits, int* cps) {
+    const int tiles = (F / 128) * (N / BN);
     int s = std::max(1, std::min(chunks, (264 + tiles - 1) / tiles));
     *cps = (chunks + s - 1) / s;
     *splits = (chunks + *cps - 1) / *cps;
+}
+// the split count a dW GEMM's partials are sized for.  It is not monotonic in the row count (ceil(c / ceil(c / s))): the largest over every
+// minibatch a step may take (an even chunk count up to max_chunks)
+int dw_max_splits(int F, int N, int BN, int max_chunks) {
+    int mx = 0;
+    for (int c = 2; c <= max_chunks; c += 2) {
+        int s = 0, cps = 0;
+        dw_split(F, N, BN, c, &s, &cps);
+        mx = std::max(mx, s);
+    }
+    return mx;
+}
+// a step's split-K plan of a dW GEMM over `chunks` row chunks, refused when it needs more partials than the workspace holds (max_splits)
+int dw_plan(const char* fn, int F, int N, int BN, int chunks, int max_splits, int* splits, int* cps) {
+    dw_split(F, N, BN, chunks, splits, cps);
+    return *splits > max_splits ? mlp_fail(std::string(fn) + ": internal error: dW split count exceeds the workspace") : 0;
+}
+// dW = X^T dY over `chunks` row chunks, split into `splits` ranges of `cps` chunks: A = x_t (F transposed features), B = dy (N outputs on
+// BN-column tiles), one fp32 partial product per split
+void launch_dw(const __half* x_t, const __half* dy, float* partial, int F, int N, int BN, int chunks, int splits, int cps, cudaStream_t st) {
+    dmk::MlpGemmParams W{};
+    W.a_tiles = x_t; W.w_tiles = dy; W.M = F; W.N = N;
+    const dmk::MlpGradParams GW{nullptr, nullptr, nullptr, partial, chunks, cps};
+    if (BN == 64) dmk::dm_mlp_grad_w_kernel<64><<<dim3(F / 128, N / 64, splits), 256, dmk::dm_mlp_smem_bytes(64), st>>>(W, GW);
+    else dmk::dm_mlp_grad_w_kernel<128><<<dim3(F / 128, N / 128, splits), 256, dmk::dm_mlp_smem_bytes(128), st>>>(W, GW);
+}
+// the column width of trunk layer i's dW GEMM: 128, the output layer's N2 = 64
+int trunk_bn(const dm_learn* l, int i) { return i == 2 ? l->m->N2 : 128; }
+// the workspace of the trunk's layers 0..2 (in[i] inputs), plain and gated: out, head_partials, F, Nout, xt, dy_a, dy_b, wt, partial (sized for
+// the largest split count a step may take); and the backward kernels' shared-memory opt-in.  l->m and l->max_rows are set
+bool trunk_workspace(dm_learn* l, const int* in) {
+    const dm_mlp* m = l->m;
+    const size_t R = l->max_rows, h = sizeof(__half);
+    l->Nout[0] = m->N0; l->Nout[1] = m->N1; l->Nout[2] = m->N2;
+    bool ok = cudaMalloc(&l->out, R * m->out_dim * sizeof(float)) == cudaSuccess && cudaMalloc(&l->head_partials, R / 128 * 3 * sizeof(float)) == cudaSuccess;
+    for (int i = 0; i < 3 && ok; ++i) {
+        l->F[i] = pad_to(in[i] + 1, 128);
+        l->max_splits[i] = dw_max_splits(l->F[i], l->Nout[i], trunk_bn(l, i), l->max_rows / 64);
+        ok = cudaMalloc(&l->xt[i], R * l->F[i] * h) == cudaSuccess && cudaMalloc(&l->dy_b[i], 2 * R * l->Nout[i] * h) == cudaSuccess &&
+             cudaMalloc(&l->partial[i], static_cast<size_t>(l->max_splits[i]) * l->Nout[i] * l->F[i] * sizeof(float)) == cudaSuccess;
+        // W_i^T as B of the dX GEMM: K = Nout[i], N = Nout[i - 1] (zero padding written once)
+        if (ok && i > 0) {
+            const size_t n = 2 * static_cast<size_t>(l->Nout[i]) * l->Nout[i - 1];
+            ok = cudaMalloc(&l->dy_a[i], 2 * R * l->Nout[i] * h) == cudaSuccess && cudaMalloc(&l->wt[i], n * h) == cudaSuccess && cudaMemset(l->wt[i], 0, n * h) == cudaSuccess;
+        }
+    }
+    return ok && cudaFuncSetAttribute(dmk::dm_mlp_grad_x_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
+           cudaFuncSetAttribute(dmk::dm_mlp_grad_w_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
+           cudaFuncSetAttribute(dmk::dm_mlp_grad_w_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess;
 }
 }  // namespace
 
@@ -290,13 +326,8 @@ extern "C" {
 
 dm_mlp* dm_mlp_create(int device, int in_dim, int h0, int h1, int out_dim, const float* w0, const float* b0, const float* w1, const float* b1, const float* w2, const float* b2,
                       const float* in_mean, const float* in_std, float in_clip, const float* out_mean, const float* out_std, int max_rows) {
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { mlp_fail("dm_mlp_create: no CUDA device (the policy network has no CPU fallback)"); return nullptr; }
+    if (!device_ok("dm_mlp_create", device)) return nullptr;
     if (in_dim <= 0 || h0 <= 0 || h1 <= 0 || out_dim <= 0 || out_dim > 64 || max_rows <= 0) { mlp_fail("dm_mlp_create: bad sizes (out_dim must be <= 64)"); return nullptr; }
-    if (cudaSetDevice(device) != cudaSuccess) { mlp_fail("dm_mlp_create: cudaSetDevice failed"); return nullptr; }
-    cudaDeviceProp prop;
-    cudaGetDeviceProperties(&prop, device);
-    if (prop.major != 9 || prop.minor != 0) { mlp_fail("dm_mlp_create: the wgmma kernels are built for sm_90a (found sm_" + std::to_string(prop.major) + std::to_string(prop.minor) + ")"); return nullptr; }
     dm_mlp* m = new dm_mlp();
     m->device = device; m->in_dim = in_dim; m->h0 = h0; m->h1 = h1; m->out_dim = out_dim; m->max_rows = pad_to(max_rows, 128);
     m->K0 = pad_to(in_dim, 64); m->N0 = pad_to(h0, 128); m->N1 = pad_to(h1, 128);
@@ -308,7 +339,6 @@ dm_mlp* dm_mlp_create(int device, int in_dim, int h0, int h1, int out_dim, const
               cudaMalloc(&m->obs_t, static_cast<size_t>(m->max_rows) * m->K0 * sizeof(__half)) == cudaSuccess &&
               cudaMalloc(&m->act0, static_cast<size_t>(m->max_rows) * m->N0 * sizeof(__half)) == cudaSuccess &&
               cudaMalloc(&m->act1, static_cast<size_t>(m->max_rows) * m->N1 * sizeof(__half)) == cudaSuccess;
-    if (ok && !out_std) { std::vector<float> one(out_dim, 1.f); ok = cudaMemcpy(m->out_std, one.data(), sizeof(float) * out_dim, cudaMemcpyHostToDevice) == cudaSuccess; }
     if (ok) {
         ok = cudaFuncSetAttribute(dmk::dm_mlp_gemm_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
              cudaFuncSetAttribute(dmk::dm_mlp_gemm_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess;
@@ -325,12 +355,15 @@ int dm_mlp_forward(dm_mlp* m, const float* d_obs, const float* d_noise, float* d
     if (rows <= 0 || rows > m->max_rows) return mlp_fail("dm_mlp_forward: rows out of range");
     if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_mlp_forward: cudaSetDevice failed");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    dmk::MlpGemmParams P = plain_trunk(m, d_obs, rows, st);
+    const int mt = (rows + 127) / 128;
+    // observations -> normalised fp16 operand tiles
+    const dmk::MlpPrepParams Q{d_obs, m->in_mean, m->in_istd, m->in_clip, m->in_dim, rows, m->K0 / 64, m->obs_t};
+    dmk::dm_mlp_prep_kernel<<<dim3(mt, m->K0 / 64), 128, 0, st>>>(Q);
+    dmk::MlpGemmParams P = plain_hidden(m, rows, st);
     // layer 2: 512 -> actions, un-normalised
     P.actions = d_actions; P.out_mean = m->out_mean; P.out_std = m->out_std; P.noise = d_noise; P.out_dim = m->out_dim;
-    dmk::dm_mlp_gemm_kernel<64, true><<<dim3((rows + 127) / 128, 1), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return mlp_fail(std::string("dm_mlp_forward: ") + cudaGetErrorString(e));
+    dmk::dm_mlp_gemm_kernel<64, true><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P);
+    if (launch_status("dm_mlp_forward")) return 1;
     m->launches += 4;
     return 0;
 }
@@ -350,28 +383,11 @@ int dm_mlp_forward_gated(dm_mlp* m, const float* d_obs, const float* d_goal, con
     // [state | goal] -> normalised fp16 trunk tiles; the normalised goal alone -> the gate trunk's tile (the extra chunk of the grid)
     dmk::MlpPrepParams Q{d_obs, m->in_mean, m->in_istd, m->in_clip, m->in_dim, rows, m->K0 / 64, m->obs_t, d_goal, m->g_mean, m->g_istd, m->g_clip, m->goal_dim, m->goal_t};
     dmk::dm_mlp_gated_prep_kernel<<<dim3(mt, m->K0 / 64 + 1), 128, 0, st>>>(Q);
-    dmk::MlpGemmParams P{};
-    P.M = rows;
-    // gate trunk: goal -> 128 + ReLU
-    P.a_tiles = m->goal_t; P.w_tiles = m->wgc; P.bias = m->bgc; P.out_tiles = m->gc_t; P.K = 64; P.N = 128;
-    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
-    // both gate hidden layers: 128 -> 2 x 64 + ReLU; K-chunk l of the output is layer l's gate in operand layout
-    P.a_tiles = m->gc_t; P.w_tiles = m->wgh; P.bias = m->bgh; P.out_tiles = m->gh_t; P.K = 128; P.N = 128;
-    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
-    // gated trunk layers: 229 -> 1024, 1024 -> 512, each scaled and shifted by its gate
-    P.gate_stride = 2 * dmk::kMlpATileHalves;
-    P.a_tiles = m->obs_t; P.w_tiles = m->w[0]; P.bias = m->b[0]; P.out_tiles = m->act0; P.K = m->K0; P.N = m->N0;
-    P.gate_tiles = m->gh_t; P.ws_tiles = m->wgs[0]; P.wb_tiles = m->wgb[0]; P.bias_s = m->bgs[0]; P.bias_b = m->bgb[0];
-    dmk::dm_mlp_gated_gemm_kernel<<<dim3(mt, m->N0 / 64), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P);
-    P.a_tiles = m->act0; P.w_tiles = m->w[1]; P.bias = m->b[1]; P.out_tiles = m->act1; P.K = m->N0; P.N = m->N1;
-    P.gate_tiles = m->gh_t + dmk::kMlpATileHalves; P.ws_tiles = m->wgs[1]; P.wb_tiles = m->wgb[1]; P.bias_s = m->bgs[1]; P.bias_b = m->bgb[1];
-    dmk::dm_mlp_gated_gemm_kernel<<<dim3(mt, m->N1 / 64), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P);
+    dmk::MlpGemmParams P = gated_hidden(m, rows, nullptr, st);
     // output layer: 512 -> actions, un-normalised
-    P.a_tiles = m->act1; P.w_tiles = m->w[2]; P.bias = m->b[2]; P.out_tiles = nullptr; P.actions = d_actions; P.out_mean = m->out_mean; P.out_std = m->out_std; P.noise = d_noise;
-    P.out_dim = m->out_dim; P.K = m->N1; P.N = m->N2;
+    P.actions = d_actions; P.out_mean = m->out_mean; P.out_std = m->out_std; P.noise = d_noise; P.out_dim = m->out_dim;
     dmk::dm_mlp_gemm_kernel<64, true><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return mlp_fail(std::string("dm_mlp_forward_gated: ") + cudaGetErrorString(e));
+    if (launch_status("dm_mlp_forward_gated")) return 1;
     m->launches += 6;
     return 0;
 }
@@ -386,12 +402,14 @@ int dm_mlp_forward_style_reward(dm_mlp* m, const float* d_amp_obs, const float* 
     if (!d_amp_obs || !d_reward) return mlp_fail("dm_mlp_forward_style_reward: null AMP observation or reward pointer");
     if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_mlp_forward_style_reward: cudaSetDevice failed");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    dmk::MlpGemmParams P = plain_trunk(m, d_amp_obs, rows, st);
+    const int mt = (rows + 127) / 128;
+    const dmk::MlpPrepParams Q{d_amp_obs, m->in_mean, m->in_istd, m->in_clip, m->in_dim, rows, m->K0 / 64, m->obs_t};
+    dmk::dm_mlp_prep_kernel<<<dim3(mt, m->K0 / 64), 128, 0, st>>>(Q);
+    const dmk::MlpGemmParams P = plain_hidden(m, rows, st);
     // logit head: 512 -> 1, then the style reward and its blend with the task reward
     const dmk::MlpStyleParams S{d_task_reward, d_logit, d_style, d_reward, task_lerp};
-    dmk::dm_mlp_style_reward_kernel<<<dim3((rows + 127) / 128, 1), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P, S);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return mlp_fail(std::string("dm_mlp_forward_style_reward: ") + cudaGetErrorString(e));
+    dmk::dm_mlp_style_reward_kernel<<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P, S);
+    if (launch_status("dm_mlp_forward_style_reward")) return 1;
     m->launches += 4;
     return 0;
 }
@@ -405,9 +423,7 @@ int dm_td_lambda_returns(const float* d_rewards, const float* d_values, const fl
     constexpr int kThreads = 64;   // N = 4096 environments -> 64 CTAs on 64 SMs: the scan is latency-bound, more SMs keep more loads in flight
     dmk::dm_td_lambda_kernel<<<(N + kThreads - 1) / kThreads, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
         d_rewards, d_values, d_end_values, d_done, d_terminate, T, N, discount, td_lambda, val_fail, val_succ, d_returns, d_advantages);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return mlp_fail(std::string("dm_td_lambda_returns: ") + cudaGetErrorString(e));
-    return 0;
+    return launch_status("dm_td_lambda_returns");
 }
 
 int dm_mlp_set_weights_device(dm_mlp* m, const float* d_w0, const float* d_b0, const float* d_w1, const float* d_b1, const float* d_w2, const float* d_b2,
@@ -420,9 +436,7 @@ int dm_mlp_set_weights_device(dm_mlp* m, const float* d_w0, const float* d_b0, c
     if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_mlp_set_weights_device: cudaSetDevice failed");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     for (int l = 0; l < 3; ++l) launch_layer(layer_params(m, l, p[2 * l], p[2 * l + 1]), st);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return mlp_fail(std::string("dm_mlp_set_weights_device: ") + cudaGetErrorString(e));
-    return 0;
+    return launch_status("dm_mlp_set_weights_device");
 }
 
 int dm_mlp_set_normalizers_device(dm_mlp* m, const float* d_in_mean, const float* d_in_std, const float* d_out_mean, const float* d_out_std, void* stream) {
@@ -433,9 +447,7 @@ int dm_mlp_set_normalizers_device(dm_mlp* m, const float* d_in_mean, const float
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     dmk::dm_learn_norm_kernel<<<(m->in_dim + 255) / 256, 256, 0, st>>>(d_in_mean, d_in_std, m->in_dim, m->in_mean, m->in_istd, 1);
     dmk::dm_learn_norm_kernel<<<(m->out_dim + 255) / 256, 256, 0, st>>>(d_out_mean, d_out_std, m->out_dim, m->out_mean, m->out_std, 0);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return mlp_fail(std::string("dm_mlp_set_normalizers_device: ") + cudaGetErrorString(e));
-    return 0;
+    return launch_status("dm_mlp_set_normalizers_device");
 }
 
 dm_learn* dm_learn_create(int device, int kind, int in_dim, int h0, int h1, int out_dim, int max_rows) {
@@ -451,39 +463,14 @@ dm_learn* dm_learn_create(int device, int kind, int in_dim, int h0, int h1, int 
     dm_mlp* m = dm_mlp_create(device, in_dim, h0, h1, out_dim, w0.data(), b0.data(), w1.data(), b1.data(), w2.data(), b2.data(), nullptr, nullptr, 0.f, nullptr, nullptr, rows);
     if (!m) return nullptr;   // dm_last_error is set
     dm_learn* l = new dm_learn();
-    l->m = m; l->actor = kind == 0; l->kind = kind; l->max_rows = m->max_rows;
-    const int in[3] = {in_dim, h0, h1}, BN[3] = {128, 128, m->N2}, chunks = m->max_rows / 64;
-    l->Nout[0] = m->N0; l->Nout[1] = m->N1; l->Nout[2] = m->N2;
-    const size_t R = m->max_rows;
-    bool ok = cudaMalloc(&l->out, R * out_dim * sizeof(float)) == cudaSuccess && cudaMalloc(&l->head_partials, R / 128 * 3 * sizeof(float)) == cudaSuccess;
-    for (int i = 0; i < 3 && ok; ++i) {
-        l->F[i] = pad_to(in[i] + 1, 128);
-        // the split count is not monotonic in the row count (ceil(c / ceil(c / s))): size the partials for the largest over every minibatch
-        // a step may take (rows in [1, max_rows]: an even chunk count up to max_rows / 64)
-        for (int c = 2; c <= chunks; c += 2) {
-            int s = 0, cps = 0;
-            dw_split((l->F[i] / 128) * (l->Nout[i] / BN[i]), c, &s, &cps);
-            l->max_splits[i] = std::max(l->max_splits[i], s);
-        }
-        ok = cudaMalloc(&l->xt[i], R * l->F[i] * sizeof(__half)) == cudaSuccess && cudaMalloc(&l->dy_b[i], 2 * R * l->Nout[i] * sizeof(__half)) == cudaSuccess &&
-             cudaMalloc(&l->partial[i], static_cast<size_t>(l->max_splits[i]) * l->Nout[i] * l->F[i] * sizeof(float)) == cudaSuccess;
-        // W_i^T as B of the dX GEMM: K = Nout[i], N = Nout[i - 1] (zero padding written once)
-        if (ok && i > 0) {
-            const size_t n = 2 * static_cast<size_t>(l->Nout[i]) * l->Nout[i - 1];
-            ok = cudaMalloc(&l->dy_a[i], 2 * R * l->Nout[i] * sizeof(__half)) == cudaSuccess && cudaMalloc(&l->wt[i], n * sizeof(__half)) == cudaSuccess &&
-                 cudaMemset(l->wt[i], 0, n * sizeof(__half)) == cudaSuccess;
-        }
-    }
+    l->m = m; l->kind = kind; l->max_rows = m->max_rows;
+    const int in[3] = {in_dim, h0, h1};
+    bool ok = trunk_workspace(l, in);
     if (ok && kind == 2) {
         l->side_rows = side; l->E = E; l->Ng = pad_to(in_dim, 128);
         const int Ng = l->Ng, N0 = m->N0, N1 = m->N1;
         l->pen_F[0] = Ng; l->pen_F[1] = N0; l->pen_F[2] = N1;
-        for (int i = 0; i < 3; ++i)
-            for (int c = 2; c <= E / 64; c += 2) {
-                int s = 0, cps = 0;
-                dw_split((l->pen_F[i] / 128) * (l->Nout[i] / BN[i]), c, &s, &cps);
-                l->pen_max_splits[i] = std::max(l->pen_max_splits[i], s);
-            }
+        for (int i = 0; i < 3; ++i) l->pen_max_splits[i] = dw_max_splits(l->pen_F[i], l->Nout[i], trunk_bn(l, i), E / 64);
         const size_t e = E, h = sizeof(__half), tw = 2 * static_cast<size_t>(N0) * Ng;   // halves of W0^T / W0 as hi + lo tiles
         ok = cudaMalloc(&l->seed_a, 2 * e * 64 * h) == cudaSuccess && cudaMalloc(&l->seed_b, 2 * e * 64 * h) == cudaSuccess &&
              cudaMalloc(&l->u_a[0], 2 * e * N0 * h) == cudaSuccess && cudaMalloc(&l->u_b[0], 2 * e * N0 * h) == cudaSuccess &&
@@ -497,11 +484,6 @@ dm_learn* dm_learn_create(int device, int kind, int in_dim, int h0, int h1, int 
                  cudaMalloc(&l->pen[i], static_cast<size_t>(l->pen_max_splits[i]) * l->Nout[i] * l->pen_F[i] * sizeof(float)) == cudaSuccess;
         ok = ok && cudaFuncSetAttribute(dmk::dm_mlp_grad_xa_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess;
     }
-    if (ok) {
-        ok = cudaFuncSetAttribute(dmk::dm_mlp_grad_x_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
-             cudaFuncSetAttribute(dmk::dm_mlp_grad_w_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
-             cudaFuncSetAttribute(dmk::dm_mlp_grad_w_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess;
-    }
     if (!ok) { mlp_fail(std::string("dm_learn_create: ") + cudaGetErrorString(cudaGetLastError())); dm_learn_destroy(l); return nullptr; }
     return l;
 }
@@ -513,14 +495,39 @@ int learn_net_check(const dm_learn_net* net, const char* fn) {
         if (!net->w[i] || !net->b[i] || !net->acc_w[i] || !net->acc_b[i]) return mlp_fail(std::string(fn) + ": null parameter or accumulator pointer");
     return 0;
 }
-// the forward tiles of the learner's handle and the transposed tiles of the dX GEMMs; with `step` also the optimiser step before the re-tiling
-void learn_layers(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, int rows, const int* splits, cudaStream_t st) {
+// the checks of a PPO step's batch b (dm_learn_step, dm_learn_gated_step); the gated step also passes gb (b = &gb->batch), whose goal pointers
+// are checked with the states'
+int ppo_batch_check(const char* fn, const dm_learn* l, const dm_learn_batch* b, const dm_learn_gated_batch* gb) {
+    const std::string f(fn);
+    const bool actor = l->kind == 0;
+    if (!b) return mlp_fail(f + ": null batch");
+    if (b->rows <= 0 || b->rows > l->max_rows) return mlp_fail(f + ": rows out of range");
+    if (!b->states || !b->idx || !b->in_mean || !b->in_istd || !b->stats || (gb && (!gb->goals || !gb->g_mean || !gb->g_istd)))
+        return mlp_fail(f + (gb ? ": null state, goal, index, normaliser or statistics pointer" : ": null state, index, normaliser or statistics pointer"));
+    if (actor && (!b->norm_actions || !b->old_logp || !b->adv || !b->logstd || !b->bound_min || !b->bound_max))
+        return mlp_fail(f + ": null action, log-probability, advantage, log-std or bound pointer");
+    if (!actor && !b->norm_targets) return mlp_fail(f + ": null target pointer");
+    if (actor && !(b->ratio_clip > 0.f)) return mlp_fail(f + ": ratio_clip must be positive");
+    if (!(b->stepsize >= 0.f) || !(b->momentum >= 0.f) || !(b->weight_decay >= 0.f)) return mlp_fail(f + ": stepsize, momentum and weight_decay must be >= 0");
+    return 0;
+}
+// a PPO step's loss head over the mt m tiles of l->out (dY of the output layer, the loss partials) and its statistics
+void launch_ppo_head(const dm_learn* l, const dm_learn_batch* b, int mt, cudaStream_t st) {
+    const bool actor = l->kind == 0;
+    const dmk::LearnHeadParams H{l->out, b->idx, b->rows, l->m->out_dim, l->dy_a[2], l->dy_b[2], l->head_partials, b->norm_actions, b->old_logp, b->adv, b->logstd,
+                                 b->bound_min, b->bound_max, b->ratio_clip, b->ratio, b->norm_targets};
+    if (actor) dmk::dm_learn_actor_head_kernel<<<mt, 128, 0, st>>>(H);
+    else dmk::dm_learn_critic_head_kernel<<<mt, 128, 0, st>>>(H);
+    dmk::dm_learn_stats_kernel<<<1, 1, 0, st>>>(l->head_partials, mt, 1.f / b->rows, actor ? 1 : 0, b->stats);
+}
+// the forward tiles of the learner's handle and the transposed tiles of the dX GEMMs; with `b` also the optimiser step before the re-tiling
+void learn_layers(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, const int* splits, cudaStream_t st) {
     for (int i = 0; i < 3; ++i) {
         dmk::LearnLayerParams L = layer_params(l->m, i, net->w[i], net->b[i]);
         if (i > 0) { L.t_tiles = l->wt[i]; L.t_NC = l->Nout[i] / 64; }
         if (b) {
-            L.acc_w = net->acc_w[i]; L.acc_b = net->acc_b[i]; L.partial = l->partial[i]; L.splits = splits[i]; L.Npad = l->Nout[i]; L.F = l->F[i];
-            L.inv_rows = 1.f / rows; L.lr = b->stepsize; L.mom = b->momentum; L.wd = b->weight_decay;
+            L.partial = l->partial[i]; L.Npad = l->Nout[i]; L.F = l->F[i];
+            optimiser_fields(L, net, i, b, splits[i]);
         }
         launch_layer(L, st);
     }
@@ -534,8 +541,8 @@ void learn_disc_layers(dm_learn* l, const dm_learn_net* net, const dm_learn_disc
         D.L.t_tiles = l->wt[i]; D.L.t_NC = l->Nout[i] / 64;
         if (i == 0) { D.p_tiles = l->w0p; D.p_NC = l->Ng / 64; }
         if (b) {
-            D.L.acc_w = net->acc_w[i]; D.L.acc_b = net->acc_b[i]; D.L.partial = l->partial[i]; D.L.splits = splits[i]; D.L.Npad = l->Nout[i]; D.L.F = l->F[i];
-            D.L.inv_rows = 1.f / b->rows; D.L.lr = b->stepsize; D.L.mom = b->momentum; D.L.wd = b->weight_decay;
+            D.L.partial = l->partial[i]; D.L.Npad = l->Nout[i]; D.L.F = l->F[i];
+            optimiser_fields(D.L, net, i, b, splits[i]);
             D.pen = l->pen[i]; D.pen_splits = psplits[i]; D.pen_F = l->pen_F[i]; D.gp_w = b->grad_penalty_weight; D.reg = i == 2 ? b->logit_reg_weight : 0.f;
         }
         dmk::dm_learn_disc_layer_kernel<<<dim3((D.L.in_dim + 1 + 255) / 256, D.L.out_dim), 256, 0, st>>>(D);
@@ -545,13 +552,7 @@ void learn_disc_layers(dm_learn* l, const dm_learn_net* net, const dm_learn_disc
 // saved activations into the dW GEMMs' A operands
 void learn_forward(dm_learn* l, int rows, int mt, cudaStream_t st) {
     dm_mlp* m = l->m;
-    dmk::MlpGemmParams P{};
-    P.M = rows;
-    P.a_tiles = m->obs_t; P.w_tiles = m->w[0]; P.bias = m->b[0]; P.out_tiles = m->act0; P.K = m->K0; P.N = m->N0;
-    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, m->N0 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
-    P.a_tiles = m->act0; P.w_tiles = m->w[1]; P.bias = m->b[1]; P.out_tiles = m->act1; P.K = m->N0; P.N = m->N1;
-    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, m->N1 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
-    P.a_tiles = m->act1; P.w_tiles = m->w[2]; P.bias = m->b[2]; P.out_tiles = nullptr; P.K = m->N1; P.N = m->N2;
+    dmk::MlpGemmParams P = plain_hidden(m, rows, st);
     P.actions = l->out; P.out_mean = m->out_mean; P.out_std = m->out_std; P.noise = nullptr; P.out_dim = m->out_dim;
     dmk::dm_mlp_gemm_kernel<64, true><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P);
     const int chunks = 2 * mt;
@@ -565,13 +566,7 @@ void learn_backward(dm_learn* l, int rows, int mt, const int* splits, const int*
     const int chunks = 2 * mt;
     const __half* act[3] = {m->obs_t, m->act0, m->act1};
     for (int i = 2; i >= 0; --i) {
-        const int BN = i == 2 ? m->N2 : 128;
-        dmk::MlpGemmParams W{};
-        W.a_tiles = l->xt[i]; W.w_tiles = l->dy_b[i]; W.M = l->F[i]; W.N = l->Nout[i];
-        const dmk::MlpGradParams GW{nullptr, nullptr, nullptr, l->partial[i], chunks, cps[i]};
-        const dim3 gw(l->F[i] / 128, l->Nout[i] / BN, splits[i]);
-        if (i == 2) dmk::dm_mlp_grad_w_kernel<64><<<gw, 256, dmk::dm_mlp_smem_bytes(64), st>>>(W, GW);
-        else dmk::dm_mlp_grad_w_kernel<128><<<gw, 256, dmk::dm_mlp_smem_bytes(128), st>>>(W, GW);
+        launch_dw(l->xt[i], l->dy_b[i], l->partial[i], l->F[i], l->Nout[i], trunk_bn(l, i), chunks, splits[i], cps[i], st);
         if (i == 0) break;
         dmk::MlpGemmParams X{};
         X.a_tiles = l->dy_a[i]; X.w_tiles = l->wt[i]; X.M = rows; X.K = l->Nout[i]; X.N = l->Nout[i - 1];
@@ -587,58 +582,42 @@ int dm_learn_set_weights(dm_learn* l, const dm_learn_net* net, void* stream) {
     if (learn_net_check(net, "dm_learn_set_weights")) return 1;
     if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_set_weights: cudaSetDevice failed");
     if (l->kind == 2) learn_disc_layers(l, net, nullptr, nullptr, nullptr, static_cast<cudaStream_t>(stream));
-    else learn_layers(l, net, nullptr, 0, nullptr, static_cast<cudaStream_t>(stream));
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return mlp_fail(std::string("dm_learn_set_weights: ") + cudaGetErrorString(e));
-    return 0;
+    else learn_layers(l, net, nullptr, nullptr, static_cast<cudaStream_t>(stream));
+    return launch_status("dm_learn_set_weights");
 }
 
 int dm_learn_step(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, void* stream) {
+    const char* fn = "dm_learn_step";
     if (!l) return mlp_fail("dm_learn_step: null handle");
     if (l->gated) return mlp_fail("dm_learn_step: the workspace holds a gated network (dm_learn_create_gated); use dm_learn_gated_step");
     if (l->kind == 2) return mlp_fail("dm_learn_step: the workspace is a discriminator's (kind 2); use dm_learn_disc_step");
-    if (learn_net_check(net, "dm_learn_step")) return 1;
-    if (!b) return mlp_fail("dm_learn_step: null batch");
-    if (b->rows <= 0 || b->rows > l->max_rows) return mlp_fail("dm_learn_step: rows out of range");
-    if (!b->states || !b->idx || !b->in_mean || !b->in_istd || !b->stats) return mlp_fail("dm_learn_step: null state, index, normaliser or statistics pointer");
-    if (l->actor && (!b->norm_actions || !b->old_logp || !b->adv || !b->logstd || !b->bound_min || !b->bound_max))
-        return mlp_fail("dm_learn_step: null action, log-probability, advantage, log-std or bound pointer");
-    if (!l->actor && !b->norm_targets) return mlp_fail("dm_learn_step: null target pointer");
-    if (l->actor && !(b->ratio_clip > 0.f)) return mlp_fail("dm_learn_step: ratio_clip must be positive");
-    if (!(b->stepsize >= 0.f) || !(b->momentum >= 0.f) || !(b->weight_decay >= 0.f)) return mlp_fail("dm_learn_step: stepsize, momentum and weight_decay must be >= 0");
+    if (learn_net_check(net, fn) || ppo_batch_check(fn, l, b, nullptr)) return 1;
     dm_mlp* m = l->m;
     if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_learn_step: cudaSetDevice failed");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int rows = b->rows, mt = (rows + 127) / 128, chunks = 2 * mt;
     // split-K of the three dW GEMMs for this row count (the workspace holds the largest over every row count, dm_learn_create)
     int splits[3], cps[3];
-    for (int i = 0; i < 3; ++i) {
-        dw_split((l->F[i] / 128) * (l->Nout[i] / (i == 2 ? m->N2 : 128)), chunks, &splits[i], &cps[i]);
-        if (splits[i] > l->max_splits[i]) return mlp_fail("dm_learn_step: internal error: dW split count exceeds the workspace");
-    }
+    for (int i = 0; i < 3; ++i)
+        if (dw_plan(fn, l->F[i], l->Nout[i], trunk_bn(l, i), chunks, l->max_splits[i], &splits[i], &cps[i])) return 1;
     // forward: gathered rows -> the plain trunk -> the normalised output (identity output normaliser)
     dmk::LearnPrepParams Q{b->states, b->idx, b->in_mean, b->in_istd, b->in_clip > 0.f ? b->in_clip : 1e30f, m->in_dim, rows, m->K0 / 64, m->obs_t};
     dmk::dm_learn_prep_kernel<<<dim3(mt, m->K0 / 64), 128, 0, st>>>(Q);
     learn_forward(l, rows, mt, st);
     // loss head: dY of the output layer, the loss partials, the statistics
-    dmk::LearnHeadParams H{l->out, b->idx, rows, m->out_dim, l->dy_a[2], l->dy_b[2], l->head_partials, b->norm_actions, b->old_logp, b->adv, b->logstd,
-                           b->bound_min, b->bound_max, b->ratio_clip, b->ratio, b->norm_targets};
-    if (l->actor) dmk::dm_learn_actor_head_kernel<<<mt, 128, 0, st>>>(H);
-    else dmk::dm_learn_critic_head_kernel<<<mt, 128, 0, st>>>(H);
-    dmk::dm_learn_stats_kernel<<<1, 1, 0, st>>>(l->head_partials, mt, 1.f / rows, l->actor ? 1 : 0, b->stats);
+    launch_ppo_head(l, b, mt, st);
     learn_backward(l, rows, mt, splits, cps, st);
     // optimiser step and re-tiling, after every GEMM that read the old weights
-    learn_layers(l, net, b, rows, splits, st);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return mlp_fail(std::string("dm_learn_step: ") + cudaGetErrorString(e));
-    return 0;
+    learn_layers(l, net, b, splits, st);
+    return launch_status(fn);
 }
 
 int dm_learn_disc_step(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* b, void* stream) {
+    const char* fn = "dm_learn_disc_step";
     if (!l) return mlp_fail("dm_learn_disc_step: null handle");
     if (l->gated) return mlp_fail("dm_learn_disc_step: the workspace holds a gated network (dm_learn_create_gated); a discriminator step needs kind 2");
     if (l->kind != 2) return mlp_fail("dm_learn_disc_step: the workspace is a PPO actor's or critic's (kind 0 or 1); a discriminator step needs kind 2");
-    if (learn_net_check(net, "dm_learn_disc_step")) return 1;
+    if (learn_net_check(net, fn)) return 1;
     if (!b) return mlp_fail("dm_learn_disc_step: null batch");
     if (b->rows <= 0 || b->rows > l->side_rows) return mlp_fail("dm_learn_disc_step: rows out of range (1 to max_rows / 2 per side)");
     if (!b->agent || !b->expert || !b->agent_idx || !b->expert_idx || !b->in_mean || !b->in_istd || !b->stats)
@@ -650,18 +629,16 @@ int dm_learn_disc_step(dm_learn* l, const dm_learn_net* net, const dm_learn_disc
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     // agent rows in m tiles [0, et), expert rows in [et, 2 et)
     const int rows = b->rows, E = pad_to(rows, 128), et = E / 128, mt = 2 * et, chunks = 2 * mt, echunks = 2 * et;
-    const int BN[3] = {128, 128, m->N2};
     int splits[3], cps[3], psplits[3], pcps[3];
-    for (int i = 0; i < 3; ++i) {
-        dw_split((l->F[i] / 128) * (l->Nout[i] / BN[i]), chunks, &splits[i], &cps[i]);
-        dw_split((l->pen_F[i] / 128) * (l->Nout[i] / BN[i]), echunks, &psplits[i], &pcps[i]);
-        if (splits[i] > l->max_splits[i] || psplits[i] > l->pen_max_splits[i]) return mlp_fail("dm_learn_disc_step: internal error: dW split count exceeds the workspace");
-    }
+    for (int i = 0; i < 3; ++i)
+        if (dw_plan(fn, l->F[i], l->Nout[i], trunk_bn(l, i), chunks, l->max_splits[i], &splits[i], &cps[i]) ||
+            dw_plan(fn, l->pen_F[i], l->Nout[i], trunk_bn(l, i), echunks, l->pen_max_splits[i], &psplits[i], &pcps[i]))
+            return 1;
     // forward over both sides: each gathered into its own m tiles
     const int NC0 = m->K0 / 64;
     dmk::LearnPrepParams Q{b->agent, b->agent_idx, b->in_mean, b->in_istd, b->in_clip > 0.f ? b->in_clip : 1e30f, m->in_dim, rows, NC0, m->obs_t};
     dmk::dm_learn_prep_kernel<<<dim3(et, NC0), 128, 0, st>>>(Q);
-    Q.x = b->expert; Q.idx = b->expert_idx; Q.tiles = m->obs_t + static_cast<size_t>(et) * NC0 * dmk::kMlpATileHalves;
+    Q.x = b->expert; Q.idx = b->expert_idx; Q.tiles = m->obs_t + static_cast<size_t>(et) * NC0 * dmk::kMlpATile;
     dmk::dm_learn_prep_kernel<<<dim3(et, NC0), 128, 0, st>>>(Q);
     learn_forward(l, 2 * E, mt, st);
     // least-squares head: dY of the logit over both sides, the penalty's seed over the expert rows, the partials
@@ -669,7 +646,7 @@ int dm_learn_disc_step(dm_learn* l, const dm_learn_net* net, const dm_learn_disc
     dmk::dm_learn_disc_head_kernel<<<mt, 128, 0, st>>>(H);
     learn_backward(l, 2 * E, mt, splits, cps, st);
     // the gradient penalty on the expert tiles, with the forward's masks: u1 = m1 w2, u0 = m0 (W1^T u1) (hi + lo A and B operands) ...
-    const size_t tile = dmk::kMlpATileHalves;
+    const size_t tile = dmk::kMlpATile;
     const __half* act0e = m->act0 + static_cast<size_t>(et) * (m->N0 / 64) * tile;
     const __half* act1e = m->act1 + static_cast<size_t>(et) * (m->N1 / 64) * tile;
     dmk::MlpGemmParams X{};
@@ -692,20 +669,11 @@ int dm_learn_disc_step(dm_learn* l, const dm_learn_net* net, const dm_learn_disc
                                       {-1, -1, -1}, {l->pen_F[0], l->pen_F[1], l->pen_F[2]}, echunks};
     dmk::dm_learn_transpose_kernel<<<dim3(std::max(l->pen_F[0], std::max(l->pen_F[1], l->pen_F[2])) / 128, echunks, 3), 256, 0, st>>>(T);
     const __half* pen_b[3] = {l->u_b[0], l->u_b[1], l->seed_b};
-    for (int i = 0; i < 3; ++i) {
-        dmk::MlpGemmParams W{};
-        W.a_tiles = l->pt[i]; W.w_tiles = pen_b[i]; W.M = l->pen_F[i]; W.N = l->Nout[i];
-        const dmk::MlpGradParams GW{nullptr, nullptr, nullptr, l->pen[i], echunks, pcps[i]};
-        const dim3 gw(l->pen_F[i] / 128, l->Nout[i] / BN[i], psplits[i]);
-        if (i == 2) dmk::dm_mlp_grad_w_kernel<64><<<gw, 256, dmk::dm_mlp_smem_bytes(64), st>>>(W, GW);
-        else dmk::dm_mlp_grad_w_kernel<128><<<gw, 256, dmk::dm_mlp_smem_bytes(128), st>>>(W, GW);
-    }
+    for (int i = 0; i < 3; ++i) launch_dw(l->pt[i], pen_b[i], l->pen[i], l->pen_F[i], l->Nout[i], trunk_bn(l, i), echunks, psplits[i], pcps[i], st);
     dmk::dm_learn_disc_stats_kernel<<<1, 1, 0, st>>>(l->head_partials, mt, l->gp_partials, et, 1.f / rows, b->stats);
     // optimiser step and re-tiling, after every GEMM that read the old weights
     learn_disc_layers(l, net, b, splits, psplits, st);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return mlp_fail(std::string("dm_learn_disc_step: ") + cudaGetErrorString(e));
-    return 0;
+    return launch_status(fn);
 }
 
 dm_learn* dm_learn_create_gated(int device, int kind, int in_dim, int goal_dim, int h0, int h1, int out_dim, int gate_common, int gate_hidden, int max_rows) {
@@ -732,35 +700,14 @@ dm_learn* dm_learn_create_gated(int device, int kind, int in_dim, int goal_dim, 
     dm_mlp* m = create_gated("dm_learn_create_gated", device, &g, max_rows, 128);
     if (!m) return nullptr;   // dm_last_error is set
     dm_learn* l = new dm_learn();
-    l->m = m; l->gated = true; l->actor = kind == 0; l->kind = kind; l->max_rows = m->max_rows;
-    const int N0 = m->N0, N1 = m->N1, in[3] = {trunk_in, h0, h1}, chunks = m->max_rows / 64;
-    l->Nout[0] = N0; l->Nout[1] = N1; l->Nout[2] = m->N2;
+    l->m = m; l->gated = true; l->kind = kind; l->max_rows = m->max_rows;
+    const int N0 = m->N0, N1 = m->N1, in[3] = {trunk_in, h0, h1};
     const int gF[4] = {128, 128, pad_to(GC + 1, 128), 128}, gN[4] = {2 * N0, 2 * N1, 128, 128};
-    // the largest split count over every minibatch a step may take (dm_learn_create)
-    auto max_splits = [&](int tiles) {
-        int mx = 0;
-        for (int c = 2; c <= chunks; c += 2) {
-            int s = 0, cps = 0;
-            dw_split(tiles, c, &s, &cps);
-            mx = std::max(mx, s);
-        }
-        return mx;
-    };
     const size_t R = m->max_rows, h = sizeof(__half);
     l->KS = (2 * N0 + 2 * N1) / 64;
-    bool ok = cudaMalloc(&l->out, R * out_dim * sizeof(float)) == cudaSuccess && cudaMalloc(&l->head_partials, R / 128 * 3 * sizeof(float)) == cudaSuccess;
-    for (int i = 0; i < 3 && ok; ++i) {
-        l->F[i] = pad_to(in[i] + 1, 128);
-        l->max_splits[i] = max_splits((l->F[i] / 128) * (l->Nout[i] / (i == 2 ? m->N2 : 128)));
-        ok = cudaMalloc(&l->xt[i], R * l->F[i] * h) == cudaSuccess && cudaMalloc(&l->dy_b[i], 2 * R * l->Nout[i] * h) == cudaSuccess &&
-             cudaMalloc(&l->partial[i], static_cast<size_t>(l->max_splits[i]) * l->Nout[i] * l->F[i] * sizeof(float)) == cudaSuccess;
-        if (ok && i > 0) {
-            const size_t n = 2 * static_cast<size_t>(l->Nout[i]) * l->Nout[i - 1];
-            ok = cudaMalloc(&l->dy_a[i], 2 * R * l->Nout[i] * h) == cudaSuccess && cudaMalloc(&l->wt[i], n * h) == cudaSuccess && cudaMemset(l->wt[i], 0, n * h) == cudaSuccess;
-        }
-    }
+    bool ok = trunk_workspace(l, in);
     for (int j = 0; j < 4 && ok; ++j) {
-        l->gF[j] = gF[j]; l->gN[j] = gN[j]; l->g_max_splits[j] = max_splits((gF[j] / 128) * (gN[j] / 128));
+        l->gF[j] = gF[j]; l->gN[j] = gN[j]; l->g_max_splits[j] = dw_max_splits(gF[j], gN[j], 128, m->max_rows / 64);
         ok = cudaMalloc(&l->gxt[j], R * gF[j] * h) == cudaSuccess && cudaMalloc(&l->gdy_b[j], 2 * R * gN[j] * h) == cudaSuccess &&
              cudaMalloc(&l->gpartial[j], static_cast<size_t>(l->g_max_splits[j]) * gN[j] * gF[j] * sizeof(float)) == cudaSuccess;
     }
@@ -774,10 +721,7 @@ dm_learn* dm_learn_create_gated(int device, int kind, int in_dim, int goal_dim, 
          cudaMalloc(&l->dg_a, 2 * R * 128 * h) == cudaSuccess && cudaMalloc(&l->wght, wght * h) == cudaSuccess && cudaMemset(l->wght, 0, wght * h) == cudaSuccess;
     if (ok) {
         ok = cudaFuncSetAttribute(dmk::dm_mlp_gated_save_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess &&
-             cudaFuncSetAttribute(dmk::dm_mlp_grad_xg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
-             cudaFuncSetAttribute(dmk::dm_mlp_grad_x_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
-             cudaFuncSetAttribute(dmk::dm_mlp_grad_w_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
-             cudaFuncSetAttribute(dmk::dm_mlp_grad_w_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess;
+             cudaFuncSetAttribute(dmk::dm_mlp_grad_xg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess;
     }
     if (!ok) { mlp_fail(std::string("dm_learn_create_gated: ") + cudaGetErrorString(cudaGetLastError())); dm_learn_destroy(l); return nullptr; }
     return l;
@@ -796,7 +740,7 @@ int t_chunk(const dm_learn* l, int layer) { return s_chunk(l, layer) + (layer ? 
 // the ten layer passes of a gated workspace: the forward tiles, and the B operands of the dX GEMMs (W1^T, W2^T, the block-diagonal
 // [Ws_l^T, Wt_l^T], [Wgh_0 | Wgh_1]^T); with `b` also the optimiser step on the dW partials (split counts: splits for the trunk, gsplits
 // for the gate's GEMMs)
-void learn_gated_layers(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_batch* b, int rows, const int* splits, const int* gsplits, cudaStream_t st) {
+void learn_gated_layers(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_batch* b, const int* splits, const int* gsplits, cudaStream_t st) {
     dm_mlp* m = l->m;
     const size_t tt = 2 * 128 * 64;   // halves of a hi + lo 128 x 64 B tile
     for (int i = 0; i < 10; ++i) {
@@ -817,10 +761,7 @@ void learn_gated_layers(dm_learn* l, const dm_learn_gated_net* net, const dm_lea
             L.t_tiles = l->wst + static_cast<size_t>(scale ? s_chunk(l, lay) : t_chunk(l, lay)) * tt + 512 * lay; L.t_NC = l->KS;
             L.partial = l->gpartial[lay] + (scale ? 0 : static_cast<size_t>(N) * l->gF[lay]); L.Npad = 2 * N; L.F = l->gF[lay]; s = b ? gsplits[lay] : 0;
         }
-        if (b) {
-            L.acc_w = net->acc_w[i]; L.acc_b = net->acc_b[i]; L.splits = s;
-            L.inv_rows = 1.f / rows; L.lr = b->stepsize; L.mom = b->momentum; L.wd = b->weight_decay;
-        }
+        if (b) optimiser_fields(L, net, i, b, s);
         launch_layer(L, st);
     }
 }
@@ -828,21 +769,8 @@ void learn_gated_layers(dm_learn* l, const dm_learn_gated_net* net, const dm_lea
 // transposition of the saved activations into the dW GEMMs' A operands
 void learn_gated_forward(dm_learn* l, int rows, int mt, cudaStream_t st) {
     dm_mlp* m = l->m;
-    const size_t tile = dmk::kMlpATileHalves;
-    dmk::MlpGemmParams P{};
-    P.M = rows;
-    P.a_tiles = m->goal_t; P.w_tiles = m->wgc; P.bias = m->bgc; P.out_tiles = m->gc_t; P.K = 64; P.N = 128;
-    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
-    P.a_tiles = m->gc_t; P.w_tiles = m->wgh; P.bias = m->bgh; P.out_tiles = m->gh_t; P.K = 128; P.N = 128;
-    dmk::dm_mlp_gemm_kernel<128, false><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(128), st>>>(P);
-    P.gate_stride = 2 * tile;
-    P.a_tiles = m->obs_t; P.w_tiles = m->w[0]; P.bias = m->b[0]; P.out_tiles = m->act0; P.K = m->K0; P.N = m->N0;
-    P.gate_tiles = m->gh_t; P.ws_tiles = m->wgs[0]; P.wb_tiles = m->wgb[0]; P.bias_s = m->bgs[0]; P.bias_b = m->bgb[0];
-    dmk::dm_mlp_gated_save_kernel<<<dim3(mt, m->N0 / 64), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P, dmk::MlpGateParams{l->fa[0], l->fb[0], nullptr, 0, 0, 0, nullptr});
-    P.a_tiles = m->act0; P.w_tiles = m->w[1]; P.bias = m->b[1]; P.out_tiles = m->act1; P.K = m->N0; P.N = m->N1;
-    P.gate_tiles = m->gh_t + tile; P.ws_tiles = m->wgs[1]; P.wb_tiles = m->wgb[1]; P.bias_s = m->bgs[1]; P.bias_b = m->bgb[1];
-    dmk::dm_mlp_gated_save_kernel<<<dim3(mt, m->N1 / 64), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P, dmk::MlpGateParams{l->fa[1], l->fb[1], nullptr, 0, 0, 0, nullptr});
-    P.a_tiles = m->act1; P.w_tiles = m->w[2]; P.bias = m->b[2]; P.out_tiles = nullptr; P.K = m->N1; P.N = m->N2;
+    const dmk::MlpGateParams save[2] = {{l->fa[0], l->fb[0], nullptr, 0, 0, 0, nullptr}, {l->fa[1], l->fb[1], nullptr, 0, 0, 0, nullptr}};
+    dmk::MlpGemmParams P = gated_hidden(m, rows, save, st);
     P.actions = l->out; P.out_mean = m->out_mean; P.out_std = m->out_std; P.noise = nullptr; P.out_dim = m->out_dim;
     dmk::dm_mlp_gemm_kernel<64, true><<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(64), st>>>(P);
     // [ns | ng], h_0, h_1; then ng, gc, g_0 (chunk 0 of gh_t) and g_1 (chunk 1: a two-chunk source whose second chunk is never used, hence
@@ -854,7 +782,7 @@ void learn_gated_forward(dm_learn* l, int rows, int mt, cudaStream_t st) {
     const dmk::LearnTransposeParams G{{m->goal_t, m->gc_t, m->gh_t}, {l->gxt[3], l->gxt[2], l->gxt[0]}, {1, 2, 2}, {m->goal_dim, m->gate_common, m->gate_hidden},
                                       {l->gF[3], l->gF[2], l->gF[0]}, chunks};
     dmk::dm_learn_transpose_kernel<<<dim3(l->gF[2] / 128, chunks, 3), 256, 0, st>>>(G);
-    const dmk::LearnTransposeParams G1{{m->gh_t + tile, nullptr, nullptr}, {l->gxt[1], nullptr, nullptr}, {2, 0, 0}, {m->gate_hidden, 0, 0}, {l->gF[1], 0, 0}, chunks};
+    const dmk::LearnTransposeParams G1{{m->gh_t + dmk::kMlpATile, nullptr, nullptr}, {l->gxt[1], nullptr, nullptr}, {2, 0, 0}, {m->gate_hidden, 0, 0}, {l->gF[1], 0, 0}, chunks};
     dmk::dm_learn_transpose_kernel<<<dim3(1, chunks, 1), 256, 0, st>>>(G1);
 }
 // the gated backward of the dY a head wrote into dy_a[2] / dy_b[2] (DESIGN.md section 8): dX GEMMs output -> h_1 -> h_0 with the gated
@@ -862,32 +790,25 @@ void learn_gated_forward(dm_learn* l, int rows, int mt, cudaStream_t st) {
 void learn_gated_backward(dm_learn* l, int mt, const int* splits, const int* cps, const int* gsplits, const int* gcps, cudaStream_t st) {
     dm_mlp* m = l->m;
     const int chunks = 2 * mt, N0 = m->N0, N1 = m->N1;
-    auto dw = [&](const __half* a, const __half* b, float* part, int F, int N, int BN, int s, int c) {
-        dmk::MlpGemmParams W{};
-        W.a_tiles = a; W.w_tiles = b; W.M = F; W.N = N;
-        const dmk::MlpGradParams GW{nullptr, nullptr, nullptr, part, chunks, c};
-        if (BN == 64) dmk::dm_mlp_grad_w_kernel<64><<<dim3(F / 128, N / 64, s), 256, dmk::dm_mlp_smem_bytes(64), st>>>(W, GW);
-        else dmk::dm_mlp_grad_w_kernel<128><<<dim3(F / 128, N / 128, s), 256, dmk::dm_mlp_smem_bytes(128), st>>>(W, GW);
-    };
-    dw(l->xt[2], l->dy_b[2], l->partial[2], l->F[2], m->N2, m->N2, splits[2], cps[2]);
+    launch_dw(l->xt[2], l->dy_b[2], l->partial[2], l->F[2], m->N2, m->N2, chunks, splits[2], cps[2], st);
     dmk::MlpGemmParams X{};
     X.a_tiles = l->dy_a[2]; X.w_tiles = l->wt[2]; X.K = m->N2; X.N = N1;
     dmk::dm_mlp_grad_xg_kernel<<<dim3(mt, N1 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(
         X, dmk::MlpGradParams{m->act1, l->dy_a[1], l->dy_b[1], nullptr, chunks, 0}, dmk::MlpGateParams{l->fa[1], l->fb[1], l->st_a, l->KS, s_chunk(l, 1), t_chunk(l, 1), l->gdy_b[1]});
-    dw(l->xt[1], l->dy_b[1], l->partial[1], l->F[1], N1, 128, splits[1], cps[1]);
-    dw(l->gxt[1], l->gdy_b[1], l->gpartial[1], l->gF[1], l->gN[1], 128, gsplits[1], gcps[1]);
+    launch_dw(l->xt[1], l->dy_b[1], l->partial[1], l->F[1], N1, 128, chunks, splits[1], cps[1], st);
+    launch_dw(l->gxt[1], l->gdy_b[1], l->gpartial[1], l->gF[1], l->gN[1], 128, chunks, gsplits[1], gcps[1], st);
     X.a_tiles = l->dy_a[1]; X.w_tiles = l->wt[1]; X.K = N1; X.N = N0;
     dmk::dm_mlp_grad_xg_kernel<<<dim3(mt, N0 / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(
         X, dmk::MlpGradParams{m->act0, nullptr, l->dy_b[0], nullptr, chunks, 0}, dmk::MlpGateParams{l->fa[0], l->fb[0], l->st_a, l->KS, s_chunk(l, 0), t_chunk(l, 0), l->gdy_b[0]});
-    dw(l->xt[0], l->dy_b[0], l->partial[0], l->F[0], N0, 128, splits[0], cps[0]);
-    dw(l->gxt[0], l->gdy_b[0], l->gpartial[0], l->gF[0], l->gN[0], 128, gsplits[0], gcps[0]);
+    launch_dw(l->xt[0], l->dy_b[0], l->partial[0], l->F[0], N0, 128, chunks, splits[0], cps[0], st);
+    launch_dw(l->gxt[0], l->gdy_b[0], l->gpartial[0], l->gF[0], l->gN[0], 128, chunks, gsplits[0], gcps[0], st);
     // [dg_0 | dg_1] = ([ds_0 | dt_0 | ds_1 | dt_1] x block-diagonal [Ws_l^T; Wt_l^T]) * 1[g > 0], in gh_t's layout; dgc = ([dg_0 | dg_1] Wgh) * 1[gc > 0]
     X.a_tiles = l->st_a; X.w_tiles = l->wst; X.K = l->KS * 64; X.N = 128;
     dmk::dm_mlp_grad_x_kernel<<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(128), st>>>(X, dmk::MlpGradParams{m->gh_t, l->dg_a, l->gdy_b[2], nullptr, chunks, 0});
-    dw(l->gxt[2], l->gdy_b[2], l->gpartial[2], l->gF[2], 128, 128, gsplits[2], gcps[2]);
+    launch_dw(l->gxt[2], l->gdy_b[2], l->gpartial[2], l->gF[2], 128, 128, chunks, gsplits[2], gcps[2], st);
     X.a_tiles = l->dg_a; X.w_tiles = l->wght; X.K = 128; X.N = 128;
     dmk::dm_mlp_grad_x_kernel<<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(128), st>>>(X, dmk::MlpGradParams{m->gc_t, nullptr, l->gdy_b[3], nullptr, chunks, 0});
-    dw(l->gxt[3], l->gdy_b[3], l->gpartial[3], l->gF[3], 128, 128, gsplits[3], gcps[3]);
+    launch_dw(l->gxt[3], l->gdy_b[3], l->gpartial[3], l->gF[3], 128, 128, chunks, gsplits[3], gcps[3], st);
 }
 }  // namespace
 
@@ -896,56 +817,36 @@ int dm_learn_set_gated_weights(dm_learn* l, const dm_learn_gated_net* net, void*
     if (!l->gated) return mlp_fail("dm_learn_set_gated_weights: the workspace holds a plain network (dm_learn_create); use dm_learn_set_weights");
     if (gated_net_check(net, "dm_learn_set_gated_weights")) return 1;
     if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_set_gated_weights: cudaSetDevice failed");
-    learn_gated_layers(l, net, nullptr, 0, nullptr, nullptr, static_cast<cudaStream_t>(stream));
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return mlp_fail(std::string("dm_learn_set_gated_weights: ") + cudaGetErrorString(e));
-    return 0;
+    learn_gated_layers(l, net, nullptr, nullptr, nullptr, static_cast<cudaStream_t>(stream));
+    return launch_status("dm_learn_set_gated_weights");
 }
 
 int dm_learn_gated_step(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_gated_batch* gb, void* stream) {
+    const char* fn = "dm_learn_gated_step";
     if (!l) return mlp_fail("dm_learn_gated_step: null handle");
     if (!l->gated) return mlp_fail("dm_learn_gated_step: the workspace holds a plain network (dm_learn_create); use dm_learn_step");
-    if (gated_net_check(net, "dm_learn_gated_step")) return 1;
-    if (!gb) return mlp_fail("dm_learn_gated_step: null batch");
-    const dm_learn_batch* b = &gb->batch;
-    if (b->rows <= 0 || b->rows > l->max_rows) return mlp_fail("dm_learn_gated_step: rows out of range");
-    if (!b->states || !b->idx || !b->in_mean || !b->in_istd || !b->stats || !gb->goals || !gb->g_mean || !gb->g_istd)
-        return mlp_fail("dm_learn_gated_step: null state, goal, index, normaliser or statistics pointer");
-    if (l->actor && (!b->norm_actions || !b->old_logp || !b->adv || !b->logstd || !b->bound_min || !b->bound_max))
-        return mlp_fail("dm_learn_gated_step: null action, log-probability, advantage, log-std or bound pointer");
-    if (!l->actor && !b->norm_targets) return mlp_fail("dm_learn_gated_step: null target pointer");
-    if (l->actor && !(b->ratio_clip > 0.f)) return mlp_fail("dm_learn_gated_step: ratio_clip must be positive");
-    if (!(b->stepsize >= 0.f) || !(b->momentum >= 0.f) || !(b->weight_decay >= 0.f)) return mlp_fail("dm_learn_gated_step: stepsize, momentum and weight_decay must be >= 0");
+    const dm_learn_batch* b = gb ? &gb->batch : nullptr;
+    if (gated_net_check(net, fn) || ppo_batch_check(fn, l, b, gb)) return 1;
     dm_mlp* m = l->m;
     if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_learn_gated_step: cudaSetDevice failed");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int rows = b->rows, mt = (rows + 127) / 128, chunks = 2 * mt;
     int splits[3], cps[3], gsplits[4], gcps[4];
-    for (int i = 0; i < 3; ++i) {
-        dw_split((l->F[i] / 128) * (l->Nout[i] / (i == 2 ? m->N2 : 128)), chunks, &splits[i], &cps[i]);
-        if (splits[i] > l->max_splits[i]) return mlp_fail("dm_learn_gated_step: internal error: dW split count exceeds the workspace");
-    }
-    for (int j = 0; j < 4; ++j) {
-        dw_split((l->gF[j] / 128) * (l->gN[j] / 128), chunks, &gsplits[j], &gcps[j]);
-        if (gsplits[j] > l->g_max_splits[j]) return mlp_fail("dm_learn_gated_step: internal error: dW split count exceeds the workspace");
-    }
+    for (int i = 0; i < 3; ++i)
+        if (dw_plan(fn, l->F[i], l->Nout[i], trunk_bn(l, i), chunks, l->max_splits[i], &splits[i], &cps[i])) return 1;
+    for (int j = 0; j < 4; ++j)
+        if (dw_plan(fn, l->gF[j], l->gN[j], 128, chunks, l->g_max_splits[j], &gsplits[j], &gcps[j])) return 1;
     // forward: gathered [state | goal] rows and goals -> the gated network -> the normalised output (identity output normaliser)
     const dmk::LearnPrepParams Q{b->states, b->idx, b->in_mean, b->in_istd, b->in_clip > 0.f ? b->in_clip : 1e30f, m->in_dim, rows, m->K0 / 64, m->obs_t};
     const dmk::LearnGoalParams Qg{gb->goals, gb->g_mean, gb->g_istd, gb->g_clip > 0.f ? gb->g_clip : 1e30f, m->goal_dim, m->goal_t};
     dmk::dm_learn_gated_prep_kernel<<<dim3(mt, m->K0 / 64 + 1), 128, 0, st>>>(Q, Qg);
     learn_gated_forward(l, rows, mt, st);
     // the loss heads act on the output only: the plain step's
-    dmk::LearnHeadParams H{l->out, b->idx, rows, m->out_dim, l->dy_a[2], l->dy_b[2], l->head_partials, b->norm_actions, b->old_logp, b->adv, b->logstd,
-                           b->bound_min, b->bound_max, b->ratio_clip, b->ratio, b->norm_targets};
-    if (l->actor) dmk::dm_learn_actor_head_kernel<<<mt, 128, 0, st>>>(H);
-    else dmk::dm_learn_critic_head_kernel<<<mt, 128, 0, st>>>(H);
-    dmk::dm_learn_stats_kernel<<<1, 1, 0, st>>>(l->head_partials, mt, 1.f / rows, l->actor ? 1 : 0, b->stats);
+    launch_ppo_head(l, b, mt, st);
     learn_gated_backward(l, mt, splits, cps, gsplits, gcps, st);
     // optimiser step and re-tiling, after every GEMM that read the old weights
-    learn_gated_layers(l, net, b, rows, splits, gsplits, st);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return mlp_fail(std::string("dm_learn_gated_step: ") + cudaGetErrorString(e));
-    return 0;
+    learn_gated_layers(l, net, b, splits, gsplits, st);
+    return launch_status(fn);
 }
 
 int dm_mlp_set_gated_weights_device(dm_mlp* m, const float* const* d_w, const float* const* d_b, void* stream) {
@@ -957,9 +858,7 @@ int dm_mlp_set_gated_weights_device(dm_mlp* m, const float* const* d_w, const fl
     if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_mlp_set_gated_weights_device: cudaSetDevice failed");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     for (int i = 0; i < 10; ++i) launch_layer(gated_layer_params(m, i, d_w[i], d_b[i]), st);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return mlp_fail(std::string("dm_mlp_set_gated_weights_device: ") + cudaGetErrorString(e));
-    return 0;
+    return launch_status("dm_mlp_set_gated_weights_device");
 }
 
 int dm_mlp_set_gated_normalizers_device(dm_mlp* m, const float* d_s_mean, const float* d_s_std, const float* d_g_mean, const float* d_g_std, const float* d_out_mean,
@@ -972,9 +871,7 @@ int dm_mlp_set_gated_normalizers_device(dm_mlp* m, const float* d_s_mean, const 
     dmk::dm_learn_norm_kernel<<<(m->in_dim + 255) / 256, 256, 0, st>>>(d_s_mean, d_s_std, m->in_dim, m->in_mean, m->in_istd, 1);
     dmk::dm_learn_norm_kernel<<<(m->goal_dim + 255) / 256, 256, 0, st>>>(d_g_mean, d_g_std, m->goal_dim, m->g_mean, m->g_istd, 1);
     dmk::dm_learn_norm_kernel<<<(m->out_dim + 255) / 256, 256, 0, st>>>(d_out_mean, d_out_std, m->out_dim, m->out_mean, m->out_std, 0);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return mlp_fail(std::string("dm_mlp_set_gated_normalizers_device: ") + cudaGetErrorString(e));
-    return 0;
+    return launch_status("dm_mlp_set_gated_normalizers_device");
 }
 
 void dm_learn_destroy(dm_learn* l) {
