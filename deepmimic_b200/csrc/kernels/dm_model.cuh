@@ -1,4 +1,4 @@
-// Flat, immutable device model ("model blob") and per-environment state layout for the batched
+// Flat, immutable device model ("model blob"), per-environment state layout and the kernel interface of the batched
 // DeepMimic step.  Everything the kernels need about a character / controller / clip is
 // pre-digested on the host (capi.cu: build_device_model) from the reference's asset files:
 //   multibody frames + inertias  <- cSimCharacter::BuildMultiBody   (R/DeepMimicCore/sim/SimCharacter.cpp:789-946)
@@ -68,7 +68,7 @@ struct DevModel {
     // AMP task scenes (dm_task.cuh); task_kind == kTaskNone for imitate / imitate_amp
     int task_kind;
     TaskParams task;
-    unsigned long long task_seed, env_id_base;   // draw stream: u01(task_seed, env_id_base + env, k)
+    unsigned long long task_seed, env_id_base;   // draw stream: task_u01(task_seed, env_id_base + env, k)
     TaskExtParams taskx;                          // heading_amp_getup / strike_amp (dm_task_ext.cuh)
     int test_mode, pad_task_;                     // cRLScene::eMode, kept current by dm_set_mode in the task scenes
     DevLink link[kMaxLinks];
@@ -163,5 +163,25 @@ struct StepLayout {
     int oU, oR, oA, oW, oV, oY, oLam, oRhs, oInv, oRl, oPp, oPi, oPr, oQ, oG, oZ;
     int env_floats, hot_floats;
 };
+
+// ---- the kernels and host helpers capi.cu launches (defined in dm_step.cu and dm_policy.cu)
+// Every templated kernel is reached through a table indexed by [tile width 16 / 32][variant]; the table is defined next to the kernel, which
+// instantiates it.  Variants: the step kernel's TASK, the observe kernel's CLIPS and the reset kernel's TASKV are "AMP task scene"; the AMP
+// kernel's TASKV is "expert observation drawn from the clip dataset" (agent observations of a task scene use the single-clip variant).
+constexpr int kPolicyBlock = 64;   // threads per block of the observe, AMP and reset kernels
+using StepKernel = void (*)(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout);
+using ObserveKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, ObsFan, int);
+using ResetKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, int, const double*, const double*, const double*,
+                             unsigned long long, unsigned long long, int, const int*);
+using AmpObsKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, float*, int, const double*, int, const int*);
+extern const StepKernel kStepKernels[2][2];
+extern const ObserveKernel kObserveKernels[2][2];
+extern const ResetKernel kResetKernels[2][2];
+extern const AmpObsKernel kAmpObsKernels[2][2];
+__global__ void dm_set_action_kernel(const DevModel*, DevState, const float*, int);
+__global__ void dm_task_reset_kernel(const DevModel*, DevState, int);
+__global__ void dm_task_observe_kernel(const DevModel*, DevState, float*, float*, int);
+int dm_step_layout(int nl, int n, int chain_len, int maxrows, int W, StepLayout* L);
+int dm_step_smem_bytes(const StepLayout& L, int tiles);
 
 }  // namespace dmk

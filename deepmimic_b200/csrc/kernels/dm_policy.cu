@@ -67,13 +67,6 @@ __device__ __forceinline__ void frame_index(const MT& M, const double* ft, doubl
     idx = lo;
     blend = (tt - ft[lo]) / (ft[lo + 1] - ft[lo]);
 }
-// stateless counter-based random numbers (splitmix64 finaliser) -> uniform [0,1)
-__device__ __forceinline__ double u01(unsigned long long seed, unsigned long long a, unsigned long long b) {
-    unsigned long long z = seed + 0x9E3779B97F4A7C15ull * (a * 2654435761ull + b + 1);
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull; z = (z ^ (z >> 27)) * 0x94D049BB133111EBull; z ^= z >> 31;
-    return static_cast<double>(z >> 11) * (1.0 / 9007199254740992.0);
-}
-
 // mocap sample for joint `lane` in DeepMimic pose layout: returns the joint quaternion (w-first stored in the table) as Q4 xyzw,
 // the revolute angle in .x, and the joint velocity
 struct KinJoint { Q4 q; V3 w; float ang, angvel; };
@@ -554,15 +547,15 @@ __global__ void __launch_bounds__(BLOCK) dm_reset_kernel(const DevModel* __restr
         // cSceneImitate::ResetKinChar draws the start time from U(0, duration of the clip that was active BEFORE the controller's reset picks
         // the new one) -- CalcRandKinResetTime runs first (SceneImitate.cpp:331-338)
         reset_time_span = CT.info[prev_clip].dur;
-        new_clip = doit ? (clip_in ? clip_in[env] : select_clip(CT, u01(seed ^ 0x636c697073ull, gid, cnt))) : prev_clip;
+        new_clip = doit ? (clip_in ? clip_in[env] : select_clip(CT, task_u01(seed ^ 0x636c697073ull, gid, cnt))) : prev_clip;
         const ClipInfo& ci = CT.info[new_clip];
         CM = clip_model(ci, M.pose_dim, M.query_dt);
         frame_times += ci.frame_off; frames += static_cast<size_t>(ci.frame_off) * M.pose_dim; frame_vel += static_cast<size_t>(ci.frame_off) * M.pose_dim;
     }
     const auto& KM = ClipPick<TASKV>::get(M, CM);
-    double kt = kin_time_in ? kin_time_in[env] : u01(seed, gid, 3 * cnt) * reset_time_span;
-    double mt = max_time_in ? max_time_in[env] : (M.time_lim_min + u01(seed, gid, 3 * cnt + 1) * (M.time_lim_max - M.time_lim_min));
-    double th = rot_theta_in ? rot_theta_in[env] : (M.rand_rot_reset ? (-3.14159265358979323846 + u01(seed, gid, 3 * cnt + 2) * 6.283185307179586) : 0.0);
+    double kt = kin_time_in ? kin_time_in[env] : task_u01(seed, gid, 3 * cnt) * reset_time_span;
+    double mt = max_time_in ? max_time_in[env] : (M.time_lim_min + task_u01(seed, gid, 3 * cnt + 1) * (M.time_lim_max - M.time_lim_min));
+    double th = rot_theta_in ? rot_theta_in[env] : (M.rand_rot_reset ? (-3.14159265358979323846 + task_u01(seed, gid, 3 * cnt + 2) * 6.283185307179586) : 0.0);
     if (!M.rand_rot_reset) th = 0.0;
     if (test_mode) mt = M.time_end_lim_max;
     if constexpr (TASKV) {
@@ -760,17 +753,11 @@ __global__ void dm_task_observe_kernel(const DevModel* __restrict__ gm, DevState
     }
 }
 
-template __global__ void dm_observe_kernel<16, 64, false>(const DevModel*, DevState, const double*, const float*, const float*, ObsFan, int);
-template __global__ void dm_observe_kernel<32, 64, false>(const DevModel*, DevState, const double*, const float*, const float*, ObsFan, int);
-template __global__ void dm_observe_kernel<16, 64, true>(const DevModel*, DevState, const double*, const float*, const float*, ObsFan, int);
-template __global__ void dm_observe_kernel<32, 64, true>(const DevModel*, DevState, const double*, const float*, const float*, ObsFan, int);
-template __global__ void dm_amp_obs_kernel<16, 64, false>(const DevModel*, DevState, const double*, const float*, const float*, float*, int, const double*, int, const int*);
-template __global__ void dm_amp_obs_kernel<32, 64, false>(const DevModel*, DevState, const double*, const float*, const float*, float*, int, const double*, int, const int*);
-template __global__ void dm_amp_obs_kernel<16, 64, true>(const DevModel*, DevState, const double*, const float*, const float*, float*, int, const double*, int, const int*);
-template __global__ void dm_amp_obs_kernel<32, 64, true>(const DevModel*, DevState, const double*, const float*, const float*, float*, int, const double*, int, const int*);
-template __global__ void dm_reset_kernel<16, 64, false>(const DevModel*, DevState, const double*, const float*, const float*, int, const double*, const double*, const double*, unsigned long long, unsigned long long, int, const int*);
-template __global__ void dm_reset_kernel<32, 64, false>(const DevModel*, DevState, const double*, const float*, const float*, int, const double*, const double*, const double*, unsigned long long, unsigned long long, int, const int*);
-template __global__ void dm_reset_kernel<16, 64, true>(const DevModel*, DevState, const double*, const float*, const float*, int, const double*, const double*, const double*, unsigned long long, unsigned long long, int, const int*);
-template __global__ void dm_reset_kernel<32, 64, true>(const DevModel*, DevState, const double*, const float*, const float*, int, const double*, const double*, const double*, unsigned long long, unsigned long long, int, const int*);
+const ObserveKernel kObserveKernels[2][2] = {{dm_observe_kernel<16, kPolicyBlock, false>, dm_observe_kernel<16, kPolicyBlock, true>},
+                                             {dm_observe_kernel<32, kPolicyBlock, false>, dm_observe_kernel<32, kPolicyBlock, true>}};
+const ResetKernel kResetKernels[2][2] = {{dm_reset_kernel<16, kPolicyBlock, false>, dm_reset_kernel<16, kPolicyBlock, true>},
+                                         {dm_reset_kernel<32, kPolicyBlock, false>, dm_reset_kernel<32, kPolicyBlock, true>}};
+const AmpObsKernel kAmpObsKernels[2][2] = {{dm_amp_obs_kernel<16, kPolicyBlock, false>, dm_amp_obs_kernel<16, kPolicyBlock, true>},
+                                           {dm_amp_obs_kernel<32, kPolicyBlock, false>, dm_amp_obs_kernel<32, kPolicyBlock, true>}};
 
 }  // namespace dmk

@@ -1542,10 +1542,6 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
 #endif
 }
 
-// explicit instantiations used by capi.cu: (tile width, AMP task scene)
-template __global__ void dm_step_kernel<16, false>(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout);
-template __global__ void dm_step_kernel<32, false>(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout);
-template __global__ void dm_step_kernel<16, true>(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout);
-template __global__ void dm_step_kernel<32, true>(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout);
+const StepKernel kStepKernels[2][2] = {{dm_step_kernel<16, false>, dm_step_kernel<16, true>}, {dm_step_kernel<32, false>, dm_step_kernel<32, true>}};
 
 }  // namespace dmk

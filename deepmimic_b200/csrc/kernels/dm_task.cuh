@@ -2,7 +2,7 @@
 //   cSceneTargetAMP   R/DeepMimicCore/scenes/SceneTargetAMP.cpp   goal, reward, target timer / position, distance failure
 //   cSceneHeadingAMP  R/DeepMimicCore/scenes/SceneHeadingAMP.cpp  goal, reward, heading / speed random walk
 // One thread (lane 0 of the environment's tile) runs these a few times per update, in double like the reference.
-// Random draws: the stateless counter stream of the reset kernel, u01(seed, global env id, k); the per-environment counter k lives in the
+// Random draws: the stateless counter stream of the reset kernel, task_u01(seed, global env id, k); the per-environment counter k lives in the
 // task block.  cRand::RandDouble(a, a) draws nothing; normal draws are Box-Muller on two consecutive uniforms (DESIGN.md section 8).
 #pragma once
 #include <cmath>
@@ -39,7 +39,7 @@ enum TaskSlot {
     kKResetSeen = 13 // reset counter of the environment the block was last initialised for
 };
 
-// splitmix64 finaliser, identical to dm_policy.cu's u01 and to the oracle's U01
+// splitmix64 finaliser, the library's one counter-based uniform (reset, task and expert draws), identical to the oracle's U01
 DM_HD double task_u01(unsigned long long seed, unsigned long long a, unsigned long long b) {
     unsigned long long z = seed + 0x9E3779B97F4A7C15ull * (a * 2654435761ull + b + 1);
     z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull; z = (z ^ (z >> 27)) * 0x94D049BB133111EBull; z ^= z >> 31;

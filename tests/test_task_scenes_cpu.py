@@ -19,7 +19,7 @@ MASK = (1 << 64) - 1
 
 
 def u01(seed, a, b):
-    """splitmix64 finaliser on seed + golden * (a * 2654435761 + b + 1) -> [0, 1): the stream of dm_policy.cu's u01."""
+    """splitmix64 finaliser on seed + golden * (a * 2654435761 + b + 1) -> [0, 1): the stream of dm_task.cuh's task_u01."""
     z = (seed + 0x9E3779B97F4A7C15 * ((a * 2654435761 + b + 1) & MASK)) & MASK
     z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & MASK
     z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & MASK
