@@ -60,7 +60,7 @@ class DmLearnGatedBatch(C.Structure):
 DM_STATE_OFFSET, DM_STATE_SCALE, DM_ACTION_OFFSET, DM_ACTION_SCALE, DM_ACTION_BOUND_MIN, DM_ACTION_BOUND_MAX, DM_STATE_NORM_GROUPS = range(7)
 
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
-           "dm_update", "dm_record_state", "dm_record_goal", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
+           "dm_update", "dm_record_state", "dm_record_goal", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
            "dm_set_snapshot", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
            "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy", "dm_td_lambda_returns", "dm_mlp_set_weights_device", "dm_learn_create",
            "dm_mlp_set_normalizers_device", "dm_learn_set_weights", "dm_learn_step", "dm_learn_disc_step", "dm_learn_destroy",
@@ -110,6 +110,8 @@ def lib():
         L.dm_record_amp_obs_agent.argtypes = [vp, fp]
         L.dm_record_amp_obs_expert.argtypes = [vp, dp, fp]
         L.dm_amp_obs_host.argtypes = [vp, C.c_int, dp, fp]
+        L.dm_sample_amp_obs_expert.argtypes = [vp, C.c_int, vp, vp, vp]
+        L.dm_expert_sample_count.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
         L.dm_observe.argtypes = [vp, fp, fp]
         L.dm_get_flags.argtypes = [vp, ip]
         L.dm_step_host.argtypes = [vp, fp, C.c_double, C.c_int, fp, fp, ip]
@@ -306,6 +308,26 @@ class BatchedCore:
         else:
             c = np.ascontiguousarray(clip, dtype=np.int32)
             self._chk(lib().dm_record_amp_obs_expert_clips(self.h, c.ctypes.data_as(C.POINTER(C.c_int)), _dptr(kt), C.c_void_p(out.data_ptr())))
+
+    def sample_amp_obs_expert(self, out, clip=None, time=None):
+        """dm_sample_amp_obs_expert: out.shape[0] expert AMP observations into out [rows, amp_obs_size] (contiguous float32 CUDA tensor), clip
+        and time drawn on the device, enqueued on the handle's stream without a host synchronisation.  clip [rows] int32 and time [rows]
+        float64 contiguous CUDA tensors receive the draws when given."""
+        import torch
+        rows = out.shape[0] if out.dim() == 2 else 0
+        _check_device_f32(out, "sample_amp_obs_expert: out", (rows, self.dims.amp_obs_size))
+        for name, t, dt in (("clip", clip, torch.int32), ("time", time, torch.float64)):
+            if t is not None and (not t.is_cuda or t.dtype != dt or tuple(t.shape) != (rows,) or not t.is_contiguous()):
+                raise ValueError("sample_amp_obs_expert: %s must be a contiguous %s CUDA tensor [%d]" % (name, dt, rows))
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+        self._chk(lib().dm_sample_amp_obs_expert(self.h, rows, ptr(out), ptr(clip), ptr(time)))
+
+    def expert_sample_count(self, set_to=None):
+        """the expert sampler's call counter (the key of its next draws); set_to replaces it.  Returns the value before the call."""
+        got = C.c_uint64(0)
+        new = None if set_to is None else C.byref(C.c_uint64(int(set_to)))
+        self._chk(lib().dm_expert_sample_count(self.h, new, C.byref(got)))
+        return int(got.value)
 
     def flags(self, out):  # torch int32 cuda tensor [N, 4]
         self._chk(lib().dm_get_flags(self.h, C.c_void_p(out.data_ptr())))

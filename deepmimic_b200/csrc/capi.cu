@@ -102,6 +102,7 @@ struct dm_handle {
     uint64_t seed = 0, env_offset = 0;
     int64_t launches = 0;
     uint64_t amp_calls = 0;
+    uint64_t expert_samples = 0;   // dm_sample_amp_obs_expert calls so far: the draw counter of its device stream
     std::vector<double> st_off, st_scale, act_off, act_scale, act_min, act_max, st_groups;
     // dm_step_host: page-locked-ness of the caller's buffers, looked up once per pointer (cudaPointerGetAttributes is a driver call)
     std::vector<std::pair<const void*, bool>> pin_cache;
@@ -904,6 +905,21 @@ int dm_record_amp_obs_expert_clips(dm_handle* h, const int* h_clip, const double
     return launch_amp(h, d_out, 1, h->d_inj[0], task ? h->d_clip_inj : nullptr);
 }
 int dm_record_amp_obs_expert(dm_handle* h, const double* h_kin_time, float* d_out) { return dm_record_amp_obs_expert_clips(h, nullptr, h_kin_time, d_out); }
+int dm_sample_amp_obs_expert(dm_handle* h, int rows, float* d_out, int* d_clip_out, double* d_time_out) {
+    DM_DEVICE(h);
+    if (rows < 1 || d_out == nullptr) { g_err = "dm_sample_amp_obs_expert: need rows >= 1 and an output buffer"; return fail(); }
+    const dmk::AmpExpertKernel kern = dmk::kAmpExpertKernels[tile_index(h)][task_scene(h)];   // task scenes: the clip drawn from the dataset
+    const int tiles = dmk::kPolicyBlock / h->W;
+    kern<<<(rows + tiles - 1) / tiles, dmk::kPolicyBlock, 0, h->stream>>>(h->d_model, h->st, h->d_frame_times, h->d_frames, h->d_frame_vel, d_out, rows, h->seed,
+                                                                          h->expert_samples, d_clip_out, d_time_out);
+    h->expert_samples++;
+    return launched(h);
+}
+int dm_expert_sample_count(dm_handle* h, const unsigned long long* h_set, unsigned long long* h_get) {
+    if (h_get) *h_get = h->expert_samples;
+    if (h_set) h->expert_samples = *h_set;
+    return 0;
+}
 int dm_calc_reward(dm_handle* h, float* d_out) { return dm_observe(h, nullptr, d_out); }
 int dm_get_flags(dm_handle* h, int32_t* d_flags) {
     DM_DEVICE(h);

@@ -167,7 +167,8 @@ struct StepLayout {
 // ---- the kernels and host helpers capi.cu launches (defined in dm_step.cu and dm_policy.cu)
 // Every templated kernel is reached through a table indexed by [tile width 16 / 32][variant]; the table is defined next to the kernel, which
 // instantiates it.  Variants: the step kernel's TASK, the observe kernel's CLIPS and the reset kernel's TASKV are "AMP task scene"; the AMP
-// kernel's TASKV is "expert observation drawn from the clip dataset" (agent observations of a task scene use the single-clip variant).
+// kernel's TASKV is "expert observation drawn from the clip dataset" (agent observations of a task scene use the single-clip variant); the
+// expert sampler's TASKV is "clip drawn from the dataset".
 constexpr int kPolicyBlock = 64;   // threads per block of the observe, AMP and reset kernels
 using StepKernel = void (*)(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout);
 using ObserveKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, ObsFan, int);
@@ -178,6 +179,9 @@ extern const StepKernel kStepKernels[2][2];
 extern const ObserveKernel kObserveKernels[2][2];
 extern const ResetKernel kResetKernels[2][2];
 extern const AmpObsKernel kAmpObsKernels[2][2];
+using AmpExpertKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, float*, int, unsigned long long, unsigned long long,
+                                 int*, double*);
+extern const AmpExpertKernel kAmpExpertKernels[2][2];
 __global__ void dm_set_action_kernel(const DevModel*, DevState, const float*, int);
 __global__ void dm_task_reset_kernel(const DevModel*, DevState, int);
 __global__ void dm_task_observe_kernel(const DevModel*, DevState, float*, float*, int);

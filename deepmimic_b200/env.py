@@ -148,6 +148,14 @@ class DeepMimicBatchEnv:
         self._pre(); self._core.amp_obs_expert(buf, kin_time); self._post()
         return buf
 
+    def sample_amp_obs_expert(self, rows):
+        """[rows, amp_obs_size] float32: `rows` expert AMP observations (any count), clip and time drawn on the device per row
+        (dm_sample_amp_obs_expert).  A new tensor each call, allocated on the caller's current stream and complete before that stream's next
+        op, like any tensor torch makes there (a consumer on another stream needs the usual record_stream); no host synchronisation."""
+        out = self.torch.empty(int(rows), self.get_amp_obs_size(), device=self.device)
+        self._pre(); self._core.sample_amp_obs_expert(out); self._post()
+        return out
+
     def is_episode_end(self):
         return self._refresh_flags()[:, 1].bool()
 

@@ -18,8 +18,9 @@ The reference tree is not vendored here; its rules are restated below, one funct
 
 Documented deviations: minibatches are shuffled / drawn by a seeded torch.Generator on the data's device, not the reference's numpy stream; the
 statistics leave out the weight-decay (and logit-regulariser) terms of the losses (the reference's logged losses include them); the normalisers
-are not updated here (DeviceNormalizer.update stays the caller's call, as the reference's normaliser schedule is), nor is a replay buffer of
-agent AMP observations kept.  Not done: a multi-GPU gradient all-reduce, TarClipFrac stepsize decay, checkpoint writing."""
+are not updated here (DeviceNormalizer.update stays the caller's call, as the reference's normaliser schedule is), nor are the AMP replay
+buffers kept (deepmimic_b200/trainer.py: DeviceReplayBuffer, with the TarClipFrac, exploration and normaliser schedules).  Not done: a
+multi-GPU gradient all-reduce, checkpoint writing."""
 import math
 
 ADV_EPS = 1e-5   # PPOAgent.ADV_EPS

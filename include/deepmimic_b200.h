@@ -126,6 +126,14 @@ int dm_record_amp_obs_agent(dm_handle* h, float* d_out);
 int dm_record_amp_obs_expert(dm_handle* h, const double* h_kin_time, float* d_out);
 /* Same with a host output buffer [num_envs x amp_obs_size] (device -> host copy inside); used by the cDeepMimicCore facade. */
 int dm_amp_obs_host(dm_handle* h, int expert, const double* h_kin_time, float* h_out);
+/* `rows` (>= 1, any count) expert AMP observations into d_out [rows x amp_obs_size], drawn on the device and enqueued on the handle's stream
+ * without a host synchronisation.  Row r draws its clip from the dataset's sampling CDF (task scenes; the scene's motion otherwise) and its
+ * time from U(0, clip duration) on the counter stream of (seed, r, call), the call counter advancing once per call; its ground height is
+ * environment r % num_envs's.  The rows equal dm_record_amp_obs_expert(_clips) fed the same clips and times.  d_clip_out [rows] int32 and
+ * d_time_out [rows] double receive the draws when not NULL.  The draws do not depend on global_env_offset: sharded handles that should draw
+ * different rows need different seeds.  dm_expert_sample_count reads (h_get) and then sets (h_set) the call counter; either may be NULL. */
+int dm_sample_amp_obs_expert(dm_handle* h, int rows, float* d_out, int* d_clip_out, double* d_time_out);
+int dm_expert_sample_count(dm_handle* h, const unsigned long long* h_set, unsigned long long* h_get);
 int dm_observe(dm_handle* h, float* d_state, float* d_reward);  /* fused record_state + calc_reward, either may be NULL */
 /* d_flags: [num_envs x 4] int32 = {need_new_action, is_episode_end, check_terminate (0 null / 1 fail), check_valid_episode} */
 int dm_get_flags(dm_handle* h, int32_t* d_flags);
