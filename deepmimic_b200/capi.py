@@ -60,7 +60,7 @@ class DmLearnGatedBatch(C.Structure):
 DM_STATE_OFFSET, DM_STATE_SCALE, DM_ACTION_OFFSET, DM_ACTION_SCALE, DM_ACTION_BOUND_MIN, DM_ACTION_BOUND_MAX, DM_STATE_NORM_GROUPS = range(7)
 
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
-           "dm_update", "dm_record_state", "dm_record_goal", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
+           "dm_update", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
            "dm_set_snapshot", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
            "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy", "dm_td_lambda_returns", "dm_mlp_set_weights_device", "dm_learn_create",
            "dm_mlp_set_normalizers_device", "dm_learn_set_weights", "dm_learn_step", "dm_learn_disc_step", "dm_learn_destroy",
@@ -96,6 +96,9 @@ def lib():
         L.dm_reset.argtypes = [vp, C.c_int, dp, dp, dp]
         L.dm_set_action.argtypes = [vp, fp]
         L.dm_update.argtypes = [vp, C.c_double, C.c_int]
+        L.dm_set_env_order.argtypes = [vp, C.c_int]
+        L.dm_plan_env_order.argtypes = [C.POINTER(C.c_int), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)]
+        L.dm_get_env_order.argtypes = [vp, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.dm_record_state.argtypes = [vp, fp]
         L.dm_record_goal.argtypes = [vp, fp]
         L.dm_calc_reward.argtypes = [vp, fp]
@@ -196,6 +199,17 @@ def td_lambda_returns(rewards, values, end_values, done, terminate, discount, td
     return returns, advantages
 
 
+def plan_env_order(keys, tiles, tile_width):
+    """dm_plan_env_order: the step kernel's placement of len(keys) (padded) environments by contact load, as host arithmetic; returns order
+    [len(keys)] int32 (order[slot] = environment)"""
+    k = np.ascontiguousarray(keys, dtype=np.int32)
+    out = np.zeros(len(k), dtype=np.int32)
+    ip = C.POINTER(C.c_int)
+    if lib().dm_plan_env_order(k.ctypes.data_as(ip), len(k), int(tiles), int(tile_width), out.ctypes.data_as(ip)) != 0:
+        raise RuntimeError(lib().dm_last_error().decode())
+    return out
+
+
 class BatchedCore:
     """Thin object wrapper over a dm_handle."""
 
@@ -259,6 +273,19 @@ class BatchedCore:
 
     def update(self, dt, n_updates=1):
         self._chk(lib().dm_update(self.h, dt, n_updates))
+
+    def set_env_order(self, on):
+        """dm_set_env_order: place the environments in the step kernel by contact load (the default; tile width 16 only) or by index"""
+        self._chk(lib().dm_set_env_order(self.h, 1 if on else 0))
+
+    def env_order(self):
+        """dm_get_env_order: (keys now, placement of the last step launch: padded_envs int32 each, environments per block, tile width)"""
+        ip = C.POINTER(C.c_int)
+        plan = np.zeros(3, dtype=np.int32)
+        self._chk(lib().dm_get_env_order(self.h, plan.ctypes.data_as(ip), None, None))
+        keys, order = np.zeros(plan[0], dtype=np.int32), np.zeros(plan[0], dtype=np.int32)
+        self._chk(lib().dm_get_env_order(self.h, plan.ctypes.data_as(ip), keys.ctypes.data_as(ip), order.ctypes.data_as(ip)))
+        return keys, order, int(plan[1]), int(plan[2])
 
     def observe(self, state=None, reward=None):
         self._chk(lib().dm_observe(self.h, C.c_void_p(state.data_ptr()) if state is not None else None,

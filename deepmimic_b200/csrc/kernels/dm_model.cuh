@@ -138,7 +138,26 @@ struct DevState {
     const ClipTable* ctab;
     int num_envs;   // padded to a multiple of the step kernel's environments per block
     int num_real;   // environments the caller asked for; [num_real, num_envs) are padding: permanently "done", never reset, never simulated
+    int* load;      // contact-load key of every env: solver rows of its last Bullet sub-step (written at the step kernel's commit); padding kLoadPadding
+    const int* order;   // step kernel: environment of every tile slot (blockIdx.x * tiles + tile), from dm_env_order_kernel; null = identity
 };
+
+// ---- placement of the environments in the step kernel's tiles (dm_env_order_kernel, dm_plan_env_order).  The constraint solve of a W = 16 warp
+// runs its two environments in lockstep at the larger row count, so environments of equal load share a warp: a stable counting sort by key,
+// descending, ties by environment id; consecutive sorted environments fill a warp.  The sorted warps are dealt to the blocks in snake order
+// (block b takes sorted warps b, 2B - 1 - b, 2B + b, ...), so every block holds its share of heavy warps, and within a block in descending load
+// on warp slots 0, 1, 2, ...
+constexpr int kLoadPadding = -1;   // key of the padding environments: sorts them last
+constexpr int kLoadBuckets = 64;   // keys kLoadPadding .. kLoadBuckets - 2 (a warp's row capacity is at most 52)
+// bucket of a key, in descending key order
+__host__ __device__ inline int env_load_bucket(int key) { const int b = kLoadBuckets - 2 - key; return b < 0 ? 0 : (b >= kLoadBuckets ? kLoadBuckets - 1 : b); }
+// tile slot of the environment of sorted rank r (0 = heaviest) among n_padded, with `tiles` environments of width W per block
+__host__ __device__ inline int env_order_slot(int r, int n_padded, int tiles, int W) {
+    const int per_warp = 32 / W, blocks = n_padded / tiles, warps = tiles / per_warp;
+    const int g = r / per_warp, round = g / blocks, j = g % blocks;
+    const int b = (round & 1) ? blocks - 1 - j : j;
+    return (b * warps + round) * per_warp + r % per_warp;
+}
 
 // Output destinations of dm_observe_kernel: [0] is local, [1..n) the same slots of the peers' exchange buffers (NVLink P2P stores).
 // obs: [num_envs x state_size], rew / done: [num_envs] floats; rew[0] / done[0] null = not wanted.
@@ -182,6 +201,8 @@ extern const AmpObsKernel kAmpObsKernels[2][2];
 using AmpExpertKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, float*, int, unsigned long long, unsigned long long,
                                  int*, double*);
 extern const AmpExpertKernel kAmpExpertKernels[2][2];
+constexpr int kEnvOrderThreads = 1024;   // dm_env_order_kernel: one block
+__global__ void dm_env_order_kernel(const int* load, int n_padded, int tiles, int W, int* order);
 __global__ void dm_set_action_kernel(const DevModel*, DevState, const float*, int);
 __global__ void dm_task_reset_kernel(const DevModel*, DevState, int);
 __global__ void dm_task_observe_kernel(const DevModel*, DevState, float*, float*, int);

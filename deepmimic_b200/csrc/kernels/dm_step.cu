@@ -1126,7 +1126,8 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
     const int tiles = blockDim.x / W;
     const int tile = threadIdx.x / W;
     const int lane = threadIdx.x % W;
-    const int env = blockIdx.x * tiles + tile;   // host guarantees num_envs (padded) is a multiple of tiles
+    const int slot = blockIdx.x * tiles + tile;   // host guarantees num_envs (padded) is a multiple of tiles
+    const int env = (W == 16 && st.order) ? st.order[slot] : slot;   // placement by contact load (dm_env_order_kernel; two environments per warp only)
     const DevModel& M = *gm;
     const int nl = LY.nl, CL = LY.chain_len;
     const bool act = lane < nl;
@@ -1279,6 +1280,7 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
 #endif
     bool need_kin = true, pending_flags = false;
     int mcnt = 4;   // cached points of this lane's link after the last collision pass; unknown at the start of a launch: forces the first read
+    int last_nr = 0;   // solver rows of the last Bullet sub-step: the environment's contact-load key (DevState::load)
     const int stages_per_upd = sim_substeps + 1;
     const int total_stages = n_updates * stages_per_upd;
 #pragma unroll 1
@@ -1369,6 +1371,7 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
                         reinterpret_cast<float4*>(sim)[3] = make_float4(sB[10], sB[11], sB[12], 0.f);
                         fl[kFNeedAction] = need_action; fl[kFDone] = end ? 1 : 0; fl[kFTerminate] = term; fl[kFValid] = (eseg == 0) ? 1 : 0; fl[kFFallen] = fallen_eff;
                         fl[kFRowOverflow] = f_over; fl[kFUpdates] = f_updates;
+                        if (W == 16) st.load[env] = last_nr;
                     }
                     if (act) {
                         reinterpret_cast<float4*>(sim + 16)[lane] = jp;
@@ -1499,6 +1502,7 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
         const unsigned lseg = (W == 32) ? lbal : ((lbal >> (threadIdx.x & 16)) & 0xffffu);
         int NL = __popc(lseg);
         const unsigned anyrow = __ballot_sync(0xffffffffu, NL + P > 0);
+        last_nr = 0;
         if (anyrow != 0) {
             {
                 const int lidx = __popc(lseg & ((1u << lane) - 1u));
@@ -1507,6 +1511,7 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
             }
             if (NL + 3 * P > LY.maxrows) { P = (LY.maxrows - NL) / 3; f_over = 1; }
             const int NR = NL + 3 * P;
+            last_nr = NR;
             __syncwarp();
             PROF(5);
 #ifdef DM_PROFILE
@@ -1543,5 +1548,78 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
 }
 
 const StepKernel kStepKernels[2][2] = {{dm_step_kernel<16, false>, dm_step_kernel<16, true>}, {dm_step_kernel<32, false>, dm_step_kernel<32, true>}};
+
+// Placement of the environments for the next step-kernel launch (dm_model.cuh: env_load_bucket, env_order_slot).  One block of kEnvOrderThreads;
+// it runs between two step launches on the same stream, so its latency is what it costs: few barriers, no serial loop over the warps.
+//   * a histogram of the load buckets (one shared atomic per bucket present in a warp) gives each bucket's first rank;
+//   * the environments are ranked in id order, kEnvOrderItems per thread at a time (environment c0 + i kEnvOrderThreads + t): a warp's rank of an
+//     environment among its equal-bucket peers (match), plus the count of its bucket in the earlier (item, warp) cells, which kParts threads per
+//     bucket form by a scan over the cells, plus the bucket's count in the earlier chunks.
+constexpr int kEnvOrderItems = 4;
+__global__ void __launch_bounds__(kEnvOrderThreads) dm_env_order_kernel(const int* __restrict__ load, int n_padded, int tiles, int W, int* __restrict__ order) {
+    constexpr int kWarps = kEnvOrderThreads / 32, kCells = kEnvOrderItems * kWarps, kChunk = kEnvOrderItems * kEnvOrderThreads;
+    constexpr int kParts = kEnvOrderThreads / kLoadBuckets, kPer = kCells / kParts;   // threads per bucket, cells per thread
+    static_assert(kParts <= 32 && 32 % kParts == 0 && kCells % kParts == 0, "the scan of a bucket's cells runs inside one warp");
+    __shared__ int base[kLoadBuckets];                 // rank of the bucket's next environment (earlier chunks included)
+    __shared__ int cnt[kLoadBuckets][kCells + 1];      // per chunk: the bucket's count in each (item, warp) cell, then the cell's first rank
+    const int t = threadIdx.x, warp = t / 32, lane = t % 32;
+    const unsigned lt = (1u << lane) - 1u;
+    int b[kEnvOrderItems];   // buckets of this thread's environments in the current chunk
+    auto load_chunk = [&](int c0) {
+#pragma unroll
+        for (int i = 0; i < kEnvOrderItems; ++i) { const int e = c0 + i * kEnvOrderThreads + t; b[i] = (e < n_padded) ? env_load_bucket(load[e]) : kLoadBuckets; }
+    };
+    auto count = [&](int bk) {
+        const unsigned peers = __match_any_sync(0xffffffffu, bk);
+        if (bk < kLoadBuckets && (peers & lt) == 0) atomicAdd(&base[bk], __popc(peers));
+    };
+    load_chunk(0);
+    if (t < kLoadBuckets) base[t] = 0;
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < kEnvOrderItems; ++i) count(b[i]);
+    for (int e = kChunk + t; e < n_padded + t; e += kEnvOrderThreads) count((e < n_padded) ? env_load_bucket(load[e]) : kLoadBuckets);
+    __syncthreads();
+    if (warp == 0) {   // exclusive prefix over the buckets, two per lane
+        const int c0 = base[2 * lane], c1 = base[2 * lane + 1];
+        int incl = c0 + c1;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+        base[2 * lane] = incl - c0 - c1; base[2 * lane + 1] = incl - c1;
+    }
+    const int sb = t / kParts, part = t % kParts;
+    for (int c0 = 0; c0 < n_padded; c0 += kChunk) {
+        if (c0 > 0) load_chunk(c0);
+        for (int k = t; k < kLoadBuckets * (kCells + 1); k += kEnvOrderThreads) (&cnt[0][0])[k] = 0;
+        __syncthreads();
+        int below[kEnvOrderItems];
+#pragma unroll
+        for (int i = 0; i < kEnvOrderItems; ++i) {
+            const unsigned peers = __match_any_sync(0xffffffffu, b[i]);
+            below[i] = __popc(peers & lt);
+            if (b[i] < kLoadBuckets && below[i] == 0) cnt[b[i]][i * kWarps + warp] = __popc(peers);
+        }
+        __syncthreads();
+        {   // bucket sb, cells [part kPer, (part + 1) kPer): first ranks
+            int v[kPer], s = 0;
+#pragma unroll
+            for (int k = 0; k < kPer; ++k) { v[k] = cnt[sb][part * kPer + k]; s += v[k]; }
+            int incl = s;
+#pragma unroll
+            for (int o = 1; o < kParts; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, incl, o, kParts); if (part >= o) incl += u; }
+            const int first = base[sb];
+            int r = first + incl - s;
+#pragma unroll
+            for (int k = 0; k < kPer; ++k) { cnt[sb][part * kPer + k] = r; r += v[k]; }
+            __syncwarp();
+            if (part == kParts - 1) base[sb] = first + incl;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int i = 0; i < kEnvOrderItems; ++i)
+            if (b[i] < kLoadBuckets) order[env_order_slot(cnt[b[i]][i * kWarps + warp] + below[i], n_padded, tiles, W)] = c0 + i * kEnvOrderThreads + t;
+        __syncthreads();
+    }
+}
 
 }  // namespace dmk

@@ -98,6 +98,19 @@ int dm_reset(dm_handle* h, int force_all, const double* h_kin_time, const double
 int dm_set_action(dm_handle* h, const float* d_actions);
 /* n_updates consecutive Update(dt) calls in one launch; envs whose episode ended freeze until dm_reset. */
 int dm_update(dm_handle* h, double dt, int n_updates);
+/* Placement of the environments in the step kernel (on by default; tile width 16 only, where two environments share a warp: tile width 32
+ * handles keep index placement, where it measured slower): every step launch is preceded by a one-block kernel that orders the
+ * environments by contact load -- the solver row count of each environment's last Bullet sub-step, its key -- so that environments of equal
+ * load share a warp and every block holds its share of heavy warps.  Results are bit-identical either way; off places environment e in tile
+ * slot e.  Stream-ordered, no host synchronisation. */
+int dm_set_env_order(dm_handle* h, int on);
+/* The rule of that placement as host arithmetic (needs no handle or device): order[slot] = environment for slot in [0, n_padded), from
+ * keys[n_padded] (padding environments carry the key -1), `tiles` environments of tile width W (16 or 32) per block. */
+int dm_plan_env_order(const int* keys, int n_padded, int tiles, int W, int* order);
+/* test hook: h_plan3 = {padded environment count, environments per block, tile width}, the keys now (h_keys) and the placement of the last
+ * step launch (h_order), padded_envs ints each; any may be NULL.  Synchronises the handle's stream.  The order is the identity when the
+ * placement is off. */
+int dm_get_env_order(dm_handle* h, int* h_plan3, int* h_keys, int* h_order);
 int dm_record_state(dm_handle* h, float* d_out);             /* [num_envs x state_size] */
 int dm_record_goal(dm_handle* h, float* d_out);              /* [num_envs x goal_size] (no-op when goal_size == 0) */
 /* AMP task scenes target_amp / heading_amp (cSceneTargetAMP / cSceneHeadingAMP: RecordGoal, CalcReward, target updates; goal_size 3).
