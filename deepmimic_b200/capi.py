@@ -61,7 +61,7 @@ DM_STATE_OFFSET, DM_STATE_SCALE, DM_ACTION_OFFSET, DM_ACTION_SCALE, DM_ACTION_BO
 
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
            "dm_update", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
-           "dm_set_snapshot", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
+           "dm_set_snapshot", "dm_state_size", "dm_save_state", "dm_load_state", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
            "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy", "dm_td_lambda_returns", "dm_mlp_set_weights_device", "dm_learn_create",
            "dm_mlp_set_normalizers_device", "dm_learn_set_weights", "dm_learn_step", "dm_learn_disc_step", "dm_learn_destroy",
            "dm_learn_create_gated", "dm_learn_set_gated_weights", "dm_learn_gated_step", "dm_mlp_set_gated_weights_device", "dm_mlp_set_gated_normalizers_device"]
@@ -131,6 +131,9 @@ def lib():
         L.dm_step_host_timing.argtypes = [vp, dp]
         L.dm_get_snapshot.argtypes = [vp, C.c_int, dp]
         L.dm_set_snapshot.argtypes = [vp, C.c_int, dp]
+        L.dm_state_size.argtypes = [vp, C.POINTER(C.c_size_t)]
+        L.dm_save_state.argtypes = [vp, C.c_void_p]
+        L.dm_load_state.argtypes = [vp, C.c_void_p]
         L.dm_get_counters.argtypes = [vp, C.POINTER(C.c_int64)]
         L.dm_get_section_profile.argtypes = [vp, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
         fpp = C.POINTER(C.c_float)
@@ -423,6 +426,23 @@ class BatchedCore:
     def set_snapshot(self, env, snap):
         s = np.ascontiguousarray(snap, dtype=np.float64)
         self._chk(lib().dm_set_snapshot(self.h, env, _dptr(s)))
+
+    def save_state(self):
+        """dm_save_state: the whole batch's simulation state as a uint8 array (synchronises the handle's stream)"""
+        n = C.c_size_t(0)
+        self._chk(lib().dm_state_size(self.h, C.byref(n)))
+        out = np.zeros(n.value, dtype=np.uint8)
+        self._chk(lib().dm_save_state(self.h, C.c_void_p(out.ctypes.data)))
+        return out
+
+    def load_state(self, buf):
+        """dm_load_state: restores a save_state() blob of a handle made with the same arguments, environment count and seed (synchronises the
+        handle's stream); a mismatch raises, naming the field"""
+        b = np.ascontiguousarray(buf, dtype=np.uint8)
+        # the header's byte count (bytes 16..23) must match the blob: dm_load_state then compares the header with this handle field by field
+        if b.ndim != 1 or b.size < 24 or int(b[16:24].view(np.uint64)[0]) != b.size:
+            raise ValueError("load_state: not a complete save_state() blob (%s bytes)" % (b.shape,))
+        self._chk(lib().dm_load_state(self.h, C.c_void_p(b.ctypes.data)))
 
     def counters(self):
         out = (C.c_int64 * 2)()

@@ -1216,6 +1216,116 @@ int dm_set_snapshot(dm_handle* h, int env, const double* s) {
     DM_CUDA(cudaMemcpy(h->st.flags + static_cast<size_t>(env) * dmk::kFlagInts, fl, sizeof(fl), cudaMemcpyHostToDevice));
     return 0;
 }
+// ---- whole-batch state (dm_state_size / dm_save_state / dm_load_state): a header, then the per-environment device blocks in DevState order
+namespace {
+constexpr char kStateMagic[8] = {'D', 'M', 'S', 'T', 'A', 'T', 'E', 0};
+constexpr uint32_t kStateVersion = 1;
+struct StateHeader {
+    char magic[8];
+    uint32_t version, pad0;
+    uint64_t bytes;
+    int32_t num_envs, padded_envs, W, links, state_size, action_size, goal_size, amp_obs_size, num_clips, pad1;
+    uint64_t seed, env_offset, model;
+    char scene[32];
+    // host state that changes later results
+    uint64_t amp_calls, expert_samples;
+    int32_t mode, pad2;
+    double time_lim_min, time_lim_max;
+};
+struct StateBlock { void* dev; size_t bytes; };
+// the device blocks of the blob, in order; null blocks of the scene (task, taskx, clip outside the task scenes) are absent
+std::vector<StateBlock> state_blocks(const dm_handle* h) {
+    const size_t N = static_cast<size_t>(h->padded_envs);
+    const auto& M = h->hm;
+    const dmk::DevState& s = h->st;
+    std::vector<StateBlock> b = {{s.sim, N * dmk::sim_stride(M.nl) * sizeof(float)}, {s.time, N * dmk::kTimeDoubles * sizeof(double)},
+                                 {s.flags, N * dmk::kFlagInts * sizeof(int)}, {s.manifold, N * M.nl * dmk::kManifoldFloats * sizeof(float)},
+                                 {s.hist, N * 2 * M.pose_dim * sizeof(float)}, {s.task, N * dmk::kTaskDoubles * sizeof(double)},
+                                 {s.taskx, N * dmk::kTaskExtDoubles * sizeof(double)}, {s.clip, N * sizeof(int)}, {s.load, N * sizeof(int)}};
+    b.erase(std::remove_if(b.begin(), b.end(), [](const StateBlock& x) { return x.dev == nullptr; }), b.end());
+    return b;
+}
+// FNV-1a over the model blob with the fields that change at run time (time limits, mode) cleared: tells handles of different characters,
+// controllers or clips apart when every count matches
+uint64_t model_hash(const dm_handle* h) {
+    dmk::DevModel m;
+    std::memcpy(&m, &h->hm, sizeof(m));   // bytewise, padding included (build_device_model clears it)
+    m.time_lim_min = m.time_lim_max = 0.0; m.test_mode = 0;
+    const unsigned char* p = reinterpret_cast<const unsigned char*>(&m);
+    uint64_t x = 1469598103934665603ull;
+    for (size_t i = 0; i < sizeof(m); ++i) { x ^= p[i]; x *= 1099511628211ull; }
+    return x;
+}
+StateHeader state_header(const dm_handle* h) {
+    StateHeader H;
+    std::memset(&H, 0, sizeof(H));
+    std::memcpy(H.magic, kStateMagic, sizeof(H.magic));
+    H.version = kStateVersion;
+    H.bytes = sizeof(StateHeader);
+    for (const StateBlock& b : state_blocks(h)) H.bytes += b.bytes;
+    const auto& M = h->hm;
+    H.num_envs = h->num_envs; H.padded_envs = h->padded_envs; H.W = h->W; H.links = M.nl; H.state_size = M.state_size; H.action_size = M.action_size;
+    H.goal_size = goal_size(M); H.amp_obs_size = M.amp_obs_size; H.num_clips = h->ctab.num_clips;
+    H.seed = h->seed; H.env_offset = h->env_offset; H.model = model_hash(h);
+    std::snprintf(H.scene, sizeof(H.scene), "%s", h->sa.cfg.scene.c_str());
+    H.amp_calls = h->amp_calls; H.expert_samples = h->expert_samples; H.mode = h->mode;
+    H.time_lim_min = M.time_lim_min; H.time_lim_max = M.time_lim_max;
+    return H;
+}
+}  // namespace
+
+int dm_state_size(dm_handle* h, size_t* bytes) {
+    DM_DEVICE(h);
+    *bytes = state_header(h).bytes;
+    return 0;
+}
+int dm_save_state(dm_handle* h, void* h_out) {
+    DM_DEVICE(h);
+    const StateHeader H = state_header(h);
+    char* o = static_cast<char*>(h_out);
+    std::memcpy(o, &H, sizeof(H));
+    o += sizeof(H);
+    for (const StateBlock& b : state_blocks(h)) {
+        DM_CUDA(cudaMemcpyAsync(o, b.dev, b.bytes, cudaMemcpyDeviceToHost, h->stream));
+        o += b.bytes;
+    }
+    DM_CUDA(cudaStreamSynchronize(h->stream));
+    return 0;
+}
+int dm_load_state(dm_handle* h, const void* h_in) {
+    DM_DEVICE(h);
+    StateHeader in;
+    std::memcpy(&in, h_in, sizeof(in));
+    const StateHeader mine = state_header(h);
+    auto refuse = [](const char* field) { g_err = std::string("dm_load_state: the state was saved by a handle with another ") + field; return fail(); };
+    if (std::memcmp(in.magic, kStateMagic, sizeof(in.magic)) != 0) { g_err = "dm_load_state: not a state blob (magic)"; return fail(); }
+    if (in.version != kStateVersion) return refuse("layout version");
+    if (std::strncmp(in.scene, mine.scene, sizeof(in.scene)) != 0) return refuse("scene");
+    if (in.num_envs != mine.num_envs) return refuse("num_envs");
+    if (in.padded_envs != mine.padded_envs) return refuse("padded_envs");
+    if (in.W != mine.W) return refuse("tile width W");
+    if (in.links != mine.links) return refuse("link count");
+    if (in.state_size != mine.state_size) return refuse("state size");
+    if (in.action_size != mine.action_size) return refuse("action size");
+    if (in.goal_size != mine.goal_size) return refuse("goal size");
+    if (in.amp_obs_size != mine.amp_obs_size) return refuse("AMP observation size");
+    if (in.num_clips != mine.num_clips) return refuse("clip count");
+    if (in.seed != mine.seed) return refuse("seed");
+    if (in.env_offset != mine.env_offset) return refuse("global env offset");
+    if (in.model != mine.model) return refuse("model (character, controller or clips)");
+    if (in.bytes != mine.bytes) return refuse("byte size");
+    const char* p = static_cast<const char*>(h_in) + sizeof(in);
+    for (const StateBlock& b : state_blocks(h)) {
+        DM_CUDA(cudaMemcpyAsync(b.dev, p, b.bytes, cudaMemcpyHostToDevice, h->stream));
+        p += b.bytes;
+    }
+    DM_CUDA(cudaStreamSynchronize(h->stream));
+    h->amp_calls = in.amp_calls; h->expert_samples = in.expert_samples;
+    h->hm.time_lim_min = in.time_lim_min; h->hm.time_lim_max = in.time_lim_max;
+    if (upload_time_limits(h)) return 1;
+    return dm_set_mode(h, in.mode);
+}
+
 int dm_get_section_profile(dm_handle* h, uint32_t* out, int* num_blocks, int* warps_per_block) {
     DM_DEVICE(h);
     if (!h->st.prof) { g_err = "dm_get_section_profile: this library is not the profile build (make -C deepmimic_b200/csrc profile)"; return fail(); }

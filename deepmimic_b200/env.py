@@ -248,6 +248,20 @@ class DeepMimicBatchEnv:
     def get_reward_succ(self, agent_id=0):
         return 1.0
 
+    def state_dict(self):
+        """the whole batch's simulation state (BatchedCore.save_state: every environment's device blocks, the draw counters, mode and time
+        limits) and get_time()'s clock; ordered after the caller's stream's work, and synchronising.  blob is a CPU uint8 tensor."""
+        import torch
+        self._pre()
+        return dict(blob=torch.from_numpy(self._core.save_state()), time=self._time)
+
+    def load_state_dict(self, s):
+        """restores state_dict() of an env made with the same arguments, num_envs and seed; the caller's stream then waits for the copies"""
+        self._pre()
+        self._core.load_state(np.asarray(s["blob"]))
+        self._time = float(s["time"])
+        self._post()
+
     def sync(self):
         self._core.sync()
 

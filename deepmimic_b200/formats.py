@@ -65,11 +65,16 @@ def read_state(path):
 
 class TableLog:
     """The learner's tabular log (R/util/logger.py): the first row fixes the headers; every cell is left-aligned in 25 characters; floats print
-    through str()."""
+    through str().  append=True continues an existing log (a resumed run): its header line fixes the headers and is not written again."""
 
-    def __init__(self, path):
-        self.file = open(path, "w")
+    def __init__(self, path, append=False):
+        import os
         self.headers, self.row, self.first = [], {}, True
+        if append and os.path.exists(path) and os.path.getsize(path) > 0:
+            with open(path) as f:
+                self.headers = f.readline().split()
+            self.first = False
+        self.file = open(path, "a" if append else "w")
 
     def log_tabular(self, key, val):
         if self.first and key not in self.headers:

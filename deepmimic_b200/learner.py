@@ -20,7 +20,7 @@ Documented deviations: minibatches are shuffled / drawn by a seeded torch.Genera
 statistics leave out the weight-decay (and logit-regulariser) terms of the losses (the reference's logged losses include them); the normalisers
 are not updated here (DeviceNormalizer.update stays the caller's call, as the reference's normaliser schedule is), nor are the AMP replay
 buffers kept (deepmimic_b200/trainer.py: DeviceReplayBuffer, with the TarClipFrac, exploration and normaliser schedules).  Not done: a
-multi-GPU gradient all-reduce, checkpoint writing."""
+multi-GPU gradient all-reduce.  The loop that drives both learners, with checkpoints, is deepmimic_b200/trainer.py: Trainer."""
 import math
 
 ADV_EPS = 1e-5   # PPOAgent.ADV_EPS

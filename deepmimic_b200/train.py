@@ -1,0 +1,114 @@
+"""Train a skill: the counterpart of the reference's `DeepMimic_Optimizer.py --arg_file args/train_*_args.txt`, on one GPU.
+
+    python -m deepmimic_b200.train --arg_file args/train_humanoid3d_spinkick_args.txt [reference arguments ...]
+        [--asset_root DIR] [--num_envs 4096] [--window_steps 32] [--max_iters K] [--backend tensor_core] [--seed 0] [--device 0] [--resume PATH]
+
+Every argument this module does not name goes to the scene, as the reference's arguments do.  --agent_files, --output_path and
+--int_output_path are read from the same argument list, the command line before the arg file (the reference's ArgParser keeps the first value
+of a key).  The log goes to <output_path>/agent0_log.txt and the checkpoint to <output_path>/agent0_checkpoint.pt (every OutputIters iterations
+and at the end); with --int_output_path, an intermediate checkpoint every IntOutputIters iterations goes to
+<int_output_path>/agent0_int_checkpoint_<iteration>.pt.  --resume continues a checkpoint of the same run (arguments, agent file, num_envs,
+window_steps, backend, seed), its log and its iteration numbering."""
+import argparse
+import os
+import re
+import sys
+
+
+def parse_arg_list(tokens):
+    """the reference's ArgParser over a token list: --key followed by its values; '#'-prefixed tokens are comments; the first occurrence of a
+    key wins"""
+    table, key, vals = {}, None, []
+    for tok in tokens:
+        if tok.startswith("#"):
+            continue
+        if tok.startswith("--"):
+            if key is not None and key not in table:
+                table[key] = vals
+            key, vals = tok[2:], []
+        else:
+            vals.append(tok)
+    if key is not None and key not in table:
+        table[key] = vals
+    return table
+
+
+def _file_tokens(path):
+    """the tokens of an arg file: lines starting with '#' are comments"""
+    out = []
+    with open(path) as f:
+        for line in re.split(r"[\n\r]+", f.read()):
+            if line and not line.lstrip().startswith("#"):
+                out += line.split()
+    return out
+
+
+def _resolve(asset_root, path):
+    """a path of the argument list: absolute, under the asset root, or relative to the working directory"""
+    if os.path.isabs(path):
+        return path
+    under = os.path.join(asset_root, path)
+    return under if os.path.exists(under) else path
+
+
+def resolve_args(scene_args, asset_root):
+    """(agent file, output path, int output path) from the scene arguments and the arg file they name (command line first)"""
+    table = parse_arg_list(scene_args)
+    if "arg_file" in table and table["arg_file"]:
+        arg_file = _resolve(asset_root, table["arg_file"][0])
+        if not os.path.exists(arg_file):
+            raise SystemExit("train: arg file %s not found" % table["arg_file"][0])
+        for k, v in parse_arg_list(_file_tokens(arg_file)).items():
+            table.setdefault(k, v)
+    first = lambda k: table[k][0] if table.get(k) else ""
+    if not first("agent_files"):
+        raise SystemExit("train: no --agent_files in the arguments or the arg file")
+    return _resolve(asset_root, first("agent_files")), first("output_path") or "output", first("int_output_path")
+
+
+def build_parser():
+    ap = argparse.ArgumentParser(prog="python -m deepmimic_b200.train", description=__doc__.split("\n\n")[0], allow_abbrev=False)
+    ap.add_argument("--asset_root", default=None, help="the reference's data / args tree (default: the bundled asset archive)")
+    ap.add_argument("--num_envs", type=int, default=4096)
+    ap.add_argument("--window_steps", type=int, default=32, help="policy steps per environment in each iteration's window")
+    ap.add_argument("--max_iters", type=int, default=None, help="stop after this many iterations in all (default: run until interrupted)")
+    ap.add_argument("--backend", default="tensor_core", choices=("tensor_core", "torch"))
+    ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--resume", default=None, help="a checkpoint of the same run to continue")
+    return ap
+
+
+def main(argv=None):
+    from .assets import asset_root as default_asset_root
+    from .trainer import AgentConfig, Trainer
+    opts, scene_args = build_parser().parse_known_args(sys.argv[1:] if argv is None else argv)
+    root = opts.asset_root or default_asset_root()
+    agent_file, out_path, int_path = resolve_args(scene_args, root)
+    cfg = AgentConfig.from_json(agent_file)
+    os.makedirs(out_path, exist_ok=True)
+    if int_path:
+        os.makedirs(int_path, exist_ok=True)
+    ckpt = os.path.join(out_path, "agent0_checkpoint.pt")
+    tr = Trainer(scene_args, cfg, root, opts.num_envs, window_steps=opts.window_steps, backend=opts.backend, seed=opts.seed, device=opts.device,
+                 log_path=os.path.join(out_path, "agent0_log.txt"), append_log=opts.resume is not None)
+    if opts.resume:
+        tr.load(opts.resume)
+    try:
+        while opts.max_iters is None or tr.iter < opts.max_iters:
+            row = tr.iteration()
+            print("iteration %d: samples %d, Train_Return %.4f, Test_Return %.4f, %.2f s" % (row["Iteration"], row["Samples"], row["Train_Return"],
+                                                                                            row["Test_Return"], row["Wall_Time"]), flush=True)
+            if tr.iter % cfg["OutputIters"] == 0:
+                tr.save(ckpt)
+            if int_path and cfg["IntOutputIters"] > 0 and tr.iter % cfg["IntOutputIters"] == 0:
+                tr.save(os.path.join(int_path, "agent0_int_checkpoint_%010d.pt" % tr.iter))
+    except KeyboardInterrupt:
+        pass
+    tr.save(ckpt)
+    tr.close()
+    print("checkpoint: %s (iteration %d)" % (ckpt, tr.iter))
+
+
+if __name__ == "__main__":
+    main()

@@ -350,6 +350,17 @@ void dm_learn_destroy(dm_learn* l);
  *  [29 + 55nl + 4j ..] PD target of joint j in DeepMimic joint-frame convention (w,x,y,z or angle) */
 int dm_get_snapshot(dm_handle* h, int env, double* h_out);
 int dm_set_snapshot(dm_handle* h, int env, const double* h_in);
+/* Whole-batch simulation state, for checkpoints and bit-exact resumption: every per-environment device block over the padded environments
+ * (SIM, TIME, FLAGS with the reset counters, MANIFOLD, the AMP history, the task blocks, the active clips, the contact-load keys) and the host
+ * state that changes later results (the expert draw counters, the mode, the current episode time limits), behind a header that names the
+ * handle's configuration.  dm_state_size gives the blob's size in bytes; dm_save_state writes it to h_out and dm_load_state reads it from h_in
+ * (host memory).  Both copy on the handle's stream and SYNCHRONISE it: they are meant for rare calls, off the per-step path.  dm_load_state
+ * refuses a blob whose header differs from this handle (scene, environment counts, tile width, sizes, clip count, seed, global offset,
+ * model) with a dm_last_error that names the field, and leaves the handle unchanged then.  A loaded handle continues exactly as the saved
+ * one would have. */
+int dm_state_size(dm_handle* h, size_t* bytes);
+int dm_save_state(dm_handle* h, void* h_out);
+int dm_load_state(dm_handle* h, const void* h_in);
 /* profile build only (DM_PROFILE, `make -C deepmimic_b200/csrc profile`; fails in a normal build): per-warp cycle counters by code section of the
  * last dm_update's step kernel, 18 uint32 per warp, block-major ([num_blocks][warps_per_block][18], tools/section_profile.py names them).
  * h_out may be NULL to query the two sizes only. */
