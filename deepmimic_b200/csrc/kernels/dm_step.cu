@@ -776,7 +776,7 @@ __device__ __noinline__ int collide(float* mani, int alive, int mcnt) {
         for (int k = 0; k < 12; ++k) mo[k] = make_float4(mp[4 * k], mp[4 * k + 1], mp[4 * k + 2], mp[4 * k + 3]);
     }
     // exclusive prefix over lanes -> point indices; publish points to the solver
-    int incl = cnt, over = 0;
+    int incl = cnt;
 #pragma unroll
     for (int o = 1; o < W; o <<= 1) { int t = __shfl_up_sync(0xffffffffu, incl, o, W); if (c.lane >= o) incl += t; }
     const int base = incl - cnt;
@@ -788,9 +788,11 @@ __device__ __noinline__ int collide(float* mani, int alive, int mcnt) {
             sPp[p * 4] = pa.x; sPp[p * 4 + 1] = pa.y; sPp[p * 4 + 2] = pa.z; sPp[p * 4 + 3] = mp[k * 12 + 10];
             sPi[p] = mp[k * 12 + 7];
             sPr[p] = c.lane * 4 + k;
-        } else over = 1;
+        }
     }
-    const int P = min(T::shfli(incl, W - 1), LY.maxpts);
+    // the overflow bit is the tile's, not the lane's: the points past maxpts belong to later lanes, and lane 0 commits the flag
+    const int total = T::shfli(incl, W - 1);
+    const int P = min(total, LY.maxpts), over = total > LY.maxpts ? 1 : 0;
     __syncwarp();
     return P | (tol << 8) | (over << 9) | (cnt << 10);
 }

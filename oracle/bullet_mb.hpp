@@ -116,6 +116,15 @@ struct BtMultiBody {
     // test/debug taps: velocities of the first sub-step of the last stepSimulation call, and the solved impulses
     std::vector<float> dbg_after_aba, dbg_after_pgs, dbg_lambda, dbg_after_aba1, dbg_after_pgs1, dbg_lambda1;
     int dbg_substep = 0;
+    // test tap: which branches of the constraint solve each sub-step of the last stepSimulation call took (counts only, no arithmetic)
+    struct RowTaps {
+        int limits = 0, points = 0;        // joint-limit rows, contact points (solver rows = limits + 3 points)
+        int clampAba = 0, clampPgs = 0;    // a generalised velocity hit maxCoordinateVelocity: unconstrained update / applyDeltaVee after PGS
+        int limitsAtUpper = 0;             // limit rows whose impulse ended at maxAppliedImpulse
+        int frictionSkipped = 0;           // friction rows skipped in the last sweep (their point's normal impulse <= 0)
+        int limitsDeep = 0;                // limit rows deeper than the split-impulse threshold (positional term dropped)
+    };
+    std::vector<RowTaps> dbg_rows;
 
     void finalize() {
         int off = 0;
@@ -271,7 +280,8 @@ struct BtMultiBody {
         F3 wd = R0t * spatAcc[0].a;
         F3 vd = R0t * (spatAcc[0].l + cross(spatVel[0].a, spatVel[0].l));
         out[0] = wd.x; out[1] = wd.y; out[2] = wd.z; out[3] = vd.x; out[4] = vd.y; out[5] = vd.z;
-        applyDeltaVee(out.data(), dt);
+        const bool clamped = applyDeltaVee(out.data(), dt);
+        if (!dbg_rows.empty()) dbg_rows.back().clampAba = clamped ? 1 : 0;
     }
 
     // btMultiBody::solveImatrix: x = Ia_base^-1 * rhs (block inverse of the 6x6 base articulated inertia)
@@ -292,12 +302,15 @@ struct BtMultiBody {
         return {vtop, vbot};
     }
 
-    // btMultiBody::applyDeltaVeeMultiDof
-    void applyDeltaVee(const float* dv, float mult) {
+    // btMultiBody::applyDeltaVeeMultiDof; returns whether a coordinate was clamped
+    bool applyDeltaVee(const float* dv, float mult) {
+        bool clamped = false;
         for (int d = 0; d < 6 + numDofs; ++d) {
             realBuf[d] += dv[d] * mult;
+            clamped |= std::fabs(realBuf[d]) > maxCoordinateVelocity;
             realBuf[d] = std::min(std::max(realBuf[d], -maxCoordinateVelocity), maxCoordinateVelocity);
         }
+        return clamped;
     }
 
     // btMultiBody::calcAccelerationDeltasMultiDof: out = M^-1 * force (generalised), reusing the ABA cache
@@ -577,6 +590,7 @@ struct BtMultiBody {
                 r.rhs = combine ? penetrationImpulse + velocityImpulse : velocityImpulse;  // m_rhsPenetration is never consumed for multibodies
                 r.cfm = 0; r.lowerLimit = 0; r.upperLimit = maxAppliedImpulse; r.appliedImpulse = 0;
                 limits.push_back(r);
+                if (!combine && !dbg_rows.empty()) dbg_rows.back().limitsDeep++;
             }
         }
         // resolveSingleConstraintRowGeneric
@@ -595,13 +609,21 @@ struct BtMultiBody {
             int nl = static_cast<int>(limits.size());
             for (int j = 0; j < nl; ++j) resolve(limits[(it & 1) ? j : nl - 1 - j]);
             for (auto& c : normals) resolve(c);
+            int skipped = 0;
             for (auto& c : frictions) {
                 float totalImpulse = normals[c.frictionIndex].appliedImpulse;
                 if (totalImpulse > 0) { c.lowerLimit = -(c.friction * totalImpulse); c.upperLimit = c.friction * totalImpulse; resolve(c); }
+                else skipped++;
             }
+            if (it == info.numIterations - 1 && !dbg_rows.empty()) dbg_rows.back().frictionSkipped = skipped;
         }
         // finish: velocities += accumulated delta (clamped like applyDeltaVeeMultiDof), impulses written back to the manifold
-        applyDeltaVee(deltaVelocities.data(), 1.0f);
+        const bool clamped = applyDeltaVee(deltaVelocities.data(), 1.0f);
+        if (!dbg_rows.empty()) {
+            RowTaps& t = dbg_rows.back();
+            t.limits = static_cast<int>(limits.size()); t.points = static_cast<int>(normals.size()); t.clampPgs = clamped ? 1 : 0;
+            for (auto& c : limits) t.limitsAtUpper += (c.appliedImpulse == c.upperLimit) ? 1 : 0;
+        }
         if (dbg_substep == 1) { dbg_lambda1.clear(); for (auto& c : normals) dbg_lambda1.push_back(c.appliedImpulse); for (auto& c : frictions) dbg_lambda1.push_back(c.appliedImpulse); for (auto& c : limits) dbg_lambda1.push_back(c.appliedImpulse); }
         if (dbg_substep == 0) { dbg_lambda.clear(); for (auto& c : normals) dbg_lambda.push_back(c.appliedImpulse); for (auto& c : frictions) dbg_lambda.push_back(c.appliedImpulse); for (auto& c : limits) dbg_lambda.push_back(c.appliedImpulse); }
         for (size_t k = 0; k < normals.size(); ++k) {
@@ -614,6 +636,7 @@ struct BtMultiBody {
     // btDiscreteDynamicsWorld::internalSingleStepSimulation for one multibody (reference call site sim/World.cpp:93-104)
     void internalSingleStep(float h, const BtContactSolverInfo& base_info, float friction) {
         for (int i = 0; i < n(); ++i) collideLinkPlane(i);          // performDiscreteCollisionDetection
+        dbg_rows.emplace_back();
         computeAccelerationsABA(h);                                  // solveConstraints: ABA, v += a h
         if (dbg_substep == 0) dbg_after_aba = realBuf; else if (dbg_substep == 1) dbg_after_aba1 = realBuf;
         BtContactSolverInfo info = base_info; info.timeStep = h;
@@ -629,6 +652,7 @@ struct BtMultiBody {
         numSub = std::min(numSub, maxSubSteps);
         for (auto& L : links) L.appliedForce += L.mass * gravity;   // applyGravity (btMultiBodyDynamicsWorld)
         dbg_substep = 0;
+        dbg_rows.clear();
         for (int s = 0; s < numSub; ++s) internalSingleStep(fixedTimeStep, info, friction);
         for (auto& L : links) { L.appliedForce = F3(); L.appliedTorque = F3(); L.jointTorque[0] = L.jointTorque[1] = L.jointTorque[2] = 0; }  // clearForces
     }

@@ -1294,6 +1294,19 @@ void dmo_debug_taps1(void* h, float* out) {
     for (int k = 0; k < n; ++k) { out[k] = k < (int)o->mb.dbg_after_aba1.size() ? o->mb.dbg_after_aba1[k] : 0; out[n + k] = k < (int)o->mb.dbg_after_pgs1.size() ? o->mb.dbg_after_pgs1[k] : 0; }
     for (int k = 0; k < 64; ++k) out[2 * n + k] = k < (int)o->mb.dbg_lambda1.size() ? o->mb.dbg_lambda1[k] : 0;
 }
+// constraint-solve branches of each Bullet sub-step of the last Update: 7 ints per sub-step (limit rows, contact points, clamp in the
+// unconstrained update, clamp after PGS, limit rows at the impulse cap, friction rows skipped in the last sweep, limit rows past the
+// split-impulse threshold), at most max_substeps sub-steps; returns the number of sub-steps
+int dmo_last_rows(void* h, int* out, int max_substeps) {
+    const auto& rows = static_cast<Oracle*>(h)->mb.dbg_rows;
+    const int n = std::min(static_cast<int>(rows.size()), max_substeps);
+    for (int s = 0; s < n; ++s) {
+        const auto& t = rows[s];
+        const int v[7] = {t.limits, t.points, t.clampAba, t.clampPgs, t.limitsAtUpper, t.frictionSkipped, t.limitsDeep};
+        std::copy(v, v + 7, out + 7 * s);
+    }
+    return n;
+}
 void dmo_kin_frame(void* h, double time, double* pose, double* vel) { Oracle* o = static_cast<Oracle*>(h); orc::VecD p, v; o->KinCalcPose(time, p); o->KinCalcVel(time, v); std::copy(p.begin(), p.end(), pose); std::copy(v.begin(), v.end(), vel); }
 void dmo_body_state(void* h, double* pos, double* rot, double* linvel, double* angvel) {
     Oracle* o = static_cast<Oracle*>(h);

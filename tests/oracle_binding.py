@@ -262,6 +262,14 @@ class Oracle:
         n = self.num_dofs
         return out[:n], out[n:2 * n], out[2 * n:]
 
+    def last_rows(self, max_substeps=8):
+        """branches of the constraint solve per Bullet sub-step of the last update: int array [sub-steps, 7] of (limit rows, contact points,
+        clamp in the unconstrained update, clamp after PGS, limit rows at the impulse cap, friction rows skipped in the last sweep,
+        limit rows past the split-impulse threshold); solver rows = limit rows + 3 contact points"""
+        out = np.zeros((max_substeps, 7), dtype=np.int32)
+        n = self.L.dmo_last_rows(self.h, out.ctypes.data_as(C.POINTER(C.c_int)), max_substeps)
+        return out[:n].copy()
+
     def bullet_aba(self, joint_tau, with_gravity=True):
         jt = np.ascontiguousarray(joint_tau, dtype=np.float32); out = np.zeros(self.num_dofs, dtype=np.float32)
         self.L.dmo_bullet_aba(self.h, fp(jt), 1 if with_gravity else 0, fp(out))

@@ -31,8 +31,21 @@ def perturb(lay, snap, rng, rel=ULP):
     return p
 
 
-def envelope(orc, orc2, lay, jt, before, after, rng, replicas):
-    worst_q = worst_qd = 0.0
+def impulse_err(lay, a, b):
+    """max |difference| of the cached points' impulses (normal, lateral 1, lateral 2) over the manifold slots both snapshots hold"""
+    worst = 0.0
+    for j in range(lay.nl):
+        for c in range(4):
+            ma, mb = lay.manifold(a, j, c), lay.manifold(b, j, c)
+            if ma[0] != 0 and mb[0] != 0:
+                worst = max(worst, float(np.abs(ma[7:10] - mb[7:10]).max()))
+    return worst
+
+
+def envelope(orc, orc2, lay, jt, before, after, rng, replicas, impulses=False):
+    """worst |dq|, |dqd| (and, with impulses, worst cached-point impulse difference) of the replicas that keep the contact counts of
+    `after`, and the number of replicas that changed them"""
+    worst_q = worst_qd = worst_imp = 0.0
     flips = 0
     for _ in range(replicas):
         orc2.set_snapshot(perturb(lay, before, rng))
@@ -43,6 +56,9 @@ def envelope(orc, orc2, lay, jt, before, after, rng, replicas):
             continue
         eq, eqd = compare_sim_state(lay, after, s2, jt)
         worst_q, worst_qd = max(worst_q, eq), max(worst_qd, eqd)
+        worst_imp = max(worst_imp, impulse_err(lay, after, s2))
+    if impulses:
+        return worst_q, worst_qd, flips, worst_imp
     return worst_q, worst_qd, flips
 
 
