@@ -64,7 +64,8 @@ EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "
            "dm_set_snapshot", "dm_state_size", "dm_save_state", "dm_load_state", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
            "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy", "dm_td_lambda_returns", "dm_mlp_set_weights_device", "dm_learn_create",
            "dm_mlp_set_normalizers_device", "dm_learn_set_weights", "dm_learn_step", "dm_learn_disc_step", "dm_learn_destroy",
-           "dm_learn_create_gated", "dm_learn_set_gated_weights", "dm_learn_gated_step", "dm_mlp_set_gated_weights_device", "dm_mlp_set_gated_normalizers_device"]
+           "dm_learn_create_gated", "dm_learn_set_gated_weights", "dm_learn_gated_step", "dm_mlp_set_gated_weights_device", "dm_mlp_set_gated_normalizers_device",
+           "dm_learn_grad_size", "dm_learn_grad", "dm_learn_apply", "dm_learn_gated_grad", "dm_learn_gated_apply", "dm_learn_disc_grad", "dm_learn_disc_apply"]
 
 
 def lib():
@@ -162,6 +163,11 @@ def lib():
         L.dm_learn_gated_step.argtypes = [vp, C.POINTER(DmLearnGatedNet), C.POINTER(DmLearnGatedBatch), vp]
         L.dm_mlp_set_gated_weights_device.argtypes = [vp, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), vp]
         L.dm_mlp_set_gated_normalizers_device.argtypes = [vp] * 8
+        L.dm_learn_grad_size.restype = C.c_longlong
+        L.dm_learn_grad_size.argtypes = [vp]
+        for kind, net, batch in (("", DmLearnNet, DmLearnBatch), ("gated_", DmLearnGatedNet, DmLearnGatedBatch), ("disc_", DmLearnNet, DmLearnDiscBatch)):
+            getattr(L, "dm_learn_%sgrad" % kind).argtypes = [vp, C.POINTER(net), C.POINTER(batch), vp, vp]
+            getattr(L, "dm_learn_%sapply" % kind).argtypes = [vp, C.POINTER(net), C.POINTER(batch), vp, C.c_float, vp]
         _lib = L
     return _lib
 
@@ -727,6 +733,38 @@ class TensorCoreLearner:
     def step(self, batch, stream=None):
         """batch: a DmLearnBatch (kinds "actor", "critic"), a DmLearnDiscBatch (kind "disc") or a DmLearnGatedBatch (TensorCoreGatedLearner)"""
         _call(self._step_fn(), self.h, C.byref(self.net), C.byref(batch), stream=stream)
+
+    # ---- the step split around its gradient (data-parallel training): step(b) == grad(b, g); apply(b, g, 1.0), bit for bit
+    def grad_size(self):
+        """dm_learn_grad_size: the floats of the flat gradient, the parameter pairs of self.layers as [weight, bias] each"""
+        return int(lib().dm_learn_grad_size(self.h))
+
+    def grad_views(self, grad):
+        """{parameter: view of the flat gradient `grad` (a tensor of grad_size() floats) with the parameter's shape}"""
+        views, off = {}, 0
+        for l in self.layers:
+            for p in (l.weight, l.bias):
+                views[p] = grad[off:off + p.numel()].view(p.shape)
+                off += p.numel()
+        return views
+
+    def _check_grad(self, grad, what):
+        import torch
+        _check_device_f32(grad, what, (self.grad_size(),), torch.device("cuda", self.device))
+
+    def grad(self, batch, grad, stream=None):
+        """dm_learn_(gated_|disc_)grad: the step's forward, head (its statistics accumulate) and backward, then the mean gradient over the
+        batch's rows without the weight decay (and logit regulariser) into `grad`, a contiguous float32 CUDA tensor of grad_size() floats;
+        the parameters are not changed"""
+        self._check_grad(grad, "grad")
+        _call(self._step_fn().replace("_step", "_grad"), self.h, C.byref(self.net), C.byref(batch), C.c_void_p(grad.data_ptr()), stream=stream)
+
+    def apply(self, batch, grad, scale=1.0, stream=None):
+        """dm_learn_(gated_|disc_)apply: the optimiser step on scale * grad plus the weight decay (and logit regulariser) with the batch's
+        stepsize and momentum, and the re-tiling"""
+        self._check_grad(grad, "apply")
+        _call(self._step_fn().replace("_step", "_apply"), self.h, C.byref(self.net), C.byref(batch), C.c_void_p(grad.data_ptr()),
+              C.c_float(scale), stream=stream)
 
     def close(self):
         if self.h:

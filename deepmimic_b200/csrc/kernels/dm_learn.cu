@@ -365,4 +365,53 @@ __global__ void __launch_bounds__(256) dm_learn_disc_layer_kernel(LearnDiscLayer
     if (D.p_tiles) learn_put(D.p_tiles, learn_tile_off(k, n, D.p_NC, 128), 128, w);
 }
 
+// ---- the step split in two for data-parallel training (dm_learn_*grad, dm_learn_*apply): the layer passes above, cut after the gradient's
+// reduction over the step's rows.  Between the halves the callers sum the ranks' gradients.  The arithmetic is the layer passes', operation
+// for operation; the intrinsics pin the rounding nvcc's contraction gives the fused kernels (an FMUL by 1 / rows, FFMAs for the penalty, the
+// weight decay, the momentum and the step), so apply(grad(b), scale 1) reproduces the fused step bit for bit.
+
+// the mean gradient of one parameter pair without its weight decay: g = (sum dW + gp_w sum dW_pen) / rows on the weights, (sum db) / rows on the
+// biases, the split partials summed in dm_learn_layer_kernel's order.  D.pen null: the PPO networks.  grid as dm_learn_layer_kernel
+__global__ void __launch_bounds__(256) dm_learn_pack_kernel(LearnDiscLayerParams D, LearnGradParams G) {
+    const LearnLayerParams& L = D.L;
+    const int k = blockIdx.x * 256 + threadIdx.x, n = blockIdx.y;
+    if (k > L.in_dim) return;
+    const bool bias = k == L.in_dim;
+    float g = 0.f;
+    for (int z = 0; z < L.splits; ++z) g += L.partial[(static_cast<size_t>(z) * L.Npad + n) * L.F + k];
+    if (!bias && D.pen) {
+        float q = 0.f;
+        for (int z = 0; z < D.pen_splits; ++z) q += D.pen[(static_cast<size_t>(z) * L.Npad + n) * D.pen_F + k];
+        g = __fmaf_rn(D.gp_w, q, g);
+    }
+    g = __fmul_rn(g, L.inv_rows);
+    if (bias) G.b[n] = g;
+    else G.w[static_cast<size_t>(n) * L.in_dim + k] = g;
+}
+
+// the optimiser half: g = scale G + (wd + reg) w on the weights, scale G on the biases; then the momentum step and the re-tiling of
+// dm_learn_disc_layer_kernel (D.reg = 0 and no p_tiles: dm_learn_layer_kernel's)
+__global__ void __launch_bounds__(256) dm_learn_apply_kernel(LearnDiscLayerParams D, LearnGradParams G) {
+    const LearnLayerParams& L = D.L;
+    const int k = blockIdx.x * 256 + threadIdx.x, n = blockIdx.y;
+    if (k > L.in_dim) return;
+    const bool bias = k == L.in_dim;
+    float* p = bias ? L.b + n : L.w + static_cast<size_t>(n) * L.in_dim + k;
+    float w = *p;
+    float g = __fmul_rn(bias ? G.b[n] : G.w[static_cast<size_t>(n) * L.in_dim + k], G.scale);
+    if (!bias) g = __fmaf_rn(__fadd_rn(L.wd, D.reg), w, g);
+    float* a = bias ? L.acc_b + n : L.acc_w + static_cast<size_t>(n) * L.in_dim + k;
+    const float acc = __fmaf_rn(L.mom, *a, g);
+    *a = acc;
+    w = __fmaf_rn(-L.lr, acc, w);
+    *p = w;
+    if (bias) {
+        L.bias_pad[n] = w;
+        return;
+    }
+    learn_put(L.tiles, learn_tile_off(k, n, L.NC, L.BN), L.BN, w);
+    if (L.t_tiles) learn_put(L.t_tiles, learn_tile_off(n, k, L.t_NC, 128), 128, w);
+    if (D.p_tiles) learn_put(D.p_tiles, learn_tile_off(k, n, D.p_NC, 128), 128, w);
+}
+
 }  // namespace dmk

@@ -161,6 +161,12 @@ struct LearnDiscLayerParams {
     __half* p_tiles;           // layer 0, or null: W0's forward tiles with K padded to p_NC * 64 (B of the penalty's W0 e GEMM)
     int p_NC;
 };
+// one parameter pair's slice of a flat gradient buffer (dm_learn_grad, dm_learn_apply): w [out x in], b [out]; the apply pass reads scale * it
+struct LearnGradParams {
+    float* w;
+    float* b;
+    float scale;
+};
 
 // ---- kernels/dm_mlp.cu
 __global__ void dm_mlp_prep_kernel(MlpPrepParams);
@@ -191,5 +197,7 @@ __global__ void dm_learn_disc_head_kernel(LearnDiscHeadParams);
 __global__ void dm_learn_disc_gp_kernel(const __half*, int, float*);
 __global__ void dm_learn_disc_stats_kernel(const float*, int, const float*, int, float, float*);
 __global__ void dm_learn_disc_layer_kernel(LearnDiscLayerParams);
+__global__ void dm_learn_pack_kernel(LearnDiscLayerParams, LearnGradParams);
+__global__ void dm_learn_apply_kernel(LearnDiscLayerParams, LearnGradParams);
 
 }  // namespace dmk

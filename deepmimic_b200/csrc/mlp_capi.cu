@@ -3,7 +3,8 @@
 // trunk layers, output layer), four for the AMP discriminator's style reward (operand preparation, two GEMMs, the logit head with the reward
 // epilogue); the learner-side TD(lambda) return scan of a rollout window (kernels/dm_returns.cu, one launch); and the PPO learner's minibatch
 // step (dm_learn_*: kernels/dm_learn.cu and the backward GEMMs of kernels/dm_mlp.cu, 15 launches; 32 for the gated networks,
-// dm_learn_gated_step) with the device-side re-tiling of plain and gated handles (dm_mlp_set_weights_device, dm_mlp_set_gated_weights_device).
+// dm_learn_gated_step), the same step split around a flat gradient for data-parallel training (dm_learn_*grad, dm_learn_*apply), with the
+// device-side re-tiling of plain and gated handles (dm_mlp_set_weights_device, dm_mlp_set_gated_weights_device).
 // The parameter structs and kernel declarations are kernels/dm_mlp.cuh, shared with the kernels.
 // Same library, same rules: no CPU fallback, errors through dm_last_error.
 #include <cuda_fp16.h>
@@ -520,21 +521,43 @@ void launch_ppo_head(const dm_learn* l, const dm_learn_batch* b, int mt, cudaStr
     else dmk::dm_learn_critic_head_kernel<<<mt, 128, 0, st>>>(H);
     dmk::dm_learn_stats_kernel<<<1, 1, 0, st>>>(l->head_partials, mt, 1.f / b->rows, actor ? 1 : 0, b->stats);
 }
+// what a layer pass does with a step's dW partials: the fused optimiser step (or, without a batch, the re-tiling alone), or one half of the
+// split step: the mean gradient packed into a flat buffer (dm_learn_*grad), or the optimiser step on scale times such a buffer (dm_learn_*apply)
+enum class Pass { step, pack, apply };
+// the pass of one parameter pair (kind 2: the discriminator's layer kernel for the fused step); its slice of the flat gradient `grad` starts
+// at *off (weights, then the bias), and *off moves past it
+void launch_pass(Pass pass, const dmk::LearnDiscLayerParams& D, bool disc, float* grad, float scale, size_t* off, cudaStream_t st) {
+    const dim3 grid((D.L.in_dim + 1 + 255) / 256, D.L.out_dim);
+    const size_t nw = static_cast<size_t>(D.L.out_dim) * D.L.in_dim;
+    const dmk::LearnGradParams G{grad ? grad + *off : nullptr, grad ? grad + *off + nw : nullptr, scale};
+    *off += nw + D.L.out_dim;
+    if (pass == Pass::pack) dmk::dm_learn_pack_kernel<<<grid, 256, 0, st>>>(D, G);
+    else if (pass == Pass::apply) dmk::dm_learn_apply_kernel<<<grid, 256, 0, st>>>(D, G);
+    else if (disc) dmk::dm_learn_disc_layer_kernel<<<grid, 256, 0, st>>>(D);
+    else launch_layer(D.L, st);
+}
 // the forward tiles of the learner's handle and the transposed tiles of the dX GEMMs; with `b` also the optimiser step before the re-tiling
-void learn_layers(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, const int* splits, cudaStream_t st) {
+// (or the split step's pass: pack, apply on the flat gradient `grad`)
+void learn_layers(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, const int* splits, cudaStream_t st, Pass pass = Pass::step,
+                  float* grad = nullptr, float scale = 1.f) {
+    size_t off = 0;
     for (int i = 0; i < 3; ++i) {
-        dmk::LearnLayerParams L = layer_params(l->m, i, net->w[i], net->b[i]);
+        dmk::LearnDiscLayerParams D{};
+        dmk::LearnLayerParams& L = D.L;
+        L = layer_params(l->m, i, net->w[i], net->b[i]);
         if (i > 0) { L.t_tiles = l->wt[i]; L.t_NC = l->Nout[i] / 64; }
         if (b) {
             L.partial = l->partial[i]; L.Npad = l->Nout[i]; L.F = l->F[i];
             optimiser_fields(L, net, i, b, splits[i]);
         }
-        launch_layer(L, st);
+        launch_pass(pass, D, false, grad, scale, &off, st);
     }
 }
 // the discriminator's layer passes (kind 2): W0^T and W0's K-padded tiles for the penalty as well; with `b` also the optimiser step with the
-// penalty's partials (psplits of them) and the logit regulariser
-void learn_disc_layers(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* b, const int* splits, const int* psplits, cudaStream_t st) {
+// penalty's partials (psplits of them) and the logit regulariser (or the split step's pass, as learn_layers)
+void learn_disc_layers(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* b, const int* splits, const int* psplits, cudaStream_t st,
+                       Pass pass = Pass::step, float* grad = nullptr, float scale = 1.f) {
+    size_t off = 0;
     for (int i = 0; i < 3; ++i) {
         dmk::LearnDiscLayerParams D{};
         D.L = layer_params(l->m, i, net->w[i], net->b[i]);
@@ -545,7 +568,7 @@ void learn_disc_layers(dm_learn* l, const dm_learn_net* net, const dm_learn_disc
             optimiser_fields(D.L, net, i, b, splits[i]);
             D.pen = l->pen[i]; D.pen_splits = psplits[i]; D.pen_F = l->pen_F[i]; D.gp_w = b->grad_penalty_weight; D.reg = i == 2 ? b->logit_reg_weight : 0.f;
         }
-        dmk::dm_learn_disc_layer_kernel<<<dim3((D.L.in_dim + 1 + 255) / 256, D.L.out_dim), 256, 0, st>>>(D);
+        launch_pass(pass, D, true, grad, scale, &off, st);
     }
 }
 // the forward over the mt m tiles prepared in the handle's obs_t (the output layer writes `rows` rows of l->out) and the transposition of the
@@ -586,18 +609,36 @@ int dm_learn_set_weights(dm_learn* l, const dm_learn_net* net, void* stream) {
     return launch_status("dm_learn_set_weights");
 }
 
-int dm_learn_step(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, void* stream) {
-    const char* fn = "dm_learn_step";
-    if (!l) return mlp_fail("dm_learn_step: null handle");
-    if (l->gated) return mlp_fail("dm_learn_step: the workspace holds a gated network (dm_learn_create_gated); use dm_learn_gated_step");
-    if (l->kind == 2) return mlp_fail("dm_learn_step: the workspace is a discriminator's (kind 2); use dm_learn_disc_step");
-    if (learn_net_check(net, fn) || ppo_batch_check(fn, l, b, nullptr)) return 1;
+namespace {
+// the checks of the split step's calls on workspace l: `gated` names the gated entries, `disc` the discriminator's; fn names the caller
+int split_kind_check(const char* fn, const dm_learn* l, bool gated, bool disc) {
+    const std::string f(fn);
+    if (!l) return mlp_fail(f + ": null handle");
+    if (gated && !l->gated) return mlp_fail(f + ": the workspace holds a plain network (dm_learn_create)");
+    if (!gated && l->gated) return mlp_fail(f + ": the workspace holds a gated network (dm_learn_create_gated)");
+    if (disc && l->kind != 2) return mlp_fail(f + ": the workspace is a PPO actor's or critic's (kind 0 or 1); the discriminator's entries need kind 2");
+    if (!disc && l->kind == 2) return mlp_fail(f + ": the workspace is a discriminator's (kind 2)");
+    return 0;
+}
+// the split counts of an apply: it reads no dW partials
+constexpr int kNoSplits[4] = {0, 0, 0, 0};
+// the optimiser fields an apply reads
+int apply_check(const char* fn, const void* b, const float* d_grad, float scale, float stepsize, float momentum, float weight_decay, float reg) {
+    const std::string f(fn);
+    if (!b) return mlp_fail(f + ": null batch");
+    if (!d_grad) return mlp_fail(f + ": null gradient pointer");
+    if (!std::isfinite(scale)) return mlp_fail(f + ": scale must be finite");
+    if (!(stepsize >= 0.f) || !(momentum >= 0.f) || !(weight_decay >= 0.f) || !(reg >= 0.f))
+        return mlp_fail(f + ": stepsize, momentum, weight_decay (and logit_reg_weight) must be >= 0");
+    return 0;
+}
+// a PPO step up to its layer pass: the split-K plan of the three dW GEMMs (splits), the forward, the loss head with its statistics and the
+// backward
+int ppo_forward_backward(dm_learn* l, const dm_learn_batch* b, const char* fn, int* splits, cudaStream_t st) {
     dm_mlp* m = l->m;
-    if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_learn_step: cudaSetDevice failed");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int rows = b->rows, mt = (rows + 127) / 128, chunks = 2 * mt;
     // split-K of the three dW GEMMs for this row count (the workspace holds the largest over every row count, dm_learn_create)
-    int splits[3], cps[3];
+    int cps[3];
     for (int i = 0; i < 3; ++i)
         if (dw_plan(fn, l->F[i], l->Nout[i], trunk_bn(l, i), chunks, l->max_splits[i], &splits[i], &cps[i])) return 1;
     // forward: gathered rows -> the plain trunk -> the normalised output (identity output normaliser)
@@ -607,8 +648,87 @@ int dm_learn_step(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b,
     // loss head: dY of the output layer, the loss partials, the statistics
     launch_ppo_head(l, b, mt, st);
     learn_backward(l, rows, mt, splits, cps, st);
+    return 0;
+}
+int disc_batch_check(const char* fn, const dm_learn* l, const dm_learn_disc_batch* b) {
+    const std::string f(fn);
+    if (!b) return mlp_fail(f + ": null batch");
+    if (b->rows <= 0 || b->rows > l->side_rows) return mlp_fail(f + ": rows out of range (1 to max_rows / 2 per side)");
+    if (!b->agent || !b->expert || !b->agent_idx || !b->expert_idx || !b->in_mean || !b->in_istd || !b->stats)
+        return mlp_fail(f + ": null observation, index, normaliser or statistics pointer");
+    if (!(b->stepsize >= 0.f) || !(b->momentum >= 0.f) || !(b->weight_decay >= 0.f) || !(b->logit_reg_weight >= 0.f) || !(b->grad_penalty_weight >= 0.f))
+        return mlp_fail(f + ": stepsize, momentum, weight_decay, logit_reg_weight and grad_penalty_weight must be >= 0");
+    return 0;
+}
+int disc_forward_backward(dm_learn* l, const dm_learn_disc_batch* b, const char* fn, int* splits, int* psplits, cudaStream_t st);
+}  // namespace
+
+int dm_learn_step(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, void* stream) {
+    const char* fn = "dm_learn_step";
+    if (!l) return mlp_fail("dm_learn_step: null handle");
+    if (l->gated) return mlp_fail("dm_learn_step: the workspace holds a gated network (dm_learn_create_gated); use dm_learn_gated_step");
+    if (l->kind == 2) return mlp_fail("dm_learn_step: the workspace is a discriminator's (kind 2); use dm_learn_disc_step");
+    if (learn_net_check(net, fn) || ppo_batch_check(fn, l, b, nullptr)) return 1;
+    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_step: cudaSetDevice failed");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int splits[3];
+    if (ppo_forward_backward(l, b, fn, splits, st)) return 1;
     // optimiser step and re-tiling, after every GEMM that read the old weights
     learn_layers(l, net, b, splits, st);
+    return launch_status(fn);
+}
+
+long long dm_learn_grad_size(const dm_learn* l) {
+    if (!l) { mlp_fail("dm_learn_grad_size: null handle"); return -1; }
+    long long n = 0;
+    for (int i = 0; i < (l->gated ? 10 : 3); ++i) {
+        const dmk::LearnLayerParams L = l->gated ? gated_layer_params(l->m, i, nullptr, nullptr) : layer_params(l->m, i, nullptr, nullptr);
+        n += static_cast<long long>(L.out_dim) * (L.in_dim + 1);
+    }
+    return n;
+}
+
+int dm_learn_grad(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, float* d_grad, void* stream) {
+    const char* fn = "dm_learn_grad";
+    if (split_kind_check(fn, l, false, false) || learn_net_check(net, fn) || ppo_batch_check(fn, l, b, nullptr)) return 1;
+    if (!d_grad) return mlp_fail("dm_learn_grad: null gradient pointer");
+    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_grad: cudaSetDevice failed");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int splits[3];
+    if (ppo_forward_backward(l, b, fn, splits, st)) return 1;
+    learn_layers(l, net, b, splits, st, Pass::pack, d_grad);
+    return launch_status(fn);
+}
+
+int dm_learn_apply(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, const float* d_grad, float scale, void* stream) {
+    const char* fn = "dm_learn_apply";
+    if (split_kind_check(fn, l, false, false) || learn_net_check(net, fn)) return 1;
+    if (apply_check(fn, b, d_grad, scale, b ? b->stepsize : 0.f, b ? b->momentum : 0.f, b ? b->weight_decay : 0.f, 0.f)) return 1;
+    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_apply: cudaSetDevice failed");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    learn_layers(l, net, b, kNoSplits, st, Pass::apply, const_cast<float*>(d_grad), scale);
+    return launch_status(fn);
+}
+
+int dm_learn_disc_grad(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* b, float* d_grad, void* stream) {
+    const char* fn = "dm_learn_disc_grad";
+    if (split_kind_check(fn, l, false, true) || learn_net_check(net, fn) || disc_batch_check(fn, l, b)) return 1;
+    if (!d_grad) return mlp_fail("dm_learn_disc_grad: null gradient pointer");
+    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_disc_grad: cudaSetDevice failed");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int splits[3], psplits[3];
+    if (disc_forward_backward(l, b, fn, splits, psplits, st)) return 1;
+    learn_disc_layers(l, net, b, splits, psplits, st, Pass::pack, d_grad);
+    return launch_status(fn);
+}
+
+int dm_learn_disc_apply(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* b, const float* d_grad, float scale, void* stream) {
+    const char* fn = "dm_learn_disc_apply";
+    if (split_kind_check(fn, l, false, true) || learn_net_check(net, fn)) return 1;
+    if (apply_check(fn, b, d_grad, scale, b ? b->stepsize : 0.f, b ? b->momentum : 0.f, b ? b->weight_decay : 0.f, b ? b->logit_reg_weight : 0.f)) return 1;
+    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_disc_apply: cudaSetDevice failed");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    learn_disc_layers(l, net, b, kNoSplits, kNoSplits, st, Pass::apply, const_cast<float*>(d_grad), scale);
     return launch_status(fn);
 }
 
@@ -617,19 +737,24 @@ int dm_learn_disc_step(dm_learn* l, const dm_learn_net* net, const dm_learn_disc
     if (!l) return mlp_fail("dm_learn_disc_step: null handle");
     if (l->gated) return mlp_fail("dm_learn_disc_step: the workspace holds a gated network (dm_learn_create_gated); a discriminator step needs kind 2");
     if (l->kind != 2) return mlp_fail("dm_learn_disc_step: the workspace is a PPO actor's or critic's (kind 0 or 1); a discriminator step needs kind 2");
-    if (learn_net_check(net, fn)) return 1;
-    if (!b) return mlp_fail("dm_learn_disc_step: null batch");
-    if (b->rows <= 0 || b->rows > l->side_rows) return mlp_fail("dm_learn_disc_step: rows out of range (1 to max_rows / 2 per side)");
-    if (!b->agent || !b->expert || !b->agent_idx || !b->expert_idx || !b->in_mean || !b->in_istd || !b->stats)
-        return mlp_fail("dm_learn_disc_step: null observation, index, normaliser or statistics pointer");
-    if (!(b->stepsize >= 0.f) || !(b->momentum >= 0.f) || !(b->weight_decay >= 0.f) || !(b->logit_reg_weight >= 0.f) || !(b->grad_penalty_weight >= 0.f))
-        return mlp_fail("dm_learn_disc_step: stepsize, momentum, weight_decay, logit_reg_weight and grad_penalty_weight must be >= 0");
-    dm_mlp* m = l->m;
-    if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_learn_disc_step: cudaSetDevice failed");
+    if (learn_net_check(net, fn) || disc_batch_check(fn, l, b)) return 1;
+    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_disc_step: cudaSetDevice failed");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int splits[3], psplits[3];
+    if (disc_forward_backward(l, b, fn, splits, psplits, st)) return 1;
+    // optimiser step and re-tiling, after every GEMM that read the old weights
+    learn_disc_layers(l, net, b, splits, psplits, st);
+    return launch_status(fn);
+}
+
+namespace {
+// a discriminator step up to its layer pass: the split-K plans of the dW GEMMs (splits) and of the penalty's (psplits), the forward over both
+// sides, the least-squares head, the backward, the gradient penalty's GEMMs and the statistics
+int disc_forward_backward(dm_learn* l, const dm_learn_disc_batch* b, const char* fn, int* splits, int* psplits, cudaStream_t st) {
+    dm_mlp* m = l->m;
     // agent rows in m tiles [0, et), expert rows in [et, 2 et)
     const int rows = b->rows, E = pad_to(rows, 128), et = E / 128, mt = 2 * et, chunks = 2 * mt, echunks = 2 * et;
-    int splits[3], cps[3], psplits[3], pcps[3];
+    int cps[3], pcps[3];
     for (int i = 0; i < 3; ++i)
         if (dw_plan(fn, l->F[i], l->Nout[i], trunk_bn(l, i), chunks, l->max_splits[i], &splits[i], &cps[i]) ||
             dw_plan(fn, l->pen_F[i], l->Nout[i], trunk_bn(l, i), echunks, l->pen_max_splits[i], &psplits[i], &pcps[i]))
@@ -671,10 +796,9 @@ int dm_learn_disc_step(dm_learn* l, const dm_learn_net* net, const dm_learn_disc
     const __half* pen_b[3] = {l->u_b[0], l->u_b[1], l->seed_b};
     for (int i = 0; i < 3; ++i) launch_dw(l->pt[i], pen_b[i], l->pen[i], l->pen_F[i], l->Nout[i], trunk_bn(l, i), echunks, psplits[i], pcps[i], st);
     dmk::dm_learn_disc_stats_kernel<<<1, 1, 0, st>>>(l->head_partials, mt, l->gp_partials, et, 1.f / rows, b->stats);
-    // optimiser step and re-tiling, after every GEMM that read the old weights
-    learn_disc_layers(l, net, b, splits, psplits, st);
-    return launch_status(fn);
+    return 0;
 }
+}  // namespace
 
 dm_learn* dm_learn_create_gated(int device, int kind, int in_dim, int goal_dim, int h0, int h1, int out_dim, int gate_common, int gate_hidden, int max_rows) {
     if (kind != 0 && kind != 1) { mlp_fail("dm_learn_create_gated: kind must be 0 (actor) or 1 (critic)"); return nullptr; }
@@ -739,12 +863,16 @@ int s_chunk(const dm_learn* l, int layer) { return layer ? 2 * l->m->N0 / 64 : 0
 int t_chunk(const dm_learn* l, int layer) { return s_chunk(l, layer) + (layer ? l->m->N1 : l->m->N0) / 64; }
 // the ten layer passes of a gated workspace: the forward tiles, and the B operands of the dX GEMMs (W1^T, W2^T, the block-diagonal
 // [Ws_l^T, Wt_l^T], [Wgh_0 | Wgh_1]^T); with `b` also the optimiser step on the dW partials (split counts: splits for the trunk, gsplits
-// for the gate's GEMMs)
-void learn_gated_layers(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_batch* b, const int* splits, const int* gsplits, cudaStream_t st) {
+// for the gate's GEMMs; or the split step's pass, as learn_layers)
+void learn_gated_layers(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_batch* b, const int* splits, const int* gsplits, cudaStream_t st,
+                        Pass pass = Pass::step, float* grad = nullptr, float scale = 1.f) {
     dm_mlp* m = l->m;
     const size_t tt = 2 * 128 * 64;   // halves of a hi + lo 128 x 64 B tile
+    size_t off = 0;
     for (int i = 0; i < 10; ++i) {
-        dmk::LearnLayerParams L = gated_layer_params(m, i, net->w[i], net->b[i]);
+        dmk::LearnDiscLayerParams D{};
+        dmk::LearnLayerParams& L = D.L;
+        L = gated_layer_params(m, i, net->w[i], net->b[i]);
         const int lay = i & 1;
         int s = 0;
         if (i < 3) {
@@ -756,13 +884,13 @@ void learn_gated_layers(dm_learn* l, const dm_learn_gated_net* net, const dm_lea
             L.t_tiles = l->wght + lay * tt; L.t_NC = 2;
             L.partial = l->gpartial[2] + static_cast<size_t>(64 * lay) * l->gF[2]; L.Npad = 128; L.F = l->gF[2]; s = b ? gsplits[2] : 0;
         } else {
-            const bool scale = i < 8;
+            const bool gate_scale = i < 8;
             const int N = lay ? m->N1 : m->N0;
-            L.t_tiles = l->wst + static_cast<size_t>(scale ? s_chunk(l, lay) : t_chunk(l, lay)) * tt + 512 * lay; L.t_NC = l->KS;
-            L.partial = l->gpartial[lay] + (scale ? 0 : static_cast<size_t>(N) * l->gF[lay]); L.Npad = 2 * N; L.F = l->gF[lay]; s = b ? gsplits[lay] : 0;
+            L.t_tiles = l->wst + static_cast<size_t>(gate_scale ? s_chunk(l, lay) : t_chunk(l, lay)) * tt + 512 * lay; L.t_NC = l->KS;
+            L.partial = l->gpartial[lay] + (gate_scale ? 0 : static_cast<size_t>(N) * l->gF[lay]); L.Npad = 2 * N; L.F = l->gF[lay]; s = b ? gsplits[lay] : 0;
         }
         if (b) optimiser_fields(L, net, i, b, s);
-        launch_layer(L, st);
+        launch_pass(pass, D, false, grad, scale, &off, st);
     }
 }
 // the gated forward over the mt m tiles prepared in obs_t / goal_t (dm_mlp_forward_gated, with the gated layers saving their factors) and the
@@ -821,17 +949,14 @@ int dm_learn_set_gated_weights(dm_learn* l, const dm_learn_gated_net* net, void*
     return launch_status("dm_learn_set_gated_weights");
 }
 
-int dm_learn_gated_step(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_gated_batch* gb, void* stream) {
-    const char* fn = "dm_learn_gated_step";
-    if (!l) return mlp_fail("dm_learn_gated_step: null handle");
-    if (!l->gated) return mlp_fail("dm_learn_gated_step: the workspace holds a plain network (dm_learn_create); use dm_learn_step");
-    const dm_learn_batch* b = gb ? &gb->batch : nullptr;
-    if (gated_net_check(net, fn) || ppo_batch_check(fn, l, b, gb)) return 1;
+namespace {
+// a gated PPO step up to its layer passes: the split-K plans of the trunk's (splits) and the gate's (gsplits) dW GEMMs, the forward, the loss
+// head with its statistics and the gated backward
+int gated_forward_backward(dm_learn* l, const dm_learn_gated_batch* gb, const char* fn, int* splits, int* gsplits, cudaStream_t st) {
     dm_mlp* m = l->m;
-    if (cudaSetDevice(m->device) != cudaSuccess) return mlp_fail("dm_learn_gated_step: cudaSetDevice failed");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const dm_learn_batch* b = &gb->batch;
     const int rows = b->rows, mt = (rows + 127) / 128, chunks = 2 * mt;
-    int splits[3], cps[3], gsplits[4], gcps[4];
+    int cps[3], gcps[4];
     for (int i = 0; i < 3; ++i)
         if (dw_plan(fn, l->F[i], l->Nout[i], trunk_bn(l, i), chunks, l->max_splits[i], &splits[i], &cps[i])) return 1;
     for (int j = 0; j < 4; ++j)
@@ -844,8 +969,46 @@ int dm_learn_gated_step(dm_learn* l, const dm_learn_gated_net* net, const dm_lea
     // the loss heads act on the output only: the plain step's
     launch_ppo_head(l, b, mt, st);
     learn_gated_backward(l, mt, splits, cps, gsplits, gcps, st);
+    return 0;
+}
+}  // namespace
+
+int dm_learn_gated_step(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_gated_batch* gb, void* stream) {
+    const char* fn = "dm_learn_gated_step";
+    if (!l) return mlp_fail("dm_learn_gated_step: null handle");
+    if (!l->gated) return mlp_fail("dm_learn_gated_step: the workspace holds a plain network (dm_learn_create); use dm_learn_step");
+    const dm_learn_batch* b = gb ? &gb->batch : nullptr;
+    if (gated_net_check(net, fn) || ppo_batch_check(fn, l, b, gb)) return 1;
+    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_gated_step: cudaSetDevice failed");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int splits[3], gsplits[4];
+    if (gated_forward_backward(l, gb, fn, splits, gsplits, st)) return 1;
     // optimiser step and re-tiling, after every GEMM that read the old weights
     learn_gated_layers(l, net, b, splits, gsplits, st);
+    return launch_status(fn);
+}
+
+int dm_learn_gated_grad(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_gated_batch* gb, float* d_grad, void* stream) {
+    const char* fn = "dm_learn_gated_grad";
+    const dm_learn_batch* b = gb ? &gb->batch : nullptr;
+    if (split_kind_check(fn, l, true, false) || gated_net_check(net, fn) || ppo_batch_check(fn, l, b, gb)) return 1;
+    if (!d_grad) return mlp_fail("dm_learn_gated_grad: null gradient pointer");
+    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_gated_grad: cudaSetDevice failed");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int splits[3], gsplits[4];
+    if (gated_forward_backward(l, gb, fn, splits, gsplits, st)) return 1;
+    learn_gated_layers(l, net, b, splits, gsplits, st, Pass::pack, d_grad);
+    return launch_status(fn);
+}
+
+int dm_learn_gated_apply(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_gated_batch* gb, const float* d_grad, float scale, void* stream) {
+    const char* fn = "dm_learn_gated_apply";
+    const dm_learn_batch* b = gb ? &gb->batch : nullptr;
+    if (split_kind_check(fn, l, true, false) || gated_net_check(net, fn)) return 1;
+    if (apply_check(fn, b, d_grad, scale, b ? b->stepsize : 0.f, b ? b->momentum : 0.f, b ? b->weight_decay : 0.f, 0.f)) return 1;
+    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_gated_apply: cudaSetDevice failed");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    learn_gated_layers(l, net, b, kNoSplits, kNoSplits, st, Pass::apply, const_cast<float*>(d_grad), scale);
     return launch_status(fn);
 }
 

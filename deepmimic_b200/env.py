@@ -148,6 +148,12 @@ class DeepMimicBatchEnv:
         self._pre(); self._core.amp_obs_expert(buf, kin_time); self._post()
         return buf
 
+    def expert_sample_count(self, set_to=None):
+        """the expert sampler's call counter, the key of sample_amp_obs_expert's next draws (dm_expert_sample_count); set_to replaces it.
+        Returns the value before the call.  Handles of one seed draw the same rows at the same count: data-parallel ranks start from
+        disjoint counts."""
+        return self._core.expert_sample_count(set_to)
+
     def sample_amp_obs_expert(self, rows):
         """[rows, amp_obs_size] float32: `rows` expert AMP observations (any count), clip and time drawn on the device per row
         (dm_sample_amp_obs_expert).  A new tensor each call, allocated on the caller's current stream and complete before that stream's next

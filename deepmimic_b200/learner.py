@@ -19,8 +19,15 @@ The reference tree is not vendored here; its rules are restated below, one funct
 Documented deviations: minibatches are shuffled / drawn by a seeded torch.Generator on the data's device, not the reference's numpy stream; the
 statistics leave out the weight-decay (and logit-regulariser) terms of the losses (the reference's logged losses include them); the normalisers
 are not updated here (DeviceNormalizer.update stays the caller's call, as the reference's normaliser schedule is), nor are the AMP replay
-buffers kept (deepmimic_b200/trainer.py: DeviceReplayBuffer, with the TarClipFrac, exploration and normaliser schedules).  Not done: a
-multi-GPU gradient all-reduce.  The loop that drives both learners, with checkpoints, is deepmimic_b200/trainer.py: Trainer."""
+buffers kept (deepmimic_b200/trainer.py: DeviceReplayBuffer, with the TarClipFrac, exploration and normaliser schedules).  The loop that
+drives both learners, with checkpoints, is deepmimic_b200/trainer.py: Trainer.
+
+Data parallelism (mpi_run.py --num_workers N, solvers/mpi_solver.py: MPISolver): both learners take process_group=; with a group of more than
+one rank, the networks are broadcast from the group's first rank at construction (MPISolver.sync), and every minibatch step averages the
+ranks' flat gradients (one torch.distributed.all_reduce per network and step) before the weight decay and the momentum step, so every rank
+applies the same update and keeps the same weights.  The tensor-core backend splits its step around that sum (TensorCoreLearner.grad /
+apply).  The weight-decay terms are added once after the average: they depend on the weights alone, which are equal on every rank, so the
+result is MPISolver's average of the whole gradient.  Without a group, or with a group of one rank, the learners run exactly as without one."""
 import math
 
 ADV_EPS = 1e-5   # PPOAgent.ADV_EPS
@@ -108,6 +115,66 @@ def momentum_step(params, accs, grads, stepsize, momentum):
         p.sub_(stepsize * a)
 
 
+class DataParallel:
+    """A learner's ranks: the torch.distributed process group `group` of world > 1 ranks (NCCL on the GPUs; gloo also takes CPU and CUDA
+    tensors).  Collectives are stream-ordered on NCCL and add no host synchronisation there."""
+
+    def __init__(self, group):
+        import torch.distributed as dist
+        self.dist, self.group = dist, group
+        self.world = dist.get_world_size(group)
+        self.src = dist.get_global_rank(group, 0)
+
+    @staticmethod
+    def of(group):
+        """a DataParallel for `group`, or None without a group or with a group of one rank"""
+        if group is None:
+            return None
+        import torch.distributed as dist
+        return DataParallel(group) if dist.get_world_size(group) > 1 else None
+
+    def broadcast(self, tensors):
+        """the group's first rank's values into `tensors` on every rank (MPISolver.sync)"""
+        for x in tensors:
+            self.dist.broadcast(x.data, self.src, group=self.group)
+
+    def sum(self, x):
+        """x summed over the ranks, in place; returns x"""
+        self.dist.all_reduce(x, group=self.group)
+        return x
+
+    def mean_grads(self, grads):
+        """the ranks' mean of each gradient in `grads`: one all-reduce of their flat concatenation"""
+        import torch
+        flat = self.sum(torch.cat([g.reshape(-1) for g in grads])) / self.world
+        return [v.view_as(g) for v, g in zip(flat.split([g.numel() for g in grads]), grads)]
+
+    def mean_stats(self, values):
+        """the ranks' means of the 0-d tensors `values` (one all-reduce of their stack)"""
+        import torch
+        return list(self.sum(torch.stack([v.float().reshape(()) for v in values])) / self.world)
+
+    def check_window(self, n, explored):
+        """refuses, on every rank at once, a window size `n` (a host int) that differs between the ranks, or a window without an explored
+        sample on any rank (`explored`: a 0-d bool device tensor): a rank that ran more minibatch steps than another, or none, would leave the
+        others waiting for ever in a collective.  One all-reduce and one host synchronisation."""
+        import torch
+        x = torch.stack([torch.tensor(n, device=explored.device), torch.tensor(-n, device=explored.device), (~explored).long()])
+        self.dist.all_reduce(x, op=self.dist.ReduceOp.MAX, group=self.group)
+        hi, lo, empty = x.tolist()
+        if hi != n or -lo != n:
+            raise ValueError("data-parallel learner: the ranks' window sizes differ (%d to %d); every rank must run the same number of "
+                             "minibatch steps" % (-lo, hi))
+        if empty:
+            raise ValueError("data-parallel learner: a rank's window has no explored sample (the actor trains on explored actions only)")
+
+
+def _weight_decay_grads(net, params, grads, weight_decay):
+    """grads plus the gradient of weight_decay * weight_decay_loss(net): weight_decay w on the weights, nothing on the biases"""
+    names = {p: n for n, p in net.named_parameters()}
+    return [g + weight_decay * p.detach() if names[p].endswith("weight") else g for p, g in zip(params, grads)]
+
+
 def _check(name, v, lo, hi, lo_open=False, hi_open=False):
     bad = v is None or not (isinstance(v, (int, float)) and math.isfinite(float(v)))
     if not bad:
@@ -123,10 +190,18 @@ class PPOLearner:
     (s_norm, g_norm, a_norm, val_norm).  Every hyperparameter is required (the reference reads them from an agent file; the asset archive has none).
     The momentum accumulators are the learner's; after update() the torch modules hold the new weights and the rollout's tensor-core actor and
     critic, where they exist, hold those weights and the normalisers' statistics that the update trained with.  A normaliser updated after
-    update() reaches those handles with the next update() or with rollout.refresh_tensor_core_policy()."""
+    update() reaches those handles with the next update() or with rollout.refresh_tensor_core_policy().
+
+    process_group (data parallelism, see the module docstring): minibatch_size is the job's total (MiniBatchSize); each rank's minibatches have
+    ceil(minibatch_size / world) rows (the maintainer's reading of the reference's _local_mini_batch_size, not checked against its source).
+    The advantages are normalised over the rank's own explored samples (the reading of PPOAgent._update, which takes their mean and std over
+    the worker's samples; not checked against its source either).  Every rank's window must have the same size, so that all ranks run the
+    same number of minibatch steps, and at least one explored sample: update() refuses, on every rank, a window that breaks either (one more
+    host synchronisation).  update()'s statistics are the ranks' means (exp_samples: the ranks' total, an integer)."""
 
     def __init__(self, rollout, *, actor_stepsize=None, actor_momentum=None, actor_weight_decay=None, critic_stepsize=None, critic_momentum=None,
-                 critic_weight_decay=None, ratio_clip=None, norm_adv_clip=None, minibatch_size=None, epochs=None, backend="torch", seed=0):
+                 critic_weight_decay=None, ratio_clip=None, norm_adv_clip=None, minibatch_size=None, epochs=None, backend="torch", seed=0,
+                 process_group=None):
         import torch
         self.torch, self.ro = torch, rollout
         if rollout.critic is None:
@@ -143,7 +218,9 @@ class PPOLearner:
         for name, v in (("minibatch_size", minibatch_size), ("epochs", epochs)):
             if not isinstance(v, int) or isinstance(v, bool) or v < 1:
                 raise ValueError("%s must be a positive int (got %r)" % (name, v))
-        self.minibatch_size, self.epochs = minibatch_size, epochs
+        self.dp = DataParallel.of(process_group)
+        self.world = self.dp.world if self.dp else 1
+        self.minibatch_size, self.epochs = -(-minibatch_size // self.world), epochs
         if backend not in ("torch", "tensor_core"):
             raise ValueError("backend must be 'torch' or 'tensor_core'")
         self.backend = backend
@@ -159,14 +236,22 @@ class PPOLearner:
         self.acc = {p: torch.zeros_like(p, memory_format=torch.contiguous_format) for p in self.actor_params + self.critic_params}
         self.gen = torch.Generator(device=dev)
         self.gen.manual_seed(seed)
+        if self.dp:
+            with torch.no_grad():
+                self.dp.broadcast(list(self.policy.parameters()) + list(self.critic.parameters()))
         if backend == "tensor_core":
             if dev.type != "cuda":
                 raise ValueError("the tensor_core learner needs a CUDA device; on the CPU, plain and gated networks train with backend='torch'")
             from .capi import TensorCoreGatedLearner, TensorCoreLearner
             di = dev.index or 0
             cls = TensorCoreGatedLearner if rollout.goal_size > 0 else TensorCoreLearner
-            self._tc_actor = cls(self.policy, self.acc, "actor", minibatch_size, device=di)
-            self._tc_critic = cls(self.critic, self.acc, "critic", minibatch_size, device=di)
+            self._tc_actor = cls(self.policy, self.acc, "actor", self.minibatch_size, device=di)
+            self._tc_critic = cls(self.critic, self.acc, "critic", self.minibatch_size, device=di)
+            if self.dp:   # the flat gradients the ranks sum
+                self._grad_actor = torch.empty(self._tc_actor.grad_size(), device=dev)
+                self._grad_critic = torch.empty(self._tc_critic.grad_size(), device=dev)
+        if self.dp:   # the rollout's tensor-core actor and critic collect with the broadcast weights
+            self._refresh_rollout()
 
     # ---- the window: everything a minibatch step reads, computed once per update
     def window(self, traj):
@@ -246,22 +331,40 @@ class PPOLearner:
                     raise ValueError("%s must be a contiguous int64 tensor of %d entries on %s" % (name, batch.rows, self.device))
             st = self.torch.cuda.current_stream(self.device).cuda_stream
             critic.idx = critic_idx.data_ptr()
-            self._tc_critic.step(critic, stream=st)
+            self._tc_step(self._tc_critic, critic, "_grad_critic", st)
             actor.idx = actor_idx.data_ptr()
-            self._tc_actor.step(actor, stream=st)
+            self._tc_step(self._tc_actor, actor, "_grad_actor", st)
             return
         t = self.torch
         total, loss = self.critic_loss(w, critic_idx)
-        grads = t.autograd.grad(total, self.critic_params)
+        grads = self._grads(total, loss, self.critic, self.critic_params, self.critic_weight_decay)
         with t.no_grad():
             momentum_step(self.critic_params, [self.acc[p] for p in self.critic_params], grads, self.critic_stepsize, self.critic_momentum)
             stats[1] += loss.detach()
         total, loss, ratio = self.actor_loss(w, actor_idx)
-        grads = t.autograd.grad(total, self.actor_params)
+        grads = self._grads(total, loss, self.policy, self.actor_params, self.actor_weight_decay)
         with t.no_grad():
             momentum_step(self.actor_params, [self.acc[p] for p in self.actor_params], grads, self.actor_stepsize, self.actor_momentum)
             stats[0] += loss.detach().abs()      # PPOAgent._update logs the mean of |actor loss| over the minibatches
             stats[2] += clip_fraction(ratio.detach(), self.ratio_clip)
+
+    def _tc_step(self, tc, batch, grad, stream):
+        """one tensor-core step: fused, or (data parallel) the gradient, its sum over the ranks and the step on the ranks' mean"""
+        if not self.dp:
+            tc.step(batch, stream=stream)
+            return
+        g = getattr(self, grad)
+        tc.grad(batch, g, stream=stream)
+        self.dp.sum(g)
+        tc.apply(batch, g, 1.0 / self.world, stream=stream)
+
+    def _grads(self, total, loss, net, params, weight_decay):
+        """the step's gradient: of `total` (the loss with its weight decay), or (data parallel) the ranks' mean gradient of `loss` plus the
+        weight decay's"""
+        t = self.torch
+        if not self.dp:
+            return t.autograd.grad(total, params)
+        return _weight_decay_grads(net, params, self.dp.mean_grads(t.autograd.grad(loss, params)), weight_decay)
 
     def update(self, traj):
         """one PPOAgent._update over the window traj (collect() with a critic); returns 0-d device tensors: actor_loss, critic_loss, clip_frac
@@ -270,6 +373,10 @@ class PPOLearner:
         same = lambda now, then: len(now) == len(then) and all(x is y for x, y in zip(now, then))
         if not same(trained_parameters(self.policy), self.actor_params) or not same(trained_parameters(self.critic), self.critic_params):
             raise ValueError("the policy's or the critic's parameters were replaced after the learner was built: build a new PPOLearner")
+        if self.dp:
+            if "explore" not in traj:
+                raise ValueError("traj has no 'explore': collect() with a critic returns it")
+            self.dp.check_window(traj["returns"].numel(), traj["explore"].any())
         w = self.window(traj)
         n_exp = w["exp_idx"].numel()
         stats = [t.zeros((), device=self.device) for _ in range(3)]
@@ -287,8 +394,13 @@ class PPOLearner:
             keep = tc[0]
             stats = [keep["stats_a"][0], keep["stats_c"][0], keep["stats_a"][1]]
         self._refresh_rollout()
-        return dict(actor_loss=stats[0] / steps, critic_loss=stats[1] / steps, clip_frac=stats[2] / steps, adv_mean=w["adv_mean"],
-                    adv_std=w["adv_std"], exp_samples=t.tensor(n_exp, device=self.device))
+        out = dict(actor_loss=stats[0] / steps, critic_loss=stats[1] / steps, clip_frac=stats[2] / steps, adv_mean=w["adv_mean"],
+                   adv_std=w["adv_std"], exp_samples=t.tensor(n_exp, device=self.device))
+        if self.dp:
+            keys = ("actor_loss", "critic_loss", "clip_frac", "adv_mean", "adv_std")
+            x = self.dp.sum(t.stack([out[k].double() for k in keys] + [out["exp_samples"].double()]))
+            out = dict(zip(keys, (x[:-1] / self.world).float()), exp_samples=x[-1].round().long())   # the explored samples of all ranks
+        return out
 
     def _refresh_rollout(self):
         """the rollout's tensor-core actor and critic take the new weights and the normalisers' current statistics, the ones this update trained
@@ -363,10 +475,15 @@ class AMPDiscLearner:
     The inputs are normalised by the rollout's amp_norm as collect() normalises them.  Every hyperparameter is required (the reference reads
     DiscStepSize, DiscMomentum, ... from the agent file; the asset archive has none).  The momentum accumulators are the learner's; keeping a
     replay buffer of agent observations and refreshing amp_norm stay the caller's.  After update() the torch discriminator holds the new
-    weights and the rollout's tensor-core discriminator, where it exists, those weights and amp_norm's current statistics."""
+    weights and the rollout's tensor-core discriminator, where it exists, those weights and amp_norm's current statistics.
+
+    process_group (data parallelism, see the module docstring): batch_size is the job's total (DiscBatchSize); each rank draws
+    ceil(batch_size / world) agent and as many expert rows per step from its own pools (the maintainer's reading of the reference's
+    _local_mini_batch_size, not checked against its source).  Every rank must run the same `steps`.  update()'s statistics are the ranks'
+    means."""
 
     def __init__(self, rollout, *, stepsize=None, momentum=None, weight_decay=None, logit_reg_weight=None, grad_penalty=None, batch_size=None,
-                 steps=None, backend="torch", seed=0):
+                 steps=None, backend="torch", seed=0, process_group=None):
         import torch
         self.torch, self.ro = torch, rollout
         if getattr(rollout, "disc", None) is None:
@@ -380,7 +497,9 @@ class AMPDiscLearner:
         for name, v in (("batch_size", batch_size), ("steps", steps)):
             if not isinstance(v, int) or isinstance(v, bool) or v < 1:
                 raise ValueError("%s must be a positive int (got %r)" % (name, v))
-        self.batch_size, self.steps = batch_size, steps
+        self.dp = DataParallel.of(process_group)
+        self.world = self.dp.world if self.dp else 1
+        self.batch_size, self.steps = -(-batch_size // self.world), steps
         if backend not in ("torch", "tensor_core"):
             raise ValueError("backend must be 'torch' or 'tensor_core'")
         self.backend = backend
@@ -389,11 +508,18 @@ class AMPDiscLearner:
         self.acc = {p: torch.zeros_like(p, memory_format=torch.contiguous_format) for p in self.params}
         self.gen = torch.Generator(device=self.device)
         self.gen.manual_seed(seed)
+        if self.dp:
+            with torch.no_grad():
+                self.dp.broadcast(self.params)
         if backend == "tensor_core":
             if self.device.type != "cuda":
                 raise ValueError("the tensor_core learner needs a CUDA device")
             from .capi import TensorCoreLearner
-            self._tc = TensorCoreLearner(self.disc, self.acc, "disc", 2 * batch_size, device=self.device.index or 0)
+            self._tc = TensorCoreLearner(self.disc, self.acc, "disc", 2 * self.batch_size, device=self.device.index or 0)
+            if self.dp:   # the flat gradient the ranks sum
+                self._grad = torch.empty(self._tc.grad_size(), device=self.device)
+        if self.dp:   # the rollout's tensor-core discriminator scores with the broadcast weights
+            self._refresh_rollout()
 
     def loss(self, norm_agent, norm_expert):
         """(total loss with the regularisers, disc_loss, grad_penalty, d_e, d_a) on normalised agent and expert rows (torch autograd)"""
@@ -426,11 +552,23 @@ class AMPDiscLearner:
                 if idx.dtype != t.int64 or not idx.is_contiguous() or idx.device != self.device or idx.numel() != batch.rows:
                     raise ValueError("%s must be a contiguous int64 tensor of %d entries on %s" % (name, batch.rows, self.device))
             batch.agent_idx, batch.expert_idx = agent_idx.data_ptr(), expert_idx.data_ptr()
-            self._tc.step(batch, stream=t.cuda.current_stream(self.device).cuda_stream)
+            st = t.cuda.current_stream(self.device).cuda_stream
+            if not self.dp:
+                self._tc.step(batch, stream=st)
+                return
+            self._tc.grad(batch, self._grad, stream=st)
+            self.dp.sum(self._grad)
+            self._tc.apply(batch, self._grad, 1.0 / self.world, stream=st)
             return
         norm = self.ro.amp_norm
         total, loss, gp, d_e, d_a = self.loss(norm.normalize(agent[agent_idx]), norm.normalize(expert[expert_idx]))
-        grads = t.autograd.grad(total, self.params)
+        if not self.dp:
+            grads = t.autograd.grad(total, self.params)
+        else:
+            # the ranks' mean gradient of the loss and the penalty, then the weight decay and the logit regulariser of the (common) weights
+            grads = _weight_decay_grads(self.disc, self.params, self.dp.mean_grads(t.autograd.grad(loss + self.grad_penalty * gp, self.params)),
+                                        self.weight_decay)
+            grads = [g + self.logit_reg_weight * p.detach() if p is self.disc.logit.weight else g for p, g in zip(self.params, grads)]
         with t.no_grad():
             momentum_step(self.params, [self.acc[p] for p in self.params], grads, self.stepsize, self.momentum)
             acc_e, acc_a = disc_accuracies(d_e, d_a)
@@ -465,7 +603,8 @@ class AMPDiscLearner:
             stats = list(tc[0]["stats"])
         self._refresh_rollout()
         keys = ("disc_loss", "grad_penalty", "acc_expert", "acc_agent", "logit_expert", "logit_agent")
-        return {k: s / self.steps for k, s in zip(keys, stats)}
+        stats = [s / self.steps for s in stats]
+        return dict(zip(keys, self.dp.mean_stats(stats) if self.dp else stats))
 
     def _refresh_rollout(self):
         """the rollout's tensor-core discriminator takes the new weights and amp_norm's current statistics (identity output normaliser), re-tiled

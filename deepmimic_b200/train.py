@@ -1,7 +1,14 @@
-"""Train a skill: the counterpart of the reference's `DeepMimic_Optimizer.py --arg_file args/train_*_args.txt`, on one GPU.
+"""Train a skill: the counterpart of the reference's `DeepMimic_Optimizer.py --arg_file args/train_*_args.txt` (one GPU) and of its
+`mpi_run.py --num_workers N` (one process per GPU under torchrun).
 
     python -m deepmimic_b200.train --arg_file args/train_humanoid3d_spinkick_args.txt [reference arguments ...]
         [--asset_root DIR] [--num_envs 4096] [--window_steps 32] [--max_iters K] [--backend tensor_core] [--seed 0] [--device 0] [--resume PATH]
+    torchrun --nproc-per-node 8 -m deepmimic_b200.train ... --num_envs 32768
+
+Under torchrun (WORLD_SIZE > 1) every rank joins an NCCL group on the GPU of its LOCAL_RANK (--device is ignored) and the Trainer splits
+--num_envs, the job's total, between the ranks (deepmimic_b200/trainer.py: Trainer, process_group).  Only the first rank prints and writes the
+log; rank r > 0 writes its checkpoints next to the first rank's, with .rank<r> before the .pt, and --resume PATH (the first rank's file)
+reads each rank's own.
 
 Every argument this module does not name goes to the scene, as the reference's arguments do.  --agent_files, --output_path and
 --int_output_path are read from the same argument list, the command line before the arg file (the reference's ArgParser keeps the first value
@@ -79,35 +86,58 @@ def build_parser():
     return ap
 
 
+def rank_path(path, rank):
+    """the checkpoint file of `rank` for the first rank's `path`: path itself for rank 0, <stem>.rank<r>.pt otherwise"""
+    if rank == 0:
+        return path
+    stem, ext = os.path.splitext(path)
+    return "%s.rank%d%s" % (stem, rank, ext or ".pt")
+
+
 def main(argv=None):
     from .assets import asset_root as default_asset_root
+    from .sharding import rank_world
     from .trainer import AgentConfig, Trainer
     opts, scene_args = build_parser().parse_known_args(sys.argv[1:] if argv is None else argv)
     root = opts.asset_root or default_asset_root()
     agent_file, out_path, int_path = resolve_args(scene_args, root)
     cfg = AgentConfig.from_json(agent_file)
+    rank, world, local_rank = rank_world()
+    group, device = None, opts.device
+    if world > 1:
+        import torch
+        import torch.distributed as dist
+        device = local_rank
+        torch.cuda.set_device(device)
+        dist.init_process_group("nccl", device_id=torch.device("cuda", device))
+        group = dist.group.WORLD
     os.makedirs(out_path, exist_ok=True)
     if int_path:
         os.makedirs(int_path, exist_ok=True)
-    ckpt = os.path.join(out_path, "agent0_checkpoint.pt")
-    tr = Trainer(scene_args, cfg, root, opts.num_envs, window_steps=opts.window_steps, backend=opts.backend, seed=opts.seed, device=opts.device,
-                 log_path=os.path.join(out_path, "agent0_log.txt"), append_log=opts.resume is not None)
+    ckpt = rank_path(os.path.join(out_path, "agent0_checkpoint.pt"), rank)
+    tr = Trainer(scene_args, cfg, root, opts.num_envs, window_steps=opts.window_steps, backend=opts.backend, seed=opts.seed, device=device,
+                 log_path=os.path.join(out_path, "agent0_log.txt"), append_log=opts.resume is not None, process_group=group)
     if opts.resume:
-        tr.load(opts.resume)
+        tr.load(rank_path(opts.resume, rank))
     try:
         while opts.max_iters is None or tr.iter < opts.max_iters:
             row = tr.iteration()
-            print("iteration %d: samples %d, Train_Return %.4f, Test_Return %.4f, %.2f s" % (row["Iteration"], row["Samples"], row["Train_Return"],
-                                                                                            row["Test_Return"], row["Wall_Time"]), flush=True)
+            if rank == 0:
+                print("iteration %d: samples %d, Train_Return %.4f, Test_Return %.4f, %.2f s" % (row["Iteration"], row["Samples"], row["Train_Return"],
+                                                                                                row["Test_Return"], row["Wall_Time"]), flush=True)
             if tr.iter % cfg["OutputIters"] == 0:
                 tr.save(ckpt)
             if int_path and cfg["IntOutputIters"] > 0 and tr.iter % cfg["IntOutputIters"] == 0:
-                tr.save(os.path.join(int_path, "agent0_int_checkpoint_%010d.pt" % tr.iter))
+                tr.save(rank_path(os.path.join(int_path, "agent0_int_checkpoint_%010d.pt" % tr.iter), rank))
     except KeyboardInterrupt:
         pass
     tr.save(ckpt)
     tr.close()
-    print("checkpoint: %s (iteration %d)" % (ckpt, tr.iter))
+    if rank == 0:
+        print("checkpoint: %s (iteration %d)" % (ckpt, tr.iter))
+    if group is not None:
+        import torch.distributed as dist
+        dist.destroy_process_group()
 
 
 if __name__ == "__main__":

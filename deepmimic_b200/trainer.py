@@ -266,25 +266,46 @@ class Trainer:
     bookkeeping with stand-ins on the CPU).
 
     Host synchronisations: none per policy step; per iteration a fixed number, independent of window_steps, of the minibatch and discriminator
-    step counts (tools/train_time.py counts them)."""
+    step counts (tools/train_time.py counts them).  With a process group of more than one rank, each PPO update adds one (the learners' check
+    that every rank's window has the same size).
+
+    Several GPUs (mpi_run.py --num_workers N): process_group, a torch.distributed group of one rank per GPU.  num_envs is the job's total, which
+    must be divisible by the world size; each rank steps its contiguous share (global_env_offset = rank * num_envs / world, so every
+    environment's reset stream is the one it has on one GPU), and evaluates ceil(TestEpisodes / world) episodes.  The learners average the
+    ranks' gradients (PPOLearner, AMPDiscLearner with the same group); the rollout, learner and disc-buffer generators are seeded with
+    seed + 1000 rank, and the expert sampler of rank r starts at call count r 2^40, so the ranks' exploration, minibatches and expert rows
+    differ.  The normalisers' statistics, the sample count, the finished episodes' returns and the evaluation's returns and episode counts are
+    summed over the ranks, so every rank logs the same row; only the first rank writes the log.  The disc buffers stay per rank (the
+    reference's per-worker buffers).  Each rank's state_dict() is its own (simulation state, generators, buffers); its run record holds the
+    world size and the state its rank, both of which load_state_dict() requires to match."""
 
     def __init__(self, args, config, asset_root, num_envs, window_steps=32, backend="tensor_core", seed=0, device=0, log_path=None, append_log=False,
-                 env=None, test_env=None):
+                 env=None, test_env=None, process_group=None):
         import torch
         from .env import DeepMimicBatchEnv
-        from .learner import AMPDiscLearner, PPOLearner
+        from .learner import AMPDiscLearner, DataParallel, PPOLearner
         from .rollout import BatchedRollout, build_critic, build_discriminator, build_gated_policy, build_policy
         self.torch = torch
         if not isinstance(config, AgentConfig):
             raise ValueError("config must be an AgentConfig")
         if window_steps < 1 or num_envs < 1:
             raise ValueError("num_envs and window_steps must be positive")
+        self.dp = DataParallel.of(process_group)
+        self.world = self.dp.world if self.dp else 1
+        self.rank = self.dp.dist.get_rank(process_group) if self.dp else 0
+        if num_envs % self.world:
+            raise ValueError("num_envs (%d, the job's total) must be divisible by the world size (%d)" % (num_envs, self.world))
+        local = num_envs // self.world
         self.args, self.config, self.backend, self.seed = list(args), config, backend, int(seed)
         self.window_steps = int(window_steps)
         # what a checkpoint must match
-        self.run = dict(args=self.args, agent=config.values, num_envs=int(num_envs), window_steps=self.window_steps, backend=backend, seed=self.seed)
+        self.run = dict(args=self.args, agent=config.values, num_envs=int(num_envs), window_steps=self.window_steps, backend=backend, seed=self.seed,
+                        world=self.world)
+        rs = self.seed + 1000 * self.rank   # the rank's generators
         cfg = config
-        self.env = env = env or DeepMimicBatchEnv(self.args, num_envs, asset_root, device=device, seed=self.seed)
+        self.env = env = env or DeepMimicBatchEnv(self.args, local, asset_root, device=device, seed=self.seed, global_env_offset=self.rank * local)
+        if env.num_envs != local:
+            raise ValueError("env has %d environments; this rank's share of num_envs is %d" % (env.num_envs, local))
         S, A, G = env.get_state_size(), env.get_action_size(), env.get_goal_size()
         net = NETS[1] if G > 0 else NETS[0]
         for key in ("ActorNet", "CriticNet"):
@@ -299,27 +320,30 @@ class Trainer:
         policy = build_gated_policy(S, G, A, init_output_scale=scale, noise=noise) if G > 0 else build_policy(S, A, init_output_scale=scale, noise=noise)
         critic = build_critic(S, G)
         disc = build_discriminator(env.get_amp_obs_size(), init_output_scale=cfg["DiscInitOutputScale"]) if self.amp else None
-        self.ro = BatchedRollout(env, policy, exp_rate=cfg["ExpParamsBeg"]["Rate"], noise=noise, seed=self.seed, backend=backend, disc=disc,
+        self.ro = BatchedRollout(env, policy, exp_rate=cfg["ExpParamsBeg"]["Rate"], noise=noise, seed=rs, backend=backend, disc=disc,
                                  task_reward_lerp=cfg["TaskRewardLerp"] if self.amp else None, critic=critic, discount=cfg["Discount"],
                                  td_lambda=cfg["TDLambda"])
         self.ppo = PPOLearner(self.ro, actor_stepsize=cfg["ActorStepsize"], actor_momentum=cfg["ActorMomentum"], actor_weight_decay=cfg["ActorWeightDecay"],
                               critic_stepsize=cfg["CriticStepsize"], critic_momentum=cfg["CriticMomentum"], critic_weight_decay=cfg["CriticWeightDecay"],
                               ratio_clip=cfg["RatioClip"], norm_adv_clip=cfg["NormAdvClip"], minibatch_size=cfg["MiniBatchSize"], epochs=cfg["Epochs"],
-                              backend=backend, seed=self.seed + 1)
+                              backend=backend, seed=rs + 1, process_group=process_group)
         self.disc = self.agent_buf = self.expert_buf = None
         if self.amp:
             self.disc = AMPDiscLearner(self.ro, stepsize=cfg["DiscStepSize"], momentum=cfg["DiscMomentum"], weight_decay=cfg["DiscWeightDecay"],
                                        logit_reg_weight=cfg["DiscLogitRegWeight"], grad_penalty=cfg["DiscGradPenalty"], batch_size=cfg["DiscBatchSize"],
-                                       steps=1, backend=backend, seed=self.seed + 2)
+                                       steps=1, backend=backend, seed=rs + 2, process_group=process_group)
             M = env.get_amp_obs_size()
-            self.agent_buf = DeviceReplayBuffer(cfg["DiscBufferSize"], M, env.device, seed=self.seed + 3)
-            self.expert_buf = DeviceReplayBuffer(cfg["DiscBufferSize"], M, env.device, seed=self.seed + 4)
+            self.agent_buf = DeviceReplayBuffer(cfg["DiscBufferSize"], M, env.device, seed=rs + 3)
+            self.expert_buf = DeviceReplayBuffer(cfg["DiscBufferSize"], M, env.device, seed=rs + 4)
+            if self.dp:
+                env.expert_sample_count(self.rank << 40)
         # evaluation: a small handle in test mode, restored to its start state before every evaluation
-        self.test_env = test_env or DeepMimicBatchEnv(self.args, cfg["TestEpisodes"], asset_root, device=device, seed=self.seed)
+        te = -(-cfg["TestEpisodes"] // self.world)
+        self.test_env = test_env or DeepMimicBatchEnv(self.args, te, asset_root, device=device, seed=self.seed, global_env_offset=self.rank * te)
         self.test_env.set_mode(1)
         self.test_env.reset(True)
         self._test_start = self.test_env.state_dict()
-        self.test_ro = BatchedRollout(self.test_env, policy, exp_rate=0.0, noise=noise, seed=self.seed, backend=backend)
+        self.test_ro = BatchedRollout(self.test_env, policy, exp_rate=0.0, noise=noise, seed=rs, backend=backend)
         self.test_ro.s_norm, self.test_ro.a_norm = self.ro.s_norm, self.ro.a_norm
         if G > 0:
             self.test_ro.g_norm = self.ro.g_norm
@@ -331,7 +355,7 @@ class Trainer:
         self.ep_len = torch.zeros(env.num_envs, device=env.device)
         self.phase_hook = None   # tools/train_time.py: phase_hook(name) -> context manager around each phase
         self.log = None
-        if log_path is not None:
+        if log_path is not None and self.rank == 0:
             from .formats import TableLog
             self.log = TableLog(log_path, append=append_log)
 
@@ -366,7 +390,7 @@ class Trainer:
             keep = 1.0 - df
             self.ep_ret *= keep
             self.ep_len *= keep
-        return sums
+        return self.dp.sum(sums) if self.dp else sums
 
     def iteration(self):
         """one iteration of the loop; returns its log row (a dict)"""
@@ -378,7 +402,7 @@ class Trainer:
         with self._phase("collect"):
             traj = ro.collect(T, record_stats=self.need_normalizer_update)
             ep = self._episode_sums(traj)
-        self.total_samples += T * N
+        self.total_samples += T * N * self.world
         env.set_sample_count(self.total_samples)
         train, self.initialized, update_norms, self.need_normalizer_update = train_schedule(
             self.total_samples, self.initialized, self.need_normalizer_update, cfg["InitSamples"], cfg["NormalizerSamples"])
@@ -393,7 +417,7 @@ class Trainer:
         if train:
             if self.amp:
                 with self._phase("disc_update"):
-                    self.disc.steps = disc_steps_per_iter(T * N, cfg["DiscStepsPerBatch"], cfg["DiscBatchSize"])
+                    self.disc.steps = disc_steps_per_iter(T * N * self.world, cfg["DiscStepsPerBatch"], cfg["DiscBatchSize"])
                     s_disc = self.disc.update(self.agent_buf.filled(), self.expert_buf.filled())
             with self._phase("ppo_update"):
                 s_ppo = self.ppo.update(traj)
@@ -402,7 +426,7 @@ class Trainer:
         if update_norms:
             with self._phase("normalizers"):
                 for n in self._updated_norms():
-                    n.update()
+                    n.update(all_reduce=self.dp.sum if self.dp else None)
                 # the rollout's tensor-core handles act on the new statistics from the next collect() on, as the torch backend does
                 self.ppo._refresh_rollout()
                 if self.amp:
@@ -436,10 +460,11 @@ class Trainer:
 
     def evaluate(self):
         """Test_Return: the mean return of one complete episode of each evaluation environment (test mode, exploration off), from the start
-        state the evaluation handle had when it was created.  One host synchronisation per 32 policy steps."""
+        state the evaluation handle had when it was created; with several ranks, the sum of every rank's returns over their number of episodes.
+        One host synchronisation per 32 policy steps."""
         t, env, ro = self.torch, self.test_env, self.test_ro
         env.load_state_dict(self._test_start)
-        ro.gen.manual_seed(self.seed)
+        ro.gen.manual_seed(self.seed + 1000 * self.rank)
         if self.backend == "tensor_core":
             ro.refresh_tensor_core_policy()
         n = env.num_envs
@@ -451,7 +476,10 @@ class Trainer:
                 ret += t.where(ended, t.zeros_like(r), r)
                 ended |= d
             if bool(ended.all()):
-                return ret.mean().item()
+                if not self.dp:
+                    return ret.mean().item()
+                s = self.dp.sum(t.stack([ret.sum(), t.tensor(float(n), device=env.device)])).tolist()
+                return s[0] / s[1]
         raise RuntimeError("evaluation: an episode ran longer than %d policy steps" % limit)
 
     # ---- checkpoints
@@ -471,7 +499,7 @@ class Trainer:
             gens["disc"] = self.disc.gen.get_state()
             bufs = dict(agent=self.agent_buf.state_dict(), expert=self.expert_buf.state_dict())
         norms = {name: dict({f: c(getattr(n, f)) for f in _NORM_FIELDS}, count=n.count, new_count=n.new_count) for name, n in self._all_norms().items()}
-        return dict(run=self.run, iteration=self.iter, samples=self.total_samples, initialized=self.initialized,
+        return dict(run=self.run, rank=self.rank, iteration=self.iter, samples=self.total_samples, initialized=self.initialized,
                     need_normalizer_update=self.need_normalizer_update, actor_stepsize=self.ppo.actor_stepsize, test_return=self.test_return,
                     nets=nets, accs=accs, norms=norms, generators=gens, buffers=bufs, episodes=dict(ret=c(self.ep_ret), len=c(self.ep_len)),
                     env=self.env.state_dict())
@@ -482,8 +510,10 @@ class Trainer:
         tensor-core handles are rebuilt from the loaded weights and normalisers."""
         t, ro = self.torch, self.ro
         for k in self.run:
-            if s["run"].get(k) != self.run[k]:
-                raise ValueError("checkpoint: its %s differs from this run's" % ("agent file" if k == "agent" else k))
+            if s["run"].get(k, 1 if k == "world" else None) != self.run[k]:   # a checkpoint without a world size is a one-rank run's
+                raise ValueError("checkpoint: its %s differs from this run's" % ("agent file" if k == "agent" else "world size" if k == "world" else k))
+        if s.get("rank", 0) != self.rank:
+            raise ValueError("checkpoint: it is rank %d's, not this rank's (%d)" % (s.get("rank", 0), self.rank))
         with t.no_grad():
             for name, net in (("actor", ro.policy), ("critic", ro.critic)) + ((("disc", ro.disc),) if self.amp else ()):
                 for k, v in net.state_dict().items():

@@ -340,6 +340,27 @@ int dm_learn_gated_step(dm_learn* l, const dm_learn_gated_net* net, const dm_lea
 int dm_mlp_set_gated_weights_device(dm_mlp* m, const float* const* d_w, const float* const* d_b, void* stream);
 int dm_mlp_set_gated_normalizers_device(dm_mlp* m, const float* d_s_mean, const float* d_s_std, const float* d_g_mean, const float* d_g_std, const float* d_out_mean,
                                         const float* d_out_std, void* stream);
+/* The minibatch step split in two around its gradient, for data-parallel training (solvers/mpi_solver.py: MPISolver averages the workers' flat
+ * gradients before the momentum step).  Between the halves the caller may sum the ranks' buffers (e.g. one all-reduce).
+ *   dm_learn_grad_size: the floats of the network's flat gradient (-1 on a NULL handle): per parameter pair, in the order of the net struct
+ *     (dm_learn_net: layers 0, 1, 2; dm_learn_gated_net: its ten pairs), the weights [units x inputs] row major, then the bias [units].
+ *     For the gated networks this is not the Python modules' parameter order (capi.py: gated_layers() gives the pairs in this order, and
+ *     TensorCoreLearner.grad_views() maps the buffer to the parameters).
+ *   *_grad: the step's launches up to its layer pass (the same forward, head, backward and statistics: `stats` accumulates as in the step),
+ *     then one pack pass that writes the mean gradient over the step's rows into d_grad: the split-K partials summed in the step's order, times
+ *     1 / rows, plus (discriminator) the weighted penalty's.  Without weight decay and the logit regulariser: they depend on the weights alone.
+ *     The parameters are read only.  Same launch count as the step.
+ *   *_apply: the layer pass on g = scale * d_grad: weight decay (and the logit regulariser) added, the momentum step and the re-tiling, one
+ *     launch per parameter pair.  Reads the batch's stepsize, momentum, weight_decay (and logit_reg_weight) only.
+ * apply(grad(b), scale 1) leaves the parameters, accumulators, tiles and statistics bit-identical to the step on b.  Refused: a NULL handle or
+ * pointer, the wrong workspace kind, what the step refuses (grad), a negative (or NaN) optimiser field or a non-finite scale (apply). */
+long long dm_learn_grad_size(const dm_learn* l);
+int dm_learn_grad(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* batch, float* d_grad, void* stream);
+int dm_learn_apply(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* batch, const float* d_grad, float scale, void* stream);
+int dm_learn_gated_grad(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_gated_batch* batch, float* d_grad, void* stream);
+int dm_learn_gated_apply(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_gated_batch* batch, const float* d_grad, float scale, void* stream);
+int dm_learn_disc_grad(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* batch, float* d_grad, void* stream);
+int dm_learn_disc_apply(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* batch, const float* d_grad, float scale, void* stream);
 void dm_learn_destroy(dm_learn* l);
 
 /* ---- test hooks: raw per-env simulator state, layout shared with the CPU oracle (doubles):

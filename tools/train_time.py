@@ -4,7 +4,9 @@ T = 32, with the agent values of tests/test_train_gpu.py.  Phases: collect (the 
 and the expert draws), disc_update, ppo_update, normalizers (the update and the refresh of the rollout's handles), each between two CUDA events
 on the current stream around --iters iterations after --warmup; evaluation (TestEpisodes episodes on the evaluation handle) and checkpoint
 (Trainer.state_dict(), which synchronises: host wall clock) are timed on their own.  Host synchronisations are counted with torch's sync debug
-mode (every synchronising torch call) plus the library's one in set_sample_count.  Prints the card and its power limit.
+mode (every synchronising torch call) plus the library's one in set_sample_count.  The run is one rank; a Trainer with a process group of
+more than one rank adds one synchronisation per PPO update (PPOLearner's check that every rank's window has the same size and an explored
+sample), and its evaluation's sum over the ranks stays within the evaluation's last synchronisation.  Prints the card and its power limit.
 
     python tools/train_time.py [--envs 4096] [--steps 32] [--warmup 2] [--iters 5]"""
 import argparse
