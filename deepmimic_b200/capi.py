@@ -60,7 +60,7 @@ class DmLearnGatedBatch(C.Structure):
 DM_STATE_OFFSET, DM_STATE_SCALE, DM_ACTION_OFFSET, DM_ACTION_SCALE, DM_ACTION_BOUND_MIN, DM_ACTION_BOUND_MAX, DM_STATE_NORM_GROUPS = range(7)
 
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
-           "dm_update", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
+           "dm_update", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_record_pose", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
            "dm_set_snapshot", "dm_state_size", "dm_save_state", "dm_load_state", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
            "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy", "dm_td_lambda_returns", "dm_mlp_set_weights_device", "dm_learn_create",
            "dm_mlp_set_normalizers_device", "dm_learn_set_weights", "dm_learn_step", "dm_learn_disc_step", "dm_learn_destroy",
@@ -102,6 +102,7 @@ def lib():
         L.dm_get_env_order.argtypes = [vp, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.dm_record_state.argtypes = [vp, fp]
         L.dm_record_goal.argtypes = [vp, fp]
+        L.dm_record_pose.argtypes = [vp, fp, fp]
         L.dm_calc_reward.argtypes = [vp, fp]
         L.dm_calc_reward_imitate.argtypes = [vp, fp]
         L.dm_goal_host.argtypes = [vp, fp]
@@ -299,6 +300,16 @@ class BatchedCore:
     def observe(self, state=None, reward=None):
         self._chk(lib().dm_observe(self.h, C.c_void_p(state.data_ptr()) if state is not None else None,
                                    C.c_void_p(reward.data_ptr()) if reward is not None else None))
+
+    def record_pose(self, pose=None, vel=None):
+        """dm_record_pose: the simulated characters' pose and velocity rows in the reference's layout (cSimCharacter::BuildPose / BuildVel) into
+        contiguous float32 CUDA tensors [N, pose_dim]; either may be None.  Stream-ordered on the handle's stream."""
+        P = self.dims.pose_dim
+        for name, t in (("pose", pose), ("vel", vel)):
+            if t is not None:
+                _check_device_f32(t, "record_pose: " + name, (self.num_envs, P))
+        self._chk(lib().dm_record_pose(self.h, C.c_void_p(pose.data_ptr()) if pose is not None else None,
+                                       C.c_void_p(vel.data_ptr()) if vel is not None else None))
 
     def reward_imitate(self, out):  # torch float32 cuda tensor [N]: CalcRewardImitate also in the task scenes (active clip of the dataset)
         self._chk(lib().dm_calc_reward_imitate(self.h, C.c_void_p(out.data_ptr())))

@@ -404,6 +404,13 @@ int launch_amp(dm_handle* h, float* d_out, int expert, const double* d_times, co
                                                               h->num_envs, d_clips);
     return launched(h);
 }
+// pose / vel: [num_envs x pose_dim] rows of the real environments, either may be null
+int launch_pose(dm_handle* h, float* d_pose, float* d_vel) {
+    const int E = dmk::kPoseEnvsPerBlock;
+    const size_t smem = static_cast<size_t>(E) * 2 * h->hm.pose_dim * sizeof(float);
+    dmk::dm_pose_kernel<<<(h->num_envs + E - 1) / E, E * h->hm.nl, smem, h->stream>>>(h->d_model, h->st, d_pose, d_vel, h->num_envs);
+    return launched(h);
+}
 
 // Copies bytes [off, off + bytes) of the host model blob into the device one, stream-ordered; host-only handles have no device blob.
 int upload_model(dm_handle* h, size_t off, size_t bytes) {
@@ -861,6 +868,11 @@ int dm_observe(dm_handle* h, float* d_state, float* d_reward) {
     return 0;
 }
 int dm_record_state(dm_handle* h, float* d_out) { return dm_observe(h, d_out, nullptr); }
+int dm_record_pose(dm_handle* h, float* d_pose, float* d_vel) {
+    DM_DEVICE(h);
+    if (d_pose == nullptr && d_vel == nullptr) return 0;
+    return launch_pose(h, d_pose, d_vel);
+}
 // cSceneImitate::CalcRewardImitate in every scene: in the AMP task scenes (where CalcReward is the task reward) against the environment's
 // active clip of the dataset -- BASELINE.json config 5 records it beside the AMP observations.
 int dm_calc_reward_imitate(dm_handle* h, float* d_out) {

@@ -204,6 +204,8 @@ extern const AmpExpertKernel kAmpExpertKernels[2][2];
 constexpr int kEnvOrderThreads = 1024;   // dm_env_order_kernel: one block
 __global__ void dm_env_order_kernel(const int* load, int n_padded, int tiles, int W, int* order);
 __global__ void dm_set_action_kernel(const DevModel*, DevState, const float*, int);
+constexpr int kPoseEnvsPerBlock = 8;   // dm_pose_kernel: kPoseEnvsPerBlock x links threads, 2 pose_dim floats of shared memory per environment
+__global__ void dm_pose_kernel(const DevModel*, DevState, float*, float*, int);
 __global__ void dm_task_reset_kernel(const DevModel*, DevState, int);
 __global__ void dm_task_observe_kernel(const DevModel*, DevState, float*, float*, int);
 int dm_step_layout(int nl, int n, int chain_len, int maxrows, int W, StepLayout* L);

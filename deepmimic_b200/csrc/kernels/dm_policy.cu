@@ -5,6 +5,7 @@
 //                         (anim/Motion.cpp:267-293,486-515; anim/KinTree.cpp:1336-1378)
 //   dm_set_action_kernel: cCtPDController::ApplyAction -> ConvertActionToTargetPose (sim/CtPDController.cpp:97-166)
 //   dm_reset_kernel     : cSceneSimChar::ResetScene chain (SURVEY.md 3d) for the environments whose done flag is set
+//   dm_pose_kernel      : cSimCharacter::BuildPose / BuildVel (sim/SimCharacter.cpp:1428-1507) of every environment
 #include "dm_model.cuh"
 
 namespace dmk {
@@ -549,6 +550,29 @@ __global__ void dm_set_action_kernel(const DevModel* __restrict__ gm, DevState s
         *tgt = make_float4(q.x, q.y, q.z, q.w);
     } else if (L.jtype == kJRevolute) {
         *tgt = make_float4(a[0], 0.f, 0.f, 0.f);
+    }
+}
+
+// pose / vel: [num_real_envs x pose_dim] floats, the simulated character in DeepMimic layout (cSimCharacter::BuildPose / BuildVel); either may be
+// null.  Block b holds environments [b kPoseEnvsPerBlock, (b + 1) kPoseEnvsPerBlock), one thread per (environment, joint): the AMP history's
+// conversion and write rule put each environment's pose | vel pair into shared memory, and the block then stores its pose rows and its vel rows
+// as two contiguous ranges.  Padding environments are not written.
+__global__ void dm_pose_kernel(const DevModel* __restrict__ gm, DevState st, float* __restrict__ pose, float* __restrict__ vel, int num_real_envs) {
+    extern __shared__ float spv[];   // [kPoseEnvsPerBlock x 2 pose_dim]
+    const DevModel& M = *gm;
+    const int P = M.pose_dim, env0 = blockIdx.x * kPoseEnvsPerBlock;
+    const int e = threadIdx.x / M.nl, j = threadIdx.x % M.nl;
+    if (e < kPoseEnvsPerBlock && env0 + e < num_real_envs) {
+        const DevLink& L = M.link[j];
+        hist_store(spv + 2 * P * e, P, L, j == 0, sim_joint_to_dm(M, L, st.sim + static_cast<size_t>(env0 + e) * sim_stride(M.nl), j, j == 0));
+    }
+    __syncthreads();
+    const int n = min(kPoseEnvsPerBlock, num_real_envs - env0) * P;
+    const size_t base = static_cast<size_t>(env0) * P;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const float* s = spv + 2 * P * (i / P) + i % P;
+        if (pose) pose[base + i] = s[0];
+        if (vel) vel[base + i] = s[P];
     }
 }
 

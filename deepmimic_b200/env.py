@@ -13,6 +13,8 @@ class DeepMimicBatchEnv:
     class Terminate:
         Null, Fail, Succ = 0, 1, 2
 
+    UPDATE_DT = 1.0 / 600.0   # the reference's update timestep (600 Hz), step()'s default
+
     def __init__(self, args, num_envs, asset_root, device=0, seed=0, global_env_offset=0):
         import torch
         self.torch = torch
@@ -59,6 +61,10 @@ class DeepMimicBatchEnv:
     def get_num_agents(self):
         return 1
 
+    def get_updates_per_action(self):
+        """updates per policy step (20 for the shipped arg files: 30 Hz queries at 600 Hz updates)"""
+        return self._core.dims.updates_per_action
+
     def get_num_update_substeps(self):
         return self._core.dims.num_update_substeps
 
@@ -100,6 +106,20 @@ class DeepMimicBatchEnv:
         self._core.record_goal(self._goal)
         self._post()
         return self._goal
+
+    def record_pose(self, agent_id=0):
+        """(pose, vel): [N, pose_dim] float32 each, every simulated character's pose and velocity in the reference's layout
+        (cSimCharacter::BuildPose / BuildVel: root position, root quaternion w x y z, joint quaternions or angles; root linear and angular
+        velocity, joint velocities), what cMotion files hold per frame.  Views of buffers rewritten by the next call, like record_state."""
+        if getattr(self, "_pose", None) is None:
+            P = self._core.dims.pose_dim
+            with self.torch.cuda.stream(self.stream):
+                self._pose = self.torch.zeros(self.num_envs, P, device=self.device)
+                self._vel = self.torch.zeros(self.num_envs, P, device=self.device)
+        self._pre()
+        self._core.record_pose(self._pose, self._vel)
+        self._post()
+        return self._pose, self._vel
 
     def set_action(self, agent_id_or_actions, actions=None):
         a = agent_id_or_actions if actions is None else actions
@@ -171,7 +191,7 @@ class DeepMimicBatchEnv:
     def check_valid_episode(self):
         return self._refresh_flags()[:, 3].bool()
 
-    def step(self, actions, timestep=1.0 / 600.0):
+    def step(self, actions, timestep=UPDATE_DT):
         """One policy step: SetAction, the controller's query period worth of Update(timestep) calls (20 at the
         reference's 600 Hz / 30 Hz), then state, reward and flags.  Returns (obs, reward, done, terminate)."""
         self.set_action(actions)
@@ -186,6 +206,10 @@ class DeepMimicBatchEnv:
 
     def get_state_size(self, agent_id=0):
         return self._core.dims.state_size
+
+    def get_pose_dim(self, agent_id=0):
+        """length of a pose or velocity row of record_pose (43 humanoid3d, 83 dog3d)"""
+        return self._core.dims.pose_dim
 
     def get_goal_size(self, agent_id=0):
         return self._core.dims.goal_size

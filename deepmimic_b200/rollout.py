@@ -521,13 +521,14 @@ class BatchedRollout:
     def stream(self):
         return self.env.stream
 
-    def collect(self, num_steps, record_stats=True):
+    def collect(self, num_steps, record_stats=True, record_pose=False):
         """num_steps policy steps of all environments; returns dict of [T, N, .] tensors (states, actions, logps, rewards, dones, terminate,
         explore = the exploration draw of each step (True: the action was sampled, False: the mode was taken); goals
         in the goal-conditioned scenes; with a discriminator amp_obs, disc_logits, style_rewards, amp_rewards; with a critic values = V(s_k),
         end_values = V(s'_k) of the state step k ended in (before the reset), returns and advantages = returns - values).  rewards is the env's
         reward.  A path still running at the last step is bootstrapped with its end value, as the reference bootstraps a path that ends by time
-        limit (a deviation: the reference stores only complete paths)."""
+        limit (a deviation: the reference stores only complete paths).  record_pose adds the simulated characters' poses (env.record_pose),
+        [T, N, pose_dim] each: poses / vels at s_k, end_poses / end_vels at s'_k, before the reset, like values / end_values."""
         t, env = self.torch, self.env
         N, S, A = env.num_envs, env.get_state_size(), env.get_action_size()
         out = dict(states=t.empty(num_steps, N, S, device=env.device), actions=t.empty(num_steps, N, A, device=env.device),
@@ -541,6 +542,10 @@ class BatchedRollout:
             out["amp_obs"] = t.empty(num_steps, N, env.get_amp_obs_size(), device=env.device)
             for key in ("disc_logits", "style_rewards", "amp_rewards"):
                 out[key] = t.empty(num_steps, N, device=env.device)
+        if record_pose:
+            P = env.get_pose_dim()
+            for key in ("poses", "vels", "end_poses", "end_vels"):
+                out[key] = t.empty(num_steps, N, P, device=env.device)
         crit = self.critic is not None
         if crit:
             for key in ("values", "end_values", "returns", "advantages"):
@@ -557,6 +562,9 @@ class BatchedRollout:
             s = env.record_state()
             for k in range(num_steps):
                 out["states"][k] = s
+                if record_pose:
+                    p, v = env.record_pose()
+                    out["poses"][k] = p; out["vels"][k] = v
                 if crit:
                     x2[:N] = s
                 if record_stats:
@@ -580,6 +588,9 @@ class BatchedRollout:
                     a = self.a_norm.unnormalize(na).contiguous()
                 s, r, done, term = env.step(a)
                 out["actions"][k] = a; out["logps"][k] = logp; out["rewards"][k] = r; out["dones"][k] = done; out["terminate"][k] = term
+                if record_pose:   # before the reset: the end pose of a finished episode is its terminal pose
+                    p, v = env.record_pose()
+                    out["end_poses"][k] = p; out["end_vels"][k] = v
                 if self.disc is not None:
                     # before the reset: the last transition of a finished episode is the agent's own motion, not the restarted state
                     amp = env.record_amp_obs_agent()
@@ -604,3 +615,47 @@ class BatchedRollout:
         if caller is not None:
             caller.wait_stream(env.stream)
         return out
+
+
+def run_episodes(ro, pose_envs=0, limit=1 << 16):
+    """One complete episode of every environment of ro's env from its current state, in chunks of 32 policy steps of ro.collect (the
+    environments that finish first keep running into their next episode, which is not counted).  Set the env's mode and ro's exploration
+    before the call (test mode, exp_rate 0 for an evaluation).  One host synchronisation per chunk.  Returns dict(returns [N] float32, lengths
+    [N] int32 = policy steps, terminate [N] int32 = the terminate code of the episode's last step: 0 time limit, 1 fail, 2 success); with
+    pose_envs > 0 also poses and end_poses of the first pose_envs environments, lists of the chunks' [32, pose_envs, pose_dim] tensors
+    (episode_motion assembles an environment's frames); the other environments' poses are not kept.
+    RuntimeError when an episode runs longer than `limit` policy steps."""
+    import torch as t
+    env = ro.env
+    n = env.num_envs
+    ret, ended = t.zeros(n, device=env.device), t.zeros(n, dtype=t.bool, device=env.device)
+    length, term = t.zeros(n, dtype=t.int32, device=env.device), t.zeros(n, dtype=t.int32, device=env.device)
+    poses, end_poses = [], []
+    for _ in range(0, limit, 32):
+        traj = ro.collect(32, record_stats=False, record_pose=True) if pose_envs else ro.collect(32, record_stats=False)
+        if pose_envs:
+            poses.append(traj["poses"][:, :pose_envs].clone()); end_poses.append(traj["end_poses"][:, :pose_envs].clone())
+        for r, d, c in zip(traj["rewards"], traj["dones"], traj["terminate"]):
+            ret += t.where(ended, t.zeros_like(r), r)
+            length += (~ended).int()
+            term = t.where(ended, term, c)
+            ended |= d
+        if bool(ended.all()):
+            out = dict(returns=ret, lengths=length, terminate=term)
+            if pose_envs:
+                out.update(poses=poses, end_poses=end_poses)
+            return out
+    raise RuntimeError("an episode ran longer than %d policy steps" % limit)
+
+
+def episode_motion(poses, end_poses, env_index, length):
+    """the frames of environment env_index's first episode of `length` policy steps: the poses it took its actions in (steps 0 .. length - 1)
+    and the terminal pose its last step ended in, [length + 1, pose_dim] float64 on the host.  poses / end_poses: [T, N, pose_dim] tensors or
+    run_episodes' lists of chunks."""
+    import torch as t
+    cat = lambda x: t.cat(list(x)) if isinstance(x, (list, tuple)) else x
+    p, e = cat(poses), cat(end_poses)
+    if not 1 <= length <= p.shape[0]:
+        raise ValueError("an episode of %d steps does not fit %d recorded steps" % (length, p.shape[0]))
+    return t.cat([p[:length, env_index], e[length - 1:length, env_index]]).double().cpu().numpy()
+

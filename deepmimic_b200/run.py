@@ -1,0 +1,106 @@
+"""Run a trained skill: the counterpart of the reference's `DeepMimic.py --arg_file args/run_*_args.txt`, without the viewer.
+
+    python -m deepmimic_b200.run --arg_file args/run_humanoid3d_spinkick_args.txt [--model_files PATH] [--num_envs 64]
+        [--record_motion K] [--episode_time 20] [--backend tensor_core] [--seed 0] [--device 0] [--asset_root DIR] [reference arguments ...]
+
+--model_files (a reference TensorBundle prefix or a Trainer checkpoint, deepmimic_b200/model_files.py) and --output_path are read from the
+argument list, the command line before the arg file, as deepmimic_b200.train reads its paths; --train_agents and --agent_files are accepted
+and not needed.  The actor is the plain or the gated network, by the scene's goal size, as the Trainer chooses.  Every environment runs one
+complete episode in test mode with exploration off, the loop of Trainer.evaluate; where the arguments set no episode time limit (the run_*
+arg files: the reference's viewer runs until the character falls), an episode ends after --episode_time seconds (default 20).  Under
+<output_path> (default "output"):
+  run_log.txt          one row per environment: its return, its length in policy steps and its terminate code (0 time limit, 1 fail, 2 success)
+  motion_<env>.txt     with --record_motion K, the first K environments' episodes as motion files (cMotion::Output, loop "none", one frame per
+                       policy step and the terminal pose)
+and a printed summary: the return's mean and standard deviation, the mean length and the fraction of episodes ended by Fail.  One GPU only."""
+import argparse
+import os
+import sys
+
+from .train import arg_table, first_arg, resolve_model_files
+
+
+def build_parser():
+    ap = argparse.ArgumentParser(prog="python -m deepmimic_b200.run", description=__doc__.split("\n\n")[0], allow_abbrev=False)
+    ap.add_argument("--asset_root", default=None, help="the reference's data / args tree (default: the bundled asset archive)")
+    ap.add_argument("--num_envs", type=int, default=64, help="environments, one episode each")
+    ap.add_argument("--record_motion", type=int, default=0, metavar="K", help="write the first K environments' episodes as motion files")
+    ap.add_argument("--backend", default="tensor_core", choices=("tensor_core", "torch"))
+    ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--episode_time", type=float, default=20.0,
+                    help="test-mode episode limit in seconds for arguments that set none (the run_* arg files; default 20, the train_* files' limit)")
+    return ap
+
+
+def write_episode_motions(path_fmt, ep, count, frame_dur):
+    """motion files of the first `count` environments of run_episodes(pose_envs >= count)'s result `ep`: path_fmt % env; returns the paths"""
+    from .formats import write_motion
+    from .rollout import episode_motion
+    lengths = ep["lengths"].cpu().tolist()
+    paths = []
+    for e in range(count):
+        frames = episode_motion(ep["poses"], ep["end_poses"], e, int(lengths[e]))
+        write_motion(path_fmt % e, frames, [frame_dur] * frames.shape[0], loop="none")
+        paths.append(path_fmt % e)
+    return paths
+
+
+def main(argv=None):
+    import numpy as np
+    from .assets import asset_root as default_asset_root
+    from .sharding import rank_world
+    opts, scene_args = build_parser().parse_known_args(sys.argv[1:] if argv is None else argv)
+    if rank_world()[1] > 1:
+        raise SystemExit("run: one GPU only; start it without torchrun")
+    if opts.num_envs < 1 or not 0 <= opts.record_motion <= opts.num_envs:
+        raise SystemExit("run: need --num_envs >= 1 and 0 <= --record_motion <= --num_envs")
+    root = opts.asset_root or default_asset_root()
+    table = arg_table(scene_args, root, "run")
+    out_path = first_arg(table, "output_path") or "output"
+    model_files = resolve_model_files(scene_args, root, "run")
+    if model_files is None:
+        raise SystemExit("run: no --model_files in the arguments or the arg file")
+    from .model_files import model_file_kind
+    try:
+        model_file_kind(model_files)
+    except FileNotFoundError as e:
+        raise SystemExit("run: %s" % e)
+    import torch
+    from .env import DeepMimicBatchEnv
+    from .formats import TableLog
+    from .model_files import load_model_files
+    from .rollout import BatchedRollout, run_episodes
+    if not (first_arg(table, "time_end_lim_max") or first_arg(table, "time_lim_max")):
+        # the reference's viewer runs an episode until the character falls; one complete episode per environment needs an end
+        scene_args = scene_args + ["--time_end_lim_min", repr(opts.episode_time), "--time_end_lim_max", repr(opts.episode_time)]
+    env = DeepMimicBatchEnv(scene_args, opts.num_envs, root, device=opts.device, seed=opts.seed)
+    env.set_mode(1)
+    env.reset(True)
+    ro = BatchedRollout(env, exp_rate=0.0, seed=opts.seed, backend=opts.backend)
+    norms = dict(s_norm=ro.s_norm, a_norm=ro.a_norm, **(dict(g_norm=ro.g_norm) if ro.goal_size > 0 else {}))
+    try:
+        load_model_files(model_files, ro.policy, norms)
+    except ValueError as e:
+        raise SystemExit("run: %s" % e)
+    ep = run_episodes(ro, pose_envs=opts.record_motion)
+    torch.cuda.synchronize(env.device)
+    ret, length, term = (ep[k].cpu().numpy() for k in ("returns", "lengths", "terminate"))
+    os.makedirs(out_path, exist_ok=True)
+    log = TableLog(os.path.join(out_path, "run_log.txt"))
+    for e in range(opts.num_envs):
+        for k, v in (("Env", e), ("Return", float(ret[e])), ("Length", int(length[e])), ("Terminate", int(term[e]))):
+            log.log_tabular(k, v)
+        log.dump_tabular()
+    log.close()
+    print("%s, %d episodes: return %.4f +- %.4f, length %.1f policy steps, ended by Fail %.3f" % (model_files, opts.num_envs, float(np.mean(ret)),
+                                                                                              float(np.std(ret)), float(np.mean(length)), float(np.mean(term == 1))))
+    if opts.record_motion:
+        paths = write_episode_motions(os.path.join(out_path, "motion_%d.txt"), ep, opts.record_motion,
+                                      env.get_updates_per_action() * env.UPDATE_DT)
+        print("motion files: %s .. %s" % (paths[0], paths[-1]))
+    return dict(returns=ret, lengths=length, terminate=term)
+
+
+if __name__ == "__main__":
+    main()

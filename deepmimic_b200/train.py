@@ -12,7 +12,9 @@ reads each rank's own.
 
 Every argument this module does not name goes to the scene, as the reference's arguments do.  --agent_files, --output_path and
 --int_output_path are read from the same argument list, the command line before the arg file (the reference's ArgParser keeps the first value
-of a key).  The log goes to <output_path>/agent0_log.txt and the checkpoint to <output_path>/agent0_checkpoint.pt (every OutputIters iterations
+of a key), and so is --model_files: a reference TensorBundle prefix or a Trainer checkpoint whose networks and normalisers the run starts from
+(deepmimic_b200/model_files.py), at iteration 0.  Such a run resumes with the arguments it started with, --model_files included: the
+checkpoint records the model files, and --resume refuses a checkpoint of a run that started from other ones (or from none).  The log goes to <output_path>/agent0_log.txt and the checkpoint to <output_path>/agent0_checkpoint.pt (every OutputIters iterations
 and at the end); with --int_output_path, an intermediate checkpoint every IntOutputIters iterations goes to
 <int_output_path>/agent0_int_checkpoint_<iteration>.pt.  --resume continues a checkpoint of the same run (arguments, agent file, num_envs,
 window_steps, backend, seed), its log and its iteration numbering."""
@@ -51,26 +53,43 @@ def _file_tokens(path):
 
 
 def _resolve(asset_root, path):
-    """a path of the argument list: absolute, under the asset root, or relative to the working directory"""
+    """a path of the argument list: absolute, under the asset root, or relative to the working directory.  A TensorBundle prefix (a model
+    file) counts as existing when its .index file does."""
     if os.path.isabs(path):
         return path
     under = os.path.join(asset_root, path)
-    return under if os.path.exists(under) else path
+    return under if os.path.exists(under) or os.path.exists(under + ".index") else path
 
 
-def resolve_args(scene_args, asset_root):
-    """(agent file, output path, int output path) from the scene arguments and the arg file they name (command line first)"""
+def arg_table(scene_args, asset_root, prog="train"):
+    """{key: values} of the scene arguments and the arg file they name, the command line first (parse_arg_list's rule)"""
     table = parse_arg_list(scene_args)
     if "arg_file" in table and table["arg_file"]:
         arg_file = _resolve(asset_root, table["arg_file"][0])
         if not os.path.exists(arg_file):
-            raise SystemExit("train: arg file %s not found" % table["arg_file"][0])
+            raise SystemExit("%s: arg file %s not found" % (prog, table["arg_file"][0]))
         for k, v in parse_arg_list(_file_tokens(arg_file)).items():
             table.setdefault(k, v)
-    first = lambda k: table[k][0] if table.get(k) else ""
-    if not first("agent_files"):
+    return table
+
+
+def first_arg(table, key):
+    """the first value of `key` in an arg_table, "" without one"""
+    return table[key][0] if table.get(key) else ""
+
+
+def resolve_args(scene_args, asset_root):
+    """(agent file, output path, int output path) from the scene arguments and the arg file they name (command line first)"""
+    table = arg_table(scene_args, asset_root)
+    if not first_arg(table, "agent_files"):
         raise SystemExit("train: no --agent_files in the arguments or the arg file")
-    return _resolve(asset_root, first("agent_files")), first("output_path") or "output", first("int_output_path")
+    return _resolve(asset_root, first_arg(table, "agent_files")), first_arg(table, "output_path") or "output", first_arg(table, "int_output_path")
+
+
+def resolve_model_files(scene_args, asset_root, prog="train"):
+    """--model_files of the scene arguments or their arg file (command line first), resolved like the other paths; None without one"""
+    m = first_arg(arg_table(scene_args, asset_root, prog), "model_files")
+    return _resolve(asset_root, m) if m else None
 
 
 def build_parser():
@@ -101,6 +120,7 @@ def main(argv=None):
     opts, scene_args = build_parser().parse_known_args(sys.argv[1:] if argv is None else argv)
     root = opts.asset_root or default_asset_root()
     agent_file, out_path, int_path = resolve_args(scene_args, root)
+    model_files = resolve_model_files(scene_args, root)
     cfg = AgentConfig.from_json(agent_file)
     rank, world, local_rank = rank_world()
     group, device = None, opts.device
@@ -116,7 +136,7 @@ def main(argv=None):
         os.makedirs(int_path, exist_ok=True)
     ckpt = rank_path(os.path.join(out_path, "agent0_checkpoint.pt"), rank)
     tr = Trainer(scene_args, cfg, root, opts.num_envs, window_steps=opts.window_steps, backend=opts.backend, seed=opts.seed, device=device,
-                 log_path=os.path.join(out_path, "agent0_log.txt"), append_log=opts.resume is not None, process_group=group)
+                 log_path=os.path.join(out_path, "agent0_log.txt"), append_log=opts.resume is not None, process_group=group, model_files=model_files)
     if opts.resume:
         tr.load(rank_path(opts.resume, rank))
     try:

@@ -265,6 +265,12 @@ class Trainer:
     read, so a run resumed from a checkpoint continues bit for bit.  env and test_env replace the two handles (tests drive the loop's
     bookkeeping with stand-ins on the CPU).
 
+    model_files (--model_files): a reference TensorBundle prefix or a Trainer checkpoint (deepmimic_b200/model_files.py) whose actor, critic,
+    discriminator (a Trainer checkpoint's, for an AMP agent) and normalisers replace the random initialisation.  The run still starts at
+    iteration 0 with zero momentum and freshly seeded generators; the loaded normalisers keep their statistics and count (NormalizerSamples
+    when the file has no count).  What the file lacks stays as initialised and is listed in model_notes.  The path joins the run record that
+    load_state_dict compares: a run started from model files resumes with the same model_files (and arguments).
+
     Host synchronisations: none per policy step; per iteration a fixed number, independent of window_steps, of the minibatch and discriminator
     step counts (tools/train_time.py counts them).  With a process group of more than one rank, each PPO update adds one (the learners' check
     that every rank's window has the same size).
@@ -280,7 +286,7 @@ class Trainer:
     world size and the state its rank, both of which load_state_dict() requires to match."""
 
     def __init__(self, args, config, asset_root, num_envs, window_steps=32, backend="tensor_core", seed=0, device=0, log_path=None, append_log=False,
-                 env=None, test_env=None, process_group=None):
+                 env=None, test_env=None, process_group=None, model_files=None):
         import torch
         from .env import DeepMimicBatchEnv
         from .learner import AMPDiscLearner, DataParallel, PPOLearner
@@ -300,7 +306,7 @@ class Trainer:
         self.window_steps = int(window_steps)
         # what a checkpoint must match
         self.run = dict(args=self.args, agent=config.values, num_envs=int(num_envs), window_steps=self.window_steps, backend=backend, seed=self.seed,
-                        world=self.world)
+                        world=self.world, model_files=model_files)
         rs = self.seed + 1000 * self.rank   # the rank's generators
         cfg = config
         self.env = env = env or DeepMimicBatchEnv(self.args, local, asset_root, device=device, seed=self.seed, global_env_offset=self.rank * local)
@@ -323,6 +329,16 @@ class Trainer:
         self.ro = BatchedRollout(env, policy, exp_rate=cfg["ExpParamsBeg"]["Rate"], noise=noise, seed=rs, backend=backend, disc=disc,
                                  task_reward_lerp=cfg["TaskRewardLerp"] if self.amp else None, critic=critic, discount=cfg["Discount"],
                                  td_lambda=cfg["TDLambda"])
+        self.model_notes = []
+        if model_files is not None:
+            # before the learners take the parameters; a normaliser without a count in the file counts NormalizerSamples samples, so the
+            # first windows' statistics are weighed against it rather than replacing it (a reading of RLAgent.load_model that has not been
+            # checked against the reference's source)
+            from .model_files import load_model_files
+            loaded = load_model_files(model_files, policy, self._all_norms(), critic=self.ro.critic, disc=self.ro.disc)
+            for name, count in loaded["counts"].items():
+                self._all_norms()[name].count = cfg["NormalizerSamples"] if count is None else count
+            self.model_notes = loaded["notes"]
         self.ppo = PPOLearner(self.ro, actor_stepsize=cfg["ActorStepsize"], actor_momentum=cfg["ActorMomentum"], actor_weight_decay=cfg["ActorWeightDecay"],
                               critic_stepsize=cfg["CriticStepsize"], critic_momentum=cfg["CriticMomentum"], critic_weight_decay=cfg["CriticWeightDecay"],
                               ratio_clip=cfg["RatioClip"], norm_adv_clip=cfg["NormAdvClip"], minibatch_size=cfg["MiniBatchSize"], epochs=cfg["Epochs"],
@@ -462,25 +478,20 @@ class Trainer:
         """Test_Return: the mean return of one complete episode of each evaluation environment (test mode, exploration off), from the start
         state the evaluation handle had when it was created; with several ranks, the sum of every rank's returns over their number of episodes.
         One host synchronisation per 32 policy steps."""
+        from .rollout import run_episodes
         t, env, ro = self.torch, self.test_env, self.test_ro
         env.load_state_dict(self._test_start)
         ro.gen.manual_seed(self.seed + 1000 * self.rank)
         if self.backend == "tensor_core":
             ro.refresh_tensor_core_policy()
-        n = env.num_envs
-        ret, ended = t.zeros(n, device=env.device), t.zeros(n, dtype=t.bool, device=env.device)
-        limit = 1 << 16
-        for _ in range(0, limit, 32):
-            traj = ro.collect(32, record_stats=False)
-            for r, d in zip(traj["rewards"], traj["dones"]):
-                ret += t.where(ended, t.zeros_like(r), r)
-                ended |= d
-            if bool(ended.all()):
-                if not self.dp:
-                    return ret.mean().item()
-                s = self.dp.sum(t.stack([ret.sum(), t.tensor(float(n), device=env.device)])).tolist()
-                return s[0] / s[1]
-        raise RuntimeError("evaluation: an episode ran longer than %d policy steps" % limit)
+        try:
+            ret = run_episodes(ro)["returns"]
+        except RuntimeError as e:
+            raise RuntimeError("evaluation: %s" % e) from None
+        if not self.dp:
+            return ret.mean().item()
+        s = self.dp.sum(t.stack([ret.sum(), t.tensor(float(env.num_envs), device=env.device)])).tolist()
+        return s[0] / s[1]
 
     # ---- checkpoints
     def state_dict(self):
@@ -509,6 +520,9 @@ class Trainer:
         is refused).  Parameters and accumulators are loaded in place (the tensor-core learners hold their addresses); the rollout's
         tensor-core handles are rebuilt from the loaded weights and normalisers."""
         t, ro = self.torch, self.ro
+        if s["run"].get("model_files") != self.run["model_files"]:   # a checkpoint without the key is a run from random initialisation
+            raise ValueError("checkpoint: its run started from model files %s, this one from %s: resume with the arguments the run started with, "
+                             "--model_files included" % (s["run"].get("model_files"), self.run["model_files"]))
         for k in self.run:
             if s["run"].get(k, 1 if k == "world" else None) != self.run[k]:   # a checkpoint without a world size is a one-rank run's
                 raise ValueError("checkpoint: its %s differs from this run's" % ("agent file" if k == "agent" else "world size" if k == "world" else k))

@@ -113,6 +113,12 @@ int dm_plan_env_order(const int* keys, int n_padded, int tiles, int W, int* orde
 int dm_get_env_order(dm_handle* h, int* h_plan3, int* h_keys, int* h_order);
 int dm_record_state(dm_handle* h, float* d_out);             /* [num_envs x state_size] */
 int dm_record_goal(dm_handle* h, float* d_out);              /* [num_envs x goal_size] (no-op when goal_size == 0) */
+/* The simulated character's pose and velocity (cSimCharacter::BuildPose / BuildVel, R/DeepMimicCore/sim/SimCharacter.cpp:1428-1507):
+ * [num_envs x pose_dim] fp32 rows in the reference's layout -- root position, root quaternion (w, x, y, z) with w >= 0, then per joint a
+ * w-first quaternion (spherical) or the angle wrapped to [-pi, pi] (revolute); the velocity rows hold the root's linear then angular velocity
+ * and a 0, then the joints' angular velocities (spherical: 3 and a 0) or rates.  Either pointer may be NULL.  Stream-ordered, no host
+ * synchronisation. */
+int dm_record_pose(dm_handle* h, float* d_pose, float* d_vel);
 /* AMP task scenes target_amp / heading_amp (cSceneTargetAMP / cSceneHeadingAMP: RecordGoal, CalcReward, target updates; goal_size 3).
  * heading_amp_getup / strike_amp are EXPERIMENTAL (device code written and host-checked, not validated on hardware): dm_create accepts
  * them only with DM_EXPERIMENTAL_TASK_SCENES=1 in the environment.  dm_goal_host is RecordGoal into a host buffer [num_envs x 3]; the task-state hooks
