@@ -60,7 +60,7 @@ class DmLearnGatedBatch(C.Structure):
 DM_STATE_OFFSET, DM_STATE_SCALE, DM_ACTION_OFFSET, DM_ACTION_SCALE, DM_ACTION_BOUND_MIN, DM_ACTION_BOUND_MAX, DM_STATE_NORM_GROUPS = range(7)
 
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
-           "dm_update", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_record_pose", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
+           "dm_update", "dm_set_pushes", "dm_get_pushes", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_record_pose", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
            "dm_set_snapshot", "dm_state_size", "dm_save_state", "dm_load_state", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
            "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy", "dm_td_lambda_returns", "dm_mlp_set_weights_device", "dm_learn_create",
            "dm_mlp_set_normalizers_device", "dm_learn_set_weights", "dm_learn_step", "dm_learn_disc_step", "dm_learn_destroy",
@@ -98,6 +98,9 @@ def lib():
         L.dm_set_action.argtypes = [vp, fp]
         L.dm_update.argtypes = [vp, C.c_double, C.c_int]
         L.dm_set_env_order.argtypes = [vp, C.c_int]
+        if hasattr(L, "dm_set_pushes"):   # a library built before pushes (the base build of tools/ab_step.py) still loads; calling them fails
+            L.dm_set_pushes.argtypes = [vp, C.POINTER(C.c_int32), fp, dp, dp]
+            L.dm_get_pushes.argtypes = [vp, C.POINTER(C.c_int32)]
         L.dm_plan_env_order.argtypes = [C.POINTER(C.c_int), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)]
         L.dm_get_env_order.argtypes = [vp, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.dm_record_state.argtypes = [vp, fp]
@@ -283,6 +286,29 @@ class BatchedCore:
 
     def update(self, dt, n_updates=1):
         self._chk(lib().dm_update(self.h, dt, n_updates))
+
+    def set_pushes(self, body, force, start, duration):
+        """dm_set_pushes: a timed external force per environment -- body [N] int32 (-1: none), force [N, 3] float32 (world axes, unscaled N,
+        at the body's COM), start and duration [N] float64 (seconds on the episode timer).  numpy arrays or tensors (copied to the host) of
+        exactly these shapes and dtypes; the library refuses out-of-range values by name.  Synchronises the handle's stream."""
+        N = self.num_envs
+        arrs = []
+        for name, a, dt, shape in (("body", body, np.int32, (N,)), ("force", force, np.float32, (N, 3)), ("start", start, np.float64, (N,)),
+                                   ("duration", duration, np.float64, (N,))):
+            if hasattr(a, "detach"):
+                a = a.detach().cpu().numpy()
+            a = np.asarray(a)
+            if a.dtype != dt or a.shape != shape:
+                raise ValueError("set_pushes: %s must be %s of shape %s, got %s of shape %s" % (name, np.dtype(dt).name, shape, a.dtype, a.shape))
+            arrs.append(np.ascontiguousarray(a))
+        b, f, s, d = arrs
+        self._chk(lib().dm_set_pushes(self.h, b.ctypes.data_as(C.POINTER(C.c_int32)), f.ctypes.data_as(C.POINTER(C.c_float)), _dptr(s), _dptr(d)))
+
+    def pushes(self):
+        """dm_get_pushes: every environment's pending push body, int32 [N] (-1: none).  Synchronises the handle's stream."""
+        out = np.zeros(self.num_envs, dtype=np.int32)
+        self._chk(lib().dm_get_pushes(self.h, out.ctypes.data_as(C.POINTER(C.c_int32))))
+        return out
 
     def set_env_order(self, on):
         """dm_set_env_order: place the environments in the step kernel by contact load (the default; tile width 16 only) or by index"""

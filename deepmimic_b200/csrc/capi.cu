@@ -98,6 +98,7 @@ struct dm_handle {
     float *p_act = nullptr, *p_obs = nullptr, *p_rew = nullptr; int32_t* p_flags = nullptr;  // pinned host staging
     cudaStream_t stream = nullptr;
     int device = 0, num_envs = 0, padded_envs = 0, W = 32, tiles = 2, maxrows = 36, smem_bytes = 0, mode = 0;
+    dmk::DevPush* d_push = nullptr;   // push table (dm_set_pushes): null until the first call, then the step launches use the push instantiations
     int* d_order = nullptr;   // placement of the environments in the step kernel's tiles (dm_set_env_order); st.order is it or null
     dmk::StepLayout lay{};
     uint64_t seed = 0, env_offset = 0;
@@ -354,14 +355,16 @@ int launched(dm_handle* h) {
 }
 
 int launch_step(dm_handle* h, double dt, int n_updates) {
-    const dmk::StepKernel kern = dmk::kStepKernels[tile_index(h)][task_scene(h)];   // AMP task scenes: the variant that also advances the task block
+    // AMP task scenes: the variant that also advances the task block; handles with a push table (dm_set_pushes): the push kernel, which applies it
+    const void* kern = h->d_push ? reinterpret_cast<const void*>(dmk::kStepPushKernels[tile_index(h)][task_scene(h)])
+                                 : reinterpret_cast<const void*>(dmk::kStepKernels[tile_index(h)][task_scene(h)]);
     // opt in to the large dynamic shared-memory carve-out; the limit is raised whenever a handle needs more than any earlier one on
     // this device (attributes are per device and per function: several handles of different sizes may live in one process)
     static std::mutex mu;
     static std::map<std::pair<int, const void*>, int> configured;   // (device, kernel) -> bytes configured
     {
         std::lock_guard<std::mutex> lock(mu);
-        int& have = configured[{h->device, reinterpret_cast<const void*>(kern)}];
+        int& have = configured[{h->device, kern}];
         if (h->smem_bytes > have) {
             DM_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_bytes));
             DM_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
@@ -374,8 +377,13 @@ int launch_step(dm_handle* h, double dt, int n_updates) {
         dmk::dm_env_order_kernel<<<1, dmk::kEnvOrderThreads, 0, h->stream>>>(h->st.load, h->padded_envs, h->tiles, h->W, h->d_order);
         if (launched(h)) return 1;
     }
-    kern<<<h->padded_envs / h->tiles, h->tiles * h->W, h->smem_bytes, h->stream>>>(h->d_model, h->st, h->d_frame_times, h->d_frames, dt, n_updates,
-                                                                                   h->sa.cfg.num_sim_substeps, h->lay);
+    const dim3 grid(h->padded_envs / h->tiles), block(h->tiles * h->W);
+    if (h->d_push)
+        dmk::kStepPushKernels[tile_index(h)][task_scene(h)]<<<grid, block, h->smem_bytes, h->stream>>>(h->d_model, h->st, h->d_frame_times, h->d_frames, dt,
+                                                                                                      n_updates, h->sa.cfg.num_sim_substeps, h->lay, h->d_push);
+    else
+        dmk::kStepKernels[tile_index(h)][task_scene(h)]<<<grid, block, h->smem_bytes, h->stream>>>(h->d_model, h->st, h->d_frame_times, h->d_frames, dt, n_updates,
+                                                                                                  h->sa.cfg.num_sim_substeps, h->lay);
     return launched(h);
 }
 int launch_observe_fan(dm_handle* h, const dmk::ObsFan& fan) {
@@ -804,6 +812,10 @@ int dm_reset_clips(dm_handle* h, int force_all, const int* h_clip, const double*
     const double* src[3] = {kt, mt, th};
     for (int k = 0; k < 3; ++k) if (src[k] && stage_envs(h, src[k], h->d_inj[k])) return 1;
     if (h_clip && stage_envs(h, h_clip, h->d_clip_inj)) return 1;
+    if (h->d_push) {   // the environments about to be reset lose their push (cWorld::Reset clears its perturbations)
+        dmk::dm_push_clear_kernel<<<(h->num_envs + 127) / 128, 128, 0, h->stream>>>(h->st, h->d_push, force_all);
+        if (launched(h)) return 1;
+    }
     if (launch_reset(h, force_all, kt ? h->d_inj[0] : nullptr, mt ? h->d_inj[1] : nullptr, th ? h->d_inj[2] : nullptr, h_clip ? h->d_clip_inj : nullptr)) return 1;
     if (!task_scene(h)) return 0;
     // cSceneTargetAMP::Reset's own part for the environments that were just reset
@@ -826,6 +838,41 @@ int dm_set_action(dm_handle* h, const float* d_actions) {
 int dm_update(dm_handle* h, double dt, int n_updates) {
     DM_DEVICE(h);
     return launch_step(h, dt, n_updates);
+}
+int dm_set_pushes(dm_handle* h, const int32_t* h_body, const float* h_force, const double* h_start, const double* h_duration) {
+    DM_DEVICE(h);
+    if (!h_body || !h_force || !h_start || !h_duration) { g_err = "dm_set_pushes: every array is required"; return fail(); }
+    const int N = h->num_envs, nl = h->hm.nl;
+    std::vector<dmk::DevPush> tab(static_cast<size_t>(N));
+    for (int e = 0; e < N; ++e) {
+        auto refuse = [&](const char* what) { g_err = std::string("dm_set_pushes: environment ") + std::to_string(e) + ": " + what; return fail(); };
+        if (h_body[e] < -1 || h_body[e] >= nl) return refuse(("body out of [-1, " + std::to_string(nl) + ")").c_str());
+        for (int k = 0; k < 3; ++k) if (!std::isfinite(h_force[3 * e + k])) return refuse("force is not finite");
+        if (!std::isfinite(h_start[e])) return refuse("start is not finite");
+        if (!std::isfinite(h_duration[e]) || h_duration[e] < 0.0) return refuse("duration is negative or not finite");
+        dmk::DevPush& p = tab[e];
+        p.force[0] = h_force[3 * e]; p.force[1] = h_force[3 * e + 1]; p.force[2] = h_force[3 * e + 2];
+        p.body = h_body[e]; p.start = h_start[e]; p.duration = h_duration[e];
+    }
+    if (h->d_push == nullptr) {   // the padding environments never run: their entries stay empty
+        if (alloc_buffer(h, &h->d_push, static_cast<size_t>(h->padded_envs))) return 1;
+        std::vector<dmk::DevPush> none(static_cast<size_t>(h->padded_envs));
+        for (auto& p : none) { p.force[0] = p.force[1] = p.force[2] = 0.f; p.body = -1; p.start = 0.0; p.duration = 0.0; }
+        DM_CUDA(cudaMemcpyAsync(h->d_push, none.data(), none.size() * sizeof(dmk::DevPush), cudaMemcpyHostToDevice, h->stream));
+        DM_CUDA(cudaStreamSynchronize(h->stream));
+    }
+    DM_CUDA(cudaMemcpyAsync(h->d_push, tab.data(), tab.size() * sizeof(dmk::DevPush), cudaMemcpyHostToDevice, h->stream));
+    DM_CUDA(cudaStreamSynchronize(h->stream));   // the staging vector is pageable
+    return 0;
+}
+int dm_get_pushes(dm_handle* h, int32_t* h_body) {
+    DM_DEVICE(h);
+    if (h->d_push == nullptr) { std::fill(h_body, h_body + h->num_envs, -1); return 0; }
+    std::vector<dmk::DevPush> tab(static_cast<size_t>(h->num_envs));
+    DM_CUDA(cudaMemcpyAsync(tab.data(), h->d_push, tab.size() * sizeof(dmk::DevPush), cudaMemcpyDeviceToHost, h->stream));
+    DM_CUDA(cudaStreamSynchronize(h->stream));
+    for (int e = 0; e < h->num_envs; ++e) h_body[e] = tab[e].body;
+    return 0;
 }
 int dm_set_env_order(dm_handle* h, int on) {
     DM_DEVICE(h);
@@ -1293,6 +1340,12 @@ int dm_state_size(dm_handle* h, size_t* bytes) {
 }
 int dm_save_state(dm_handle* h, void* h_out) {
     DM_DEVICE(h);
+    if (h->d_push) {   // a pending push is not part of the state blob
+        std::vector<int32_t> body(static_cast<size_t>(h->num_envs));
+        if (dm_get_pushes(h, body.data())) return 1;
+        for (int e = 0; e < h->num_envs; ++e)
+            if (body[e] >= 0) { g_err = "dm_save_state: environment " + std::to_string(e) + " has a pending push (dm_set_pushes); the state blob does not carry pushes"; return fail(); }
+    }
     const StateHeader H = state_header(h);
     char* o = static_cast<char*>(h_out);
     std::memcpy(o, &H, sizeof(H));

@@ -125,6 +125,18 @@ constexpr int kFlagInts = 8;
 enum FlagSlot { kFNeedAction = 0, kFDone = 1, kFTerminate = 2, kFValid = 3, kFFallen = 4, kFRowOverflow = 5, kFUpdates = 6 };
 // MANIFOLD block, floats: nl x 4 points x 12 = {valid, lAx,lAy,lAz, wBx,wBy,wBz, impN, impL1, impL2, dist, life}
 
+// A timed external force on one body (dm_set_pushes): force (world axes, unscaled N) at the body's COM in both Bullet sub-steps of every update
+// whose timer value at its start t satisfies start <= t < start + duration.  body -1: none; the step kernel sets it at the commit of the update
+// after which t >= start + duration, dm_reset at the environment's reset.  A handle's push table holds one entry per environment id (not tile
+// slot, so placement by contact load moves a push with its environment) and reaches dm_step_push_kernel as its last parameter, not as a
+// DevState field: a larger DevState would move every later parameter of every kernel that takes it.
+struct DevPush {
+    float force[3];
+    int body;
+    double start, duration;
+};
+static_assert(sizeof(DevPush) == 32, "DevPush: the step kernel reads force and body as one float4");
+
 struct DevState {
     float* sim;
     double* time;
@@ -190,11 +202,13 @@ struct StepLayout {
 // expert sampler's TASKV is "clip drawn from the dataset".
 constexpr int kPolicyBlock = 64;   // threads per block of the observe, AMP and reset kernels
 using StepKernel = void (*)(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout);
+using StepPushKernel = void (*)(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout, DevPush*);
 using ObserveKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, ObsFan, int);
 using ResetKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, int, const double*, const double*, const double*,
                              unsigned long long, unsigned long long, int, const int*);
 using AmpObsKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, float*, int, const double*, int, const int*);
 extern const StepKernel kStepKernels[2][2];
+extern const StepPushKernel kStepPushKernels[2][2];   // dm_step_push_kernel: handles with a push table (dm_set_pushes)
 extern const ObserveKernel kObserveKernels[2][2];
 extern const ResetKernel kResetKernels[2][2];
 extern const AmpObsKernel kAmpObsKernels[2][2];
@@ -207,6 +221,7 @@ __global__ void dm_set_action_kernel(const DevModel*, DevState, const float*, in
 constexpr int kPoseEnvsPerBlock = 8;   // dm_pose_kernel: kPoseEnvsPerBlock x links threads, 2 pose_dim floats of shared memory per environment
 __global__ void dm_pose_kernel(const DevModel*, DevState, float*, float*, int);
 __global__ void dm_task_reset_kernel(const DevModel*, DevState, int);
+__global__ void dm_push_clear_kernel(DevState, DevPush*, int);
 __global__ void dm_task_observe_kernel(const DevModel*, DevState, float*, float*, int);
 int dm_step_layout(int nl, int n, int chain_len, int maxrows, int W, StepLayout* L);
 int dm_step_smem_bytes(const StepLayout& L, int tiles);

@@ -803,8 +803,12 @@ __device__ __noinline__ int collide(float* mani, int alive, int mcnt) {
 //   (deepest first) = one step of the tree-structured L^T D L; base: 6x6 Cholesky in world axes (= the generalised base coordinates);
 //   root -> leaves: accelerations.  Bullet sub-steps (bullet != 0) also publish the factors (sU, sG), advance the link velocities in sV
 //   and the base velocity in sB by h * acceleration.  Returns this link's joint accelerations.
-template <int W>
-__device__ __noinline__ float3 aba_solve(float g0, float g1, float g2, float kdt, int bullet, float jvx, float jvy, float jvz) {
+// PUSH (aba_solve_push) with bullet == 2: a Bullet sub-step with an external force on one body at its COM, staged by the caller in the limit-row
+// slots (sQ: force, body), which are dead until the constraint rows of the sub-step are written.  The lane of the dynamics body that holds the
+// body subtracts the spatial force about its reference point from its bias force (the root's lane: the base origin; a lumped leaf's force goes
+// to its parent's lane, applied at the leaf's own COM).
+template <int W, bool PUSH>
+__device__ __forceinline__ float3 aba_solve_body(float g0, float g1, float g2, float kdt, int bullet, float jvx, float jvy, float jvz) {
     const Ctx c = make_ctx<W>();
     const float gx = step_smem()[kHGrav], gy = step_smem()[kHGrav + 1], gz = step_smem()[kHGrav + 2], h = step_smem()[kHh];
     using T = Tl<W>;
@@ -881,6 +885,24 @@ __device__ __noinline__ float3 aba_solve(float g0, float g1, float g2, float kdt
         const V3 hn = sym_mul(IA.ww, vel.a) + cross(md, vel.l), hf = mass * vel.l + cross(vel.a, md);
         const V3 an = sym_mul(IA.ww, ab.a) + cross(md, ab.l), af = mass * ab.l + cross(ab.a, md);
         pA = mks(an + cross(vel.a, hn) + cross(vel.l, hf), af + cross(vel.a, hf));
+    }
+    if constexpr (PUSH) {
+        if (bullet == 2) {
+            const float4 pf = ld4(c.E + LY.oQ);
+            const int b = __float_as_int(pf.w);
+            const int bdyn = reinterpret_cast<const int*>(c.LK + b * kLkFloats)[kLDyn];
+            const int lane_b = (((bdyn >> 8) & 0xff) == 100) ? (reinterpret_cast<const int*>(c.LK + b * kLkFloats)[kLInt] & 0xff) : b;
+            if (c.lane == lane_b) {
+                const float s = step_smem()[kHScale];
+                const V3 F = mk3(s * pf.x, s * pf.y, s * pf.z);
+                const float* wb = sW + b * 12; const float* vb = sV + b * 12;
+                const V3 xcom = mk3(wb[9] + vb[6], wb[10] + vb[7], wb[11] + vb[8]);
+                const float* wr = sW + c.li * 12;
+                const V3 xref = isroot ? mk3(sB[0], sB[1], sB[2]) : mk3(wr[9], wr[10], wr[11]);
+                pA.a -= cross(xcom - xref, F);
+                pA.l -= F;
+            }
+        }
     }
     // U_d = IA s_d goes straight to the environment's factor table (sU: read back by the acceleration pass below and, in the Bullet sub-steps,
     // by the constraint rows and the velocity correction) instead of living in 18 registers across the leaves -> root loop
@@ -1035,6 +1057,14 @@ __device__ __noinline__ float3 aba_solve(float g0, float g1, float g2, float kdt
     __syncwarp();
     return make_float3(qd0, qd1, qd2);
 }
+template <int W>
+__device__ __noinline__ float3 aba_solve(float g0, float g1, float g2, float kdt, int bullet, float jvx, float jvy, float jvz) {
+    return aba_solve_body<W, false>(g0, g1, g2, kdt, bullet, jvx, jvy, jvz);
+}
+template <int W>
+__device__ __noinline__ float3 aba_solve_push(float g0, float g1, float g2, float kdt, int bullet, float jvx, float jvy, float jvz) {
+    return aba_solve_body<W, true>(g0, g1, g2, kdt, bullet, jvx, jvy, jvz);
+}
 
 // Velocity correction of the constraint impulses: dv = L^-1 D^-1/2 z with z = Y^T lambda (sZ), by the root -> leaves pass over the factors
 // published by aba_solve.  Lane 0 also corrects the base velocity in sB.  Returns this link's joint-rate corrections.
@@ -1131,7 +1161,8 @@ enum LoopField : int {
     kLsClock = 6 + 3 * 32,       // clocks of the update: bit 0 new-action edge, bit 1 time limit reached, bit 2 non-looping clip finished
     kLsMcnt = 9 + 3 * 32,        // cached points of this lane's link after the last collision pass; 4 (unknown) at the start of a launch
     kLsNpts = 12 + 5 * 32,       // contact points of the current Bullet sub-step (<= maxpts = 17)
-    kLsRows = 17 + 8 * 32        // solver rows of the last Bullet sub-step: the environment's contact-load key (DevState::load)
+    kLsRows = 17 + 8 * 32,       // solver rows of the last Bullet sub-step: the environment's contact-load key (DevState::load)
+    kLsPush = 25 + 32            // PUSH: the environment's push acts in this update's Bullet sub-steps
 };
 static_assert(dm_step_y_stride(32) / 3 < 32 && dm_step_y_stride(32) < 256, "contact points and solver rows must fit their LoopBits fields");
 // One 32-bit word, fields by shift and mask: the compiler keeps a struct of C++ bit-fields in a register per few fields.
@@ -1170,10 +1201,13 @@ struct EnvRefs {
 };
 
 // TASK: the AMP task scenes' instantiation, which also advances the environment's task block after every update (dm_task.cuh); the plain
-// imitate kernel carries none of that code.
-template <int W, bool TASK>
-__global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevModel* __restrict__ gm, DevState st, const double* __restrict__ frame_times,
-                                                                       const float* __restrict__ frames, double dt, int n_updates, int sim_substeps, StepLayout LY) {
+// imitate kernel carries none of that code.  PUSH: the body of dm_step_push_kernel, the kernel of handles with a push table (dm_set_pushes),
+// which applies the environment's push (push_in, by environment id) in the Bullet sub-steps of the updates inside its window and clears the
+// entry once the window has passed.
+template <int W, bool TASK, bool PUSH>
+__device__ __forceinline__ void dm_step_body(const DevModel* __restrict__ gm, const DevState& st, const double* __restrict__ frame_times,
+                                             const float* __restrict__ frames, double dt, int n_updates, int sim_substeps, const StepLayout& LY,
+                                             DevPush* push_in) {
     using T = Tl<W>;
     extern __shared__ __align__(16) float sm[];
     const int tiles = blockDim.x / W;
@@ -1411,6 +1445,10 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
                 if (!term && (ls.get(kLsClock) & 4)) term = 1;
                 if (TASK && !term && task_fail) term = task_fail;
                 if (lane == 0) ++reinterpret_cast<int*>(sB)[kBUpdates];
+                if constexpr (PUSH) {
+                    DevPush* pu = push_in + r.env;
+                    if (lane == 0 && pu->body >= 0 && r.tm[kTTimer] >= pu->start + pu->duration) pu->body = -1;
+                }
                 const bool end = (ls.get(kLsClock) & 2) || term;
                 if (end || stage == total_stages) {   // commit
                     float* sim = r.sim; int* fl = r.fl;
@@ -1451,7 +1489,7 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
             const EnvRefs<W> r(st, LY, env);
             const int lane = r.lane, li = r.li;
             float* sB = r.sB;
-            int cb = 0;
+            int cb = 0, pushed = 0;
             if constexpr (TASK) {
                 // cDeepMimicCharController::HandleNewAction (DeepMimicCharController.cpp:262-267): COM of the state the new action starts from
                 if (__ballot_sync(0xffffffffu, ls.get(kLsAlive) && ls.get(kLsNeedAction)) != 0u) {
@@ -1464,6 +1502,10 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
             if (lane == 0 && ls.get(kLsAlive)) {
                 double* tm = r.tm;
                 const double timer = tm[kTTimer] + dt;
+                if constexpr (PUSH) {
+                    const DevPush& pu = push_in[r.env];
+                    pushed = (pu.body >= 0 && pu.start <= tm[kTTimer] && tm[kTTimer] < pu.start + pu.duration) ? 1 : 0;
+                }
                 double kin_time = tm[kTKin];
                 double dur_ = M.motion_dur;
                 if constexpr (TASK) dur_ = st.ctab->info[st.clip[r.env]].dur;   // the environment's own clip of the dataset
@@ -1497,6 +1539,7 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
                 if (M.end_at_clip_end && kin_time >= dur) cb |= 4;
             }
             ls.set(kLsClock, T::shfli(cb, 0));
+            if constexpr (PUSH) ls.set(kLsPush, T::shfli(pushed, 0));
             ls.set(kLsNeedAction, 0);
             PROF(3);
             // ---------------- cImpPDController::CalcControlForces (ImpPDController.cpp:136-195) in the body-frame joint coordinates of the sim state
@@ -1543,7 +1586,17 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
         }
         PROF(3);
         {   // unconstrained accelerations, v += a h (the base and the link velocities are advanced inside)
-            const float3 qdd = aba_solve<W>(tau0, tau1, tau2, 0.f, 1, jv.x, jv.y, jv.z);
+            float3 qdd;
+            if constexpr (PUSH) {
+                {   // the environment's push into its limit-row slots (aba_solve_body)
+                    const EnvRefs<W> r(st, LY, env);
+                    if (r.lane == 0 && ls.get(kLsPush)) *reinterpret_cast<float4*>(r.E + LY.oQ) = *reinterpret_cast<const float4*>(push_in + r.env);
+                    __syncwarp();
+                }
+                qdd = aba_solve_push<W>(tau0, tau1, tau2, 0.f, ls.get(kLsPush) ? 2 : 1, jv.x, jv.y, jv.z);
+            } else {
+                qdd = aba_solve<W>(tau0, tau1, tau2, 0.f, 1, jv.x, jv.y, jv.z);
+            }
             const EnvRefs<W> r(st, LY, env);
             const float h = step_smem()[kHh];
             const int ndof = r.act ? ((r.lk_int(kLInt) >> 16) & 0xff) : 0;
@@ -1625,7 +1678,29 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevMo
 #endif
 }
 
+template <int W, bool TASK>
+__global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevModel* __restrict__ gm, DevState st, const double* __restrict__ frame_times,
+                                                                       const float* __restrict__ frames, double dt, int n_updates, int sim_substeps, StepLayout LY) {
+    dm_step_body<W, TASK, false>(gm, st, frame_times, frames, dt, n_updates, sim_substeps, LY, nullptr);
+}
+// a kernel of its own (not a third flag of dm_step_kernel): its own signature, and the plain kernels stay exactly what they were
+template <int W, bool TASK>
+__global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_push_kernel(const DevModel* __restrict__ gm, DevState st, const double* __restrict__ frame_times,
+                                                                            const float* __restrict__ frames, double dt, int n_updates, int sim_substeps, StepLayout LY,
+                                                                            DevPush* push) {
+    dm_step_body<W, TASK, true>(gm, st, frame_times, frames, dt, n_updates, sim_substeps, LY, push);
+}
+
 const StepKernel kStepKernels[2][2] = {{dm_step_kernel<16, false>, dm_step_kernel<16, true>}, {dm_step_kernel<32, false>, dm_step_kernel<32, true>}};
+const StepPushKernel kStepPushKernels[2][2] = {{dm_step_push_kernel<16, false>, dm_step_push_kernel<16, true>}, {dm_step_push_kernel<32, false>, dm_step_push_kernel<32, true>}};
+
+// dm_reset's part of the push table: the environments the reset kernel is about to restart (the same rule) lose their push, as cWorld::Reset
+// clears its perturbations.  Launched before the reset kernel, only on handles with a push table.
+__global__ void dm_push_clear_kernel(DevState st, DevPush* push, int force) {
+    const int env = blockIdx.x * blockDim.x + threadIdx.x;
+    if (env >= st.num_real) return;
+    if (force || st.flags[static_cast<size_t>(env) * kFlagInts + kFDone] != 0) push[env].body = -1;
+}
 
 // Placement of the environments for the next step-kernel launch (dm_model.cuh: env_load_bucket, env_order_slot).  One block of kEnvOrderThreads;
 // it runs between two step launches on the same stream, so its latency is what it costs: few barriers, no serial loop over the warps.

@@ -51,6 +51,13 @@ class DeepMimicBatchEnv:
     def get_time(self):
         return self._time
 
+    def set_pushes(self, body, force, start, duration):
+        """Push the characters: environment e's body body[e] (-1: none) gets force[e] (world axes, unscaled N, at the body's COM) in every
+        update whose episode time at its start t satisfies start[e] <= t < start[e] + duration[e].  Shapes [N], [N, 3], [N], [N]; dtypes int32,
+        float32, float64, float64 (numpy arrays or tensors).  An entry clears once its window has passed and at the environment's reset."""
+        self._pre()
+        self._core.set_pushes(body, force, start, duration)
+
     def get_name(self):
         """cScene::GetName of the configured scene (SceneImitate.cpp:209, SceneImitateAMP.cpp:211, SceneTargetAMP.cpp:233, ...)"""
         return self._core.scene_name()

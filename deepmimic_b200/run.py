@@ -1,7 +1,8 @@
 """Run a trained skill: the counterpart of the reference's `DeepMimic.py --arg_file args/run_*_args.txt`, without the viewer.
 
     python -m deepmimic_b200.run --arg_file args/run_humanoid3d_spinkick_args.txt [--model_files PATH] [--num_envs 64]
-        [--record_motion K] [--episode_time 20] [--backend tensor_core] [--seed 0] [--device 0] [--asset_root DIR] [reference arguments ...]
+        [--record_motion K] [--episode_time 20] [--backend tensor_core] [--seed 0] [--device 0] [--asset_root DIR]
+        [--push_forces F1,F2,... [--push_body 0] [--push_time 2.0] [--push_duration 0.2]] [reference arguments ...]
 
 --model_files (a reference TensorBundle prefix or a Trainer checkpoint, deepmimic_b200/model_files.py) and --output_path are read from the
 argument list, the command line before the arg file, as deepmimic_b200.train reads its paths; --train_agents and --agent_files are accepted
@@ -12,7 +13,13 @@ arg files: the reference's viewer runs until the character falls), an episode en
   run_log.txt          one row per environment: its return, its length in policy steps and its terminate code (0 time limit, 1 fail, 2 success)
   motion_<env>.txt     with --record_motion K, the first K environments' episodes as motion files (cMotion::Output, loop "none", one frame per
                        policy step and the terminal pose)
-and a printed summary: the return's mean and standard deviation, the mean length and the fraction of episodes ended by Fail.  One GPU only."""
+and a printed summary: the return's mean and standard deviation, the mean length and the fraction of episodes ended by Fail.  One GPU only.
+
+Push robustness (--push_forces, the DeepMimic paper's test of a trained skill): environment e is pushed on body --push_body (default the root)
+with the horizontal force of magnitude F[e % K] in N, for --push_duration seconds from --push_time seconds into its episode (defaults 0.2 and
+2.0).  Each environment's direction is an angle drawn from --seed, the same every run.  run_log.txt then also has the columns Push_Force and
+Push_Dir (radians, about the vertical axis from +x towards +z), and the summary one line per force: episodes, the fraction not ended by Fail
+and the mean return."""
 import argparse
 import os
 import sys
@@ -30,7 +37,32 @@ def build_parser():
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--episode_time", type=float, default=20.0,
                     help="test-mode episode limit in seconds for arguments that set none (the run_* arg files; default 20, the train_* files' limit)")
+    ap.add_argument("--push_forces", type=parse_forces, default=None, metavar="F1,F2,...",
+                    help="push-robustness sweep: horizontal push magnitudes in N (>= 0), environment e gets F[e %% K]")
+    ap.add_argument("--push_body", type=int, default=0, help="body pushed in the sweep (default 0, the root)")
+    ap.add_argument("--push_time", type=float, default=2.0, help="episode time of the push in seconds (default 2.0)")
+    ap.add_argument("--push_duration", type=float, default=0.2, help="length of the push in seconds (default 0.2)")
     return ap
+
+
+def parse_forces(text):
+    try:
+        forces = [float(x) for x in text.split(",")]
+    except ValueError:
+        raise argparse.ArgumentTypeError("need comma-separated numbers, got %r" % text)
+    if not forces or any(not (f >= 0.0) or f == float("inf") for f in forces):
+        raise argparse.ArgumentTypeError("push forces must be finite and >= 0, got %r" % text)
+    return forces
+
+
+def push_plan(forces, num_envs, seed):
+    """the sweep's pushes: magnitude [N] (environment e gets forces[e % K]), direction [N] (an angle in [0, 2 pi) about the vertical axis per
+    environment, drawn from seed) and the world-axes force [N, 3] float32"""
+    import numpy as np
+    mag = np.asarray([forces[e % len(forces)] for e in range(num_envs)], dtype=np.float64)
+    ang = np.random.default_rng(seed).uniform(0.0, 2.0 * np.pi, num_envs)
+    force = np.stack([mag * np.cos(ang), np.zeros(num_envs), mag * np.sin(ang)], axis=1).astype(np.float32)
+    return mag, ang, force
 
 
 def write_episode_motions(path_fmt, ep, count, frame_dur):
@@ -55,6 +87,8 @@ def main(argv=None):
         raise SystemExit("run: one GPU only; start it without torchrun")
     if opts.num_envs < 1 or not 0 <= opts.record_motion <= opts.num_envs:
         raise SystemExit("run: need --num_envs >= 1 and 0 <= --record_motion <= --num_envs")
+    if opts.push_forces is not None and not (opts.push_duration >= 0.0 and np.isfinite(opts.push_duration) and np.isfinite(opts.push_time)):
+        raise SystemExit("run: need a finite --push_time and a finite --push_duration >= 0")
     root = opts.asset_root or default_asset_root()
     table = arg_table(scene_args, root, "run")
     out_path = first_arg(table, "output_path") or "output"
@@ -77,6 +111,10 @@ def main(argv=None):
     env = DeepMimicBatchEnv(scene_args, opts.num_envs, root, device=opts.device, seed=opts.seed)
     env.set_mode(1)
     env.reset(True)
+    if opts.push_forces is not None:
+        N = opts.num_envs
+        mag, ang, force = push_plan(opts.push_forces, N, opts.seed)
+        env.set_pushes(np.full(N, opts.push_body, dtype=np.int32), force, np.full(N, opts.push_time), np.full(N, opts.push_duration))
     ro = BatchedRollout(env, exp_rate=0.0, seed=opts.seed, backend=opts.backend)
     norms = dict(s_norm=ro.s_norm, a_norm=ro.a_norm, **(dict(g_norm=ro.g_norm) if ro.goal_size > 0 else {}))
     try:
@@ -91,10 +129,18 @@ def main(argv=None):
     for e in range(opts.num_envs):
         for k, v in (("Env", e), ("Return", float(ret[e])), ("Length", int(length[e])), ("Terminate", int(term[e]))):
             log.log_tabular(k, v)
+        if opts.push_forces is not None:
+            log.log_tabular("Push_Force", float(mag[e]))
+            log.log_tabular("Push_Dir", float(ang[e]))
         log.dump_tabular()
     log.close()
     print("%s, %d episodes: return %.4f +- %.4f, length %.1f policy steps, ended by Fail %.3f" % (model_files, opts.num_envs, float(np.mean(ret)),
                                                                                               float(np.std(ret)), float(np.mean(length)), float(np.mean(term == 1))))
+    if opts.push_forces is not None:
+        for f in opts.push_forces:
+            sel = mag == f
+            print("push %g N on body %d at %g s for %g s: %d episodes, not ended by Fail %.3f, return %.4f" % (
+                f, opts.push_body, opts.push_time, opts.push_duration, int(sel.sum()), float(np.mean(term[sel] != 1)), float(np.mean(ret[sel]))))
     if opts.record_motion:
         paths = write_episode_motions(os.path.join(out_path, "motion_%d.txt"), ep, opts.record_motion,
                                       env.get_updates_per_action() * env.UPDATE_DT)

@@ -98,6 +98,19 @@ int dm_reset(dm_handle* h, int force_all, const double* h_kin_time, const double
 int dm_set_action(dm_handle* h, const float* d_actions);
 /* n_updates consecutive Update(dt) calls in one launch; envs whose episode ended freeze until dm_reset. */
 int dm_update(dm_handle* h, double dt, int n_updates);
+/* Pushes: a timed external force on one body per environment -- the robustness test of a trained skill (the reference applies such
+ * perturbations by hand, one environment at a time, from its viewer).  Host arrays of num_envs entries: h_body [N] (a body / joint id of the
+ * character file, -1 = no push), h_force [N x 3] (world axes, the reference's unscaled N), h_start [N] and h_duration [N] (seconds on the
+ * environment's episode timer, which every reset sets to 0).  The force acts at the body's COM, times the world scale like gravity, in both
+ * Bullet sub-steps of every Update(dt) whose timer value at its start t satisfies start <= t < start + duration; the Stable-PD stage does not
+ * see it.  An entry is cleared (body -1) at the end of the update after which t >= start + duration, and by every reset of its environment.
+ * dm_set_pushes replaces every entry; it refuses, naming the environment and the argument, a body outside [-1, links), a non-finite force or
+ * start, a negative or non-finite duration, and host-only handles.  The first call allocates the handle's push table and switches its step
+ * launches to the step kernel's push instantiations; handles that never call it run exactly as before.  Stream-ordered, then synchronises
+ * the stream (the staging copy is pageable).  dm_get_pushes writes each environment's current body (-1 when none is pending) to h_body [N].
+ * dm_save_state refuses a handle with a pending push; dm_load_state leaves the push table as it is. */
+int dm_set_pushes(dm_handle* h, const int32_t* h_body, const float* h_force, const double* h_start, const double* h_duration);
+int dm_get_pushes(dm_handle* h, int32_t* h_body);
 /* Placement of the environments in the step kernel (on by default; tile width 16 only, where two environments share a warp: tile width 32
  * handles keep index placement, where it measured slower): every step launch is preceded by a one-block kernel that orders the
  * environments by contact load -- the solver row count of each environment's last Bullet sub-step, its key -- so that environments of equal
