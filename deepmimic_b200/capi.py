@@ -733,8 +733,9 @@ class TensorCoreLearner:
         if getattr(net, "goal_size", 0) or hasattr(net, "gate_common") or len(net.hidden) != 2:
             raise ValueError("the tensor-core learner implements the plain network with exactly two hidden layers (gated networks: "
                              "TensorCoreGatedLearner)")
-        self.kind = kind
-        self.layers = list(net.hidden) + [dict(actor=getattr(net, "mean", None), critic=getattr(net, "out", None), disc=getattr(net, "logit", None))[kind]]
+        self.layers = tc_layers(net, kind)
+        self._step_fn, self._grad_fn, self._apply_fn = (("dm_learn_disc_step", "dm_learn_disc_grad", "dm_learn_disc_apply") if kind == "disc" else
+                                                        ("dm_learn_step", "dm_learn_grad", "dm_learn_apply"))
         self.acc, self.device = acc, device
         ins, outs = [l.weight.shape[1] for l in self.layers], [l.weight.shape[0] for l in self.layers]
         L = lib()
@@ -764,12 +765,9 @@ class TensorCoreLearner:
         self._bind()
         _call(self._SET, self.h, C.byref(self.net), stream=stream)
 
-    def _step_fn(self):
-        return "dm_learn_disc_step" if self.kind == "disc" else "dm_learn_step"
-
     def step(self, batch, stream=None):
         """batch: a DmLearnBatch (kinds "actor", "critic"), a DmLearnDiscBatch (kind "disc") or a DmLearnGatedBatch (TensorCoreGatedLearner)"""
-        _call(self._step_fn(), self.h, C.byref(self.net), C.byref(batch), stream=stream)
+        _call(self._step_fn, self.h, C.byref(self.net), C.byref(batch), stream=stream)
 
     # ---- the step split around its gradient (data-parallel training): step(b) == grad(b, g); apply(b, g, 1.0), bit for bit
     def grad_size(self):
@@ -794,14 +792,13 @@ class TensorCoreLearner:
         batch's rows without the weight decay (and logit regulariser) into `grad`, a contiguous float32 CUDA tensor of grad_size() floats;
         the parameters are not changed"""
         self._check_grad(grad, "grad")
-        _call(self._step_fn().replace("_step", "_grad"), self.h, C.byref(self.net), C.byref(batch), C.c_void_p(grad.data_ptr()), stream=stream)
+        _call(self._grad_fn, self.h, C.byref(self.net), C.byref(batch), C.c_void_p(grad.data_ptr()), stream=stream)
 
     def apply(self, batch, grad, scale=1.0, stream=None):
         """dm_learn_(gated_|disc_)apply: the optimiser step on scale * grad plus the weight decay (and logit regulariser) with the batch's
         stepsize and momentum, and the re-tiling"""
         self._check_grad(grad, "apply")
-        _call(self._step_fn().replace("_step", "_apply"), self.h, C.byref(self.net), C.byref(batch), C.c_void_p(grad.data_ptr()),
-              C.c_float(scale), stream=stream)
+        _call(self._apply_fn, self.h, C.byref(self.net), C.byref(batch), C.c_void_p(grad.data_ptr()), C.c_float(scale), stream=stream)
 
     def close(self):
         if self.h:
@@ -821,6 +818,12 @@ def gated_layers(net, head):
     return (list(net.hidden) + [head, net.gate_common] + list(net.gate_hidden) + list(net.gate_scale) + list(net.gate_bias))
 
 
+def tc_layers(net, role):
+    """the layers the tensor-core entries take for `net` in `role`: the hidden layers and the head (actor: mean, critic: out, disc: logit), or gated_layers()"""
+    head = getattr(net, dict(actor="mean", critic="out", disc="logit")[role])
+    return gated_layers(net, head) if hasattr(net, "gate_common") else list(net.hidden) + [head]
+
+
 def _gated_shapes(S, G, h0, h1, A, GC, GH):
     """the [out, in] weight shapes of gated_layers() for state size S, goal size G, hidden (h0, h1), A outputs and gate sizes GC, GH"""
     return [(h0, S + G), (h1, h0), (A, h1), (GC, G), (GH, GC), (GH, GC), (h0, GH), (h1, GH), (h0, GH), (h1, GH)]
@@ -832,7 +835,7 @@ class TensorCoreGatedLearner(TensorCoreLearner):
     accumulators; the ten parameter pairs of gated_layers()).  The sizes dm_mlp_create_gated accepts: two hidden layers, goal size <= 64,
     gate_common <= 128, gate_hidden <= 64, at most 64 outputs."""
     KINDS = dict(actor=0, critic=1)
-    _NET, _SET = DmLearnGatedNet, "dm_learn_set_gated_weights"
+    _NET, _SET, _step_fn, _grad_fn, _apply_fn = DmLearnGatedNet, "dm_learn_set_gated_weights", "dm_learn_gated_step", "dm_learn_gated_grad", "dm_learn_gated_apply"
 
     def __init__(self, net, acc, kind, max_rows, device=0):
         if kind not in self.KINDS:
@@ -841,8 +844,7 @@ class TensorCoreGatedLearner(TensorCoreLearner):
         if not G or not hasattr(net, "gate_common") or len(net.hidden) != 2 or len(net.gate_hidden) != 2:
             raise ValueError("the gated tensor-core learner implements the gated network with exactly two hidden layers (plain networks: "
                              "TensorCoreLearner)")
-        self.kind = kind
-        self.layers = gated_layers(net, net.mean if kind == "actor" else net.out)
+        self.layers = tc_layers(net, kind)
         h0, h1, A = (l.weight.shape[0] for l in self.layers[:3])
         S = self.layers[0].weight.shape[1] - G
         GC, GH = net.gate_common.weight.shape[0], net.gate_hidden[0].weight.shape[0]
@@ -860,6 +862,3 @@ class TensorCoreGatedLearner(TensorCoreLearner):
         self.h = C.c_void_p(self.h)
         self.net = None
         self._bind()
-
-    def _step_fn(self):
-        return "dm_learn_gated_step"

@@ -5,6 +5,8 @@
 // step (dm_learn_*: kernels/dm_learn.cu and the backward GEMMs of kernels/dm_mlp.cu, 15 launches; 32 for the gated networks,
 // dm_learn_gated_step), the same step split around a flat gradient for data-parallel training (dm_learn_*grad, dm_learn_*apply), with the
 // device-side re-tiling of plain and gated handles (dm_mlp_set_weights_device, dm_mlp_set_gated_weights_device).
+// Every dm_learn_* step, grad, apply and set-weights entry is one call of `learn`, the checks, forward, backward and layer pass of its
+// network family; every device buffer of a dm_mlp or dm_learn handle is allocated by `alloc` or `upload`, which record it for destroy.
 // The parameter structs and kernel declarations are kernels/dm_mlp.cuh, shared with the kernels.
 // Same library, same rules: no CPU fallback, errors through dm_last_error.
 #include <cuda_fp16.h>
@@ -14,7 +16,9 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <iterator>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/deepmimic_b200.h"
@@ -36,6 +40,7 @@ struct dm_mlp {
     __half *wgc = nullptr, *wgh = nullptr, *wgs[2] = {nullptr, nullptr}, *wgb[2] = {nullptr, nullptr}, *goal_t = nullptr, *gc_t = nullptr, *gh_t = nullptr;
     float *bgc = nullptr, *bgh = nullptr, *bgs[2] = {nullptr, nullptr}, *bgb[2] = {nullptr, nullptr}, *g_mean = nullptr, *g_istd = nullptr;
     float g_clip = 1e30f;
+    std::vector<void*> bufs;   // every device buffer the handle owns (alloc, upload), freed by dm_mlp_destroy
 };
 
 namespace {
@@ -67,10 +72,17 @@ std::vector<__half> tile_weights(const float* w, int k_in, int n_out, int K, int
         }
     return out;
 }
-template <class T>
-bool upload(T** dst, const std::vector<T>& src) {
-    if (cudaMalloc(dst, src.size() * sizeof(T)) != cudaSuccess) return false;
-    return cudaMemcpy(*dst, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice) == cudaSuccess;
+// a device buffer of `count` T (zeroed: cleared there) that handle h owns until its destroy function
+template <class H, class T>
+bool alloc(H* h, T** p, size_t count, bool zeroed = false) {
+    if (cudaMalloc(p, count * sizeof(T)) != cudaSuccess) return false;
+    h->bufs.push_back(*p);
+    return !zeroed || cudaMemset(*p, 0, count * sizeof(T)) == cudaSuccess;
+}
+// a device buffer that handle h owns, holding a copy of src
+template <class H, class T>
+bool upload(H* h, T** dst, const std::vector<T>& src) {
+    return alloc(h, dst, src.size()) && cudaMemcpy(*dst, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice) == cudaSuccess;
 }
 std::vector<float> padded(const float* v, int n, int N, float fill = 0.f) { std::vector<float> o(N, fill); if (v) std::memcpy(o.data(), v, sizeof(float) * n); return o; }
 std::vector<float> inverse_std(const float* std_dev, int n) { std::vector<float> o(n, 1.f); for (int i = 0; i < n; ++i) o[i] = std_dev ? 1.0f / std_dev[i] : 1.f; return o; }
@@ -205,6 +217,7 @@ struct dm_learn {
     __half* st_a = nullptr;                                  // [ds_0 | dt_0 | ds_1 | dt_1] as hi + lo A of the dg GEMM
     __half* wst = nullptr;                                   // its B: Ws_l^T, Wt_l^T block-diagonal (layer l in columns [64 l, 64 l + GH))
     __half *dg_a = nullptr, *wght = nullptr;                 // [dg_0 | dg_1] as hi + lo A of the dgc GEMM, and its B: [Wgh_0 | Wgh_1]^T
+    std::vector<void*> bufs;                                 // every device buffer of the workspace (alloc), freed by dm_learn_destroy
 };
 
 namespace {
@@ -239,23 +252,22 @@ dm_mlp* create_gated(const char* fn, int device, const dm_mlp_gated_weights* g, 
         for (int n = 0; n < GH; ++n) bgh[64 * l + n] = g->gh_b[l][n];
     }
     const size_t R = m->max_rows;
-    bool ok = upload(&m->w[0], tile_weights(g->w0, trunk_in, g->h0, m->K0, m->N0, 64)) && upload(&m->w[1], tile_weights(g->w1, g->h0, g->h1, m->N0, m->N1, 64)) &&
-              upload(&m->w[2], tile_weights(g->w2, g->h1, g->out_dim, m->N1, m->N2, m->N2)) && upload(&m->b[0], padded(g->b0, g->h0, m->N0)) &&
-              upload(&m->b[1], padded(g->b1, g->h1, m->N1)) && upload(&m->b[2], padded(g->b2, g->out_dim, m->N2)) &&
-              upload(&m->wgc, tile_weights(g->gc_w, g->goal_dim, GC, 64, 128, 128)) && upload(&m->bgc, padded(g->gc_b, GC, 128)) &&
-              upload(&m->wgh, tile_weights(wgh.data(), GC, 128, 128, 128, 128)) && upload(&m->bgh, bgh);
+    bool ok = upload(m, &m->w[0], tile_weights(g->w0, trunk_in, g->h0, m->K0, m->N0, 64)) && upload(m, &m->w[1], tile_weights(g->w1, g->h0, g->h1, m->N0, m->N1, 64)) &&
+              upload(m, &m->w[2], tile_weights(g->w2, g->h1, g->out_dim, m->N1, m->N2, m->N2)) && upload(m, &m->b[0], padded(g->b0, g->h0, m->N0)) &&
+              upload(m, &m->b[1], padded(g->b1, g->h1, m->N1)) && upload(m, &m->b[2], padded(g->b2, g->out_dim, m->N2)) &&
+              upload(m, &m->wgc, tile_weights(g->gc_w, g->goal_dim, GC, 64, 128, 128)) && upload(m, &m->bgc, padded(g->gc_b, GC, 128)) &&
+              upload(m, &m->wgh, tile_weights(wgh.data(), GC, 128, 128, 128, 128)) && upload(m, &m->bgh, bgh);
     const int hl[2] = {g->h0, g->h1}, Nl[2] = {m->N0, m->N1};
     for (int l = 0; l < 2 && ok; ++l)
-        ok = upload(&m->wgs[l], tile_weights(g->gs_w[l], GH, hl[l], 64, Nl[l], 64)) && upload(&m->bgs[l], padded(g->gs_b[l], hl[l], Nl[l])) &&
-             upload(&m->wgb[l], tile_weights(g->gb_w[l], GH, hl[l], 64, Nl[l], 64)) && upload(&m->bgb[l], padded(g->gb_b[l], hl[l], Nl[l]));
+        ok = upload(m, &m->wgs[l], tile_weights(g->gs_w[l], GH, hl[l], 64, Nl[l], 64)) && upload(m, &m->bgs[l], padded(g->gs_b[l], hl[l], Nl[l])) &&
+             upload(m, &m->wgb[l], tile_weights(g->gb_w[l], GH, hl[l], 64, Nl[l], 64)) && upload(m, &m->bgb[l], padded(g->gb_b[l], hl[l], Nl[l]));
     // gh_t has one tile more than its rows need: the learner transposes layer 1's gate (chunk 1 of every m tile) as a two-chunk source, which
     // also reads the chunk after it (learn_gated_forward)
-    ok = ok && upload(&m->in_mean, padded(g->s_mean, g->in_dim, g->in_dim)) && upload(&m->in_istd, inverse_std(g->s_std, g->in_dim)) &&
-         upload(&m->g_mean, padded(g->g_mean, g->goal_dim, g->goal_dim)) && upload(&m->g_istd, inverse_std(g->g_std, g->goal_dim)) &&
-         upload(&m->out_mean, padded(g->a_mean, g->out_dim, g->out_dim)) && upload(&m->out_std, padded(g->a_std, g->out_dim, g->out_dim, 1.f)) &&
-         cudaMalloc(&m->obs_t, R * m->K0 * sizeof(__half)) == cudaSuccess && cudaMalloc(&m->goal_t, R * 64 * sizeof(__half)) == cudaSuccess &&
-         cudaMalloc(&m->gc_t, R * 128 * sizeof(__half)) == cudaSuccess && cudaMalloc(&m->gh_t, (R * 128 + dmk::kMlpATile) * sizeof(__half)) == cudaSuccess &&
-         cudaMalloc(&m->act0, R * m->N0 * sizeof(__half)) == cudaSuccess && cudaMalloc(&m->act1, R * m->N1 * sizeof(__half)) == cudaSuccess;
+    ok = ok && upload(m, &m->in_mean, padded(g->s_mean, g->in_dim, g->in_dim)) && upload(m, &m->in_istd, inverse_std(g->s_std, g->in_dim)) &&
+         upload(m, &m->g_mean, padded(g->g_mean, g->goal_dim, g->goal_dim)) && upload(m, &m->g_istd, inverse_std(g->g_std, g->goal_dim)) &&
+         upload(m, &m->out_mean, padded(g->a_mean, g->out_dim, g->out_dim)) && upload(m, &m->out_std, padded(g->a_std, g->out_dim, g->out_dim, 1.f)) &&
+         alloc(m, &m->obs_t, R * m->K0) && alloc(m, &m->goal_t, R * 64) && alloc(m, &m->gc_t, R * 128) && alloc(m, &m->gh_t, R * 128 + dmk::kMlpATile) &&
+         alloc(m, &m->act0, R * m->N0) && alloc(m, &m->act1, R * m->N1);
     if (ok) {
         ok = cudaFuncSetAttribute(dmk::dm_mlp_gemm_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
              cudaFuncSetAttribute(dmk::dm_mlp_gated_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess &&
@@ -303,19 +315,16 @@ int trunk_bn(const dm_learn* l, int i) { return i == 2 ? l->m->N2 : 128; }
 // the largest split count a step may take); and the backward kernels' shared-memory opt-in.  l->m and l->max_rows are set
 bool trunk_workspace(dm_learn* l, const int* in) {
     const dm_mlp* m = l->m;
-    const size_t R = l->max_rows, h = sizeof(__half);
+    const size_t R = l->max_rows;
     l->Nout[0] = m->N0; l->Nout[1] = m->N1; l->Nout[2] = m->N2;
-    bool ok = cudaMalloc(&l->out, R * m->out_dim * sizeof(float)) == cudaSuccess && cudaMalloc(&l->head_partials, R / 128 * 3 * sizeof(float)) == cudaSuccess;
+    bool ok = alloc(l, &l->out, R * m->out_dim) && alloc(l, &l->head_partials, R / 128 * 3);
     for (int i = 0; i < 3 && ok; ++i) {
         l->F[i] = pad_to(in[i] + 1, 128);
         l->max_splits[i] = dw_max_splits(l->F[i], l->Nout[i], trunk_bn(l, i), l->max_rows / 64);
-        ok = cudaMalloc(&l->xt[i], R * l->F[i] * h) == cudaSuccess && cudaMalloc(&l->dy_b[i], 2 * R * l->Nout[i] * h) == cudaSuccess &&
-             cudaMalloc(&l->partial[i], static_cast<size_t>(l->max_splits[i]) * l->Nout[i] * l->F[i] * sizeof(float)) == cudaSuccess;
+        ok = alloc(l, &l->xt[i], R * l->F[i]) && alloc(l, &l->dy_b[i], 2 * R * l->Nout[i]) &&
+             alloc(l, &l->partial[i], static_cast<size_t>(l->max_splits[i]) * l->Nout[i] * l->F[i]);
         // W_i^T as B of the dX GEMM: K = Nout[i], N = Nout[i - 1] (zero padding written once)
-        if (ok && i > 0) {
-            const size_t n = 2 * static_cast<size_t>(l->Nout[i]) * l->Nout[i - 1];
-            ok = cudaMalloc(&l->dy_a[i], 2 * R * l->Nout[i] * h) == cudaSuccess && cudaMalloc(&l->wt[i], n * h) == cudaSuccess && cudaMemset(l->wt[i], 0, n * h) == cudaSuccess;
-        }
+        if (ok && i > 0) ok = alloc(l, &l->dy_a[i], 2 * R * l->Nout[i]) && alloc(l, &l->wt[i], 2 * static_cast<size_t>(l->Nout[i]) * l->Nout[i - 1], true);
     }
     return ok && cudaFuncSetAttribute(dmk::dm_mlp_grad_x_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
            cudaFuncSetAttribute(dmk::dm_mlp_grad_w_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
@@ -333,13 +342,12 @@ dm_mlp* dm_mlp_create(int device, int in_dim, int h0, int h1, int out_dim, const
     m->device = device; m->in_dim = in_dim; m->h0 = h0; m->h1 = h1; m->out_dim = out_dim; m->max_rows = pad_to(max_rows, 128);
     m->K0 = pad_to(in_dim, 64); m->N0 = pad_to(h0, 128); m->N1 = pad_to(h1, 128);
     m->in_clip = in_clip > 0.f ? in_clip : 1e30f;
-    bool ok = upload(&m->w[0], tile_weights(w0, in_dim, h0, m->K0, m->N0, 128)) && upload(&m->w[1], tile_weights(w1, h0, h1, m->N0, m->N1, 128)) &&
-              upload(&m->w[2], tile_weights(w2, h1, out_dim, m->N1, m->N2, m->N2)) && upload(&m->b[0], padded(b0, h0, m->N0)) && upload(&m->b[1], padded(b1, h1, m->N1)) &&
-              upload(&m->b[2], padded(b2, out_dim, m->N2)) && upload(&m->in_mean, padded(in_mean, in_dim, in_dim)) && upload(&m->in_istd, inverse_std(in_std, in_dim)) &&
-              upload(&m->out_mean, padded(out_mean, out_dim, out_dim)) && upload(&m->out_std, padded(out_std, out_dim, out_dim, 1.f)) &&
-              cudaMalloc(&m->obs_t, static_cast<size_t>(m->max_rows) * m->K0 * sizeof(__half)) == cudaSuccess &&
-              cudaMalloc(&m->act0, static_cast<size_t>(m->max_rows) * m->N0 * sizeof(__half)) == cudaSuccess &&
-              cudaMalloc(&m->act1, static_cast<size_t>(m->max_rows) * m->N1 * sizeof(__half)) == cudaSuccess;
+    const size_t R = m->max_rows;
+    bool ok = upload(m, &m->w[0], tile_weights(w0, in_dim, h0, m->K0, m->N0, 128)) && upload(m, &m->w[1], tile_weights(w1, h0, h1, m->N0, m->N1, 128)) &&
+              upload(m, &m->w[2], tile_weights(w2, h1, out_dim, m->N1, m->N2, m->N2)) && upload(m, &m->b[0], padded(b0, h0, m->N0)) && upload(m, &m->b[1], padded(b1, h1, m->N1)) &&
+              upload(m, &m->b[2], padded(b2, out_dim, m->N2)) && upload(m, &m->in_mean, padded(in_mean, in_dim, in_dim)) && upload(m, &m->in_istd, inverse_std(in_std, in_dim)) &&
+              upload(m, &m->out_mean, padded(out_mean, out_dim, out_dim)) && upload(m, &m->out_std, padded(out_std, out_dim, out_dim, 1.f)) &&
+              alloc(m, &m->obs_t, R * m->K0) && alloc(m, &m->act0, R * m->N0) && alloc(m, &m->act1, R * m->N1);
     if (ok) {
         ok = cudaFuncSetAttribute(dmk::dm_mlp_gemm_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess &&
              cudaFuncSetAttribute(dmk::dm_mlp_gemm_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess;
@@ -472,33 +480,38 @@ dm_learn* dm_learn_create(int device, int kind, int in_dim, int h0, int h1, int 
         const int Ng = l->Ng, N0 = m->N0, N1 = m->N1;
         l->pen_F[0] = Ng; l->pen_F[1] = N0; l->pen_F[2] = N1;
         for (int i = 0; i < 3; ++i) l->pen_max_splits[i] = dw_max_splits(l->pen_F[i], l->Nout[i], trunk_bn(l, i), E / 64);
-        const size_t e = E, h = sizeof(__half), tw = 2 * static_cast<size_t>(N0) * Ng;   // halves of W0^T / W0 as hi + lo tiles
-        ok = cudaMalloc(&l->seed_a, 2 * e * 64 * h) == cudaSuccess && cudaMalloc(&l->seed_b, 2 * e * 64 * h) == cudaSuccess &&
-             cudaMalloc(&l->u_a[0], 2 * e * N0 * h) == cudaSuccess && cudaMalloc(&l->u_b[0], 2 * e * N0 * h) == cudaSuccess &&
-             cudaMalloc(&l->u_a[1], 2 * e * N1 * h) == cudaSuccess && cudaMalloc(&l->u_b[1], 2 * e * N1 * h) == cudaSuccess &&
-             cudaMalloc(&l->e_a, 2 * e * Ng * h) == cudaSuccess && cudaMalloc(&l->q_a[0], 2 * e * N0 * h) == cudaSuccess &&
-             cudaMalloc(&l->q_a[1], 2 * e * N1 * h) == cudaSuccess && cudaMalloc(&l->gp_partials, e / 128 * sizeof(float)) == cudaSuccess &&
-             cudaMalloc(&l->wt[0], tw * h) == cudaSuccess && cudaMemset(l->wt[0], 0, tw * h) == cudaSuccess &&
-             cudaMalloc(&l->w0p, tw * h) == cudaSuccess && cudaMemset(l->w0p, 0, tw * h) == cudaSuccess;
+        const size_t e = E, tw = 2 * static_cast<size_t>(N0) * Ng;   // halves of W0^T / W0 as hi + lo tiles
+        ok = alloc(l, &l->seed_a, 2 * e * 64) && alloc(l, &l->seed_b, 2 * e * 64) && alloc(l, &l->u_a[0], 2 * e * N0) && alloc(l, &l->u_b[0], 2 * e * N0) &&
+             alloc(l, &l->u_a[1], 2 * e * N1) && alloc(l, &l->u_b[1], 2 * e * N1) && alloc(l, &l->e_a, 2 * e * Ng) && alloc(l, &l->q_a[0], 2 * e * N0) &&
+             alloc(l, &l->q_a[1], 2 * e * N1) && alloc(l, &l->gp_partials, e / 128) && alloc(l, &l->wt[0], tw, true) && alloc(l, &l->w0p, tw, true);
         for (int i = 0; i < 3 && ok; ++i)
-            ok = cudaMalloc(&l->pt[i], e * l->pen_F[i] * h) == cudaSuccess &&
-                 cudaMalloc(&l->pen[i], static_cast<size_t>(l->pen_max_splits[i]) * l->Nout[i] * l->pen_F[i] * sizeof(float)) == cudaSuccess;
+            ok = alloc(l, &l->pt[i], e * l->pen_F[i]) && alloc(l, &l->pen[i], static_cast<size_t>(l->pen_max_splits[i]) * l->Nout[i] * l->pen_F[i]);
         ok = ok && cudaFuncSetAttribute(dmk::dm_mlp_grad_xa_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess;
     }
     if (!ok) { mlp_fail(std::string("dm_learn_create: ") + cudaGetErrorString(cudaGetLastError())); dm_learn_destroy(l); return nullptr; }
     return l;
 }
 
+}  // extern "C"
+
 namespace {
-int learn_net_check(const dm_learn_net* net, const char* fn) {
+// what a learner entry runs after its checks: the re-tiling alone (set-weights, no batch), the fused step (forward, backward, optimiser step
+// and re-tiling), or one half of the split step: the mean gradient packed into a flat buffer (grad), or the optimiser step on scale times
+// such a buffer (apply, no forward or backward)
+enum class Pass { retile, step, pack, apply };
+// the split counts of a step's dW GEMMs: the trunk's, the discriminator penalty's and the gate's.  A step's forward and backward fill them
+// and its layer pass reads them; a re-tiling or an apply reads no dW partials and leaves them zero
+struct Splits { int trunk[3] = {0, 0, 0}, pen[3] = {0, 0, 0}, gate[4] = {0, 0, 0, 0}; };
+// the parameter and accumulator pointers of a plain (3 pairs) or gated (10 pairs) network
+template <class Net>
+int net_check(const char* fn, const Net* net) {
     if (!net) return mlp_fail(std::string(fn) + ": null parameters");
-    for (int i = 0; i < 3; ++i)
+    for (size_t i = 0; i < std::size(net->w); ++i)
         if (!net->w[i] || !net->b[i] || !net->acc_w[i] || !net->acc_b[i]) return mlp_fail(std::string(fn) + ": null parameter or accumulator pointer");
     return 0;
 }
-// the checks of a PPO step's batch b (dm_learn_step, dm_learn_gated_step); the gated step also passes gb (b = &gb->batch), whose goal pointers
-// are checked with the states'
-int ppo_batch_check(const char* fn, const dm_learn* l, const dm_learn_batch* b, const dm_learn_gated_batch* gb) {
+// the checks of a PPO step's batch b; the gated step also passes gb (b = &gb->batch), whose goal pointers are checked with the states'
+int batch_check(const char* fn, const dm_learn* l, const dm_learn_batch* b, const dm_learn_gated_batch* gb = nullptr) {
     const std::string f(fn);
     const bool actor = l->kind == 0;
     if (!b) return mlp_fail(f + ": null batch");
@@ -512,6 +525,17 @@ int ppo_batch_check(const char* fn, const dm_learn* l, const dm_learn_batch* b, 
     if (!(b->stepsize >= 0.f) || !(b->momentum >= 0.f) || !(b->weight_decay >= 0.f)) return mlp_fail(f + ": stepsize, momentum and weight_decay must be >= 0");
     return 0;
 }
+int batch_check(const char* fn, const dm_learn* l, const dm_learn_gated_batch* gb) { return batch_check(fn, l, gb ? &gb->batch : nullptr, gb); }
+int batch_check(const char* fn, const dm_learn* l, const dm_learn_disc_batch* b) {
+    const std::string f(fn);
+    if (!b) return mlp_fail(f + ": null batch");
+    if (b->rows <= 0 || b->rows > l->side_rows) return mlp_fail(f + ": rows out of range (1 to max_rows / 2 per side)");
+    if (!b->agent || !b->expert || !b->agent_idx || !b->expert_idx || !b->in_mean || !b->in_istd || !b->stats)
+        return mlp_fail(f + ": null observation, index, normaliser or statistics pointer");
+    if (!(b->stepsize >= 0.f) || !(b->momentum >= 0.f) || !(b->weight_decay >= 0.f) || !(b->logit_reg_weight >= 0.f) || !(b->grad_penalty_weight >= 0.f))
+        return mlp_fail(f + ": stepsize, momentum, weight_decay, logit_reg_weight and grad_penalty_weight must be >= 0");
+    return 0;
+}
 // a PPO step's loss head over the mt m tiles of l->out (dY of the output layer, the loss partials) and its statistics
 void launch_ppo_head(const dm_learn* l, const dm_learn_batch* b, int mt, cudaStream_t st) {
     const bool actor = l->kind == 0;
@@ -521,11 +545,8 @@ void launch_ppo_head(const dm_learn* l, const dm_learn_batch* b, int mt, cudaStr
     else dmk::dm_learn_critic_head_kernel<<<mt, 128, 0, st>>>(H);
     dmk::dm_learn_stats_kernel<<<1, 1, 0, st>>>(l->head_partials, mt, 1.f / b->rows, actor ? 1 : 0, b->stats);
 }
-// what a layer pass does with a step's dW partials: the fused optimiser step (or, without a batch, the re-tiling alone), or one half of the
-// split step: the mean gradient packed into a flat buffer (dm_learn_*grad), or the optimiser step on scale times such a buffer (dm_learn_*apply)
-enum class Pass { step, pack, apply };
-// the pass of one parameter pair (kind 2: the discriminator's layer kernel for the fused step); its slice of the flat gradient `grad` starts
-// at *off (weights, then the bias), and *off moves past it
+// the pass of one parameter pair (disc: the discriminator's layer kernel for the re-tiling and the fused step); its slice of the flat gradient
+// `grad` starts at *off (weights, then the bias), and *off moves past it
 void launch_pass(Pass pass, const dmk::LearnDiscLayerParams& D, bool disc, float* grad, float scale, size_t* off, cudaStream_t st) {
     const dim3 grid((D.L.in_dim + 1 + 255) / 256, D.L.out_dim);
     const size_t nw = static_cast<size_t>(D.L.out_dim) * D.L.in_dim;
@@ -536,39 +557,26 @@ void launch_pass(Pass pass, const dmk::LearnDiscLayerParams& D, bool disc, float
     else if (disc) dmk::dm_learn_disc_layer_kernel<<<grid, 256, 0, st>>>(D);
     else launch_layer(D.L, st);
 }
-// the forward tiles of the learner's handle and the transposed tiles of the dX GEMMs; with `b` also the optimiser step before the re-tiling
-// (or the split step's pass: pack, apply on the flat gradient `grad`)
-void learn_layers(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, const int* splits, cudaStream_t st, Pass pass = Pass::step,
-                  float* grad = nullptr, float scale = 1.f) {
-    size_t off = 0;
-    for (int i = 0; i < 3; ++i) {
-        dmk::LearnDiscLayerParams D{};
-        dmk::LearnLayerParams& L = D.L;
-        L = layer_params(l->m, i, net->w[i], net->b[i]);
-        if (i > 0) { L.t_tiles = l->wt[i]; L.t_NC = l->Nout[i] / 64; }
-        if (b) {
-            L.partial = l->partial[i]; L.Npad = l->Nout[i]; L.F = l->F[i];
-            optimiser_fields(L, net, i, b, splits[i]);
-        }
-        launch_pass(pass, D, false, grad, scale, &off, st);
-    }
-}
-// the discriminator's layer passes (kind 2): W0^T and W0's K-padded tiles for the penalty as well; with `b` also the optimiser step with the
-// penalty's partials (psplits of them) and the logit regulariser (or the split step's pass, as learn_layers)
-void learn_disc_layers(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* b, const int* splits, const int* psplits, cudaStream_t st,
-                       Pass pass = Pass::step, float* grad = nullptr, float scale = 1.f) {
+// the layer passes of a plain workspace: the forward tiles of the learner's handle and the transposed tiles of the dX GEMMs (kind 2: also W0^T
+// and W0's K-padded tiles for the penalty); with a batch `b` also the optimiser step on the dW partials (kind 2: with the penalty's partials
+// and the logit regulariser), or the split step's pass: pack, apply on the flat gradient `grad`
+template <class Batch>
+void learn_layers(dm_learn* l, const dm_learn_net* net, const Batch* b, const Splits& s, Pass pass, float* grad, float scale, cudaStream_t st) {
+    const bool disc = l->kind == 2;
     size_t off = 0;
     for (int i = 0; i < 3; ++i) {
         dmk::LearnDiscLayerParams D{};
         D.L = layer_params(l->m, i, net->w[i], net->b[i]);
-        D.L.t_tiles = l->wt[i]; D.L.t_NC = l->Nout[i] / 64;
-        if (i == 0) { D.p_tiles = l->w0p; D.p_NC = l->Ng / 64; }
+        if (i > 0 || disc) { D.L.t_tiles = l->wt[i]; D.L.t_NC = l->Nout[i] / 64; }
+        if (i == 0 && disc) { D.p_tiles = l->w0p; D.p_NC = l->Ng / 64; }
         if (b) {
             D.L.partial = l->partial[i]; D.L.Npad = l->Nout[i]; D.L.F = l->F[i];
-            optimiser_fields(D.L, net, i, b, splits[i]);
-            D.pen = l->pen[i]; D.pen_splits = psplits[i]; D.pen_F = l->pen_F[i]; D.gp_w = b->grad_penalty_weight; D.reg = i == 2 ? b->logit_reg_weight : 0.f;
+            optimiser_fields(D.L, net, i, b, s.trunk[i]);
+            if constexpr (std::is_same_v<Batch, dm_learn_disc_batch>) {
+                D.pen = l->pen[i]; D.pen_splits = s.pen[i]; D.pen_F = l->pen_F[i]; D.gp_w = b->grad_penalty_weight; D.reg = i == 2 ? b->logit_reg_weight : 0.f;
+            }
         }
-        launch_pass(pass, D, true, grad, scale, &off, st);
+        launch_pass(pass, D, disc, grad, scale, &off, st);
     }
 }
 // the forward over the mt m tiles prepared in the handle's obs_t (the output layer writes `rows` rows of l->out) and the transposition of the
@@ -597,167 +605,34 @@ void learn_backward(dm_learn* l, int rows, int mt, const int* splits, const int*
         dmk::dm_mlp_grad_x_kernel<<<dim3(mt, l->Nout[i - 1] / 128), 256, dmk::dm_mlp_smem_bytes(128), st>>>(X, GX);
     }
 }
-}  // namespace
-
-int dm_learn_set_weights(dm_learn* l, const dm_learn_net* net, void* stream) {
-    if (!l) return mlp_fail("dm_learn_set_weights: null handle");
-    if (l->gated) return mlp_fail("dm_learn_set_weights: the workspace holds a gated network (dm_learn_create_gated); use dm_learn_set_gated_weights");
-    if (learn_net_check(net, "dm_learn_set_weights")) return 1;
-    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_set_weights: cudaSetDevice failed");
-    if (l->kind == 2) learn_disc_layers(l, net, nullptr, nullptr, nullptr, static_cast<cudaStream_t>(stream));
-    else learn_layers(l, net, nullptr, nullptr, static_cast<cudaStream_t>(stream));
-    return launch_status("dm_learn_set_weights");
-}
-
-namespace {
-// the checks of the split step's calls on workspace l: `gated` names the gated entries, `disc` the discriminator's; fn names the caller
-int split_kind_check(const char* fn, const dm_learn* l, bool gated, bool disc) {
-    const std::string f(fn);
-    if (!l) return mlp_fail(f + ": null handle");
-    if (gated && !l->gated) return mlp_fail(f + ": the workspace holds a plain network (dm_learn_create)");
-    if (!gated && l->gated) return mlp_fail(f + ": the workspace holds a gated network (dm_learn_create_gated)");
-    if (disc && l->kind != 2) return mlp_fail(f + ": the workspace is a PPO actor's or critic's (kind 0 or 1); the discriminator's entries need kind 2");
-    if (!disc && l->kind == 2) return mlp_fail(f + ": the workspace is a discriminator's (kind 2)");
-    return 0;
-}
-// the split counts of an apply: it reads no dW partials
-constexpr int kNoSplits[4] = {0, 0, 0, 0};
-// the optimiser fields an apply reads
-int apply_check(const char* fn, const void* b, const float* d_grad, float scale, float stepsize, float momentum, float weight_decay, float reg) {
-    const std::string f(fn);
-    if (!b) return mlp_fail(f + ": null batch");
-    if (!d_grad) return mlp_fail(f + ": null gradient pointer");
-    if (!std::isfinite(scale)) return mlp_fail(f + ": scale must be finite");
-    if (!(stepsize >= 0.f) || !(momentum >= 0.f) || !(weight_decay >= 0.f) || !(reg >= 0.f))
-        return mlp_fail(f + ": stepsize, momentum, weight_decay (and logit_reg_weight) must be >= 0");
-    return 0;
-}
-// a PPO step up to its layer pass: the split-K plan of the three dW GEMMs (splits), the forward, the loss head with its statistics and the
+// a PPO step up to its layer pass: the split-K plan of the three dW GEMMs (s.trunk), the forward, the loss head with its statistics and the
 // backward
-int ppo_forward_backward(dm_learn* l, const dm_learn_batch* b, const char* fn, int* splits, cudaStream_t st) {
+int forward_backward(const char* fn, dm_learn* l, const dm_learn_batch* b, Splits& s, cudaStream_t st) {
     dm_mlp* m = l->m;
     const int rows = b->rows, mt = (rows + 127) / 128, chunks = 2 * mt;
     // split-K of the three dW GEMMs for this row count (the workspace holds the largest over every row count, dm_learn_create)
     int cps[3];
     for (int i = 0; i < 3; ++i)
-        if (dw_plan(fn, l->F[i], l->Nout[i], trunk_bn(l, i), chunks, l->max_splits[i], &splits[i], &cps[i])) return 1;
+        if (dw_plan(fn, l->F[i], l->Nout[i], trunk_bn(l, i), chunks, l->max_splits[i], &s.trunk[i], &cps[i])) return 1;
     // forward: gathered rows -> the plain trunk -> the normalised output (identity output normaliser)
     dmk::LearnPrepParams Q{b->states, b->idx, b->in_mean, b->in_istd, b->in_clip > 0.f ? b->in_clip : 1e30f, m->in_dim, rows, m->K0 / 64, m->obs_t};
     dmk::dm_learn_prep_kernel<<<dim3(mt, m->K0 / 64), 128, 0, st>>>(Q);
     learn_forward(l, rows, mt, st);
     // loss head: dY of the output layer, the loss partials, the statistics
     launch_ppo_head(l, b, mt, st);
-    learn_backward(l, rows, mt, splits, cps, st);
+    learn_backward(l, rows, mt, s.trunk, cps, st);
     return 0;
 }
-int disc_batch_check(const char* fn, const dm_learn* l, const dm_learn_disc_batch* b) {
-    const std::string f(fn);
-    if (!b) return mlp_fail(f + ": null batch");
-    if (b->rows <= 0 || b->rows > l->side_rows) return mlp_fail(f + ": rows out of range (1 to max_rows / 2 per side)");
-    if (!b->agent || !b->expert || !b->agent_idx || !b->expert_idx || !b->in_mean || !b->in_istd || !b->stats)
-        return mlp_fail(f + ": null observation, index, normaliser or statistics pointer");
-    if (!(b->stepsize >= 0.f) || !(b->momentum >= 0.f) || !(b->weight_decay >= 0.f) || !(b->logit_reg_weight >= 0.f) || !(b->grad_penalty_weight >= 0.f))
-        return mlp_fail(f + ": stepsize, momentum, weight_decay, logit_reg_weight and grad_penalty_weight must be >= 0");
-    return 0;
-}
-int disc_forward_backward(dm_learn* l, const dm_learn_disc_batch* b, const char* fn, int* splits, int* psplits, cudaStream_t st);
-}  // namespace
-
-int dm_learn_step(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, void* stream) {
-    const char* fn = "dm_learn_step";
-    if (!l) return mlp_fail("dm_learn_step: null handle");
-    if (l->gated) return mlp_fail("dm_learn_step: the workspace holds a gated network (dm_learn_create_gated); use dm_learn_gated_step");
-    if (l->kind == 2) return mlp_fail("dm_learn_step: the workspace is a discriminator's (kind 2); use dm_learn_disc_step");
-    if (learn_net_check(net, fn) || ppo_batch_check(fn, l, b, nullptr)) return 1;
-    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_step: cudaSetDevice failed");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    int splits[3];
-    if (ppo_forward_backward(l, b, fn, splits, st)) return 1;
-    // optimiser step and re-tiling, after every GEMM that read the old weights
-    learn_layers(l, net, b, splits, st);
-    return launch_status(fn);
-}
-
-long long dm_learn_grad_size(const dm_learn* l) {
-    if (!l) { mlp_fail("dm_learn_grad_size: null handle"); return -1; }
-    long long n = 0;
-    for (int i = 0; i < (l->gated ? 10 : 3); ++i) {
-        const dmk::LearnLayerParams L = l->gated ? gated_layer_params(l->m, i, nullptr, nullptr) : layer_params(l->m, i, nullptr, nullptr);
-        n += static_cast<long long>(L.out_dim) * (L.in_dim + 1);
-    }
-    return n;
-}
-
-int dm_learn_grad(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, float* d_grad, void* stream) {
-    const char* fn = "dm_learn_grad";
-    if (split_kind_check(fn, l, false, false) || learn_net_check(net, fn) || ppo_batch_check(fn, l, b, nullptr)) return 1;
-    if (!d_grad) return mlp_fail("dm_learn_grad: null gradient pointer");
-    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_grad: cudaSetDevice failed");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    int splits[3];
-    if (ppo_forward_backward(l, b, fn, splits, st)) return 1;
-    learn_layers(l, net, b, splits, st, Pass::pack, d_grad);
-    return launch_status(fn);
-}
-
-int dm_learn_apply(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, const float* d_grad, float scale, void* stream) {
-    const char* fn = "dm_learn_apply";
-    if (split_kind_check(fn, l, false, false) || learn_net_check(net, fn)) return 1;
-    if (apply_check(fn, b, d_grad, scale, b ? b->stepsize : 0.f, b ? b->momentum : 0.f, b ? b->weight_decay : 0.f, 0.f)) return 1;
-    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_apply: cudaSetDevice failed");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    learn_layers(l, net, b, kNoSplits, st, Pass::apply, const_cast<float*>(d_grad), scale);
-    return launch_status(fn);
-}
-
-int dm_learn_disc_grad(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* b, float* d_grad, void* stream) {
-    const char* fn = "dm_learn_disc_grad";
-    if (split_kind_check(fn, l, false, true) || learn_net_check(net, fn) || disc_batch_check(fn, l, b)) return 1;
-    if (!d_grad) return mlp_fail("dm_learn_disc_grad: null gradient pointer");
-    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_disc_grad: cudaSetDevice failed");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    int splits[3], psplits[3];
-    if (disc_forward_backward(l, b, fn, splits, psplits, st)) return 1;
-    learn_disc_layers(l, net, b, splits, psplits, st, Pass::pack, d_grad);
-    return launch_status(fn);
-}
-
-int dm_learn_disc_apply(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* b, const float* d_grad, float scale, void* stream) {
-    const char* fn = "dm_learn_disc_apply";
-    if (split_kind_check(fn, l, false, true) || learn_net_check(net, fn)) return 1;
-    if (apply_check(fn, b, d_grad, scale, b ? b->stepsize : 0.f, b ? b->momentum : 0.f, b ? b->weight_decay : 0.f, b ? b->logit_reg_weight : 0.f)) return 1;
-    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_disc_apply: cudaSetDevice failed");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    learn_disc_layers(l, net, b, kNoSplits, kNoSplits, st, Pass::apply, const_cast<float*>(d_grad), scale);
-    return launch_status(fn);
-}
-
-int dm_learn_disc_step(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* b, void* stream) {
-    const char* fn = "dm_learn_disc_step";
-    if (!l) return mlp_fail("dm_learn_disc_step: null handle");
-    if (l->gated) return mlp_fail("dm_learn_disc_step: the workspace holds a gated network (dm_learn_create_gated); a discriminator step needs kind 2");
-    if (l->kind != 2) return mlp_fail("dm_learn_disc_step: the workspace is a PPO actor's or critic's (kind 0 or 1); a discriminator step needs kind 2");
-    if (learn_net_check(net, fn) || disc_batch_check(fn, l, b)) return 1;
-    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_disc_step: cudaSetDevice failed");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    int splits[3], psplits[3];
-    if (disc_forward_backward(l, b, fn, splits, psplits, st)) return 1;
-    // optimiser step and re-tiling, after every GEMM that read the old weights
-    learn_disc_layers(l, net, b, splits, psplits, st);
-    return launch_status(fn);
-}
-
-namespace {
-// a discriminator step up to its layer pass: the split-K plans of the dW GEMMs (splits) and of the penalty's (psplits), the forward over both
+// a discriminator step up to its layer pass: the split-K plans of the dW GEMMs (s.trunk) and of the penalty's (s.pen), the forward over both
 // sides, the least-squares head, the backward, the gradient penalty's GEMMs and the statistics
-int disc_forward_backward(dm_learn* l, const dm_learn_disc_batch* b, const char* fn, int* splits, int* psplits, cudaStream_t st) {
+int forward_backward(const char* fn, dm_learn* l, const dm_learn_disc_batch* b, Splits& s, cudaStream_t st) {
     dm_mlp* m = l->m;
     // agent rows in m tiles [0, et), expert rows in [et, 2 et)
     const int rows = b->rows, E = pad_to(rows, 128), et = E / 128, mt = 2 * et, chunks = 2 * mt, echunks = 2 * et;
     int cps[3], pcps[3];
     for (int i = 0; i < 3; ++i)
-        if (dw_plan(fn, l->F[i], l->Nout[i], trunk_bn(l, i), chunks, l->max_splits[i], &splits[i], &cps[i]) ||
-            dw_plan(fn, l->pen_F[i], l->Nout[i], trunk_bn(l, i), echunks, l->pen_max_splits[i], &psplits[i], &pcps[i]))
+        if (dw_plan(fn, l->F[i], l->Nout[i], trunk_bn(l, i), chunks, l->max_splits[i], &s.trunk[i], &cps[i]) ||
+            dw_plan(fn, l->pen_F[i], l->Nout[i], trunk_bn(l, i), echunks, l->pen_max_splits[i], &s.pen[i], &pcps[i]))
             return 1;
     // forward over both sides: each gathered into its own m tiles
     const int NC0 = m->K0 / 64;
@@ -769,7 +644,7 @@ int disc_forward_backward(dm_learn* l, const dm_learn_disc_batch* b, const char*
     // least-squares head: dY of the logit over both sides, the penalty's seed over the expert rows, the partials
     const dmk::LearnDiscHeadParams H{l->out, rows, E, l->dy_a[2], l->dy_b[2], l->seed_a, l->seed_b, l->head_partials};
     dmk::dm_learn_disc_head_kernel<<<mt, 128, 0, st>>>(H);
-    learn_backward(l, 2 * E, mt, splits, cps, st);
+    learn_backward(l, 2 * E, mt, s.trunk, cps, st);
     // the gradient penalty on the expert tiles, with the forward's masks: u1 = m1 w2, u0 = m0 (W1^T u1) (hi + lo A and B operands) ...
     const size_t tile = dmk::kMlpATile;
     const __half* act0e = m->act0 + static_cast<size_t>(et) * (m->N0 / 64) * tile;
@@ -794,11 +669,23 @@ int disc_forward_backward(dm_learn* l, const dm_learn_disc_batch* b, const char*
                                       {-1, -1, -1}, {l->pen_F[0], l->pen_F[1], l->pen_F[2]}, echunks};
     dmk::dm_learn_transpose_kernel<<<dim3(std::max(l->pen_F[0], std::max(l->pen_F[1], l->pen_F[2])) / 128, echunks, 3), 256, 0, st>>>(T);
     const __half* pen_b[3] = {l->u_b[0], l->u_b[1], l->seed_b};
-    for (int i = 0; i < 3; ++i) launch_dw(l->pt[i], pen_b[i], l->pen[i], l->pen_F[i], l->Nout[i], trunk_bn(l, i), echunks, psplits[i], pcps[i], st);
+    for (int i = 0; i < 3; ++i) launch_dw(l->pt[i], pen_b[i], l->pen[i], l->pen_F[i], l->Nout[i], trunk_bn(l, i), echunks, s.pen[i], pcps[i], st);
     dmk::dm_learn_disc_stats_kernel<<<1, 1, 0, st>>>(l->head_partials, mt, l->gp_partials, et, 1.f / rows, b->stats);
     return 0;
 }
 }  // namespace
+
+extern "C" {
+
+long long dm_learn_grad_size(const dm_learn* l) {
+    if (!l) { mlp_fail("dm_learn_grad_size: null handle"); return -1; }
+    long long n = 0;
+    for (int i = 0; i < (l->gated ? 10 : 3); ++i) {
+        const dmk::LearnLayerParams L = l->gated ? gated_layer_params(l->m, i, nullptr, nullptr) : layer_params(l->m, i, nullptr, nullptr);
+        n += static_cast<long long>(L.out_dim) * (L.in_dim + 1);
+    }
+    return n;
+}
 
 dm_learn* dm_learn_create_gated(int device, int kind, int in_dim, int goal_dim, int h0, int h1, int out_dim, int gate_common, int gate_hidden, int max_rows) {
     if (kind != 0 && kind != 1) { mlp_fail("dm_learn_create_gated: kind must be 0 (actor) or 1 (critic)"); return nullptr; }
@@ -827,22 +714,17 @@ dm_learn* dm_learn_create_gated(int device, int kind, int in_dim, int goal_dim, 
     l->m = m; l->gated = true; l->kind = kind; l->max_rows = m->max_rows;
     const int N0 = m->N0, N1 = m->N1, in[3] = {trunk_in, h0, h1};
     const int gF[4] = {128, 128, pad_to(GC + 1, 128), 128}, gN[4] = {2 * N0, 2 * N1, 128, 128};
-    const size_t R = m->max_rows, h = sizeof(__half);
+    const size_t R = m->max_rows;
     l->KS = (2 * N0 + 2 * N1) / 64;
     bool ok = trunk_workspace(l, in);
     for (int j = 0; j < 4 && ok; ++j) {
         l->gF[j] = gF[j]; l->gN[j] = gN[j]; l->g_max_splits[j] = dw_max_splits(gF[j], gN[j], 128, m->max_rows / 64);
-        ok = cudaMalloc(&l->gxt[j], R * gF[j] * h) == cudaSuccess && cudaMalloc(&l->gdy_b[j], 2 * R * gN[j] * h) == cudaSuccess &&
-             cudaMalloc(&l->gpartial[j], static_cast<size_t>(l->g_max_splits[j]) * gN[j] * gF[j] * sizeof(float)) == cudaSuccess;
+        ok = alloc(l, &l->gxt[j], R * gF[j]) && alloc(l, &l->gdy_b[j], 2 * R * gN[j]) && alloc(l, &l->gpartial[j], static_cast<size_t>(l->g_max_splits[j]) * gN[j] * gF[j]);
     }
-    for (int i = 0; i < 2 && ok; ++i) {
-        const size_t n = R * (i ? N1 : N0) * sizeof(float);
-        ok = cudaMalloc(&l->fa[i], n) == cudaSuccess && cudaMalloc(&l->fb[i], n) == cudaSuccess;
-    }
+    for (int i = 0; i < 2 && ok; ++i) ok = alloc(l, &l->fa[i], R * (i ? N1 : N0)) && alloc(l, &l->fb[i], R * (i ? N1 : N0));
     // the block-diagonal and transposed B operands keep their zero blocks and padding from here on (the layer passes write the weights only)
-    const size_t wst = 2 * static_cast<size_t>(l->KS) * 64 * 128, wght = 2 * 128 * 128;
-    ok = ok && cudaMalloc(&l->st_a, 2 * R * l->KS * 64 * h) == cudaSuccess && cudaMalloc(&l->wst, wst * h) == cudaSuccess && cudaMemset(l->wst, 0, wst * h) == cudaSuccess &&
-         cudaMalloc(&l->dg_a, 2 * R * 128 * h) == cudaSuccess && cudaMalloc(&l->wght, wght * h) == cudaSuccess && cudaMemset(l->wght, 0, wght * h) == cudaSuccess;
+    ok = ok && alloc(l, &l->st_a, 2 * R * l->KS * 64) && alloc(l, &l->wst, 2 * static_cast<size_t>(l->KS) * 64 * 128, true) && alloc(l, &l->dg_a, 2 * R * 128) &&
+         alloc(l, &l->wght, 2 * 128 * 128, true);
     if (ok) {
         ok = cudaFuncSetAttribute(dmk::dm_mlp_gated_save_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(64)) == cudaSuccess &&
              cudaFuncSetAttribute(dmk::dm_mlp_grad_xg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dmk::dm_mlp_smem_bytes(128)) == cudaSuccess;
@@ -851,22 +733,19 @@ dm_learn* dm_learn_create_gated(int device, int kind, int in_dim, int goal_dim, 
     return l;
 }
 
+}  // extern "C"
+
 namespace {
-int gated_net_check(const dm_learn_gated_net* net, const char* fn) {
-    if (!net) return mlp_fail(std::string(fn) + ": null parameters");
-    for (int i = 0; i < 10; ++i)
-        if (!net->w[i] || !net->b[i] || !net->acc_w[i] || !net->acc_b[i]) return mlp_fail(std::string(fn) + ": null parameter or accumulator pointer");
-    return 0;
-}
 // chunk offsets of ds_l and dt_l in [ds_0 | dt_0 | ds_1 | dt_1]
 int s_chunk(const dm_learn* l, int layer) { return layer ? 2 * l->m->N0 / 64 : 0; }
 int t_chunk(const dm_learn* l, int layer) { return s_chunk(l, layer) + (layer ? l->m->N1 : l->m->N0) / 64; }
 // the ten layer passes of a gated workspace: the forward tiles, and the B operands of the dX GEMMs (W1^T, W2^T, the block-diagonal
-// [Ws_l^T, Wt_l^T], [Wgh_0 | Wgh_1]^T); with `b` also the optimiser step on the dW partials (split counts: splits for the trunk, gsplits
-// for the gate's GEMMs; or the split step's pass, as learn_layers)
-void learn_gated_layers(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_batch* b, const int* splits, const int* gsplits, cudaStream_t st,
-                        Pass pass = Pass::step, float* grad = nullptr, float scale = 1.f) {
+// [Ws_l^T, Wt_l^T], [Wgh_0 | Wgh_1]^T); with a batch `gb` also the optimiser step on the dW partials (split counts: sp.trunk for the trunk,
+// sp.gate for the gate's GEMMs; or the split step's pass, as for a plain workspace)
+void learn_layers(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_gated_batch* gb, const Splits& sp, Pass pass, float* grad, float scale,
+                  cudaStream_t st) {
     dm_mlp* m = l->m;
+    const dm_learn_batch* b = gb ? &gb->batch : nullptr;
     const size_t tt = 2 * 128 * 64;   // halves of a hi + lo 128 x 64 B tile
     size_t off = 0;
     for (int i = 0; i < 10; ++i) {
@@ -877,17 +756,17 @@ void learn_gated_layers(dm_learn* l, const dm_learn_gated_net* net, const dm_lea
         int s = 0;
         if (i < 3) {
             if (i > 0) { L.t_tiles = l->wt[i]; L.t_NC = l->Nout[i] / 64; }
-            L.partial = l->partial[i]; L.Npad = l->Nout[i]; L.F = l->F[i]; s = b ? splits[i] : 0;
+            L.partial = l->partial[i]; L.Npad = l->Nout[i]; L.F = l->F[i]; s = sp.trunk[i];
         } else if (i == 3) {
-            L.partial = l->gpartial[3]; L.Npad = 128; L.F = l->gF[3]; s = b ? gsplits[3] : 0;
+            L.partial = l->gpartial[3]; L.Npad = 128; L.F = l->gF[3]; s = sp.gate[3];
         } else if (i < 6) {
             L.t_tiles = l->wght + lay * tt; L.t_NC = 2;
-            L.partial = l->gpartial[2] + static_cast<size_t>(64 * lay) * l->gF[2]; L.Npad = 128; L.F = l->gF[2]; s = b ? gsplits[2] : 0;
+            L.partial = l->gpartial[2] + static_cast<size_t>(64 * lay) * l->gF[2]; L.Npad = 128; L.F = l->gF[2]; s = sp.gate[2];
         } else {
             const bool gate_scale = i < 8;
             const int N = lay ? m->N1 : m->N0;
             L.t_tiles = l->wst + static_cast<size_t>(gate_scale ? s_chunk(l, lay) : t_chunk(l, lay)) * tt + 512 * lay; L.t_NC = l->KS;
-            L.partial = l->gpartial[lay] + (gate_scale ? 0 : static_cast<size_t>(N) * l->gF[lay]); L.Npad = 2 * N; L.F = l->gF[lay]; s = b ? gsplits[lay] : 0;
+            L.partial = l->gpartial[lay] + (gate_scale ? 0 : static_cast<size_t>(N) * l->gF[lay]); L.Npad = 2 * N; L.F = l->gF[lay]; s = sp.gate[lay];
         }
         if (b) optimiser_fields(L, net, i, b, s);
         launch_pass(pass, D, false, grad, scale, &off, st);
@@ -938,29 +817,17 @@ void learn_gated_backward(dm_learn* l, int mt, const int* splits, const int* cps
     dmk::dm_mlp_grad_x_kernel<<<dim3(mt, 1), 256, dmk::dm_mlp_smem_bytes(128), st>>>(X, dmk::MlpGradParams{m->gc_t, nullptr, l->gdy_b[3], nullptr, chunks, 0});
     launch_dw(l->gxt[3], l->gdy_b[3], l->gpartial[3], l->gF[3], 128, 128, chunks, gsplits[3], gcps[3], st);
 }
-}  // namespace
-
-int dm_learn_set_gated_weights(dm_learn* l, const dm_learn_gated_net* net, void* stream) {
-    if (!l) return mlp_fail("dm_learn_set_gated_weights: null handle");
-    if (!l->gated) return mlp_fail("dm_learn_set_gated_weights: the workspace holds a plain network (dm_learn_create); use dm_learn_set_weights");
-    if (gated_net_check(net, "dm_learn_set_gated_weights")) return 1;
-    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_set_gated_weights: cudaSetDevice failed");
-    learn_gated_layers(l, net, nullptr, nullptr, nullptr, static_cast<cudaStream_t>(stream));
-    return launch_status("dm_learn_set_gated_weights");
-}
-
-namespace {
-// a gated PPO step up to its layer passes: the split-K plans of the trunk's (splits) and the gate's (gsplits) dW GEMMs, the forward, the loss
-// head with its statistics and the gated backward
-int gated_forward_backward(dm_learn* l, const dm_learn_gated_batch* gb, const char* fn, int* splits, int* gsplits, cudaStream_t st) {
+// a gated PPO step up to its layer passes: the split-K plans of the trunk's (s.trunk) and the gate's (s.gate) dW GEMMs, the forward, the
+// loss head with its statistics and the gated backward
+int forward_backward(const char* fn, dm_learn* l, const dm_learn_gated_batch* gb, Splits& s, cudaStream_t st) {
     dm_mlp* m = l->m;
     const dm_learn_batch* b = &gb->batch;
     const int rows = b->rows, mt = (rows + 127) / 128, chunks = 2 * mt;
     int cps[3], gcps[4];
     for (int i = 0; i < 3; ++i)
-        if (dw_plan(fn, l->F[i], l->Nout[i], trunk_bn(l, i), chunks, l->max_splits[i], &splits[i], &cps[i])) return 1;
+        if (dw_plan(fn, l->F[i], l->Nout[i], trunk_bn(l, i), chunks, l->max_splits[i], &s.trunk[i], &cps[i])) return 1;
     for (int j = 0; j < 4; ++j)
-        if (dw_plan(fn, l->gF[j], l->gN[j], 128, chunks, l->g_max_splits[j], &gsplits[j], &gcps[j])) return 1;
+        if (dw_plan(fn, l->gF[j], l->gN[j], 128, chunks, l->g_max_splits[j], &s.gate[j], &gcps[j])) return 1;
     // forward: gathered [state | goal] rows and goals -> the gated network -> the normalised output (identity output normaliser)
     const dmk::LearnPrepParams Q{b->states, b->idx, b->in_mean, b->in_istd, b->in_clip > 0.f ? b->in_clip : 1e30f, m->in_dim, rows, m->K0 / 64, m->obs_t};
     const dmk::LearnGoalParams Qg{gb->goals, gb->g_mean, gb->g_istd, gb->g_clip > 0.f ? gb->g_clip : 1e30f, m->goal_dim, m->goal_t};
@@ -968,48 +835,104 @@ int gated_forward_backward(dm_learn* l, const dm_learn_gated_batch* gb, const ch
     learn_gated_forward(l, rows, mt, st);
     // the loss heads act on the output only: the plain step's
     launch_ppo_head(l, b, mt, st);
-    learn_gated_backward(l, mt, splits, cps, gsplits, gcps, st);
+    learn_gated_backward(l, mt, s.trunk, cps, s.gate, gcps, st);
     return 0;
+}
+// the workspace check of a learner entry: a gated entry needs a gated workspace, a plain one a plain workspace; beyond the re-tiling, the
+// discriminator's entries need kind 2 and the PPO entries kind 0 or 1
+int family_check(const char* fn, const dm_learn* l, bool gated, bool disc, Pass pass) {
+    const std::string f(fn);
+    if (!l) return mlp_fail(f + ": null handle");
+    if (gated && !l->gated) return mlp_fail(f + ": the workspace holds a plain network (dm_learn_create)");
+    if (!gated && l->gated) return mlp_fail(f + ": the workspace holds a gated network (dm_learn_create_gated)");
+    if (pass == Pass::retile) return 0;
+    if (disc && l->kind != 2) return mlp_fail(f + ": the workspace is a PPO actor's or critic's (kind 0 or 1); the discriminator's entries need kind 2");
+    if (!disc && l->kind == 2) return mlp_fail(f + ": the workspace is a discriminator's (kind 2)");
+    return 0;
+}
+// the checks of an apply: the optimiser fields it reads (a gated batch: those of its PPO batch), the flat gradient and its scale
+template <class Batch>
+int apply_check(const char* fn, const Batch* b, const float* d_grad, float scale) {
+    if constexpr (std::is_same_v<Batch, dm_learn_gated_batch>) {
+        return apply_check(fn, b ? &b->batch : nullptr, d_grad, scale);
+    } else {
+        const std::string f(fn);
+        if (!b) return mlp_fail(f + ": null batch");
+        if (!d_grad) return mlp_fail(f + ": null gradient pointer");
+        if (!std::isfinite(scale)) return mlp_fail(f + ": scale must be finite");
+        float reg = 0.f;
+        if constexpr (std::is_same_v<Batch, dm_learn_disc_batch>) reg = b->logit_reg_weight;
+        if (!(b->stepsize >= 0.f) || !(b->momentum >= 0.f) || !(b->weight_decay >= 0.f) || !(reg >= 0.f))
+            return mlp_fail(f + ": stepsize, momentum, weight_decay (and logit_reg_weight) must be >= 0");
+        return 0;
+    }
+}
+// the dm_learn_* entry fn: the workspace check, the checks of the net and of the batch (an apply: apply_check), device and stream, the
+// forward and backward of a step or grad (they fill the split counts), the layer pass and the launch status.  Net and Batch name the
+// family: dm_learn_net with dm_learn_batch (the PPO networks; for set-weights, every plain workspace) or dm_learn_disc_batch, and
+// dm_learn_gated_net with dm_learn_gated_batch.  b is null for the re-tiling
+template <class Batch, class Net>
+int learn(const char* fn, Pass pass, dm_learn* l, const Net* net, const Batch* b, float* grad, float scale, void* stream) {
+    constexpr bool gated = std::is_same_v<Net, dm_learn_gated_net>, disc = std::is_same_v<Batch, dm_learn_disc_batch>;
+    const bool steps = pass == Pass::step || pass == Pass::pack;   // a forward and backward before the layer pass
+    if (family_check(fn, l, gated, disc, pass) || net_check(fn, net)) return 1;
+    if (steps && batch_check(fn, l, b)) return 1;
+    if (pass == Pass::apply && apply_check(fn, b, grad, scale)) return 1;
+    if (pass == Pass::pack && !grad) return mlp_fail(std::string(fn) + ": null gradient pointer");
+    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail(std::string(fn) + ": cudaSetDevice failed");
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    Splits s;
+    if (steps && forward_backward(fn, l, b, s, st)) return 1;
+    // optimiser step and re-tiling, after every GEMM that read the old weights
+    learn_layers(l, net, b, s, pass, grad, scale, st);
+    return launch_status(fn);
 }
 }  // namespace
 
+extern "C" {
+
+int dm_learn_set_weights(dm_learn* l, const dm_learn_net* net, void* stream) {
+    return learn<dm_learn_batch>("dm_learn_set_weights", Pass::retile, l, net, nullptr, nullptr, 1.f, stream);
+}
+
+int dm_learn_step(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, void* stream) {
+    return learn("dm_learn_step", Pass::step, l, net, b, nullptr, 1.f, stream);
+}
+
+int dm_learn_grad(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, float* d_grad, void* stream) {
+    return learn("dm_learn_grad", Pass::pack, l, net, b, d_grad, 1.f, stream);
+}
+
+int dm_learn_apply(dm_learn* l, const dm_learn_net* net, const dm_learn_batch* b, const float* d_grad, float scale, void* stream) {
+    return learn("dm_learn_apply", Pass::apply, l, net, b, const_cast<float*>(d_grad), scale, stream);
+}
+
+int dm_learn_disc_step(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* b, void* stream) {
+    return learn("dm_learn_disc_step", Pass::step, l, net, b, nullptr, 1.f, stream);
+}
+
+int dm_learn_disc_grad(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* b, float* d_grad, void* stream) {
+    return learn("dm_learn_disc_grad", Pass::pack, l, net, b, d_grad, 1.f, stream);
+}
+
+int dm_learn_disc_apply(dm_learn* l, const dm_learn_net* net, const dm_learn_disc_batch* b, const float* d_grad, float scale, void* stream) {
+    return learn("dm_learn_disc_apply", Pass::apply, l, net, b, const_cast<float*>(d_grad), scale, stream);
+}
+
+int dm_learn_set_gated_weights(dm_learn* l, const dm_learn_gated_net* net, void* stream) {
+    return learn<dm_learn_gated_batch>("dm_learn_set_gated_weights", Pass::retile, l, net, nullptr, nullptr, 1.f, stream);
+}
+
 int dm_learn_gated_step(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_gated_batch* gb, void* stream) {
-    const char* fn = "dm_learn_gated_step";
-    if (!l) return mlp_fail("dm_learn_gated_step: null handle");
-    if (!l->gated) return mlp_fail("dm_learn_gated_step: the workspace holds a plain network (dm_learn_create); use dm_learn_step");
-    const dm_learn_batch* b = gb ? &gb->batch : nullptr;
-    if (gated_net_check(net, fn) || ppo_batch_check(fn, l, b, gb)) return 1;
-    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_gated_step: cudaSetDevice failed");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    int splits[3], gsplits[4];
-    if (gated_forward_backward(l, gb, fn, splits, gsplits, st)) return 1;
-    // optimiser step and re-tiling, after every GEMM that read the old weights
-    learn_gated_layers(l, net, b, splits, gsplits, st);
-    return launch_status(fn);
+    return learn("dm_learn_gated_step", Pass::step, l, net, gb, nullptr, 1.f, stream);
 }
 
 int dm_learn_gated_grad(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_gated_batch* gb, float* d_grad, void* stream) {
-    const char* fn = "dm_learn_gated_grad";
-    const dm_learn_batch* b = gb ? &gb->batch : nullptr;
-    if (split_kind_check(fn, l, true, false) || gated_net_check(net, fn) || ppo_batch_check(fn, l, b, gb)) return 1;
-    if (!d_grad) return mlp_fail("dm_learn_gated_grad: null gradient pointer");
-    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_gated_grad: cudaSetDevice failed");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    int splits[3], gsplits[4];
-    if (gated_forward_backward(l, gb, fn, splits, gsplits, st)) return 1;
-    learn_gated_layers(l, net, b, splits, gsplits, st, Pass::pack, d_grad);
-    return launch_status(fn);
+    return learn("dm_learn_gated_grad", Pass::pack, l, net, gb, d_grad, 1.f, stream);
 }
 
 int dm_learn_gated_apply(dm_learn* l, const dm_learn_gated_net* net, const dm_learn_gated_batch* gb, const float* d_grad, float scale, void* stream) {
-    const char* fn = "dm_learn_gated_apply";
-    const dm_learn_batch* b = gb ? &gb->batch : nullptr;
-    if (split_kind_check(fn, l, true, false) || gated_net_check(net, fn)) return 1;
-    if (apply_check(fn, b, d_grad, scale, b ? b->stepsize : 0.f, b ? b->momentum : 0.f, b ? b->weight_decay : 0.f, 0.f)) return 1;
-    if (cudaSetDevice(l->m->device) != cudaSuccess) return mlp_fail("dm_learn_gated_apply: cudaSetDevice failed");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    learn_gated_layers(l, net, b, kNoSplits, kNoSplits, st, Pass::apply, const_cast<float*>(d_grad), scale);
-    return launch_status(fn);
+    return learn("dm_learn_gated_apply", Pass::apply, l, net, gb, const_cast<float*>(d_grad), scale, stream);
 }
 
 int dm_mlp_set_gated_weights_device(dm_mlp* m, const float* const* d_w, const float* const* d_b, void* stream) {
@@ -1039,17 +962,9 @@ int dm_mlp_set_gated_normalizers_device(dm_mlp* m, const float* d_s_mean, const 
 
 void dm_learn_destroy(dm_learn* l) {
     if (!l) return;
-    if (l->m) {
-        cudaSetDevice(l->m->device);
-        dm_mlp_destroy(l->m);
-    }
-    cudaFree(l->out); cudaFree(l->head_partials);
-    for (int i = 0; i < 3; ++i) { cudaFree(l->xt[i]); cudaFree(l->dy_a[i]); cudaFree(l->dy_b[i]); cudaFree(l->wt[i]); cudaFree(l->partial[i]); cudaFree(l->pt[i]); cudaFree(l->pen[i]); }
-    for (int i = 0; i < 2; ++i) { cudaFree(l->u_a[i]); cudaFree(l->u_b[i]); cudaFree(l->q_a[i]); }
-    cudaFree(l->seed_a); cudaFree(l->seed_b); cudaFree(l->e_a); cudaFree(l->w0p); cudaFree(l->gp_partials);
-    for (int j = 0; j < 4; ++j) { cudaFree(l->gxt[j]); cudaFree(l->gdy_b[j]); cudaFree(l->gpartial[j]); }
-    for (int i = 0; i < 2; ++i) { cudaFree(l->fa[i]); cudaFree(l->fb[i]); }
-    cudaFree(l->st_a); cudaFree(l->wst); cudaFree(l->dg_a); cudaFree(l->wght);
+    cudaSetDevice(l->m->device);
+    for (void* p : l->bufs) cudaFree(p);
+    dm_mlp_destroy(l->m);
     delete l;
 }
 
@@ -1058,11 +973,7 @@ long long dm_mlp_launches(dm_mlp* m) { return m ? m->launches : 0; }
 void dm_mlp_destroy(dm_mlp* m) {
     if (!m) return;
     cudaSetDevice(m->device);
-    for (auto& p : m->w) cudaFree(p);
-    for (auto& p : m->b) cudaFree(p);
-    cudaFree(m->obs_t); cudaFree(m->act0); cudaFree(m->act1); cudaFree(m->in_mean); cudaFree(m->in_istd); cudaFree(m->out_mean); cudaFree(m->out_std);
-    for (int l = 0; l < 2; ++l) { cudaFree(m->wgs[l]); cudaFree(m->wgb[l]); cudaFree(m->bgs[l]); cudaFree(m->bgb[l]); }
-    cudaFree(m->wgc); cudaFree(m->wgh); cudaFree(m->bgc); cudaFree(m->bgh); cudaFree(m->goal_t); cudaFree(m->gc_t); cudaFree(m->gh_t); cudaFree(m->g_mean); cudaFree(m->g_istd);
+    for (void* p : m->bufs) cudaFree(p);
     delete m;
 }
 

@@ -169,6 +169,26 @@ class DataParallel:
             raise ValueError("data-parallel learner: a rank's window has no explored sample (the actor trains on explored actions only)")
 
 
+def _check_indices(device, *indices):
+    """refuses a minibatch index tensor the tensor-core step cannot read.  indices: (name, index tensor, rows of its batch) triples; each tensor
+    must be contiguous int64 with the batch's rows entries on `device`"""
+    import torch
+    for name, idx, rows in indices:
+        if idx.dtype != torch.int64 or not idx.is_contiguous() or idx.device != device or idx.numel() != rows:
+            raise ValueError("%s must be a contiguous int64 tensor of %d entries on %s" % (name, rows, device))
+
+
+def _tc_step(tc, batch, dp, grad, stream):
+    """one tensor-core minibatch step of the workspace tc: fused without a group (dp None), or the flat gradient into `grad`, its sum over the
+    ranks and the step on the ranks' mean"""
+    if dp is None:
+        tc.step(batch, stream=stream)
+        return
+    tc.grad(batch, grad, stream=stream)
+    dp.sum(grad)
+    tc.apply(batch, grad, 1.0 / dp.world, stream=stream)
+
+
 def _weight_decay_grads(net, params, grads, weight_decay):
     """grads plus the gradient of weight_decay * weight_decay_loss(net): weight_decay w on the weights, nothing on the biases"""
     names = {p: n for n, p in net.named_parameters()}
@@ -247,11 +267,11 @@ class PPOLearner:
             cls = TensorCoreGatedLearner if rollout.goal_size > 0 else TensorCoreLearner
             self._tc_actor = cls(self.policy, self.acc, "actor", self.minibatch_size, device=di)
             self._tc_critic = cls(self.critic, self.acc, "critic", self.minibatch_size, device=di)
-            if self.dp:   # the flat gradients the ranks sum
-                self._grad_actor = torch.empty(self._tc_actor.grad_size(), device=dev)
-                self._grad_critic = torch.empty(self._tc_critic.grad_size(), device=dev)
+            # the flat gradients the ranks sum
+            self._grad_actor = torch.empty(self._tc_actor.grad_size(), device=dev) if self.dp else None
+            self._grad_critic = torch.empty(self._tc_critic.grad_size(), device=dev) if self.dp else None
         if self.dp:   # the rollout's tensor-core actor and critic collect with the broadcast weights
-            self._refresh_rollout()
+            rollout.retile_tensor_core("actor", "critic")
 
     # ---- the window: everything a minibatch step reads, computed once per update
     def window(self, traj):
@@ -326,14 +346,12 @@ class PPOLearner:
         critic loss, clip fraction) accumulate"""
         if self.backend == "tensor_core":
             keep, actor, critic = tc
-            for name, idx, batch in (("critic_idx", critic_idx, critic), ("actor_idx", actor_idx, actor)):
-                if idx.dtype != self.torch.int64 or not idx.is_contiguous() or idx.device != self.device or idx.numel() != batch.rows:
-                    raise ValueError("%s must be a contiguous int64 tensor of %d entries on %s" % (name, batch.rows, self.device))
+            _check_indices(self.device, ("critic_idx", critic_idx, critic.rows), ("actor_idx", actor_idx, actor.rows))
             st = self.torch.cuda.current_stream(self.device).cuda_stream
             critic.idx = critic_idx.data_ptr()
-            self._tc_step(self._tc_critic, critic, "_grad_critic", st)
+            _tc_step(self._tc_critic, critic, self.dp, self._grad_critic, st)
             actor.idx = actor_idx.data_ptr()
-            self._tc_step(self._tc_actor, actor, "_grad_actor", st)
+            _tc_step(self._tc_actor, actor, self.dp, self._grad_actor, st)
             return
         t = self.torch
         total, loss = self.critic_loss(w, critic_idx)
@@ -347,16 +365,6 @@ class PPOLearner:
             momentum_step(self.actor_params, [self.acc[p] for p in self.actor_params], grads, self.actor_stepsize, self.actor_momentum)
             stats[0] += loss.detach().abs()      # PPOAgent._update logs the mean of |actor loss| over the minibatches
             stats[2] += clip_fraction(ratio.detach(), self.ratio_clip)
-
-    def _tc_step(self, tc, batch, grad, stream):
-        """one tensor-core step: fused, or (data parallel) the gradient, its sum over the ranks and the step on the ranks' mean"""
-        if not self.dp:
-            tc.step(batch, stream=stream)
-            return
-        g = getattr(self, grad)
-        tc.grad(batch, g, stream=stream)
-        self.dp.sum(g)
-        tc.apply(batch, g, 1.0 / self.world, stream=stream)
 
     def _grads(self, total, loss, net, params, weight_decay):
         """the step's gradient: of `total` (the loss with its weight decay), or (data parallel) the ranks' mean gradient of `loss` plus the
@@ -393,7 +401,7 @@ class PPOLearner:
         if tc is not None:
             keep = tc[0]
             stats = [keep["stats_a"][0], keep["stats_c"][0], keep["stats_a"][1]]
-        self._refresh_rollout()
+        self.ro.retile_tensor_core("actor", "critic")
         out = dict(actor_loss=stats[0] / steps, critic_loss=stats[1] / steps, clip_frac=stats[2] / steps, adv_mean=w["adv_mean"],
                    adv_std=w["adv_std"], exp_samples=t.tensor(n_exp, device=self.device))
         if self.dp:
@@ -401,30 +409,6 @@ class PPOLearner:
             x = self.dp.sum(t.stack([out[k].double() for k in keys] + [out["exp_samples"].double()]))
             out = dict(zip(keys, (x[:-1] / self.world).float()), exp_samples=x[-1].round().long())   # the explored samples of all ranks
         return out
-
-    def _refresh_rollout(self):
-        """the rollout's tensor-core actor and critic take the new weights and the normalisers' current statistics, the ones this update trained
-        with: re-tiled and copied on the device, plain and gated handles alike"""
-        ro = self.ro
-        if ro._tc is None and ro._tc_critic is None:
-            return
-        st = self.torch.cuda.current_stream(self.device).cuda_stream
-        c = lambda n: (n.mean.contiguous(), n.std.contiguous())
-        if ro.goal_size > 0:
-            from .capi import gated_layers
-            if ro._tc is not None:
-                ro._tc.set_weights_device(gated_layers(self.policy, self.policy.mean), stream=st)
-                ro._tc.set_normalizers_device(*c(ro.s_norm), *c(ro.g_norm), *c(ro.a_norm), stream=st)
-            if ro._tc_critic is not None:
-                ro._tc_critic.set_weights_device(gated_layers(self.critic, self.critic.out), stream=st)
-                ro._tc_critic.set_normalizers_device(*c(ro.s_norm), *c(ro.g_norm), *c(ro.val_norm), stream=st)
-            return
-        if ro._tc is not None:
-            ro._tc.set_weights_device(list(self.policy.hidden) + [self.policy.mean], stream=st)
-            ro._tc.set_normalizers_device(*c(ro.s_norm), *c(ro.a_norm), stream=st)
-        if ro._tc_critic is not None:
-            ro._tc_critic.set_weights_device(list(self.critic.hidden) + [self.critic.out], stream=st)
-            ro._tc_critic.set_normalizers_device(*c(ro.s_norm), *c(ro.val_norm), stream=st)
 
 
 # ---- the AMP discriminator (R/learning/amp_agent.py)
@@ -516,10 +500,9 @@ class AMPDiscLearner:
                 raise ValueError("the tensor_core learner needs a CUDA device")
             from .capi import TensorCoreLearner
             self._tc = TensorCoreLearner(self.disc, self.acc, "disc", 2 * self.batch_size, device=self.device.index or 0)
-            if self.dp:   # the flat gradient the ranks sum
-                self._grad = torch.empty(self._tc.grad_size(), device=self.device)
+            self._grad = torch.empty(self._tc.grad_size(), device=self.device) if self.dp else None   # the flat gradient the ranks sum
         if self.dp:   # the rollout's tensor-core discriminator scores with the broadcast weights
-            self._refresh_rollout()
+            rollout.retile_tensor_core("disc")
 
     def loss(self, norm_agent, norm_expert):
         """(total loss with the regularisers, disc_loss, grad_penalty, d_e, d_a) on normalised agent and expert rows (torch autograd)"""
@@ -548,17 +531,9 @@ class AMPDiscLearner:
         t = self.torch
         if self.backend == "tensor_core":
             keep, batch = tc
-            for name, idx in (("agent_idx", agent_idx), ("expert_idx", expert_idx)):
-                if idx.dtype != t.int64 or not idx.is_contiguous() or idx.device != self.device or idx.numel() != batch.rows:
-                    raise ValueError("%s must be a contiguous int64 tensor of %d entries on %s" % (name, batch.rows, self.device))
+            _check_indices(self.device, ("agent_idx", agent_idx, batch.rows), ("expert_idx", expert_idx, batch.rows))
             batch.agent_idx, batch.expert_idx = agent_idx.data_ptr(), expert_idx.data_ptr()
-            st = t.cuda.current_stream(self.device).cuda_stream
-            if not self.dp:
-                self._tc.step(batch, stream=st)
-                return
-            self._tc.grad(batch, self._grad, stream=st)
-            self.dp.sum(self._grad)
-            self._tc.apply(batch, self._grad, 1.0 / self.world, stream=st)
+            _tc_step(self._tc, batch, self.dp, self._grad, t.cuda.current_stream(self.device).cuda_stream)
             return
         norm = self.ro.amp_norm
         total, loss, gp, d_e, d_a = self.loss(norm.normalize(agent[agent_idx]), norm.normalize(expert[expert_idx]))
@@ -601,19 +576,7 @@ class AMPDiscLearner:
             self.minibatch_step(agent, expert, a, e, stats, tc)
         if tc is not None:
             stats = list(tc[0]["stats"])
-        self._refresh_rollout()
+        self.ro.retile_tensor_core("disc")
         keys = ("disc_loss", "grad_penalty", "acc_expert", "acc_agent", "logit_expert", "logit_agent")
         stats = [s / self.steps for s in stats]
         return dict(zip(keys, self.dp.mean_stats(stats) if self.dp else stats))
-
-    def _refresh_rollout(self):
-        """the rollout's tensor-core discriminator takes the new weights and amp_norm's current statistics (identity output normaliser), re-tiled
-        and copied on the device"""
-        ro = self.ro
-        if getattr(ro, "_tc_disc", None) is None:
-            return
-        t = self.torch
-        st = t.cuda.current_stream(self.device).cuda_stream
-        ro._tc_disc.set_weights_device(list(self.disc.hidden) + [self.disc.logit], stream=st)
-        ro._tc_disc.set_normalizers_device(ro.amp_norm.mean.contiguous(), ro.amp_norm.std.contiguous(), t.zeros(1, device=self.device),
-                                           t.ones(1, device=self.device), stream=st)

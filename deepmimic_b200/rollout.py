@@ -463,6 +463,24 @@ class BatchedRollout:
                                                 in_clip=self.s_norm.clip, out_mean=vm, out_std=vs, max_rows=2 * env.num_envs, device=env.device.index or 0)
         return self._tc
 
+    def retile_tensor_core(self, *roles):
+        """the existing tensor-core handles of `roles` ("actor", "critic", "disc") take the torch modules' current weights and the normalisers'
+        current statistics, re-tiled and copied on the device (the discriminator: amp_norm and the identity output normaliser)"""
+        from .capi import tc_layers
+        t, dev = self.torch, self.env.device
+        c = lambda n: (n.mean.contiguous(), n.std.contiguous())
+        for role in roles:
+            tc, net = dict(actor=(self._tc, self.policy), critic=(self._tc_critic, self.critic), disc=(self._tc_disc, self.disc))[role]
+            if tc is None:
+                continue
+            st = t.cuda.current_stream(dev).cuda_stream
+            tc.set_weights_device(tc_layers(net, role), stream=st)
+            if role == "disc":
+                tc.set_normalizers_device(*c(self.amp_norm), t.zeros(1, device=dev), t.ones(1, device=dev), stream=st)
+            else:
+                goal = c(self.g_norm) if self.goal_size > 0 else ()
+                tc.set_normalizers_device(*c(self.s_norm), *goal, *c(self.a_norm if role == "actor" else self.val_norm), stream=st)
+
     def _act_tensor_core(self, s, explore, g=None):
         """un-normalised actions and log-probabilities from the tensor-core actor (exploration noise is drawn in torch, added in the kernel's epilogue);
         g: the goals, for the gated actor of the goal-conditioned scenes"""

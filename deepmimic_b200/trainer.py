@@ -444,9 +444,7 @@ class Trainer:
                 for n in self._updated_norms():
                     n.update(all_reduce=self.dp.sum if self.dp else None)
                 # the rollout's tensor-core handles act on the new statistics from the next collect() on, as the torch backend does
-                self.ppo._refresh_rollout()
-                if self.amp:
-                    self.disc._refresh_rollout()
+                ro.retile_tensor_core("actor", "critic", "disc")
         it = self.iter
         self.iter += 1
         if it % cfg["OutputIters"] == 0:
