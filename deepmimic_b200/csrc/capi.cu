@@ -548,17 +548,13 @@ static bool load_host_model(dm_handle& H, const char* asset_root, int argc, cons
                 if (t["Type"].asString("") != "plane") throw std::runtime_error("Unsupported terrain type: " + t["Type"].asString("") + " (supported: plane)");
             }
         }
-        // Scenes on the accelerated path: imitate, imitate_amp, and the AMP task scenes target_amp / heading_amp (goals, task rewards, clip
-        // datasets; validated on hardware against the oracle in round 2: tests/test_task_scenes_gpu.py).  heading_amp_getup / strike_amp have
-        // their device code written and host-checked but are not validated on hardware: opt-in with DM_EXPERIMENTAL_TASK_SCENES=1.  Every other
-        // scene name is refused.
-        const char* exp_env = std::getenv("DM_EXPERIMENTAL_TASK_SCENES");
-        const bool experimental = exp_env != nullptr && exp_env[0] == '1';
+        // Scenes on the accelerated path: imitate, imitate_amp, and the AMP task scenes target_amp / heading_amp / heading_amp_getup /
+        // strike_amp (goals, task rewards, clip datasets; checked against the oracle on the GPU: tests/test_task_scenes_gpu.py,
+        // tests/test_task_ext_gpu.py).  Every other scene name is refused.
         const bool task_scene = H.sa.cfg.is_task_scene();   // target_amp, heading_amp, heading_amp_getup, strike_amp
         const std::string& scn = H.sa.cfg.scene;
-        const bool validated = scn == "imitate" || scn == "imitate_amp" || scn == "target_amp" || scn == "heading_amp";
-        if (!validated && !(task_scene && experimental))
-            throw std::runtime_error("Unsupported scene: " + scn + " (supported: imitate, imitate_amp, target_amp, heading_amp)");
+        if (!task_scene && scn != "imitate" && scn != "imitate_amp")
+            throw std::runtime_error("Unsupported scene: " + scn + " (supported: imitate, imitate_amp, target_amp, heading_amp, heading_amp_getup, strike_amp)");
         if (H.sa.clips.size() != 1 && !task_scene)
             throw std::runtime_error("Unsupported kinematic controller: clips with more than one clip outside the AMP task scenes (supported: motion)");
         if (static_cast<int>(H.sa.clips.size()) > dmk::kMaxClips) throw std::runtime_error("clip dataset larger than the device clip table (" + std::to_string(dmk::kMaxClips) + ")");

@@ -744,9 +744,7 @@ __global__ void __launch_bounds__(BLOCK) dm_reset_kernel(const DevModel* __restr
 }
 
 // ---------------------------------------------------------------------------------------------------------------- AMP task scenes
-// One thread per environment; the per-update part of the task logic runs inside dm_step_kernel<.., TASK = true> (dm_task.cuh).
-// NOT YET RUN ON HARDWARE (written after round 1's GPU budget was spent): the scenes stay refused by dm_create unless
-// DM_EXPERIMENTAL_TASK_SCENES=1, and their GPU parity tests are opt-in.
+// One thread per environment; the per-update part of the task logic runs inside dm_step_kernel<.., TASK = true> (dm_task.cuh, dm_task_ext.cuh).
 
 // After dm_reset_kernel: environments whose reset counter moved get cSceneTargetAMP::Reset's part (SceneTargetAMP.cpp:129-134):
 // target timer, target position around the new root, heading 0 and a fresh speed (heading scene), previous-action COM 0.

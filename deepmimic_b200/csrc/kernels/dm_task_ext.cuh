@@ -1,6 +1,7 @@
 // Per-environment logic of two more AMP task scenes, written as host / device-shared code like dm_task.cuh and checked against the oracle on the
 // host (tests/test_task_scenes_cpu.py through tests/task_shim.cpp).  The device glue (what the tile publishes to lane 0 every update in
-// dm_step_kernel<.., kVarTask>, the task reset / observe kernels) is written but has not run on hardware: opt-in, DM_EXPERIMENTAL_TASK_SCENES=1.
+// dm_step_kernel<.., TASK>, the recovery branch of the reset kernel, the task reset / observe kernels) is checked against the oracle update by
+// update on the GPU (tests/test_task_ext_gpu.py).
 //   cSceneHeadingAMPGetup  R/DeepMimicCore/scenes/SceneHeadingAMPGetup.cpp  get-up timer, phase goal, get-up reward, recovery episodes
 //   cSceneStrikeAMP        R/DeepMimicCore/scenes/SceneStrikeAMP.cpp        point target, hit detection, three-regime reward, success
 // Both sit on top of the target / heading logic of dm_task.cuh (task block t, draw stream TaskRng); their own state lives in an extension block x.

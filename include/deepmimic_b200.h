@@ -133,10 +133,10 @@ int dm_record_goal(dm_handle* h, float* d_out);              /* [num_envs x goal
  * synchronisation. */
 int dm_record_pose(dm_handle* h, float* d_pose, float* d_vel);
 /* AMP task scenes target_amp / heading_amp (cSceneTargetAMP / cSceneHeadingAMP: RecordGoal, CalcReward, target updates; goal_size 3).
- * heading_amp_getup / strike_amp are EXPERIMENTAL (device code written and host-checked, not validated on hardware): dm_create accepts
- * them only with DM_EXPERIMENTAL_TASK_SCENES=1 in the environment.  dm_goal_host is RecordGoal into a host buffer [num_envs x 3]; the task-state hooks
- * expose one environment's task block (16 doubles: target x, z, speed, heading, timer, timer max, previous-action COM[3], COM[3], draw
- * counter, reset counter) and the scene constants + draw-stream key for the parity tests. */
+ * heading_amp_getup / strike_amp (cSceneHeadingAMPGetup / cSceneStrikeAMP) add a phase to the goal (goal_size 4).  dm_goal_host is RecordGoal
+ * into a host buffer [num_envs x goal_size]; the task-state hooks expose one environment's task block (16 doubles: target x, z, speed, heading,
+ * timer, timer max, previous-action COM[3], COM[3], draw counter, reset counter, then the 8 doubles of the get-up / strike extension block)
+ * and the scene constants + draw-stream key for the parity tests. */
 int dm_goal_host(dm_handle* h, float* h_out);
 /* Clip datasets (--kin_ctrl clips, cClipsController; task scenes only, experimental like them).  dm_reset_clips = dm_reset with the
  * controller's clip draw injected (h_clip: num_envs ints, may be NULL); dm_record_amp_obs_expert_clips = the expert observation from a given

@@ -1241,6 +1241,7 @@ void dmo_get_getup_state(void* h, double* out) {
     Oracle* o = static_cast<Oracle*>(h);
     out[0] = o->getup_timer_time; out[1] = o->getup_time; out[2] = o->CheckGettingUp() ? 1 : 0; out[3] = o->ContactFall() ? 1 : 0;
 }
+void dmo_set_getup_timer(void* h, double t) { static_cast<Oracle*>(h)->getup_timer_time = t; }
 // strike_amp: out[0] = target hit (0 / 1), out[1] = hit time, out[2] = hit phase, out[3] = target height
 void dmo_get_strike_state(void* h, double* out) { Oracle* o = static_cast<Oracle*>(h); out[0] = o->target_hit ? 1 : 0; out[1] = o->target_hit_time; out[2] = o->CalcHitPhase(); out[3] = o->target_pos.y; }
 void dmo_set_strike_state(void* h, int hit, double hit_time) { Oracle* o = static_cast<Oracle*>(h); o->target_hit = hit != 0; o->target_hit_time = hit_time; }

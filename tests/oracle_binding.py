@@ -119,6 +119,9 @@ class Oracle:
         self.L.dmo_get_getup_state(self.h, dp(o))
         return dict(timer=o[0], getup_time=o[1], getting_up=bool(o[2]), contact_fall=bool(o[3]))
 
+    def set_getup_timer(self, t):
+        self.L.dmo_set_getup_timer(self.h, C.c_double(t))
+
     def strike_state(self):
         """strike_amp: dict(hit, hit_time, phase, target_height)"""
         o = np.zeros(4)
@@ -138,6 +141,10 @@ class Oracle:
         o = np.zeros(3)
         self.L.dmo_calc_com(self.h, dp(o))
         return o
+
+    def set_mode(self, mode):
+        """0 train, 1 test (cRLScene::SetMode): test-mode timer limits, no recovery episodes or initial hits, test-mode get-ups and rewards"""
+        self.L.dmo_set_mode(self.h, int(mode))
 
     def update(self, dt):
         self.L.dmo_update(self.h, C.c_double(dt))

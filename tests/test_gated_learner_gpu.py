@@ -13,6 +13,8 @@ pytestmark = pytest.mark.gpu
 MINI = ["--motion_file", "data/datasets/test_clips_mini.txt"]
 TARGET = MINI + ["--arg_file", "args/train_amp_target_humanoid3d_locomotion_args.txt"]
 HEADING = MINI + ["--arg_file", "args/train_amp_heading_humanoid3d_locomotion_args.txt"]
+TASK_ARGS = dict(target=TARGET, heading=HEADING, heading_getup=["--arg_file", "args/train_amp_heading_getup_humanoid3d_locomotion_getup_args.txt"],
+                 strike=MINI + ["--arg_file", "args/train_amp_strike_humanoid3d_walk_punch_args.txt"])
 HP = dict(actor_stepsize=2.5e-6, actor_momentum=0.9, actor_weight_decay=5e-4, critic_stepsize=1e-2, critic_momentum=0.9, critic_weight_decay=1e-3,
           ratio_clip=0.2, norm_adv_clip=4.0, epochs=1)
 DISC_HP = dict(stepsize=1e-3, momentum=0.9, weight_decay=5e-4, logit_reg_weight=0.05, grad_penalty=10.0)
@@ -36,7 +38,7 @@ def _task_rollout(asset_root, task, n, backend, disc=False, seed=11):
     from deepmimic_b200.rollout import BatchedRollout, build_critic, build_discriminator, build_gated_policy, load_actor_weights
     from tests.test_task_scenes_cpu import fixture_task_actor
     a = fixture_task_actor(task)
-    env = DeepMimicBatchEnv(TARGET if task == "target" else HEADING, num_envs=n, asset_root=asset_root, seed=seed)
+    env = DeepMimicBatchEnv(TASK_ARGS[task], num_envs=n, asset_root=asset_root, seed=seed)
     env._core.set_episode_limit(0.5, 3.0)
     env.reset(True)
     S, G = env.get_state_size(), env.get_goal_size()
@@ -327,9 +329,21 @@ def test_gated_steps_go_downhill(asset_root):
 def test_target_amp_training_loop_on_the_tensor_cores(asset_root):
     """512 target_amp environments: collect(32) with the discriminator and the critic, then the PPO update and the discriminator update, all
     on the tensor cores, three times: every output finite"""
+    _training_loop(asset_root, "target")
+
+
+@pytest.mark.parametrize("task", ["heading_getup", "strike"])
+def test_goal_size_4_training_loop_on_the_tensor_cores(asset_root, task):
+    """the same loop on 512 heading_amp_getup or strike_amp environments: a goal of size 4 (heading or target + get-up / hit phase) through
+    the rollout, the PPO update and the discriminator update on the tensor cores, every output finite"""
+    _training_loop(asset_root, task)
+
+
+def _training_loop(asset_root, task):
     import torch
     from deepmimic_b200.learner import AMPDiscLearner, PPOLearner
-    env, ro = _task_rollout(asset_root, "target", 512, "tensor_core", disc=True)
+    env, ro = _task_rollout(asset_root, task, 512, "tensor_core", disc=True)
+    assert env.get_goal_size() == (3 if task == "target" else 4)
     ppo = PPOLearner(ro, **HP, minibatch_size=4096, backend="tensor_core")
     dl = AMPDiscLearner(ro, **DISC_HP, batch_size=2048, steps=8, backend="tensor_core")
     M = env.get_amp_obs_size()

@@ -338,12 +338,11 @@ def _ptr(a):
 
 
 @pytest.mark.parametrize("args", [TARGET, HEADING])
-def test_device_task_logic_matches_the_oracle_on_the_host(asset_root, task_shim, args, monkeypatch):
+def test_device_task_logic_matches_the_oracle_on_the_host(asset_root, task_shim, args):
     """Drives dm_task.cuh (host build) with the oracle's root positions and compares the whole task block, the goal, the reward and the
     distance failure with the oracle after every update of a 6 s episode under a random policy.  Also checks that the C-ABI host loader
     fills the scene constants the device code receives."""
     from deepmimic_b200 import capi
-    monkeypatch.setenv("DM_EXPERIMENTAL_TASK_SCENES", "1")
     single = ["--kin_ctrl", "motion", "--motion_file", "data/motions/humanoid3d_run.txt"] + args[2:]   # the device path takes one clip for now
     if args is TARGET:
         single = ["--rand_target_time_min", "1", "--rand_target_time_max", "2", "--tar_fail_dist", "6"] + single   # several re-targets and a distance failure in 6 s
@@ -396,17 +395,15 @@ def test_device_task_logic_matches_the_oracle_on_the_host(asset_root, task_shim,
     assert n_goal == 180 and o.task_counter() > (3 if args is TARGET else 50) and (n_far > 0) == (args is TARGET)
 
 
-def test_unvalidated_task_scenes_stay_refused_without_the_opt_in(asset_root, monkeypatch):
-    """target_amp / heading_amp are on the default path since round 2 (validated on hardware); heading_amp_getup / strike_amp and every other
-    scene name are still refused unless DM_EXPERIMENTAL_TASK_SCENES=1."""
+def test_task_scenes_load_and_other_scenes_stay_refused(asset_root):
+    """The four AMP task scenes load with no environment variable set (goal size 3 or 4); dribble_amp (it needs a simulated ball), kin_char
+    and every other scene name are refused by name."""
     from deepmimic_b200 import capi
-    monkeypatch.delenv("DM_EXPERIMENTAL_TASK_SCENES", raising=False)
-    for bad in (GETUP, STRIKE, ["--scene", "dribble_amp"] + TARGET, ["--scene", "kin_char"] + TARGET):
+    for bad in (["--scene", "dribble_amp"] + TARGET, ["--scene", "kin_char"] + TARGET, ["--scene", "no_such_scene"] + TARGET):
         with pytest.raises(RuntimeError, match="Unsupported scene"):
             capi.HostModel(bad, asset_root)
     assert capi.HostModel(HEADING, asset_root).dims.goal_size == 3
     m = capi.HostModel(TARGET, asset_root)                                      # the mini dataset (4 clips) loads in a task scene ...
-    monkeypatch.setenv("DM_EXPERIMENTAL_TASK_SCENES", "1")
     assert m.dims.goal_size == 3
     dur, cdf = m.clip_table()
     o = Oracle(TARGET, asset_root)

@@ -3,7 +3,6 @@ step's goal with a host recomputation from the snapshot."""
 import os, sys
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-os.environ["DM_EXPERIMENTAL_TASK_SCENES"] = "1"
 import torch
 from deepmimic_b200.assets import asset_root
 from deepmimic_b200.env import DeepMimicBatchEnv
