@@ -640,7 +640,11 @@ __global__ void __launch_bounds__(BLOCK) dm_reset_kernel(const DevModel* __restr
     const float bl = static_cast<float>(bld);
     const float* f0 = frames + static_cast<size_t>(idx) * M.pose_dim; const float* f1 = f0 + M.pose_dim;
     const float* v0 = frame_vel + static_cast<size_t>(idx) * M.pose_dim; const float* v1 = v0 + M.pose_dim;
+    // a non-looping clip at or past its end is at rest (cMotion::CalcFrameVel; clip_joint and the observe kernel apply the same rule): a task
+    // scene draws the start time from the previous clip's duration, which can lie past the end of a shorter new clip
+    const bool clip_over = !KM.loop_motion && kt >= KM.motion_dur;
     KinJoint kj = sample_joint(L, f0, f1, v0, v1, bl, lane == 0);
+    if (clip_over) { kj.w = mk3(0, 0, 0); kj.angvel = 0; }
     const float sth = sinf(0.5f * static_cast<float>(th)), cth = cosf(0.5f * static_cast<float>(th));
     const Q4 orot = mkq(0.f, sth, 0.f, cth);
     // root
@@ -648,6 +652,7 @@ __global__ void __launch_bounds__(BLOCK) dm_reset_kernel(const DevModel* __restr
                 (1 - bl) * f0[2] + bl * f1[2] + (KM.loop_motion ? cyc * KM.cycle_delta[2] : 0.f));
     V3 rv = mk3((1 - bl) * v0[0] + bl * v1[0], (1 - bl) * v0[1] + bl * v1[1], (1 - bl) * v0[2] + bl * v1[2]);
     KinJoint kr = sample_joint(M.link[0], f0, f1, v0, v1, bl, true);
+    if (clip_over) { rv = mk3(0, 0, 0); kr.w = mk3(0, 0, 0); }
     Q4 rq = qmul(orot, kr.q); if (rq.w < 0) rq = mkq(-rq.x, -rq.y, -rq.z, -rq.w);
     rq = qnormalize(rq);
     V3 rw = qrot(orot, kr.w);
