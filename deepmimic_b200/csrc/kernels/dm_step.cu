@@ -15,8 +15,8 @@
 // inertias (their unconstrained accelerations are btMultiBody::computeAccelerationsArticulatedBodyAlgorithmMultiDof's).
 // Constraint rows are built with lanes = rows (each lane walks its row's link chain once), the row coupling matrix
 // J M^-1 J^T is formed explicitly in shared memory with lanes = pairs of contact points (3 x 3 blocks), and PGS runs in impulse
-// space: w = A lambda lives in registers (lane = row), the sequential sweep is evaluated in blocks of two solver steps by every lane
-// redundantly from broadcast row data (the figure of merit is warp instructions per step: the sweeps are issue-bound).
+// space: w = A lambda and the impulses live in registers (lane = row), the sequential sweep is evaluated in blocks of two solver steps by every
+// lane redundantly from broadcast row data.
 // All spatial quantities of a link are expressed in WORLD axes about the link's own joint pivot, so passing them between
 // parent and child is a pure shift (no rotation of 6x6 blocks).
 // The update is split into phase routines (kinematics, collision, articulated-body solve, constraint rows + PGS, velocity correction)
@@ -162,12 +162,16 @@ constexpr int kPgsBlock = 2;   // solver steps evaluated per block of the projec
 // Projected Gauss-Seidel in impulse space, 10 sweeps in btMultiBodyConstraintSolver::solveSingleIteration's row order (joint limits in
 // alternating order, contact normals, friction pairs).  Lanes = rows for the state that is wide: every lane keeps w = (A lambda)_row of ITS rows in
 // registers (S rows per lane: row = lane + s W).  The sequential part is evaluated in blocks of B consecutive solver steps of one section:
-//     B independent shuffles fetch the block's w values from their owners; the rows' right-hand side, 1 / A_ii and impulse are broadcast loads,
-//     EVERY lane then evaluates the B sequential Gauss-Seidel updates redundantly (row k+1 sees row k's update through A(k+1, k), B (B-1) / 2
-//     broadcast entries of A), one lane per row commits the new impulse to shared memory,
-//     and every lane adds A(own row, row_k) * delta_k, k = 0..B-1 in order, to its own w's.
-// During the sweeps the warps of a block are issue-bound (3.5 warps per scheduler all inside this loop), so the figure of merit is warp
-// instructions per solver step: ~40 with one shuffle per step (the owner computed and broadcast its update), ~20 here.  Every floating-point
+//     B independent shuffles fetch the block's w values and impulses from their owners (the owner of row r keeps both in registers); the rows'
+//     right-hand side and 1 / A_ii are broadcast loads, EVERY lane then evaluates the B sequential Gauss-Seidel updates redundantly (row k+1 sees
+//     row k's update through A(k+1, k), B (B-1) / 2 broadcast entries of A), each row's owner keeps its new impulse,
+//     and every lane adds A(own row, row_k) * delta_k, k = 0..B-1 in order, to its own w's.  The impulses reach shared memory once, after the
+//     last sweep.  Nothing of the sweeps goes through shared memory but read-only operands, so a block needs no barrier.  The normal and
+//     friction sections run two blocks per iteration and fetch both blocks' impulses before the first block updates any (no row is solved twice
+//     in one section of one sweep): the second block's loads and impulse shuffles are then issued under the first block's dependent chain.
+// The blocks were sized when 3.5 warps per scheduler were all inside this loop (issue-bound: ~40 warp instructions per solver step with one
+// shuffle per step, ~20 here).  Under placement by contact load the warps that set the launch's length sweep with few or no other sweeping
+// warps beside them, and the length of a block's dependent chain counts (DESIGN.md section 9).  Every floating-point
 // operation on w and the update, and their order, are those of the row-by-row sweep (resolveSingleConstraintRowGeneric: delta = rhs - w *
 // jacDiagABInv, clamped sum; friction bounds +-mu * the point's current normal impulse, row skipped while that is <= 0).  Bounds are applied to
 // the UPDATE: clamp(delta, lo - lambda, hi - lambda) equals Bullet's "clamp the sum, then delta = limit - applied" in every branch; the stored
@@ -205,37 +209,62 @@ __device__ __forceinline__ void pgs_sweeps(const float* sA, float* sLam, const f
 #pragma unroll
         for (int s = 0; s < S; ++s) w[s] = fmaf(a_own(s, i, tri(i)), l0, w[s]);
     }
-    bool writer[B];   // lane k of the tile commits the impulse of the block's k-th step
+    // The owner of row r (lane r mod W, slot r / W: the owner of its w) keeps the row's impulse in a register during the sweeps.  Slots without
+    // a row read words of the environment block like a_own does; a step that fetches one is past its section's end, its update is forced to 0.
+    float lamo[S];
 #pragma unroll
-    for (int k = 0; k < B; ++k) writer[k] = lane == k;
-    // one block of B consecutive solver steps of section SEC, starting at position pos0 of the section
-    auto block = [&](int pos0, int it, auto sec_tag) {
+    for (int s = 0; s < S; ++s) lamo[s] = sLam[lane + s * W];
+    auto own = [&](const float (&v)[S], int i) -> float {   // row i's value of v, from its owner
+        float sel = v[0];
+#pragma unroll
+        for (int s = 1; s < S; ++s) if (i >= s * W) sel = v[s];
+        return T::shfl(sel, (S == 1) ? i : (i & (W - 1)));   // one row per lane: the row index is the owner's lane (the shuffle wraps indices past W itself)
+    };
+    // row indices of the block of B consecutive solver steps of section SEC that starts at position pos0 of the section
+    auto rows = [&](int pos0, int it, auto sec_tag, int (&ik)[B], bool (&vk)[B]) {
         constexpr int SEC = decltype(sec_tag)::value;
-        int ik[B], tk[B]; bool vk[B];
-        float tot = 0.f;
-        float wk[B], rhs[B], inv[B], lam[B], lo[B], hi[B], ain[B * (B - 1) / 2 > 0 ? B * (B - 1) / 2 : 1], ao[S][B];
         if (SEC == kSecLimit) {
 #pragma unroll
             for (int k = 0; k < B; ++k) { const int pos = pos0 + k; vk[k] = pos < NL; ik[k] = vk[k] ? ((it & 1) ? pos : NL - 1 - pos) : 0; }
         } else {
             // normals / friction rows are consecutive: one base index, immediate offsets.  Steps past the section's end (the other environment of
             // the warp has more rows, or an odd count) keep their natural index: they read initialised words of the environment block (zeroed
-            // at kernel start, see dm_step_kernel) and their update is forced to 0 below.
+            // at kernel start, see dm_step_kernel) and their update is forced to 0.
             const int i0 = ((SEC == kSecNormal) ? NL : NL + P) + pos0, cnt = (SEC == kSecNormal) ? P : 2 * P;
 #pragma unroll
             for (int k = 0; k < B; ++k) { ik[k] = i0 + k; vk[k] = pos0 + k < cnt; }
         }
+    };
+    // the impulses a block starts from, from their owners, and for friction the pair's normal impulse of this sweep (the two friction rows
+    // of a point are consecutive: one fetch per pair when B is even)
+    auto impulses = [&](int pos0, int it, auto sec_tag, float (&lam)[B], float (&tot)[B]) {
+        constexpr int SEC = decltype(sec_tag)::value;
+        int ik[B]; bool vk[B];
+        rows(pos0, it, sec_tag, ik, vk);
+#pragma unroll
+        for (int k = 0; k < B; ++k) {
+            lam[k] = own(lamo, ik[k]);
+            if (SEC == kSecFriction) tot[k] = ((B & 1) != 0 || (k & 1) == 0) ? own(lamo, NL + ((pos0 + k) >> 1)) : tot[k - 1];
+            else tot[k] = 0.f;
+        }
+    };
+    // one block of B consecutive solver steps of section SEC, starting at position pos0 of the section, from the impulses lam / tot.  Every
+    // operation on w, c, wk and the impulse is written out (__fmaf_rn / __fmul_rn / __fadd_rn / __fsub_rn): ptxas decides contraction from the
+    // distance between instructions, and these must round as the row-by-row sweep does whatever the schedule around them.
+    auto block = [&](int pos0, int it, auto sec_tag, const float (&lam)[B], const float (&tot)[B]) {
+        constexpr int SEC = decltype(sec_tag)::value;
+        int ik[B], tk[B]; bool vk[B];
+        float wk[B], rhs[B], inv[B], lo[B], hi[B], ain[B * (B - 1) / 2 > 0 ? B * (B - 1) / 2 : 1], ao[S][B];
+        rows(pos0, it, sec_tag, ik, vk);
 #pragma unroll
         for (int k = 0; k < B; ++k) tk[k] = (ST > 0) ? 0 : tri(ik[k]);
 #pragma unroll
         for (int k = 0; k < B; ++k) {
             const float2 ri = sRI[ik[k]];
-            rhs[k] = ri.x; inv[k] = ri.y; lam[k] = sLam[ik[k]];
+            rhs[k] = ri.x; inv[k] = ri.y;
             if (SEC == kSecFriction) {
-                // the point's normal impulse of this sweep; the two friction rows of a point are consecutive: one load per pair when B is even
-                if ((B & 1) != 0 || (k & 1) == 0) tot = sLam[NL + ((pos0 + k) >> 1)];
-                const bool on = tot > 0.f;
-                hi[k] = on ? mu * tot : lam[k]; lo[k] = on ? -hi[k] : lam[k];   // normal impulse not positive: the row is skipped
+                const bool on = tot[k] > 0.f;
+                hi[k] = on ? __fmul_rn(mu, tot[k]) : lam[k]; lo[k] = on ? -hi[k] : lam[k];   // normal impulse not positive: the row is skipped
             } else { lo[k] = 0.f; hi[k] = (SEC == kSecLimit) ? 100.f : 1e10f; }     // joint limits [0, 100], contact normals [0, inf)
         }
         {
@@ -250,34 +279,60 @@ __device__ __forceinline__ void pgs_sweeps(const float* sA, float* sLam, const f
 #pragma unroll
             for (int k = 0; k < B; ++k) ao[s][k] = a_own(s, ik[k], tk[k]);
 #pragma unroll
-        for (int k = 0; k < B; ++k) {
-            float sel = w[0];
-#pragma unroll
-            for (int s = 1; s < S; ++s) if (ik[k] >= s * W) sel = w[s];
-            wk[k] = T::shfl(sel, (S == 1) ? ik[k] : (ik[k] & (W - 1)));   // one row per lane: the row index is the owner's lane (the shuffle wraps indices past W itself)
-        }
+        for (int k = 0; k < B; ++k) wk[k] = own(w, ik[k]);
 #pragma unroll
         for (int k = 0; k < B; ++k) {
-            float c = fmaxf(fmaf(-inv[k], wk[k], rhs[k]), lo[k] - lam[k]);
-            if (SEC != kSecNormal) c = fminf(c, hi[k] - lam[k]);     // contact normals have no upper bound (Bullet: 1e10)
+            float c = fmaxf(__fmaf_rn(-inv[k], wk[k], rhs[k]), __fsub_rn(lo[k], lam[k]));
+            if (SEC != kSecNormal) c = fminf(c, __fsub_rn(hi[k], lam[k]));     // contact normals have no upper bound (Bullet: 1e10)
             c = vk[k] ? c : 0.f;
 #pragma unroll
-            for (int j = k + 1; j < B; ++j) wk[j] = fmaf(ain[j * (j - 1) / 2 + k], c, wk[j]);
-            if (vk[k] && writer[k]) sLam[ik[k]] = (SEC == kSecNormal) ? fmaxf(lam[k] + c, 0.f) : fminf(fmaxf(lam[k] + c, lo[k]), hi[k]);
+            for (int j = k + 1; j < B; ++j) wk[j] = __fmaf_rn(ain[j * (j - 1) / 2 + k], c, wk[j]);
+            const float l = (SEC == kSecNormal) ? fmaxf(__fadd_rn(lam[k], c), 0.f) : fminf(fmaxf(__fadd_rn(lam[k], c), lo[k]), hi[k]);
 #pragma unroll
-            for (int s = 0; s < S; ++s) w[s] = fmaf(ao[s][k], c, w[s]);
+            for (int s = 0; s < S; ++s) if (vk[k] && ik[k] == lane + s * W) lamo[s] = l;   // the owner keeps the new impulse
+#pragma unroll
+            for (int s = 0; s < S; ++s) w[s] = __fmaf_rn(ao[s][k], c, w[s]);
         }
-        __syncwarp();
+    };
+    // A section's blocks, two per iteration.  Within one section of one sweep no row is solved twice, so both blocks' impulses are fetched
+    // before the first block updates any, and nothing but the fetch of w orders the second block after the first.  The limit rows stay one
+    // block per iteration: pairing them as well measured slower (DESIGN.md section 9 has the measurements).
+    auto section = [&](int n, int it, auto sec_tag) {
+        constexpr int SEC = decltype(sec_tag)::value;
+        if (SEC == kSecLimit) {
+#pragma unroll 1
+            for (int p0 = 0; p0 < n; p0 += B) {
+                float l0[B], t0[B];
+                impulses(p0, it, sec_tag, l0, t0);
+                block(p0, it, sec_tag, l0, t0);
+            }
+            return;
+        }
+        int p0 = 0;
+#pragma unroll 1
+        for (; p0 + B < n; p0 += 2 * B) {
+            float l0[B], t0[B], l1[B], t1[B];
+            impulses(p0, it, sec_tag, l0, t0);
+            impulses(p0 + B, it, sec_tag, l1, t1);
+            block(p0, it, sec_tag, l0, t0);
+            block(p0 + B, it, sec_tag, l1, t1);
+        }
+        if (p0 < n) {   // an odd number of blocks: the last one alone
+            float l0[B], t0[B];
+            impulses(p0, it, sec_tag, l0, t0);
+            block(p0, it, sec_tag, l0, t0);
+        }
     };
 #pragma unroll 1
     for (int it = 0; it < 10; ++it) {
-#pragma unroll 1
-        for (int p0 = 0; p0 < NLmax; p0 += B) block(p0, it, std::integral_constant<int, kSecLimit>{});
-#pragma unroll 1
-        for (int p0 = 0; p0 < Pmax; p0 += B) block(p0, it, std::integral_constant<int, kSecNormal>{});
-#pragma unroll 1
-        for (int p0 = 0; p0 < 2 * Pmax; p0 += B) block(p0, it, std::integral_constant<int, kSecFriction>{});
+        section(NLmax, it, std::integral_constant<int, kSecLimit>{});
+        section(Pmax, it, std::integral_constant<int, kSecNormal>{});
+        section(2 * Pmax, it, std::integral_constant<int, kSecFriction>{});
     }
+    // the impulses go to shared memory once: the manifold write-back and z = Y^T lambda read them there
+#pragma unroll
+    for (int s = 0; s < S; ++s) { const int rid = lane + s * W; if (rid < NL + 3 * P) sLam[rid] = lamo[s]; }
+    __syncwarp();
 }
 
 // Constraint rows of one Bullet sub-step for the environment owned by this tile (warp-collective; both environments of a W = 16 warp
