@@ -125,6 +125,17 @@ struct BtMultiBody {
         int limitsDeep = 0;                // limit rows deeper than the split-impulse threshold (positional term dropped)
     };
     std::vector<RowTaps> dbg_rows;
+    // test tap: which branch of the link-plane collision each link took in each sub-step of the last stepSimulation call (no arithmetic)
+    enum { kEvNone = 0, kEvAdd = 1, kEvReplace = 2, kEvFull = 3 };
+    struct ContactTap {
+        int event = kEvNone;   // new point: none, added to a free slot, replaced the nearest cached point, inserted into a full cache
+        int slot = -1;         // slot written by the new point
+        int deepest = -1;      // full cache: the deepest slot sortCachedPoints kept out of the choice (-1: the new point is the deepest)
+        int rmDist = 0;        // refresh: 4-bit masks of the slots (as numbered when the refresh started) removed by distance ...
+        int rmDrift = 0;       // ... and by lateral drift of anchor B
+        int count = 0;         // points after the refresh
+    };
+    std::vector<std::vector<ContactTap>> dbg_contacts;
 
     void finalize() {
         int off = 0;
@@ -433,7 +444,7 @@ struct BtMultiBody {
         return sup + radius * vn;
     }
     // btPersistentManifold::sortCachedPoints (KEEP_DEEPEST_POINT, gContactCalcArea3Points = true)
-    static int sortCachedPoints(const BtManifold& m, const BtManifoldPoint& pt) {
+    static int sortCachedPoints(const BtManifold& m, const BtManifoldPoint& pt, int* deepest = nullptr) {
         int maxPenetrationIndex = -1;
         float maxPenetration = pt.distance1;
         for (int i = 0; i < 4; ++i) if (m.pt[i].distance1 < maxPenetration) { maxPenetrationIndex = i; maxPenetration = m.pt[i].distance1; }
@@ -445,6 +456,7 @@ struct BtMultiBody {
         if (maxPenetrationIndex != 3) res[3] = area(pt.localPointA - m.pt[0].localPointA, m.pt[2].localPointA - m.pt[1].localPointA);
         int best = -1; float bv = -1e18f;
         for (int i = 0; i < 4; ++i) if (std::fabs(res[i]) > bv) { bv = std::fabs(res[i]); best = i; }
+        if (deepest) *deepest = maxPenetrationIndex;
         return best;
     }
     // btConvexPlaneCollisionAlgorithm::processCollision (one new point per frame, numPerturbationIterations gated off)
@@ -452,6 +464,7 @@ struct BtMultiBody {
     void collideLinkPlane(int i) {
         BtLink& L = links[i];
         BtManifold& m = L.manifold;
+        ContactTap tap;
         const F3 n(0, 1, 0);
         F3 dirLocal = transpose(L.worldBasis) * (-n);
         F3 vtx = supportVertex(L, dirLocal);
@@ -480,11 +493,14 @@ struct BtMultiBody {
                     np.appliedImpulseLateral2 = m.pt[nearest].appliedImpulseLateral2;
                     np.lifeTime = m.pt[nearest].lifeTime;
                     m.pt[nearest] = np;
+                    tap.event = kEvReplace; tap.slot = nearest;
                 } else {  // addManifoldPoint
                     int idx = m.n;
-                    if (idx == 4) idx = sortCachedPoints(m, np); else m.n++;
+                    tap.event = kEvAdd;
+                    if (idx == 4) { idx = sortCachedPoints(m, np, &tap.deepest); tap.event = kEvFull; } else m.n++;
                     if (idx < 0) idx = 0;
                     m.pt[idx] = np;
+                    tap.slot = idx;
                 }
             }
         }
@@ -505,8 +521,13 @@ struct BtMultiBody {
                 F3 diff = p.positionWorldOnB - projectedPoint;
                 if (dot(diff, diff) > m.breakingThreshold * m.breakingThreshold) remove = true;
             }
-            if (remove) { int last = m.n - 1; if (k != last) m.pt[k] = m.pt[last]; m.n--; }
+            if (remove) {
+                (p.distance1 <= m.breakingThreshold ? tap.rmDrift : tap.rmDist) |= 1 << k;
+                int last = m.n - 1; if (k != last) m.pt[k] = m.pt[last]; m.n--;
+            }
         }
+        tap.count = m.n;
+        if (!dbg_contacts.empty()) dbg_contacts.back()[i] = tap;
     }
 
     // ------------------------------------------------------------------ constraint solve
@@ -635,6 +656,7 @@ struct BtMultiBody {
 
     // btDiscreteDynamicsWorld::internalSingleStepSimulation for one multibody (reference call site sim/World.cpp:93-104)
     void internalSingleStep(float h, const BtContactSolverInfo& base_info, float friction) {
+        dbg_contacts.emplace_back(n());
         for (int i = 0; i < n(); ++i) collideLinkPlane(i);          // performDiscreteCollisionDetection
         dbg_rows.emplace_back();
         computeAccelerationsABA(h);                                  // solveConstraints: ABA, v += a h
@@ -653,6 +675,7 @@ struct BtMultiBody {
         for (auto& L : links) L.appliedForce += L.mass * gravity;   // applyGravity (btMultiBodyDynamicsWorld)
         dbg_substep = 0;
         dbg_rows.clear();
+        dbg_contacts.clear();
         for (int s = 0; s < numSub; ++s) internalSingleStep(fixedTimeStep, info, friction);
         for (auto& L : links) { L.appliedForce = F3(); L.appliedTorque = F3(); L.jointTorque[0] = L.jointTorque[1] = L.jointTorque[2] = 0; }  // clearForces
     }

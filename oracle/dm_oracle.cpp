@@ -35,6 +35,7 @@ struct Oracle {
     std::vector<DQ> child_rot; std::vector<D3> child_pos;  // cSimBodyJoint::tParams::mChildRot / mChildPos
     DQ inv_root_attach_rot;
     BtMultiBody mb;
+    std::vector<float> snap_frames;   // test tap: each link's collider worldBasis (row-major) and worldPos as of the last SetSnapshot
     BtContactSolverInfo info;
     double friction = 0.9 * 0.9;  // link 0.9 (SimCharacter.cpp:26) x ground 0.9 (Ground.cpp:17)
     // ---- cImpPDController
@@ -1147,6 +1148,12 @@ struct Oracle {
             }
         }
         mb.updateCollisionObjectWorldTransforms();
+        snap_frames.assign(12 * nj, 0.0f);
+        for (int j = 0; j < nj; ++j) {
+            const BtLink& L = mb.links[j];
+            for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) snap_frames[12 * j + 3 * r + c] = L.worldBasis.m[r][c];
+            snap_frames[12 * j + 9] = L.worldPos.x; snap_frames[12 * j + 10] = L.worldPos.y; snap_frames[12 * j + 11] = L.worldPos.z;
+        }
         const double* q = s + 13 + 55 * nj;
         kin_time = q[0]; origin = D3(q[1], q[2], q[3]); origin_rot = DQ(q[4], q[5], q[6], q[7]);
         ctrl_time = q[8]; init_time_offset = q[9]; prev_action_time = q[10]; need_new_action = q[11] != 0; timer_time = q[12]; timer_max = q[13];
@@ -1307,6 +1314,25 @@ int dmo_last_rows(void* h, int* out, int max_substeps) {
         std::copy(v, v + 7, out + 7 * s);
     }
     return n;
+}
+// link-plane collision branches of each Bullet sub-step of the last Update: 6 ints per (sub-step, link) (event: 0 none / 1 add / 2 replace
+// nearest / 3 full-cache insert, slot written, deepest slot kept by sortCachedPoints or -1, mask of slots removed by distance, mask removed
+// by lateral drift, points after the refresh), at most max_substeps sub-steps; returns the number of sub-steps
+int dmo_last_contacts(void* h, int* out, int max_substeps) {
+    const auto& taps = static_cast<Oracle*>(h)->mb.dbg_contacts;
+    const int n = std::min(static_cast<int>(taps.size()), max_substeps);
+    for (int s = 0; s < n; ++s)
+        for (size_t i = 0; i < taps[s].size(); ++i) {
+            const auto& t = taps[s][i];
+            const int v[6] = {t.event, t.slot, t.deepest, t.rmDist, t.rmDrift, t.count};
+            std::copy(v, v + 6, out + 6 * (s * taps[s].size() + i));
+        }
+    return n;
+}
+// each link's collider frame as of the last set_snapshot: 12 doubles per link (worldBasis row-major, worldPos), scaled units
+void dmo_collider_frames(void* h, double* out) {
+    const auto& f = static_cast<Oracle*>(h)->snap_frames;
+    std::copy(f.begin(), f.end(), out);
 }
 void dmo_kin_frame(void* h, double time, double* pose, double* vel) { Oracle* o = static_cast<Oracle*>(h); orc::VecD p, v; o->KinCalcPose(time, p); o->KinCalcVel(time, v); std::copy(p.begin(), p.end(), pose); std::copy(v.begin(), v.end(), vel); }
 void dmo_body_state(void* h, double* pos, double* rot, double* linvel, double* angvel) {

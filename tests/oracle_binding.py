@@ -277,6 +277,21 @@ class Oracle:
         n = self.L.dmo_last_rows(self.h, out.ctypes.data_as(C.POINTER(C.c_int)), max_substeps)
         return out[:n].copy()
 
+    def last_contacts(self, max_substeps=8):
+        """branches of the link-plane collision per Bullet sub-step of the last update: int array [sub-steps, links, 6] of (event, slot written,
+        deepest slot kept out of a full cache or -1, mask of slots removed by distance, mask removed by lateral drift, points after the
+        refresh); events 0 none, 1 added to a free slot, 2 replaced the nearest cached point, 3 inserted into a full cache (sortCachedPoints);
+        removal masks number the slots as they were when the refresh started"""
+        out = np.zeros((max_substeps, self.num_joints, 6), dtype=np.int32)
+        n = self.L.dmo_last_contacts(self.h, out.ctypes.data_as(C.POINTER(C.c_int)), max_substeps)
+        return out[:n].copy()
+
+    def collider_frames(self):
+        """each link's collider frame as of the last set_snapshot: (worldBasis [links, 3, 3], worldPos [links, 3]), scaled units"""
+        out = np.zeros((self.num_joints, 12))
+        self.L.dmo_collider_frames(self.h, dp(out))
+        return out[:, :9].reshape(-1, 3, 3).copy(), out[:, 9:].copy()
+
     def bullet_aba(self, joint_tau, with_gravity=True):
         jt = np.ascontiguousarray(joint_tau, dtype=np.float32); out = np.zeros(self.num_dofs, dtype=np.float32)
         self.L.dmo_bullet_aba(self.h, fp(jt), 1 if with_gravity else 0, fp(out))
