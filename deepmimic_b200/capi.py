@@ -60,7 +60,7 @@ class DmLearnGatedBatch(C.Structure):
 DM_STATE_OFFSET, DM_STATE_SCALE, DM_ACTION_OFFSET, DM_ACTION_SCALE, DM_ACTION_BOUND_MIN, DM_ACTION_BOUND_MAX, DM_STATE_NORM_GROUPS = range(7)
 
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
-           "dm_update", "dm_set_pushes", "dm_get_pushes", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_record_pose", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
+           "dm_update", "dm_set_pushes", "dm_get_pushes", "dm_set_push_schedule", "dm_get_push_table", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_record_pose", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
            "dm_set_snapshot", "dm_state_size", "dm_save_state", "dm_load_state", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
            "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy", "dm_td_lambda_returns", "dm_mlp_set_weights_device", "dm_learn_create",
            "dm_mlp_set_normalizers_device", "dm_learn_set_weights", "dm_learn_step", "dm_learn_disc_step", "dm_learn_destroy",
@@ -101,6 +101,9 @@ def lib():
         if hasattr(L, "dm_set_pushes"):   # a library built before pushes (the base build of tools/ab_step.py) still loads; calling them fails
             L.dm_set_pushes.argtypes = [vp, C.POINTER(C.c_int32), fp, dp, dp]
             L.dm_get_pushes.argtypes = [vp, C.POINTER(C.c_int32)]
+        if hasattr(L, "dm_set_push_schedule"):   # likewise a library built before push schedules
+            L.dm_set_push_schedule.argtypes = [vp, C.POINTER(C.c_int32), C.c_int, dp, dp, dp]
+            L.dm_get_push_table.argtypes = [vp, C.POINTER(C.c_int32), fp, dp, dp]
         L.dm_plan_env_order.argtypes = [C.POINTER(C.c_int), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)]
         L.dm_get_env_order.argtypes = [vp, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.dm_record_state.argtypes = [vp, fp]
@@ -308,6 +311,36 @@ class BatchedCore:
         """dm_get_pushes: every environment's pending push body, int32 [N] (-1: none).  Synchronises the handle's stream."""
         out = np.zeros(self.num_envs, dtype=np.int32)
         self._chk(lib().dm_get_pushes(self.h, out.ctypes.data_as(C.POINTER(C.c_int32))))
+        return out
+
+    def set_push_schedule(self, bodies, force, duration, gap):
+        """dm_set_push_schedule: random pushes drawn on the device at every update() -- bodies (1 to 32 body ids drawn from), force, duration and
+        gap (lo, hi) of the magnitude in N, the push length in s and the time after the previous push in s.  The library refuses out-of-range
+        values by name.  Synchronises the handle's stream on the first call (allocation)."""
+        b = np.ascontiguousarray(np.asarray(bodies).reshape(-1))
+        if b.dtype.kind not in "iu":
+            raise ValueError("set_push_schedule: bodies must be integers, got %s" % b.dtype)
+        b = b.astype(np.int32)
+        pairs = []
+        for name, a in (("force", force), ("duration", duration), ("gap", gap)):
+            a = np.ascontiguousarray(a, dtype=np.float64)
+            if a.shape != (2,):
+                raise ValueError("set_push_schedule: %s must be a (lo, hi) pair, got shape %s" % (name, a.shape))
+            pairs.append(a)
+        f, d, g = pairs
+        self._chk(lib().dm_set_push_schedule(self.h, b.ctypes.data_as(C.POINTER(C.c_int32)), int(b.size), _dptr(f), _dptr(d), _dptr(g)))
+
+    def push_table(self, schedule=False):
+        """dm_get_push_table: every environment's push-table entry as dict(body [N] int32 (-1: none), force [N, 3] float32, start [N], duration
+        [N] float64) and, with schedule=True (handles with a push schedule only), sched [N, 3] float64: the schedule block (reset counter seen,
+        draw counter, last_end).  Synchronises the handle's stream."""
+        N = self.num_envs
+        body, force, window = np.zeros(N, dtype=np.int32), np.zeros((N, 3), dtype=np.float32), np.zeros((N, 2))
+        sched = np.zeros((N, 3)) if schedule else None
+        self._chk(lib().dm_get_push_table(self.h, body.ctypes.data_as(C.POINTER(C.c_int32)), C.c_void_p(force.ctypes.data), _dptr(window), _dptr(sched)))
+        out = dict(body=body, force=force, start=window[:, 0].copy(), duration=window[:, 1].copy())
+        if schedule:
+            out["sched"] = sched
         return out
 
     def set_env_order(self, on):

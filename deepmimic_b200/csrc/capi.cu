@@ -98,7 +98,9 @@ struct dm_handle {
     float *p_act = nullptr, *p_obs = nullptr, *p_rew = nullptr; int32_t* p_flags = nullptr;  // pinned host staging
     cudaStream_t stream = nullptr;
     int device = 0, num_envs = 0, padded_envs = 0, W = 32, tiles = 2, maxrows = 36, smem_bytes = 0, mode = 0;
-    dmk::DevPush* d_push = nullptr;   // push table (dm_set_pushes): null until the first call, then the step launches use the push instantiations
+    dmk::DevPush* d_push = nullptr;   // push table (dm_set_pushes, dm_set_push_schedule): null until the first call, then the step launches use the push instantiations
+    double* d_push_sched = nullptr;   // schedule block (dm_set_push_schedule): null on handles without a schedule; then d_push is the schedule's
+    dmk::PushSchedule push_sched{};
     int* d_order = nullptr;   // placement of the environments in the step kernel's tiles (dm_set_env_order); st.order is it or null
     dmk::StepLayout lay{};
     uint64_t seed = 0, env_offset = 0;
@@ -833,11 +835,25 @@ int dm_set_action(dm_handle* h, const float* d_actions) {
 }
 int dm_update(dm_handle* h, double dt, int n_updates) {
     DM_DEVICE(h);
+    if (h->d_push_sched) {   // the schedule refills the empty entries first, on the device: no host synchronisation
+        dmk::dm_push_schedule_kernel<<<(h->num_envs + 127) / 128, 128, 0, h->stream>>>(h->st, h->d_push, h->d_push_sched, h->push_sched);
+        if (launched(h)) return 1;
+    }
     return launch_step(h, dt, n_updates);
+}
+// the handle's push table, every entry empty (the padding environments never run: theirs stay empty)
+static int alloc_push_table(dm_handle* h) {
+    if (alloc_buffer(h, &h->d_push, static_cast<size_t>(h->padded_envs))) return 1;
+    std::vector<dmk::DevPush> none(static_cast<size_t>(h->padded_envs));
+    for (auto& p : none) { p.force[0] = p.force[1] = p.force[2] = 0.f; p.body = -1; p.start = 0.0; p.duration = 0.0; }
+    DM_CUDA(cudaMemcpyAsync(h->d_push, none.data(), none.size() * sizeof(dmk::DevPush), cudaMemcpyHostToDevice, h->stream));
+    DM_CUDA(cudaStreamSynchronize(h->stream));
+    return 0;
 }
 int dm_set_pushes(dm_handle* h, const int32_t* h_body, const float* h_force, const double* h_start, const double* h_duration) {
     DM_DEVICE(h);
     if (!h_body || !h_force || !h_start || !h_duration) { g_err = "dm_set_pushes: every array is required"; return fail(); }
+    if (h->d_push_sched) { g_err = "dm_set_pushes: the handle has a push schedule (dm_set_push_schedule), which owns its push table"; return fail(); }
     const int N = h->num_envs, nl = h->hm.nl;
     std::vector<dmk::DevPush> tab(static_cast<size_t>(N));
     for (int e = 0; e < N; ++e) {
@@ -850,15 +866,54 @@ int dm_set_pushes(dm_handle* h, const int32_t* h_body, const float* h_force, con
         p.force[0] = h_force[3 * e]; p.force[1] = h_force[3 * e + 1]; p.force[2] = h_force[3 * e + 2];
         p.body = h_body[e]; p.start = h_start[e]; p.duration = h_duration[e];
     }
-    if (h->d_push == nullptr) {   // the padding environments never run: their entries stay empty
-        if (alloc_buffer(h, &h->d_push, static_cast<size_t>(h->padded_envs))) return 1;
-        std::vector<dmk::DevPush> none(static_cast<size_t>(h->padded_envs));
-        for (auto& p : none) { p.force[0] = p.force[1] = p.force[2] = 0.f; p.body = -1; p.start = 0.0; p.duration = 0.0; }
-        DM_CUDA(cudaMemcpyAsync(h->d_push, none.data(), none.size() * sizeof(dmk::DevPush), cudaMemcpyHostToDevice, h->stream));
-        DM_CUDA(cudaStreamSynchronize(h->stream));
-    }
+    if (h->d_push == nullptr && alloc_push_table(h)) return 1;
     DM_CUDA(cudaMemcpyAsync(h->d_push, tab.data(), tab.size() * sizeof(dmk::DevPush), cudaMemcpyHostToDevice, h->stream));
     DM_CUDA(cudaStreamSynchronize(h->stream));   // the staging vector is pageable
+    return 0;
+}
+int dm_set_push_schedule(dm_handle* h, const int32_t* h_bodies, int n_bodies, const double* force2, const double* duration2, const double* gap2) {
+    DM_DEVICE(h);
+    auto refuse = [](const std::string& what) { g_err = "dm_set_push_schedule: " + what; return fail(); };
+    if (h->d_push && !h->d_push_sched) return refuse("the handle has pushes set by dm_set_pushes, which own its push table");
+    if (!h_bodies || !force2 || !duration2 || !gap2) return refuse("every array is required");
+    if (n_bodies < 1 || n_bodies > dmk::kMaxPushBodies) return refuse("n_bodies " + std::to_string(n_bodies) + " outside [1, 32]");
+    dmk::PushSchedule P;
+    std::memset(&P, 0, sizeof(P));   // padding included: the state header hashes the bytes
+    P.n_bodies = n_bodies;
+    for (int i = 0; i < n_bodies; ++i) {
+        if (h_bodies[i] < 0 || h_bodies[i] >= h->hm.nl)
+            return refuse("h_bodies[" + std::to_string(i) + "] = " + std::to_string(h_bodies[i]) + " outside [0, " + std::to_string(h->hm.nl) + ")");
+        P.bodies[i] = h_bodies[i];
+    }
+    const std::pair<const char*, const double*> bounds[3] = {{"force2", force2}, {"duration2", duration2}, {"gap2", gap2}};
+    for (const auto& b : bounds) {
+        const double lo = b.second[0], hi = b.second[1];
+        if (!std::isfinite(lo) || !std::isfinite(hi)) return refuse(std::string(b.first) + ": a bound is not finite");
+        if (lo < 0.0 || hi < 0.0) return refuse(std::string(b.first) + ": a bound is negative");
+        if (lo > hi) return refuse(std::string(b.first) + ": lo > hi");
+    }
+    for (int k = 0; k < 2; ++k) { P.force[k] = force2[k]; P.duration[k] = duration2[k]; P.gap[k] = gap2[k]; }
+    P.seed = h->seed ^ dmk::kPushSeedKey; P.env_base = h->env_offset;
+    if (h->d_push_sched == nullptr) {   // zeroed: reset counter 0 never matches a live environment's (dm_create's reset makes it 1)
+        if (alloc_push_table(h) || alloc_buffer(h, &h->d_push_sched, static_cast<size_t>(h->padded_envs) * dmk::kPushSchedDoubles, kZeroed)) return 1;
+    }
+    h->push_sched = P;
+    return 0;
+}
+int dm_get_push_table(dm_handle* h, int32_t* h_body, float* h_force, double* h_window, double* h_sched) {
+    DM_DEVICE(h);
+    if (h_sched && !h->d_push_sched) { g_err = "dm_get_push_table: the handle has no push schedule"; return fail(); }
+    const size_t N = static_cast<size_t>(h->num_envs);
+    std::vector<dmk::DevPush> tab(N);
+    for (auto& p : tab) { p.force[0] = p.force[1] = p.force[2] = 0.f; p.body = -1; p.start = 0.0; p.duration = 0.0; }
+    if (h->d_push) DM_CUDA(cudaMemcpyAsync(tab.data(), h->d_push, N * sizeof(dmk::DevPush), cudaMemcpyDeviceToHost, h->stream));
+    if (h_sched) DM_CUDA(cudaMemcpyAsync(h_sched, h->d_push_sched, N * dmk::kPushSchedDoubles * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    DM_CUDA(cudaStreamSynchronize(h->stream));
+    for (size_t e = 0; e < N; ++e) {
+        if (h_body) h_body[e] = tab[e].body;
+        if (h_force) for (int k = 0; k < 3; ++k) h_force[3 * e + k] = tab[e].force[k];
+        if (h_window) { h_window[2 * e] = tab[e].start; h_window[2 * e + 1] = tab[e].duration; }
+    }
     return 0;
 }
 int dm_get_pushes(dm_handle* h, int32_t* h_body) {
@@ -1284,7 +1339,8 @@ struct StateHeader {
     char scene[32];
     // host state that changes later results
     uint64_t amp_calls, expert_samples;
-    int32_t mode, pad2;
+    int32_t mode;
+    uint32_t push_schedule;   // 0: no push schedule; otherwise a hash of its parameters (push_schedule_hash), whose blocks end the blob
     double time_lim_min, time_lim_max;
 };
 struct StateBlock { void* dev; size_t bytes; };
@@ -1298,7 +1354,20 @@ std::vector<StateBlock> state_blocks(const dm_handle* h) {
                                  {s.hist, N * 2 * M.pose_dim * sizeof(float)}, {s.task, N * dmk::kTaskDoubles * sizeof(double)},
                                  {s.taskx, N * dmk::kTaskExtDoubles * sizeof(double)}, {s.clip, N * sizeof(int)}, {s.load, N * sizeof(int)}};
     b.erase(std::remove_if(b.begin(), b.end(), [](const StateBlock& x) { return x.dev == nullptr; }), b.end());
+    if (h->d_push_sched) {   // a push schedule: its push table and schedule block (manual dm_set_pushes tables are not part of the blob)
+        b.push_back({h->d_push, N * sizeof(dmk::DevPush)});
+        b.push_back({h->d_push_sched, N * dmk::kPushSchedDoubles * sizeof(double)});
+    }
     return b;
+}
+// the state header's push_schedule field: 0 without a schedule, else FNV-1a over its parameters folded to 32 bits and never 0
+uint32_t push_schedule_hash(const dm_handle* h) {
+    if (!h->d_push_sched) return 0;
+    const unsigned char* p = reinterpret_cast<const unsigned char*>(&h->push_sched);
+    uint64_t x = 1469598103934665603ull;
+    for (size_t i = 0; i < sizeof(h->push_sched); ++i) { x ^= p[i]; x *= 1099511628211ull; }
+    const uint32_t v = static_cast<uint32_t>(x ^ (x >> 32));
+    return v ? v : 1u;
 }
 // FNV-1a over the model blob with the fields that change at run time (time limits, mode) cleared: tells handles of different characters,
 // controllers or clips apart when every count matches
@@ -1323,7 +1392,7 @@ StateHeader state_header(const dm_handle* h) {
     H.goal_size = goal_size(M); H.amp_obs_size = M.amp_obs_size; H.num_clips = h->ctab.num_clips;
     H.seed = h->seed; H.env_offset = h->env_offset; H.model = model_hash(h);
     std::snprintf(H.scene, sizeof(H.scene), "%s", h->sa.cfg.scene.c_str());
-    H.amp_calls = h->amp_calls; H.expert_samples = h->expert_samples; H.mode = h->mode;
+    H.amp_calls = h->amp_calls; H.expert_samples = h->expert_samples; H.mode = h->mode; H.push_schedule = push_schedule_hash(h);
     H.time_lim_min = M.time_lim_min; H.time_lim_max = M.time_lim_max;
     return H;
 }
@@ -1336,7 +1405,7 @@ int dm_state_size(dm_handle* h, size_t* bytes) {
 }
 int dm_save_state(dm_handle* h, void* h_out) {
     DM_DEVICE(h);
-    if (h->d_push) {   // a pending push is not part of the state blob
+    if (h->d_push && !h->d_push_sched) {   // a pending push set by dm_set_pushes is not part of the state blob
         std::vector<int32_t> body(static_cast<size_t>(h->num_envs));
         if (dm_get_pushes(h, body.data())) return 1;
         for (int e = 0; e < h->num_envs; ++e)
@@ -1374,6 +1443,7 @@ int dm_load_state(dm_handle* h, const void* h_in) {
     if (in.seed != mine.seed) return refuse("seed");
     if (in.env_offset != mine.env_offset) return refuse("global env offset");
     if (in.model != mine.model) return refuse("model (character, controller or clips)");
+    if (in.push_schedule != mine.push_schedule) return refuse("push schedule (dm_set_push_schedule: none, or other parameters)");
     if (in.bytes != mine.bytes) return refuse("byte size");
     const char* p = static_cast<const char*>(h_in) + sizeof(in);
     for (const StateBlock& b : state_blocks(h)) {

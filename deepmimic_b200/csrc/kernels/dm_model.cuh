@@ -11,6 +11,7 @@
 
 #include "dm_math.cuh"
 
+#include "dm_push.cuh"
 #include "dm_task.cuh"
 #include "dm_task_ext.cuh"
 
@@ -120,22 +121,12 @@ __host__ __device__ inline int sim_stride(int nl) { return 16 + 12 * nl; }
 // TIME block, doubles: kin_time, ctrl_time, init_time_offset, prev_action_time, timer_time, timer_max, origin[3], origin_rot[4] (w,x,y,z)
 constexpr int kTimeDoubles = 16;
 enum TimeSlot { kTKin = 0, kTCtrl = 1, kTInitOff = 2, kTPrevAct = 3, kTTimer = 4, kTTimerMax = 5, kTOrigin = 6, kTOriginRot = 9 };
-// FLAG block, ints: need_new_action, done (sticky until reset), terminate, valid, fallen, overflow_rows
+// FLAG block, ints: need_new_action, done (sticky until reset), terminate, valid, fallen, overflow_rows, updates, resets (the reset counter)
 constexpr int kFlagInts = 8;
-enum FlagSlot { kFNeedAction = 0, kFDone = 1, kFTerminate = 2, kFValid = 3, kFFallen = 4, kFRowOverflow = 5, kFUpdates = 6 };
+enum FlagSlot { kFNeedAction = 0, kFDone = 1, kFTerminate = 2, kFValid = 3, kFFallen = 4, kFRowOverflow = 5, kFUpdates = 6, kFResets = 7 };
 // MANIFOLD block, floats: nl x 4 points x 12 = {valid, lAx,lAy,lAz, wBx,wBy,wBz, impN, impL1, impL2, dist, life}
 
-// A timed external force on one body (dm_set_pushes): force (world axes, unscaled N) at the body's COM in both Bullet sub-steps of every update
-// whose timer value at its start t satisfies start <= t < start + duration.  body -1: none; the step kernel sets it at the commit of the update
-// after which t >= start + duration, dm_reset at the environment's reset.  A handle's push table holds one entry per environment id (not tile
-// slot, so placement by contact load moves a push with its environment) and reaches dm_step_push_kernel as its last parameter, not as a
-// DevState field: a larger DevState would move every later parameter of every kernel that takes it.
-struct DevPush {
-    float force[3];
-    int body;
-    double start, duration;
-};
-static_assert(sizeof(DevPush) == 32, "DevPush: the step kernel reads force and body as one float4");
+// the push-table entry (DevPush) and the push schedule: dm_push.cuh
 
 struct DevState {
     float* sim;
@@ -222,6 +213,7 @@ constexpr int kPoseEnvsPerBlock = 8;   // dm_pose_kernel: kPoseEnvsPerBlock x li
 __global__ void dm_pose_kernel(const DevModel*, DevState, float*, float*, int);
 __global__ void dm_task_reset_kernel(const DevModel*, DevState, int);
 __global__ void dm_push_clear_kernel(DevState, DevPush*, int);
+__global__ void dm_push_schedule_kernel(DevState, DevPush*, double*, PushSchedule);
 __global__ void dm_task_observe_kernel(const DevModel*, DevState, float*, float*, int);
 int dm_step_layout(int nl, int n, int chain_len, int maxrows, int W, StepLayout* L);
 int dm_step_smem_bytes(const StepLayout& L, int tiles);

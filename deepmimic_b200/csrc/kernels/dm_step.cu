@@ -1757,6 +1757,17 @@ __global__ void dm_push_clear_kernel(DevState st, DevPush* push, int force) {
     if (force || st.flags[static_cast<size_t>(env) * kFlagInts + kFDone] != 0) push[env].body = -1;
 }
 
+// The push schedule (dm_push.cuh): refills the empty entries of the real environments that are not frozen.  Launched at the head of every
+// dm_update of a handle with a schedule; the step kernel and dm_push_clear_kernel empty the entries.
+__global__ void dm_push_schedule_kernel(DevState st, DevPush* push, double* sched, PushSchedule P) {
+    const int env = blockIdx.x * blockDim.x + threadIdx.x;
+    if (env >= st.num_real) return;
+    const int* fl = st.flags + static_cast<size_t>(env) * kFlagInts;
+    if (fl[kFDone] != 0) return;
+    push_schedule_env(P, P.env_base + static_cast<unsigned long long>(env), fl[kFResets], st.time[static_cast<size_t>(env) * kTimeDoubles + kTTimer],
+                      sched + static_cast<size_t>(env) * kPushSchedDoubles, push[env]);
+}
+
 // Placement of the environments for the next step-kernel launch (dm_model.cuh: env_load_bucket, env_order_slot).  One block of kEnvOrderThreads;
 // it runs between two step launches on the same stream, so its latency is what it costs: few barriers, no serial loop over the warps.
 //   * a histogram of the load buckets (one shared atomic per bucket present in a warp) gives each bucket's first rank;

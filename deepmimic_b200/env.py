@@ -58,6 +58,14 @@ class DeepMimicBatchEnv:
         self._pre()
         self._core.set_pushes(body, force, start, duration)
 
+    def set_push_schedule(self, bodies, force, duration, gap):
+        """Push the characters at random, for training under pushes: at every update() each running environment whose push has ended gets the
+        next one, on a body drawn from `bodies`, horizontal, of magnitude in force = (lo, hi) N, for duration = (lo, hi) s, starting gap = (lo,
+        hi) s after the end of the previous push of its episode.  The draws are made on the device from the env's seed and each environment's
+        global id (include/deepmimic_b200.h: dm_set_push_schedule); state_dict() carries them."""
+        self._pre()
+        self._core.set_push_schedule(bodies, force, duration, gap)
+
     def get_name(self):
         """cScene::GetName of the configured scene (SceneImitate.cpp:209, SceneImitateAMP.cpp:211, SceneTargetAMP.cpp:233, ...)"""
         return self._core.scene_name()

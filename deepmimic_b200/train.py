@@ -17,8 +17,15 @@ of a key), and so is --model_files: a reference TensorBundle prefix or a Trainer
 checkpoint records the model files, and --resume refuses a checkpoint of a run that started from other ones (or from none).  The log goes to <output_path>/agent0_log.txt and the checkpoint to <output_path>/agent0_checkpoint.pt (every OutputIters iterations
 and at the end); with --int_output_path, an intermediate checkpoint every IntOutputIters iterations goes to
 <int_output_path>/agent0_int_checkpoint_<iteration>.pt.  --resume continues a checkpoint of the same run (arguments, agent file, num_envs,
-window_steps, backend, seed), its log and its iteration numbering."""
+window_steps, backend, seed), its log and its iteration numbering.
+
+Training under pushes: --push_force LO,HI (N), --push_bodies B1[,B2...] (body ids), --push_duration LO,HI (s) and --push_interval LO,HI (s, the
+gap after the previous push), all four or none, push every training environment at random (DeepMimicBatchEnv.set_push_schedule): after each
+push its environment waits a gap drawn from the interval, then a body from the list is pushed horizontally with a magnitude and for a duration
+drawn from their ranges.  The evaluation (Test_Return) runs without pushes.  The schedule is part of the run record: --resume needs the same
+four options."""
 import argparse
+import math
 import os
 import re
 import sys
@@ -92,6 +99,42 @@ def resolve_model_files(scene_args, asset_root, prog="train"):
     return _resolve(asset_root, m) if m else None
 
 
+def parse_range(text):
+    """LO,HI: two finite numbers >= 0 with LO <= HI"""
+    try:
+        v = [float(x) for x in text.split(",")]
+    except ValueError:
+        v = []
+    if len(v) != 2 or not all(math.isfinite(x) and x >= 0.0 for x in v) or v[0] > v[1]:
+        raise argparse.ArgumentTypeError("need LO,HI: two finite numbers >= 0 with LO <= HI, got %r" % text)
+    return v
+
+
+def parse_bodies(text):
+    """B1[,B2...]: 1 to 32 body ids >= 0"""
+    try:
+        v = [int(x) for x in text.split(",")]
+    except ValueError:
+        v = []
+    if not 1 <= len(v) <= 32 or min(v) < 0:
+        raise argparse.ArgumentTypeError("need 1 to 32 comma-separated body ids >= 0, got %r" % text)
+    return v
+
+
+PUSH_OPTIONS = ("push_force", "push_bodies", "push_duration", "push_interval")
+
+
+def push_schedule(opts):
+    """the Trainer's push_schedule from the four push options: None without them; all four or none"""
+    given = [k for k in PUSH_OPTIONS if getattr(opts, k) is not None]
+    if not given:
+        return None
+    if len(given) != len(PUSH_OPTIONS):
+        raise SystemExit("train: --%s need each other: missing %s" % (", --".join(PUSH_OPTIONS),
+                                                                     ", ".join("--" + k for k in PUSH_OPTIONS if k not in given)))
+    return dict(bodies=opts.push_bodies, force=opts.push_force, duration=opts.push_duration, gap=opts.push_interval)
+
+
 def build_parser():
     ap = argparse.ArgumentParser(prog="python -m deepmimic_b200.train", description=__doc__.split("\n\n")[0], allow_abbrev=False)
     ap.add_argument("--asset_root", default=None, help="the reference's data / args tree (default: the bundled asset archive)")
@@ -102,6 +145,11 @@ def build_parser():
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--resume", default=None, help="a checkpoint of the same run to continue")
+    ap.add_argument("--push_force", type=parse_range, default=None, metavar="LO,HI", help="training under pushes: push magnitude range in N")
+    ap.add_argument("--push_bodies", type=parse_bodies, default=None, metavar="B1[,B2...]", help="training under pushes: the bodies pushed")
+    ap.add_argument("--push_duration", type=parse_range, default=None, metavar="LO,HI", help="training under pushes: push length range in s")
+    ap.add_argument("--push_interval", type=parse_range, default=None, metavar="LO,HI",
+                    help="training under pushes: range of the gap after an environment's previous push in s")
     return ap
 
 
@@ -118,6 +166,7 @@ def main(argv=None):
     from .sharding import rank_world
     from .trainer import AgentConfig, Trainer
     opts, scene_args = build_parser().parse_known_args(sys.argv[1:] if argv is None else argv)
+    pushes = push_schedule(opts)
     root = opts.asset_root or default_asset_root()
     agent_file, out_path, int_path = resolve_args(scene_args, root)
     model_files = resolve_model_files(scene_args, root)
@@ -136,7 +185,8 @@ def main(argv=None):
         os.makedirs(int_path, exist_ok=True)
     ckpt = rank_path(os.path.join(out_path, "agent0_checkpoint.pt"), rank)
     tr = Trainer(scene_args, cfg, root, opts.num_envs, window_steps=opts.window_steps, backend=opts.backend, seed=opts.seed, device=device,
-                 log_path=os.path.join(out_path, "agent0_log.txt"), append_log=opts.resume is not None, process_group=group, model_files=model_files)
+                 log_path=os.path.join(out_path, "agent0_log.txt"), append_log=opts.resume is not None, process_group=group, model_files=model_files,
+                 push_schedule=pushes)
     if opts.resume:
         tr.load(rank_path(opts.resume, rank))
     try:

@@ -252,6 +252,23 @@ def _store_rows(buf, rows):
 
 
 _NORM_FIELDS = ("mean", "mean_sq", "std", "new_sum", "new_sum_sq")
+PUSH_SCHEDULE_KEYS = ("bodies", "force", "duration", "gap")
+
+
+def push_schedule_record(ps):
+    """a push schedule dict(bodies, force, duration, gap) in the run record's form: bodies a list of ints, the other three [lo, hi] lists of
+    floats.  Only the form is checked here; the library refuses out-of-range values by name (DeepMimicBatchEnv.set_push_schedule)."""
+    if ps is None:
+        return None
+    if not isinstance(ps, dict) or set(ps) != set(PUSH_SCHEDULE_KEYS):
+        raise ValueError("push_schedule: a dict with exactly the keys %s expected" % ", ".join(PUSH_SCHEDULE_KEYS))
+    out = dict(bodies=[int(b) for b in ps["bodies"]])
+    for k in PUSH_SCHEDULE_KEYS[1:]:
+        v = [float(x) for x in ps[k]]
+        if len(v) != 2:
+            raise ValueError("push_schedule: %s must be a (lo, hi) pair" % k)
+        out[k] = v
+    return out
 
 
 class Trainer:
@@ -275,6 +292,10 @@ class Trainer:
     step counts (tools/train_time.py counts them).  With a process group of more than one rank, each PPO update adds one (the learners' check
     that every rank's window has the same size).
 
+    push_schedule (train --push_force etc.): dict(bodies, force, duration, gap) of DeepMimicBatchEnv.set_push_schedule, applied to the training
+    handle only (Test_Return stays an evaluation without pushes).  It joins the run record, so a checkpoint resumes only with the same schedule;
+    the training handle's state blob carries the pushes drawn so far.
+
     Several GPUs (mpi_run.py --num_workers N): process_group, a torch.distributed group of one rank per GPU.  num_envs is the job's total, which
     must be divisible by the world size; each rank steps its contiguous share (global_env_offset = rank * num_envs / world, so every
     environment's reset stream is the one it has on one GPU), and evaluates ceil(TestEpisodes / world) episodes.  The learners average the
@@ -286,7 +307,7 @@ class Trainer:
     world size and the state its rank, both of which load_state_dict() requires to match."""
 
     def __init__(self, args, config, asset_root, num_envs, window_steps=32, backend="tensor_core", seed=0, device=0, log_path=None, append_log=False,
-                 env=None, test_env=None, process_group=None, model_files=None):
+                 env=None, test_env=None, process_group=None, model_files=None, push_schedule=None):
         import torch
         from .env import DeepMimicBatchEnv
         from .learner import AMPDiscLearner, DataParallel, PPOLearner
@@ -307,11 +328,16 @@ class Trainer:
         # what a checkpoint must match
         self.run = dict(args=self.args, agent=config.values, num_envs=int(num_envs), window_steps=self.window_steps, backend=backend, seed=self.seed,
                         world=self.world, model_files=model_files)
+        push_schedule = push_schedule_record(push_schedule)
+        if push_schedule is not None:   # runs without a schedule keep the record they had
+            self.run["push_schedule"] = push_schedule
         rs = self.seed + 1000 * self.rank   # the rank's generators
         cfg = config
         self.env = env = env or DeepMimicBatchEnv(self.args, local, asset_root, device=device, seed=self.seed, global_env_offset=self.rank * local)
         if env.num_envs != local:
             raise ValueError("env has %d environments; this rank's share of num_envs is %d" % (env.num_envs, local))
+        if push_schedule is not None:
+            env.set_push_schedule(**push_schedule)
         S, A, G = env.get_state_size(), env.get_action_size(), env.get_goal_size()
         net = NETS[1] if G > 0 else NETS[0]
         for key in ("ActorNet", "CriticNet"):
@@ -521,6 +547,9 @@ class Trainer:
         if s["run"].get("model_files") != self.run["model_files"]:   # a checkpoint without the key is a run from random initialisation
             raise ValueError("checkpoint: its run started from model files %s, this one from %s: resume with the arguments the run started with, "
                              "--model_files included" % (s["run"].get("model_files"), self.run["model_files"]))
+        if s["run"].get("push_schedule") != self.run.get("push_schedule"):   # a checkpoint without the key is a run without pushes
+            raise ValueError("checkpoint: its run trained under the push schedule %s, this one under %s: resume with the push options the run "
+                             "started with" % (s["run"].get("push_schedule"), self.run.get("push_schedule")))
         for k in self.run:
             if s["run"].get(k, 1 if k == "world" else None) != self.run[k]:   # a checkpoint without a world size is a one-rank run's
                 raise ValueError("checkpoint: its %s differs from this run's" % ("agent file" if k == "agent" else "world size" if k == "world" else k))

@@ -111,6 +111,23 @@ int dm_update(dm_handle* h, double dt, int n_updates);
  * dm_save_state refuses a handle with a pending push; dm_load_state leaves the push table as it is. */
 int dm_set_pushes(dm_handle* h, const int32_t* h_body, const float* h_force, const double* h_start, const double* h_duration);
 int dm_get_pushes(dm_handle* h, int32_t* h_body);
+/* Random pushes for training: a schedule drawn on the device refills every environment's push-table entry (same push semantics as above).
+ * h_bodies [n_bodies] (1 to 32 body ids in [0, links)) are the bodies drawn from; force2, duration2 and gap2 are {lo, hi} of the magnitude
+ * (N), the duration (s) and the gap after the previous push (s): finite, >= 0, lo <= hi.  At the head of every dm_update a kernel runs, for each
+ * real environment whose done flag is clear: when its reset counter has moved since it last ran there, a new episode (draw counter k = 0,
+ * last_end = 0); when its entry is empty, five uniforms u = splitmix64(seed ^ "pushes", global env id, k++) in the order gap, body index,
+ * magnitude, direction angle a in [0, 2 pi), duration, and the entry becomes body, force (F cos a, 0, F sin a), start = max(last_end + gap,
+ * t) with t the episode timer now (a start already passed moves to t), and that duration; last_end = start + duration.  A given global
+ * environment gets the same pushes at any GPU count.  The first call allocates the push table and a schedule block of 3 doubles per environment
+ * (reset counter seen, k, last_end) and switches the step launches to the push instantiations; later calls replace the parameters.  No host
+ * synchronisation per dm_update.  Refused, naming the argument: a body outside [0, links), n_bodies outside [1, 32], a bound that is not
+ * finite, negative or with lo > hi, a host-only handle, and a handle with dm_set_pushes tables (dm_set_pushes refuses a scheduled handle).
+ * dm_save_state / dm_load_state carry the push table and the schedule block of a scheduled handle; the header's push_schedule field makes a
+ * load refuse a blob of a handle with another schedule or none, and the reverse.  Handles without a schedule keep the blob as it was.
+ * dm_get_push_table: every environment's entry, body [N], force [N x 3], window [N x 2] (start, duration), and the schedule block [N x 3]
+ * (NULL on a handle without a schedule); any pointer may be NULL; synchronises the stream. */
+int dm_set_push_schedule(dm_handle* h, const int32_t* h_bodies, int n_bodies, const double* force2, const double* duration2, const double* gap2);
+int dm_get_push_table(dm_handle* h, int32_t* h_body, float* h_force, double* h_window, double* h_sched);
 /* Placement of the environments in the step kernel (on by default; tile width 16 only, where two environments share a warp: tile width 32
  * handles keep index placement, where it measured slower): every step launch is preceded by a one-block kernel that orders the
  * environments by contact load -- the solver row count of each environment's last Bullet sub-step, its key -- so that environments of equal
