@@ -59,8 +59,12 @@ class DmLearnGatedBatch(C.Structure):
 
 DM_STATE_OFFSET, DM_STATE_SCALE, DM_ACTION_OFFSET, DM_ACTION_SCALE, DM_ACTION_BOUND_MIN, DM_ACTION_BOUND_MAX, DM_STATE_NORM_GROUPS = range(7)
 
+class DmCamera(C.Structure):
+    _fields_ = [("yaw", C.c_float), ("pitch", C.c_float), ("distance", C.c_float), ("target_height", C.c_float), ("fov_y", C.c_float)]
+
+
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
-           "dm_update", "dm_set_pushes", "dm_get_pushes", "dm_set_push_schedule", "dm_get_push_table", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_record_pose", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
+           "dm_update", "dm_set_pushes", "dm_get_pushes", "dm_set_push_schedule", "dm_get_push_table", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_record_pose", "dm_render_poses", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
            "dm_set_snapshot", "dm_state_size", "dm_save_state", "dm_load_state", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
            "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy", "dm_td_lambda_returns", "dm_mlp_set_weights_device", "dm_learn_create",
            "dm_mlp_set_normalizers_device", "dm_learn_set_weights", "dm_learn_step", "dm_learn_disc_step", "dm_learn_destroy",
@@ -104,6 +108,8 @@ def lib():
         if hasattr(L, "dm_set_push_schedule"):   # likewise a library built before push schedules
             L.dm_set_push_schedule.argtypes = [vp, C.POINTER(C.c_int32), C.c_int, dp, dp, dp]
             L.dm_get_push_table.argtypes = [vp, C.POINTER(C.c_int32), fp, dp, dp]
+        if hasattr(L, "dm_render_poses"):   # likewise a library built before the renderer
+            L.dm_render_poses.argtypes = [vp, C.c_int, C.c_void_p, C.POINTER(DmCamera), C.c_int, C.c_int, C.c_void_p, C.c_void_p]
         L.dm_plan_env_order.argtypes = [C.POINTER(C.c_int), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)]
         L.dm_get_env_order.argtypes = [vp, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.dm_record_state.argtypes = [vp, fp]
@@ -189,6 +195,19 @@ def _check_device_f32(t, what, shape=None, device=None):
                          else "%s %s on %s%s" % (t.dtype, tuple(t.shape), t.device, "" if t.is_contiguous() else ", not contiguous")))
 
 
+# the renderer's default view: from the front-right, a little above the pelvis, 45 degrees vertical field of view
+DEFAULT_CAMERA = dict(yaw=0.6, pitch=0.25, distance=4.0, target_height=0.9, fov_y=0.7853981633974483)
+
+
+def camera_struct(camera=None):
+    """dm_camera of a dict with the keys of DEFAULT_CAMERA (missing keys take its values), or of DEFAULT_CAMERA for None"""
+    c = dict(DEFAULT_CAMERA, **(camera or {}))
+    unknown = set(c) - set(DEFAULT_CAMERA)
+    if unknown:
+        raise ValueError("camera: unknown keys %s" % sorted(unknown))
+    return DmCamera(*(float(c[k]) for k in ("yaw", "pitch", "distance", "target_height", "fov_y")))
+
+
 def _dptr(a):
     return a.ctypes.data_as(C.POINTER(C.c_double)) if a is not None else None
 
@@ -241,6 +260,7 @@ class BatchedCore:
         L.dm_get_dims(self.h, C.byref(d))
         self.dims = d
         self.num_envs = d.num_envs
+        self.device = device
 
     def _chk(self, rc):
         if rc != 0:
@@ -369,6 +389,33 @@ class BatchedCore:
                 _check_device_f32(t, "record_pose: " + name, (self.num_envs, P))
         self._chk(lib().dm_record_pose(self.h, C.c_void_p(pose.data_ptr()) if pose is not None else None,
                                        C.c_void_p(vel.data_ptr()) if vel is not None else None))
+
+    def render_poses(self, pose, camera=None, width=640, height=360, rgb=None, ids=None):
+        """dm_render_poses: pose rows [V, pose_dim] (a contiguous float32 tensor on the handle's device, dm_record_pose's layout) drawn as this handle's
+        character by the device ray caster, seen from `camera` (a dict of yaw, pitch, distance, target_height, fov_y in radians and metres;
+        missing keys and None: DEFAULT_CAMERA).  Returns (rgb uint8 [V, height, width, 3], ids int16 [V, height, width]: -1 sky, -2 ground, k link
+        k); pass rgb / ids tensors to fill them in place, or False to skip that output.  Stream-ordered on the handle's stream."""
+        import torch
+        P = self.dims.pose_dim
+        if pose.dim() != 2 or pose.shape[1] != P:
+            raise ValueError("render_poses: pose must be [V, %d], got %s" % (P, tuple(pose.shape)))
+        dev = torch.device("cuda", self.device)
+        _check_device_f32(pose, "render_poses: pose", device=dev)
+        V = pose.shape[0]
+        outs = []
+        for name, t, dt, shape in (("rgb", rgb, torch.uint8, (V, height, width, 3)), ("ids", ids, torch.int16, (V, height, width))):
+            if t is False:
+                outs.append(None)
+                continue
+            if t is None:
+                t = torch.empty(shape, dtype=dt, device=dev)
+            elif (not isinstance(t, torch.Tensor) or t.dtype != dt or tuple(t.shape) != shape or t.device != dev or not t.is_contiguous()):
+                raise ValueError("render_poses: %s must be a contiguous %s tensor of shape %s on %s" % (name, dt, shape, dev))
+            outs.append(t)
+        cam = camera_struct(camera)
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+        self._chk(lib().dm_render_poses(self.h, V, ptr(pose), C.byref(cam), int(width), int(height), ptr(outs[0]), ptr(outs[1])))
+        return outs[0], outs[1]
 
     def reward_imitate(self, out):  # torch float32 cuda tensor [N]: CalcRewardImitate also in the task scenes (active clip of the dataset)
         self._chk(lib().dm_calc_reward_imitate(self.h, C.c_void_p(out.data_ptr())))

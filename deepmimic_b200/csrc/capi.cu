@@ -21,6 +21,7 @@
 #include "../../include/deepmimic_b200.h"
 #include "host/assets.hpp"
 #include "kernels/dm_model.cuh"
+#include "kernels/dm_render.cuh"
 
 namespace dmk {
 __global__ void dm_flags_kernel(DevState st, int32_t* out, int num_real_envs) {
@@ -970,6 +971,36 @@ int dm_record_pose(dm_handle* h, float* d_pose, float* d_vel) {
     DM_DEVICE(h);
     if (d_pose == nullptr && d_vel == nullptr) return 0;
     return launch_pose(h, d_pose, d_vel);
+}
+int dm_render_poses(dm_handle* h, int n_views, const float* d_pose, const dm_camera* cam, int width, int height, uint8_t* d_rgb, int16_t* d_ids) {
+    DM_DEVICE(h);
+    auto refuse = [](const std::string& what) { g_err = "dm_render_poses: " + what; return fail(); };
+    if (n_views < 1 || n_views > 65535) return refuse("n_views " + std::to_string(n_views) + " outside [1, 65535]");
+    if (width < 16 || width > 4096) return refuse("width " + std::to_string(width) + " outside [16, 4096]");
+    if (height < 16 || height > 4096) return refuse("height " + std::to_string(height) + " outside [16, 4096]");
+    if (d_pose == nullptr) return refuse("d_pose is NULL");
+    if (d_rgb == nullptr && d_ids == nullptr) return refuse("d_rgb and d_ids are both NULL");
+    if (cam == nullptr) return refuse("cam is NULL");
+    const char* names[5] = {"yaw", "pitch", "distance", "target_height", "fov_y"};
+    const float vals[5] = {cam->yaw, cam->pitch, cam->distance, cam->target_height, cam->fov_y};
+    for (int k = 0; k < 5; ++k)
+        if (!std::isfinite(vals[k])) return refuse(std::string("camera ") + names[k] + " is not finite");
+    if (!(cam->distance > 0.f)) return refuse("camera distance " + std::to_string(cam->distance) + " <= 0");
+    if (!(cam->fov_y > 0.f && cam->fov_y < static_cast<float>(M_PI))) return refuse("camera fov_y " + std::to_string(cam->fov_y) + " outside (0, pi)");
+    // the camera basis in double: fwd from the eye to the target, right = fwd x up normalised (cos yaw, 0, -sin yaw), up = right x fwd
+    const double cy = std::cos(cam->yaw), sy = std::sin(cam->yaw), cp = std::cos(cam->pitch), sp = std::sin(cam->pitch);
+    const V3 back(cp * sy, sp, cp * cy), right(cy, 0.0, -sy);
+    const V3 fwd = -1.0 * back, up(right.y * fwd.z - right.z * fwd.y, right.z * fwd.x - right.x * fwd.z, right.x * fwd.y - right.y * fwd.x);
+    dmk::RenderCam rc;
+    put3(rc.back, back, cam->distance); put3(rc.fwd, fwd); put3(rc.right, right); put3(rc.up, up);
+    rc.tan_y = static_cast<float>(std::tan(0.5 * cam->fov_y));
+    rc.tan_x = static_cast<float>(std::tan(0.5 * cam->fov_y) * width / height);
+    rc.target_height = cam->target_height;
+    const int T = dmk::kRenderTile;
+    const dim3 grid(((width + T - 1) / T) * ((height + T - 1) / T), n_views);
+    dmk::dm_render_kernel<<<grid, T * T, 0, h->stream>>>(h->d_model, d_pose, width, height, rc, d_rgb, d_ids);
+    DM_CUDA(cudaGetLastError());
+    return 0;
 }
 // cSceneImitate::CalcRewardImitate in every scene: in the AMP task scenes (where CalcReward is the task reward) against the environment's
 // active clip of the dataset -- BASELINE.json config 5 records it beside the AMP observations.

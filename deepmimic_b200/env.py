@@ -136,6 +136,22 @@ class DeepMimicBatchEnv:
         self._post()
         return self._pose, self._vel
 
+    def render(self, env_ids=None, **kw):
+        """(rgb uint8 [V, H, W, 3], ids int16 [V, H, W]) device tensors: the current simulated characters of env_ids (default all; a sequence
+        or tensor of environment indices) drawn by the device ray caster from their record_pose rows; keyword arguments are
+        BatchedCore.render_poses' (camera, width, height, rgb, ids).  Ordered on the caller's stream like record_state, no host
+        synchronisation (host indices go to the device through pinned memory); the simulation state is not touched."""
+        pose, _ = self.record_pose()
+        if env_ids is not None:
+            idx = self.torch.as_tensor(env_ids, dtype=self.torch.long)
+            if not idx.is_cuda:
+                idx = idx.pin_memory()
+            pose = pose[idx.to(self.device, non_blocking=True)].contiguous()
+        self._pre()
+        out = self._core.render_poses(pose, **kw)
+        self._post()
+        return out
+
     def set_action(self, agent_id_or_actions, actions=None):
         a = agent_id_or_actions if actions is None else actions
         if tuple(a.shape) != (self.num_envs, self.get_action_size()) or a.dtype != self.torch.float32 or not a.is_cuda:

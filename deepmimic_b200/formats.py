@@ -4,10 +4,15 @@ the reference and files produced by the reference load here.  Pure host code, no
   motion clip    cMotion::Output / LoadJson           R/DeepMimicCore/anim/Motion.cpp:104-141,303-360,581-646
   state snapshot cCharacter::WriteState / ReadState   R/DeepMimicCore/anim/Character.cpp:320-385,434-443
   training log   Logger.log_tabular / dump_tabular    R/util/logger.py:63-127 (fixed-width 25-character columns)
+  animated PNG   the APNG extension of PNG (acTL / fcTL / fdAT chunks): rendered episodes and motion files (deepmimic_b200/render.py)
 
 The BVH importer (R/DeepMimicCore/util/BVHReader.cpp) is deepmimic_b200/bvh.py."""
+import binascii
 import json
 import re
+import struct
+import zlib
+from fractions import Fraction
 
 import numpy as np
 
@@ -111,3 +116,42 @@ def read_table_log(path):
             except ValueError:
                 cols[h].append(float("nan"))
     return {h: np.asarray(v) for h, v in cols.items()}
+
+
+def _png_chunk(kind, data):
+    return struct.pack(">I", len(data)) + kind + data + struct.pack(">I", binascii.crc32(kind + data) & 0xFFFFFFFF)
+
+
+def write_apng(path, frames, durations):
+    """An animated PNG of T RGB frames: frames is a uint8 array [T, H, W, 3] or an iterable of T [H, W, 3] arrays (consumed one frame at a
+    time), durations the T frame delays in seconds.  Frame 0 is also the default image (IDAT), so a viewer without APNG support shows it;
+    every frame has its own fcTL delay, the nearest fraction with a 16-bit denominator; the animation loops.  Pixels are stored losslessly."""
+    durations = [float(d) for d in durations]
+    if not durations or any(not (d >= 0.0) or d == float("inf") for d in durations):
+        raise ValueError("write_apng: need one finite duration >= 0 per frame")
+    with open(path, "wb") as f:
+        n, shape = 0, None
+        for frame in frames:
+            frame = np.asarray(frame)
+            if frame.dtype != np.uint8 or frame.ndim != 3 or frame.shape[2] != 3 or (shape is not None and frame.shape != shape):
+                raise ValueError("write_apng: every frame must be uint8 [H, W, 3] of one size, got %s %s" % (frame.dtype, frame.shape))
+            if n >= len(durations):
+                raise ValueError("write_apng: more frames than durations")
+            H, W = frame.shape[:2]
+            if n == 0:
+                shape = frame.shape
+                f.write(b"\x89PNG\r\n\x1a\n")
+                f.write(_png_chunk(b"IHDR", struct.pack(">IIBBBBB", W, H, 8, 2, 0, 0, 0)))
+                f.write(_png_chunk(b"acTL", struct.pack(">II", len(durations), 0)))
+            delay = Fraction(durations[n]).limit_denominator(65535)
+            if delay.numerator > 65535:
+                raise ValueError("write_apng: a frame duration of %g s does not fit a 16-bit delay" % durations[n])
+            seq = 0 if n == 0 else 2 * n - 1   # fcTL and fdAT chunks share one sequence: fcTL 0, (fcTL 1, fdAT 2), (fcTL 3, fdAT 4), ...
+            f.write(_png_chunk(b"fcTL", struct.pack(">IIIIIHHBB", seq, W, H, 0, 0, delay.numerator, delay.denominator, 0, 0)))
+            rows = np.concatenate([np.zeros((H, 1), dtype=np.uint8), frame.reshape(H, 3 * W)], axis=1)   # filter type 0 on every row
+            data = zlib.compress(rows.tobytes(), 6)
+            f.write(_png_chunk(b"IDAT", data) if n == 0 else _png_chunk(b"fdAT", struct.pack(">I", seq + 1) + data))
+            n += 1
+        if n != len(durations):
+            raise ValueError("write_apng: %d frames for %d durations" % (n, len(durations)))
+        f.write(_png_chunk(b"IEND", b""))

@@ -1,7 +1,7 @@
 """Run a trained skill: the counterpart of the reference's `DeepMimic.py --arg_file args/run_*_args.txt`, without the viewer.
 
     python -m deepmimic_b200.run --arg_file args/run_humanoid3d_spinkick_args.txt [--model_files PATH] [--num_envs 64]
-        [--record_motion K] [--episode_time 20] [--backend tensor_core] [--seed 0] [--device 0] [--asset_root DIR]
+        [--record_motion K] [--render K [--render_size WxH] [--camera yaw,pitch,distance,height,fov_deg]] [--episode_time 20] [--backend tensor_core] [--seed 0] [--device 0] [--asset_root DIR]
         [--push_forces F1,F2,... [--push_body 0] [--push_time 2.0] [--push_duration 0.2]] [reference arguments ...]
 
 --model_files (a reference TensorBundle prefix or a Trainer checkpoint, deepmimic_b200/model_files.py) and --output_path are read from the
@@ -13,6 +13,8 @@ arg files: the reference's viewer runs until the character falls), an episode en
   run_log.txt          one row per environment: its return, its length in policy steps and its terminate code (0 time limit, 1 fail, 2 success)
   motion_<env>.txt     with --record_motion K, the first K environments' episodes as motion files (cMotion::Output, loop "none", one frame per
                        policy step and the terminal pose)
+  render_<env>.png     with --render K, the first K environments' episodes as animated PNGs drawn by the device ray caster from the same
+                       frames, each shown for one policy step (deepmimic_b200/render.py: --render_size, default 640x360, and --camera)
 and a printed summary: the return's mean and standard deviation, the mean length and the fraction of episodes ended by Fail.  One GPU only.
 
 Push robustness (--push_forces, the DeepMimic paper's test of a trained skill): environment e is pushed on body --push_body (default the root)
@@ -24,6 +26,7 @@ import argparse
 import os
 import sys
 
+from .render import add_view_options
 from .train import arg_table, first_arg, resolve_model_files
 
 
@@ -32,6 +35,8 @@ def build_parser():
     ap.add_argument("--asset_root", default=None, help="the reference's data / args tree (default: the bundled asset archive)")
     ap.add_argument("--num_envs", type=int, default=64, help="environments, one episode each")
     ap.add_argument("--record_motion", type=int, default=0, metavar="K", help="write the first K environments' episodes as motion files")
+    ap.add_argument("--render", type=int, default=0, metavar="K", help="write the first K environments' episodes as animated PNGs")
+    add_view_options(ap)
     ap.add_argument("--backend", default="tensor_core", choices=("tensor_core", "torch"))
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--device", type=int, default=0)
@@ -78,6 +83,20 @@ def write_episode_motions(path_fmt, ep, count, frame_dur):
     return paths
 
 
+def write_episode_renders(path_fmt, ep, count, frame_dur, core, camera=None, size=(640, 360)):
+    """animated PNGs of the first `count` environments of run_episodes(pose_envs >= count)'s result `ep`, the frames of write_episode_motions
+    drawn as core's character: path_fmt % env; returns the paths"""
+    from .render import write_pose_apng
+    from .rollout import episode_motion
+    lengths = ep["lengths"].cpu().tolist()
+    paths = []
+    for e in range(count):
+        frames = episode_motion(ep["poses"], ep["end_poses"], e, int(lengths[e]))
+        write_pose_apng(core, path_fmt % e, frames, [frame_dur] * frames.shape[0], camera, size)
+        paths.append(path_fmt % e)
+    return paths
+
+
 def main(argv=None):
     import numpy as np
     from .assets import asset_root as default_asset_root
@@ -85,8 +104,8 @@ def main(argv=None):
     opts, scene_args = build_parser().parse_known_args(sys.argv[1:] if argv is None else argv)
     if rank_world()[1] > 1:
         raise SystemExit("run: one GPU only; start it without torchrun")
-    if opts.num_envs < 1 or not 0 <= opts.record_motion <= opts.num_envs:
-        raise SystemExit("run: need --num_envs >= 1 and 0 <= --record_motion <= --num_envs")
+    if opts.num_envs < 1 or not 0 <= opts.record_motion <= opts.num_envs or not 0 <= opts.render <= opts.num_envs:
+        raise SystemExit("run: need --num_envs >= 1, 0 <= --record_motion <= --num_envs and 0 <= --render <= --num_envs")
     if opts.push_forces is not None and not (opts.push_duration >= 0.0 and np.isfinite(opts.push_duration) and np.isfinite(opts.push_time)):
         raise SystemExit("run: need a finite --push_time and a finite --push_duration >= 0")
     root = opts.asset_root or default_asset_root()
@@ -121,7 +140,7 @@ def main(argv=None):
         load_model_files(model_files, ro.policy, norms)
     except ValueError as e:
         raise SystemExit("run: %s" % e)
-    ep = run_episodes(ro, pose_envs=opts.record_motion)
+    ep = run_episodes(ro, pose_envs=max(opts.record_motion, opts.render))
     torch.cuda.synchronize(env.device)
     ret, length, term = (ep[k].cpu().numpy() for k in ("returns", "lengths", "terminate"))
     os.makedirs(out_path, exist_ok=True)
@@ -145,6 +164,10 @@ def main(argv=None):
         paths = write_episode_motions(os.path.join(out_path, "motion_%d.txt"), ep, opts.record_motion,
                                       env.get_updates_per_action() * env.UPDATE_DT)
         print("motion files: %s .. %s" % (paths[0], paths[-1]))
+    if opts.render:
+        paths = write_episode_renders(os.path.join(out_path, "render_%d.png"), ep, opts.render, env.get_updates_per_action() * env.UPDATE_DT,
+                                      env._core, opts.camera, opts.render_size)
+        print("renders: %s .. %s" % (paths[0], paths[-1]))
     return dict(returns=ret, lengths=length, terminate=term)
 
 

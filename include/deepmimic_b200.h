@@ -149,6 +149,19 @@ int dm_record_goal(dm_handle* h, float* d_out);              /* [num_envs x goal
  * and a 0, then the joints' angular velocities (spherical: 3 and a 0) or rates.  Either pointer may be NULL.  Stream-ordered, no host
  * synchronisation. */
 int dm_record_pose(dm_handle* h, float* d_pose, float* d_vel);
+/* Rendering of pose rows (the counterpart of the reference's viewer drawing a kin_char, cDrawSceneKinChar / cDrawCharacter, without
+ * OpenGL): n_views rows d_pose [n_views x pose_dim] fp32 in dm_record_pose's layout (a motion-file frame; quaternions need not be unit length)
+ * are drawn as the handle's character, its collision shapes (box, capsule along the link's y axis, sphere) ray cast on the ground plane
+ * y = 0 (a 1 m checker of two greys) under a sky gradient, with one directional light, an ambient term and hard shadows.  One camera for every
+ * view, in radians and unscaled metres: it looks at (root x, target_height, root z) of each row from eye = target + distance * (cos pitch sin
+ * yaw, sin pitch, cos pitch cos yaw), +y up, fov_y the vertical field of view; one ray per pixel, through its centre.  Outputs (either may
+ * be NULL, not both): d_rgb uint8 [n_views x height x width x 3], row 0 at the top; d_ids int16 [n_views x height x width], what each pixel
+ * sees: -1 sky, -2 ground, k link k.  Uses the handle's character only, so a handle with num_envs = 1 renders any number of rows.
+ * Stream-ordered on the handle's stream, no host synchronisation.  Refused, naming the argument: a host-only handle, n_views outside
+ * [1, 65535], width or height outside [16, 4096], a NULL pose, both outputs NULL, a camera value that is not finite, distance <= 0 and
+ * fov_y outside (0, pi). */
+typedef struct { float yaw, pitch, distance, target_height, fov_y; } dm_camera;
+int dm_render_poses(dm_handle* h, int n_views, const float* d_pose, const dm_camera* cam, int width, int height, uint8_t* d_rgb, int16_t* d_ids);
 /* AMP task scenes target_amp / heading_amp (cSceneTargetAMP / cSceneHeadingAMP: RecordGoal, CalcReward, target updates; goal_size 3).
  * heading_amp_getup / strike_amp (cSceneHeadingAMPGetup / cSceneStrikeAMP) add a phase to the goal (goal_size 4).  dm_goal_host is RecordGoal
  * into a host buffer [num_envs x goal_size]; the task-state hooks expose one environment's task block (16 doubles: target x, z, speed, heading,
