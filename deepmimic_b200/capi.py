@@ -64,7 +64,7 @@ class DmCamera(C.Structure):
 
 
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
-           "dm_update", "dm_set_pushes", "dm_get_pushes", "dm_set_push_schedule", "dm_get_push_table", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_record_pose", "dm_render_poses", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
+           "dm_update", "dm_set_pushes", "dm_get_pushes", "dm_set_push_schedule", "dm_get_push_table", "dm_set_dynamics", "dm_get_dynamics", "dm_set_dynamics_randomization", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_record_pose", "dm_render_poses", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
            "dm_set_snapshot", "dm_state_size", "dm_save_state", "dm_load_state", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
            "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy", "dm_td_lambda_returns", "dm_mlp_set_weights_device", "dm_learn_create",
            "dm_mlp_set_normalizers_device", "dm_learn_set_weights", "dm_learn_step", "dm_learn_disc_step", "dm_learn_destroy",
@@ -108,6 +108,10 @@ def lib():
         if hasattr(L, "dm_set_push_schedule"):   # likewise a library built before push schedules
             L.dm_set_push_schedule.argtypes = [vp, C.POINTER(C.c_int32), C.c_int, dp, dp, dp]
             L.dm_get_push_table.argtypes = [vp, C.POINTER(C.c_int32), fp, dp, dp]
+        if hasattr(L, "dm_set_dynamics"):   # likewise a library built before dynamics tables
+            L.dm_set_dynamics.argtypes = [vp, fp]
+            L.dm_get_dynamics.argtypes = [vp, C.c_void_p]
+            L.dm_set_dynamics_randomization.argtypes = [vp, dp]
         if hasattr(L, "dm_render_poses"):   # likewise a library built before the renderer
             L.dm_render_poses.argtypes = [vp, C.c_int, C.c_void_p, C.POINTER(DmCamera), C.c_int, C.c_int, C.c_void_p, C.c_void_p]
         L.dm_plan_env_order.argtypes = [C.POINTER(C.c_int), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)]
@@ -362,6 +366,41 @@ class BatchedCore:
         if schedule:
             out["sched"] = sched
         return out
+
+    DYNAMICS_KINDS = ("friction", "kp", "kd", "torque_limit", "mass")
+
+    def set_dynamics(self, factors):
+        """dm_set_dynamics: explicit per-environment factors, float32 [N, 4 + links] (friction, kp, kd, torque_limit, one mass factor per link),
+        kept across resets.  A numpy array or tensor (copied to the host); the library refuses out-of-range values by name.  Synchronises the
+        handle's stream."""
+        if hasattr(factors, "detach"):
+            factors = factors.detach().cpu().numpy()
+        a = np.asarray(factors)
+        shape = (self.num_envs, 4 + self.dims.num_joints)
+        if a.dtype != np.float32 or a.shape != shape:
+            raise ValueError("set_dynamics: factors must be float32 of shape %s, got %s of shape %s" % (shape, a.dtype, a.shape))
+        a = np.ascontiguousarray(a)
+        self._chk(lib().dm_set_dynamics(self.h, a.ctypes.data_as(C.POINTER(C.c_float))))
+
+    def dynamics(self, out=None):
+        """dm_get_dynamics: every environment's factors as a float32 tensor [N, 4 + links] on the handle's device (stream-ordered, no host
+        synchronisation).  Refused on a handle without a dynamics table."""
+        import torch
+        shape = (self.num_envs, 4 + self.dims.num_joints)
+        if out is None:
+            out = torch.empty(shape, dtype=torch.float32, device=torch.device("cuda", self.device))
+        elif out.dtype != torch.float32 or tuple(out.shape) != shape or not out.is_contiguous() or out.device != torch.device("cuda", self.device):
+            raise ValueError("dynamics: out must be a contiguous float32 tensor of shape %s on cuda:%d" % (shape, self.device))
+        self._chk(lib().dm_get_dynamics(self.h, C.c_void_p(out.data_ptr())))
+        return out
+
+    def set_dynamics_randomization(self, lohi):
+        """dm_set_dynamics_randomization: draw every environment's factors on the device now and at every reset; lohi: 10 floats, (lo, hi) of
+        friction, kp, kd, torque_limit and mass in that order.  The library refuses out-of-range bounds by name."""
+        a = np.ascontiguousarray(lohi, dtype=np.float64).reshape(-1)
+        if a.shape != (10,):
+            raise ValueError("set_dynamics_randomization: lohi must hold 10 bounds, got %d" % a.size)
+        self._chk(lib().dm_set_dynamics_randomization(self.h, _dptr(a)))
 
     def set_env_order(self, on):
         """dm_set_env_order: place the environments in the step kernel by contact load (the default; tile width 16 only) or by index"""

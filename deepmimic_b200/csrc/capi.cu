@@ -102,6 +102,11 @@ struct dm_handle {
     dmk::DevPush* d_push = nullptr;   // push table (dm_set_pushes, dm_set_push_schedule): null until the first call, then the step launches use the push instantiations
     double* d_push_sched = nullptr;   // schedule block (dm_set_push_schedule): null on handles without a schedule; then d_push is the schedule's
     dmk::PushSchedule push_sched{};
+    dmk::DevDyn* d_dyn = nullptr;       // dynamics table (dm_set_dynamics, dm_set_dynamics_randomization): null until the first call, then the step and
+                                        // observation launches use the dynamics instantiations
+    dmk::DevPush* d_push_none = nullptr;   // the dynamics step kernel's push table on a handle without pushes: every entry empty
+    bool dyn_random = false;            // the table is drawn by dyn_rand at every reset (and owned by it)
+    dmk::DynRand dyn_rand{};
     int* d_order = nullptr;   // placement of the environments in the step kernel's tiles (dm_set_env_order); st.order is it or null
     dmk::StepLayout lay{};
     uint64_t seed = 0, env_offset = 0;
@@ -359,7 +364,9 @@ int launched(dm_handle* h) {
 
 int launch_step(dm_handle* h, double dt, int n_updates) {
     // AMP task scenes: the variant that also advances the task block; handles with a push table (dm_set_pushes): the push kernel, which applies it
-    const void* kern = h->d_push ? reinterpret_cast<const void*>(dmk::kStepPushKernels[tile_index(h)][task_scene(h)])
+    // handles with a dynamics table (dm_set_dynamics*): the dynamics kernel, which also applies the push table if there is one
+    const void* kern = h->d_dyn ? reinterpret_cast<const void*>(dmk::kStepDynKernels[tile_index(h)][task_scene(h)])
+                     : h->d_push ? reinterpret_cast<const void*>(dmk::kStepPushKernels[tile_index(h)][task_scene(h)])
                                  : reinterpret_cast<const void*>(dmk::kStepKernels[tile_index(h)][task_scene(h)]);
     // opt in to the large dynamic shared-memory carve-out; the limit is raised whenever a handle needs more than any earlier one on
     // this device (attributes are per device and per function: several handles of different sizes may live in one process)
@@ -381,7 +388,11 @@ int launch_step(dm_handle* h, double dt, int n_updates) {
         if (launched(h)) return 1;
     }
     const dim3 grid(h->padded_envs / h->tiles), block(h->tiles * h->W);
-    if (h->d_push)
+    if (h->d_dyn)
+        dmk::kStepDynKernels[tile_index(h)][task_scene(h)]<<<grid, block, h->smem_bytes, h->stream>>>(h->d_model, h->st, h->d_frame_times, h->d_frames, dt,
+                                                                                                     n_updates, h->sa.cfg.num_sim_substeps, h->lay,
+                                                                                                     h->d_push ? h->d_push : h->d_push_none, h->d_dyn);
+    else if (h->d_push)
         dmk::kStepPushKernels[tile_index(h)][task_scene(h)]<<<grid, block, h->smem_bytes, h->stream>>>(h->d_model, h->st, h->d_frame_times, h->d_frames, dt,
                                                                                                       n_updates, h->sa.cfg.num_sim_substeps, h->lay, h->d_push);
     else
@@ -390,8 +401,13 @@ int launch_step(dm_handle* h, double dt, int n_updates) {
     return launched(h);
 }
 int launch_observe_fan(dm_handle* h, const dmk::ObsFan& fan) {
-    const dmk::ObserveKernel kern = dmk::kObserveKernels[tile_index(h)][task_scene(h)];   // task scenes: every environment's own active clip
     const size_t smem = static_cast<size_t>(dmk::kPolicyBlock / h->W) * h->hm.state_size * sizeof(float);   // the block's observation rows, staged for 16-byte stores
+    if (h->d_dyn) {   // the reward's COM velocities with the environments' own masses
+        const dmk::ObserveDynKernel kern = dmk::kObserveDynKernels[tile_index(h)][task_scene(h)];
+        kern<<<policy_grid(h), dmk::kPolicyBlock, smem, h->stream>>>(h->d_model, h->st, h->d_frame_times, h->d_frames, h->d_frame_vel, fan, h->num_envs, h->d_dyn);
+        return launched(h);
+    }
+    const dmk::ObserveKernel kern = dmk::kObserveKernels[tile_index(h)][task_scene(h)];   // task scenes: every environment's own active clip
     kern<<<policy_grid(h), dmk::kPolicyBlock, smem, h->stream>>>(h->d_model, h->st, h->d_frame_times, h->d_frames, h->d_frame_vel, fan, h->num_envs);
     return launched(h);
 }
@@ -816,6 +832,10 @@ int dm_reset_clips(dm_handle* h, int force_all, const int* h_clip, const double*
         if (launched(h)) return 1;
     }
     if (launch_reset(h, force_all, kt ? h->d_inj[0] : nullptr, mt ? h->d_inj[1] : nullptr, th ? h->d_inj[2] : nullptr, h_clip ? h->d_clip_inj : nullptr)) return 1;
+    if (h->dyn_random) {   // the restarted environments' factors for their new episode (the others' draws do not change)
+        dmk::dm_dyn_draw_kernel<<<(h->num_envs + 127) / 128, 128, 0, h->stream>>>(h->st, h->d_dyn, h->dyn_rand);
+        if (launched(h)) return 1;
+    }
     if (!task_scene(h)) return 0;
     // cSceneTargetAMP::Reset's own part for the environments that were just reset
     dmk::dm_task_reset_kernel<<<(h->padded_envs + 127) / 128, 128, 0, h->stream>>>(h->d_model, h->st, h->padded_envs);
@@ -925,6 +945,105 @@ int dm_get_pushes(dm_handle* h, int32_t* h_body) {
     DM_CUDA(cudaStreamSynchronize(h->stream));
     for (int e = 0; e < h->num_envs; ++e) h_body[e] = tab[e].body;
     return 0;
+}
+// ---- dynamics (dm_dynamics.cuh)
+namespace {
+// a fixed leaf lumped into its parent's composite body by the step kernel (dm_step.cu: the dynamics tree)
+int lumped_parent(const dmk::DevModel& M, int l) {
+    const dmk::DevLink& L = M.link[l];
+    return (L.ndof == 0 && L.nchild == 0 && L.parent >= 0 && M.link[L.parent].ndof > 0) ? L.parent : -1;
+}
+float link_mass_counted(const dmk::DevModel& M, int l) { return M.link[l].shape != 0 ? M.link[l].mass : 0.f; }   // CharModel::total_mass skips shapeless bodies
+// the table and the empty push table of the dynamics kernel, every entry the plain model
+int alloc_dyn_table(dm_handle* h) {
+    const dmk::DevModel& M = h->hm;
+    if (alloc_buffer(h, &h->d_dyn, static_cast<size_t>(h->padded_envs))) return 1;
+    if (h->d_push_none == nullptr) {
+        if (alloc_buffer(h, &h->d_push_none, static_cast<size_t>(h->padded_envs))) return 1;
+        std::vector<dmk::DevPush> none(static_cast<size_t>(h->padded_envs));
+        for (auto& p : none) { p.force[0] = p.force[1] = p.force[2] = 0.f; p.body = -1; p.start = 0.0; p.duration = 0.0; }
+        DM_CUDA(cudaMemcpyAsync(h->d_push_none, none.data(), none.size() * sizeof(dmk::DevPush), cudaMemcpyHostToDevice, h->stream));
+        DM_CUDA(cudaStreamSynchronize(h->stream));
+    }
+    std::vector<dmk::DevDyn> unit(static_cast<size_t>(h->padded_envs));
+    std::vector<float> mass(M.nl);
+    for (int l = 0; l < M.nl; ++l) mass[l] = link_mass_counted(M, l);
+    for (auto& d : unit) {
+        for (int k = 0; k < dmk::kDynFloats; ++k) d.f[k] = (k < dmk::kDTotalMass) ? 1.f : 0.f;
+        d.f[dmk::kDTotalMass] = dmk::dyn_total_mass(mass.data(), M.nl, d.f);
+    }
+    DM_CUDA(cudaMemcpyAsync(h->d_dyn, unit.data(), unit.size() * sizeof(dmk::DevDyn), cudaMemcpyHostToDevice, h->stream));
+    DM_CUDA(cudaStreamSynchronize(h->stream));
+    return 0;
+}
+const char* const kDynKindNames[dmk::kDynKinds] = {"friction", "kp", "kd", "torque_limit", "mass"};
+}  // namespace
+int dm_set_dynamics(dm_handle* h, const float* h_factors) {
+    DM_DEVICE(h);
+    auto refuse = [](const std::string& what) { g_err = "dm_set_dynamics: " + what; return fail(); };
+    if (!h_factors) return refuse("h_factors is required");
+    if (h->dyn_random) return refuse("the handle's dynamics are randomised (dm_set_dynamics_randomization), which owns its table");
+    const dmk::DevModel& M = h->hm;
+    const int N = h->num_envs, nl = M.nl, row = 4 + nl;
+    std::vector<float> mass(nl);
+    for (int l = 0; l < nl; ++l) mass[l] = link_mass_counted(M, l);
+    std::vector<dmk::DevDyn> tab(static_cast<size_t>(h->padded_envs));
+    for (int e = 0; e < N; ++e) {
+        const float* f = h_factors + static_cast<size_t>(e) * row;
+        const std::string env = "environment " + std::to_string(e) + ": ";
+        for (int j = 0; j < 4; ++j)
+            if (!std::isfinite(f[j]) || f[j] < 0.f) return refuse(env + kDynKindNames[j] + " " + std::to_string(f[j]) + " is not finite and >= 0");
+        for (int l = 0; l < nl; ++l)
+            if (!std::isfinite(f[4 + l]) || !(f[4 + l] > 0.f))
+                return refuse(env + "mass of link " + std::to_string(l) + " " + std::to_string(f[4 + l]) + " is not finite and > 0");
+        for (int l = 0; l < nl; ++l) {
+            const int p = lumped_parent(M, l);
+            if (p >= 0 && f[4 + l] != f[4 + p])
+                return refuse(env + "mass of link " + std::to_string(l) + " differs from its parent link " + std::to_string(p) +
+                              "'s: a fixed leaf is part of its parent's composite body");
+        }
+        dmk::DevDyn& d = tab[e];
+        for (int k = 0; k < dmk::kDynFloats; ++k) d.f[k] = (k < dmk::kDTotalMass) ? 1.f : 0.f;
+        for (int j = 0; j < row; ++j) d.f[j] = f[j];
+        d.f[dmk::kDTotalMass] = dmk::dyn_total_mass(mass.data(), nl, d.f);
+    }
+    for (int e = N; e < h->padded_envs; ++e) tab[e] = tab[N - 1];   // padding: never simulated
+    if (h->d_dyn == nullptr && alloc_dyn_table(h)) return 1;
+    DM_CUDA(cudaMemcpyAsync(h->d_dyn, tab.data(), tab.size() * sizeof(dmk::DevDyn), cudaMemcpyHostToDevice, h->stream));
+    DM_CUDA(cudaStreamSynchronize(h->stream));   // the staging vector is pageable
+    return 0;
+}
+int dm_get_dynamics(dm_handle* h, float* d_out) {
+    DM_DEVICE(h);
+    if (!d_out) { g_err = "dm_get_dynamics: d_out is required"; return fail(); }
+    if (h->d_dyn == nullptr) { g_err = "dm_get_dynamics: the handle has no dynamics table (dm_set_dynamics, dm_set_dynamics_randomization)"; return fail(); }
+    const size_t row = static_cast<size_t>(4 + h->hm.nl) * sizeof(float);
+    DM_CUDA(cudaMemcpy2DAsync(d_out, row, h->d_dyn, sizeof(dmk::DevDyn), row, static_cast<size_t>(h->num_envs), cudaMemcpyDeviceToDevice, h->stream));
+    return 0;
+}
+int dm_set_dynamics_randomization(dm_handle* h, const double* lohi) {
+    DM_DEVICE(h);
+    auto refuse = [](const std::string& what) { g_err = "dm_set_dynamics_randomization: " + what; return fail(); };
+    if (!lohi) return refuse("lohi is required");
+    if (h->d_dyn && !h->dyn_random) return refuse("the handle has factors set by dm_set_dynamics, which own its table");
+    for (int k = 0; k < dmk::kDynKinds; ++k) {
+        const double lo = lohi[2 * k], hi = lohi[2 * k + 1];
+        const std::string kind = kDynKindNames[k];
+        if (!std::isfinite(lo) || !std::isfinite(hi)) return refuse(kind + ": a bound is not finite");
+        if (lo < 0.0 || hi < 0.0) return refuse(kind + ": a bound is negative");
+        if (lo > hi) return refuse(kind + ": lo > hi");
+        if (k == 4 && !(lo > 0.0)) return refuse(kind + ": lo must be > 0");
+    }
+    const dmk::DevModel& M = h->hm;
+    dmk::DynRand R;
+    std::memset(&R, 0, sizeof(R));   // padding included: the state header hashes the bytes
+    for (int k = 0; k < 2 * dmk::kDynKinds; ++k) R.lohi[k] = lohi[k];
+    R.seed = h->seed ^ dmk::kDynSeedKey; R.env_base = h->env_offset; R.nl = M.nl;
+    for (int l = 0; l < 32; ++l) { R.leaf_parent[l] = l < M.nl ? lumped_parent(M, l) : -1; R.link_mass[l] = l < M.nl ? link_mass_counted(M, l) : 0.f; }
+    if (h->d_dyn == nullptr && alloc_dyn_table(h)) return 1;
+    h->dyn_rand = R; h->dyn_random = true;
+    dmk::dm_dyn_draw_kernel<<<(h->num_envs + 127) / 128, 128, 0, h->stream>>>(h->st, h->d_dyn, h->dyn_rand);
+    return launched(h);
 }
 int dm_set_env_order(dm_handle* h, int on) {
     DM_DEVICE(h);
@@ -1363,9 +1482,10 @@ constexpr char kStateMagic[8] = {'D', 'M', 'S', 'T', 'A', 'T', 'E', 0};
 constexpr uint32_t kStateVersion = 1;
 struct StateHeader {
     char magic[8];
-    uint32_t version, pad0;
+    uint32_t version, dynamics;   // dynamics: 0 without a randomised dynamics table, else a hash of its bounds (dynamics_hash)
     uint64_t bytes;
-    int32_t num_envs, padded_envs, W, links, state_size, action_size, goal_size, amp_obs_size, num_clips, pad1;
+    int32_t num_envs, padded_envs, W, links, state_size, action_size, goal_size, amp_obs_size, num_clips;
+    int32_t dyn_table;   // 1: the blob ends with a dynamics table (dm_set_dynamics or dm_set_dynamics_randomization); 0: none
     uint64_t seed, env_offset, model;
     char scene[32];
     // host state that changes later results
@@ -1389,6 +1509,7 @@ std::vector<StateBlock> state_blocks(const dm_handle* h) {
         b.push_back({h->d_push, N * sizeof(dmk::DevPush)});
         b.push_back({h->d_push_sched, N * dmk::kPushSchedDoubles * sizeof(double)});
     }
+    if (h->d_dyn) b.push_back({h->d_dyn, N * sizeof(dmk::DevDyn)});   // a dynamics table ends the blob
     return b;
 }
 // the state header's push_schedule field: 0 without a schedule, else FNV-1a over its parameters folded to 32 bits and never 0
@@ -1397,6 +1518,15 @@ uint32_t push_schedule_hash(const dm_handle* h) {
     const unsigned char* p = reinterpret_cast<const unsigned char*>(&h->push_sched);
     uint64_t x = 1469598103934665603ull;
     for (size_t i = 0; i < sizeof(h->push_sched); ++i) { x ^= p[i]; x *= 1099511628211ull; }
+    const uint32_t v = static_cast<uint32_t>(x ^ (x >> 32));
+    return v ? v : 1u;
+}
+// the state header's dynamics field: 0 without a randomised table (none, or dm_set_dynamics), else FNV-1a over the bounds, folded, never 0
+uint32_t dynamics_hash(const dm_handle* h) {
+    if (!h->dyn_random) return 0;
+    const unsigned char* p = reinterpret_cast<const unsigned char*>(h->dyn_rand.lohi);
+    uint64_t x = 1469598103934665603ull;
+    for (size_t i = 0; i < sizeof(h->dyn_rand.lohi); ++i) { x ^= p[i]; x *= 1099511628211ull; }
     const uint32_t v = static_cast<uint32_t>(x ^ (x >> 32));
     return v ? v : 1u;
 }
@@ -1415,7 +1545,7 @@ StateHeader state_header(const dm_handle* h) {
     StateHeader H;
     std::memset(&H, 0, sizeof(H));
     std::memcpy(H.magic, kStateMagic, sizeof(H.magic));
-    H.version = kStateVersion;
+    H.version = kStateVersion; H.dynamics = dynamics_hash(h); H.dyn_table = h->d_dyn ? 1 : 0;
     H.bytes = sizeof(StateHeader);
     for (const StateBlock& b : state_blocks(h)) H.bytes += b.bytes;
     const auto& M = h->hm;
@@ -1475,6 +1605,8 @@ int dm_load_state(dm_handle* h, const void* h_in) {
     if (in.env_offset != mine.env_offset) return refuse("global env offset");
     if (in.model != mine.model) return refuse("model (character, controller or clips)");
     if (in.push_schedule != mine.push_schedule) return refuse("push schedule (dm_set_push_schedule: none, or other parameters)");
+    if (in.dyn_table != mine.dyn_table) return refuse("dynamics table (dm_set_dynamics, dm_set_dynamics_randomization: one, or none)");
+    if (in.dynamics != mine.dynamics) return refuse("dynamics randomisation (dm_set_dynamics_randomization: none, or other bounds)");
     if (in.bytes != mine.bytes) return refuse("byte size");
     const char* p = static_cast<const char*>(h_in) + sizeof(in);
     for (const StateBlock& b : state_blocks(h)) {

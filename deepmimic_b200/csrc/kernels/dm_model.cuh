@@ -11,6 +11,7 @@
 
 #include "dm_math.cuh"
 
+#include "dm_dynamics.cuh"
 #include "dm_push.cuh"
 #include "dm_task.cuh"
 #include "dm_task_ext.cuh"
@@ -18,6 +19,7 @@
 namespace dmk {
 
 constexpr int kMaxLinks = 32;   // one lane per link
+static_assert(kDTotalMass == kDMass + kMaxLinks, "DevDyn holds one mass factor per lane");
 constexpr int kMaxDofs = 96;    // 6 + joint dofs (humanoid3d 34, dog3d 70)
 constexpr int kMaxChain = 24;   // longest root->leaf dof chain (humanoid3d 13, dog3d 22)
 constexpr int kMaxChildren = 4;
@@ -194,13 +196,17 @@ struct StepLayout {
 constexpr int kPolicyBlock = 64;   // threads per block of the observe, AMP and reset kernels
 using StepKernel = void (*)(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout);
 using StepPushKernel = void (*)(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout, DevPush*);
+using StepDynKernel = void (*)(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout, DevPush*, const DevDyn*);
 using ObserveKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, ObsFan, int);
+using ObserveDynKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, ObsFan, int, const DevDyn*);
 using ResetKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, int, const double*, const double*, const double*,
                              unsigned long long, unsigned long long, int, const int*);
 using AmpObsKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, float*, int, const double*, int, const int*);
 extern const StepKernel kStepKernels[2][2];
 extern const StepPushKernel kStepPushKernels[2][2];   // dm_step_push_kernel: handles with a push table (dm_set_pushes)
+extern const StepDynKernel kStepDynKernels[2][2];     // dm_step_dyn_kernel: handles with a dynamics table (dm_set_dynamics, dm_set_dynamics_randomization)
 extern const ObserveKernel kObserveKernels[2][2];
+extern const ObserveDynKernel kObserveDynKernels[2][2];   // dm_observe_dyn_kernel: the imitation reward's COM with the environment's masses
 extern const ResetKernel kResetKernels[2][2];
 extern const AmpObsKernel kAmpObsKernels[2][2];
 using AmpExpertKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, float*, int, unsigned long long, unsigned long long,
@@ -214,6 +220,7 @@ __global__ void dm_pose_kernel(const DevModel*, DevState, float*, float*, int);
 __global__ void dm_task_reset_kernel(const DevModel*, DevState, int);
 __global__ void dm_push_clear_kernel(DevState, DevPush*, int);
 __global__ void dm_push_schedule_kernel(DevState, DevPush*, double*, PushSchedule);
+__global__ void dm_dyn_draw_kernel(DevState, DevDyn*, DynRand);
 __global__ void dm_task_observe_kernel(const DevModel*, DevState, float*, float*, int);
 int dm_step_layout(int nl, int n, int chain_len, int maxrows, int W, StepLayout* L);
 int dm_step_smem_bytes(const StepLayout& L, int tiles);

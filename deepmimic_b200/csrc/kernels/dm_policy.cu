@@ -166,10 +166,11 @@ template <> struct ClipPick<true> { static __device__ __forceinline__ const Clip
 // 16-byte stores, so the multi-GPU "all-gather" of the policy step is the store phase of this kernel (NVLink P2P writes), not a collective.
 // CLIPS (--kin_ctrl clips, AMP task scenes): the imitation reward is taken against the environment's own active clip of the dataset
 // (st.clip / st.ctab) -- BASELINE.json config 5 records it next to the AMP observations and the task reward.
-template <int W, int BLOCK, bool CLIPS>
-__global__ void __launch_bounds__(BLOCK) dm_observe_kernel(const DevModel* __restrict__ gm, DevState st, const double* __restrict__ frame_times,
-                                                            const float* __restrict__ frames, const float* __restrict__ frame_vel,
-                                                            ObsFan fan, int num_real_envs) {
+// DYN (dm_observe_dyn_kernel, handles with a dynamics table): the COM velocities of the reward weigh the links by the environment's own masses.
+template <int W, int BLOCK, bool CLIPS, bool DYN>
+__device__ __forceinline__ void observe_body(const DevModel* __restrict__ gm, DevState st, const double* __restrict__ frame_times,
+                                             const float* __restrict__ frames, const float* __restrict__ frame_vel,
+                                             ObsFan fan, int num_real_envs, const DevDyn* __restrict__ dyn) {
     using T = TileP<W>;
     extern __shared__ __align__(16) float srow[];   // [tiles x state_size] observation rows of this block
     const bool want_obs = fan.obs[0] != nullptr, want_reward = fan.rew[0] != nullptr;
@@ -360,7 +361,9 @@ __global__ void __launch_bounds__(BLOCK) dm_observe_kernel(const DevModel* __res
         vel_e = M.link[0].joint_w * dot(d, d);
     }
     const float pose_err = T::sum(act ? pose_e : 0.f), vel_err = T::sum(act ? vel_e : 0.f), end_eff_err = T::sum(act ? ee_e : 0.f);
-    const float mfrac = act ? L.mass / M.total_mass : 0.f;
+    float mfrac;
+    if constexpr (DYN) { const float* df = dyn[env].f; mfrac = act ? (L.mass * df[kDMass + li]) / df[kDTotalMass] : 0.f; }
+    else mfrac = act ? L.mass / M.total_mass : 0.f;
     const V3 com_v0 = mk3(T::sum(mfrac * lin_w.x), T::sum(mfrac * lin_w.y), T::sum(mfrac * lin_w.z));
     const V3 com_v1 = mk3(T::sum(mfrac * kcom_v.x), T::sum(mfrac * kcom_v.y), T::sum(mfrac * kcom_v.z));
     if (lane == 0 && env < num_real_envs) {
@@ -377,6 +380,18 @@ __global__ void __launch_bounds__(BLOCK) dm_observe_kernel(const DevModel* __res
         if (fl[kFFallen]) rwd = 0.f;
         for (int d = 0; d < fan.n; ++d) fan.rew[d][env] = rwd;
     }
+}
+template <int W, int BLOCK, bool CLIPS>
+__global__ void __launch_bounds__(BLOCK) dm_observe_kernel(const DevModel* __restrict__ gm, DevState st, const double* __restrict__ frame_times,
+                                                            const float* __restrict__ frames, const float* __restrict__ frame_vel,
+                                                            ObsFan fan, int num_real_envs) {
+    observe_body<W, BLOCK, CLIPS, false>(gm, st, frame_times, frames, frame_vel, fan, num_real_envs, nullptr);
+}
+template <int W, int BLOCK, bool CLIPS>
+__global__ void __launch_bounds__(BLOCK) dm_observe_dyn_kernel(const DevModel* __restrict__ gm, DevState st, const double* __restrict__ frame_times,
+                                                                const float* __restrict__ frames, const float* __restrict__ frame_vel,
+                                                                ObsFan fan, int num_real_envs, const DevDyn* dyn) {
+    observe_body<W, BLOCK, CLIPS, true>(gm, st, frame_times, frames, frame_vel, fan, num_real_envs, dyn);
 }
 
 namespace {
@@ -822,6 +837,8 @@ __global__ void dm_task_observe_kernel(const DevModel* __restrict__ gm, DevState
 
 const ObserveKernel kObserveKernels[2][2] = {{dm_observe_kernel<16, kPolicyBlock, false>, dm_observe_kernel<16, kPolicyBlock, true>},
                                              {dm_observe_kernel<32, kPolicyBlock, false>, dm_observe_kernel<32, kPolicyBlock, true>}};
+const ObserveDynKernel kObserveDynKernels[2][2] = {{dm_observe_dyn_kernel<16, kPolicyBlock, false>, dm_observe_dyn_kernel<16, kPolicyBlock, true>},
+                                                   {dm_observe_dyn_kernel<32, kPolicyBlock, false>, dm_observe_dyn_kernel<32, kPolicyBlock, true>}};
 const ResetKernel kResetKernels[2][2] = {{dm_reset_kernel<16, kPolicyBlock, false>, dm_reset_kernel<16, kPolicyBlock, true>},
                                          {dm_reset_kernel<32, kPolicyBlock, false>, dm_reset_kernel<32, kPolicyBlock, true>}};
 const AmpObsKernel kAmpObsKernels[2][2] = {{dm_amp_obs_kernel<16, kPolicyBlock, false>, dm_amp_obs_kernel<16, kPolicyBlock, true>},

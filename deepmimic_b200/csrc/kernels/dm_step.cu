@@ -157,6 +157,7 @@ int dm_step_layout(int nl, int n, int chain_len, int maxrows, int W, StepLayout*
 }
 int dm_step_smem_bytes(const StepLayout& L, int tiles) { return (L.hot_floats + L.env_floats * tiles) * static_cast<int>(sizeof(float)); }
 
+constexpr int kBMu = 14;   // sB slot (float, base state + 14, free in the plain kernels): DYN, the environment's friction coefficient
 constexpr int kSubstepBarriers = 2;   // block barriers inside a Bullet sub-step stage (dm_step_kernel's main loop)
 constexpr int kPgsBlock = 2;   // solver steps evaluated per block of the projected Gauss-Seidel sweeps (chosen by measuring 1, 2, 4 and 8; 2 was the fastest)
 // Projected Gauss-Seidel in impulse space, 10 sweeps in btMultiBodyConstraintSolver::solveSingleIteration's row order (joint limits in
@@ -339,7 +340,9 @@ __device__ __forceinline__ void pgs_sweeps(const float* sA, float* sLam, const f
 // run it in lockstep).  Input (shared memory): per-link factors U / 1/D, joint axes, pivots, link velocities, contact points, limit
 // rows, base Cholesky factor.  Output: impulses in sLam (also written to the persistent manifold), z = Y^T lambda in sZ.
 // Row ids in solver order: limits [0,NL) | normals [NL, NL+P) | friction pairs NL+P+2p+{0,1} (t1 = -x, t2 = +z).
-template <int W>
+// DYN: the friction bounds take the environment's own coefficient (the model's times its friction factor, staged in its base-state slot kBMu
+// at the start of the launch) instead of the model's in the block header.
+template <int W, bool DYN>
 __device__ __noinline__ void solve_rows(int NL, int P, float* mani, int alive, unsigned int* prf) {
     using T = Tl<W>;
     // context from threadIdx and the block-shared header (nothing but scalars crosses the call, see Ctx below)
@@ -570,9 +573,9 @@ __device__ __noinline__ void solve_rows(int NL, int P, float* mani, int alive, u
         }
         __syncwarp();
         SPROF(8);
-        if (mode == 0) pgs_sweeps<W, 1, W, kPgsBlock>(sA, sLam, sRI, lane, NL, P, NLmax, Pmax, mu);
-        else if (mode == 1) pgs_sweeps<W, kSlots, kSq2, kPgsBlock>(sA, sLam, sRI, lane, NL, P, NLmax, Pmax, mu);
-        else pgs_sweeps<W, kSlots, 0, kPgsBlock>(sA, sLam, sRI, lane, NL, P, NLmax, Pmax, mu);
+        if (mode == 0) pgs_sweeps<W, 1, W, kPgsBlock>(sA, sLam, sRI, lane, NL, P, NLmax, Pmax, DYN ? sG[21 + kBMu] : mu);
+        else if (mode == 1) pgs_sweeps<W, kSlots, kSq2, kPgsBlock>(sA, sLam, sRI, lane, NL, P, NLmax, Pmax, DYN ? sG[21 + kBMu] : mu);
+        else pgs_sweeps<W, kSlots, 0, kPgsBlock>(sA, sLam, sRI, lane, NL, P, NLmax, Pmax, DYN ? sG[21 + kBMu] : mu);
     }
     SPROF(9);
     // write impulses back to the manifold (warm start of the next sub-step)
@@ -862,7 +865,10 @@ __device__ __noinline__ int collide(float* mani, int alive, int mcnt) {
 // slots (sQ: force, body), which are dead until the constraint rows of the sub-step are written.  The lane of the dynamics body that holds the
 // body subtracts the spatial force about its reference point from its bias force (the root's lane: the base origin; a lumped leaf's force goes
 // to its parent's lane, applied at the leaf's own COM).
-template <int W, bool PUSH>
+// DYN (aba_solve_dyn): the lane's composite rigid body (mass, first moment and either inertia) times its link's mass factor, staged by the caller
+// in the lane's impulse slot (sLam), which is dead until the constraint rows of the sub-step are written.  Gravity enters as a base
+// acceleration, so its force follows the mass.
+template <int W, bool PUSH, bool DYN>
 __device__ __forceinline__ float3 aba_solve_body(float g0, float g1, float g2, float kdt, int bullet, float jvx, float jvy, float jvz) {
     const Ctx c = make_ctx<W>();
     const float gx = step_smem()[kHGrav], gy = step_smem()[kHGrav + 1], gz = step_smem()[kHGrav + 2], h = step_smem()[kHh];
@@ -878,7 +884,8 @@ __device__ __forceinline__ float3 aba_solve_body(float g0, float g1, float g2, f
     const int dmax = reinterpret_cast<const int*>(step_smem())[kHDmax];
     const bool isroot = c.lane == 0;
     const float4 dc4 = ld4(LKo + kLDc);           // reference point -> composite COM (link axes) | composite mass
-    const float mass = c.act ? dc4.w : 0.f;       // composite mass (own + lumped leaves; 0 for a lumped leaf itself)
+    const float mf = DYN ? c.E[LY.oLam + c.lane] : 1.f;   // DYN: the lane's mass factor
+    const float mass = c.act ? (DYN ? mf * dc4.w : dc4.w) : 0.f;   // composite mass (own + lumped leaves; 0 for a lumped leaf itself)
     float q[12];
     ld12(sS + c.li * 12, q);
     const V3 S0 = mk3(q[0], q[1], q[2]), S1 = mk3(q[3], q[4], q[5]), S2 = mk3(q[6], q[7], q[8]), cwk = mk3(q[9], q[10], q[11]);   // cwk: kinematic parent's pivot -> pivot
@@ -924,7 +931,7 @@ __device__ __forceinline__ float3 aba_solve_body(float g0, float g1, float g2, f
         const float4 w4 = ld4(wsel); const float2 w2 = *reinterpret_cast<const float2*>(wsel + 4);
         float wl[6] = {w4.x, w4.y, w4.z, w4.w, w2.x, w2.y};
 #pragma unroll
-        for (int k = 0; k < 6; ++k) wl[k] = c.act ? wl[k] : 0.f;
+        for (int k = 0; k < 6; ++k) wl[k] = c.act ? (DYN ? mf * wl[k] : wl[k]) : 0.f;
         M3 Rwl;
         {
             float w[12];
@@ -1114,11 +1121,20 @@ __device__ __forceinline__ float3 aba_solve_body(float g0, float g1, float g2, f
 }
 template <int W>
 __device__ __noinline__ float3 aba_solve(float g0, float g1, float g2, float kdt, int bullet, float jvx, float jvy, float jvz) {
-    return aba_solve_body<W, false>(g0, g1, g2, kdt, bullet, jvx, jvy, jvz);
+    return aba_solve_body<W, false, false>(g0, g1, g2, kdt, bullet, jvx, jvy, jvz);
 }
 template <int W>
 __device__ __noinline__ float3 aba_solve_push(float g0, float g1, float g2, float kdt, int bullet, float jvx, float jvy, float jvz) {
-    return aba_solve_body<W, true>(g0, g1, g2, kdt, bullet, jvx, jvy, jvz);
+    return aba_solve_body<W, true, false>(g0, g1, g2, kdt, bullet, jvx, jvy, jvz);
+}
+// the dynamics kernel's Stable-PD solve and its Bullet sub-steps' (with the push), two routines as in the push kernel
+template <int W>
+__device__ __noinline__ float3 aba_solve_dyn_pd(float g0, float g1, float g2, float kdt, int bullet, float jvx, float jvy, float jvz) {
+    return aba_solve_body<W, false, true>(g0, g1, g2, kdt, bullet, jvx, jvy, jvz);
+}
+template <int W>
+__device__ __noinline__ float3 aba_solve_dyn(float g0, float g1, float g2, float kdt, int bullet, float jvx, float jvy, float jvz) {
+    return aba_solve_body<W, true, true>(g0, g1, g2, kdt, bullet, jvx, jvy, jvz);
 }
 
 // Velocity correction of the constraint impulses: dv = L^-1 D^-1/2 z with z = Y^T lambda (sZ), by the root -> leaves pass over the factors
@@ -1258,11 +1274,14 @@ struct EnvRefs {
 // TASK: the AMP task scenes' instantiation, which also advances the environment's task block after every update (dm_task.cuh); the plain
 // imitate kernel carries none of that code.  PUSH: the body of dm_step_push_kernel, the kernel of handles with a push table (dm_set_pushes),
 // which applies the environment's push (push_in, by environment id) in the Bullet sub-steps of the updates inside its window and clears the
-// entry once the window has passed.
-template <int W, bool TASK, bool PUSH>
+// entry once the window has passed.  DYN (with PUSH): the body of dm_step_dyn_kernel, the kernel of handles with a dynamics table
+// (dm_set_dynamics, dm_set_dynamics_randomization): the environment's factors (dyn_in, by environment id) scale the composite bodies of the
+// articulated-body solves, Kp, Kd and the torque limit of the Stable-PD stage, the friction bounds of the constraint solve and the masses of the
+// task scenes' COM.  They are read from global memory where they are used, not kept across the main loop.
+template <int W, bool TASK, bool PUSH, bool DYN>
 __device__ __forceinline__ void dm_step_body(const DevModel* __restrict__ gm, const DevState& st, const double* __restrict__ frame_times,
                                              const float* __restrict__ frames, double dt, int n_updates, int sim_substeps, const StepLayout& LY,
-                                             DevPush* push_in) {
+                                             DevPush* push_in, const DevDyn* __restrict__ dyn_in) {
     using T = Tl<W>;
     extern __shared__ __align__(16) float sm[];
     const int tiles = blockDim.x / W;
@@ -1381,6 +1400,7 @@ __device__ __forceinline__ void dm_step_body(const DevModel* __restrict__ gm, co
             sB[0] = b0.x; sB[1] = b0.y; sB[2] = b0.z; sB[3] = b1.x; sB[4] = b1.y; sB[5] = b1.z; sB[6] = b1.w;
             sB[7] = b2.x; sB[8] = b2.y; sB[9] = b2.z; sB[10] = b3.x; sB[11] = b3.y; sB[12] = b3.z;
             reinterpret_cast<int*>(sB)[kBUpdates] = r.fl[kFUpdates];
+            if constexpr (DYN) sB[kBMu] = __fmul_rn(step_smem()[kHMu], dyn_in[r.env].f[kDFriction]);
         }
         jp = reinterpret_cast<const float4*>(sim + 16)[li];
         jv = reinterpret_cast<const float4*>(sim + 16 + 4 * nl)[li];
@@ -1450,7 +1470,13 @@ __device__ __forceinline__ void dm_step_body(const DevModel* __restrict__ gm, co
                 // cSceneTargetAMP::Update: target timer / position / heading / speed after the scene update, then the distance failure of
                 // CheckTerminate; the COM is kept for CalcReward (SceneTargetAMP.cpp:3-80,136-145,294-319).  heading_amp_getup and strike_amp
                 // (dm_task_ext.cuh) additionally need a few bodies' positions / velocities, published to lane 0 by shuffles.
-                const V3 com = tile_com<W>(E + LY.oW + li * 12, v, act ? LKo[kLM] : 0.f, 1.0f / (M.total_mass * scale));
+                V3 com;
+                if constexpr (DYN) {
+                    const float* df = dyn_in[r.env].f;
+                    com = tile_com<W>(E + LY.oW + li * 12, v, act ? LKo[kLM] * df[kDMass + li] : 0.f, 1.0f / (df[kDTotalMass] * scale));
+                } else {
+                    com = tile_com<W>(E + LY.oW + li * 12, v, act ? LKo[kLM] : 0.f, 1.0f / (M.total_mass * scale));
+                }
                 const int kind = M.task_kind;
                 TaskBodies B;
                 if (kind >= kTaskHeadingGetup) {
@@ -1549,7 +1575,13 @@ __device__ __forceinline__ void dm_step_body(const DevModel* __restrict__ gm, co
                 // cDeepMimicCharController::HandleNewAction (DeepMimicCharController.cpp:262-267): COM of the state the new action starts from
                 if (__ballot_sync(0xffffffffu, ls.get(kLsAlive) && ls.get(kLsNeedAction)) != 0u) {
                     const float scale = step_smem()[kHScale];
-                    const V3 com = tile_com<W>(r.E + LY.oW + li * 12, r.E + LY.oV + li * 12, r.act ? r.LKo[kLM] : 0.f, 1.0f / (M.total_mass * scale));
+                    V3 com;
+                    if constexpr (DYN) {
+                        const float* df = dyn_in[r.env].f;
+                        com = tile_com<W>(r.E + LY.oW + li * 12, r.E + LY.oV + li * 12, r.act ? r.LKo[kLM] * df[kDMass + li] : 0.f, 1.0f / (df[kDTotalMass] * scale));
+                    } else {
+                        com = tile_com<W>(r.E + LY.oW + li * 12, r.E + LY.oV + li * 12, r.act ? r.LKo[kLM] : 0.f, 1.0f / (M.total_mass * scale));
+                    }
                     double* tk = st.task + static_cast<size_t>(r.env) * kTaskDoubles;
                     if (lane == 0 && ls.get(kLsAlive) && ls.get(kLsNeedAction)) { tk[kKPrevCom] = com.x; tk[kKPrevCom + 1] = com.y; tk[kKPrevCom + 2] = com.z; }
                 }
@@ -1615,19 +1647,27 @@ __device__ __forceinline__ void dm_step_body(const DevModel* __restrict__ gm, co
                 } else if (jtype == kJRevolute) {
                     e0 = tg.x - (normalize_angle3(jp.x) + fdt * jv.x);
                 }
-                const float kp = r.LKo[kLKp], kd = r.LKo[kLKd];
+                float kp = r.LKo[kLKp], kd = r.LKo[kLKd];
+                if constexpr (DYN) {
+                    const float* df = dyn_in[r.env].f;
+                    kp *= df[kDKp]; kd *= df[kDKd];
+                    r.E[LY.oLam + lane] = df[kDMass + li];   // the lane's mass factor (aba_solve_body)
+                }
                 pe0 = kp * e0; pe1 = kp * e1; pe2 = kp * e2;
-                qdd = aba_solve<W>(pe0 - kd * jv.x, pe1 - kd * jv.y, pe2 - kd * jv.z, fdt * kd, 0, jv.x, jv.y, jv.z);
+                if constexpr (DYN) qdd = aba_solve_dyn_pd<W>(pe0 - kd * jv.x, pe1 - kd * jv.y, pe2 - kd * jv.z, fdt * kd, 0, jv.x, jv.y, jv.z);
+                else qdd = aba_solve<W>(pe0 - kd * jv.x, pe1 - kd * jv.y, pe2 - kd * jv.z, fdt * kd, 0, jv.x, jv.y, jv.z);
             }
             // Kd, dt and the joint's dofs are read again after the call
             const EnvRefs<W> r2(st, LY, env);
-            const float fdt = step_smem()[kHFdt], kd = r2.LKo[kLKd];
+            const float fdt = step_smem()[kHFdt];
+            float kd = r2.LKo[kLKd];
+            if constexpr (DYN) kd *= dyn_in[r2.env].f[kDKd];
             const int ndof = r2.act ? ((r2.lk_int(kLInt) >> 16) & 0xff) : 0;
             // ---------------- torques: tau = Kp e + Kd (edot - dt a), clamped by norm (cSimBodyJoint::ClampTotalTorque, SimBodyJoint.cpp:299-307)
             float t0 = 0, t1 = 0, t2 = 0;
             if (ndof >= 1) t0 = pe0 + kd * (-jv.x - fdt * qdd.x);
             if (ndof == 3) { t1 = pe1 + kd * (-jv.y - fdt * qdd.y); t2 = pe2 + kd * (-jv.z - fdt * qdd.z); }
-            const float mag = sqrtf(t0 * t0 + t1 * t1 + t2 * t2), tlim = r2.LKo[kLTl];
+            const float mag = sqrtf(t0 * t0 + t1 * t1 + t2 * t2), tlim = DYN ? r2.LKo[kLTl] * dyn_in[r2.env].f[kDTlim] : r2.LKo[kLTl];
             if (mag > tlim) { float s = tlim / mag; t0 *= s; t1 *= s; t2 *= s; }
             tau0 = t0; tau1 = t1; tau2 = t2;
             PROF(4);
@@ -1646,9 +1686,11 @@ __device__ __forceinline__ void dm_step_body(const DevModel* __restrict__ gm, co
                 {   // the environment's push into its limit-row slots (aba_solve_body)
                     const EnvRefs<W> r(st, LY, env);
                     if (r.lane == 0 && ls.get(kLsPush)) *reinterpret_cast<float4*>(r.E + LY.oQ) = *reinterpret_cast<const float4*>(push_in + r.env);
+                    if constexpr (DYN) r.E[LY.oLam + r.lane] = dyn_in[r.env].f[kDMass + r.li];   // the lane's mass factor (aba_solve_body)
                     __syncwarp();
                 }
-                qdd = aba_solve_push<W>(tau0, tau1, tau2, 0.f, ls.get(kLsPush) ? 2 : 1, jv.x, jv.y, jv.z);
+                if constexpr (DYN) qdd = aba_solve_dyn<W>(tau0, tau1, tau2, 0.f, ls.get(kLsPush) ? 2 : 1, jv.x, jv.y, jv.z);
+                else qdd = aba_solve_push<W>(tau0, tau1, tau2, 0.f, ls.get(kLsPush) ? 2 : 1, jv.x, jv.y, jv.z);
             } else {
                 qdd = aba_solve<W>(tau0, tau1, tau2, 0.f, 1, jv.x, jv.y, jv.z);
             }
@@ -1698,7 +1740,7 @@ __device__ __forceinline__ void dm_step_body(const DevModel* __restrict__ gm, co
 #ifdef DM_PROFILE
             { const int nrm = wmax(NR); if ((threadIdx.x & 31) == 0) { PRF[13] += nrm; PRF[14] += 1; if (nrm > W) PRF[15] += 1; } }
 #endif
-            solve_rows<W>(NL, P, r.mani, ls.get(kLsAlive) ? 1 : 0, PRFP);
+            solve_rows<W, DYN>(NL, P, r.mani, ls.get(kLsAlive) ? 1 : 0, PRFP);
             PROF(10);
             const float3 dq = dv_pass<W>();
             if (ls.get(kLsRows) > 0) {   // NR > 0
@@ -1736,18 +1778,26 @@ __device__ __forceinline__ void dm_step_body(const DevModel* __restrict__ gm, co
 template <int W, bool TASK>
 __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_kernel(const DevModel* __restrict__ gm, DevState st, const double* __restrict__ frame_times,
                                                                        const float* __restrict__ frames, double dt, int n_updates, int sim_substeps, StepLayout LY) {
-    dm_step_body<W, TASK, false>(gm, st, frame_times, frames, dt, n_updates, sim_substeps, LY, nullptr);
+    dm_step_body<W, TASK, false, false>(gm, st, frame_times, frames, dt, n_updates, sim_substeps, LY, nullptr, nullptr);
 }
 // a kernel of its own (not a third flag of dm_step_kernel): its own signature, and the plain kernels stay exactly what they were
 template <int W, bool TASK>
 __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_push_kernel(const DevModel* __restrict__ gm, DevState st, const double* __restrict__ frame_times,
                                                                             const float* __restrict__ frames, double dt, int n_updates, int sim_substeps, StepLayout LY,
                                                                             DevPush* push) {
-    dm_step_body<W, TASK, true>(gm, st, frame_times, frames, dt, n_updates, sim_substeps, LY, push);
+    dm_step_body<W, TASK, true, false>(gm, st, frame_times, frames, dt, n_updates, sim_substeps, LY, push, nullptr);
+}
+// handles with a dynamics table: the push kernel's body with the factors (an empty push table when the handle has no pushes)
+template <int W, bool TASK>
+__global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_dyn_kernel(const DevModel* __restrict__ gm, DevState st, const double* __restrict__ frame_times,
+                                                                           const float* __restrict__ frames, double dt, int n_updates, int sim_substeps, StepLayout LY,
+                                                                           DevPush* push, const DevDyn* dyn) {
+    dm_step_body<W, TASK, true, true>(gm, st, frame_times, frames, dt, n_updates, sim_substeps, LY, push, dyn);
 }
 
 const StepKernel kStepKernels[2][2] = {{dm_step_kernel<16, false>, dm_step_kernel<16, true>}, {dm_step_kernel<32, false>, dm_step_kernel<32, true>}};
 const StepPushKernel kStepPushKernels[2][2] = {{dm_step_push_kernel<16, false>, dm_step_push_kernel<16, true>}, {dm_step_push_kernel<32, false>, dm_step_push_kernel<32, true>}};
+const StepDynKernel kStepDynKernels[2][2] = {{dm_step_dyn_kernel<16, false>, dm_step_dyn_kernel<16, true>}, {dm_step_dyn_kernel<32, false>, dm_step_dyn_kernel<32, true>}};
 
 // dm_reset's part of the push table: the environments the reset kernel is about to restart (the same rule) lose their push, as cWorld::Reset
 // clears its perturbations.  Launched before the reset kernel, only on handles with a push table.
@@ -1755,6 +1805,14 @@ __global__ void dm_push_clear_kernel(DevState st, DevPush* push, int force) {
     const int env = blockIdx.x * blockDim.x + threadIdx.x;
     if (env >= st.num_real) return;
     if (force || st.flags[static_cast<size_t>(env) * kFlagInts + kFDone] != 0) push[env].body = -1;
+}
+
+// dm_reset's and dm_set_dynamics_randomization's part of a randomised dynamics table: every real environment's factors for its current episode.
+// The draw is a pure function of the environment's reset counter, so the environments the reset did not restart keep theirs.
+__global__ void dm_dyn_draw_kernel(DevState st, DevDyn* dyn, DynRand R) {
+    const int env = blockIdx.x * blockDim.x + threadIdx.x;
+    if (env >= st.num_real) return;
+    dyn_draw_env(R, R.env_base + static_cast<unsigned long long>(env), st.flags[static_cast<size_t>(env) * kFlagInts + kFResets], dyn[env]);
 }
 
 // The push schedule (dm_push.cuh): refills the empty entries of the real environments that are not frozen.  Launched at the head of every

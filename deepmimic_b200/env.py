@@ -66,6 +66,46 @@ class DeepMimicBatchEnv:
         self._pre()
         self._core.set_push_schedule(bodies, force, duration, gap)
 
+    def set_dynamics(self, friction=None, kp=None, kd=None, torque_limit=None, mass=None):
+        """Vary the dynamics per environment: friction, kp, kd and torque_limit [N] multiply the contact friction coefficient, every PD
+        controller's Kp and Kd and every joint's torque limit; mass [N, links] multiplies every body's mass (and with it both inertias).  An
+        omitted kind is 1.  Kept across resets; state_dict() carries them.  The policy's observations do not see them."""
+        N, nl = self._core.num_envs, self._core.dims.num_joints
+        f = np.ones((N, 4 + nl), dtype=np.float32)
+        for j, (name, a) in enumerate((("friction", friction), ("kp", kp), ("kd", kd), ("torque_limit", torque_limit))):
+            if a is not None:
+                a = np.asarray(a.detach().cpu().numpy() if hasattr(a, "detach") else a, dtype=np.float32)
+                if a.shape != (N,):
+                    raise ValueError("set_dynamics: %s must have shape (%d,), got %s" % (name, N, a.shape))
+                f[:, j] = a
+        if mass is not None:
+            m = np.asarray(mass.detach().cpu().numpy() if hasattr(mass, "detach") else mass, dtype=np.float32)
+            if m.shape != (N, nl):
+                raise ValueError("set_dynamics: mass must have shape (%d, %d), got %s" % (N, nl, m.shape))
+            f[:, 4:] = m
+        self._pre()
+        self._core.set_dynamics(f)
+
+    def dynamics(self):
+        """every environment's factors as device tensors: dict(friction, kp, kd, torque_limit [N], mass [N, links]).  No host synchronisation."""
+        self._pre()
+        t = self._core.dynamics()
+        self._post()
+        return dict(friction=t[:, 0], kp=t[:, 1], kd=t[:, 2], torque_limit=t[:, 3], mass=t[:, 4:])
+
+    def set_dynamics_randomization(self, friction=(1.0, 1.0), kp=(1.0, 1.0), kd=(1.0, 1.0), torque_limit=(1.0, 1.0), mass=(1.0, 1.0)):
+        """Randomise the dynamics for training: every environment draws its factors (as in set_dynamics; one mass factor per body) uniformly in
+        each kind's (lo, hi) on the device, now and at every reset, from the env's seed and its global id
+        (include/deepmimic_b200.h: dm_set_dynamics_randomization).  An omitted kind stays 1.  state_dict() carries the table."""
+        lohi = []
+        for name, p in (("friction", friction), ("kp", kp), ("kd", kd), ("torque_limit", torque_limit), ("mass", mass)):
+            p = tuple(float(v) for v in p)
+            if len(p) != 2:
+                raise ValueError("set_dynamics_randomization: %s must be a (lo, hi) pair" % name)
+            lohi += p
+        self._pre()
+        self._core.set_dynamics_randomization(lohi)
+
     def get_name(self):
         """cScene::GetName of the configured scene (SceneImitate.cpp:209, SceneImitateAMP.cpp:211, SceneTargetAMP.cpp:233, ...)"""
         return self._core.scene_name()

@@ -2,7 +2,8 @@
 
     python -m deepmimic_b200.run --arg_file args/run_humanoid3d_spinkick_args.txt [--model_files PATH] [--num_envs 64]
         [--record_motion K] [--render K [--render_size WxH] [--camera yaw,pitch,distance,height,fov_deg]] [--episode_time 20] [--backend tensor_core] [--seed 0] [--device 0] [--asset_root DIR]
-        [--push_forces F1,F2,... [--push_body 0] [--push_time 2.0] [--push_duration 0.2]] [reference arguments ...]
+        [--push_forces F1,F2,... [--push_body 0] [--push_time 2.0] [--push_duration 0.2]] [--dynamics_sweep KIND=V1,V2,...]
+        [reference arguments ...]
 
 --model_files (a reference TensorBundle prefix or a Trainer checkpoint, deepmimic_b200/model_files.py) and --output_path are read from the
 argument list, the command line before the arg file, as deepmimic_b200.train reads its paths; --train_agents and --agent_files are accepted
@@ -21,7 +22,11 @@ Push robustness (--push_forces, the DeepMimic paper's test of a trained skill): 
 with the horizontal force of magnitude F[e % K] in N, for --push_duration seconds from --push_time seconds into its episode (defaults 0.2 and
 2.0).  Each environment's direction is an angle drawn from --seed, the same every run.  run_log.txt then also has the columns Push_Force and
 Push_Dir (radians, about the vertical axis from +x towards +z), and the summary one line per force: episodes, the fraction not ended by Fail
-and the mean return."""
+and the mean return.
+
+Dynamics sweep (--dynamics_sweep KIND=V1,V2,..., KIND one of friction, kp, kd, torque_limit, mass): environment e runs with the factor V[e % K]
+on that kind (DeepMimicBatchEnv.set_dynamics; for mass, every body's factor), the others 1.  run_log.txt then also has the column Dyn_<KIND>,
+and the summary one line per value: episodes, the fraction not ended by Fail and the mean return.  It combines with --push_forces."""
 import argparse
 import os
 import sys
@@ -47,7 +52,33 @@ def build_parser():
     ap.add_argument("--push_body", type=int, default=0, help="body pushed in the sweep (default 0, the root)")
     ap.add_argument("--push_time", type=float, default=2.0, help="episode time of the push in seconds (default 2.0)")
     ap.add_argument("--push_duration", type=float, default=0.2, help="length of the push in seconds (default 0.2)")
+    ap.add_argument("--dynamics_sweep", type=parse_dynamics_sweep, default=None, metavar="KIND=V1,V2,...",
+                    help="dynamics sweep: factors on friction, kp, kd, torque_limit or mass, environment e gets V[e %% K]")
     return ap
+
+
+DYNAMICS_KINDS = ("friction", "kp", "kd", "torque_limit", "mass")
+
+
+def parse_dynamics_sweep(text):
+    """KIND=V1,V2,...: (kind, [values]); finite values >= 0, > 0 for mass"""
+    kind, _, vals = text.partition("=")
+    if kind not in DYNAMICS_KINDS:
+        raise argparse.ArgumentTypeError("need KIND=V1,V2,... with KIND one of %s, got %r" % (", ".join(DYNAMICS_KINDS), text))
+    try:
+        v = [float(x) for x in vals.split(",")]
+    except ValueError:
+        raise argparse.ArgumentTypeError("need comma-separated numbers after %s=, got %r" % (kind, text))
+    if not v or any(not (x >= 0.0) or x == float("inf") for x in v) or (kind == "mass" and min(v) <= 0.0):
+        raise argparse.ArgumentTypeError("%s factors must be finite and %s, got %r" % (kind, "> 0" if kind == "mass" else ">= 0", text))
+    return kind, v
+
+
+def dynamics_plan(sweep, num_envs):
+    """the sweep's per-environment factor [N] (environment e gets values[e % K])"""
+    import numpy as np
+    kind, values = sweep
+    return np.asarray([values[e % len(values)] for e in range(num_envs)], dtype=np.float32)
 
 
 def parse_forces(text):
@@ -134,6 +165,9 @@ def main(argv=None):
         N = opts.num_envs
         mag, ang, force = push_plan(opts.push_forces, N, opts.seed)
         env.set_pushes(np.full(N, opts.push_body, dtype=np.int32), force, np.full(N, opts.push_time), np.full(N, opts.push_duration))
+    if opts.dynamics_sweep is not None:
+        kind, fac = opts.dynamics_sweep[0], dynamics_plan(opts.dynamics_sweep, opts.num_envs)
+        env.set_dynamics(**{kind: (np.repeat(fac[:, None], env._core.dims.num_joints, axis=1) if kind == "mass" else fac)})
     ro = BatchedRollout(env, exp_rate=0.0, seed=opts.seed, backend=opts.backend)
     norms = dict(s_norm=ro.s_norm, a_norm=ro.a_norm, **(dict(g_norm=ro.g_norm) if ro.goal_size > 0 else {}))
     try:
@@ -151,6 +185,8 @@ def main(argv=None):
         if opts.push_forces is not None:
             log.log_tabular("Push_Force", float(mag[e]))
             log.log_tabular("Push_Dir", float(ang[e]))
+        if opts.dynamics_sweep is not None:
+            log.log_tabular("Dyn_" + kind, opts.dynamics_sweep[1][e % len(opts.dynamics_sweep[1])])
         log.dump_tabular()
     log.close()
     print("%s, %d episodes: return %.4f +- %.4f, length %.1f policy steps, ended by Fail %.3f" % (model_files, opts.num_envs, float(np.mean(ret)),
@@ -160,6 +196,11 @@ def main(argv=None):
             sel = mag == f
             print("push %g N on body %d at %g s for %g s: %d episodes, not ended by Fail %.3f, return %.4f" % (
                 f, opts.push_body, opts.push_time, opts.push_duration, int(sel.sum()), float(np.mean(term[sel] != 1)), float(np.mean(ret[sel]))))
+    if opts.dynamics_sweep is not None:
+        for v in opts.dynamics_sweep[1]:
+            sel = fac == np.float32(v)
+            print("%s x %g: %d episodes, not ended by Fail %.3f, return %.4f" % (kind, v, int(sel.sum()), float(np.mean(term[sel] != 1)),
+                                                                                  float(np.mean(ret[sel]))))
     if opts.record_motion:
         paths = write_episode_motions(os.path.join(out_path, "motion_%d.txt"), ep, opts.record_motion,
                                       env.get_updates_per_action() * env.UPDATE_DT)

@@ -23,7 +23,13 @@ Training under pushes: --push_force LO,HI (N), --push_bodies B1[,B2...] (body id
 gap after the previous push), all four or none, push every training environment at random (DeepMimicBatchEnv.set_push_schedule): after each
 push its environment waits a gap drawn from the interval, then a body from the list is pushed horizontally with a magnitude and for a duration
 drawn from their ranges.  The evaluation (Test_Return) runs without pushes.  The schedule is part of the run record: --resume needs the same
-four options."""
+four options.
+
+Training under randomised dynamics: --rand_friction, --rand_kp, --rand_kd, --rand_torque_limit and --rand_mass LO,HI, each optional (any one
+switches randomisation on, a kind not given stays 1), draw every training environment's factors at every reset
+(DeepMimicBatchEnv.set_dynamics_randomization; --rand_mass draws one factor per body).  The evaluation (Test_Return) runs on the nominal
+model.  The bounds are part of the run record: --resume needs the same options.  They combine with the push options.
+"""
 import argparse
 import math
 import os
@@ -135,6 +141,17 @@ def push_schedule(opts):
     return dict(bodies=opts.push_bodies, force=opts.push_force, duration=opts.push_duration, gap=opts.push_interval)
 
 
+RAND_OPTIONS = ("rand_friction", "rand_kp", "rand_kd", "rand_torque_limit", "rand_mass")
+
+
+def dynamics_randomization(opts):
+    """the Trainer's dynamics_randomization from the --rand_* options: None without any; a kind not given stays (1, 1)"""
+    given = {k[len("rand_"):]: getattr(opts, k) for k in RAND_OPTIONS if getattr(opts, k) is not None}
+    if given.get("mass") is not None and not given["mass"][0] > 0.0:
+        raise SystemExit("train: --rand_mass needs LO > 0, got %g" % given["mass"][0])
+    return given or None
+
+
 def build_parser():
     ap = argparse.ArgumentParser(prog="python -m deepmimic_b200.train", description=__doc__.split("\n\n")[0], allow_abbrev=False)
     ap.add_argument("--asset_root", default=None, help="the reference's data / args tree (default: the bundled asset archive)")
@@ -150,6 +167,10 @@ def build_parser():
     ap.add_argument("--push_duration", type=parse_range, default=None, metavar="LO,HI", help="training under pushes: push length range in s")
     ap.add_argument("--push_interval", type=parse_range, default=None, metavar="LO,HI",
                     help="training under pushes: range of the gap after an environment's previous push in s")
+    for k, what in (("friction", "contact friction"), ("kp", "every PD controller's Kp"), ("kd", "every PD controller's Kd"),
+                    ("torque_limit", "every joint's torque limit"), ("mass", "every body's mass (one factor per body)")):
+        ap.add_argument("--rand_" + k, type=parse_range, default=None, metavar="LO,HI",
+                        help="training under randomised dynamics: range of the factor on %s, drawn per environment at every reset" % what)
     return ap
 
 
@@ -167,6 +188,7 @@ def main(argv=None):
     from .trainer import AgentConfig, Trainer
     opts, scene_args = build_parser().parse_known_args(sys.argv[1:] if argv is None else argv)
     pushes = push_schedule(opts)
+    dyn = dynamics_randomization(opts)
     root = opts.asset_root or default_asset_root()
     agent_file, out_path, int_path = resolve_args(scene_args, root)
     model_files = resolve_model_files(scene_args, root)
@@ -186,7 +208,7 @@ def main(argv=None):
     ckpt = rank_path(os.path.join(out_path, "agent0_checkpoint.pt"), rank)
     tr = Trainer(scene_args, cfg, root, opts.num_envs, window_steps=opts.window_steps, backend=opts.backend, seed=opts.seed, device=device,
                  log_path=os.path.join(out_path, "agent0_log.txt"), append_log=opts.resume is not None, process_group=group, model_files=model_files,
-                 push_schedule=pushes)
+                 push_schedule=pushes, dynamics_randomization=dyn)
     if opts.resume:
         tr.load(rank_path(opts.resume, rank))
     try:

@@ -271,6 +271,26 @@ def push_schedule_record(ps):
     return out
 
 
+DYNAMICS_KINDS = ("friction", "kp", "kd", "torque_limit", "mass")
+
+
+def dynamics_record(dr):
+    """a dynamics randomisation dict(friction=(lo, hi), kp=..., kd=..., torque_limit=..., mass=...) in the run record's form: every kind a
+    [lo, hi] list of floats, an omitted kind [1, 1].  Only the form is checked here; the library refuses out-of-range bounds by name
+    (DeepMimicBatchEnv.set_dynamics_randomization)."""
+    if dr is None:
+        return None
+    if not isinstance(dr, dict) or not set(dr) <= set(DYNAMICS_KINDS):
+        raise ValueError("dynamics_randomization: a dict with keys among %s expected" % ", ".join(DYNAMICS_KINDS))
+    out = {}
+    for k in DYNAMICS_KINDS:
+        v = [float(x) for x in dr.get(k, (1.0, 1.0))]
+        if len(v) != 2:
+            raise ValueError("dynamics_randomization: %s must be a (lo, hi) pair" % k)
+        out[k] = v
+    return out
+
+
 class Trainer:
     """RLAgent's training loop over one batched environment (a reading of the reference, not checked against its source).
 
@@ -296,6 +316,10 @@ class Trainer:
     handle only (Test_Return stays an evaluation without pushes).  It joins the run record, so a checkpoint resumes only with the same schedule;
     the training handle's state blob carries the pushes drawn so far.
 
+    dynamics_randomization (train --rand_friction etc.): dict of (lo, hi) per kind of DeepMimicBatchEnv.set_dynamics_randomization, applied to
+    the training handle only (Test_Return stays an evaluation on the nominal model).  It joins the run record, so a checkpoint resumes only with
+    the same bounds; the training handle's state blob carries the factors.
+
     Several GPUs (mpi_run.py --num_workers N): process_group, a torch.distributed group of one rank per GPU.  num_envs is the job's total, which
     must be divisible by the world size; each rank steps its contiguous share (global_env_offset = rank * num_envs / world, so every
     environment's reset stream is the one it has on one GPU), and evaluates ceil(TestEpisodes / world) episodes.  The learners average the
@@ -307,7 +331,8 @@ class Trainer:
     world size and the state its rank, both of which load_state_dict() requires to match."""
 
     def __init__(self, args, config, asset_root, num_envs, window_steps=32, backend="tensor_core", seed=0, device=0, log_path=None, append_log=False,
-                 env=None, test_env=None, process_group=None, model_files=None, push_schedule=None):
+                 env=None, test_env=None, process_group=None, model_files=None, push_schedule=None,
+                 dynamics_randomization=None):
         import torch
         from .env import DeepMimicBatchEnv
         from .learner import AMPDiscLearner, DataParallel, PPOLearner
@@ -331,6 +356,9 @@ class Trainer:
         push_schedule = push_schedule_record(push_schedule)
         if push_schedule is not None:   # runs without a schedule keep the record they had
             self.run["push_schedule"] = push_schedule
+        dynamics_randomization = dynamics_record(dynamics_randomization)
+        if dynamics_randomization is not None:   # runs without randomised dynamics keep the record they had
+            self.run["dynamics_randomization"] = dynamics_randomization
         rs = self.seed + 1000 * self.rank   # the rank's generators
         cfg = config
         self.env = env = env or DeepMimicBatchEnv(self.args, local, asset_root, device=device, seed=self.seed, global_env_offset=self.rank * local)
@@ -338,6 +366,8 @@ class Trainer:
             raise ValueError("env has %d environments; this rank's share of num_envs is %d" % (env.num_envs, local))
         if push_schedule is not None:
             env.set_push_schedule(**push_schedule)
+        if dynamics_randomization is not None:
+            env.set_dynamics_randomization(**dynamics_randomization)
         S, A, G = env.get_state_size(), env.get_action_size(), env.get_goal_size()
         net = NETS[1] if G > 0 else NETS[0]
         for key in ("ActorNet", "CriticNet"):
@@ -550,6 +580,9 @@ class Trainer:
         if s["run"].get("push_schedule") != self.run.get("push_schedule"):   # a checkpoint without the key is a run without pushes
             raise ValueError("checkpoint: its run trained under the push schedule %s, this one under %s: resume with the push options the run "
                              "started with" % (s["run"].get("push_schedule"), self.run.get("push_schedule")))
+        if s["run"].get("dynamics_randomization") != self.run.get("dynamics_randomization"):   # a checkpoint without the key is a nominal run
+            raise ValueError("checkpoint: its run trained under the dynamics randomisation %s, this one under %s: resume with the --rand_* "
+                             "options the run started with" % (s["run"].get("dynamics_randomization"), self.run.get("dynamics_randomization")))
         for k in self.run:
             if s["run"].get(k, 1 if k == "world" else None) != self.run[k]:   # a checkpoint without a world size is a one-rank run's
                 raise ValueError("checkpoint: its %s differs from this run's" % ("agent file" if k == "agent" else "world size" if k == "world" else k))

@@ -128,6 +128,27 @@ int dm_get_pushes(dm_handle* h, int32_t* h_body);
  * (NULL on a handle without a schedule); any pointer may be NULL; synchronises the stream. */
 int dm_set_push_schedule(dm_handle* h, const int32_t* h_bodies, int n_bodies, const double* force2, const double* duration2, const double* gap2);
 int dm_get_push_table(dm_handle* h, int32_t* h_body, float* h_force, double* h_window, double* h_sched);
+/* Per-environment dynamics: every environment e carries 4 + links float factors, friction, kp, kd, torque_limit, then one mass factor per link.
+ * The environment steps as the model built from edited asset files would: every PD controller's Kp times kp and Kd times kd, every joint's
+ * torque limit times torque_limit, every body's mass times its mass factor (both inertia tensors follow), the contact friction coefficient
+ * (0.9 link x 0.9 ground) times friction; the imitation reward's and the task scenes' centre of mass use the environment's masses.
+ * Observations are unchanged: the policy is not told the factors.  All factors 1 is the plain model.
+ * dm_set_dynamics: explicit factors, h_factors [N x (4 + links)], kept across resets.  friction, kp, kd and torque_limit must be finite and
+ * >= 0, a mass factor finite and > 0, and a fixed leaf that the step kernel lumps into its parent (humanoid3d's wrists) must carry its parent's
+ * mass factor; a refusal names the environment, the kind and the link.  Stream-ordered, then synchronises the stream.
+ * dm_set_dynamics_randomization: lohi [10] = [lo, hi] of friction, kp, kd, torque_limit and mass (finite, >= 0, lo <= hi, mass lo > 0; a
+ * refusal names the kind).  Draws every real environment's factors for its current episode, then again at each reset: factor j of the episode
+ * with reset counter r is lo + u (hi - lo), u = splitmix64(seed ^ "dynamics", global env id, 64 r + j), j = 0..3 friction, kp, kd,
+ * torque_limit, j = 4 + l the mass factor of link l (a lumped leaf copies its parent's).  The same factors at any GPU count.  The first call
+ * of either setter allocates the table and synchronises the stream; later randomisation calls and the draws at resets do not.  The table has one owner: each of the two refuses a handle set up by the other.  The first call of either allocates the table
+ * and switches the step and observation launches to their dynamics instantiations; handles that never call them run exactly as before.
+ * dm_get_dynamics: the factors into d_out [N x (4 + links)] on the device, stream-ordered, no host synchronisation; refuses a handle without a
+ * table.  dm_save_state / dm_load_state carry the table of a handle that has one at the end of the blob; the header's dyn_table field makes a
+ * load refuse a blob with a table into a handle without one, and the reverse, and its dynamics field (0 without randomisation) a blob of
+ * another randomisation or none. */
+int dm_set_dynamics(dm_handle* h, const float* h_factors);
+int dm_get_dynamics(dm_handle* h, float* d_out);
+int dm_set_dynamics_randomization(dm_handle* h, const double* lohi);
 /* Placement of the environments in the step kernel (on by default; tile width 16 only, where two environments share a warp: tile width 32
  * handles keep index placement, where it measured slower): every step launch is preceded by a one-block kernel that orders the
  * environments by contact load -- the solver row count of each environment's last Bullet sub-step, its key -- so that environments of equal
