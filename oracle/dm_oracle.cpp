@@ -1256,6 +1256,21 @@ int dmo_check_target_succ(void* h) { return static_cast<Oracle*>(h)->CheckTarget
 int dmo_enable_amp_task_reward(void* h) { return static_cast<Oracle*>(h)->IsTask() ? 1 : 0; }   // SceneTargetAMP.cpp:222-225
 void dmo_calc_com(void* h, double* out) { orc::D3 c = static_cast<Oracle*>(h)->CalcCOM(); out[0] = c.x; out[1] = c.y; out[2] = c.z; }
 void dmo_update(void* h, double dt) { static_cast<Oracle*>(h)->Update(dt); }
+// test hook: a timed push, an external force for one Update.  cWorld::Update keeps applied forces through stepSimulation until its final
+// clearForces, and nothing in cSceneSimChar::Update before stepSimulation touches them, so the force is added to the body's link (Bullet's
+// link frame sits at the body's COM) right before the oracle's own Update and acts in both of its sub-steps.
+// One Update(dt), with force (world axes, unscaled N) times the world scale on `body` when body >= 0 and the timer value at the update's start t
+// satisfies start <= t < start + duration (the scale rule of gravity: the unscaled character sees F / m).
+void dmo_update_pushed(void* h, double dt, int body, const double* force, double start, double duration) {
+    orc::Oracle* o = static_cast<orc::Oracle*>(h);
+    const double t = o->timer_time;
+    if (body >= 0 && start <= t && t < start + duration)
+        o->mb.links[body].appliedForce += orc::F3(static_cast<float>(force[0] * o->scale), static_cast<float>(force[1] * o->scale), static_cast<float>(force[2] * o->scale));
+    o->Update(dt);
+}
+// test hook: the contact friction coefficient Bullet's solver uses for every contact (the reference's link friction times the ground's).
+// Masses, gains and torque limits need no hook: the tests edit them in a copy of the asset files.
+void dmo_set_contact_friction(void* h, double mu) { static_cast<orc::Oracle*>(h)->friction = mu; }
 void dmo_set_action(void* h, const double* a) { static_cast<Oracle*>(h)->SetAction(a); }
 void dmo_record_state(void* h, double* out) { static_cast<Oracle*>(h)->RecordState(out); }
 int dmo_amp_obs_size(void* h) { return static_cast<Oracle*>(h)->AmpObsSize(); }

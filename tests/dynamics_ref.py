@@ -1,7 +1,9 @@
 """A Python restatement of the dynamics draw (deepmimic_b200/csrc/kernels/dm_dynamics.cuh: dyn_draw_env) and of the character's part of its
 rule, for the CPU shim test and the GPU tests.  Plain IEEE double arithmetic with one rounding per operation, float32 rounding of the stored
-factors."""
+factors.  Also the edited asset tree that restates a dynamics factor set in the reference's own files."""
 import json
+import os
+import shutil
 
 import numpy as np
 
@@ -9,6 +11,7 @@ from tests.push_schedule_ref import u01
 
 DYN_SEED_KEY = 0x64796e616d696373   # "dynamics"
 KINDS = ("friction", "kp", "kd", "torque_limit", "mass")
+FRICTION = 0.9 * 0.9   # link x ground: the oracle's default contact friction
 
 
 def dyn_seed(handle_seed):
@@ -56,3 +59,24 @@ def total_mass(masses, f):
     for l, ml in enumerate(masses):
         m += float(np.float32(ml)) * float(f[4 + l])
     return np.float32(m)
+
+
+def edited_asset_tree(src_root, dst, char_file, ctrl_file, kp, kd, torque_limit, mass):
+    """a copy of the asset tree at dst with the character's Mass (times mass[link]) and TorqueLim (times torque_limit) and the controller's
+    Kp and Kd (times kp, kd) edited: the reference built from these files is the model the factors stand for"""
+    shutil.copytree(src_root, dst, copy_function=shutil.copyfile)   # the files without their modes: the tree may be read-only
+    cp = os.path.join(dst, char_file)
+    c = json.load(open(cp))
+    for b in c["BodyDefs"]:
+        b["Mass"] = float(b["Mass"]) * float(mass[b["ID"]])
+    for j in c["Skeleton"]["Joints"]:
+        if "TorqueLim" in j:
+            j["TorqueLim"] = float(j["TorqueLim"]) * float(torque_limit)
+    json.dump(c, open(cp, "w"), indent=1)
+    kp_ = os.path.join(dst, ctrl_file)
+    k = json.load(open(kp_))
+    for p in k["PDControllers"]:
+        p["Kp"] = float(p["Kp"]) * float(kp)
+        p["Kd"] = float(p["Kd"]) * float(kd)
+    json.dump(k, open(kp_, "w"), indent=1)
+    return dst

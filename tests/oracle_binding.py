@@ -1,23 +1,22 @@
 """ctypes binding of the CPU oracle (oracle/libdm_oracle.so).  TEST INFRASTRUCTURE: only tests/,
 __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may import this."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from deepmimic_b200.build import build_oracle
+from tests.dynamics_ref import FRICTION
+
 _LIB = None
 
 
 def load_oracle():
+    """the oracle library, loaded once per process after `make` in oracle/: a change to the oracle or to a header it includes rebuilds it,
+    and a current library is loaded as it is"""
     global _LIB
     if _LIB is not None:
         return _LIB
-    path = os.path.join(REPO, "oracle", "libdm_oracle.so")
-    if not os.path.exists(path):
-        subprocess.check_call(["make"], cwd=os.path.join(REPO, "oracle"))
-    L = C.CDLL(path)
+    L = C.CDLL(build_oracle())
     L.dmo_create.restype = C.c_void_p
     L.dmo_create.argtypes = [C.c_char_p, C.c_int, C.POINTER(C.c_char_p)]
     L.dmo_last_error.restype = C.c_char_p
@@ -27,6 +26,8 @@ def load_oracle():
     L.dmo_set_task_stream.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64]
     L.dmo_task_counter.restype = C.c_uint64
     L.dmo_task_counter.argtypes = [C.c_void_p]
+    L.dmo_update_pushed.argtypes = [C.c_void_p, C.c_double, C.c_int, C.POINTER(C.c_double), C.c_double, C.c_double]
+    L.dmo_set_contact_friction.argtypes = [C.c_void_p, C.c_double]
     _LIB = L
     return L
 
@@ -148,6 +149,10 @@ class Oracle:
 
     def update(self, dt):
         self.L.dmo_update(self.h, C.c_double(dt))
+
+    def set_friction(self, factor):
+        """the contact friction coefficient becomes 0.81 x factor"""
+        self.L.dmo_set_contact_friction(self.h, C.c_double(FRICTION * float(factor)))
 
     def set_action(self, a):
         a = np.ascontiguousarray(a, dtype=np.float64)
@@ -296,3 +301,27 @@ class Oracle:
         jt = np.ascontiguousarray(joint_tau, dtype=np.float32); out = np.zeros(self.num_dofs, dtype=np.float32)
         self.L.dmo_bullet_aba(self.h, fp(jt), 1 if with_gravity else 0, fp(out))
         return out
+
+
+class PushOracle(Oracle):
+    """Oracle with set_push: like the device's push table, a push acts in every update whose timer value at its start t satisfies
+    start <= t < start + duration, and a reset clears it (cWorld::Reset clears its perturbations)"""
+    _push = None
+
+    def set_push(self, body, force, start, duration):
+        """push body `body` (-1: none) with `force` (world axes, unscaled N) at its COM in every update whose timer value at its start t
+        satisfies start <= t < start + duration"""
+        self._push = None if body < 0 else (int(body), np.ascontiguousarray(force, dtype=np.float64), float(start), float(duration))
+
+    def push_body(self):
+        return -1 if self._push is None else self._push[0]
+
+    def reset(self, *a, **k):
+        super().reset(*a, **k)
+        self._push = None
+
+    def update(self, dt):
+        if self._push is None:
+            return super().update(dt)
+        b, f, s, d = self._push
+        self.L.dmo_update_pushed(self.h, C.c_double(dt), b, dp(f), C.c_double(s), C.c_double(d))

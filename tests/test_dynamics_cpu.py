@@ -3,25 +3,20 @@
 environment's argument checks; and the ptxas resources of the dynamics step kernels."""
 import ctypes as C
 import os
-import re
-import subprocess
 
 import numpy as np
 import pytest
 
 from tests import dynamics_ref as ref
-from tests.test_step_resources_cpu import nvcc
+from tests.native import nvcc, ptxas_report, shared_library
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 @pytest.fixture(scope="module")
-def shim(tmp_path_factory):
+def shim():
     """dm_dynamics.cuh compiled with g++ (no contraction of a product into an add, as on the device with its explicit roundings)"""
-    so = str(tmp_path_factory.mktemp("dyn_shim") / "libdynamics_shim.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-shared", "-fPIC", "-x", "c++", os.path.join(HERE, "dynamics_shim.cpp"),
-                           "-o", so])
-    L = C.CDLL(so)
+    L = shared_library(os.path.join(HERE, "dynamics_shim.cpp"), ["-O2", "-ffp-contract=off"])
     dp, ip, fp = C.POINTER(C.c_double), C.POINTER(C.c_int), C.POINTER(C.c_float)
     L.shim_dyn_draw.argtypes = [dp, C.c_uint64, C.c_uint64, C.c_int, C.c_int, ip, fp, fp]
     L.shim_dyn_seed_key.restype = C.c_uint64
@@ -130,22 +125,16 @@ def test_dynamics_step_kernel_resources(tmp_path):
     """ptxas's figures for the four dynamics step kernels, pinned at what they reach: 128 registers each (the launch plan's count); for the
     imitate instantiations no stack beyond the W = 32 kernel's 40 B sin / cos frame (W = 16: 48 B with 12 B of spills around the collision
     pass) and none in their routines.  The task instantiations keep the task code's frame, as the push kernels do."""
-    from tests.test_step_resources_cpu import CSRC, makefile_flags
-    r = subprocess.run([nvcc()] + makefile_flags() + ["-Xptxas", "-v", "-c", os.path.join("kernels", "dm_step.cu"), "-o", str(tmp_path / "o.o")],
-                       cwd=CSRC, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert r.returncode == 0, r.stdout[-4000:]
+    rep = ptxas_report(os.path.join("kernels", "dm_step.cu"), str(tmp_path))
     want = {(16, 0): (48, 12, 12), (32, 0): (40, 0, 0), (16, 1): (352, 24, 0), (32, 1): (368, 36, 0)}
     for (w, task), (frame, stores, loads) in want.items():
-        m = re.search(r"Compiling entry function '(\S*dm_step_dyn_kernelILi%dELb%dE\S*)'(.*?)(?=Compiling entry function|\Z)" % (w, task), r.stdout, re.S)
-        assert m, (w, task)
-        entry, body = m.group(1), m.group(2)
-        funcs = re.findall(r"Function properties for (\S+)\n\s+(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", body)
-        assert funcs[0][0] == entry and tuple(int(x) for x in funcs[0][1:]) == (frame, stores, loads), (w, task, funcs[0])
-        regs = re.search(r"Used (\d+) registers", body)
-        assert regs and int(regs.group(1)) == 128, (w, task, regs and regs.group(1))
+        (entry,) = [e for e in rep if "dm_step_dyn_kernelILi%dELb%dE" % (w, task) in e]
+        regs, funcs = rep[entry]
+        assert funcs[0][0] == entry and funcs[0][1:] == (frame, stores, loads), (w, task, funcs[0])
+        assert regs == 128, (w, task, regs)
         if not task:   # the imitate routines store nothing to local memory
             for callee, cfr, cst, cld in funcs[1:]:
-                assert int(cfr) == 0 and int(cst) == 0, (w, task, callee, cfr, cst)
+                assert cfr == 0 and cst == 0, (w, task, callee, cfr, cst)
 
 def test_train_rand_options_parse_and_refuse(capsys):
     """--rand_* options: each optional, any one switches randomisation on, kinds not given stay 1; bad ranges and a mass lo of 0 refused"""

@@ -248,7 +248,7 @@ def test_factors_match_the_oracle_built_from_edited_assets(asset_root, tmp_path,
     import json
     import torch
     from deepmimic_b200.capi import BatchedCore
-    from tests.dynamics_oracle import DynamicsOracle, edited_asset_tree
+    from tests.oracle_binding import Oracle
     name, args, char, ctrl, placement = case
     char_file = "data/characters/%s.txt" % char
     if ctrl is None:   # the scene's own controller file, from its arg file
@@ -264,9 +264,9 @@ def test_factors_match_the_oracle_built_from_edited_assets(asset_root, tmp_path,
         if p >= 0:
             mass[l] = mass[p]
     fr, kp, kd, tl = 0.6, 1.2, 0.8, 0.9
-    tree = edited_asset_tree(asset_root, str(tmp_path / "assets"), char_file, ctrl_file, kp, kd, tl, mass)
+    tree = ref.edited_asset_tree(asset_root, str(tmp_path / "assets"), char_file, ctrl_file, kp, kd, tl, mass)
     assert json.load(open(os.path.join(tree, char_file)))["BodyDefs"][1]["Mass"] != json.load(open(os.path.join(asset_root, char_file)))["BodyDefs"][1]["Mass"]
-    orc = DynamicsOracle(args, tree)
+    orc = Oracle(args, tree)
     orc.set_friction(fr)
     N = 64
     core = BatchedCore(args, N, asset_root, device=0, seed=1)

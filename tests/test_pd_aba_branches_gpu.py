@@ -25,7 +25,7 @@ import numpy as np
 import pytest
 
 from tests import char_shapes as C
-from tests.oracle_binding import Oracle
+from tests.oracle_binding import Oracle, PushOracle
 from tests.parity_util import SnapLayout, compare_sim_state
 
 pytestmark = pytest.mark.gpu
@@ -159,7 +159,6 @@ def test_partners_do_not_change_an_environments_result(roots):
 
 def test_push_kernel_on_each_body_class(roots):
     """c32: 10 is a leaf lumped into spherical 7, 4 a fixed leaf under fixed 1, 5 a fixed leaf under the root, 1 a fixed link with children"""
-    from tests.push_oracle import PushOracle
     name = "c32"
     args = C.args_of(name)
     root = roots[0]
@@ -199,8 +198,7 @@ def test_push_kernel_on_each_body_class(roots):
 
 @pytest.mark.parametrize("name", ["c16", "c32"])
 def test_dynamics_kernel_matches_the_oracle_built_from_edited_assets(roots, tmp_path, name):
-    from tests.dynamics_oracle import DynamicsOracle, edited_asset_tree
-    from tests.dynamics_ref import lumped_leaves
+    from tests.dynamics_ref import edited_asset_tree, lumped_leaves
     import os
     root = roots[0]
     args = C.args_of(name)
@@ -213,7 +211,7 @@ def test_dynamics_kernel_matches_the_oracle_built_from_edited_assets(roots, tmp_
             mass[l] = mass[p]
     kp, kd, tl = 1.2, 0.8, 0.9
     tree = edited_asset_tree(root, str(tmp_path / "edited"), C.char_file(name), "data/controllers/%s_ctrl.txt" % name, kp, kd, tl, mass)
-    orc, orc2 = DynamicsOracle(args, tree), DynamicsOracle(args, tree)
+    orc, orc2 = Oracle(args, tree), Oracle(args, tree)
     J = C.load_joints(root, name)
     lay = SnapLayout(nl); jt = [j["Type"] for j in J]
     states = [st for st in C.library(Oracle(args, root), root, name) if st.cls in ("free", "clamp", "rev_wrap", "integ")]

@@ -3,7 +3,7 @@
 import numpy as np
 import pytest
 
-from tests.push_oracle import PushOracle
+from tests.oracle_binding import PushOracle
 
 SPINKICK = ["--arg_file", "args/run_humanoid3d_spinkick_args.txt"]
 # The semi-implicit Bullet step conserves the linear momentum only up to terms of second order in the step (the second sub-step's velocities

@@ -8,7 +8,7 @@ import sys
 import numpy as np
 import pytest
 
-from tests.push_oracle import PushOracle
+from tests.oracle_binding import PushOracle
 from tests.parity_util import SnapLayout, compare_sim_state, joint_types_from_assets, random_policy_action
 from tests.test_run_cpu import _bundle, _fixture
 

@@ -3,24 +3,21 @@
 Trainer's run record with and without a schedule, and the refusal of a checkpoint from another schedule."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from tests import push_schedule_ref as ref
+from tests.native import shared_library
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 DT = 1.0 / 600.0
 
 
 @pytest.fixture(scope="module")
-def shim(tmp_path_factory):
+def shim():
     """dm_push.cuh compiled with g++ (no contraction of a product into an add, as on the device with its explicit roundings)"""
-    so = str(tmp_path_factory.mktemp("push_shim") / "libpush_schedule_shim.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-shared", "-fPIC", "-x", "c++", os.path.join(HERE, "push_schedule_shim.cpp"),
-                           "-o", so])
-    L = C.CDLL(so)
+    L = shared_library(os.path.join(HERE, "push_schedule_shim.cpp"), ["-O2", "-ffp-contract=off"])
     dp, ip = C.POINTER(C.c_double), C.POINTER(C.c_int)
     L.shim_push_schedule.argtypes = [ip, C.c_int, dp, C.c_uint64, C.c_uint64, C.c_int, C.c_double, dp, ip, C.POINTER(C.c_float), dp]
     L.shim_push_seed_key.restype = C.c_uint64

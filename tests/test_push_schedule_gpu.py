@@ -5,8 +5,8 @@ import numpy as np
 import pytest
 
 from tests import push_schedule_ref as ref
+from tests.oracle_binding import PushOracle
 from tests.parity_util import SnapLayout, compare_sim_state, joint_types_from_assets, random_policy_action
-from tests.push_oracle import PushOracle
 from tests.test_train_gpu import AGENT, SPINKICK_TRAIN, _equal_states, _trainer
 
 pytestmark = pytest.mark.gpu

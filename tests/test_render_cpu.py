@@ -239,10 +239,10 @@ def test_render_handle_arguments_leave_the_motion_file_to_the_command(asset_root
 # ---- resources
 
 def test_render_kernel_keeps_out_of_local_memory(tmp_path):
-    from tests.test_step_resources_cpu import nvcc, ptxas_report
+    from tests.native import nvcc, ptxas_report
     if nvcc() is None:
         pytest.skip("needs nvcc")
     rep = ptxas_report(os.path.join("kernels", "dm_render.cu"), str(tmp_path))
     (entry,) = [e for e in rep if "dm_render_kernel" in e]
-    for name, stack, stores, loads in rep[entry]:
+    for name, stack, stores, loads in rep[entry][1]:
         assert stack == 0 and stores == 0 and loads == 0, (name, stack, stores, loads)

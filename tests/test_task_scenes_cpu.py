@@ -313,15 +313,12 @@ def test_pretrained_heading_policy_follows_heading_and_speed_in_the_oracle(seed,
 
 # ------------------------------------------------------------------------------------------------ device-side task logic, run on the host
 @pytest.fixture(scope="module")
-def task_shim(tmp_path_factory):
+def task_shim():
     """deepmimic_b200/csrc/kernels/dm_task.cuh (what the TASK instantiation of dm_step_kernel and the dm_task_* kernels execute per
     environment) compiled with g++ through tests/task_shim.cpp."""
     import ctypes as C
-    import subprocess
-    here = os.path.dirname(os.path.abspath(__file__))
-    so = str(tmp_path_factory.mktemp("shim") / "libtask_shim.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-x", "c++", os.path.join(here, "task_shim.cpp"), "-o", so])
-    L = C.CDLL(so)
+    from tests.native import shared_library
+    L = shared_library(os.path.join(os.path.dirname(os.path.abspath(__file__)), "task_shim.cpp"), ["-O2"])
     d, dp_, u64 = C.c_double, C.POINTER(C.c_double), C.c_uint64
     L.shim_reset.argtypes = [dp_, dp_, u64, u64, d, d]
     L.shim_update.argtypes = [dp_, dp_, u64, u64, d, d, d]
