@@ -64,7 +64,7 @@ class DmCamera(C.Structure):
 
 
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
-           "dm_update", "dm_set_pushes", "dm_get_pushes", "dm_set_push_schedule", "dm_get_push_table", "dm_set_dynamics", "dm_get_dynamics", "dm_set_dynamics_randomization", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_record_pose", "dm_render_poses", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
+           "dm_update", "dm_set_pushes", "dm_get_pushes", "dm_set_push_schedule", "dm_get_push_table", "dm_set_dynamics", "dm_get_dynamics", "dm_set_dynamics_randomization", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_record_pose", "dm_render_poses", "dm_record_kin_pose", "dm_pose_error", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
            "dm_set_snapshot", "dm_state_size", "dm_save_state", "dm_load_state", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
            "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy", "dm_td_lambda_returns", "dm_mlp_set_weights_device", "dm_learn_create",
            "dm_mlp_set_normalizers_device", "dm_learn_set_weights", "dm_learn_step", "dm_learn_disc_step", "dm_learn_destroy",
@@ -114,6 +114,9 @@ def lib():
             L.dm_set_dynamics_randomization.argtypes = [vp, dp]
         if hasattr(L, "dm_render_poses"):   # likewise a library built before the renderer
             L.dm_render_poses.argtypes = [vp, C.c_int, C.c_void_p, C.POINTER(DmCamera), C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+        if hasattr(L, "dm_pose_error"):   # and before the tracking error
+            L.dm_record_kin_pose.argtypes = [vp, fp]
+            L.dm_pose_error.argtypes = [vp, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.dm_plan_env_order.argtypes = [C.POINTER(C.c_int), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)]
         L.dm_get_env_order.argtypes = [vp, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.dm_record_state.argtypes = [vp, fp]
@@ -428,6 +431,40 @@ class BatchedCore:
                 _check_device_f32(t, "record_pose: " + name, (self.num_envs, P))
         self._chk(lib().dm_record_pose(self.h, C.c_void_p(pose.data_ptr()) if pose is not None else None,
                                        C.c_void_p(vel.data_ptr()) if vel is not None else None))
+
+    def record_kin_pose(self, pose):
+        """dm_record_kin_pose: the kinematic characters' poses (the clip at every environment's kin time, in the world; what the imitation reward
+        compares against) in record_pose's layout into a contiguous float32 CUDA tensor [N, pose_dim].  Stream-ordered on the handle's stream."""
+        _check_device_f32(pose, "record_kin_pose: pose", (self.num_envs, self.dims.pose_dim))
+        self._chk(lib().dm_record_kin_pose(self.h, C.c_void_p(pose.data_ptr())))
+
+    def pose_error(self, a, r, lengths, lock=None, dtw=None):
+        """dm_pose_error: the phase-locked and the time-warped tracking error in metres of n episodes, a and r [T, n, pose_dim] pose rows (contiguous
+        float32 tensors on the handle's device, record_pose's layout), lengths [n] int32 frames.  Returns (lock [n], dtw [n]) float32; pass tensors
+        to fill them in place, or False to skip that output.  A length outside [1, T] gives NaN.  Stream-ordered on the handle's stream."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        P = self.dims.pose_dim
+        if a.dim() != 3 or a.shape[2] != P:
+            raise ValueError("pose_error: a must be [T, n, %d], got %s" % (P, tuple(a.shape)))
+        T, n = a.shape[0], a.shape[1]
+        _check_device_f32(a, "pose_error: a", device=dev)
+        _check_device_f32(r, "pose_error: r", (T, n, P), device=dev)
+        if (not isinstance(lengths, torch.Tensor) or lengths.dtype != torch.int32 or tuple(lengths.shape) != (n,) or lengths.device != dev
+                or not lengths.is_contiguous()):
+            raise ValueError("pose_error: lengths must be a contiguous int32 tensor of shape (%d,) on %s" % (n, dev))
+        outs = []
+        for name, t in (("lock", lock), ("dtw", dtw)):
+            if t is False:
+                outs.append(None)
+                continue
+            if t is None:
+                t = torch.empty(n, dtype=torch.float32, device=dev)
+            _check_device_f32(t, "pose_error: " + name, (n,), device=dev)
+            outs.append(t)
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+        self._chk(lib().dm_pose_error(self.h, T, n, ptr(a), ptr(r), ptr(lengths), ptr(outs[0]), ptr(outs[1])))
+        return outs[0], outs[1]
 
     def render_poses(self, pose, camera=None, width=640, height=360, rgb=None, ids=None):
         """dm_render_poses: pose rows [V, pose_dim] (a contiguous float32 tensor on the handle's device, dm_record_pose's layout) drawn as this handle's

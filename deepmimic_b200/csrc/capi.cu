@@ -21,6 +21,7 @@
 #include "../../include/deepmimic_b200.h"
 #include "host/assets.hpp"
 #include "kernels/dm_model.cuh"
+#include "kernels/dm_pose_error.cuh"
 #include "kernels/dm_render.cuh"
 
 namespace dmk {
@@ -1119,6 +1120,44 @@ int dm_render_poses(dm_handle* h, int n_views, const float* d_pose, const dm_cam
     const dim3 grid(((width + T - 1) / T) * ((height + T - 1) / T), n_views);
     dmk::dm_render_kernel<<<grid, T * T, 0, h->stream>>>(h->d_model, d_pose, width, height, rc, d_rgb, d_ids);
     DM_CUDA(cudaGetLastError());
+    return 0;
+}
+int dm_record_kin_pose(dm_handle* h, float* d_pose) {
+    DM_DEVICE(h);
+    if (d_pose == nullptr) return 0;
+    const int threads = 256, total = h->num_envs * h->hm.nl;
+    dmk::kKinPoseKernels[task_scene(h)]<<<(total + threads - 1) / threads, threads, 0, h->stream>>>(h->d_model, h->st, h->d_frame_times, h->d_frames,
+                                                                                                   h->d_frame_vel, d_pose, h->num_envs);
+    return launched(h);
+}
+int dm_pose_error(dm_handle* h, int T, int n, const float* d_a, const float* d_r, const int32_t* d_len, float* d_lock, float* d_dtw) {
+    DM_DEVICE(h);
+    auto refuse = [](const std::string& what) { g_err = "dm_pose_error: " + what; return fail(); };
+    if (T < 1) return refuse("T " + std::to_string(T) + " < 1");
+    if (n < 1) return refuse("n " + std::to_string(n) + " < 1");
+    if (d_a == nullptr) return refuse("d_a is NULL");
+    if (d_r == nullptr) return refuse("d_r is NULL");
+    if (d_len == nullptr) return refuse("d_len is NULL");
+    const int nj = h->hm.nl - 1;
+    if (nj < 1) return refuse("the character has no joint besides the root");
+    if (d_lock == nullptr && d_dtw == nullptr) return 0;
+    const size_t rows = static_cast<size_t>(T) * n, F = 3 * static_cast<size_t>(nj);
+    if ((rows + dmk::kPoseFeatureThreads / 32 - 1) / (dmk::kPoseFeatureThreads / 32) > 0x7fffffffu) return refuse("T x n too large");
+    // scratch from the stream's memory pool, released in stream order: both sequences' features [2][n][T][F] and the DP's boundary rows [n][T]
+    float* scratch = nullptr;
+    DM_CUDA(cudaMallocAsync(&scratch, sizeof(float) * (2 * rows * F + rows), h->stream));
+    const unsigned fblocks = static_cast<unsigned>((rows + dmk::kPoseFeatureThreads / 32 - 1) / (dmk::kPoseFeatureThreads / 32));
+    dmk::dm_pose_feature_kernel<<<dim3(fblocks, 2), dmk::kPoseFeatureThreads, 0, h->stream>>>(h->d_model, d_a, d_r, T, n, scratch);
+    const size_t smem = dmk::dm_pose_dtw_smem(nj);
+    const dmk::PoseDtwKernel kern = dmk::kPoseDtwKernels[nj <= 15 ? 0 : 1];
+    cudaError_t err = cudaGetLastError();
+    if (err == cudaSuccess) err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    if (err == cudaSuccess) {
+        kern<<<n, dmk::kPoseDtwThreads, smem, h->stream>>>(scratch, T, n, nj, d_len, scratch + 2 * rows * F, d_lock, d_dtw);
+        err = cudaGetLastError();
+    }
+    DM_CUDA(cudaFreeAsync(scratch, h->stream));
+    DM_CUDA(err);
     return 0;
 }
 // cSceneImitate::CalcRewardImitate in every scene: in the AMP task scenes (where CalcReward is the task reward) against the environment's

@@ -217,6 +217,8 @@ __global__ void dm_env_order_kernel(const int* load, int n_padded, int tiles, in
 __global__ void dm_set_action_kernel(const DevModel*, DevState, const float*, int);
 constexpr int kPoseEnvsPerBlock = 8;   // dm_pose_kernel: kPoseEnvsPerBlock x links threads, 2 pose_dim floats of shared memory per environment
 __global__ void dm_pose_kernel(const DevModel*, DevState, float*, float*, int);
+using KinPoseKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, float*, int);
+extern const KinPoseKernel kKinPoseKernels[2];   // dm_kin_pose_kernel: [clip dataset]
 __global__ void dm_task_reset_kernel(const DevModel*, DevState, int);
 __global__ void dm_push_clear_kernel(DevState, DevPush*, int);
 __global__ void dm_push_schedule_kernel(DevState, DevPush*, double*, PushSchedule);

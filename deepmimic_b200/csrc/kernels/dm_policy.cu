@@ -158,6 +158,54 @@ template <bool CLIPS> struct ClipPick;
 template <> struct ClipPick<false> { static __device__ __forceinline__ const DevModel& get(const DevModel& m, const ClipModel&) { return m; } };
 template <> struct ClipPick<true> { static __device__ __forceinline__ const ClipModel& get(const DevModel&, const ClipModel& c) { return c; } };
 
+// The kinematic character at the environment's kin time (cKinCharacter::CalcPose / CalcVel, KinCharacter.cpp:363-406): the clip sample of
+// joint `L` (kj; a finished non-looping clip is at rest) and the root in the world -- cycle offset of a looping clip, origin rotation and
+// position applied, quaternion with w >= 0.  CLIPS: the environment `clip_env`'s own clip of the dataset.  What dm_observe's imitation reward
+// compares against and dm_record_kin_pose writes.
+struct KinSample {
+    KinJoint kj;
+    V3 org, kroot, kroot_v, kroot_w;
+    Q4 krootq;
+};
+template <bool CLIPS>
+__device__ __forceinline__ KinSample kin_sample(const DevModel& M, const DevLink& L, const DevState& st, const double* __restrict__ frame_times,
+                                                const float* __restrict__ frames, const float* __restrict__ frame_vel, const double* tm, int clip_env,
+                                                bool is_root) {
+    KinSample s;
+    ClipModel CM;
+    if constexpr (CLIPS) {
+        const ClipInfo& ci = st.ctab->info[st.clip[clip_env]];
+        CM = clip_model(ci, M.pose_dim, M.query_dt);
+        frame_times += ci.frame_off; frames += static_cast<size_t>(ci.frame_off) * M.pose_dim; frame_vel += static_cast<size_t>(ci.frame_off) * M.pose_dim;
+    }
+    const auto& KM = ClipPick<CLIPS>::get(M, CM);
+    int idx, cyc; double bld;
+    frame_index(KM, frame_times, tm[kTKin], idx, bld, cyc);
+    bld = fmin(fmax(bld, 0.0), 1.0);
+    const float bl = static_cast<float>(bld);
+    const float* f0 = frames + static_cast<size_t>(idx) * M.pose_dim; const float* f1 = f0 + M.pose_dim;
+    const float* v0 = frame_vel + static_cast<size_t>(idx) * M.pose_dim; const float* v1 = v0 + M.pose_dim;
+    const bool clip_over = !KM.loop_motion && tm[kTKin] >= KM.motion_dur;
+    s.kj = sample_joint(L, f0, f1, v0, v1, bl, is_root);
+    if (clip_over) { s.kj.w = mk3(0, 0, 0); s.kj.angvel = 0; }
+    const Q4 orot = mkq(static_cast<float>(tm[kTOriginRot + 1]), static_cast<float>(tm[kTOriginRot + 2]), static_cast<float>(tm[kTOriginRot + 3]), static_cast<float>(tm[kTOriginRot]));
+    s.org = mk3(static_cast<float>(tm[kTOrigin]), static_cast<float>(tm[kTOrigin + 1]), static_cast<float>(tm[kTOrigin + 2]));
+    // kinematic root in the world
+    V3 kroot = mk3((1 - bl) * f0[0] + bl * f1[0] + (KM.loop_motion ? cyc * KM.cycle_delta[0] : 0.f), (1 - bl) * f0[1] + bl * f1[1],
+                   (1 - bl) * f0[2] + bl * f1[2] + (KM.loop_motion ? cyc * KM.cycle_delta[2] : 0.f));
+    s.kroot = qrot(orot, kroot) + s.org;
+    V3 kroot_v = mk3((1 - bl) * v0[0] + bl * v1[0], (1 - bl) * v0[1] + bl * v1[1], (1 - bl) * v0[2] + bl * v1[2]);
+    if (clip_over) kroot_v = mk3(0, 0, 0);
+    s.kroot_v = qrot(orot, kroot_v);
+    {
+        KinJoint kr = sample_joint(M.link[0], f0, f1, v0, v1, bl, true);
+        s.krootq = qmul(orot, kr.q);
+        if (s.krootq.w < 0) s.krootq = mkq(-s.krootq.x, -s.krootq.y, -s.krootq.z, -s.krootq.w);
+        s.kroot_w = clip_over ? mk3(0, 0, 0) : qrot(orot, kr.w);
+    }
+    return s;
+}
+
 }  // namespace
 
 // obs: [N x state_size] floats, reward: [N] floats.  Either pointer may be null.
@@ -276,38 +324,10 @@ __device__ __forceinline__ void observe_body(const DevModel* __restrict__ gm, De
     if (!want_reward) return;
 
     // ---- mocap frame at kin_time
-    ClipModel CM;
-    if constexpr (CLIPS) {
-        const ClipInfo& ci = st.ctab->info[st.clip[env < num_real_envs ? env : 0]];
-        CM = clip_model(ci, M.pose_dim, M.query_dt);
-        frame_times += ci.frame_off; frames += static_cast<size_t>(ci.frame_off) * M.pose_dim; frame_vel += static_cast<size_t>(ci.frame_off) * M.pose_dim;
-    }
-    const auto& KM = ClipPick<CLIPS>::get(M, CM);
-    int idx, cyc; double bld;
-    frame_index(KM, frame_times, tm[kTKin], idx, bld, cyc);
-    bld = fmin(fmax(bld, 0.0), 1.0);
-    const float bl = static_cast<float>(bld);
-    const float* f0 = frames + static_cast<size_t>(idx) * M.pose_dim; const float* f1 = f0 + M.pose_dim;
-    const float* v0 = frame_vel + static_cast<size_t>(idx) * M.pose_dim; const float* v1 = v0 + M.pose_dim;
-    const bool clip_over = !KM.loop_motion && tm[kTKin] >= KM.motion_dur;
-    KinJoint kj = sample_joint(L, f0, f1, v0, v1, bl, lane == 0);
-    if (clip_over) { kj.w = mk3(0, 0, 0); kj.angvel = 0; }
-    const Q4 orot = mkq(static_cast<float>(tm[kTOriginRot + 1]), static_cast<float>(tm[kTOriginRot + 2]), static_cast<float>(tm[kTOriginRot + 3]), static_cast<float>(tm[kTOriginRot]));
-    const V3 org = mk3(static_cast<float>(tm[kTOrigin]), static_cast<float>(tm[kTOrigin + 1]), static_cast<float>(tm[kTOrigin + 2]));
-    // kinematic root in the world
-    V3 kroot = mk3((1 - bl) * f0[0] + bl * f1[0] + (KM.loop_motion ? cyc * KM.cycle_delta[0] : 0.f), (1 - bl) * f0[1] + bl * f1[1],
-                   (1 - bl) * f0[2] + bl * f1[2] + (KM.loop_motion ? cyc * KM.cycle_delta[2] : 0.f));
-    kroot = qrot(orot, kroot) + org;
-    V3 kroot_v = mk3((1 - bl) * v0[0] + bl * v1[0], (1 - bl) * v0[1] + bl * v1[1], (1 - bl) * v0[2] + bl * v1[2]);
-    if (clip_over) kroot_v = mk3(0, 0, 0);
-    kroot_v = qrot(orot, kroot_v);
-    Q4 krootq = mkq(0, 0, 0, 1); V3 kroot_w = mk3(0, 0, 0);
-    {
-        KinJoint kr = sample_joint(M.link[0], f0, f1, v0, v1, bl, true);
-        krootq = qmul(orot, kr.q);
-        if (krootq.w < 0) krootq = mkq(-krootq.x, -krootq.y, -krootq.z, -krootq.w);
-        kroot_w = clip_over ? mk3(0, 0, 0) : qrot(orot, kr.w);
-    }
+    const KinSample ks = kin_sample<CLIPS>(M, L, st, frame_times, frames, frame_vel, tm, env < num_real_envs ? env : 0, lane == 0);
+    const KinJoint kj = ks.kj;
+    const V3 org = ks.org, kroot = ks.kroot, kroot_v = ks.kroot_v, kroot_w = ks.kroot_w;
+    const Q4 krootq = ks.krootq;
     // ---- kinematic FK in the world: joint frames (DeepMimic tree), joint origin position, twist
     const Q4 attq = mkq(L.child_rot[0], L.child_rot[1], L.child_rot[2], L.child_rot[3]);   // joint -> body
     const V3 att_pt = mk3(L.att_pt[0], L.att_pt[1], L.att_pt[2]);
@@ -590,6 +610,28 @@ __global__ void dm_pose_kernel(const DevModel* __restrict__ gm, DevState st, flo
         if (vel) vel[base + i] = s[P];
     }
 }
+
+// pose: [num_real_envs x pose_dim] floats, the kinematic character of every environment (kin_sample: cKinCharacter's pose in the world) in
+// dm_pose_kernel's layout, quaternions with w >= 0.  One thread per (environment, joint); padding environments are not written.
+template <bool CLIPS>
+__global__ void dm_kin_pose_kernel(const DevModel* __restrict__ gm, DevState st, const double* __restrict__ frame_times, const float* __restrict__ frames,
+                                   const float* __restrict__ frame_vel, float* __restrict__ pose, int num_real_envs) {
+    const DevModel& M = *gm;
+    const int gid = blockIdx.x * blockDim.x + threadIdx.x;
+    const int env = gid / M.nl, j = gid % M.nl;
+    if (env >= num_real_envs) return;
+    const DevLink& L = M.link[j];
+    const KinSample ks = kin_sample<CLIPS>(M, L, st, frame_times, frames, frame_vel, st.time + static_cast<size_t>(env) * kTimeDoubles, env, j == 0);
+    float* p = pose + static_cast<size_t>(env) * M.pose_dim + L.pose_off;
+    if (j == 0) {
+        p[0] = ks.kroot.x; p[1] = ks.kroot.y; p[2] = ks.kroot.z;
+        p[3] = ks.krootq.w; p[4] = ks.krootq.x; p[5] = ks.krootq.y; p[6] = ks.krootq.z;
+    } else if (L.jtype == kJSpherical) {
+        const Q4 q = ks.kj.q.w < 0 ? mkq(-ks.kj.q.x, -ks.kj.q.y, -ks.kj.q.z, -ks.kj.q.w) : ks.kj.q;
+        p[0] = q.w; p[1] = q.x; p[2] = q.y; p[3] = q.z;
+    } else if (L.jtype == kJRevolute) p[0] = ks.kj.ang;
+}
+const KinPoseKernel kKinPoseKernels[2] = {dm_kin_pose_kernel<false>, dm_kin_pose_kernel<true>};
 
 // Resets every environment whose done flag is set (or all when force != 0).  kin_time_in / max_time_in (may be null) inject the
 // random draws of the reference's reset (CalcRandKinResetTime, cTimer::Reset) so tests can bypass the RNG.

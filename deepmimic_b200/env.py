@@ -176,6 +176,17 @@ class DeepMimicBatchEnv:
         self._post()
         return self._pose, self._vel
 
+    def record_kin_pose(self, agent_id=0):
+        """[N, pose_dim] float32: every kinematic character's pose (the clip at the environment's kin time, placed in the world as the imitation
+        reward compares it) in record_pose's layout.  A view of a buffer rewritten by the next call, like record_pose."""
+        if getattr(self, "_kin_pose", None) is None:
+            with self.torch.cuda.stream(self.stream):
+                self._kin_pose = self.torch.zeros(self.num_envs, self._core.dims.pose_dim, device=self.device)
+        self._pre()
+        self._core.record_kin_pose(self._kin_pose)
+        self._post()
+        return self._kin_pose
+
     def render(self, env_ids=None, **kw):
         """(rgb uint8 [V, H, W, 3], ids int16 [V, H, W]) device tensors: the current simulated characters of env_ids (default all; a sequence
         or tensor of environment indices) drawn by the device ray caster from their record_pose rows; keyword arguments are

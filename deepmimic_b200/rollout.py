@@ -539,14 +539,15 @@ class BatchedRollout:
     def stream(self):
         return self.env.stream
 
-    def collect(self, num_steps, record_stats=True, record_pose=False):
+    def collect(self, num_steps, record_stats=True, record_pose=False, record_kin_pose=False):
         """num_steps policy steps of all environments; returns dict of [T, N, .] tensors (states, actions, logps, rewards, dones, terminate,
         explore = the exploration draw of each step (True: the action was sampled, False: the mode was taken); goals
         in the goal-conditioned scenes; with a discriminator amp_obs, disc_logits, style_rewards, amp_rewards; with a critic values = V(s_k),
         end_values = V(s'_k) of the state step k ended in (before the reset), returns and advantages = returns - values).  rewards is the env's
         reward.  A path still running at the last step is bootstrapped with its end value, as the reference bootstraps a path that ends by time
         limit (a deviation: the reference stores only complete paths).  record_pose adds the simulated characters' poses (env.record_pose),
-        [T, N, pose_dim] each: poses / vels at s_k, end_poses / end_vels at s'_k, before the reset, like values / end_values."""
+        [T, N, pose_dim] each: poses / vels at s_k, end_poses / end_vels at s'_k, before the reset, like values / end_values.  record_kin_pose
+        adds kin_poses [T, N, pose_dim], the kinematic characters' poses (env.record_kin_pose) at s_k, recorded next to poses."""
         t, env = self.torch, self.env
         N, S, A = env.num_envs, env.get_state_size(), env.get_action_size()
         out = dict(states=t.empty(num_steps, N, S, device=env.device), actions=t.empty(num_steps, N, A, device=env.device),
@@ -564,6 +565,8 @@ class BatchedRollout:
             P = env.get_pose_dim()
             for key in ("poses", "vels", "end_poses", "end_vels"):
                 out[key] = t.empty(num_steps, N, P, device=env.device)
+        if record_kin_pose:
+            out["kin_poses"] = t.empty(num_steps, N, env.get_pose_dim(), device=env.device)
         crit = self.critic is not None
         if crit:
             for key in ("values", "end_values", "returns", "advantages"):
@@ -583,6 +586,8 @@ class BatchedRollout:
                 if record_pose:
                     p, v = env.record_pose()
                     out["poses"][k] = p; out["vels"][k] = v
+                if record_kin_pose:
+                    out["kin_poses"][k] = env.record_kin_pose()
                 if crit:
                     x2[:N] = s
                 if record_stats:
@@ -635,24 +640,30 @@ class BatchedRollout:
         return out
 
 
-def run_episodes(ro, pose_envs=0, limit=1 << 16):
+def run_episodes(ro, pose_envs=0, limit=1 << 16, pose_error=False):
     """One complete episode of every environment of ro's env from its current state, in chunks of 32 policy steps of ro.collect (the
     environments that finish first keep running into their next episode, which is not counted).  Set the env's mode and ro's exploration
     before the call (test mode, exp_rate 0 for an evaluation).  One host synchronisation per chunk.  Returns dict(returns [N] float32, lengths
     [N] int32 = policy steps, terminate [N] int32 = the terminate code of the episode's last step: 0 time limit, 1 fail, 2 success); with
     pose_envs > 0 also poses and end_poses of the first pose_envs environments, lists of the chunks' [32, pose_envs, pose_dim] tensors
-    (episode_motion assembles an environment's frames); the other environments' poses are not kept.
+    (episode_motion assembles an environment's frames); the other environments' poses are not kept.  pose_error=True keeps every environment's
+    poses and kin poses (the simulated and the kinematic character at the step's start, collect's poses and kin_poses) and adds pose_err and
+    pose_err_dtw [N] float32, the phase-locked and the time-warped tracking error in metres of each episode (one BatchedCore.pose_error call;
+    the terminal pose is not scored).  That keeps 2 x T x N x pose_dim floats: 2 x 428 MB at N = 4096, T = 608 and pose_dim 43 (humanoid3d),
+    plus the call's scratch of about as much again.
     RuntimeError when an episode runs longer than `limit` policy steps."""
     import torch as t
     env = ro.env
     n = env.num_envs
     ret, ended = t.zeros(n, device=env.device), t.zeros(n, dtype=t.bool, device=env.device)
     length, term = t.zeros(n, dtype=t.int32, device=env.device), t.zeros(n, dtype=t.int32, device=env.device)
-    poses, end_poses = [], []
+    poses, end_poses, all_poses, kin_poses = [], [], [], []
     for _ in range(0, limit, 32):
-        traj = ro.collect(32, record_stats=False, record_pose=True) if pose_envs else ro.collect(32, record_stats=False)
+        traj = ro.collect(32, record_stats=False, record_pose=bool(pose_envs or pose_error), record_kin_pose=pose_error)
         if pose_envs:
             poses.append(traj["poses"][:, :pose_envs].clone()); end_poses.append(traj["end_poses"][:, :pose_envs].clone())
+        if pose_error:
+            all_poses.append(traj["poses"]); kin_poses.append(traj["kin_poses"])
         for r, d, c in zip(traj["rewards"], traj["dones"], traj["terminate"]):
             ret += t.where(ended, t.zeros_like(r), r)
             length += (~ended).int()
@@ -662,6 +673,13 @@ def run_episodes(ro, pose_envs=0, limit=1 << 16):
             out = dict(returns=ret, lengths=length, terminate=term)
             if pose_envs:
                 out.update(poses=poses, end_poses=end_poses)
+            if pose_error:
+                a, r = t.cat(all_poses), t.cat(kin_poses)
+                del all_poses[:], kin_poses[:]
+                env._pre()   # the call runs on the handle's stream
+                lock, dtw = env._core.pose_error(a, r, length)
+                env._post()
+                out.update(pose_err=lock, pose_err_dtw=dtw)
             return out
     raise RuntimeError("an episode ran longer than %d policy steps" % limit)
 

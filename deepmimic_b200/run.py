@@ -2,7 +2,7 @@
 
     python -m deepmimic_b200.run --arg_file args/run_humanoid3d_spinkick_args.txt [--model_files PATH] [--num_envs 64]
         [--record_motion K] [--render K [--render_size WxH] [--camera yaw,pitch,distance,height,fov_deg]] [--episode_time 20] [--backend tensor_core] [--seed 0] [--device 0] [--asset_root DIR]
-        [--push_forces F1,F2,... [--push_body 0] [--push_time 2.0] [--push_duration 0.2]] [--dynamics_sweep KIND=V1,V2,...]
+        [--push_forces F1,F2,... [--push_body 0] [--push_time 2.0] [--push_duration 0.2]] [--dynamics_sweep KIND=V1,V2,...] [--pose_error]
         [reference arguments ...]
 
 --model_files (a reference TensorBundle prefix or a Trainer checkpoint, deepmimic_b200/model_files.py) and --output_path are read from the
@@ -26,7 +26,13 @@ and the mean return.
 
 Dynamics sweep (--dynamics_sweep KIND=V1,V2,..., KIND one of friction, kp, kd, torque_limit, mass): environment e runs with the factor V[e % K]
 on that kind (DeepMimicBatchEnv.set_dynamics; for mass, every body's factor), the others 1.  run_log.txt then also has the column Dyn_<KIND>,
-and the summary one line per value: episodes, the fraction not ended by Fail and the mean return.  It combines with --push_forces."""
+and the summary one line per value: episodes, the fraction not ended by Fail and the mean return.  It combines with --push_forces.
+
+Tracking error (--pose_error): how closely each episode followed its clip, in metres -- the mean over the non-root joints of the distance between
+the simulated and the kinematic character's joint positions relative to the root, in each one's heading frame, over the poses the episode took
+its actions in (BatchedCore.pose_error).  run_log.txt then also has the columns Pose_Err (phase-locked: frame i against the clip at the same
+moment) and Pose_Err_DTW (after aligning the two motions by dynamic time warping, which forgives a skill that runs ahead of or behind its clip's
+phase), the summary a line with the mean and standard deviation of both, and every per-force and per-value line both means."""
 import argparse
 import os
 import sys
@@ -54,6 +60,8 @@ def build_parser():
     ap.add_argument("--push_duration", type=float, default=0.2, help="length of the push in seconds (default 0.2)")
     ap.add_argument("--dynamics_sweep", type=parse_dynamics_sweep, default=None, metavar="KIND=V1,V2,...",
                     help="dynamics sweep: factors on friction, kp, kd, torque_limit or mass, environment e gets V[e %% K]")
+    ap.add_argument("--pose_error", action="store_true",
+                    help="score each episode's tracking of its clip: phase-locked and time-warped joint-position error in metres")
     return ap
 
 
@@ -174,9 +182,12 @@ def main(argv=None):
         load_model_files(model_files, ro.policy, norms)
     except ValueError as e:
         raise SystemExit("run: %s" % e)
-    ep = run_episodes(ro, pose_envs=max(opts.record_motion, opts.render))
+    ep = run_episodes(ro, pose_envs=max(opts.record_motion, opts.render), pose_error=opts.pose_error)
     torch.cuda.synchronize(env.device)
     ret, length, term = (ep[k].cpu().numpy() for k in ("returns", "lengths", "terminate"))
+    if opts.pose_error:
+        perr, perr_dtw = ep["pose_err"].cpu().numpy(), ep["pose_err_dtw"].cpu().numpy()
+    err_means = lambda sel: (", pose error %.4f m, DTW %.4f m" % (float(np.mean(perr[sel])), float(np.mean(perr_dtw[sel])))) if opts.pose_error else ""
     os.makedirs(out_path, exist_ok=True)
     log = TableLog(os.path.join(out_path, "run_log.txt"))
     for e in range(opts.num_envs):
@@ -187,20 +198,27 @@ def main(argv=None):
             log.log_tabular("Push_Dir", float(ang[e]))
         if opts.dynamics_sweep is not None:
             log.log_tabular("Dyn_" + kind, opts.dynamics_sweep[1][e % len(opts.dynamics_sweep[1])])
+        if opts.pose_error:
+            log.log_tabular("Pose_Err", float(perr[e]))
+            log.log_tabular("Pose_Err_DTW", float(perr_dtw[e]))
         log.dump_tabular()
     log.close()
     print("%s, %d episodes: return %.4f +- %.4f, length %.1f policy steps, ended by Fail %.3f" % (model_files, opts.num_envs, float(np.mean(ret)),
                                                                                               float(np.std(ret)), float(np.mean(length)), float(np.mean(term == 1))))
+    if opts.pose_error:
+        print("pose error %.4f +- %.4f m, time-warped %.4f +- %.4f m" % (float(np.mean(perr)), float(np.std(perr)), float(np.mean(perr_dtw)),
+                                                                     float(np.std(perr_dtw))))
     if opts.push_forces is not None:
         for f in opts.push_forces:
             sel = mag == f
-            print("push %g N on body %d at %g s for %g s: %d episodes, not ended by Fail %.3f, return %.4f" % (
-                f, opts.push_body, opts.push_time, opts.push_duration, int(sel.sum()), float(np.mean(term[sel] != 1)), float(np.mean(ret[sel]))))
+            print("push %g N on body %d at %g s for %g s: %d episodes, not ended by Fail %.3f, return %.4f%s" % (
+                f, opts.push_body, opts.push_time, opts.push_duration, int(sel.sum()), float(np.mean(term[sel] != 1)), float(np.mean(ret[sel])),
+                err_means(sel)))
     if opts.dynamics_sweep is not None:
         for v in opts.dynamics_sweep[1]:
             sel = fac == np.float32(v)
-            print("%s x %g: %d episodes, not ended by Fail %.3f, return %.4f" % (kind, v, int(sel.sum()), float(np.mean(term[sel] != 1)),
-                                                                                  float(np.mean(ret[sel]))))
+            print("%s x %g: %d episodes, not ended by Fail %.3f, return %.4f%s" % (kind, v, int(sel.sum()), float(np.mean(term[sel] != 1)),
+                                                                                    float(np.mean(ret[sel])), err_means(sel)))
     if opts.record_motion:
         paths = write_episode_motions(os.path.join(out_path, "motion_%d.txt"), ep, opts.record_motion,
                                       env.get_updates_per_action() * env.UPDATE_DT)
@@ -209,7 +227,10 @@ def main(argv=None):
         paths = write_episode_renders(os.path.join(out_path, "render_%d.png"), ep, opts.render, env.get_updates_per_action() * env.UPDATE_DT,
                                       env._core, opts.camera, opts.render_size)
         print("renders: %s .. %s" % (paths[0], paths[-1]))
-    return dict(returns=ret, lengths=length, terminate=term)
+    out = dict(returns=ret, lengths=length, terminate=term)
+    if opts.pose_error:
+        out.update(pose_err=perr, pose_err_dtw=perr_dtw)
+    return out
 
 
 if __name__ == "__main__":

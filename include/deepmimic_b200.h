@@ -183,6 +183,20 @@ int dm_record_pose(dm_handle* h, float* d_pose, float* d_vel);
  * fov_y outside (0, pi). */
 typedef struct { float yaw, pitch, distance, target_height, fov_y; } dm_camera;
 int dm_render_poses(dm_handle* h, int n_views, const float* d_pose, const dm_camera* cam, int width, int height, uint8_t* d_rgb, int16_t* d_ids);
+/* The kinematic character's pose (cKinCharacter::GetPose): [num_envs x pose_dim] fp32 rows in dm_record_pose's layout, every environment's clip
+ * sampled at its kin time with the loop's cycle offset and the origin rotation and position applied -- what dm_observe's imitation reward
+ * compares against; quaternions with w >= 0.  In --kin_ctrl clips scenes the environment's own clip of the dataset; past the end of a non-looping
+ * clip its last frame.  Rows past the real environments are not written; NULL is a no-op.  Stream-ordered, no host synchronisation. */
+int dm_record_kin_pose(dm_handle* h, float* d_pose);
+/* Tracking error of n episodes: d_a and d_r [T x n x pose_dim] fp32 pose rows in dm_record_pose's layout ([T, N, P]: frame t of episode e at
+ * row t n + e), d_len [n] int32 the episodes' lengths in frames.  The feature of a pose is every non-root joint's world origin minus the root's,
+ * rotated about y by minus the root's heading; the frame distance d(a, r) is the mean over those joints of the features' Euclidean distance, in
+ * metres.  d_lock [n] receives the phase-locked error (1/L) sum_i d(a_i, r_i); d_dtw [n] the time-warped error D(L-1, L-1) / 2L of the DTW
+ * recursion over the whole L x L grid, D(0, 0) = 2 d_00, D(i, j) = min(D(i-1, j-1) + 2 d_ij, D(i-1, j) + d_ij, D(i, j-1) + d_ij).  Either output
+ * may be NULL.  A length outside [1, T] gives NaN for that episode and reads nothing of it.  Deterministic: an episode's results do not depend
+ * on the rest of the batch.  Uses the handle's character only; scratch of (6 (num_joints - 1) + 1) T n floats from the device's stream-ordered
+ * memory pool.  Stream-ordered, no host synchronisation.  Refused, naming the argument: a host-only handle, T < 1, n < 1, a NULL input. */
+int dm_pose_error(dm_handle* h, int T, int n, const float* d_a, const float* d_r, const int32_t* d_len, float* d_lock, float* d_dtw);
 /* AMP task scenes target_amp / heading_amp (cSceneTargetAMP / cSceneHeadingAMP: RecordGoal, CalcReward, target updates; goal_size 3).
  * heading_amp_getup / strike_amp (cSceneHeadingAMPGetup / cSceneStrikeAMP) add a phase to the goal (goal_size 4).  dm_goal_host is RecordGoal
  * into a host buffer [num_envs x goal_size]; the task-state hooks expose one environment's task block (16 doubles: target x, z, speed, heading,
