@@ -670,7 +670,7 @@ static int create_device_state(dm_handle* h, int num_envs, int device) {
         alloc_buffer(h, &h->st.flags, N * dmk::kFlagInts, kZeroed) || alloc_buffer(h, &h->st.manifold, N * M.nl * dmk::kManifoldFloats, kZeroed) ||
         alloc_buffer(h, &h->d_frame_times, TF) || alloc_buffer(h, &h->d_frames, TF * M.pose_dim) || alloc_buffer(h, &h->d_frame_vel, TF * M.pose_dim) ||
         alloc_buffer(h, &h->d_flags4, N * 4) || alloc_buffer(h, &h->d_amp, N * M.amp_obs_size) || alloc_buffer(h, &h->p_amp, N * M.amp_obs_size, kPinned) ||
-        alloc_buffer(h, &h->st.hist, N * 2 * M.pose_dim, kZeroed) || alloc_buffer(h, &h->d_act, N * std::max(1, M.action_size)) ||
+        alloc_buffer(h, &h->st.hist, N * 2 * M.pose_dim) || alloc_buffer(h, &h->d_act, N * std::max(1, M.action_size)) ||
         alloc_buffer(h, &h->d_obs, N * M.state_size) || alloc_buffer(h, &h->d_rew, N) || alloc_buffer(h, &h->p_act, N * std::max(1, M.action_size), kPinned) ||
         alloc_buffer(h, &h->p_obs, N * M.state_size, kPinned) || alloc_buffer(h, &h->p_rew, N, kPinned) || alloc_buffer(h, &h->p_flags, N * 4, kPinned))
         return 1;
@@ -727,6 +727,15 @@ static int create_device_state(dm_handle* h, int num_envs, int device) {
         else t[0] = static_cast<float>(h->sa.ctrl.pd[j].target_theta[0]);
     }
     DM_CUDA(cudaMemcpy(h->st.sim, sim.data(), sim.size() * sizeof(float), cudaMemcpyHostToDevice));
+    // the AMP history of every environment: the identity pose at rest (cSceneImitateAMP's mPrevPose / mPrevVel before any action, which the task
+    // scenes keep across resets); the reset kernel overwrites it only in the non-task scenes (InitHist)
+    std::vector<float> hist(N * 2 * M.pose_dim, 0.f);
+    for (size_t e = 0; e < N; ++e) {
+        float* p = &hist[e * 2 * M.pose_dim];
+        p[3] = 1.f;
+        for (int j = 1; j < M.nl; ++j) if (M.link[j].jtype == dmk::kJSpherical) p[M.link[j].pose_off] = 1.f;
+    }
+    DM_CUDA(cudaMemcpy(h->st.hist, hist.data(), hist.size() * sizeof(float), cudaMemcpyHostToDevice));
     return 0;
 }
 

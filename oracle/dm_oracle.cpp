@@ -1275,6 +1275,8 @@ void dmo_set_action(void* h, const double* a) { static_cast<Oracle*>(h)->SetActi
 void dmo_record_state(void* h, double* out) { static_cast<Oracle*>(h)->RecordState(out); }
 int dmo_amp_obs_size(void* h) { return static_cast<Oracle*>(h)->AmpObsSize(); }
 void dmo_record_amp_obs_agent(void* h, double* out) { static_cast<Oracle*>(h)->RecordAMPObsAgent(out); }
+// test hook: the AMP history := the current pose / vel, as the first update after a new action sets it (cSceneImitateAMP::UpdateHist)
+void dmo_update_hist(void* h) { static_cast<Oracle*>(h)->UpdateHist(); }
 void dmo_record_amp_obs_expert(void* h, double kin_time, double* out) { static_cast<Oracle*>(h)->RecordAMPObsExpert(-1, kin_time, out); }
 void dmo_record_amp_obs_expert_clip(void* h, int clip, double kin_time, double* out) { static_cast<Oracle*>(h)->RecordAMPObsExpert(clip, kin_time, out); }
 double dmo_calc_reward(void* h) { return static_cast<Oracle*>(h)->CalcReward(); }

@@ -177,6 +177,10 @@ class Oracle:
         self.L.dmo_record_amp_obs_agent(self.h, dp(out))
         return out
 
+    def update_hist(self):
+        """the AMP history := the current pose / vel (UpdateHist, what the first update after set_action does)"""
+        self.L.dmo_update_hist(self.h)
+
     def record_amp_obs_expert(self, kin_time, clip=None):
         out = np.zeros(self.amp_obs_size())
         if clip is None:

@@ -205,61 +205,3 @@ def test_many_contacts_general_solver_path(asset_root):
     assert flips <= max(2, len(eqs) // 50)
     assert np.median(eqds) <= 2e-3 and np.percentile(eqds, 99) <= 5e-2 and eqds.max() <= 0.5
     assert core.counters()[1] == 0   # row capacity (36 rows) not exceeded
-
-
-@pytest.mark.parametrize("arg_file,extra", [("args/run_humanoid3d_spinkick_args.txt", []), ("args/train_dog3d_trot_args.txt", ["--enable_amp_obs_local_root", "true"])])
-def test_amp_observations_match_oracle(asset_root, arg_file, extra):
-    """cSceneImitateAMP::BuildAMPObs (SURVEY 8a last row): agent observation right after a reset (InitHist), after actions (UpdateHist at
-    the applied action) and the expert observation at given clip times; tolerance 2e-4 (fp32 pose / clip tables vs the oracle's f64),
-    velocities 2e-3."""
-    import torch
-    from deepmimic_b200.capi import BatchedCore
-    args = extra + ["--arg_file", arg_file]
-    N = 8
-    core = BatchedCore(args, N, asset_root, device=0, seed=9)
-    orc = Oracle(args, asset_root)
-    A = orc.amp_obs_size()
-    assert core.dims.amp_obs_size == A
-    nv = 6 + orc.pose_dim - 7
-    P = A // 2 - nv
-    times = np.linspace(0.02, 0.97 * orc.motion_duration, N)      # the first one makes the history time negative (previous cycle)
-    thetas = np.linspace(-2.5, 2.5, N) if "--enable_amp_obs_local_root" in extra else np.zeros(N)
-    core.reset(True, kin_time=times, max_time=np.full(N, 20.0), rot_theta=thetas)
-    out = torch.zeros(N, A, device="cuda")
-
-    def check(g, o, what):
-        assert np.isfinite(g).all(), what
-        assert np.abs(g[:2 * P] - o[:2 * P]).max() < 2e-4, (what, "pose", np.abs(g[:2 * P] - o[:2 * P]).max(), int(np.abs(g[:2 * P] - o[:2 * P]).argmax()))
-        assert np.abs(g[2 * P:] - o[2 * P:]).max() < 2e-3, (what, "vel", np.abs(g[2 * P:] - o[2 * P:]).max(), int(np.abs(g[2 * P:] - o[2 * P:]).argmax()))
-
-    core.amp_obs_agent(out); core.sync()
-    g = out.cpu().numpy().astype(np.float64)
-    for e in range(N):
-        orc.reset(float(times[e]), float(thetas[e]), 20.0)
-        check(g[e], orc.record_amp_obs_agent(), ("reset", e))
-    # expert samples at given clip times (incl. one before 0 + 1/30 and one across the cycle end)
-    et = np.array([0.01, 0.2, 0.5 * orc.motion_duration, orc.motion_duration - 0.001, orc.motion_duration + 0.1, 0.031, 0.77 * orc.motion_duration, 1.9 * orc.motion_duration])
-    core.amp_obs_expert(out, et); core.sync()
-    g = out.cpu().numpy().astype(np.float64)
-    for e in range(N):
-        orc.reset(float(times[e]), float(thetas[e]), 20.0)   # the expert's ground height is the kinematic origin's y of that env
-        check(g[e], orc.record_amp_obs_expert(float(et[e])), ("expert", e, et[e]))
-    # agent after two policy steps, teacher-forced: history = the pose the last action was chosen from
-    off, scl, lo, hi = orc.action_statics()
-    rng = np.random.default_rng(3)
-    e = 3
-    orc.reset(float(times[e]), float(thetas[e]), 20.0)
-    acts = torch.zeros(N, orc.action_size, device="cuda")
-    for step in range(2):
-        a = random_policy_action(rng, off, scl, lo, hi)
-        core.set_snapshot(e, orc.get_snapshot())
-        acts[e] = torch.tensor(a, dtype=torch.float32)
-        core.set_action(acts)
-        orc.set_action(a)
-        for _ in range(20):
-            core.set_snapshot(e, orc.get_snapshot())
-            core.update(1.0 / 600.0, 1)
-            orc.update(1.0 / 600.0)
-        core.set_snapshot(e, orc.get_snapshot())
-        core.amp_obs_agent(out); core.sync()
-        check(out[e].cpu().numpy().astype(np.float64), orc.record_amp_obs_agent(), ("step", step))
