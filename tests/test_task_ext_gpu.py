@@ -15,6 +15,7 @@ import pytest
 
 from tests import amp_states as A
 from tests.oracle_binding import Oracle
+from tests.task_states import airborne as _airborne, load as _load, lying as _lying, set_clocks as _set_clocks
 from tests.parity_util import SnapLayout, random_policy_action
 
 pytestmark = pytest.mark.gpu
@@ -80,55 +81,10 @@ def _outputs(core):
     return goal.cpu().numpy().astype(np.float64), rew.cpu().numpy().astype(np.float64), fl.cpu().numpy()
 
 
-def _load(core, e, o):
-    """teacher forcing: the oracle's simulator snapshot and task block into environment e (the draw counter included; the reset counter kept)"""
-    core.set_snapshot(e, o.get_snapshot())
-    tb = core.task_state(e); ts = o.task_state()
-    tb[0], tb[1] = ts["target_pos"][0], ts["target_pos"][2]
-    tb[2:6] = [ts["target_speed"], ts["target_heading"], ts["timer"], ts["timer_max"]]
-    tb[6:9] = ts["prev_action_com"]; tb[K_COUNTER] = o.task_counter()
-    if o.goal_size == 4 and core.scene_name().startswith("Heading"):
-        tb[X_GETUP] = o.getup_state()["timer"]
-    else:
-        ss = o.strike_state()
-        tb[X_TAR_Y], tb[X_HIT], tb[X_HIT_TIME] = ss["target_height"], float(ss["hit"]), ss["hit_time"]
-    core.set_task_state(e, tb)
-
-
 def _set_target(o, pos, hit=False, hit_time=-1.0):
     ts = o.task_state()
     o.set_task_state(np.asarray(pos, dtype=np.float64), ts["target_speed"], ts["target_heading"], ts["timer"], ts["timer_max"], ts["prev_action_com"])
     o.set_strike_state(hit, hit_time)
-
-
-def _set_clocks(o, **kw):
-    s = o.get_snapshot()
-    for k, v in kw.items():
-        s[CLK + {"timer": 12, "timer_max": 13}[k]] = v
-    o.set_snapshot(s)
-
-
-def _airborne(o, lift=2.0, vel=None):
-    """the character lifted by `lift` m; with vel the joint velocities zeroed and every body moving with the root velocity vel (m/s)"""
-    p, v = o.get_pose()
-    p = p.copy(); p[1] += lift
-    if vel is not None:
-        v = np.zeros_like(v); v[0:3] = vel
-    o.set_pose_vel(p, v)
-
-
-def _lying(o, seed):
-    """brings the oracle's character to the ground: 1.5 s of wild random actions, then 0.5 s under the zero action, which keeps fall-contact
-    bodies on the ground in every later update (checked by the callers against the oracle)"""
-    off, scl, lo, hi = o.action_statics()
-    rng = np.random.default_rng(seed)
-    for _ in range(900):
-        if o.need_new_action():
-            o.set_action(random_policy_action(rng, off, scl, lo, hi, sigma=1.0))
-        o.update(DT)
-    o.set_action(-off)
-    for _ in range(300):
-        o.update(DT)
 
 
 def _mirror_bodies(mirror, core, e):

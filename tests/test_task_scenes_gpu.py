@@ -91,11 +91,14 @@ def test_task_goal_reward_and_updates_match_the_oracle(asset_root, args):
                 worst_rew = max(worst_rew, abs(float(r[e]) - o.calc_reward()))
                 worst_im = max(worst_im, abs(float(ri[e]) - o.calc_reward_imitate()))   # CalcRewardImitate against the env's clip, on the free-run state
             checked += 1
-    # random actions make most characters fall within the first second: the count only guards against an empty comparison
+    # random actions make most characters fall within the first second: the count only guards against an empty comparison.  The bounds are the
+    # measured maxima on an H100 (80 GB HBM3, 700 W limit) times 2.5: goal 9.6e-4 / 1.0e-3 (target / heading), task reward 5.7e-5 / 1.4e-3,
+    # imitation reward 6.4e-4.  Each is 20 free updates of fp32 drift from the teacher-forced start; the branch-by-branch comparison with
+    # derived bounds is tests/test_task_branches_gpu.py
     print("task scene %s: %d environment-steps compared, worst goal error %.2e, worst task reward error %.2e, worst imitation reward error %.2e"
           % (args[-1], checked, worst_goal, worst_rew, worst_im))
     assert checked > 250
-    assert worst_goal < 5e-3 and worst_rew < 1e-2 and worst_im < 2e-2, (worst_goal, worst_rew, worst_im)
+    assert worst_goal < 2.5e-3 and worst_rew < 3.5e-3 and worst_im < 1.6e-3, (worst_goal, worst_rew, worst_im)
     core.close()
 
 
