@@ -106,6 +106,16 @@ __global__ void __launch_bounds__(256) dm_learn_transpose_kernel(LearnTransposeP
     }
 }
 
+// hi + lo fp16 parts of a head's dY g.  |g| <= 65504 splits as __float2half_rn gives it; past fp16's range hi saturates at +-65504 and lo
+// carries the rest (|g| beyond 131008 saturates there), so such a row reaches the backward GEMMs finite instead of as inf + -inf = NaN.  NaN
+// stays NaN
+__device__ __forceinline__ void head_split(float g, __half& hi, __half& lo) {
+    constexpr float kHalfMax = 65504.f;
+    const auto sat = [](float v) { return fabsf(v) > kHalfMax ? copysignf(kHalfMax, v) : v; };
+    hi = __float2half_rn(sat(g));
+    lo = __float2half_rn(sat(g - __half2float(hi)));
+}
+
 // the per-row loss gradients w.r.t. the normalised output; one thread per row, grid = m tiles
 template <bool ACTOR>
 __device__ __forceinline__ void learn_head(const LearnHeadParams& P) {
@@ -154,7 +164,8 @@ __device__ __forceinline__ void learn_head(const LearnHeadParams& P) {
                 part[0] = 0.5f * d * d;
             }
         }
-        const __half hi = __float2half_rn(g), lo = __float2half_rn(g - __half2float(hi));
+        __half hi, lo;
+        head_split(g, hi, lo);
         const int oa = ((j >> 3) * 16 + (tid >> 3)) * 64 + (tid & 7) * 8 + (j & 7);
         dya[oa] = hi;
         dya[oa + kMlpATile] = lo;

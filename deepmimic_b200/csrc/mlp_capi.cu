@@ -26,12 +26,17 @@
 
 extern "C" void dm_set_last_error(const char* msg);
 
+// the clip of a normalised input before its fp16 operand: the caller's (<= 0: none), never past fp16's largest finite value, so an input
+// the normaliser puts beyond +-65504 saturates there instead of reaching the GEMMs as inf (in range, the operand's bits do not change)
+constexpr float kNoClip = 65504.f;
+inline float operand_clip(float clip) { return clip > 0.f && clip < kNoClip ? clip : kNoClip; }
+
 struct dm_mlp {
     int device = 0, in_dim = 0, h0 = 0, h1 = 0, out_dim = 0, max_rows = 0;
     int K0 = 0, N0 = 0, N1 = 0, N2 = 64;  // padded sizes: K0 = pad64(in), N0 = pad128(h0) = K1, N1 = pad128(h1) = K2, N2 = 64 (gated: K0 = pad64(in + goal), pad64(h))
     __half *w[3] = {nullptr, nullptr, nullptr}, *obs_t = nullptr, *act0 = nullptr, *act1 = nullptr;   // activations: operand tiles [m tiles][K / 64][128 x 64]
     float *b[3] = {nullptr, nullptr, nullptr}, *in_mean = nullptr, *in_istd = nullptr, *out_mean = nullptr, *out_std = nullptr;
-    float in_clip = 1e30f;
+    float in_clip = kNoClip;
     long long launches = 0;
     // gated actor (dm_mlp_create_gated) only: gate trunk (goal -> 128), both gate hidden layers as one 128 -> 128 GEMM (layer l in columns
     // [64 l, 64 l + 64)), per trunk layer the gate's scale and bias weights (64 -> h_l)
@@ -39,7 +44,7 @@ struct dm_mlp {
     int goal_dim = 0, gate_common = 0, gate_hidden = 0;
     __half *wgc = nullptr, *wgh = nullptr, *wgs[2] = {nullptr, nullptr}, *wgb[2] = {nullptr, nullptr}, *goal_t = nullptr, *gc_t = nullptr, *gh_t = nullptr;
     float *bgc = nullptr, *bgh = nullptr, *bgs[2] = {nullptr, nullptr}, *bgb[2] = {nullptr, nullptr}, *g_mean = nullptr, *g_istd = nullptr;
-    float g_clip = 1e30f;
+    float g_clip = kNoClip;
     std::vector<void*> bufs;   // every device buffer the handle owns (alloc, upload), freed by dm_mlp_destroy
 };
 
@@ -242,8 +247,8 @@ dm_mlp* create_gated(const char* fn, int device, const dm_mlp_gated_weights* g, 
     m->device = device; m->in_dim = g->in_dim; m->goal_dim = g->goal_dim; m->gate_common = g->gate_common; m->gate_hidden = g->gate_hidden; m->h0 = g->h0; m->h1 = g->h1; m->out_dim = g->out_dim; m->max_rows = pad_to(max_rows, 128);
     const int trunk_in = g->in_dim + g->goal_dim, GC = g->gate_common, GH = g->gate_hidden;
     m->K0 = pad_to(trunk_in, 64); m->N0 = pad_to(g->h0, trunk_pad); m->N1 = pad_to(g->h1, trunk_pad);   // the gated layers run on 64-column tiles
-    m->in_clip = g->s_clip > 0.f ? g->s_clip : 1e30f;
-    m->g_clip = g->g_clip > 0.f ? g->g_clip : 1e30f;
+    m->in_clip = operand_clip(g->s_clip);
+    m->g_clip = operand_clip(g->g_clip);
     // both gate hidden layers side by side: layer l's GH units in columns [64 l, 64 l + GH), zero columns (relu(0) = 0) up to 64 l + 64
     std::vector<float> wgh(static_cast<size_t>(GC) * 128, 0.f), bgh(128, 0.f);
     for (int l = 0; l < 2; ++l) {
@@ -341,7 +346,7 @@ dm_mlp* dm_mlp_create(int device, int in_dim, int h0, int h1, int out_dim, const
     dm_mlp* m = new dm_mlp();
     m->device = device; m->in_dim = in_dim; m->h0 = h0; m->h1 = h1; m->out_dim = out_dim; m->max_rows = pad_to(max_rows, 128);
     m->K0 = pad_to(in_dim, 64); m->N0 = pad_to(h0, 128); m->N1 = pad_to(h1, 128);
-    m->in_clip = in_clip > 0.f ? in_clip : 1e30f;
+    m->in_clip = operand_clip(in_clip);
     const size_t R = m->max_rows;
     bool ok = upload(m, &m->w[0], tile_weights(w0, in_dim, h0, m->K0, m->N0, 128)) && upload(m, &m->w[1], tile_weights(w1, h0, h1, m->N0, m->N1, 128)) &&
               upload(m, &m->w[2], tile_weights(w2, h1, out_dim, m->N1, m->N2, m->N2)) && upload(m, &m->b[0], padded(b0, h0, m->N0)) && upload(m, &m->b[1], padded(b1, h1, m->N1)) &&
@@ -615,7 +620,7 @@ int forward_backward(const char* fn, dm_learn* l, const dm_learn_batch* b, Split
     for (int i = 0; i < 3; ++i)
         if (dw_plan(fn, l->F[i], l->Nout[i], trunk_bn(l, i), chunks, l->max_splits[i], &s.trunk[i], &cps[i])) return 1;
     // forward: gathered rows -> the plain trunk -> the normalised output (identity output normaliser)
-    dmk::LearnPrepParams Q{b->states, b->idx, b->in_mean, b->in_istd, b->in_clip > 0.f ? b->in_clip : 1e30f, m->in_dim, rows, m->K0 / 64, m->obs_t};
+    dmk::LearnPrepParams Q{b->states, b->idx, b->in_mean, b->in_istd, operand_clip(b->in_clip), m->in_dim, rows, m->K0 / 64, m->obs_t};
     dmk::dm_learn_prep_kernel<<<dim3(mt, m->K0 / 64), 128, 0, st>>>(Q);
     learn_forward(l, rows, mt, st);
     // loss head: dY of the output layer, the loss partials, the statistics
@@ -636,7 +641,7 @@ int forward_backward(const char* fn, dm_learn* l, const dm_learn_disc_batch* b, 
             return 1;
     // forward over both sides: each gathered into its own m tiles
     const int NC0 = m->K0 / 64;
-    dmk::LearnPrepParams Q{b->agent, b->agent_idx, b->in_mean, b->in_istd, b->in_clip > 0.f ? b->in_clip : 1e30f, m->in_dim, rows, NC0, m->obs_t};
+    dmk::LearnPrepParams Q{b->agent, b->agent_idx, b->in_mean, b->in_istd, operand_clip(b->in_clip), m->in_dim, rows, NC0, m->obs_t};
     dmk::dm_learn_prep_kernel<<<dim3(et, NC0), 128, 0, st>>>(Q);
     Q.x = b->expert; Q.idx = b->expert_idx; Q.tiles = m->obs_t + static_cast<size_t>(et) * NC0 * dmk::kMlpATile;
     dmk::dm_learn_prep_kernel<<<dim3(et, NC0), 128, 0, st>>>(Q);
@@ -829,8 +834,8 @@ int forward_backward(const char* fn, dm_learn* l, const dm_learn_gated_batch* gb
     for (int j = 0; j < 4; ++j)
         if (dw_plan(fn, l->gF[j], l->gN[j], 128, chunks, l->g_max_splits[j], &s.gate[j], &gcps[j])) return 1;
     // forward: gathered [state | goal] rows and goals -> the gated network -> the normalised output (identity output normaliser)
-    const dmk::LearnPrepParams Q{b->states, b->idx, b->in_mean, b->in_istd, b->in_clip > 0.f ? b->in_clip : 1e30f, m->in_dim, rows, m->K0 / 64, m->obs_t};
-    const dmk::LearnGoalParams Qg{gb->goals, gb->g_mean, gb->g_istd, gb->g_clip > 0.f ? gb->g_clip : 1e30f, m->goal_dim, m->goal_t};
+    const dmk::LearnPrepParams Q{b->states, b->idx, b->in_mean, b->in_istd, operand_clip(b->in_clip), m->in_dim, rows, m->K0 / 64, m->obs_t};
+    const dmk::LearnGoalParams Qg{gb->goals, gb->g_mean, gb->g_istd, operand_clip(gb->g_clip), m->goal_dim, m->goal_t};
     dmk::dm_learn_gated_prep_kernel<<<dim3(mt, m->K0 / 64 + 1), 128, 0, st>>>(Q, Qg);
     learn_gated_forward(l, rows, mt, st);
     // the loss heads act on the output only: the plain step's
