@@ -64,7 +64,7 @@ class DmCamera(C.Structure):
 
 
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
-           "dm_update", "dm_set_pushes", "dm_get_pushes", "dm_set_push_schedule", "dm_get_push_table", "dm_set_dynamics", "dm_get_dynamics", "dm_set_dynamics_randomization", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_record_pose", "dm_render_poses", "dm_record_kin_pose", "dm_pose_error", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
+           "dm_update", "dm_set_pushes", "dm_get_pushes", "dm_set_push_schedule", "dm_get_push_table", "dm_set_dynamics", "dm_get_dynamics", "dm_set_dynamics_randomization", "dm_set_action_latency", "dm_set_action_latency_randomization", "dm_get_action_latency", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_record_pose", "dm_render_poses", "dm_record_kin_pose", "dm_pose_error", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
            "dm_set_snapshot", "dm_state_size", "dm_save_state", "dm_load_state", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
            "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy", "dm_td_lambda_returns", "dm_mlp_set_weights_device", "dm_learn_create",
            "dm_mlp_set_normalizers_device", "dm_learn_set_weights", "dm_learn_step", "dm_learn_disc_step", "dm_learn_destroy",
@@ -112,6 +112,10 @@ def lib():
             L.dm_set_dynamics.argtypes = [vp, fp]
             L.dm_get_dynamics.argtypes = [vp, C.c_void_p]
             L.dm_set_dynamics_randomization.argtypes = [vp, dp]
+        if hasattr(L, "dm_set_action_latency"):   # likewise a library built before latency tables
+            L.dm_set_action_latency.argtypes = [vp, C.POINTER(C.c_int32)]
+            L.dm_set_action_latency_randomization.argtypes = [vp, C.c_int, C.c_int]
+            L.dm_get_action_latency.argtypes = [vp, C.c_void_p]
         if hasattr(L, "dm_render_poses"):   # likewise a library built before the renderer
             L.dm_render_poses.argtypes = [vp, C.c_int, C.c_void_p, C.POINTER(DmCamera), C.c_int, C.c_int, C.c_void_p, C.c_void_p]
         if hasattr(L, "dm_pose_error"):   # and before the tracking error
@@ -213,6 +217,23 @@ def camera_struct(camera=None):
     if unknown:
         raise ValueError("camera: unknown keys %s" % sorted(unknown))
     return DmCamera(*(float(c[k]) for k in ("yaw", "pitch", "distance", "target_height", "fov_y")))
+
+
+UPDATE_DT = 1.0 / 600.0   # the library's update timestep; a control latency is a whole number of these
+UPDATES_PER_ACTION = 20   # dm_dims::updates_per_action of every shipped controller (capi.cu: kUpdatesPerAction); a delay is below it
+
+
+def latency_updates(seconds, updates_per_action=UPDATES_PER_ACTION, what="latency"):
+    """a control latency in seconds -> whole updates (nearest), refused unless finite and within [0, (updates_per_action - 1) UPDATE_DT] after
+    rounding"""
+    s = float(seconds)
+    if not np.isfinite(s):
+        raise ValueError("%s: %r s is not a finite number" % (what, seconds))
+    d = int(round(s / UPDATE_DT))
+    if d < 0 or d > updates_per_action - 1:
+        raise ValueError("%s: %r s rounds to %d updates, outside [0, %d] (0 to %.4f s)" % (what, seconds, d, updates_per_action - 1,
+                                                                                             (updates_per_action - 1) * UPDATE_DT))
+    return d
 
 
 def _dptr(a):
@@ -404,6 +425,35 @@ class BatchedCore:
         if a.shape != (10,):
             raise ValueError("set_dynamics_randomization: lohi must hold 10 bounds, got %d" % a.size)
         self._chk(lib().dm_set_dynamics_randomization(self.h, _dptr(a)))
+
+    def set_action_latency(self, seconds):
+        """dm_set_action_latency: every environment's control latency, [N] seconds (a sequence, numpy array or tensor), each rounded to the
+        nearest whole update and refused outside [0, (updates_per_action - 1) dt]; kept across resets.  Synchronises the handle's stream."""
+        if hasattr(seconds, "detach"):
+            seconds = seconds.detach().cpu().numpy()
+        a = np.asarray(seconds, dtype=np.float64).reshape(-1)
+        if a.shape != (self.num_envs,):
+            raise ValueError("set_action_latency: need %d delays, got %d" % (self.num_envs, a.size))
+        U = self.dims.updates_per_action
+        d = np.array([latency_updates(x, U, "set_action_latency: environment %d" % e) for e, x in enumerate(a)], dtype=np.int32)
+        self._chk(lib().dm_set_action_latency(self.h, d.ctypes.data_as(C.POINTER(C.c_int32))))
+
+    def set_action_latency_randomization(self, lo, hi):
+        """dm_set_action_latency_randomization: draw every environment's control latency uniformly among the whole updates of [lo, hi] seconds
+        (each bound rounded to the nearest update), on the device, now and at every reset"""
+        U = self.dims.updates_per_action
+        dlo, dhi = latency_updates(lo, U, "set_action_latency_randomization: lo"), latency_updates(hi, U, "set_action_latency_randomization: hi")
+        self._chk(lib().dm_set_action_latency_randomization(self.h, dlo, dhi))
+
+    def action_latency(self):
+        """dm_get_action_latency: every environment's current control latency in seconds, a float64 tensor [N] on the handle's device
+        (stream-ordered, no host synchronisation).  Refused on a handle without a latency table."""
+        import torch
+        # the scratch tensor belongs to the handle's stream, which writes and reads it: the caching allocator reuses it only after that work
+        with torch.cuda.stream(torch.cuda.ExternalStream(self.stream(), device=self.device)):
+            out = torch.empty(self.num_envs, dtype=torch.int32, device=torch.device("cuda", self.device))
+            self._chk(lib().dm_get_action_latency(self.h, C.c_void_p(out.data_ptr())))
+            return out.to(torch.float64) * UPDATE_DT
 
     def set_env_order(self, on):
         """dm_set_env_order: place the environments in the step kernel by contact load (the default; tile width 16 only) or by index"""

@@ -108,6 +108,11 @@ struct dm_handle {
     dmk::DevPush* d_push_none = nullptr;   // the dynamics step kernel's push table on a handle without pushes: every entry empty
     bool dyn_random = false;            // the table is drawn by dyn_rand at every reset (and owned by it)
     dmk::DynRand dyn_rand{};
+    dmk::DevLat* d_lat = nullptr;       // latency table (dm_set_action_latency, dm_set_action_latency_randomization): null until the first call, then
+                                        // the action and step launches use the latency instantiations
+    dmk::DevDyn* d_dyn_unit = nullptr;  // the latency step kernel's dynamics table on a handle without one: every factor 1
+    bool lat_random = false;            // the delays are drawn by lat_rand at every reset (and owned by it)
+    dmk::LatRand lat_rand{};
     int* d_order = nullptr;   // placement of the environments in the step kernel's tiles (dm_set_env_order); st.order is it or null
     dmk::StepLayout lay{};
     uint64_t seed = 0, env_offset = 0;
@@ -356,6 +361,9 @@ int goal_size(const dmk::DevModel& M) { return M.task_kind == dmk::kTaskNone ? 0
 int tile_index(const dm_handle* h) { return h->W == 32 ? 1 : 0; }
 int policy_grid(const dm_handle* h) { return h->padded_envs / (dmk::kPolicyBlock / h->W); }
 
+// dm_dims::updates_per_action: every shipped controller runs 20 updates of 1/600 s per 1/30 s policy step
+constexpr int kUpdatesPerAction = 20;
+
 // the tail of every launch
 int launched(dm_handle* h) {
     DM_CUDA(cudaGetLastError());
@@ -366,7 +374,9 @@ int launched(dm_handle* h) {
 int launch_step(dm_handle* h, double dt, int n_updates) {
     // AMP task scenes: the variant that also advances the task block; handles with a push table (dm_set_pushes): the push kernel, which applies it
     // handles with a dynamics table (dm_set_dynamics*): the dynamics kernel, which also applies the push table if there is one
-    const void* kern = h->d_dyn ? reinterpret_cast<const void*>(dmk::kStepDynKernels[tile_index(h)][task_scene(h)])
+    // handles with a latency table (dm_set_action_latency*): the latency kernel, which also applies the push and dynamics tables if there are any
+    const void* kern = h->d_lat ? reinterpret_cast<const void*>(dmk::kStepLatKernels[tile_index(h)][task_scene(h)])
+                     : h->d_dyn ? reinterpret_cast<const void*>(dmk::kStepDynKernels[tile_index(h)][task_scene(h)])
                      : h->d_push ? reinterpret_cast<const void*>(dmk::kStepPushKernels[tile_index(h)][task_scene(h)])
                                  : reinterpret_cast<const void*>(dmk::kStepKernels[tile_index(h)][task_scene(h)]);
     // opt in to the large dynamic shared-memory carve-out; the limit is raised whenever a handle needs more than any earlier one on
@@ -389,7 +399,12 @@ int launch_step(dm_handle* h, double dt, int n_updates) {
         if (launched(h)) return 1;
     }
     const dim3 grid(h->padded_envs / h->tiles), block(h->tiles * h->W);
-    if (h->d_dyn)
+    if (h->d_lat)
+        dmk::kStepLatKernels[tile_index(h)][task_scene(h)]<<<grid, block, h->smem_bytes, h->stream>>>(h->d_model, dmk::DevStateLat{h->st, h->d_lat}, h->d_frame_times,
+                                                                                                     h->d_frames, dt, n_updates, h->sa.cfg.num_sim_substeps, h->lay,
+                                                                                                     h->d_push ? h->d_push : h->d_push_none,
+                                                                                                     h->d_dyn ? h->d_dyn : h->d_dyn_unit);
+    else if (h->d_dyn)
         dmk::kStepDynKernels[tile_index(h)][task_scene(h)]<<<grid, block, h->smem_bytes, h->stream>>>(h->d_model, h->st, h->d_frame_times, h->d_frames, dt,
                                                                                                      n_updates, h->sa.cfg.num_sim_substeps, h->lay,
                                                                                                      h->d_push ? h->d_push : h->d_push_none, h->d_dyn);
@@ -772,7 +787,7 @@ int dm_get_dims(dm_handle* h, dm_dims* o) {
     o->num_envs = h->num_envs; o->num_joints = M.nl; o->pose_dim = M.pose_dim; o->num_dofs = M.n; o->state_size = M.state_size; o->goal_size = goal_size(M); o->amp_obs_size = M.amp_obs_size;
     o->action_size = M.action_size; o->snapshot_size = SnapshotOffsets(M.nl).size;
     o->num_update_substeps = h->sa.cfg.num_update_substeps;
-    o->updates_per_action = 20;
+    o->updates_per_action = kUpdatesPerAction;
     o->motion_duration = M.motion_dur;
     return 0;
 }
@@ -846,6 +861,10 @@ int dm_reset_clips(dm_handle* h, int force_all, const int* h_clip, const double*
         dmk::dm_dyn_draw_kernel<<<(h->num_envs + 127) / 128, 128, 0, h->stream>>>(h->st, h->d_dyn, h->dyn_rand);
         if (launched(h)) return 1;
     }
+    if (h->d_lat) {   // the restarted environments drop their pending action and hold the reset pose; a randomised table draws their delay
+        dmk::dm_latency_reset_kernel<<<(h->num_envs + 127) / 128, 128, 0, h->stream>>>(h->d_model, h->st, h->d_lat, h->lat_rand, h->lat_random ? 1 : 0, 0);
+        if (launched(h)) return 1;
+    }
     if (!task_scene(h)) return 0;
     // cSceneTargetAMP::Reset's own part for the environments that were just reset
     dmk::dm_task_reset_kernel<<<(h->padded_envs + 127) / 128, 128, 0, h->stream>>>(h->d_model, h->st, h->padded_envs);
@@ -861,7 +880,10 @@ int dm_get_clip_table(dm_handle* h, int* num_clips, double* h_dur, double* h_cdf
 int dm_set_action(dm_handle* h, const float* d_actions) {
     DM_DEVICE(h);
     const int total = h->num_envs * h->hm.nl;
-    dmk::dm_set_action_kernel<<<(total + 127) / 128, 128, 0, h->stream>>>(h->d_model, h->st, d_actions, h->num_envs);
+    if (h->d_lat)   // an environment with a delay gets the action as its pending one (dm_latency.cuh)
+        dmk::dm_set_action_latency_kernel<<<(total + 127) / 128, 128, 0, h->stream>>>(h->d_model, h->st, d_actions, h->num_envs, h->d_lat);
+    else
+        dmk::dm_set_action_kernel<<<(total + 127) / 128, 128, 0, h->stream>>>(h->d_model, h->st, d_actions, h->num_envs);
     return launched(h);
 }
 int dm_update(dm_handle* h, double dt, int n_updates) {
@@ -1054,6 +1076,70 @@ int dm_set_dynamics_randomization(dm_handle* h, const double* lohi) {
     h->dyn_rand = R; h->dyn_random = true;
     dmk::dm_dyn_draw_kernel<<<(h->num_envs + 127) / 128, 128, 0, h->stream>>>(h->st, h->d_dyn, h->dyn_rand);
     return launched(h);
+}
+// ---- control latency (dm_latency.cuh)
+namespace {
+// the table (every delay 0, no action pending, the current reset counters adopted) and, on a handle without them, the empty push table and the
+// unit-factor table of the latency kernel.  The unit table carries the model's own total mass, so that its centres of mass are the plain kernel's.
+int alloc_lat_table(dm_handle* h) {
+    const size_t n = static_cast<size_t>(h->padded_envs);
+    if (alloc_buffer(h, &h->d_lat, n, kZeroed)) return 1;
+    if (h->d_push_none == nullptr) {
+        if (alloc_buffer(h, &h->d_push_none, n)) return 1;
+        std::vector<dmk::DevPush> none(n);
+        for (auto& p : none) { p.force[0] = p.force[1] = p.force[2] = 0.f; p.body = -1; p.start = 0.0; p.duration = 0.0; }
+        DM_CUDA(cudaMemcpyAsync(h->d_push_none, none.data(), none.size() * sizeof(dmk::DevPush), cudaMemcpyHostToDevice, h->stream));
+    }
+    if (alloc_buffer(h, &h->d_dyn_unit, n)) return 1;
+    std::vector<dmk::DevDyn> unit(n);
+    for (auto& d : unit) {
+        for (int k = 0; k < dmk::kDynFloats; ++k) d.f[k] = (k < dmk::kDTotalMass) ? 1.f : 0.f;
+        d.f[dmk::kDTotalMass] = h->hm.total_mass;
+    }
+    DM_CUDA(cudaMemcpyAsync(h->d_dyn_unit, unit.data(), unit.size() * sizeof(dmk::DevDyn), cudaMemcpyHostToDevice, h->stream));
+    dmk::dm_latency_reset_kernel<<<(h->num_envs + 127) / 128, 128, 0, h->stream>>>(h->d_model, h->st, h->d_lat, h->lat_rand, 0, 1);
+    if (launched(h)) return 1;
+    DM_CUDA(cudaStreamSynchronize(h->stream));   // the staging vectors are pageable
+    return 0;
+}
+}  // namespace
+int dm_set_action_latency(dm_handle* h, const int32_t* h_updates) {
+    DM_DEVICE(h);
+    auto refuse = [](const std::string& what) { g_err = "dm_set_action_latency: " + what; return fail(); };
+    if (!h_updates) return refuse("h_updates is required");
+    if (h->lat_random) return refuse("the handle's delays are randomised (dm_set_action_latency_randomization), which owns its table");
+    for (int e = 0; e < h->num_envs; ++e)
+        if (h_updates[e] < 0 || h_updates[e] > kUpdatesPerAction - 1)
+            return refuse("environment " + std::to_string(e) + ": delay " + std::to_string(h_updates[e]) + " is outside [0, " + std::to_string(kUpdatesPerAction - 1) +
+                          "] updates");
+    if (h->d_lat == nullptr && alloc_lat_table(h)) return 1;
+    // the delays alone: the pending actions, their due updates and the reset counters stay
+    DM_CUDA(cudaMemcpy2DAsync(h->d_lat, sizeof(dmk::DevLat), h_updates, sizeof(int32_t), sizeof(int32_t), static_cast<size_t>(h->num_envs), cudaMemcpyHostToDevice,
+                              h->stream));
+    DM_CUDA(cudaStreamSynchronize(h->stream));   // h_updates is the caller's pageable memory
+    return 0;
+}
+int dm_set_action_latency_randomization(dm_handle* h, int lo, int hi) {
+    DM_DEVICE(h);
+    auto refuse = [](const std::string& what) { g_err = "dm_set_action_latency_randomization: " + what; return fail(); };
+    if (h->d_lat && !h->lat_random) return refuse("the handle has delays set by dm_set_action_latency, which own its table");
+    if (lo < 0 || lo > kUpdatesPerAction - 1) return refuse("lo " + std::to_string(lo) + " is outside [0, " + std::to_string(kUpdatesPerAction - 1) + "] updates");
+    if (hi < 0 || hi > kUpdatesPerAction - 1) return refuse("hi " + std::to_string(hi) + " is outside [0, " + std::to_string(kUpdatesPerAction - 1) + "] updates");
+    if (lo > hi) return refuse("lo " + std::to_string(lo) + " > hi " + std::to_string(hi));
+    dmk::LatRand R;
+    std::memset(&R, 0, sizeof(R));   // padding included: the state header hashes the bounds
+    R.lo = lo; R.hi = hi; R.seed = h->seed ^ dmk::kLatSeedKey; R.env_base = h->env_offset;
+    if (h->d_lat == nullptr && alloc_lat_table(h)) return 1;
+    h->lat_rand = R; h->lat_random = true;
+    dmk::dm_latency_reset_kernel<<<(h->num_envs + 127) / 128, 128, 0, h->stream>>>(h->d_model, h->st, h->d_lat, h->lat_rand, 1, 0);
+    return launched(h);
+}
+int dm_get_action_latency(dm_handle* h, int32_t* d_out) {
+    DM_DEVICE(h);
+    if (!d_out) { g_err = "dm_get_action_latency: d_out is required"; return fail(); }
+    if (h->d_lat == nullptr) { g_err = "dm_get_action_latency: the handle has no latency table (dm_set_action_latency, dm_set_action_latency_randomization)"; return fail(); }
+    DM_CUDA(cudaMemcpy2DAsync(d_out, sizeof(int32_t), h->d_lat, sizeof(dmk::DevLat), sizeof(int32_t), static_cast<size_t>(h->num_envs), cudaMemcpyDeviceToDevice, h->stream));
+    return 0;
 }
 int dm_set_env_order(dm_handle* h, int on) {
     DM_DEVICE(h);
@@ -1533,7 +1619,8 @@ struct StateHeader {
     uint32_t version, dynamics;   // dynamics: 0 without a randomised dynamics table, else a hash of its bounds (dynamics_hash)
     uint64_t bytes;
     int32_t num_envs, padded_envs, W, links, state_size, action_size, goal_size, amp_obs_size, num_clips;
-    int32_t dyn_table;   // 1: the blob ends with a dynamics table (dm_set_dynamics or dm_set_dynamics_randomization); 0: none
+    int16_t dyn_table;       // 1: the blob carries a dynamics table (dm_set_dynamics or dm_set_dynamics_randomization); 0: none
+    int16_t latency_table;   // 1: a LatencyHeader follows this header and the blob ends with a latency table (dm_set_action_latency*); 0: neither
     uint64_t seed, env_offset, model;
     char scene[32];
     // host state that changes later results
@@ -1542,6 +1629,13 @@ struct StateHeader {
     uint32_t push_schedule;   // 0: no push schedule; otherwise a hash of its parameters (push_schedule_hash), whose blocks end the blob
     double time_lim_min, time_lim_max;
 };
+static_assert(sizeof(StateHeader) == 160, "StateHeader: a blob without a latency table keeps its layout");
+// after the header of a blob with a latency table
+struct LatencyHeader {
+    uint32_t randomization;   // 0 without a randomised latency table, else a hash of its bounds (latency_hash)
+    uint32_t pad;
+};
+size_t header_bytes(const dm_handle* h) { return sizeof(StateHeader) + (h->d_lat ? sizeof(LatencyHeader) : 0); }
 struct StateBlock { void* dev; size_t bytes; };
 // the device blocks of the blob, in order; null blocks of the scene (task, taskx, clip outside the task scenes) are absent
 std::vector<StateBlock> state_blocks(const dm_handle* h) {
@@ -1557,7 +1651,8 @@ std::vector<StateBlock> state_blocks(const dm_handle* h) {
         b.push_back({h->d_push, N * sizeof(dmk::DevPush)});
         b.push_back({h->d_push_sched, N * dmk::kPushSchedDoubles * sizeof(double)});
     }
-    if (h->d_dyn) b.push_back({h->d_dyn, N * sizeof(dmk::DevDyn)});   // a dynamics table ends the blob
+    if (h->d_dyn) b.push_back({h->d_dyn, N * sizeof(dmk::DevDyn)});   // then a dynamics table
+    if (h->d_lat) b.push_back({h->d_lat, N * sizeof(dmk::DevLat)});   // a latency table (delays, pending actions, their due updates) ends the blob
     return b;
 }
 // the state header's push_schedule field: 0 without a schedule, else FNV-1a over its parameters folded to 32 bits and never 0
@@ -1578,6 +1673,16 @@ uint32_t dynamics_hash(const dm_handle* h) {
     const uint32_t v = static_cast<uint32_t>(x ^ (x >> 32));
     return v ? v : 1u;
 }
+// the latency header's randomization field: 0 without a randomised table (none, or dm_set_action_latency), else FNV-1a over the bounds, never 0
+uint32_t latency_hash(const dm_handle* h) {
+    if (!h->lat_random) return 0;
+    const int lohi[2] = {h->lat_rand.lo, h->lat_rand.hi};
+    const unsigned char* p = reinterpret_cast<const unsigned char*>(lohi);
+    uint64_t x = 1469598103934665603ull;
+    for (size_t i = 0; i < sizeof(lohi); ++i) { x ^= p[i]; x *= 1099511628211ull; }
+    const uint32_t v = static_cast<uint32_t>(x ^ (x >> 32));
+    return v ? v : 1u;
+}
 // FNV-1a over the model blob with the fields that change at run time (time limits, mode) cleared: tells handles of different characters,
 // controllers or clips apart when every count matches
 uint64_t model_hash(const dm_handle* h) {
@@ -1593,8 +1698,8 @@ StateHeader state_header(const dm_handle* h) {
     StateHeader H;
     std::memset(&H, 0, sizeof(H));
     std::memcpy(H.magic, kStateMagic, sizeof(H.magic));
-    H.version = kStateVersion; H.dynamics = dynamics_hash(h); H.dyn_table = h->d_dyn ? 1 : 0;
-    H.bytes = sizeof(StateHeader);
+    H.version = kStateVersion; H.dynamics = dynamics_hash(h); H.dyn_table = h->d_dyn ? 1 : 0; H.latency_table = h->d_lat ? 1 : 0;
+    H.bytes = header_bytes(h);
     for (const StateBlock& b : state_blocks(h)) H.bytes += b.bytes;
     const auto& M = h->hm;
     H.num_envs = h->num_envs; H.padded_envs = h->padded_envs; H.W = h->W; H.links = M.nl; H.state_size = M.state_size; H.action_size = M.action_size;
@@ -1624,6 +1729,11 @@ int dm_save_state(dm_handle* h, void* h_out) {
     char* o = static_cast<char*>(h_out);
     std::memcpy(o, &H, sizeof(H));
     o += sizeof(H);
+    if (h->d_lat) {
+        const LatencyHeader LH{latency_hash(h), 0u};
+        std::memcpy(o, &LH, sizeof(LH));
+        o += sizeof(LH);
+    }
     for (const StateBlock& b : state_blocks(h)) {
         DM_CUDA(cudaMemcpyAsync(o, b.dev, b.bytes, cudaMemcpyDeviceToHost, h->stream));
         o += b.bytes;
@@ -1655,8 +1765,14 @@ int dm_load_state(dm_handle* h, const void* h_in) {
     if (in.push_schedule != mine.push_schedule) return refuse("push schedule (dm_set_push_schedule: none, or other parameters)");
     if (in.dyn_table != mine.dyn_table) return refuse("dynamics table (dm_set_dynamics, dm_set_dynamics_randomization: one, or none)");
     if (in.dynamics != mine.dynamics) return refuse("dynamics randomisation (dm_set_dynamics_randomization: none, or other bounds)");
+    if (in.latency_table != mine.latency_table) return refuse("action latency table (dm_set_action_latency, dm_set_action_latency_randomization: one, or none)");
+    if (h->d_lat) {
+        LatencyHeader lh;
+        std::memcpy(&lh, static_cast<const char*>(h_in) + sizeof(in), sizeof(lh));
+        if (lh.randomization != latency_hash(h)) return refuse("action latency randomisation (dm_set_action_latency_randomization: none, or other bounds)");
+    }
     if (in.bytes != mine.bytes) return refuse("byte size");
-    const char* p = static_cast<const char*>(h_in) + sizeof(in);
+    const char* p = static_cast<const char*>(h_in) + header_bytes(h);
     for (const StateBlock& b : state_blocks(h)) {
         DM_CUDA(cudaMemcpyAsync(b.dev, p, b.bytes, cudaMemcpyHostToDevice, h->stream));
         p += b.bytes;

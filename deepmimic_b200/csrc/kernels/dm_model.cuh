@@ -12,6 +12,7 @@
 #include "dm_math.cuh"
 
 #include "dm_dynamics.cuh"
+#include "dm_latency.cuh"
 #include "dm_push.cuh"
 #include "dm_task.cuh"
 #include "dm_task_ext.cuh"
@@ -197,6 +198,11 @@ constexpr int kPolicyBlock = 64;   // threads per block of the observe, AMP and 
 using StepKernel = void (*)(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout);
 using StepPushKernel = void (*)(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout, DevPush*);
 using StepDynKernel = void (*)(const DevModel*, DevState, const double*, const float*, double, int, int, StepLayout, DevPush*, const DevDyn*);
+// the latency step kernel's state: the handle's DevState and its latency table (indexed by environment id)
+struct DevStateLat : DevState {
+    const DevLat* lat;
+};
+using StepLatKernel = void (*)(const DevModel*, DevStateLat, const double*, const float*, double, int, int, StepLayout, DevPush*, const DevDyn*);
 using ObserveKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, ObsFan, int);
 using ObserveDynKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, ObsFan, int, const DevDyn*);
 using ResetKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, int, const double*, const double*, const double*,
@@ -205,6 +211,7 @@ using AmpObsKernel = void (*)(const DevModel*, DevState, const double*, const fl
 extern const StepKernel kStepKernels[2][2];
 extern const StepPushKernel kStepPushKernels[2][2];   // dm_step_push_kernel: handles with a push table (dm_set_pushes)
 extern const StepDynKernel kStepDynKernels[2][2];     // dm_step_dyn_kernel: handles with a dynamics table (dm_set_dynamics, dm_set_dynamics_randomization)
+extern const StepLatKernel kStepLatKernels[2][2];     // dm_step_latency_kernel: handles with a latency table (dm_set_action_latency*)
 extern const ObserveKernel kObserveKernels[2][2];
 extern const ObserveDynKernel kObserveDynKernels[2][2];   // dm_observe_dyn_kernel: the imitation reward's COM with the environment's masses
 extern const ResetKernel kResetKernels[2][2];
@@ -215,6 +222,7 @@ extern const AmpExpertKernel kAmpExpertKernels[2][2];
 constexpr int kEnvOrderThreads = 1024;   // dm_env_order_kernel: one block
 __global__ void dm_env_order_kernel(const int* load, int n_padded, int tiles, int W, int* order);
 __global__ void dm_set_action_kernel(const DevModel*, DevState, const float*, int);
+__global__ void dm_set_action_latency_kernel(const DevModel*, DevState, const float*, int, DevLat*);
 constexpr int kPoseEnvsPerBlock = 8;   // dm_pose_kernel: kPoseEnvsPerBlock x links threads, 2 pose_dim floats of shared memory per environment
 __global__ void dm_pose_kernel(const DevModel*, DevState, float*, float*, int);
 using KinPoseKernel = void (*)(const DevModel*, DevState, const double*, const float*, const float*, float*, int);
@@ -223,6 +231,7 @@ __global__ void dm_task_reset_kernel(const DevModel*, DevState, int);
 __global__ void dm_push_clear_kernel(DevState, DevPush*, int);
 __global__ void dm_push_schedule_kernel(DevState, DevPush*, double*, PushSchedule);
 __global__ void dm_dyn_draw_kernel(DevState, DevDyn*, DynRand);
+__global__ void dm_latency_reset_kernel(const DevModel*, DevState, DevLat*, LatRand, int, int);
 __global__ void dm_task_observe_kernel(const DevModel*, DevState, float*, float*, int);
 int dm_step_layout(int nl, int n, int chain_len, int maxrows, int W, StepLayout* L);
 int dm_step_smem_bytes(const StepLayout& L, int tiles);

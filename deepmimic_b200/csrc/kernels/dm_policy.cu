@@ -556,7 +556,11 @@ __global__ void __launch_bounds__(BLOCK) dm_amp_expert_sample_kernel(const DevMo
 }
 
 // actions: [N x action_size] floats (DeepMimic action layout)
-__global__ void dm_set_action_kernel(const DevModel* __restrict__ gm, DevState st, const float* __restrict__ actions, int num_real_envs) {
+// LAT (dm_set_action_latency_kernel, handles with a latency table): an environment with a delay d > 0 gets the targets in its pending slot, due at
+// the update counter + d (dm_latency.cuh), replacing any action still pending; d = 0 writes the target slot and drops a pending action.  The
+// AMP history stays at the action's time.
+template <bool LAT>
+__device__ __forceinline__ void set_action_body(const DevModel* __restrict__ gm, DevState st, const float* __restrict__ actions, int num_real_envs, DevLat* lat) {
     const DevModel& M = *gm;
     const int gid = blockIdx.x * blockDim.x + threadIdx.x;
     const int env = gid / M.nl, j = gid % M.nl;
@@ -564,9 +568,18 @@ __global__ void dm_set_action_kernel(const DevModel* __restrict__ gm, DevState s
     const DevLink& L = M.link[j];
     // cSceneImitateAMP::UpdateHist (SceneImitateAMP.cpp:167-172): the pose / vel the new action was chosen from
     if (st.hist) hist_store(st.hist + static_cast<size_t>(env) * 2 * M.pose_dim, M.pose_dim, L, j == 0, sim_joint_to_dm(M, L, st.sim + static_cast<size_t>(env) * sim_stride(M.nl), j, j == 0));
-    if (j == 0) return;
+    if (j == 0) {
+        if constexpr (LAT) {
+            const int d = lat[env].delay;
+            lat[env].due = d > 0 ? st.flags[static_cast<size_t>(env) * kFlagInts + kFUpdates] + d : -1;
+        }
+        return;
+    }
     const float* a = actions + static_cast<size_t>(env) * M.action_size + L.act_off;
     float4* tgt = reinterpret_cast<float4*>(st.sim + static_cast<size_t>(env) * sim_stride(M.nl) + 16 + 8 * M.nl) + j;
+    if constexpr (LAT) {
+        if (lat[env].delay > 0) tgt = reinterpret_cast<float4*>(lat[env].tg) + j;
+    }
     if (L.jtype == kJSpherical) {
         V3 em = mk3(a[0], a[1], a[2]);
         float len = sqrtf(dot(em, em));
@@ -586,6 +599,12 @@ __global__ void dm_set_action_kernel(const DevModel* __restrict__ gm, DevState s
     } else if (L.jtype == kJRevolute) {
         *tgt = make_float4(a[0], 0.f, 0.f, 0.f);
     }
+}
+__global__ void dm_set_action_kernel(const DevModel* __restrict__ gm, DevState st, const float* __restrict__ actions, int num_real_envs) {
+    set_action_body<false>(gm, st, actions, num_real_envs, nullptr);
+}
+__global__ void dm_set_action_latency_kernel(const DevModel* __restrict__ gm, DevState st, const float* __restrict__ actions, int num_real_envs, DevLat* lat) {
+    set_action_body<true>(gm, st, actions, num_real_envs, lat);
 }
 
 // pose / vel: [num_real_envs x pose_dim] floats, the simulated character in DeepMimic layout (cSimCharacter::BuildPose / BuildVel); either may be

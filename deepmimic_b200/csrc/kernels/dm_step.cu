@@ -1277,8 +1277,12 @@ struct EnvRefs {
 // entry once the window has passed.  DYN (with PUSH): the body of dm_step_dyn_kernel, the kernel of handles with a dynamics table
 // (dm_set_dynamics, dm_set_dynamics_randomization): the environment's factors (dyn_in, by environment id) scale the composite bodies of the
 // articulated-body solves, Kp, Kd and the torque limit of the Stable-PD stage, the friction bounds of the constraint solve and the masses of the
-// task scenes' COM.  They are read from global memory where they are used, not kept across the main loop.
-template <int W, bool TASK, bool PUSH, bool DYN>
+// task scenes' COM.  They are read from global memory where they are used, not kept across the main loop.  LAT (with PUSH and DYN): the body of
+// dm_step_latency_kernel, the kernel of handles with a latency table (dm_set_action_latency*): at the Stable-PD stage of the update whose
+// counter (kBUpdates) equals the environment's pending action's due (DevStateLat::lat, by environment id; dm_latency.cuh), the pending targets
+// replace the target slot before it is read.  The table arrives inside st, which is then a DevStateLat: a parameter of its own, even one
+// always null in the other instantiations, changes the code the compiler makes of the plain and dynamics task kernels.
+template <int W, bool TASK, bool PUSH, bool DYN, bool LAT = false>
 __device__ __forceinline__ void dm_step_body(const DevModel* __restrict__ gm, const DevState& st, const double* __restrict__ frame_times,
                                              const float* __restrict__ frames, double dt, int n_updates, int sim_substeps, const StepLayout& LY,
                                              DevPush* push_in, const DevDyn* __restrict__ dyn_in) {
@@ -1635,7 +1639,14 @@ __device__ __forceinline__ void dm_step_body(const DevModel* __restrict__ gm, co
             {   // scope: only Kp e crosses the call
                 const float fdt = step_smem()[kHFdt];
                 const int jtype = (r.lk_int(kLInt) >> 8) & 0xff;
-                const float4 tg = reinterpret_cast<const float4*>(r.sim + 16 + 8 * nl)[li];
+                float4 tg = reinterpret_cast<const float4*>(r.sim + 16 + 8 * nl)[li];
+                if constexpr (LAT) {   // the pending action takes effect at this update: its targets into the target slot (the root's is never read)
+                    const DevLat& la = static_cast<const DevStateLat&>(st).lat[r.env];
+                    if (ls.get(kLsAlive) && la.due == reinterpret_cast<const int*>(r.sB)[kBUpdates] && li > 0) {
+                        tg = reinterpret_cast<const float4*>(la.tg)[li];
+                        if (r.act) reinterpret_cast<float4*>(r.sim + 16 + 8 * nl)[li] = tg;
+                    }
+                }
                 float e0 = 0, e1 = 0, e2 = 0;
                 if (jtype == kJSpherical) {
                     Q4 q = mkq(jp.x, jp.y, jp.z, jp.w);
@@ -1794,10 +1805,19 @@ __global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_dyn_kernel(const D
                                                                            DevPush* push, const DevDyn* dyn) {
     dm_step_body<W, TASK, true, true>(gm, st, frame_times, frames, dt, n_updates, sim_substeps, LY, push, dyn);
 }
+// handles with a latency table: the dynamics kernel's body with the pending actions (a unit-factor table when the handle has no dynamics)
+template <int W, bool TASK>
+__global__ void __launch_bounds__(kStepMaxThreads, 1) dm_step_latency_kernel(const DevModel* __restrict__ gm, DevStateLat st, const double* __restrict__ frame_times,
+                                                                               const float* __restrict__ frames, double dt, int n_updates, int sim_substeps, StepLayout LY,
+                                                                               DevPush* push, const DevDyn* dyn) {
+    dm_step_body<W, TASK, true, true, true>(gm, st, frame_times, frames, dt, n_updates, sim_substeps, LY, push, dyn);
+}
 
 const StepKernel kStepKernels[2][2] = {{dm_step_kernel<16, false>, dm_step_kernel<16, true>}, {dm_step_kernel<32, false>, dm_step_kernel<32, true>}};
 const StepPushKernel kStepPushKernels[2][2] = {{dm_step_push_kernel<16, false>, dm_step_push_kernel<16, true>}, {dm_step_push_kernel<32, false>, dm_step_push_kernel<32, true>}};
 const StepDynKernel kStepDynKernels[2][2] = {{dm_step_dyn_kernel<16, false>, dm_step_dyn_kernel<16, true>}, {dm_step_dyn_kernel<32, false>, dm_step_dyn_kernel<32, true>}};
+const StepLatKernel kStepLatKernels[2][2] = {{dm_step_latency_kernel<16, false>, dm_step_latency_kernel<16, true>},
+                                             {dm_step_latency_kernel<32, false>, dm_step_latency_kernel<32, true>}};
 
 // dm_reset's part of the push table: the environments the reset kernel is about to restart (the same rule) lose their push, as cWorld::Reset
 // clears its perturbations.  Launched before the reset kernel, only on handles with a push table.
@@ -1813,6 +1833,29 @@ __global__ void dm_dyn_draw_kernel(DevState st, DevDyn* dyn, DynRand R) {
     const int env = blockIdx.x * blockDim.x + threadIdx.x;
     if (env >= st.num_real) return;
     dyn_draw_env(R, R.env_base + static_cast<unsigned long long>(env), st.flags[static_cast<size_t>(env) * kFlagInts + kFResets], dyn[env]);
+}
+
+// dm_reset's and the latency setters' part of a latency table, one thread per real environment.  init (the table's first setter call): the
+// entry adopts the environment's reset counter, with no action pending, and an environment that has not run an update of its episode yet
+// (the handle's constructor resets every environment before any table exists) gets the hold below.  Otherwise an environment whose reset
+// counter moved since the entry last saw it was restarted: its pending action is dropped and its PD targets hold the pose the reset wrote (the rotations of the spherical
+// and the angles of the revolute joints, which share the target slot's body-frame convention; the slots dm_set_action never writes stay).  random: every environment's delay for its current episode (lat_draw, a pure
+// function of its reset counter, so the environments the reset did not restart keep theirs).
+__global__ void dm_latency_reset_kernel(const DevModel* __restrict__ gm, DevState st, DevLat* lat, LatRand R, int random, int init) {
+    const int env = blockIdx.x * blockDim.x + threadIdx.x;
+    if (env >= st.num_real) return;
+    DevLat& la = lat[env];
+    const int resets = st.flags[static_cast<size_t>(env) * kFlagInts + kFResets];
+    const bool restarted = init ? st.flags[static_cast<size_t>(env) * kFlagInts + kFUpdates] == 0 : la.resets != resets;
+    if (restarted) {
+        const DevModel& M = *gm;
+        const int nl = M.nl;
+        float4* sim = reinterpret_cast<float4*>(st.sim + static_cast<size_t>(env) * sim_stride(nl) + 16);
+        for (int l = 1; l < nl; ++l)
+            if (M.link[l].jtype == kJSpherical || M.link[l].jtype == kJRevolute) sim[2 * nl + l] = sim[l];
+    }
+    if (init || restarted) { la.due = -1; la.resets = resets; }
+    if (random) la.delay = lat_draw(R.lo, R.hi, R.seed, R.env_base + static_cast<unsigned long long>(env), resets);
 }
 
 // The push schedule (dm_push.cuh): refills the empty entries of the real environments that are not frozen.  Launched at the head of every

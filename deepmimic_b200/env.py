@@ -106,6 +106,26 @@ class DeepMimicBatchEnv:
         self._pre()
         self._core.set_dynamics_randomization(lohi)
 
+    def set_action_latency(self, seconds):
+        """Delay every environment's actions: the PD targets of an action take effect seconds[e] after set_action (a whole number of updates,
+        rounded to the nearest, in [0, (updates_per_action - 1) UPDATE_DT]); until then the previous targets act, and a reset holds the start
+        pose.  [N] seconds; kept across resets; state_dict() carries them and any pending action.  The policy's observations do not see it."""
+        self._pre()
+        self._core.set_action_latency(seconds)
+
+    def set_action_latency_randomization(self, lo, hi):
+        """Randomise the control latency for training: every environment draws its delay uniformly among the whole updates of [lo, hi] seconds on
+        the device, now and at every reset, from the env's seed and its global id (include/deepmimic_b200.h: dm_set_action_latency_randomization)"""
+        self._pre()
+        self._core.set_action_latency_randomization(lo, hi)
+
+    def action_latency(self):
+        """every environment's current control latency in seconds, a float64 device tensor [N].  No host synchronisation."""
+        self._pre()
+        t = self._core.action_latency()
+        self._post()
+        return t
+
     def get_name(self):
         """cScene::GetName of the configured scene (SceneImitate.cpp:209, SceneImitateAMP.cpp:211, SceneTargetAMP.cpp:233, ...)"""
         return self._core.scene_name()

@@ -2,8 +2,8 @@
 
     python -m deepmimic_b200.run --arg_file args/run_humanoid3d_spinkick_args.txt [--model_files PATH] [--num_envs 64]
         [--record_motion K] [--render K [--render_size WxH] [--camera yaw,pitch,distance,height,fov_deg]] [--episode_time 20] [--backend tensor_core] [--seed 0] [--device 0] [--asset_root DIR]
-        [--push_forces F1,F2,... [--push_body 0] [--push_time 2.0] [--push_duration 0.2]] [--dynamics_sweep KIND=V1,V2,...] [--pose_error]
-        [reference arguments ...]
+        [--push_forces F1,F2,... [--push_body 0] [--push_time 2.0] [--push_duration 0.2]] [--dynamics_sweep KIND=V1,V2,...] [--latency_sweep S1,S2,...]
+        [--pose_error] [reference arguments ...]
 
 --model_files (a reference TensorBundle prefix or a Trainer checkpoint, deepmimic_b200/model_files.py) and --output_path are read from the
 argument list, the command line before the arg file, as deepmimic_b200.train reads its paths; --train_agents and --agent_files are accepted
@@ -27,6 +27,11 @@ and the mean return.
 Dynamics sweep (--dynamics_sweep KIND=V1,V2,..., KIND one of friction, kp, kd, torque_limit, mass): environment e runs with the factor V[e % K]
 on that kind (DeepMimicBatchEnv.set_dynamics; for mass, every body's factor), the others 1.  run_log.txt then also has the column Dyn_<KIND>,
 and the summary one line per value: episodes, the fraction not ended by Fail and the mean return.  It combines with --push_forces.
+
+Latency sweep (--latency_sweep S1,S2,..., seconds): environment e runs with the control latency S[e % K], rounded to a whole 1/600 s update and
+at most 19 updates (0.0317 s) (DeepMimicBatchEnv.set_action_latency): the PD targets of each action take effect that long after the policy
+chose it.  run_log.txt then also has the column Latency (the rounded seconds), and the summary one line per value: episodes, the fraction not
+ended by Fail and the mean return.  It combines with --push_forces and --dynamics_sweep.
 
 Tracking error (--pose_error): how closely each episode followed its clip, in metres -- the mean over the non-root joints of the distance between
 the simulated and the kinematic character's joint positions relative to the root, in each one's heading frame, over the poses the episode took
@@ -60,6 +65,8 @@ def build_parser():
     ap.add_argument("--push_duration", type=float, default=0.2, help="length of the push in seconds (default 0.2)")
     ap.add_argument("--dynamics_sweep", type=parse_dynamics_sweep, default=None, metavar="KIND=V1,V2,...",
                     help="dynamics sweep: factors on friction, kp, kd, torque_limit or mass, environment e gets V[e %% K]")
+    ap.add_argument("--latency_sweep", type=parse_latency_sweep, default=None, metavar="S1,S2,...",
+                    help="latency sweep: control latencies in s (whole 1/600 s updates, at most 0.0317 s), environment e gets S[e %% K]")
     ap.add_argument("--pose_error", action="store_true",
                     help="score each episode's tracking of its clip: phase-locked and time-warped joint-position error in metres")
     return ap
@@ -87,6 +94,19 @@ def dynamics_plan(sweep, num_envs):
     import numpy as np
     kind, values = sweep
     return np.asarray([values[e % len(values)] for e in range(num_envs)], dtype=np.float32)
+
+
+def parse_latency_sweep(text):
+    """S1,S2,...: the latencies in seconds, each rounded to a whole update in [0, 19]; returns the rounded seconds"""
+    from .capi import UPDATE_DT, UPDATES_PER_ACTION, latency_updates
+    try:
+        v = [float(x) for x in text.split(",")]
+    except ValueError:
+        raise argparse.ArgumentTypeError("need comma-separated latencies in seconds, got %r" % text)
+    try:
+        return [latency_updates(x, UPDATES_PER_ACTION, "--latency_sweep") * UPDATE_DT for x in v]
+    except ValueError as e:
+        raise argparse.ArgumentTypeError(str(e))
 
 
 def parse_forces(text):
@@ -176,6 +196,9 @@ def main(argv=None):
     if opts.dynamics_sweep is not None:
         kind, fac = opts.dynamics_sweep[0], dynamics_plan(opts.dynamics_sweep, opts.num_envs)
         env.set_dynamics(**{kind: (np.repeat(fac[:, None], env._core.dims.num_joints, axis=1) if kind == "mass" else fac)})
+    if opts.latency_sweep is not None:
+        lat = np.asarray([opts.latency_sweep[e % len(opts.latency_sweep)] for e in range(opts.num_envs)])
+        env.set_action_latency(lat)
     ro = BatchedRollout(env, exp_rate=0.0, seed=opts.seed, backend=opts.backend)
     norms = dict(s_norm=ro.s_norm, a_norm=ro.a_norm, **(dict(g_norm=ro.g_norm) if ro.goal_size > 0 else {}))
     try:
@@ -198,6 +221,8 @@ def main(argv=None):
             log.log_tabular("Push_Dir", float(ang[e]))
         if opts.dynamics_sweep is not None:
             log.log_tabular("Dyn_" + kind, opts.dynamics_sweep[1][e % len(opts.dynamics_sweep[1])])
+        if opts.latency_sweep is not None:
+            log.log_tabular("Latency", float(lat[e]))
         if opts.pose_error:
             log.log_tabular("Pose_Err", float(perr[e]))
             log.log_tabular("Pose_Err_DTW", float(perr_dtw[e]))
@@ -219,6 +244,11 @@ def main(argv=None):
             sel = fac == np.float32(v)
             print("%s x %g: %d episodes, not ended by Fail %.3f, return %.4f%s" % (kind, v, int(sel.sum()), float(np.mean(term[sel] != 1)),
                                                                                     float(np.mean(ret[sel])), err_means(sel)))
+    if opts.latency_sweep is not None:
+        for v in dict.fromkeys(opts.latency_sweep):
+            sel = lat == v
+            print("latency %.4f s (%d updates): %d episodes, not ended by Fail %.3f, return %.4f%s" % (
+                v, round(v / env.UPDATE_DT), int(sel.sum()), float(np.mean(term[sel] != 1)), float(np.mean(ret[sel])), err_means(sel)))
     if opts.record_motion:
         paths = write_episode_motions(os.path.join(out_path, "motion_%d.txt"), ep, opts.record_motion,
                                       env.get_updates_per_action() * env.UPDATE_DT)

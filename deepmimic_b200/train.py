@@ -29,6 +29,11 @@ Training under randomised dynamics: --rand_friction, --rand_kp, --rand_kd, --ran
 switches randomisation on, a kind not given stays 1), draw every training environment's factors at every reset
 (DeepMimicBatchEnv.set_dynamics_randomization; --rand_mass draws one factor per body).  The evaluation (Test_Return) runs on the nominal
 model.  The bounds are part of the run record: --resume needs the same options.  They combine with the push options.
+
+Training under control latency: --rand_latency LO,HI (s) draws every training environment's actuation delay at every reset, a whole number of
+1/600 s updates between LO and HI rounded to the nearest update, at most 19 updates (0.0317 s) (DeepMimicBatchEnv.set_action_latency_randomization).
+The evaluation (Test_Return) runs without delay.  The bounds are part of the run record: --resume needs the same option.  It combines with the
+push and dynamics options.
 """
 import argparse
 import math
@@ -152,6 +157,18 @@ def dynamics_randomization(opts):
     return given or None
 
 
+def parse_latency_range(text):
+    """LO,HI seconds: each rounds to a whole update in [0, 19] (0 to 0.0317 s), LO <= HI"""
+    from .capi import UPDATES_PER_ACTION, latency_updates
+    v = parse_range(text)
+    try:
+        for x in v:
+            latency_updates(x, UPDATES_PER_ACTION)
+    except ValueError as e:
+        raise argparse.ArgumentTypeError(str(e))
+    return v
+
+
 def build_parser():
     ap = argparse.ArgumentParser(prog="python -m deepmimic_b200.train", description=__doc__.split("\n\n")[0], allow_abbrev=False)
     ap.add_argument("--asset_root", default=None, help="the reference's data / args tree (default: the bundled asset archive)")
@@ -171,6 +188,9 @@ def build_parser():
                     ("torque_limit", "every joint's torque limit"), ("mass", "every body's mass (one factor per body)")):
         ap.add_argument("--rand_" + k, type=parse_range, default=None, metavar="LO,HI",
                         help="training under randomised dynamics: range of the factor on %s, drawn per environment at every reset" % what)
+    ap.add_argument("--rand_latency", type=parse_latency_range, default=None, metavar="LO,HI",
+                    help="training under control latency: range of the actuation delay in s (whole 1/600 s updates, at most 0.0317 s), drawn per "
+                         "environment at every reset")
     return ap
 
 
@@ -208,7 +228,7 @@ def main(argv=None):
     ckpt = rank_path(os.path.join(out_path, "agent0_checkpoint.pt"), rank)
     tr = Trainer(scene_args, cfg, root, opts.num_envs, window_steps=opts.window_steps, backend=opts.backend, seed=opts.seed, device=device,
                  log_path=os.path.join(out_path, "agent0_log.txt"), append_log=opts.resume is not None, process_group=group, model_files=model_files,
-                 push_schedule=pushes, dynamics_randomization=dyn)
+                 push_schedule=pushes, dynamics_randomization=dyn, latency_randomization=opts.rand_latency)
     if opts.resume:
         tr.load(rank_path(opts.resume, rank))
     try:

@@ -291,6 +291,22 @@ def dynamics_record(dr):
     return out
 
 
+def latency_record(lr):
+    """a latency randomisation (lo_s, hi_s) in the run record's form: [lo, hi] in seconds, each rounded to a whole update
+    (DeepMimicBatchEnv.set_action_latency_randomization).  Refused unless both lie in [0, (updates_per_action - 1) UPDATE_DT] after rounding and
+    lo <= hi."""
+    from .capi import UPDATE_DT, UPDATES_PER_ACTION, latency_updates
+    if lr is None:
+        return None
+    v = list(lr)
+    if len(v) != 2:
+        raise ValueError("latency_randomization: a (lo, hi) pair in seconds expected")
+    d = [latency_updates(x, UPDATES_PER_ACTION, "latency_randomization") for x in v]
+    if d[0] > d[1]:
+        raise ValueError("latency_randomization: lo %r s > hi %r s" % (v[0], v[1]))
+    return [x * UPDATE_DT for x in d]
+
+
 class Trainer:
     """RLAgent's training loop over one batched environment (a reading of the reference, not checked against its source).
 
@@ -320,6 +336,10 @@ class Trainer:
     the training handle only (Test_Return stays an evaluation on the nominal model).  It joins the run record, so a checkpoint resumes only with
     the same bounds; the training handle's state blob carries the factors.
 
+    latency_randomization (train --rand_latency): (lo, hi) seconds of DeepMimicBatchEnv.set_action_latency_randomization, applied to the
+    training handle only (Test_Return stays an evaluation without delay).  It joins the run record, rounded to whole updates, so a checkpoint
+    resumes only with the same bounds; the training handle's state blob carries the delays and pending actions.
+
     Several GPUs (mpi_run.py --num_workers N): process_group, a torch.distributed group of one rank per GPU.  num_envs is the job's total, which
     must be divisible by the world size; each rank steps its contiguous share (global_env_offset = rank * num_envs / world, so every
     environment's reset stream is the one it has on one GPU), and evaluates ceil(TestEpisodes / world) episodes.  The learners average the
@@ -332,7 +352,7 @@ class Trainer:
 
     def __init__(self, args, config, asset_root, num_envs, window_steps=32, backend="tensor_core", seed=0, device=0, log_path=None, append_log=False,
                  env=None, test_env=None, process_group=None, model_files=None, push_schedule=None,
-                 dynamics_randomization=None):
+                 dynamics_randomization=None, latency_randomization=None):
         import torch
         from .env import DeepMimicBatchEnv
         from .learner import AMPDiscLearner, DataParallel, PPOLearner
@@ -359,6 +379,9 @@ class Trainer:
         dynamics_randomization = dynamics_record(dynamics_randomization)
         if dynamics_randomization is not None:   # runs without randomised dynamics keep the record they had
             self.run["dynamics_randomization"] = dynamics_randomization
+        latency_randomization = latency_record(latency_randomization)
+        if latency_randomization is not None:   # runs without latency keep the record they had
+            self.run["latency_randomization"] = latency_randomization
         rs = self.seed + 1000 * self.rank   # the rank's generators
         cfg = config
         self.env = env = env or DeepMimicBatchEnv(self.args, local, asset_root, device=device, seed=self.seed, global_env_offset=self.rank * local)
@@ -368,6 +391,8 @@ class Trainer:
             env.set_push_schedule(**push_schedule)
         if dynamics_randomization is not None:
             env.set_dynamics_randomization(**dynamics_randomization)
+        if latency_randomization is not None:
+            env.set_action_latency_randomization(*latency_randomization)
         S, A, G = env.get_state_size(), env.get_action_size(), env.get_goal_size()
         net = NETS[1] if G > 0 else NETS[0]
         for key in ("ActorNet", "CriticNet"):
@@ -583,6 +608,9 @@ class Trainer:
         if s["run"].get("dynamics_randomization") != self.run.get("dynamics_randomization"):   # a checkpoint without the key is a nominal run
             raise ValueError("checkpoint: its run trained under the dynamics randomisation %s, this one under %s: resume with the --rand_* "
                              "options the run started with" % (s["run"].get("dynamics_randomization"), self.run.get("dynamics_randomization")))
+        if s["run"].get("latency_randomization") != self.run.get("latency_randomization"):   # a checkpoint without the key is a run without delay
+            raise ValueError("checkpoint: its run trained under the latency randomisation %s, this one under %s: resume with the --rand_latency "
+                             "option the run started with" % (s["run"].get("latency_randomization"), self.run.get("latency_randomization")))
         for k in self.run:
             if s["run"].get(k, 1 if k == "world" else None) != self.run[k]:   # a checkpoint without a world size is a one-rank run's
                 raise ValueError("checkpoint: its %s differs from this run's" % ("agent file" if k == "agent" else "world size" if k == "world" else k))

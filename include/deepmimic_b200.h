@@ -149,6 +149,30 @@ int dm_get_push_table(dm_handle* h, int32_t* h_body, float* h_force, double* h_w
 int dm_set_dynamics(dm_handle* h, const float* h_factors);
 int dm_get_dynamics(dm_handle* h, float* d_out);
 int dm_set_dynamics_randomization(dm_handle* h, const double* lohi);
+/* Control latency: every environment e has a delay d_e, a whole number of updates in [0, updates_per_action - 1] (0-31.7 ms at 600 Hz / 30 Hz).
+ * The PD targets of an action set by dm_set_action take effect at the Stable-PD stage of the (d_e + 1)-th update after it; until then the
+ * previous targets act.  One action at most is pending per environment: a dm_set_action that arrives while one is still pending replaces it.
+ * need_new_action, the AMP history, the task scenes' previous-action COM, observations and rewards stay at the action's time: the policy is not
+ * told its delay.  A reset drops the environment's pending action and makes its PD targets the pose the reset wrote, so the first d_e updates
+ * of an episode hold the start pose.  d_e = 0 is the plain handle.
+ * dm_set_action_latency: h_updates [N] delays, kept across resets; a delay outside [0, updates_per_action - 1] is refused with its environment.
+ * Stream-ordered, then synchronises the stream.
+ * dm_set_action_latency_randomization: draws every real environment's delay for its current episode, then again at each reset: the delay of the
+ * episode with reset counter r is lo + min(hi - lo, floor(u (hi - lo + 1))), u = task_u01(seed ^ "latency", global env id, r), the library's counter-based uniform.  The same
+ * delays at any GPU count.  0 <= lo <= hi <= updates_per_action - 1, or a refusal naming the bound.
+ * The first call of either setter allocates the table, and every environment that has not run an update of its episode yet (after the handle's
+ * own first reset, say) holds its start pose as after a reset; set the table before the episode's first dm_set_action.  That call also
+ * switches the action and step launches to their latency instantiations (which also
+ * apply the handle's push and dynamics tables), and synchronises the stream; later randomisation calls and the draws at resets do not.  The
+ * table has one owner: each of the two refuses a handle set up by the other.  Handles that never call them run exactly as before.
+ * dm_get_action_latency: every environment's current delay into d_out [N] on the device, stream-ordered, no host synchronisation; refuses a
+ * handle without a table.  dm_save_state / dm_load_state carry the table -- delays, pending targets and the update each takes effect at -- at
+ * the end of the blob of a handle that has one, so a save in the middle of a policy step resumes bit for bit; the header's latency_table field
+ * makes a load refuse a blob with a table into a handle without one, and the reverse, and the randomisation hash a blob of other bounds or
+ * none.  Handles without a table write the blob they wrote before. */
+int dm_set_action_latency(dm_handle* h, const int32_t* h_updates);
+int dm_set_action_latency_randomization(dm_handle* h, int lo, int hi);
+int dm_get_action_latency(dm_handle* h, int32_t* d_out);
 /* Placement of the environments in the step kernel (on by default; tile width 16 only, where two environments share a warp: tile width 32
  * handles keep index placement, where it measured slower): every step launch is preceded by a one-block kernel that orders the
  * environments by contact load -- the solver row count of each environment's last Bullet sub-step, its key -- so that environments of equal
