@@ -64,7 +64,7 @@ class DmCamera(C.Structure):
 
 
 EXPORTS = ["dm_create", "dm_load_host", "dm_plan_launch", "dm_get_model_info", "dm_get_link_table", "dm_destroy", "dm_last_error", "dm_get_dims", "dm_get_static", "dm_get_scene_name", "dm_stream", "dm_sync", "dm_set_mode", "dm_set_sample_count", "dm_get_time_limits", "dm_reset", "dm_set_action",
-           "dm_update", "dm_set_pushes", "dm_get_pushes", "dm_set_push_schedule", "dm_get_push_table", "dm_set_dynamics", "dm_get_dynamics", "dm_set_dynamics_randomization", "dm_set_action_latency", "dm_set_action_latency_randomization", "dm_get_action_latency", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_record_pose", "dm_render_poses", "dm_record_kin_pose", "dm_pose_error", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
+           "dm_update", "dm_set_pushes", "dm_get_pushes", "dm_set_push_schedule", "dm_get_push_table", "dm_set_dynamics", "dm_get_dynamics", "dm_set_dynamics_randomization", "dm_set_action_latency", "dm_set_action_latency_randomization", "dm_get_action_latency", "dm_set_goal_course", "dm_get_course_record", "dm_set_env_order", "dm_plan_env_order", "dm_get_env_order", "dm_record_state", "dm_record_goal", "dm_record_pose", "dm_render_poses", "dm_render_poses_marked", "dm_record_kin_pose", "dm_pose_error", "dm_goal_host", "dm_reset_clips", "dm_record_amp_obs_expert_clips", "dm_get_clip_table", "dm_get_task_state", "dm_set_task_state", "dm_get_task_params", "dm_calc_reward", "dm_calc_reward_imitate", "dm_record_amp_obs_agent", "dm_record_amp_obs_expert", "dm_amp_obs_host", "dm_sample_amp_obs_expert", "dm_expert_sample_count", "dm_observe", "dm_get_flags", "dm_step_host", "dm_step_host_reset", "dm_set_time_limits", "dm_exchange_create", "dm_exchange_connect", "dm_exchange_publish", "dm_exchange_acquire", "dm_exchange_release", "dm_exchange_status", "dm_exchange_destroy", "dm_set_timing", "dm_step_host_timing", "dm_get_snapshot",
            "dm_set_snapshot", "dm_state_size", "dm_save_state", "dm_load_state", "dm_get_counters", "dm_get_section_profile", "dm_mlp_create", "dm_mlp_forward", "dm_mlp_create_gated", "dm_mlp_forward_gated",
            "dm_mlp_forward_style_reward", "dm_mlp_launches", "dm_mlp_destroy", "dm_td_lambda_returns", "dm_mlp_set_weights_device", "dm_learn_create",
            "dm_mlp_set_normalizers_device", "dm_learn_set_weights", "dm_learn_step", "dm_learn_disc_step", "dm_learn_destroy",
@@ -118,6 +118,10 @@ def lib():
             L.dm_get_action_latency.argtypes = [vp, C.c_void_p]
         if hasattr(L, "dm_render_poses"):   # likewise a library built before the renderer
             L.dm_render_poses.argtypes = [vp, C.c_int, C.c_void_p, C.POINTER(DmCamera), C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+        if hasattr(L, "dm_set_goal_course"):   # and before goal courses and the marked renderer
+            L.dm_set_goal_course.argtypes = [vp, C.POINTER(C.c_int32), dp]
+            L.dm_get_course_record.argtypes = [vp, C.c_void_p]
+            L.dm_render_poses_marked.argtypes = [vp, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(DmCamera), C.c_int, C.c_int, C.c_void_p, C.c_void_p]
         if hasattr(L, "dm_pose_error"):   # and before the tracking error
             L.dm_record_kin_pose.argtypes = [vp, fp]
             L.dm_pose_error.argtypes = [vp, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -234,6 +238,9 @@ def latency_updates(seconds, updates_per_action=UPDATES_PER_ACTION, what="latenc
         raise ValueError("%s: %r s rounds to %d updates, outside [0, %d] (0 to %.4f s)" % (what, seconds, d, updates_per_action - 1,
                                                                                              (updates_per_action - 1) * UPDATE_DT))
     return d
+
+
+MAX_COURSE_POINTS = 16   # rows of a goal course per environment (dm_course.cuh: kMaxCoursePoints)
 
 
 def _dptr(a):
@@ -455,6 +462,31 @@ class BatchedCore:
             self._chk(lib().dm_get_action_latency(self.h, C.c_void_p(out.data_ptr())))
             return out.to(torch.float64) * UPDATE_DT
 
+    def set_goal_course(self, counts, rows):
+        """dm_set_goal_course: every environment's goal course, counts [N] int (0 to MAX_COURSE_POINTS; 0 keeps the scene's own goals) and rows
+        [N, MAX_COURSE_POINTS, 3] float64 (heading scenes: episode time s, heading rad, speed m/s; target scene: waypoint dx, dz in m and an
+        unused value).  Numpy arrays or tensors (copied to the host); the library refuses bad values by name.  Every course restarts now, from
+        the current root and episode time.  Synchronises the handle's stream."""
+        if hasattr(counts, "detach"):
+            counts = counts.detach().cpu().numpy()
+        if hasattr(rows, "detach"):
+            rows = rows.detach().cpu().numpy()
+        n = np.ascontiguousarray(counts, dtype=np.int32).reshape(-1)
+        r = np.ascontiguousarray(rows, dtype=np.float64)
+        if n.shape != (self.num_envs,):
+            raise ValueError("set_goal_course: counts must hold %d values, got %d" % (self.num_envs, n.size))
+        if r.shape != (self.num_envs, MAX_COURSE_POINTS, 3):
+            raise ValueError("set_goal_course: rows must be [%d, %d, 3], got %s" % (self.num_envs, MAX_COURSE_POINTS, r.shape))
+        self._chk(lib().dm_set_goal_course(self.h, n.ctypes.data_as(C.POINTER(C.c_int32)), _dptr(r)))
+
+    def course_record(self, out):
+        """dm_get_course_record: every environment's record of its last course call into out, a contiguous float32 tensor [N, 4] on the
+        handle's device (heading: goal point x, z, along-track speed error, cross-track speed; target: goal waypoint x, z, waypoints reached,
+        distance to the goal waypoint).  Stream-ordered, no host synchronisation.  Refused on a handle without a course."""
+        _check_device_f32(out, "course_record: out", (self.num_envs, 4))
+        self._chk(lib().dm_get_course_record(self.h, C.c_void_p(out.data_ptr())))
+        return out
+
     def set_env_order(self, on):
         """dm_set_env_order: place the environments in the step kernel by contact load (the default; tile width 16 only) or by index"""
         self._chk(lib().dm_set_env_order(self.h, 1 if on else 0))
@@ -516,11 +548,13 @@ class BatchedCore:
         self._chk(lib().dm_pose_error(self.h, T, n, ptr(a), ptr(r), ptr(lengths), ptr(outs[0]), ptr(outs[1])))
         return outs[0], outs[1]
 
-    def render_poses(self, pose, camera=None, width=640, height=360, rgb=None, ids=None):
+    def render_poses(self, pose, camera=None, width=640, height=360, rgb=None, ids=None, markers=None):
         """dm_render_poses: pose rows [V, pose_dim] (a contiguous float32 tensor on the handle's device, dm_record_pose's layout) drawn as this handle's
         character by the device ray caster, seen from `camera` (a dict of yaw, pitch, distance, target_height, fov_y in radians and metres;
         missing keys and None: DEFAULT_CAMERA).  Returns (rgb uint8 [V, height, width, 3], ids int16 [V, height, width]: -1 sky, -2 ground, k link
-        k); pass rgb / ids tensors to fill them in place, or False to skip that output.  Stream-ordered on the handle's stream."""
+        k, -3 marker); pass rgb / ids tensors to fill them in place, or False to skip that output.  markers: [V, 4] float32 (x, y, z, radius in
+        metres; radius <= 0 draws none) on the handle's device draws one sphere per view (dm_render_poses_marked).  Stream-ordered on the
+        handle's stream."""
         import torch
         P = self.dims.pose_dim
         if pose.dim() != 2 or pose.shape[1] != P:
@@ -540,7 +574,12 @@ class BatchedCore:
             outs.append(t)
         cam = camera_struct(camera)
         ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
-        self._chk(lib().dm_render_poses(self.h, V, ptr(pose), C.byref(cam), int(width), int(height), ptr(outs[0]), ptr(outs[1])))
+        if markers is None:
+            self._chk(lib().dm_render_poses(self.h, V, ptr(pose), C.byref(cam), int(width), int(height), ptr(outs[0]), ptr(outs[1])))
+        else:
+            _check_device_f32(markers, "render_poses: markers", (V, 4), device=dev)
+            self._chk(lib().dm_render_poses_marked(self.h, V, ptr(pose), ptr(markers), C.byref(cam), int(width), int(height), ptr(outs[0]),
+                                                   ptr(outs[1])))
         return outs[0], outs[1]
 
     def reward_imitate(self, out):  # torch float32 cuda tensor [N]: CalcRewardImitate also in the task scenes (active clip of the dataset)

@@ -113,6 +113,8 @@ struct dm_handle {
     dmk::DevDyn* d_dyn_unit = nullptr;  // the latency step kernel's dynamics table on a handle without one: every factor 1
     bool lat_random = false;            // the delays are drawn by lat_rand at every reset (and owned by it)
     dmk::LatRand lat_rand{};
+    dmk::DevCourse* d_course = nullptr;   // goal courses (dm_set_goal_course): null until the first call, then dm_course_kernel follows every reset
+    float* d_course_rec = nullptr;        // and step launch, and writes the record here ([num_envs x 4], dm_get_course_record)
     int* d_order = nullptr;   // placement of the environments in the step kernel's tiles (dm_set_env_order); st.order is it or null
     dmk::StepLayout lay{};
     uint64_t seed = 0, env_offset = 0;
@@ -414,6 +416,11 @@ int launch_step(dm_handle* h, double dt, int n_updates) {
     else
         dmk::kStepKernels[tile_index(h)][task_scene(h)]<<<grid, block, h->smem_bytes, h->stream>>>(h->d_model, h->st, h->d_frame_times, h->d_frames, dt, n_updates,
                                                                                                   h->sa.cfg.num_sim_substeps, h->lay);
+    return launched(h);
+}
+// dm_course_kernel (dm_course.cuh) on every real environment of a handle with a course table
+int launch_course(dm_handle* h, int mode) {
+    dmk::dm_course_kernel<<<(h->num_envs + 127) / 128, 128, 0, h->stream>>>(h->d_model, h->st, h->d_course, h->d_course_rec, h->num_envs, mode);
     return launched(h);
 }
 int launch_observe_fan(dm_handle* h, const dmk::ObsFan& fan) {
@@ -868,7 +875,8 @@ int dm_reset_clips(dm_handle* h, int force_all, const int* h_clip, const double*
     if (!task_scene(h)) return 0;
     // cSceneTargetAMP::Reset's own part for the environments that were just reset
     dmk::dm_task_reset_kernel<<<(h->padded_envs + 127) / 128, 128, 0, h->stream>>>(h->d_model, h->st, h->padded_envs);
-    return launched(h);
+    if (launched(h)) return 1;
+    return h->d_course ? launch_course(h, dmk::kCourseReset) : 0;   // the restarted course environments start their course
 }
 int dm_reset(dm_handle* h, int force_all, const double* kt, const double* mt, const double* th) { return dm_reset_clips(h, force_all, nullptr, kt, mt, th); }
 int dm_get_clip_table(dm_handle* h, int* num_clips, double* h_dur, double* h_cdf) {
@@ -892,7 +900,8 @@ int dm_update(dm_handle* h, double dt, int n_updates) {
         dmk::dm_push_schedule_kernel<<<(h->num_envs + 127) / 128, 128, 0, h->stream>>>(h->st, h->d_push, h->d_push_sched, h->push_sched);
         if (launched(h)) return 1;
     }
-    return launch_step(h, dt, n_updates);
+    if (launch_step(h, dt, n_updates)) return 1;
+    return h->d_course ? launch_course(h, dmk::kCourseStep) : 0;   // record, waypoints and goal for the new episode time
 }
 // the handle's push table, every entry empty (the padding environments never run: theirs stay empty)
 static int alloc_push_table(dm_handle* h) {
@@ -1141,6 +1150,53 @@ int dm_get_action_latency(dm_handle* h, int32_t* d_out) {
     DM_CUDA(cudaMemcpy2DAsync(d_out, sizeof(int32_t), h->d_lat, sizeof(dmk::DevLat), sizeof(int32_t), static_cast<size_t>(h->num_envs), cudaMemcpyDeviceToDevice, h->stream));
     return 0;
 }
+// ---- goal courses (dm_course.cuh)
+int dm_set_goal_course(dm_handle* h, const int32_t* h_count, const double* h_rows) {
+    DM_DEVICE(h);
+    auto refuse = [](const std::string& what) { g_err = "dm_set_goal_course: " + what; return fail(); };
+    const int kind = task_scene(h) ? dmk::task_base_kind(h->hm.task_kind) : dmk::kTaskNone;
+    if (h->hm.task_kind == dmk::kTaskStrike || kind == dmk::kTaskNone)
+        return refuse("the scene has no courses (heading_amp, heading_amp_getup and target_amp have; this is " + h->sa.cfg.scene + ")");
+    if (!h_count) return refuse("h_count is required");
+    if (!h_rows) return refuse("h_rows is required");
+    const bool heading = kind == dmk::kTaskHeading;
+    for (int e = 0; e < h->num_envs; ++e) {
+        const std::string env = "environment " + std::to_string(e) + ": ";
+        const int n = h_count[e];
+        if (n < 0 || n > dmk::kMaxCoursePoints) return refuse(env + "count " + std::to_string(n) + " is outside [0, " + std::to_string(dmk::kMaxCoursePoints) + "]");
+        const double* r = h_rows + static_cast<size_t>(e) * dmk::kMaxCoursePoints * 3;
+        for (int k = 0; k < n; ++k) {
+            const std::string row = env + "row " + std::to_string(k) + ": ";
+            for (int i = 0; i < (heading ? 3 : 2); ++i)
+                if (!std::isfinite(r[3 * k + i])) return refuse(row + (heading ? (i == 0 ? "time" : i == 1 ? "heading" : "speed") : (i == 0 ? "dx" : "dz")) + " is not finite");
+            if (!heading) continue;
+            if (k == 0 && r[0] < 0.0) return refuse(row + "time " + std::to_string(r[0]) + " is negative");
+            if (k > 0 && !(r[3 * k] > r[3 * (k - 1)])) return refuse(row + "time " + std::to_string(r[3 * k]) + " is not after the previous row's " + std::to_string(r[3 * (k - 1)]));
+            if (r[3 * k + 2] < 0.0) return refuse(row + "speed " + std::to_string(r[3 * k + 2]) + " is negative");
+        }
+    }
+    const size_t N = static_cast<size_t>(h->num_envs);
+    if (h->d_course == nullptr) {
+        if (alloc_buffer(h, &h->d_course, N, kZeroed) || alloc_buffer(h, &h->d_course_rec, N * dmk::kCourseRecordFloats, kZeroed)) return 1;
+    }
+    std::vector<dmk::DevCourse> c(N);
+    std::memset(c.data(), 0, N * sizeof(dmk::DevCourse));
+    for (size_t e = 0; e < N; ++e) {
+        c[e].n = h_count[e];
+        std::memcpy(c[e].row, h_rows + e * dmk::kMaxCoursePoints * 3, static_cast<size_t>(c[e].n) * 3 * sizeof(double));
+    }
+    DM_CUDA(cudaMemcpyAsync(h->d_course, c.data(), N * sizeof(dmk::DevCourse), cudaMemcpyHostToDevice, h->stream));
+    if (launch_course(h, dmk::kCourseStartAll)) return 1;   // every course environment restarts from its root and episode time now
+    DM_CUDA(cudaStreamSynchronize(h->stream));   // the staging vector is pageable
+    return 0;
+}
+int dm_get_course_record(dm_handle* h, float* d_out) {
+    DM_DEVICE(h);
+    if (!d_out) { g_err = "dm_get_course_record: d_out is required"; return fail(); }
+    if (h->d_course == nullptr) { g_err = "dm_get_course_record: the handle has no course (dm_set_goal_course)"; return fail(); }
+    DM_CUDA(cudaMemcpyAsync(d_out, h->d_course_rec, static_cast<size_t>(h->num_envs) * dmk::kCourseRecordFloats * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
+    return 0;
+}
 int dm_set_env_order(dm_handle* h, int on) {
     DM_DEVICE(h);
     // placement by contact load pays where two environments share a warp (W = 16).  With one environment per warp (dog3d, W = 32) it measured
@@ -1187,9 +1243,10 @@ int dm_record_pose(dm_handle* h, float* d_pose, float* d_vel) {
     if (d_pose == nullptr && d_vel == nullptr) return 0;
     return launch_pose(h, d_pose, d_vel);
 }
-int dm_render_poses(dm_handle* h, int n_views, const float* d_pose, const dm_camera* cam, int width, int height, uint8_t* d_rgb, int16_t* d_ids) {
-    DM_DEVICE(h);
-    auto refuse = [](const std::string& what) { g_err = "dm_render_poses: " + what; return fail(); };
+// dm_render_poses (dm_render_kernel) and dm_render_poses_marked (then the dm_render_marked_kernel overlay): the checks, the camera and the launches
+static int render_poses(dm_handle* h, const char* fn, int n_views, const float* d_pose, const float* d_marker, const dm_camera* cam, int width, int height,
+                        uint8_t* d_rgb, int16_t* d_ids) {
+    auto refuse = [fn](const std::string& what) { g_err = std::string(fn) + ": " + what; return fail(); };
     if (n_views < 1 || n_views > 65535) return refuse("n_views " + std::to_string(n_views) + " outside [1, 65535]");
     if (width < 16 || width > 4096) return refuse("width " + std::to_string(width) + " outside [16, 4096]");
     if (height < 16 || height > 4096) return refuse("height " + std::to_string(height) + " outside [16, 4096]");
@@ -1214,8 +1271,22 @@ int dm_render_poses(dm_handle* h, int n_views, const float* d_pose, const dm_cam
     const int T = dmk::kRenderTile;
     const dim3 grid(((width + T - 1) / T) * ((height + T - 1) / T), n_views);
     dmk::dm_render_kernel<<<grid, T * T, 0, h->stream>>>(h->d_model, d_pose, width, height, rc, d_rgb, d_ids);
+    if (d_marker) {   // the marker overlay: only the pixels the markers change
+        DM_CUDA(cudaGetLastError());
+        dmk::dm_render_marked_kernel<<<grid, T * T, 0, h->stream>>>(h->d_model, d_pose, d_marker, width, height, rc, d_rgb, d_ids);
+    }
     DM_CUDA(cudaGetLastError());
     return 0;
+}
+int dm_render_poses(dm_handle* h, int n_views, const float* d_pose, const dm_camera* cam, int width, int height, uint8_t* d_rgb, int16_t* d_ids) {
+    DM_DEVICE(h);
+    return render_poses(h, "dm_render_poses", n_views, d_pose, nullptr, cam, width, height, d_rgb, d_ids);
+}
+int dm_render_poses_marked(dm_handle* h, int n_views, const float* d_pose, const float* d_marker, const dm_camera* cam, int width, int height, uint8_t* d_rgb,
+                           int16_t* d_ids) {
+    DM_DEVICE(h);
+    if (d_marker == nullptr) { g_err = "dm_render_poses_marked: d_marker is NULL"; return fail(); }
+    return render_poses(h, "dm_render_poses_marked", n_views, d_pose, d_marker, cam, width, height, d_rgb, d_ids);
 }
 int dm_record_kin_pose(dm_handle* h, float* d_pose) {
     DM_DEVICE(h);
@@ -1719,6 +1790,7 @@ int dm_state_size(dm_handle* h, size_t* bytes) {
 }
 int dm_save_state(dm_handle* h, void* h_out) {
     DM_DEVICE(h);
+    if (h->d_course) { g_err = "dm_save_state: the handle has a goal course (dm_set_goal_course); courses belong to runs, and the state blob does not carry them"; return fail(); }
     if (h->d_push && !h->d_push_sched) {   // a pending push set by dm_set_pushes is not part of the state blob
         std::vector<int32_t> body(static_cast<size_t>(h->num_envs));
         if (dm_get_pushes(h, body.data())) return 1;
@@ -1743,6 +1815,7 @@ int dm_save_state(dm_handle* h, void* h_out) {
 }
 int dm_load_state(dm_handle* h, const void* h_in) {
     DM_DEVICE(h);
+    if (h->d_course) { g_err = "dm_load_state: the handle has a goal course (dm_set_goal_course); courses belong to runs, and the state blob does not carry them"; return fail(); }
     StateHeader in;
     std::memcpy(&in, h_in, sizeof(in));
     const StateHeader mine = state_header(h);

@@ -11,6 +11,7 @@
 
 #include "dm_math.cuh"
 
+#include "dm_course.cuh"
 #include "dm_dynamics.cuh"
 #include "dm_latency.cuh"
 #include "dm_push.cuh"
@@ -232,6 +233,8 @@ __global__ void dm_push_clear_kernel(DevState, DevPush*, int);
 __global__ void dm_push_schedule_kernel(DevState, DevPush*, double*, PushSchedule);
 __global__ void dm_dyn_draw_kernel(DevState, DevDyn*, DynRand);
 __global__ void dm_latency_reset_kernel(const DevModel*, DevState, DevLat*, LatRand, int, int);
+enum CourseMode { kCourseReset = 0, kCourseStep = 1, kCourseStartAll = 2 };
+__global__ void dm_course_kernel(const DevModel*, DevState, DevCourse*, float*, int, int);   // dm_course.cu
 __global__ void dm_task_observe_kernel(const DevModel*, DevState, float*, float*, int);
 int dm_step_layout(int nl, int n, int chain_len, int maxrows, int W, StepLayout* L);
 int dm_step_smem_bytes(const StepLayout& L, int tiles);

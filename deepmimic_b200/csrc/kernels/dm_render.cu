@@ -12,6 +12,7 @@ namespace {
 constexpr float kLightX = 0.40824829f, kLightY = 0.81649658f, kLightZ = 0.40824829f;   // towards the light: (1, 2, 1) / sqrt(6)
 constexpr float kAmbient = 0.35f, kDiffuse = 0.65f;        // colour = base * (ambient + diffuse * max(n . light, 0) unless shadowed)
 constexpr float kCharR = 0.80f, kCharG = 0.45f, kCharB = 0.25f;
+constexpr float kMarkR = 0.15f, kMarkG = 0.75f, kMarkB = 0.30f;   // the goal marker (dm_render_poses_marked)
 constexpr float kGroundLight = 0.62f, kGroundDark = 0.50f;   // 1 m checker: (floor(x) + floor(z)) even / odd
 constexpr float kSkyHorizonR = 0.80f, kSkyHorizonG = 0.87f, kSkyHorizonB = 0.95f;   // at ray y <= 0
 constexpr float kSkyZenithR = 0.40f, kSkyZenithG = 0.60f, kSkyZenithB = 0.90f;      // at ray y = 1
@@ -78,13 +79,21 @@ __device__ __forceinline__ uint8_t to_u8(float c) { return static_cast<uint8_t>(
 }  // namespace
 
 // pose: [gridDim.y x pose_dim] rows; rgb [views x height x width x 3] and ids [views x height x width] (-1 sky, -2 ground, k link k), row 0
-// at the top; either may be null
-__global__ void __launch_bounds__(kRenderTile * kRenderTile) dm_render_kernel(const DevModel* __restrict__ gm, const float* __restrict__ pose, int width,
-                                                                                int height, RenderCam cam, uint8_t* __restrict__ rgb, int16_t* __restrict__ ids) {
+// at the top; either may be null.
+// MARK (dm_render_marked_kernel): an overlay on the plain kernel's output.  marker [gridDim.y x 4] (x, y, z, radius; radius <= 0: none) is a
+// sphere hit after the links, shaded like them in a colour of its own (id kRenderMarkerId), and casting shadows like them; the overlay writes
+// only the pixels the marker changes -- its own, and the lit ones whose shadow ray only the marker blocks -- so every other pixel keeps the
+// plain kernel's bytes
+template <bool MARK>
+__device__ __forceinline__ void render_body(const DevModel* __restrict__ gm, const float* __restrict__ pose, const float* __restrict__ marker, int width,
+                                            int height, RenderCam cam, uint8_t* __restrict__ rgb, int16_t* __restrict__ ids) {
     __shared__ RLink sl[kMaxLinks];
     const DevModel& M = *gm;
     const int nl = M.nl;
     const float* p = pose + static_cast<size_t>(blockIdx.y) * M.pose_dim;
+    if constexpr (MARK) {
+        if (!(marker[4 * static_cast<size_t>(blockIdx.y) + 3] > 0.f)) return;   // the whole block: one view without a marker
+    }
     if (threadIdx.x < 32) {
         // link frames, lane = link (cKinTree::JointWorldTrans as amp_obs_tile walks it): joint frames level by level from att_pt / att_rot and
         // the joint rotations, then each body frame from body_att and child_rot -- the collision pass's link frame, in unscaled metres
@@ -138,9 +147,21 @@ __global__ void __launch_bounds__(kRenderTile * kRenderTile) dm_render_kernel(co
         float t; V3 nk;
         if (hit_link(sl[k], eye, d, t, nk) && t < tbest) { tbest = t; n = nk; id = k; }
     }
+    RLink mk;
+    if constexpr (MARK) {
+        const float* m = marker + 4 * static_cast<size_t>(blockIdx.y);
+#pragma unroll
+        for (int i = 0; i < 9; ++i) mk.R[i] = (i % 4 == 0) ? 1.f : 0.f;
+        mk.c[0] = m[0]; mk.c[1] = m[1]; mk.c[2] = m[2];
+        mk.he[0] = m[3]; mk.he[1] = mk.he[2] = 0.f;
+        mk.shape = kSSphere;
+        float t; V3 nk;
+        if (hit_link(mk, eye, d, t, nk) && t < tbest) { tbest = t; n = nk; id = kRenderMarkerId; }
+    }
     const size_t pix = (static_cast<size_t>(blockIdx.y) * height + py) * width + px;
-    if (ids) ids[pix] = static_cast<int16_t>(id);
+    if (ids && (!MARK || id == kRenderMarkerId)) ids[pix] = static_cast<int16_t>(id);
     if (!rgb) return;
+    bool mark_shadow = false;   // MARK: the marker alone blocks the pixel's shadow ray
     float cr, cg, cb;
     if (id == -1) {
         const float s = fmaxf(d.y, 0.f);
@@ -150,7 +171,8 @@ __global__ void __launch_bounds__(kRenderTile * kRenderTile) dm_render_kernel(co
         if (id == -2) {
             const float g = ((static_cast<int>(floorf(P.x)) + static_cast<int>(floorf(P.z))) & 1) ? kGroundDark : kGroundLight;
             cr = cg = cb = g;
-        } else { cr = kCharR; cg = kCharG; cb = kCharB; }
+        } else if (MARK && id == kRenderMarkerId) { cr = kMarkR; cg = kMarkG; cb = kMarkB; }
+        else { cr = kCharR; cg = kCharG; cb = kCharB; }
         const V3 light = mk3(kLightX, kLightY, kLightZ);
         const float ndl = dot(n, light);
         float k = kAmbient;
@@ -158,12 +180,24 @@ __global__ void __launch_bounds__(kRenderTile * kRenderTile) dm_render_kernel(co
             const V3 so = P + kShadowBias * n;
             bool shadow = false;
             for (int j = 0; j < nl && !shadow; ++j) { float t; V3 nj; shadow = hit_link(sl[j], so, light, t, nj); }
+            if (MARK && !shadow) { float t; V3 nj; shadow = mark_shadow = hit_link(mk, so, light, t, nj); }
             if (!shadow) k += kDiffuse * ndl;
         }
         cr *= k; cg *= k; cb *= k;
     }
+    if (MARK && id != kRenderMarkerId && !mark_shadow) return;
     uint8_t* o = rgb + 3 * pix;
     o[0] = to_u8(cr); o[1] = to_u8(cg); o[2] = to_u8(cb);
+}
+
+__global__ void __launch_bounds__(kRenderTile * kRenderTile) dm_render_kernel(const DevModel* __restrict__ gm, const float* __restrict__ pose, int width,
+                                                                                int height, RenderCam cam, uint8_t* __restrict__ rgb, int16_t* __restrict__ ids) {
+    render_body<false>(gm, pose, nullptr, width, height, cam, rgb, ids);
+}
+__global__ void __launch_bounds__(kRenderTile * kRenderTile) dm_render_marked_kernel(const DevModel* __restrict__ gm, const float* __restrict__ pose,
+                                                                                       const float* __restrict__ marker, int width, int height, RenderCam cam,
+                                                                                       uint8_t* __restrict__ rgb, int16_t* __restrict__ ids) {
+    render_body<true>(gm, pose, marker, width, height, cam, rgb, ids);
 }
 
 }  // namespace dmk

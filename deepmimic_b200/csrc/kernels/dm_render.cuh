@@ -1,4 +1,4 @@
-// Ray-cast rendering of pose rows (dm_render.cu, C ABI dm_render_poses): the character's collision shapes on a checkered ground plane, seen
+// Ray-cast rendering of pose rows (dm_render.cu, C ABI dm_render_poses and dm_render_poses_marked): the character's collision shapes on a checkered ground plane, seen
 // from a camera that tracks each row's root.
 #pragma once
 #include <cstdint>
@@ -17,5 +17,10 @@ struct RenderCam {
 };
 
 __global__ void dm_render_kernel(const DevModel* gm, const float* pose, int width, int height, RenderCam cam, uint8_t* rgb, int16_t* ids);
+// one marker sphere per view (dm_render_poses_marked), an overlay launched after dm_render_kernel on the same outputs that writes only the
+// pixels the marker changes: marker [views x 4] = x, y, z, radius (unscaled metres; radius <= 0: none)
+constexpr int kRenderMarkerId = -3;   // the ids value of the marker's pixels
+__global__ void dm_render_marked_kernel(const DevModel* gm, const float* pose, const float* marker, int width, int height, RenderCam cam, uint8_t* rgb,
+                                        int16_t* ids);
 
 }  // namespace dmk

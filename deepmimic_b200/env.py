@@ -126,6 +126,49 @@ class DeepMimicBatchEnv:
         self._post()
         return t
 
+    def set_goal_course(self, rows, counts=None):
+        """Steer the heading and target scenes: commanded goals instead of the scene's random ones (include/deepmimic_b200.h:
+        dm_set_goal_course).  heading_amp / heading_amp_getup: rows of (episode time s, heading rad, speed m/s), times increasing from >= 0, the
+        goal linear in time between them; target_amp: rows of (dx, dz) m, waypoints relative to the root where the course starts, each
+        reached within the scene's success radius.  rows [K, 3 or 2] gives every environment the same course; [N, K, 3 or 2] with counts [N]
+        (default K each; 0 keeps the scene's own goals) gives each its own.  K <= 16.  Every course restarts now and at each reset;
+        course_record() reports how it is followed.  Synchronises the stream."""
+        from .capi import MAX_COURSE_POINTS
+        kind = int(self._core.task_params()[0][0])
+        width = 2 if kind == 1 else 3   # target_amp: (dx, dz); the heading scenes (t, h, v); the library refuses the other scenes
+        r = np.asarray(rows.detach().cpu().numpy() if hasattr(rows, "detach") else rows, dtype=np.float64)
+        N = self.num_envs
+        if r.ndim == 2:
+            if counts is not None:
+                raise ValueError("set_goal_course: counts go with per-environment rows [N, K, %d]" % width)
+            r = np.broadcast_to(r, (N,) + r.shape)
+        if r.ndim != 3 or r.shape[0] != N or r.shape[2] != width or not 1 <= r.shape[1] <= MAX_COURSE_POINTS:
+            raise ValueError("set_goal_course: rows must be [K, %d] or [%d, K, %d] with 1 <= K <= %d in this scene, got %s" % (
+                width, N, width, MAX_COURSE_POINTS, r.shape))
+        K = r.shape[1]
+        n = np.full(N, K, dtype=np.int32) if counts is None else np.asarray(counts, dtype=np.int64).reshape(-1)
+        if n.shape != (N,) or n.min() < 0 or n.max() > K:
+            raise ValueError("set_goal_course: counts must be %d values in [0, %d]" % (N, K))
+        full = np.zeros((N, MAX_COURSE_POINTS, 3))
+        full[:, :K, :width] = r
+        self._pre()
+        self._core.set_goal_course(n.astype(np.int32), full)
+        self.course_counts = n.astype(np.int32)
+        self.course_kind = "target" if kind == 1 else "heading"
+
+    def course_record(self):
+        """[N, 4] float32: every environment's record of its last step (or course start): heading scenes (goal point 1.5 m ahead of the root
+        along the commanded heading x, z; along-track speed minus the commanded speed; cross-track speed towards heading + pi / 2, m/s); the
+        target scene (the goal waypoint's x, z; waypoints reached; distance to the goal waypoint, m).  A view of a buffer rewritten by the next
+        call, like record_state; no host synchronisation."""
+        if getattr(self, "_course_rec", None) is None:
+            with self.torch.cuda.stream(self.stream):
+                self._course_rec = self.torch.zeros(self.num_envs, 4, device=self.device)
+        self._pre()
+        self._core.course_record(self._course_rec)
+        self._post()
+        return self._course_rec
+
     def get_name(self):
         """cScene::GetName of the configured scene (SceneImitate.cpp:209, SceneImitateAMP.cpp:211, SceneTargetAMP.cpp:233, ...)"""
         return self._core.scene_name()

@@ -50,10 +50,11 @@ def add_view_options(ap):
                         math.degrees(DEFAULT_CAMERA["fov_y"]))))
 
 
-def write_pose_apng(core, path, poses, durations, camera=None, size=(640, 360), chunk=32):
+def write_pose_apng(core, path, poses, durations, camera=None, size=(640, 360), chunk=32, markers=None):
     """pose rows [F, pose_dim] (numpy or tensor, the dm_record_pose layout) drawn as core's character (a BatchedCore) into the animated PNG
-    `path`, frame f shown for durations[f] seconds.  The rows are rendered and copied to the host `chunk` at a time on the handle's stream, so
-    device memory does not grow with F; the frames go to the file as they arrive."""
+    `path`, frame f shown for durations[f] seconds; markers [F, 4] (x, y, z, radius) adds a sphere to each frame (BatchedCore.render_poses).
+    The rows are rendered and copied to the host `chunk` at a time on the handle's stream, so device memory does not grow with F; the frames
+    go to the file as they arrive."""
     import torch
     width, height = size
     dev = torch.device("cuda", core.device)
@@ -62,7 +63,8 @@ def write_pose_apng(core, path, poses, durations, camera=None, size=(640, 360), 
         with torch.cuda.device(dev), torch.cuda.stream(torch.cuda.ExternalStream(core.stream(), device=dev)):
             for a in range(0, len(poses), chunk):
                 rows = torch.as_tensor(poses[a:a + chunk], dtype=torch.float32).to(dev).contiguous()
-                rgb, _ = core.render_poses(rows, camera, width, height, ids=False)
+                mk = None if markers is None else torch.as_tensor(markers[a:a + chunk], dtype=torch.float32).to(dev).contiguous()
+                rgb, _ = core.render_poses(rows, camera, width, height, ids=False, markers=mk)
                 yield from rgb.cpu().numpy()   # a copy to pageable memory: waits for the handle's stream
 
     from .formats import write_apng

@@ -539,7 +539,7 @@ class BatchedRollout:
     def stream(self):
         return self.env.stream
 
-    def collect(self, num_steps, record_stats=True, record_pose=False, record_kin_pose=False):
+    def collect(self, num_steps, record_stats=True, record_pose=False, record_kin_pose=False, record_course=False):
         """num_steps policy steps of all environments; returns dict of [T, N, .] tensors (states, actions, logps, rewards, dones, terminate,
         explore = the exploration draw of each step (True: the action was sampled, False: the mode was taken); goals
         in the goal-conditioned scenes; with a discriminator amp_obs, disc_logits, style_rewards, amp_rewards; with a critic values = V(s_k),
@@ -547,7 +547,8 @@ class BatchedRollout:
         reward.  A path still running at the last step is bootstrapped with its end value, as the reference bootstraps a path that ends by time
         limit (a deviation: the reference stores only complete paths).  record_pose adds the simulated characters' poses (env.record_pose),
         [T, N, pose_dim] each: poses / vels at s_k, end_poses / end_vels at s'_k, before the reset, like values / end_values.  record_kin_pose
-        adds kin_poses [T, N, pose_dim], the kinematic characters' poses (env.record_kin_pose) at s_k, recorded next to poses."""
+        adds kin_poses [T, N, pose_dim], the kinematic characters' poses (env.record_kin_pose) at s_k, recorded next to poses.  record_course
+        (an env with a goal course, env.set_goal_course) adds course [T, N, 4], env.course_record() after step k and before its reset."""
         t, env = self.torch, self.env
         N, S, A = env.num_envs, env.get_state_size(), env.get_action_size()
         out = dict(states=t.empty(num_steps, N, S, device=env.device), actions=t.empty(num_steps, N, A, device=env.device),
@@ -567,6 +568,8 @@ class BatchedRollout:
                 out[key] = t.empty(num_steps, N, P, device=env.device)
         if record_kin_pose:
             out["kin_poses"] = t.empty(num_steps, N, env.get_pose_dim(), device=env.device)
+        if record_course:
+            out["course"] = t.empty(num_steps, N, 4, device=env.device)
         crit = self.critic is not None
         if crit:
             for key in ("values", "end_values", "returns", "advantages"):
@@ -614,6 +617,8 @@ class BatchedRollout:
                 if record_pose:   # before the reset: the end pose of a finished episode is its terminal pose
                     p, v = env.record_pose()
                     out["end_poses"][k] = p; out["end_vels"][k] = v
+                if record_course:
+                    out["course"][k] = env.course_record()
                 if self.disc is not None:
                     # before the reset: the last transition of a finished episode is the agent's own motion, not the restarted state
                     amp = env.record_amp_obs_agent()
@@ -640,7 +645,27 @@ class BatchedRollout:
         return out
 
 
-def run_episodes(ro, pose_envs=0, limit=1 << 16, pose_error=False):
+def course_stats(kind, course, dones, counts, step_dt):
+    """aggregates of every environment's first episode from collect's course records [T, N, 4] and dones [T, N] (T covering it): kind
+    "heading" -> dict(speed_err [N], the mean |along-track speed - commanded speed|, and cross_speed [N], the mean |cross-track speed|, over the
+    episode's steps, m/s); "target" -> dict(waypoints [N], the waypoints reached, and course_time [N], the episode time in s at the end of the
+    step that reached the last of counts[e] waypoints, NaN if none did; step_dt: the policy step in s)"""
+    import torch as t
+    d = dones.to(t.int32)
+    first = (t.cumsum(d, 0) - d) == 0   # the steps of the first episode: no episode end before them
+    steps = first.sum(0)
+    if kind == "heading":
+        f = first.to(course.dtype)
+        return dict(speed_err=(course[..., 2].abs() * f).sum(0) / steps, cross_speed=(course[..., 3].abs() * f).sum(0) / steps)
+    last = (steps - 1).clamp(min=0).long()
+    reached = course[last, t.arange(course.shape[1], device=course.device), 2]
+    done_all = first & (course[..., 2] >= t.as_tensor(counts, device=course.device).to(course.dtype))
+    k = t.argmax(done_all.to(t.int32), 0)
+    ctime = t.where(done_all.any(0), (k + 1).to(course.dtype) * step_dt, t.full_like(reached, float("nan")))
+    return dict(waypoints=reached, course_time=ctime)
+
+
+def run_episodes(ro, pose_envs=0, limit=1 << 16, pose_error=False, course=False):
     """One complete episode of every environment of ro's env from its current state, in chunks of 32 policy steps of ro.collect (the
     environments that finish first keep running into their next episode, which is not counted).  Set the env's mode and ro's exploration
     before the call (test mode, exp_rate 0 for an evaluation).  One host synchronisation per chunk.  Returns dict(returns [N] float32, lengths
@@ -650,16 +675,20 @@ def run_episodes(ro, pose_envs=0, limit=1 << 16, pose_error=False):
     poses and kin poses (the simulated and the kinematic character at the step's start, collect's poses and kin_poses) and adds pose_err and
     pose_err_dtw [N] float32, the phase-locked and the time-warped tracking error in metres of each episode (one BatchedCore.pose_error call;
     the terminal pose is not scored).  That keeps 2 x T x N x pose_dim floats: 2 x 428 MB at N = 4096, T = 608 and pose_dim 43 (humanoid3d),
-    plus the call's scratch of about as much again.
+    plus the call's scratch of about as much again.  course=True (an env with a goal course) adds course [T, N, 4] (collect's records of
+    every step run) and course_stats' aggregates of each first episode: speed_err and cross_speed in the heading scenes, waypoints and
+    course_time in the target scene.
     RuntimeError when an episode runs longer than `limit` policy steps."""
     import torch as t
     env = ro.env
     n = env.num_envs
     ret, ended = t.zeros(n, device=env.device), t.zeros(n, dtype=t.bool, device=env.device)
     length, term = t.zeros(n, dtype=t.int32, device=env.device), t.zeros(n, dtype=t.int32, device=env.device)
-    poses, end_poses, all_poses, kin_poses = [], [], [], []
+    poses, end_poses, all_poses, kin_poses, courses, dones = [], [], [], [], [], []
     for _ in range(0, limit, 32):
-        traj = ro.collect(32, record_stats=False, record_pose=bool(pose_envs or pose_error), record_kin_pose=pose_error)
+        traj = ro.collect(32, record_stats=False, record_pose=bool(pose_envs or pose_error), record_kin_pose=pose_error, record_course=course)
+        if course:
+            courses.append(traj["course"]); dones.append(traj["dones"])
         if pose_envs:
             poses.append(traj["poses"][:, :pose_envs].clone()); end_poses.append(traj["end_poses"][:, :pose_envs].clone())
         if pose_error:
@@ -680,6 +709,10 @@ def run_episodes(ro, pose_envs=0, limit=1 << 16, pose_error=False):
                 lock, dtw = env._core.pose_error(a, r, length)
                 env._post()
                 out.update(pose_err=lock, pose_err_dtw=dtw)
+            if course:
+                rec = t.cat(courses)
+                out.update(course=rec, **course_stats(env.course_kind, rec, t.cat(dones), env.course_counts,
+                                                      env.get_updates_per_action() * env.UPDATE_DT))
             return out
     raise RuntimeError("an episode ran longer than %d policy steps" % limit)
 

@@ -3,7 +3,7 @@
     python -m deepmimic_b200.run --arg_file args/run_humanoid3d_spinkick_args.txt [--model_files PATH] [--num_envs 64]
         [--record_motion K] [--render K [--render_size WxH] [--camera yaw,pitch,distance,height,fov_deg]] [--episode_time 20] [--backend tensor_core] [--seed 0] [--device 0] [--asset_root DIR]
         [--push_forces F1,F2,... [--push_body 0] [--push_time 2.0] [--push_duration 0.2]] [--dynamics_sweep KIND=V1,V2,...] [--latency_sweep S1,S2,...]
-        [--pose_error] [reference arguments ...]
+        [--pose_error] [--heading_course T:H:V,... | --target_course DX:DZ,...] [reference arguments ...]
 
 --model_files (a reference TensorBundle prefix or a Trainer checkpoint, deepmimic_b200/model_files.py) and --output_path are read from the
 argument list, the command line before the arg file, as deepmimic_b200.train reads its paths; --train_agents and --agent_files are accepted
@@ -37,7 +37,19 @@ Tracking error (--pose_error): how closely each episode followed its clip, in me
 the simulated and the kinematic character's joint positions relative to the root, in each one's heading frame, over the poses the episode took
 its actions in (BatchedCore.pose_error).  run_log.txt then also has the columns Pose_Err (phase-locked: frame i against the clip at the same
 moment) and Pose_Err_DTW (after aligning the two motions by dynamic time warping, which forgives a skill that runs ahead of or behind its clip's
-phase), the summary a line with the mean and standard deviation of both, and every per-force and per-value line both means."""
+phase), the summary a line with the mean and standard deviation of both, and every per-force and per-value line both means.
+
+Goal courses (DeepMimicBatchEnv.set_goal_course; one course for every environment, restarted at its reset):
+  --heading_course T:H:V,...  (heading_amp, heading_amp_getup) commanded heading H (radians about the vertical axis, h = 0 along +x, the
+      convention of --camera and Push_Dir) and speed V (m/s) from episode time T (s) on, linear in between; times increasing from >= 0.
+      run_log.txt then also has Speed_Err (the mean |along-track speed - V| over the episode, m/s) and Cross_Speed (the mean |cross-track
+      speed|), and the summary a line with their means and the fraction not ended by Fail.
+  --target_course DX:DZ,...   (target_amp) waypoints in metres from where the character starts, each reached within the scene's success
+      radius, in order.  run_log.txt then also has Waypoints (the number reached) and Course_Time (the episode time at which the last one was
+      reached, nan if never), and the summary a line with the mean reached, the fraction that reached all and their mean time.
+At most 16 points.  Both combine with the push, dynamics and latency sweeps, whose per-value lines then carry the course's means, and with
+--render, whose frames draw the recorded goal (the point 1.5 m ahead along the commanded heading, or the waypoint) as a green sphere on the
+ground."""
 import argparse
 import os
 import sys
@@ -69,7 +81,56 @@ def build_parser():
                     help="latency sweep: control latencies in s (whole 1/600 s updates, at most 0.0317 s), environment e gets S[e %% K]")
     ap.add_argument("--pose_error", action="store_true",
                     help="score each episode's tracking of its clip: phase-locked and time-warped joint-position error in metres")
+    course = ap.add_mutually_exclusive_group()
+    course.add_argument("--heading_course", type=parse_heading_course, default=None, metavar="T:H:V,...",
+                        help="heading scenes: commanded heading H (rad) and speed V (m/s) from episode time T (s), linear in between")
+    course.add_argument("--target_course", type=parse_target_course, default=None, metavar="DX:DZ,...",
+                        help="target scene: waypoints in m from the start position, visited in order")
     return ap
+
+
+MAX_COURSE_POINTS = 16
+MARKER_HEIGHT, MARKER_RADIUS = 0.1, 0.1   # m: the goal drawn by --render with a course, a sphere resting on the ground
+
+
+def _parse_points(text, width, form):
+    """comma-separated points of `width` colon-separated finite numbers: [K, width] lists, 1 <= K <= MAX_COURSE_POINTS"""
+    import math
+    try:
+        pts = [[float(x) for x in p.split(":")] for p in text.split(",")]
+    except ValueError:
+        raise argparse.ArgumentTypeError("need %s, got %r" % (form, text))
+    if any(len(p) != width for p in pts) or not 1 <= len(pts) <= MAX_COURSE_POINTS:
+        raise argparse.ArgumentTypeError("need 1 to %d points %s, got %r" % (MAX_COURSE_POINTS, form, text))
+    if any(not math.isfinite(x) for p in pts for x in p):
+        raise argparse.ArgumentTypeError("course values must be finite, got %r" % text)
+    return pts
+
+
+def parse_heading_course(text):
+    """T:H:V,...: [K, 3] rows (episode time s, heading rad, speed m/s), times strictly increasing from >= 0, speeds >= 0"""
+    pts = _parse_points(text, 3, "T:H:V,... (seconds, radians, m/s)")
+    if pts[0][0] < 0.0 or any(b[0] <= a[0] for a, b in zip(pts, pts[1:])):
+        raise argparse.ArgumentTypeError("heading course times must increase from >= 0, got %r" % text)
+    if any(p[2] < 0.0 for p in pts):
+        raise argparse.ArgumentTypeError("heading course speeds must be >= 0, got %r" % text)
+    return pts
+
+
+def parse_target_course(text):
+    """DX:DZ,...: [K, 2] waypoints in metres from the start position"""
+    return _parse_points(text, 2, "DX:DZ,... (metres)")
+
+
+def course_markers(rec, length):
+    """[length + 1, 4] marker rows (x, MARKER_HEIGHT, z, MARKER_RADIUS) of one environment's episode frames from its course records [T, 4]:
+    frame f > 0 draws the record of step f - 1 (the step that ended in it), frame 0 that of step 0"""
+    import numpy as np
+    rec = np.asarray(rec, dtype=np.float64)
+    idx = np.maximum(np.arange(length + 1) - 1, 0)
+    m = np.empty((length + 1, 4), dtype=np.float32)
+    m[:, 0], m[:, 1], m[:, 2], m[:, 3] = rec[idx, 0], MARKER_HEIGHT, rec[idx, 1], MARKER_RADIUS
+    return m
 
 
 DYNAMICS_KINDS = ("friction", "kp", "kd", "torque_limit", "mass")
@@ -144,14 +205,18 @@ def write_episode_motions(path_fmt, ep, count, frame_dur):
 
 def write_episode_renders(path_fmt, ep, count, frame_dur, core, camera=None, size=(640, 360)):
     """animated PNGs of the first `count` environments of run_episodes(pose_envs >= count)'s result `ep`, the frames of write_episode_motions
-    drawn as core's character: path_fmt % env; returns the paths"""
+    drawn as core's character, with the goal of each frame (course_markers) when ep has course records: path_fmt % env; returns the paths"""
     from .render import write_pose_apng
     from .rollout import episode_motion
     lengths = ep["lengths"].cpu().tolist()
     paths = []
     for e in range(count):
         frames = episode_motion(ep["poses"], ep["end_poses"], e, int(lengths[e]))
-        write_pose_apng(core, path_fmt % e, frames, [frame_dur] * frames.shape[0], camera, size)
+        if "course" in ep:
+            marks = course_markers(ep["course"][:, e].cpu().numpy(), int(lengths[e]))
+            write_pose_apng(core, path_fmt % e, frames, [frame_dur] * frames.shape[0], camera, size, markers=marks)
+        else:
+            write_pose_apng(core, path_fmt % e, frames, [frame_dur] * frames.shape[0], camera, size)
         paths.append(path_fmt % e)
     return paths
 
@@ -199,18 +264,43 @@ def main(argv=None):
     if opts.latency_sweep is not None:
         lat = np.asarray([opts.latency_sweep[e % len(opts.latency_sweep)] for e in range(opts.num_envs)])
         env.set_action_latency(lat)
+    course = opts.heading_course or opts.target_course
+    if course is not None:
+        kind = int(env._core.task_params()[0][0])   # 1 target_amp, 2 heading_amp, 3 heading_amp_getup
+        if (opts.heading_course is not None and kind not in (2, 3)) or (opts.target_course is not None and kind != 1):
+            raise SystemExit("run: --%s needs the %s scene, not %s" % ("heading_course" if opts.heading_course is not None else "target_course",
+                                                                     "heading_amp or heading_amp_getup" if opts.heading_course is not None
+                                                                     else "target_amp", env.get_name()))
+        env.set_goal_course(np.asarray(course, dtype=np.float64))
     ro = BatchedRollout(env, exp_rate=0.0, seed=opts.seed, backend=opts.backend)
     norms = dict(s_norm=ro.s_norm, a_norm=ro.a_norm, **(dict(g_norm=ro.g_norm) if ro.goal_size > 0 else {}))
     try:
         load_model_files(model_files, ro.policy, norms)
     except ValueError as e:
         raise SystemExit("run: %s" % e)
-    ep = run_episodes(ro, pose_envs=max(opts.record_motion, opts.render), pose_error=opts.pose_error)
+    ep = run_episodes(ro, pose_envs=max(opts.record_motion, opts.render), pose_error=opts.pose_error, course=course is not None)
     torch.cuda.synchronize(env.device)
     ret, length, term = (ep[k].cpu().numpy() for k in ("returns", "lengths", "terminate"))
     if opts.pose_error:
         perr, perr_dtw = ep["pose_err"].cpu().numpy(), ep["pose_err_dtw"].cpu().numpy()
-    err_means = lambda sel: (", pose error %.4f m, DTW %.4f m" % (float(np.mean(perr[sel])), float(np.mean(perr_dtw[sel])))) if opts.pose_error else ""
+    course_cols = {}
+    if opts.heading_course is not None:
+        course_cols = dict(Speed_Err=ep["speed_err"].cpu().numpy(), Cross_Speed=ep["cross_speed"].cpu().numpy())
+    elif opts.target_course is not None:
+        course_cols = dict(Waypoints=ep["waypoints"].cpu().numpy(), Course_Time=ep["course_time"].cpu().numpy())
+
+    def course_means(sel):
+        if opts.heading_course is not None:
+            return ", speed error %.4f m/s, cross-track speed %.4f m/s" % (float(np.mean(course_cols["Speed_Err"][sel])),
+                                                                           float(np.mean(course_cols["Cross_Speed"][sel])))
+        if opts.target_course is not None:
+            wp, ct = course_cols["Waypoints"][sel], course_cols["Course_Time"][sel]
+            done = np.isfinite(ct)
+            return ", waypoints %.2f of %d, all reached %.3f in %s s" % (float(np.mean(wp)), len(course), float(np.mean(done)),
+                                                                       "%.3f" % float(np.mean(ct[done])) if done.any() else "nan")
+        return ""
+    err_means = lambda sel: ((", pose error %.4f m, DTW %.4f m" % (float(np.mean(perr[sel])), float(np.mean(perr_dtw[sel]))))
+                             if opts.pose_error else "") + course_means(sel)
     os.makedirs(out_path, exist_ok=True)
     log = TableLog(os.path.join(out_path, "run_log.txt"))
     for e in range(opts.num_envs):
@@ -226,6 +316,8 @@ def main(argv=None):
         if opts.pose_error:
             log.log_tabular("Pose_Err", float(perr[e]))
             log.log_tabular("Pose_Err_DTW", float(perr_dtw[e]))
+        for k, v in course_cols.items():
+            log.log_tabular(k, float(v[e]))
         log.dump_tabular()
     log.close()
     print("%s, %d episodes: return %.4f +- %.4f, length %.1f policy steps, ended by Fail %.3f" % (model_files, opts.num_envs, float(np.mean(ret)),
@@ -233,6 +325,10 @@ def main(argv=None):
     if opts.pose_error:
         print("pose error %.4f +- %.4f m, time-warped %.4f +- %.4f m" % (float(np.mean(perr)), float(np.std(perr)), float(np.mean(perr_dtw)),
                                                                      float(np.std(perr_dtw))))
+    if course is not None:
+        print("%s course of %d points: %d episodes, not ended by Fail %.3f%s" % ("heading" if opts.heading_course is not None else "target",
+                                                                             len(course), opts.num_envs, float(np.mean(term != 1)),
+                                                                             course_means(np.ones(opts.num_envs, dtype=bool))))
     if opts.push_forces is not None:
         for f in opts.push_forces:
             sel = mag == f
@@ -260,6 +356,7 @@ def main(argv=None):
     out = dict(returns=ret, lengths=length, terminate=term)
     if opts.pose_error:
         out.update(pose_err=perr, pose_err_dtw=perr_dtw)
+    out.update({k.lower(): v for k, v in course_cols.items()})
     return out
 
 

@@ -173,6 +173,33 @@ int dm_set_dynamics_randomization(dm_handle* h, const double* lohi);
 int dm_set_action_latency(dm_handle* h, const int32_t* h_updates);
 int dm_set_action_latency_randomization(dm_handle* h, int lo, int hi);
 int dm_get_action_latency(dm_handle* h, int32_t* d_out);
+/* Goal courses of the heading and target scenes (heading_amp, heading_amp_getup, target_amp): commanded goals instead of the scene's random
+ * ones.  Environment e has h_count[e] in [0, 16] rows of 3 doubles at h_rows + e * 16 * 3; a count of 0 keeps the scene's own goals bit for bit.
+ *   heading scenes: rows (t, h, v): episode time in s (strictly increasing, t_0 >= 0), heading in radians (direction (cos h, -sin h) in the
+ *     x-z plane, h = 0 along +x, the scene's goal convention) and speed in m/s (>= 0).  The goal at episode time tau is row 0 before t_0, the
+ *     last row after t_{n-1}, h and v linear in tau in between; angles are not wrapped (0 -> 2 pi is one full turn about +y).
+ *   target scene: rows (dx, dz, unused): waypoints, offsets in metres in world axes from the root's horizontal position when the course
+ *     started.  The first is the goal; the goal advances when the root comes within the scene's target_succ_dist of it (two waypoints within
+ *     one radius both count at once), and the last stays the goal once reached.  A waypoint further than tar_fail_dist from the character
+ *     ends the episode through the scene's own distance failure.
+ * A course starts at every reset of its environment and at this call: the target origin is the root then, and the goal for the episode time
+ * then is in the task block before the next observation.  After every dm_update a course environment records the interval just stepped,
+ * advances its waypoints and writes the goal for its new episode time, and the scene's timed redraw never fires (its task draw counter does
+ * not move until the next reset).  The step, observation and reward kernels are unchanged: a steered episode's goal observation and reward
+ * are the scene's own for the commanded goal.  An environment whose count drops to 0 keeps its last goal until its next reset, where the
+ * scene draws its own goals again.  The first call allocates the table; handles that never call it run exactly as before.  The call
+ * synchronises the stream; the course launches after resets and updates do not.  Refused by name: a scene without courses, a count outside
+ * [0, 16], a row value that is not finite (the target scene's third value is not read), heading times that are not increasing or a negative
+ * first time, and a negative speed.  dm_save_state / dm_load_state refuse a handle with a course: courses belong to runs.
+ * dm_get_course_record: every environment's record of its last course call into d_out [N x 4] floats on the device, stream-ordered:
+ *   heading scenes: (x, z of the point 1.5 m from the root along the heading in force during the interval; along-track speed minus the
+ *     commanded speed; cross-track speed, positive towards heading h + pi / 2), the speeds the root's horizontal displacement over the
+ *     interval divided by its episode time, 0 for an interval of no time;
+ *   target scene: (x, z of the goal waypoint; the waypoints reached so far; the root's horizontal distance to the goal waypoint), after the
+ *     call's advance.
+ * Environments without a course keep whatever their record last held (zeros at first).  Refused on a handle without a course table. */
+int dm_set_goal_course(dm_handle* h, const int32_t* h_count, const double* h_rows);
+int dm_get_course_record(dm_handle* h, float* d_out);
 /* Placement of the environments in the step kernel (on by default; tile width 16 only, where two environments share a warp: tile width 32
  * handles keep index placement, where it measured slower): every step launch is preceded by a one-block kernel that orders the
  * environments by contact load -- the solver row count of each environment's last Bullet sub-step, its key -- so that environments of equal
@@ -207,6 +234,11 @@ int dm_record_pose(dm_handle* h, float* d_pose, float* d_vel);
  * fov_y outside (0, pi). */
 typedef struct { float yaw, pitch, distance, target_height, fov_y; } dm_camera;
 int dm_render_poses(dm_handle* h, int n_views, const float* d_pose, const dm_camera* cam, int width, int height, uint8_t* d_rgb, int16_t* d_ids);
+/* dm_render_poses with one marker per view, such as a goal: d_marker [n_views x 4] fp32 (x, y, z, radius) in unscaled metres, a sphere in a
+ * colour of its own (green), shaded and shadowed like a link and casting its shadow like one; its pixels have id -3.  A radius <= 0 draws no
+ * marker, and a view without one is dm_render_poses's, byte for byte.  Refuses what dm_render_poses refuses and a NULL d_marker. */
+int dm_render_poses_marked(dm_handle* h, int n_views, const float* d_pose, const float* d_marker, const dm_camera* cam, int width, int height,
+                           uint8_t* d_rgb, int16_t* d_ids);
 /* The kinematic character's pose (cKinCharacter::GetPose): [num_envs x pose_dim] fp32 rows in dm_record_pose's layout, every environment's clip
  * sampled at its kin time with the loop's cycle offset and the origin rotation and position applied -- what dm_observe's imitation reward
  * compares against; quaternions with w >= 0.  In --kin_ctrl clips scenes the environment's own clip of the dataset; past the end of a non-looping
